@@ -1,14 +1,14 @@
 #!/usr/bin/env python
 """Benchmark of the MoGe-2 hot path (BASELINE.json metric: images/sec, ViT-L, 518 px, fp16).
 
-  python bench.py --gpus 1 --steps K --warmup W                 engine arm (this repo, sm_100a kernels)
+  python bench.py --gpus 1 --steps K --warmup W                 engine arm (this repo, sm_90a kernels)
   torchrun ... bench.py --gpus N ...                              one rank per GPU, weak scaling (fixed images per GPU)
   python bench.py --impl reference ...                            the reference algorithm on the host cores (oracle port)
 
 A "step" is one `MoGeModel.infer()` over one batch of synthetic 518x518 images per GPU.  Rank 0 prints ONE JSON line.
   value  : images/s with the inputs already resident in HBM (device-timed, max over ranks)
   e2e    : images/s through the public API with HOST buffers: pinned host -> H2D -> infer -> D2H of every output
-  roofline      : encoder GEMM launches of the tcgen05 kernel (tensor bound), flops / CUDA-event time, live
+  roofline      : encoder GEMM launches of the wgmma kernel (tensor bound), flops / CUDA-event time, live
   roofline_decoder / roofline_attention : the other two kernel classes
   cpu_baseline  : the oracle port (restated reference algorithm, fp32) timed on this box's host cores (rank 0, N=1)
 """
@@ -52,6 +52,9 @@ def parse():
                     "~700-token ViT-L-normal bf16 batch (configs[2]); 5: ViT-B resolution / aspect sweep (configs[4])")
     ap.add_argument("--no-gpu-baseline", action="store_true", help="skip the same-box PyTorch-CUDA comparator (gpu_baseline)")
     ap.add_argument("--gpu-baseline-kernels", default=None, help="write the torch.profiler kernel list of one batch-1 comparator pass here")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step returned as DIR/<output>.npy (float32, 64 MB in all: a fixed, seeded "
+                         "sample of the larger outputs; pixels outside the mask as 0), for output-by-output comparison of two builds")
     return ap.parse_args()
 
 
@@ -60,7 +63,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return {"hbm_gbs": d["hbm_gbs"], "tflops": d["bf16_tflops_sustained"], "source": "measured (MEASURED_PEAKS.json, sustained)"}
-    return {"hbm_gbs": 6650.0, "tflops": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tflops": 989.0, "source": "H100 SXM data sheet (HBM3; dense fp16/bf16 tensor core), not measured"}
 
 
 class ClockSampler:
@@ -96,6 +99,18 @@ class ClockSampler:
         reasons = sorted({names[i] for r in self.rows if len(r) >= 7 for i in range(4) if r[3 + i].lower().startswith("active")})
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
                 "reasons": reasons, "samples": len(self.rows)}
+
+
+def gpu_identity(index):
+    """Name and power limit of the GPU the numbers were measured on (a number is only meaningful with both)."""
+    out = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        q = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=10).stdout.strip()
+        out["power_limit_w"] = float(q)
+    except Exception:
+        pass
+    return out
 
 
 def host_threads():
@@ -195,6 +210,30 @@ def gpu_baseline(cfg, sd, dev, res, tokens, batch, iters_b1=200, kernels_path=No
     return out
 
 
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out, path):
+    """Every output of one infer() as float32 .npy files, DUMP_MAX_BYTES in all: an output with more than its share of elements
+    is replaced by the values at that many flat indices drawn once from a fixed seed (sorted; the same indices for the same
+    shape).  Pixels that infer() marks invalid (mask false: +inf in points / depth, as in the reference) are written as 0 --
+    mask.npy says which they are -- so that every dumped value is finite and a non-finite one is a defect."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    cap = DUMP_MAX_BYTES // 4 // len(out)
+    mask = out.get("mask")
+    for k, v in out.items():
+        v = v.detach().float()
+        if mask is not None and k != "mask" and v.shape[:mask.dim()] == mask.shape:
+            v = torch.where(mask.reshape(mask.shape + (1,) * (v.dim() - mask.dim())), v, torch.zeros_like(v))
+        flat = v.reshape(-1)
+        if flat.numel() > cap:
+            g = torch.Generator().manual_seed(20240601)
+            idx = torch.randperm(flat.numel(), generator=g)[:cap].sort().values
+            flat = flat[idx.to(flat.device)]
+        np.save(os.path.join(path, f"{k}.npy"), flat.cpu().numpy().astype(np.float32))
+
+
 def workload_name(a, h, w):
     return (f"MoGe-2 {a.size} {a.dtype} infer(), {a.batch} x {a.res}x{a.res} images per GPU, num_tokens={a.tokens} -> {h}x{w} grid "
             f"(BASELINE.json configs[1]/[3] shape; random-init weights)")
@@ -290,8 +329,10 @@ def run_engine(a):
         barrier()
         return float(ms.item())
 
+    last = {}
+
     def step_dev():
-        model.infer(dev_in, num_tokens=a.tokens)
+        last["out"] = model.infer(dev_in, num_tokens=a.tokens)
 
     def step_e2e():
         x = host_in.to(dev, non_blocking=True)
@@ -306,6 +347,9 @@ def run_engine(a):
         sampler.start()
     ms_dev = timed(step_dev, a.steps)
     clocks = sampler.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:
+        dump_outputs(last["out"], a.dump_outputs)
+    del last
     for _ in range(min(a.warmup, 2)):
         step_e2e()
     ms_e2e_serial = timed(step_e2e, a.steps)
@@ -390,22 +434,13 @@ def run_engine(a):
         t = sum(ms_op[i] for i in idx) / 1e3
         return idx, t, sum(ops[i][1] for i in idx), sum(ops[i][2] for i in idx)
 
-    # DRAM traffic of the dominant launch of each class, from the committed `ncu --set full` capture of this workload
-    # (profiles/r2_ncu_traffic.json; per launch, like `achieved`); null for any other workload
-    traffic = {}
-    tpath = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles", "r2_ncu_traffic.json")
-    if a.size == "vitl" and B == 32 and R == 518 and a.tokens == 1369 and a.dtype == "fp16" and os.path.exists(tpath):
-        with open(tpath) as fh:
-            traffic = json.load(fh)
-
+    # DRAM traffic per launch is not measured (no hardware-counter profiler here): reported as null
     def traffic_of(key):
-        t_ = traffic.get(key)
-        return (None, None) if not t_ else (t_["dram_bytes"], {"kernel": t_["kernel"], "algorithmic_bytes": t_["algorithmic_bytes"],
-                                                                "ratio_to_algorithmic": t_["dram_bytes"] / t_["algorithmic_bytes"], "source": t_["file"]})
+        return None, None
 
     total_prof_ms = sum(ms_op)
     idx, t, fl, by = cls(("gemm.",))
-    roofline = {"kernel": "umma2_kernel (cta_group::2) + umma_kernel<AMODE_ROWS>: encoder linears patch/qkv/proj/fc1/fc2/taps", "bound": "tensor",
+    roofline = {"kernel": "umma_kernel<AMODE_ROWS> (wgmma): encoder linears patch/qkv/proj/fc1/fc2/taps", "bound": "tensor",
                 "achieved": fl / t / 1e12, "peak": pk["tflops"], "unit": "TFLOP/s", "frac": fl / t / 1e12 / pk["tflops"],
                 "traffic": traffic_of("gemm")[0], "traffic_detail": traffic_of("gemm")[1], "launches": len(idx), "ms_per_step": t * 1e3,
                 "share_of_step": t * 1e3 / total_prof_ms, "peak_source": pk["source"]}
@@ -414,7 +449,7 @@ def run_engine(a):
     # algorithmic bytes: SURVEY.md 8(d) "every tensor that crosses a conv boundary once": 501 760 elements x T per image at 2 bytes
     # (the engine's own per-launch count `by` is LOWER -- its load-time folds removed tensors -- and is reported beside it)
     by_survey = 501760.0 * (h * w) * 2 * B
-    roofline_decoder = {"kernel": "umma_kernel<AMODE_TILES> + convh_kernel + conv64_kernel (implicit-GEMM convs)", "bound": "hbm",
+    roofline_decoder = {"kernel": "umma_kernel<AMODE_TILES> in its GEMM / CONVH / CONV64 modes (implicit-GEMM convs)", "bound": "hbm",
                         "achieved": by_survey / t / 1e9, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": by_survey / t / 1e9 / pk["hbm_gbs"],
                         "bytes_definition": "SURVEY.md 8(d): 501760 * T elements * 2 B per image (conv-boundary tensors once)",
                         "engine_bytes_per_step": by, "frac_engine_bytes": by / t / 1e9 / pk["hbm_gbs"],
@@ -461,8 +496,9 @@ def run_engine(a):
         "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms_value / a.steps, "higher_is_better": True, "scaling": "weak",
         "vs_baseline": None, "dtype": a.dtype, "data": "synthetic",
         "config": {"workload": workload_name(a, h, w), "images_per_gpu": B, "grid": [h, w],
-                   "l2": "per-step working set (activation workspace, GBs) far exceeds the 126 MB L2; no explicit flush",
-                   "weights": "seeded random init (moge_b200.synthetic), broadcast from rank 0 over NCCL" if world > 1 else "seeded random init"},
+                   "l2": "per-step working set (activation workspace, GBs) far exceeds the 50 MB L2; no explicit flush",
+                   "weights": "seeded random init (moge_b200.synthetic), broadcast from rank 0 over NCCL" if world > 1 else "seeded random init",
+                   "gpu": gpu_identity(local)},
         "e2e": {"value": images / (ms_e2e / 1e3), "unit": "images/s", "h2d_bytes_per_step": h2d_bytes, "d2h_bytes_per_step": d2h_bytes,
                 "ms_per_step": ms_e2e / a.steps, "api": "moge_b200.serving.InferPipeline(model).submit(pinned_in, pinned_out) / join()",
                 "overlap": "H2D(i+1) | infer(i) | D2H(i-1) on three streams, depth 2",
@@ -527,7 +563,7 @@ def decoder_bytes_survey(c0, tokens, images):
 
 
 def run_config3(a):
-    """BASELINE.json configs[2]: ViT-L-normal bf16, 32 images of ~700 tokens in five aspect ratios on ONE B200 -- encoder tensor-pipe
+    """BASELINE.json configs[2]: ViT-L-normal bf16, 32 images of ~700 tokens in five aspect ratios on ONE H100 -- encoder tensor-pipe
     roofline.  (a) the reference's only option, same-shape sub-batches (five infer() calls); (b) ragged packing, ONE engine call
     (infer_many): every linear over the concatenated token rows, attention over a ragged work list."""
     from moge.model.v2 import MoGeModel

@@ -1,4 +1,4 @@
-/* moge_b200 -- C ABI of the B200-native MoGe-2 inference engine (libmoge_b200.so, sm_100a).
+/* moge_b200 -- C ABI of the H100-native MoGe-2 inference engine (libmoge_b200.so, sm_90a).
  *
  * The reference (microsoft/MoGe) has no FFI / plugin boundary on this path: the hot path is the Python nn.Module
  * `moge.model.v2.MoGeModel` (/root/reference/moge/model/v2.py).  This header is the boundary the replacement exports;
@@ -12,7 +12,7 @@
  *   - the caller owns every input/output tensor and the workspace; the engine owns its packed weights.
  *   - calls on one engine must be serialised by the caller (stream order); engines on different devices (or several engines
  *     on one device) may live in one process and be driven from different threads.
- *   - there is NO CPU fallback: without a sm_100 device every compute entry point fails.
+ *   - there is NO CPU fallback: without a sm_90 (H100) device every compute entry point fails.
  */
 #ifndef MOGE_B200_H
 #define MOGE_B200_H
@@ -62,7 +62,7 @@ typedef struct moge_config {
 typedef struct moge_engine moge_engine_t;
 
 const char* moge_last_error(void);
-/* library / build identification: "moge_b200 <version> sm_100a" */
+/* library / build identification: "moge_b200 <version> sm_90a" */
 const char* moge_version(void);
 
 /* replaces MoGeModel.__init__ (v2.py:30-57) + .to(device) */

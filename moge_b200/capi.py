@@ -1,7 +1,7 @@
 """ctypes binding of libmoge_b200.so (the C ABI declared in include/moge_b200.h).
 
 The library is built in-tree by `__graft_entry__.build()` / moge_b200/csrc/build.sh into moge_b200/_lib/.  There is
-no CPU fallback: if the shared object is missing or no sm_100 device is present the compute calls raise.
+no CPU fallback: if the shared object is missing or no sm_90 (H100) device is present the compute calls raise.
 """
 from __future__ import annotations
 

@@ -1,27 +1,19 @@
 // Multi-head self-attention of the DINOv2 blocks (reference: dinov2/layers/attention.py:70-81, SDPA with
-// scale hd^-0.5, no mask) as one tcgen05 kernel: S = Q K^T and O~ = P V on the tensor cores with TMEM accumulators,
-// single-pass online softmax in registers (the whole 128-wide score row lives in registers; FMNMX3 + MUFU.EX2),
-// O accumulated in TMEM by the MMA itself and rescaled lazily (only when the running max grows by more than 2^8),
-// two 128-row query tiles per CTA ping-ponging on the tensor pipe.  The probabilities P never touch shared memory: the
-// softmax threads store them (16-bit, packed) into tensor memory and the P V MMA reads its A operand from there -- with
-// P in smem the kernel was shared-memory-bandwidth-bound (P write + P read were half of all smem traffic and the MMAs
-// ran at 2.3x their nominal duration waiting for operands).
+// scale hd^-0.5, no mask) as one wgmma kernel: S = Q K^T from shared memory, single-pass online softmax in registers,
+// O~ += P V with P taken straight from the registers that held S (the fp32 accumulator fragment of S is, after packing to
+// 16 bit, the A-operand fragment of the P V MMA), O accumulated in registers.
 //
 // Layout: qkv is the QKV-GEMM output [rows, 3*D] (16-bit), the token rows of all images PACKED back to back (images may have
 // different token counts: ragged batches); Q/K/V tiles of head h are the column windows [h*64, D+h*64, 2D+h*64) fetched by
-// TMA straight from that buffer (no head-major repack): Q and K tiles are K-major UMMA operands, the V tile ([kv][hd], hd
+// TMA straight from that buffer (no head-major repack): Q and K tiles are K-major wgmma operands, the V tile ([kv][hd], hd
 // contiguous) is consumed as an MN-major B operand.  A K/V box that runs past the image's last token reads the next image's
 // rows (or TMA zero fill past the buffer): those columns are masked to -inf before the softmax.
 // Output: out[row0 + q, h*64 + d] (16-bit), the A operand of the projection GEMM.
 //
 // PERSISTENT: one CTA per SM walks a contiguous range of work items (image, head, pair of 128-row query tiles) from a host-built
-// list (cost-balanced ranges, consecutive query tiles of one (image, head) on the same SM -> K/V come from L2).  Barriers,
-// the TMEM allocation and the smem ring live across items; the next item's Q load and first S = Q K^T are issued under the
-// current item's O normalise + store.
-//
-// exp2: a compile-time subset (MG_ATT_POLY_MASK, default 8 of every 32) of the exponentials is evaluated on the FMA pipe (Cody-Waite range reduction by the 1.5*2^23 magic add +
-// a degree-3 minimax polynomial on [-0.5, 0.5], max rel. error 7.5e-5 -- below the 16-bit rounding of P -- exponent inserted by
-// an integer shift-add), the rest on MUFU.EX2: the 16 MUFU lanes of an SM were the limiter (128 ex2 per row and tile).
+// list (cost-balanced ranges, consecutive query tiles of one (image, head) on the same SM -> K/V come from L2).  Warpgroup 0
+// streams Q and the K/V ring by TMA; consumer warpgroup g (1 + g) owns query tile g of the item and runs it as two 64-row
+// halves, each with its own O accumulator and running max / sum.
 #include "common.cuh"
 #include "host_api.h"
 #include <vector>
@@ -29,32 +21,15 @@
 namespace mg {
 
 constexpr int ATT_HD = 64;
-constexpr int ATT_BQ = 128;       // query rows per softmax warpgroup
+constexpr int ATT_BQ = 128;       // query rows per consumer warpgroup
 constexpr int ATT_BKV = 128;      // keys per tile
 constexpr int ATT_KV_STAGES = 5;
 constexpr int ATT_TILE_BYTES = 128 * 128;   // [128 rows][64 x 16-bit]
-#ifndef MG_ATT_POLY_MASK
-#define MG_ATT_POLY_MASK 0x1248u     // pairs 3, 6, 9, 12 of the 16 pairs of a 32-column chunk: 8 of 32 exponentials on the FMA pipe
-                                     // (same-box A/B of the whole step, attention ms: 0/32 12.75, 8/32 11.33, 10/32 11.95, 16/32 12.49)
-#endif
-constexpr uint32_t ATT_POLY_MASK = MG_ATT_POLY_MASK;
-constexpr int ATT_THREADS = 128 + 256;   // warpgroup 0: TMA warp, MMA warp, 2 idle; warpgroups 1,2: softmax
+constexpr int ATT_THREADS = 128 + 256;   // warpgroup 0: TMA; warpgroups 1, 2: MMA + softmax
 // smem: Q0,Q1 | K[stages] | V[stages] | barriers
 constexpr int ATT_SMEM = (2 + 2 * ATT_KV_STAGES) * ATT_TILE_BYTES + 1024 + 256;
 static_assert(ATT_SMEM <= kMaxDynSmem, "attention_kernel: Q + K/V ring exceed the shared memory of one CTA");
-static_assert((2 + 4 * ATT_KV_STAGES + 8) * 8 + 4 <= 256, "attention_kernel: barrier block overflows its 256 bytes");
-
-#ifdef MG_ATT_DEBUG
-// wait-time attribution (debug builds only; tools/att_debug.py), summed over CTAs, warp 4 lane 0 / warp 1 lane 0:
-// [0] softmax waits S  [1] softmax waits PV(j-1)  [2] softmax loop total  [3] MMA waits P  [4] MMA waits K/V
-// [5] CTA lifetime  [6] prologue (start -> first S)  [7] epilogue (O normalise + store)
-__device__ unsigned long long mg_att_dbg[8];
-#define ATT_T0() const long long _t0 = clock64()
-#define ATT_ACC(var) var += clock64() - _t0
-#else
-#define ATT_T0()
-#define ATT_ACC(var)
-#endif
+static_assert((2 + 4 * ATT_KV_STAGES) * 8 <= 256, "attention_kernel: barrier block overflows its 256 bytes");
 
 struct AttnParams {
     void* out;               // [rows, D] 16-bit
@@ -64,26 +39,10 @@ struct AttnParams {
     float scale_log2;        // hd^-0.5 * log2(e)
 };
 
-// 2^x for two lanes on the FMA pipe.  x = n + f with n = round(x) (magic add), f in [-0.5, 0.5]; 2^f by a degree-3 minimax
-// polynomial; 2^n by adding n to the exponent field.  Inputs are clamped at -126 (masked scores are -inf).
-__device__ __forceinline__ float2 ex2_poly2(float2 x) {
-    const float kMagic = 12582912.0f;      // 1.5 * 2^23
-    x.x = fmaxf(x.x, -126.0f); x.y = fmaxf(x.y, -126.0f);
-    const float2 y = fadd2(x, make_float2(kMagic, kMagic));
-    const float2 r = fadd2(y, make_float2(-kMagic, -kMagic));
-    const float2 f = ffma2(r, make_float2(-1.0f, -1.0f), x);
-    float2 q = ffma2(make_float2(0.0551716685f, 0.0551716685f), f, make_float2(0.2426111400f, 0.2426111400f));
-    q = ffma2(q, f, make_float2(0.6932609677f, 0.6932609677f));
-    q = ffma2(q, f, make_float2(0.9999280572f, 0.9999280572f));
-    // bits(y) = bits(magic) + n and bits(magic) << 23 == 0  =>  (bits(y) << 23) is n in the exponent field
-    return make_float2(__uint_as_float(__float_as_uint(q.x) + (__float_as_uint(y.x) << 23)),
-                       __uint_as_float(__float_as_uint(q.y) + (__float_as_uint(y.y) << 23)));
-}
-
 template <bool BF16>
 __global__ void __launch_bounds__(ATT_THREADS, 1)
 attention_kernel(const __grid_constant__ CUtensorMap mapQKV, const AttnParams p) {
-    pdl_launch_dependents();      // (the wait sits after the barrier / TMEM set-up below: that prologue overlaps the previous kernel's tail)
+    pdl_launch_dependents();      // (the wait sits after the barrier set-up below: that prologue overlaps the previous kernel's tail)
     using H = H16<BF16>;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
@@ -93,63 +52,44 @@ attention_kernel(const __grid_constant__ CUtensorMap mapQKV, const AttnParams p)
     uint8_t* sV = sK + ST * ATT_TILE_BYTES;
     uint64_t* bars = reinterpret_cast<uint64_t*>(sV + ST * ATT_TILE_BYTES);
     uint64_t* q_full = bars;                 // 1: Q tiles of the current item landed
-    uint64_t* q_empty = bars + 1;            // 1: every S MMA of the current item has read Q -> the next item's Q may be loaded
+    uint64_t* q_empty = bars + 1;            // every S MMA of the current item has completed -> the next item's Q may be loaded
     uint64_t* k_full = bars + 2;
     uint64_t* k_empty = k_full + ST;
     uint64_t* v_full = k_empty + ST;
     uint64_t* v_empty = v_full + ST;
-    uint64_t* s_full = v_empty + ST;         // 2
-    uint64_t* p_full = s_full + 2;           // 2
-    uint64_t* o_full = p_full + 2;           // 2 (one per group; completes once per kv tile)
-    uint64_t* s_free = o_full + 2;           // 2: the softmax threads hold the whole score tile in registers -> S may be overwritten
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(s_free + 2);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-#ifdef MG_ATT_DEBUG
-    long long dbg_a = 0, dbg_b = 0, dbg_c = 0, dbg_d = 0, dbg_e = 0;
-    const long long dbg_start = clock64();
-#endif
     const int2 rng = p.ranges[blockIdx.x];
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&mapQKV);
-        mbar_init(q_full, 1); mbar_init(q_empty, 1);
-        for (int s = 0; s < ATT_KV_STAGES; ++s) {
-            mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 1);
-            mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 1);
-        }
-        for (int g = 0; g < 2; ++g) {
-            mbar_init(&s_full[g], 1); mbar_init(&p_full[g], 4);
-            mbar_init(&o_full[g], 1); mbar_init(&s_free[g], 4);
+        // empty barriers: one arrival per consumer warp (8) once its warpgroup's MMAs reading the buffer have completed
+        mbar_init(q_full, 1); mbar_init(q_empty, 8);
+        for (int s = 0; s < ST; ++s) {
+            mbar_init(&k_full[s], 1); mbar_init(&k_empty[s], 8);
+            mbar_init(&v_full[s], 1); mbar_init(&v_empty[s], 8);
         }
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, 512);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = *tmem_slot;
     pdl_wait();
-    // TMEM columns: S0 [0,128)  S1 [128,256)  O0 [256,320)  O1 [320,384)  P0 [384,448)  P1 [448,512)  (P: 2 x 16-bit per column)
-    // Barrier phases: every barrier is waited on by "completion index" (a running count that survives item boundaries):
-    // completion k of a barrier is observed with parity k & 1.
 
-    // register re-balancing between the control warpgroup and the two softmax warpgroups (row of 128 scores in registers)
-    if (warp == 0) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-        // The warp stays converged and ONE ELECTED lane issues (here and in the MMA warp): under `if (lane == 0)` the
-        // compiler wraps every TMA / tcgen05 instruction in an elect-and-retry loop, ~9 dependent instructions per MMA.
+    if (warp < 4) {
+        // ========================================================== TMA producer (warp 0, converged, one elected lane issues)
+        regs_dec<40>();
+        if (warp != 0) return;
         int s = 0; uint32_t ph = 0;
         for (int it = rng.x; it < rng.y; ++it) {
             const AttnItem item = p.items[it];
             const int li = it - rng.x;
             const int nkv = (item.n + ATT_BKV - 1) / ATT_BKV;
-            const int ng = (item.q0 + ATT_BQ < item.n) ? 2 : 1;   // the second query tile of an image's last item may lie entirely past N: skipped
             if (li > 0) mbar_wait(q_empty, (li - 1) & 1);
             if (elect_one()) {
-                mbar_arrive_expect_tx(q_full, ng * ATT_TILE_BYTES);
+                // both query tiles always: the second one of an image's last item may lie past the image (its rows are computed and
+                // not stored), so that every consumer warpgroup walks every K/V stage
+                mbar_arrive_expect_tx(q_full, 2 * ATT_TILE_BYTES);
                 tma_load_2d(sQ, &mapQKV, q_full, item.head * ATT_HD, item.row0 + item.q0);
-                if (ng == 2) tma_load_2d(sQ + ATT_TILE_BYTES, &mapQKV, q_full, item.head * ATT_HD, item.row0 + item.q0 + ATT_BQ);
+                tma_load_2d(sQ + ATT_TILE_BYTES, &mapQKV, q_full, item.head * ATT_HD, item.row0 + item.q0 + ATT_BQ);
             }
             __syncwarp();
             for (int j = 0; j < nkv; ++j) {
@@ -165,231 +105,119 @@ attention_kernel(const __grid_constant__ CUtensorMap mapQKV, const AttnParams p)
                     tma_load_2d(sV + s * ATT_TILE_BYTES, &mapQKV, &v_full[s], 2 * p.D + item.head * ATT_HD, item.row0 + j * ATT_BKV);
                 }
                 __syncwarp();
-                if (++s == ATT_KV_STAGES) { s = 0; ph ^= 1; }
+                if (++s == ST) { s = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-        {
-            constexpr uint32_t idesc_s = make_idesc(128, ATT_BKV, BF16 ? 1u : 0u, 0, 0);   // Q (K-major) x K (K-major)
-            constexpr uint32_t idesc_o = make_idesc(128, ATT_HD, BF16 ? 1u : 0u, 0, 1);    // P (TMEM) x V (MN-major)
-            // S_g = Q_g K_stage^T; `release` != 0: the K stage is free once these MMAs retire; `last`: Q is free as well
-            auto issue_s = [&](int g, int stage, bool release, bool last) {
-                if (elect_one()) {
-                    const uint64_t a = make_sdesc_sw128(smem_u32(sQ + g * ATT_TILE_BYTES));
-                    const uint64_t bd = make_sdesc_sw128(smem_u32(sK + stage * ATT_TILE_BYTES));
+        return;
+    }
+    // ============================================================== consumers: S = Q K^T, softmax, O += P V, normalise + store
+    regs_inc<232>();
+    const int g = (warp - 4) >> 2;          // query tile of the item
+    const int wl = warp & 3;
+    const float sc = p.scale_log2;
+    // accumulator fragment: this thread's rows r0 and r0 + 8 of a 64-row half; columns 8 (i / 4) + 2 (lane % 4) + i % 2
+    const int r0 = 16 * wl + (lane >> 2);
+    const int cq = 2 * (lane & 3);
+    int s = 0; uint32_t ph = 0;
+    for (int it = rng.x; it < rng.y; ++it) {
+        const AttnItem item = p.items[it];
+        const int li = it - rng.x;
+        const int nkv = (item.n + ATT_BKV - 1) / ATT_BKV;
+        mbar_wait(q_full, li & 1);
+        float o[2][32];
+        float m[2][2], l[2][2];
 #pragma unroll
-                    for (int k = 0; k < ATT_HD / 16; ++k) umma_f16(tmem + g * 128, a + 2 * k, bd + 2 * k, idesc_s, k != 0);
-                    umma_commit(&s_full[g]);
-                    if (release) umma_commit(&k_empty[stage]);
-                    if (last) umma_commit(q_empty);
-                }
-                __syncwarp();
-            };
-            // O_g (+)= P_g V_stage
-            auto issue_pv = [&](int g, int stage, bool first, bool release) {
-                if (elect_one()) {
-                    const uint32_t pa = tmem + 384 + g * 64;
-                    const uint32_t va = smem_u32(sV + stage * ATT_TILE_BYTES);
-                    const uint32_t d = tmem + 256 + g * 64;
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-                    for (int k = 0; k < ATT_BKV / 16; ++k) {
-                        // A: P in tensor memory, 16 keys (= 8 columns of packed 16-bit pairs) per K-step
-                        // B: V tile [kv][hd]: MN-major, 16 kv rows (= 2 groups of 8 x 128 B) per K-step
-                        const uint64_t bd = make_sdesc_sw128(va + k * 16 * 128, /*lbo=*/ATT_TILE_BYTES, /*sbo=*/1024);
-                        umma_f16_ts(d, pa + 8 * k, bd, idesc_o, !(first && k == 0));   // O accumulates across kv tiles in TMEM
-                    }
-                    umma_commit(&o_full[g]);
-                    if (release) umma_commit(&v_empty[stage]);
-                }
-                __syncwarp();
-            };
-            int sk = 0, sv = 0; uint32_t phk = 0, phv = 0;     // K / V ring positions (K runs one tile ahead of V)
-            uint32_t cs0 = 0, cs1 = 0;                          // kv tiles completed so far by group 0 / 1
-            for (int it = rng.x; it < rng.y; ++it) {
-                const AttnItem item = p.items[it];
-                const int li = it - rng.x;
-                const int nkv = (item.n + ATT_BKV - 1) / ATT_BKV;
-                const int ng = (item.q0 + ATT_BQ < item.n) ? 2 : 1;
-                // S(0) of both groups: issued right behind the previous item's last P V, i.e. under its O normalise + store
-                { ATT_T0(); mbar_wait(q_full, li & 1); mbar_wait(&k_full[sk], phk); ATT_ACC(dbg_b); }
-                for (int g = 0; g < ng; ++g) {
-                    const uint32_t cs = g ? cs1 : cs0;
-                    if (cs > 0) mbar_wait(&s_free[g], (cs - 1) & 1);
-                    tc_fence_after();
-                    issue_s(g, sk, g == ng - 1, nkv == 1 && g == ng - 1);
-                }
-                if (++sk == ATT_KV_STAGES) { sk = 0; phk ^= 1; }
-                for (int j = 0; j < nkv; ++j) {
-                    // S(j+1) of both groups first: it only needs the score registers of tile j to be loaded (s_free), not the
-                    // softmax of tile j to be finished -- the next scores are ready before the softmax threads ask for them
-                    if (j + 1 < nkv) {
-                        { ATT_T0(); mbar_wait(&k_full[sk], phk); ATT_ACC(dbg_b); }
-                        for (int g = 0; g < ng; ++g) {
-                            { ATT_T0(); mbar_wait(&s_free[g], ((g ? cs1 : cs0) + j) & 1); ATT_ACC(dbg_a); }
-                            tc_fence_after();
-                            issue_s(g, sk, g == ng - 1, j + 2 == nkv && g == ng - 1);
-                        }
-                        if (++sk == ATT_KV_STAGES) { sk = 0; phk ^= 1; }
-                    }
-                    { ATT_T0(); mbar_wait(&v_full[sv], phv); ATT_ACC(dbg_b); }
-                    for (int g = 0; g < ng; ++g) {
-                        { ATT_T0(); mbar_wait(&p_full[g], ((g ? cs1 : cs0) + j) & 1); ATT_ACC(dbg_a); }
-                        tc_fence_after();
-                        issue_pv(g, sv, j == 0, g == ng - 1);
-                    }
-                    if (++sv == ATT_KV_STAGES) { sv = 0; phv ^= 1; }
-                }
-                cs0 += nkv;
-                if (ng == 2) cs1 += nkv;
-            }
+            for (int i = 0; i < 32; ++i) o[h][i] = 0.f;
+            m[h][0] = m[h][1] = -INFINITY;
+            l[h][0] = l[h][1] = 0.f;
         }
-    } else if (warp < 4) {
-        asm volatile("setmaxnreg.dec.sync.aligned.u32 56;");
-    } else {
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-        // ========================================================== softmax / accumulate / store (one row per thread)
-        const int g = (warp - 4) >> 2;
-        const int quarter = warp & 3;
-        const int row = quarter * 32 + lane;
-        const uint32_t lane_sel = static_cast<uint32_t>(quarter * 32) << 16;
-        const uint32_t tS = tmem + lane_sel + g * 128;
-        const uint32_t tO = tmem + lane_sel + 256 + g * 64;
-        const uint32_t tP = tmem + lane_sel + 384 + g * 64;
-        const float sc = p.scale_log2;
-        uint32_t cs = 0;                    // kv tiles this group has completed so far (all items)
-        AttnItem nxt = p.items[rng.x < rng.y ? rng.x : 0];       // descriptors are fetched one item ahead (ncu: 3 % of the samples sat on this load)
-        for (int it = rng.x; it < rng.y; ++it) {
-            const AttnItem item = nxt;
-            if (it + 1 < rng.y) nxt = p.items[it + 1];
-            const int nkv = (item.n + ATT_BKV - 1) / ATT_BKV;
-            if (g == 1 && !(item.q0 + ATT_BQ < item.n)) continue;       // this group's query tile lies past the image
-            const int qrow = item.q0 + g * ATT_BQ + row;
-            float m = -INFINITY;            // reference max of the exponent (may lag the true running max by < 2^8)
-            float l = 0.f;
-#ifdef MG_ATT_DEBUG
-            const long long dbg_loop0 = clock64();
-#endif
-            for (int j = 0; j < nkv; ++j) {
-                { ATT_T0(); mbar_wait(&s_full[g], (cs + j) & 1); ATT_ACC(dbg_a); }
-                tc_fence_after();
-                float v[ATT_BKV];
+        for (int j = 0; j < nkv; ++j) {
+            const int kv_left = item.n - j * ATT_BKV;
+            mbar_wait(&k_full[s], ph);
+            mbar_wait(&v_full[s], ph);
+            const uint32_t kaddr = smem_u32(sK + s * ATT_TILE_BYTES);
+            const uint32_t vaddr = smem_u32(sV + s * ATT_TILE_BYTES);
 #pragma unroll
-                for (int c = 0; c < ATT_BKV; c += 32) tmem_ld32(tS + c, v + c);
-                tc_wait_ld();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&s_free[g]);
-                const int kv_left = item.n - j * ATT_BKV;
+            for (int h = 0; h < 2; ++h) {
+                float sv[64];
+#pragma unroll
+                for (int i = 0; i < 64; ++i) sv[i] = 0.f;
+                wgmma_fence();
+                const uint64_t qd = make_sdesc_sw128(smem_u32(sQ + g * ATT_TILE_BYTES + h * 64 * 128));
+                const uint64_t kd = make_sdesc_sw128(kaddr);
+#pragma unroll
+                for (int k = 0; k < ATT_HD / 16; ++k) Wgmma<ATT_BKV, BF16>::ss(sv, qd + 2 * k, kd + 2 * k, 1u);
+                wgmma_commit();
+                wgmma_wait<0>();
+                reg_fence(sv);
                 if (kv_left < ATT_BKV) {                    // only the last tile has padding columns
 #pragma unroll
-                    for (int i = 0; i < ATT_BKV; ++i) v[i] = (i < kv_left) ? v[i] : -INFINITY;
+                    for (int i = 0; i < 64; ++i)
+                        if (8 * (i >> 2) + cq + (i & 1) >= kv_left) sv[i] = -INFINITY;
                 }
-                // four independent max chains (a single serial chain of 64 dependent FMNMX3 costs ~300 cycles per tile with only
-                // two softmax warps per scheduler to hide it)
-                float mx0 = fmax3(v[0], v[1], v[2]), mx1 = fmax3(v[3], v[4], v[5]), mx2 = fmax3(v[6], v[7], v[8]), mx3 = fmax3(v[9], v[10], v[11]);
+                // row max over the quad of lanes sharing a row
+                float mx[2] = {-INFINITY, -INFINITY};
 #pragma unroll
-                for (int i = 12; i + 7 < ATT_BKV; i += 8) {
-                    mx0 = fmax3(mx0, v[i], v[i + 1]); mx1 = fmax3(mx1, v[i + 2], v[i + 3]);
-                    mx2 = fmax3(mx2, v[i + 4], v[i + 5]); mx3 = fmax3(mx3, v[i + 6], v[i + 7]);
+                for (int i = 0; i < 64; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], sv[i]);
+                float alpha[2], mb[2];
+#pragma unroll
+                for (int r = 0; r < 2; ++r) {
+                    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+                    mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+                    const float m_new = fmaxf(m[h][r], mx[r]);
+                    alpha[r] = ex2_approx((m[h][r] - m_new) * sc);        // 0 on the first tile (m = -inf)
+                    m[h][r] = m_new;
+                    mb[r] = m_new * sc;
+                    l[h][r] *= alpha[r];
                 }
-                mx0 = fmax3(mx0, v[ATT_BKV - 4], v[ATT_BKV - 3]); mx1 = fmax3(mx1, v[ATT_BKV - 2], v[ATT_BKV - 1]);
-                const float mx = fmaxf(fmaxf(mx0, mx1), fmaxf(mx2, mx3));
-                const float m_new = fmaxf(m, mx);
-                const bool grow = (m_new - m) * sc > 8.0f;        // true on the first tile (m = -inf)
-                if (j > 0) {
-                    // PV(j-1) must have finished before P is overwritten (and before O is touched)
-                    { ATT_T0(); mbar_wait(&o_full[g], (cs + j - 1) & 1); ATT_ACC(dbg_b); }
-                    tc_fence_after();
-                    if (__any_sync(0xffffffffu, grow)) {
-                        const float alpha = grow ? ex2_approx((m - m_new) * sc) : 1.0f;
 #pragma unroll
-                        for (int c = 0; c < ATT_HD; c += 32) {
-                            float o[32];
-                            tmem_ld32(tO + c, o);
-                            tc_wait_ld();
+                for (int i = 0; i < 32; ++i) o[h][i] *= alpha[(i >> 1) & 1];
+                // P = 2^(S sc - m sc), packed to 16 bit in the A-operand fragment order of the P V MMA (k-step kk: columns 16 kk ..)
+                uint32_t pa[32];
 #pragma unroll
-                            for (int i = 0; i < 32; ++i) o[i] *= alpha;
-                            tmem_st32(tO + c, o);
-                        }
-                        tc_wait_st();
-                        l *= alpha;
-                    }
+                for (int i = 0; i < 64; i += 2) {
+                    const int r = (i >> 1) & 1;
+                    const float e0 = ex2_approx(fmaf(sv[i], sc, -mb[r])), e1 = ex2_approx(fmaf(sv[i + 1], sc, -mb[r]));
+                    l[h][r] += e0 + e1;
+                    pa[i >> 1] = H::pack(e0, e1);
                 }
-                if (grow) m = m_new;
-                const float mb = m * sc;
-                // exponent argument and row sum with packed 2 x fp32 instructions (FFMA2 / FADD2); of every 8 exponentials 5 go to
-                // MUFU.EX2 and 3 to the FMA-pipe polynomial (ATT_POLY pairs per 32-column chunk), interleaved so both pipes stay busy
-                const float2 sc2 = make_float2(sc, sc), nmb2 = make_float2(-mb, -mb);
-                float2 ls01 = make_float2(0.f, 0.f), ls23 = ls01;       // independent partial sums (no serial FADD chain)
+                wgmma_fence();
 #pragma unroll
-                for (int c = 0; c < ATT_BKV; c += 32) {
-                    uint32_t w[16];
-#pragma unroll
-                    for (int i = 0; i < 32; i += 4) {
-                        const float2 t0 = ffma2(make_float2(v[c + i], v[c + i + 1]), sc2, nmb2);
-                        const float2 t1 = ffma2(make_float2(v[c + i + 2], v[c + i + 3]), sc2, nmb2);
-                        // pair index within the chunk: 2 * (i / 4) and 2 * (i / 4) + 1; pairs listed in ATT_POLY_MASK use the polynomial
-                        const float2 e0 = ((ATT_POLY_MASK >> (i >> 1)) & 1) ? ex2_poly2(t0) : make_float2(ex2_approx(t0.x), ex2_approx(t0.y));
-                        const float2 e1 = ((ATT_POLY_MASK >> ((i >> 1) + 1)) & 1) ? ex2_poly2(t1) : make_float2(ex2_approx(t1.x), ex2_approx(t1.y));
-                        ls01 = fadd2(ls01, e0); ls23 = fadd2(ls23, e1);
-                        w[(i >> 1)] = H::pack(e0.x, e0.y); w[(i >> 1) + 1] = H::pack(e1.x, e1.y);
-                    }
-                    tmem_st16(tP + (c >> 1), w);
+                for (int kk = 0; kk < ATT_BKV / 16; ++kk) {
+                    // B: V tile [kv][hd], MN-major, 16 kv rows (= 2 groups of 8 x 128 B) per K-step
+                    const uint64_t vd = make_sdesc_sw128(vaddr + kk * 16 * 128, /*lbo=*/ATT_TILE_BYTES, /*sbo=*/1024);
+                    wgmma_rs_n64_tb<BF16>(o[h], pa + 4 * kk, vd, 1u);
                 }
-                l += (ls01.x + ls01.y) + (ls23.x + ls23.y);
-                tc_wait_st();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&p_full[g]);
+                wgmma_commit();
+                wgmma_wait<0>();
+                reg_fence(o[h]);
             }
-#ifdef MG_ATT_DEBUG
-            dbg_c += clock64() - dbg_loop0;
-            const long long dbg_ep0 = clock64();
-#endif
-            mbar_wait(&o_full[g], (cs + nkv - 1) & 1);
-            tc_fence_after();
-            cs += nkv;
-            const float inv = 1.0f / l;
+            __syncwarp();
+            if (lane == 0) { mbar_arrive(&k_empty[s]); mbar_arrive(&v_empty[s]); }
+            if (++s == ST) { s = 0; ph ^= 1; }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(q_empty);
 #pragma unroll
-            for (int c = 0; c < ATT_HD; c += 32) {
-                float o[32];
-                tmem_ld32(tO + c, o);
-                tc_wait_ld();
-                if (qrow < item.n) {
-                    uint4 q[4];
-                    uint32_t* qw = reinterpret_cast<uint32_t*>(q);
+        for (int h = 0; h < 2; ++h) {
 #pragma unroll
-                    for (int i = 0; i < 32; i += 2) qw[i >> 1] = H::pack(o[i] * inv, o[i + 1] * inv);
-                    uint4* dst = reinterpret_cast<uint4*>(static_cast<typename H::T*>(p.out) +
-                                                          (static_cast<size_t>(item.row0) + qrow) * p.D + item.head * ATT_HD + c);
-                    dst[0] = q[0]; dst[1] = q[1]; dst[2] = q[2]; dst[3] = q[3];
-                }
-                __syncwarp();
+            for (int r = 0; r < 2; ++r) {
+                l[h][r] += __shfl_xor_sync(0xffffffffu, l[h][r], 1);
+                l[h][r] += __shfl_xor_sync(0xffffffffu, l[h][r], 2);
             }
-            tc_fence_before();          // the O reads above are ordered before this group's next p_full arrive (first P V of the next item overwrites O)
-#ifdef MG_ATT_DEBUG
-            dbg_e += clock64() - dbg_ep0;
-#endif
+            const float inv[2] = {1.0f / l[h][0], 1.0f / l[h][1]};
+#pragma unroll
+            for (int r = 0; r < 2; ++r) {
+                const int qrow = item.q0 + g * ATT_BQ + h * 64 + r0 + 8 * r;
+                if (qrow >= item.n) continue;
+                typename H::T* dst = static_cast<typename H::T*>(p.out) + (static_cast<size_t>(item.row0) + qrow) * p.D + item.head * ATT_HD + cq;
+#pragma unroll
+                for (int c = 0; c < 8; ++c)
+                    *reinterpret_cast<uint32_t*>(dst + 8 * c) = H::pack(o[h][4 * c + 2 * r] * inv[r], o[h][4 * c + 2 * r + 1] * inv[r]);
+            }
         }
-#ifdef MG_ATT_DEBUG
-        if (warp == 4 && lane == 0) {
-            const long long now = clock64();
-            atomicAdd(&mg_att_dbg[0], (unsigned long long)dbg_a); atomicAdd(&mg_att_dbg[1], (unsigned long long)dbg_b);
-            atomicAdd(&mg_att_dbg[2], (unsigned long long)dbg_c); atomicAdd(&mg_att_dbg[5], (unsigned long long)(now - dbg_start));
-            atomicAdd(&mg_att_dbg[6], (unsigned long long)dbg_d);
-            atomicAdd(&mg_att_dbg[7], (unsigned long long)dbg_e);
-        }
-#endif
-    }
-#ifdef MG_ATT_DEBUG
-    if (warp == 1 && lane == 0) { atomicAdd(&mg_att_dbg[3], (unsigned long long)dbg_a); atomicAdd(&mg_att_dbg[4], (unsigned long long)dbg_b); }
-#endif
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem, 512);
     }
 }
 
@@ -445,12 +273,3 @@ int launch_attention(const CUtensorMap& mapQKV, void* out, const AttnItem* items
 }
 
 }  // namespace mg
-
-#ifdef MG_ATT_DEBUG
-extern "C" int mg_debug_att(unsigned long long* out, int reset) {
-    cudaDeviceSynchronize();
-    cudaMemcpyFromSymbol(out, mg::mg_att_dbg, sizeof(unsigned long long) * 8);
-    if (reset) { unsigned long long z[8] = {0}; cudaMemcpyToSymbol(mg::mg_att_dbg, z, sizeof(z)); }
-    return 0;
-}
-#endif

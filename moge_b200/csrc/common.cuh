@@ -1,6 +1,6 @@
-// moge_b200 device-side primitives for sm_100a: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (UMMA/TMEM).
-// Hand-written inline PTX; no CUTLASS/CuTe.  Bit layouts of the UMMA shared-memory and instruction
-// descriptors follow the PTX ISA "tcgen05 matrix descriptors" section.
+// moge_b200 device-side primitives for sm_90a: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
+// Hand-written inline PTX; no CUTLASS/CuTe.  The bit layout of the wgmma shared-memory descriptor follows the PTX ISA
+// "Matrix Descriptor Format" of the asynchronous warpgroup MMA section.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -8,6 +8,7 @@
 #include <cuda_bf16.h>
 #include <stdint.h>
 #include <stdio.h>
+#include "wgmma.cuh"
 
 namespace mg {
 
@@ -42,7 +43,7 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 __device__ __forceinline__ void fence_mbar_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
-// generic-proxy writes (st.shared) -> visible to the async proxy (TMA / UMMA operand reads)
+// generic-proxy writes (st.shared) -> visible to the async proxy (TMA / wgmma operand reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -64,12 +65,12 @@ __device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
     return ok != 0;
 }
 // Bounded wait: a broken pipeline traps (-> cudaErrorLaunchFailure on the host) instead of hanging the GPU.
-// (every failed try_wait suspends the thread for a system-dependent time, measured ~5 us on B200: 2^21 spins ~ 10 s, far beyond
-// any legitimate wait inside a millisecond kernel; 2^26 turned a deadlock into a 5-minute hang)
+// (every failed try_wait suspends the thread for a system-dependent time, up to microseconds: 2^21 spins are seconds, far beyond
+// any legitimate wait inside a millisecond kernel)
 #ifndef MG_WATCHDOG_SPINS
 #define MG_WATCHDOG_SPINS (1u << 21)
 #endif
-constexpr int kMaxDynSmem = 232448;       // 227 KB: the opt-in dynamic shared memory limit of one CTA on sm_100
+constexpr int kMaxDynSmem = 232448;       // 227 KB: the opt-in dynamic shared memory limit of one CTA on sm_90
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t spins = 0;
     while (!mbar_try_wait(bar, parity)) {
@@ -102,159 +103,38 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
         : "memory");
 }
 
-// ---------------------------------------------------------------------------------------- tcgen05/TMEM
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem, uint32_t ncols) {   // whole warp
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)),
-                 "r"(ncols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {     // whole warp (the allocating one)
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// mbarrier arrive when all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync)
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; fp16/bf16 operands, fp32 accumulate.  One thread issues.
-__device__ __forceinline__ void umma_f16(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                         uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// Same, with the A operand read from TENSOR MEMORY (M lanes x K 16-bit elements, two per 32-bit column) instead of smem.
-__device__ __forceinline__ void umma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-
-// Instruction descriptor for kind::f16: D fp32; A,B fp16 (fmt 0) or bf16 (fmt 1).
-//   [4,6) c_format=1(F32)  [7,10) a_format  [10,13) b_format  [15] a_major  [16] b_major (0 = K-major, 1 = MN-major)
-//   [17,23) N>>3   [24,29) M>>4
-__host__ __device__ constexpr uint32_t make_idesc(uint32_t M, uint32_t N, uint32_t fmt, uint32_t a_mn_major = 0,
-                                                  uint32_t b_mn_major = 0) {
-    return (1u << 4) | (fmt << 7) | (fmt << 10) | (a_mn_major << 15) | (b_mn_major << 16) | ((N >> 3) << 17) |
-           ((M >> 4) << 24);
-}
-
-// Shared-memory matrix descriptor, 128-byte swizzle, 8-row groups 1024 B apart (dense [rows][64 x 16-bit] tiles as
-// written by a SWIZZLE_128B TMA box with a 128-byte inner extent).  Tile base must be 1024-byte aligned.
-//   [0,14) addr>>4   [16,30) LBO>>4   [32,46) SBO>>4   [46,48) version=1   [61,64) layout=2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr, uint32_t lbo_bytes = 16,
-                                                     uint32_t sbo_bytes = 1024) {
+// ------------------------------------------------------------------------------------------------ wgmma
+// Shared-memory matrix descriptor (sm_90 wgmma), 128-byte swizzle: dense [rows][64 x 16-bit] tiles as written by a SWIZZLE_128B
+// TMA box with a 128-byte inner extent, 8-row groups `sbo_bytes` apart.  Tile base must be 1024-byte aligned.
+//   [0,14) addr>>4   [16,30) LBO>>4   [32,46) SBO>>4   [62,64) layout=1 (SWIZZLE_128B)
+// K-major operands advance 16 elements (32 bytes) along K by adding 2 to the descriptor.
+__device__ __forceinline__ uint64_t make_sdesc_sw128(uint32_t smem_addr, uint32_t lbo_bytes = 16, uint32_t sbo_bytes = 1024) {
     uint64_t d = 0;
     d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
     d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
     d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= static_cast<uint64_t>(1) << 46;
-    d |= static_cast<uint64_t>(2) << 61;
+    d |= static_cast<uint64_t>(1) << 62;
     return d;
 }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accesses of the accumulator registers across a wgmma wait
+template <int N> __device__ __forceinline__ void reg_fence(float (&r)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+// named barrier over `count` threads (the consumer warpgroups of a CTA; id 0 is __syncthreads)
+__device__ __forceinline__ void named_sync(uint32_t id, uint32_t count) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(count) : "memory");
+}
+template <uint32_t R> __device__ __forceinline__ void regs_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+template <uint32_t R> __device__ __forceinline__ void regs_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 
-// TMEM -> registers: this warp's 32 lanes x N consecutive 32-bit columns; thread i <- lane (base+i).
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t* r = reinterpret_cast<uint32_t*>(v);
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-}
-
-// registers -> TMEM (this warp's 32 lanes x 32 consecutive columns)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-    const uint32_t* r = reinterpret_cast<const uint32_t*>(v);
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-// registers -> TMEM, 16 consecutive 32-bit columns (e.g. 32 packed 16-bit values of this thread's row)
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-        : "memory");
-}
-__device__ __forceinline__ float tmem_ld1(uint32_t taddr) {
-    uint32_t r;
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(r) : "r"(taddr) : "memory");
-    return __uint_as_float(r);
-}
-__device__ __forceinline__ void tmem_st1(uint32_t taddr, float v) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(__float_as_uint(v)) : "memory");
-}
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// Packed 2 x fp32 arithmetic (Blackwell FFMA2 / FADD2): one issue slot and one fma-pipe pass for two lanes of work.
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-    unsigned long long ra, rb, rc, rd;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-    float2 d;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-    return d;
-}
-__device__ __forceinline__ float2 fadd2(float2 a, float2 b) {
-    unsigned long long ra, rb, rd;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-    asm("add.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-    float2 d;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-    return d;
-}
-
-__device__ __forceinline__ float2 fmul2(float2 a, float2 b) {
-    unsigned long long ra, rb, rd;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-    asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-    float2 d;
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-    return d;
-}
+// Two lanes of fp32 arithmetic (sm_90 has no packed fp32 instructions: one FFMA / FADD / FMUL per lane).
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
+__device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
+__device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 
 __device__ __forceinline__ float fmax3(float a, float b, float c) {
     float r;

@@ -1,23 +1,7 @@
-// conv64_kernel instantiations + launcher.
-#include "conv64_kernel.cuh"
-#include "host_api.h"
-#include <cstdlib>
+// umma_kernel<MODE_CONV64> instantiations + launcher: 3x3 convs with C_in = 64, resident weights (umma_kernel.cuh).
+#include "umma_launch.cuh"
 
 namespace mg {
-
-template <int BN, int EPI, bool BF16, int DF, int MW>
-static int launch_inst(const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& w, const UmmaParams& p, int num_sms, cudaStream_t st) {
-    using Cfg = Conv64Cfg<BN, MW>;
-    if (MW == 2 && p.kb_aux != 0) return set_error("conv64: the two-issuer form has no aux stage");
-    auto kern = conv64_kernel<BN, EPI, BF16, DF, MW>;
-    MG_SET_SMEM_ONCE(kern, Cfg::kSmemBytes);
-    const int nnt = p.num_n_tiles;
-    int grid = (num_sms / nnt) * nnt;
-    if (p.num_m_tiles * nnt < grid) grid = p.num_m_tiles * nnt;
-    if (grid <= 0) return 0;
-    CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(Cfg::kThreads), Cfg::kSmemBytes, st, a, aux, w, p));
-    return 0;
-}
 
 int launch_conv64(int bn, int epi, bool bf16, const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& w, const UmmaParams& p,
                   int num_sms, cudaStream_t st) {
@@ -27,17 +11,10 @@ int launch_conv64(int bn, int epi, bool bf16, const CUtensorMap& a, const CUtens
     // anything else runs the generic run-time-flag variant.
     int df = -1;
     if (epi == EPI_DEC) df = (p.out0 ? DF_RAW : 0) | (p.out1 ? DF_RELU : 0) | (p.skip ? DF_SKIP : 0) | (p.vec1 ? DF_UV : 0) | (p.shuffle ? DF_SHUFFLE : 0);
-    // two MMA-issuing warps (alternate tiles) unless the tile has the extra 1x1 aux stage (conv64_kernel.cuh); MOGE_B200_C64_MMA2=0
-    // forces the single-issuer form for A/B runs
-    static const bool mma2_on = [] { const char* v = getenv("MOGE_B200_C64_MMA2"); return !(v != nullptr && v[0] == '0'); }();
-    const bool mma2 = mma2_on && p.kb_aux == 0;
-#define INST1(BN, EPI, DFV, MW)                                                                                  \
-        return bf16 ? launch_inst<BN, EPI, true, DFV, MW>(a, aux, w, p, num_sms, st) : launch_inst<BN, EPI, false, DFV, MW>(a, aux, w, p, num_sms, st);
 #define INST(BN, EPI, DFV)                                                                                       \
-    if (bn == BN && epi == EPI && df == (DFV)) {                                                                 \
-        if (mma2) { INST1(BN, EPI, DFV, 2) }                                                                     \
-        INST1(BN, EPI, DFV, 1)                                                                                   \
-    }
+    if (bn == BN && epi == EPI && df == (DFV))                                                                   \
+        return bf16 ? launch_umma_inst<BN, MODE_CONV64, AMODE_TILES, EPI, true, DFV>(a, aux, w, p, num_sms, st)  \
+                    : launch_umma_inst<BN, MODE_CONV64, AMODE_TILES, EPI, false, DFV>(a, aux, w, p, num_sms, st);
     INST(64, EPI_DEC, DF_RELU)
     INST(64, EPI_DEC, DF_RAW | DF_SKIP)
     INST(64, EPI_DEC, DF_RAW | DF_RELU | DF_SKIP)
@@ -49,17 +26,7 @@ int launch_conv64(int bn, int epi, bool bf16, const CUtensorMap& a, const CUtens
     INST(16, EPI_HEADOUT, -1)
     INST(32, EPI_NECKOUT, -1)
 #undef INST
-#undef INST1
     return set_error("no conv64 instantiation for bn=%d epi=%d", bn, epi);
 }
 
 }  // namespace mg
-
-#ifdef MG_C64_DEBUG
-extern "C" int mg_debug_c64(unsigned long long* out, int reset) {
-    cudaDeviceSynchronize();
-    cudaMemcpyFromSymbol(out, mg::mg_c64_dbg, sizeof(unsigned long long) * 8);
-    if (reset) { unsigned long long z[8] = {0}; cudaMemcpyToSymbol(mg::mg_c64_dbg, z, sizeof(z)); }
-    return 0;
-}
-#endif

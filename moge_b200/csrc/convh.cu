@@ -1,23 +1,10 @@
-// convh_kernel instantiations + launcher.
-#include "convh_kernel.cuh"
-#include "host_api.h"
+// umma_kernel<MODE_CONVH> instantiations + launcher: 3x3 convs with C_in >= 128, halo boxes + streamed weights (umma_kernel.cuh).
+#include "umma_launch.cuh"
 
 namespace mg {
 
-template <int BN, bool BF16, int DF>
-static int launch_inst(const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& w, const UmmaParams& p, int num_sms, cudaStream_t st) {
-    using Cfg = ConvhCfg<BN>;
-    auto kern = convh_kernel<BN, BF16, DF>;
-    MG_SET_SMEM_ONCE(kern, Cfg::kSmemBytes);
-    const int tiles = p.num_m_tiles * p.num_n_tiles;
-    if (tiles <= 0) return 0;
-    const int grid = tiles < num_sms ? tiles : num_sms;
-    CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(Cfg::kThreads), Cfg::kSmemBytes, st, a, aux, w, p));
-    return 0;
-}
-
 bool convh_supports(int bn, const UmmaParams& p) {
-    if (p.ntaps != 9 || p.kb_main < 1 || (bn != 128 && bn != 256) || p.N % bn) return false;
+    if (p.ntaps != 9 || p.kb_main < 1 || bn != 128 || p.N % bn) return false;      // 256-wide stages do not fit beside the tile
     const int df = (p.out0 ? DF_RAW : 0) | (p.out1 ? DF_RELU : 0) | (p.skip ? DF_SKIP : 0) | (p.vec1 ? DF_UV : 0) | (p.shuffle ? DF_SHUFFLE : 0);
     return df == DF_RELU || df == (DF_RAW | DF_SKIP) || df == (DF_RAW | DF_RELU | DF_SKIP) || df == (DF_RAW | DF_RELU) ||
            df == (DF_RAW | DF_RELU | DF_UV);
@@ -29,17 +16,13 @@ int launch_convh(int bn, bool bf16, const CUtensorMap& a, const CUtensorMap& aux
     const int df = (p.out0 ? DF_RAW : 0) | (p.out1 ? DF_RELU : 0) | (p.skip ? DF_SKIP : 0) | (p.vec1 ? DF_UV : 0) | (p.shuffle ? DF_SHUFFLE : 0);
 #define INST(BN, DFV)                                                                                            \
     if (bn == BN && df == (DFV))                                                                                 \
-        return bf16 ? launch_inst<BN, true, DFV>(a, aux, w, p, num_sms, st) : launch_inst<BN, false, DFV>(a, aux, w, p, num_sms, st);
+        return bf16 ? launch_umma_inst<BN, MODE_CONVH, AMODE_TILES, EPI_DEC, true, DFV>(a, aux, w, p, num_sms, st)        \
+                    : launch_umma_inst<BN, MODE_CONVH, AMODE_TILES, EPI_DEC, false, DFV>(a, aux, w, p, num_sms, st);
     INST(128, DF_RELU)
     INST(128, DF_RAW | DF_SKIP)
     INST(128, DF_RAW | DF_RELU | DF_SKIP)
     INST(128, DF_RAW | DF_RELU)
     INST(128, DF_RAW | DF_RELU | DF_UV)
-    INST(256, DF_RELU)
-    INST(256, DF_RAW | DF_SKIP)
-    INST(256, DF_RAW | DF_RELU | DF_SKIP)
-    INST(256, DF_RAW | DF_RELU)
-    INST(256, DF_RAW | DF_RELU | DF_UV)
 #undef INST
     return set_error("no convh instantiation for bn=%d df=%d", bn, df);
 }

@@ -82,7 +82,7 @@ int launch_preprocess(const void* image, int image_dtype, int B, int H, int W, i
                       bool bf16, cudaStream_t st) {
     const size_t total = static_cast<size_t>(B) * h * w * Kp;
     const int threads = 256;
-    const int blocks = static_cast<int>(std::min<size_t>((total + threads - 1) / threads, 148 * 16));
+    const int blocks = static_cast<int>(std::min<size_t>((total + threads - 1) / threads, 132 * 16));
     if (bf16) CUDA_TRY(launch_pdl(preprocess_kernel<true>, dim3(blocks), dim3(threads), 0, st, image, image_dtype, B, H, W, h, w, static_cast<__nv_bfloat16*>(patches), Kp));
     else CUDA_TRY(launch_pdl(preprocess_kernel<false>, dim3(blocks), dim3(threads), 0, st, image, image_dtype, B, H, W, h, w, static_cast<__half*>(patches), Kp));
     CUDA_TRY(cudaGetLastError());
@@ -166,8 +166,8 @@ int launch_init_cls(float* x, const float* cls_row, int B, int N, int D, cudaStr
 //   with  W' = W diag(gamma),  W'' = W' (I - 1 1^T / D)  (every row of W' centred: the mean removal is a linear map and lives
 //   in the weight),  b' = b + W beta.
 // The GEMM consumes the ROUNDED residual rows x16 directly and its epilogue only scales by rstd[row] and adds b' -- the same
-// instruction count as a plain bias epilogue (these epilogues run neck and neck with the MMAs: an explicit rank-1 mean
-// correction in the epilogue measured +30 % on the qkv / fc1 GEMMs).  rstd comes from per-row partial sums (sum, sum of squares
+// instruction count as a plain bias epilogue (an explicit rank-1 mean correction would add work to every output element of the
+// qkv / fc1 GEMMs).  rstd comes from per-row partial sums (sum, sum of squares
 // of the rounded values) that the producing epilogue (patch embed, proj, fc2) writes next to x16, reduced by ln_rstd_kernel.
 // Rounding W'' to 16 bit leaves a column-sum residual of ~sqrt(D) * 2^-11 * |W''|: the mean is removed to that relative
 // precision, which is below the 16-bit rounding of the activations for |mu| <~ 10 sigma.
@@ -422,7 +422,7 @@ int launch_head_output(const float4* pts_lr, const float4* nrm_lr, const float* 
                        int remap_mode, float* points, float* normal, float* mask, cudaStream_t st) {
     const size_t total = static_cast<size_t>(B) * H * W;
     const int threads = 256;
-    const int blocks = static_cast<int>(std::min<size_t>((total + threads - 1) / threads, 148 * 16));
+    const int blocks = static_cast<int>(std::min<size_t>((total + threads - 1) / threads, 132 * 16));
     CUDA_TRY(launch_pdl(head_output_kernel, dim3(blocks), dim3(threads), 0, st, pts_lr, nrm_lr, msk_lr, B, Hl, Wl, H, W, remap_mode, points, normal, mask));
     CUDA_TRY(cudaGetLastError());
     return 0;
@@ -699,7 +699,7 @@ int launch_postprocess(float* points, const float* normal_in, const float* mask_
                        const float* focal, const float* shift, int B, int H, int W, int force_projection, int apply_mask,
                        float* depth, float* normal_out, uint8_t* mask_out, float* intrinsics, cudaStream_t st) {
     const size_t npix = static_cast<size_t>(H) * W;
-    dim3 grid(static_cast<unsigned>(std::min<size_t>((npix + 255) / 256, 148 * 8)), B);
+    dim3 grid(static_cast<unsigned>(std::min<size_t>((npix + 255) / 256, 132 * 8)), B);
     CUDA_TRY(launch_pdl(postprocess_kernel, grid, dim3(256), 0, st, points, normal_in, mask_prob, metric_scale, focal, shift, H, W, force_projection,
                         apply_mask, depth, normal_out, mask_out, intrinsics));
     return 0;

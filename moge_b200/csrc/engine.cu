@@ -120,7 +120,7 @@ using namespace mg;
 
 struct moge_engine {
     moge_config_t cfg;
-    int device = 0, num_sms = 148;
+    int device = 0, num_sms = 132;
     bool bf16 = false, finalized = false;
     std::map<std::string, RawWeight> raw;
     std::vector<void*> owned;         // cudaMalloc'd, freed at destroy
@@ -142,7 +142,6 @@ struct moge_engine {
     Plan* last_plan = nullptr;
     std::vector<void*> temps;         // load-time scratch (fp32 folds), freed at the end of finalize
     bool use_graphs = true;
-    bool use_2cta = false;
     bool neck_fold = false;       // last neck level folded through the heads (EPI_NECKOUT); decided at finalize
     bool ln_fold = true;          // LayerNorm folded into qkv / fc1 (SURVEY K4/K7); MOGE_B200_LNFOLD=0: separate layernorm kernel
     cudaStream_t own_stream = nullptr;
@@ -549,7 +548,7 @@ static int add_conv(moge_engine* e, Plan* pl, const ConvW& cw, const void* src, 
     int bn;
     if (epi == EPI_HEADOUT) bn = 16;
     else if (epi == EPI_NECKOUT) bn = 32;
-    else bn = pick_bn(cw.N, {256, 128, 64, 32});
+    else bn = pick_bn(cw.N, {128, 64, 32});
     if (!bn) return set_error("conv: N=%d has no tile width", cw.N);
     p.num_n_tiles = cw.N / bn;
     p.out0 = out_raw; p.out1 = out_relu; p.bias = cw.bias;
@@ -567,7 +566,7 @@ static int add_conv(moge_engine* e, Plan* pl, const ConvW& cw, const void* src, 
     else if (epi == EPI_NECKOUT) bytes += 4 * px * ((out_raw ? 16 : 0) + (out_relu ? 16 : 0) + (out2 ? 4 : 0));
     else bytes += px * cw.N * 2 * ((out_raw ? 1 : 0) + (out_relu ? 1 : 0)) + (skip ? px * cw.N * 2 : 0);
     CUtensorMap ma, mx, mb;
-    // C_in = 64 3x3 convs (levels 3/4): resident weights + one halo box per horizontal tap (conv64_kernel.cuh)
+    // C_in = 64 3x3 convs (levels 3/4): resident weights + one halo box per horizontal tap (umma_kernel<MODE_CONV64>)
     const bool use64 = cw.taps == 9 && cw.cin == 64 && (cw.caux == 0 || cw.caux == 64) && gs.Hp >= 10 &&
                        ((epi == EPI_HEADOUT && cw.N == 16) || (epi == EPI_NECKOUT && cw.N == 32) || (epi == EPI_DEC && cw.N % 64 == 0));
     if (use64) {
@@ -580,10 +579,10 @@ static int add_conv(moge_engine* e, Plan* pl, const ConvW& cw, const void* src, 
         pl->ops.add([=](cudaStream_t st) { return launch_conv64(bn64, epi, bf16, ma, mx, mb, p, sms, st); }, name, flops, bytes);
         return 0;
     }
-    // C_in >= 128 3x3 convs (levels 1/2): halo boxes for the pixels + streamed weights (convh_kernel.cuh); MOGE_B200_CONVH=0 disables, =1 restricts it to 128-wide tiles
+    // C_in >= 128 3x3 convs (levels 1/2): halo boxes for the pixels + streamed weights (umma_kernel<MODE_CONVH>); MOGE_B200_CONVH=0 disables
     static const int convh_mode = [] { const char* v = getenv("MOGE_B200_CONVH"); return v ? atoi(v) : 2; }();
     const bool useh = convh_mode != 0 && epi == EPI_DEC && cw.taps == 9 && cw.cin >= 128 && cw.cin % 64 == 0 && cw.caux % 64 == 0 &&
-                      gs.Hp >= 10 && (bn == 128 || (bn == 256 && convh_mode >= 2)) && convh_supports(bn, p);
+                      gs.Hp >= 10 && convh_supports(bn, p);
     if (useh) {
         MG_TRY(make_map_nhwc(&ma, src, cw.cin, gs.Wp, gs.Hp, B, 10));
         if (cw.caux) MG_TRY(make_map_nhwc(&mx, aux, cw.caux, gs.Wp, gs.Hp, B, 8));
@@ -613,10 +612,8 @@ static int add_linear(moge_engine* e, Plan* pl, const void* A, int M, int K, int
     UmmaParams p{};
     p.M = M; p.N = N; p.ntaps = 1; p.kb_main = (K + 63) / 64; p.kb_aux = 0;
     p.num_m_tiles = (M + TILE_M - 1) / TILE_M;
-    int bn = pick_bn(N, {256, 128});
+    int bn = pick_bn(N, {128});
     if (!bn) return set_error("linear: N=%d must be a multiple of 128", N);
-    // small batches: when 128x256 tiles cannot fill the SMs, halve the tile width (N = 128 MMAs still run at N/2 cycles)
-    if (bn == 256 && p.num_m_tiles * (N / 256) * 4 < e->num_sms * 3) bn = 128;
     if (force_bn) bn = force_bn;
     if (bn_out) *bn_out = bn;
     p.num_n_tiles = N / bn;
@@ -636,26 +633,6 @@ static int add_linear(moge_engine* e, Plan* pl, const void* A, int M, int K, int
     CUtensorMap ma, mb;
     MG_TRY(make_map_2d(&ma, A, K, M, lda, TILE_M));
     const bool bf16 = e->bf16; const int sms = e->num_sms;
-    const double flops2 = 2.0 * M * static_cast<double>(N) * K;
-    if (bn == 256 && e->use_2cta && (epi == EPI_STORE16 || epi == EPI_GELU16 || epi == EPI_RESID)) {
-        MG_TRY(make_map_2d(&mb, W, K, N, lda, 128));
-        double bytes2 = static_cast<double>(M) * K * 2 + static_cast<double>(N) * K * 2 + ((epi == EPI_RESID) ? static_cast<double>(M) * N * 8 : static_cast<double>(M) * N * 2) + ln_extra_bytes;
-        // EPI_RESID with a short reduction (proj: K = D): the fp32 residual is staged through shared memory by TMA, two 32 x 32
-        // chunks per epilogue warp ahead of their use, in place of two of the six ring stages -- same-box A/B: proj 3.38 -> 3.03 ms
-        // per step.  fc2 (K = 4 D) keeps the six-stage ring and reads the residual from global memory: with four stages it loses
-        // more in the main loop than the staging wins (6.93 -> 7.77 ms).  MOGE_B200_RESID_TMA=0 disables the staging.
-        static const bool resid_tma = [] { const char* v = getenv("MOGE_B200_RESID_TMA"); return !(v != nullptr && v[0] == '0'); }();
-        static const bool resid_tma_long = [] { const char* v = getenv("MOGE_B200_RESID_TMA_LONGK"); return v != nullptr && v[0] == '1'; }();
-        if (epi == EPI_RESID && resid_tma && (N % 32) == 0 && (K <= N || resid_tma_long)) {
-            CUtensorMap mr;
-            MG_TRY(make_map_2d_f32(&mr, out, N, M, ldo));
-            const int nbuf = (K <= N) ? 2 : 1;
-            pl->ops.add([=](cudaStream_t st) { return launch_umma2(epi, bf16, ma, mb, p, sms, st, &mr, nbuf); }, name, flops2, bytes2);
-            return 0;
-        }
-        pl->ops.add([=](cudaStream_t st) { return launch_umma2(epi, bf16, ma, mb, p, sms, st); }, name, flops2, bytes2);
-        return 0;
-    }
     MG_TRY(make_map_2d(&mb, W, K, N, lda, bn));
     const double flops = 2.0 * M * static_cast<double>(N) * K;
     double bytes = static_cast<double>(M) * K * 2 + static_cast<double>(N) * K * 2;
@@ -810,11 +787,9 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     // ---- per group: K1 resize + normalise + patchify (phase 0: reads the caller's image), K2/K3 patch embed + pos embed, cls rows
     int parts_x = 0;              // column groups per row of the statistics the NEXT consumer reads
     int bn_patch = 0;
-    {   // one tile width for every group's patch-embed GEMM (the statistics layout must agree): chosen from the total row count
-        const int mt = static_cast<int>((TT + TILE_M - 1) / TILE_M);
-        bn_patch = pick_bn(D, {256, 128});
+    {   // one tile width for every group's patch-embed GEMM (the statistics layout must agree)
+        bn_patch = pick_bn(D, {128});
         if (!bn_patch) return set_error("embed_dim=%d must be a multiple of 128", D);
-        if (bn_patch == 256 && mt * (D / 256) * 4 < sms * 3) bn_patch = 128;
     }
     long prow = 0;                // first patch row of the group in `patches` / `taps`
     std::vector<long> prow0(G);
@@ -937,7 +912,7 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
             p.M = B * T; p.N = f.N; p.ntaps = 1; p.kb_main = f.Ktot / 64; p.kb_aux = 0;
             if (f.Ktot % 64) return set_error("num_taps*embed_dim must be a multiple of 64");
             p.num_m_tiles = (p.M + TILE_M - 1) / TILE_M;
-            const int bn = pick_bn(f.N, {256, 128});
+            const int bn = pick_bn(f.N, {128});
             if (!bn) return set_error("neck width %d must be a multiple of 128", f.N);
             p.num_n_tiles = f.N / bn;
             p.B = B; p.H = h; p.W = w; p.T = T;
@@ -1066,7 +1041,7 @@ static int validate_cfg(const moge_config_t& c) {
 extern "C" {
 
 const char* moge_last_error(void) { return mg::last_error(); }
-const char* moge_version(void) { return "moge_b200 0.1.0 sm_100a"; }
+const char* moge_version(void) { return "moge_b200 0.1.0 sm_90a"; }
 
 int moge_engine_create(const moge_config_t* cfg, int device, moge_engine_t** out) {
     if (!cfg || !out) return set_error("null argument");
@@ -1076,13 +1051,11 @@ int moge_engine_create(const moge_config_t* cfg, int device, moge_engine_t** out
     CUDA_TRY(cudaSetDevice(device));
     cudaDeviceProp prop;
     CUDA_TRY(cudaGetDeviceProperties(&prop, device));
-    if (prop.major != 10) return set_error("device %d is sm_%d%d; libmoge_b200 contains sm_100a code only", device, prop.major, prop.minor);
+    if (prop.major != 9 || prop.minor != 0) return set_error("device %d is sm_%d%d; libmoge_b200 contains sm_90a code only", device, prop.major, prop.minor);
     moge_engine* e = new moge_engine();
     e->cfg = *cfg; e->device = device; e->num_sms = prop.multiProcessorCount; e->bf16 = cfg->compute_dtype == MOGE_BF16;
     const char* env = getenv("MOGE_B200_GRAPHS");
     e->use_graphs = !(env && env[0] == '0');
-    const char* env2 = getenv("MOGE_B200_2CTA");
-    e->use_2cta = !(env2 != nullptr && env2[0] == '0');
     const char* env3 = getenv("MOGE_B200_LNFOLD");
     e->ln_fold = !(env3 != nullptr && env3[0] == '0');
     if (cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
@@ -1119,7 +1092,7 @@ int moge_engine_set_weight(moge_engine_t* e, const char* key, const void* dev_pt
     for (int i = 0; i < ndim; ++i) { rw.shape.push_back(shape[i]); rw.numel *= static_cast<size_t>(shape[i]); }
     // squeeze leading singleton dims of parameter-like tensors so shape checks see the logical shape
     CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&rw.p), std::max<size_t>(rw.numel, 4) * 4));
-    const int blocks = static_cast<int>(std::min<size_t>((rw.numel + 255) / 256, 148 * 8));
+    const int blocks = static_cast<int>(std::min<size_t>((rw.numel + 255) / 256, 132 * 8));
     to_f32_kernel<<<std::max(blocks, 1), 256, 0, static_cast<cudaStream_t>(stream)>>>(dev_ptr, dtype, rw.p, rw.numel);
     CUDA_TRY(cudaGetLastError());
     auto it = e->raw.find(key);
@@ -1293,13 +1266,8 @@ int moge_postprocess(float* points, const float* normal_in, const float* mask_pr
 }
 
 // ---------------------------------------------------------------------------------- operator-level entry points
-static bool use_2cta() {
-    const char* v = getenv("MOGE_B200_2CTA");      // default on; MOGE_B200_2CTA=0 falls back to the 1-CTA kernel
-    return !(v != nullptr && v[0] == '0');
-}
-
 static int dev_sms() {
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     return sms;
@@ -1308,7 +1276,7 @@ static int dev_sms() {
 int moge_op_linear(const void* x, const void* w, const float* bias, const float* gamma, void* out, int M, int N, int K, int epi,
                    int dtype, void* stream) {
     if (K % 8) return set_error("op_linear: K must be a multiple of 8");
-    const int bn = pick_bn(N, {256, 128});
+    const int bn = pick_bn(N, {128});
     if (!bn) return set_error("op_linear: N must be a multiple of 128");
     if (epi < 0 || epi > 2) return set_error("op_linear: epi must be 0..2");
     UmmaParams p{};
@@ -1317,10 +1285,6 @@ int moge_op_linear(const void* x, const void* w, const float* bias, const float*
     p.out0 = out; p.bias = bias; p.vec1 = gamma; p.ldo = N;
     CUtensorMap ma, mb;
     MG_TRY(make_map_2d(&ma, x, K, M, K, TILE_M));
-    if (bn == 256 && use_2cta()) {
-        MG_TRY(make_map_2d(&mb, w, K, N, K, 128));
-        return launch_umma2(epi, dtype == MOGE_BF16, ma, mb, p, dev_sms(), static_cast<cudaStream_t>(stream));
-    }
     MG_TRY(make_map_2d(&mb, w, K, N, K, bn));
     return launch_umma(bn, AMODE_ROWS, epi, dtype == MOGE_BF16, ma, ma, mb, p, dev_sms(), static_cast<cudaStream_t>(stream));
 }
@@ -1378,7 +1342,7 @@ int moge_op_linear_ln(const float* x, const float* ln_gamma, const float* ln_bet
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const bool bf16 = dtype == MOGE_BF16;
     if (K % 64) return set_error("op_linear_ln: K must be a multiple of 64");
-    const int bn = pick_bn(N, {256, 128});
+    const int bn = pick_bn(N, {128});
     if (!bn) return set_error("op_linear_ln: N must be a multiple of 128");
     if (epi != EPI_STORE16 && epi != EPI_GELU16) return set_error("op_linear_ln: epi must be 0 (store) or 1 (GELU)");
     void *x16 = nullptr, *w16 = nullptr;
@@ -1400,10 +1364,7 @@ int moge_op_linear_ln(const float* x, const float* ln_gamma, const float* ln_bet
         p.ln_rstd = rstd;
         CUtensorMap ma, mb;
         rc = make_map_2d(&ma, x16, K, M, K, TILE_M);
-        if (rc == 0 && bn == 256 && use_2cta()) {
-            rc = make_map_2d(&mb, w16, K, N, K, 128);
-            if (rc == 0) rc = launch_umma2(epi, bf16, ma, mb, p, dev_sms(), st);
-        } else if (rc == 0) {
+        if (rc == 0) {
             rc = make_map_2d(&mb, w16, K, N, K, bn);
             if (rc == 0) rc = launch_umma(bn, AMODE_ROWS, epi, bf16, ma, ma, mb, p, dev_sms(), st);
         }
@@ -1425,7 +1386,7 @@ int moge_op_conv(const void* x, const float* w, const float* bias, const void* s
     if (taps != 1 && taps != 9) return set_error("op_conv: taps must be 1 or 9");
     if (shuffle && taps != 1) return set_error("op_conv: shuffle requires taps=1");
     const int N = shuffle ? 4 * Cout : Cout;
-    const int bn = pick_bn(N, {256, 128, 64, 32});
+    const int bn = pick_bn(N, {128, 64, 32});
     if (!bn) return set_error("op_conv: Cout must be a multiple of 32");
     const int Ktot = taps * Cin;
     void* wp = nullptr;
@@ -1449,7 +1410,7 @@ int moge_op_conv(const void* x, const float* w, const float* bias, const void* s
             if (rc == 0) rc = make_map_2d(&mb, wp, Ktot, N, Ktot, 64);
             if (rc == 0) rc = launch_conv64(64, EPI_DEC, bf16, ma, ma, mb, p, dev_sms(), st);
         } else if (taps == 9 && Cin >= 128 && gs.Hp >= 10 && convh_supports(bn, p) &&
-                   [&] { const char* v = getenv("MOGE_B200_CONVH"); const int m = v ? atoi(v) : 2; return m != 0 && (bn == 128 || m >= 2); }()) {
+                   [] { const char* v = getenv("MOGE_B200_CONVH"); return v == nullptr || atoi(v) != 0; }()) {
             rc = make_map_nhwc(&ma, x, Cin, gs.Wp, gs.Hp, B, 10);
             if (rc == 0) rc = make_map_2d(&mb, wp, Ktot, N, Ktot, bn);
             if (rc == 0) rc = launch_convh(bn, bf16, ma, ma, mb, p, dev_sms(), st);

@@ -52,10 +52,9 @@ struct DevOnce {
 // griddepcontrol.launch_dependents, then griddepcontrol.wait) and is launched with programmatic stream serialization, so the NEXT
 // kernel's launch, block scheduling and prologue overlap the tail of this one instead of waiting for the full drain of the grid;
 // correctness is unchanged (the wait returns only when the predecessor grid has completed and flushed).  It matters at batch 1,
-// where a forward is ~245 kernels of a few microseconds each (also inside the captured CUDA graph): measured 3.554 -> 3.515 ms p50.
-// At batch 32 the kernels are long and early-resident dependents only get in the way (same-box A/B: 50.2 -> 51.0 ms per step), so
-// the engine switches it on per call, for the small (graph-replayed) calls only: `pdl_scope` is thread-local state read by
-// `launch_pdl`.  MOGE_B200_PDL=0 disables it altogether.
+// where a forward is ~245 kernels of a few microseconds each (also inside the captured CUDA graph).  At large batches the kernels
+// are long and early-resident dependents only get in the way, so the engine switches it on per call, for the small
+// (graph-replayed) calls only: `pdl_scope` is thread-local state read by `launch_pdl`.  MOGE_B200_PDL=0 disables it altogether.
 bool pdl_enabled();
 bool& pdl_scope();
 template <typename... KArgs, typename... Args>
@@ -73,26 +72,19 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
 // 16-bit element maps with a 64-element (128-byte) inner box and SWIZZLE_128B.
 int make_map_2d(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint64_t row_pitch_elems, uint32_t box_rows);
 int make_map_3d(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint64_t batch, uint32_t box_rows);
-// fp32 row-major matrix: box {32 columns (128 bytes), 32 rows}, SWIZZLE_128B (the residual stream of the EPI_RESID epilogue)
-int make_map_2d_f32(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint64_t row_pitch_elems);
 // padded NHWC image [B, Hp, Wp, C]: box {64 ch, 16 px, 8 rows, 1}
 int make_map_nhwc(CUtensorMap* m, const void* base, uint64_t C, uint64_t Wp, uint64_t Hp, uint64_t B, uint32_t box_rows = 8);
 
 struct UmmaParams;
-// bn in {16,32,64,128,256}; amode/epi as in umma_kernel.cuh
+// bn in {16,32,64,128}; amode/epi as in umma_kernel.cuh
 int launch_umma(int bn, int amode, int epi, bool bf16, const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& b,
                 const UmmaParams& p, int num_sms, cudaStream_t st);
 
-// 2-CTA (cta_group::2) encoder GEMM, 256x256 pair tiles; a, b: box {64,128}
-// `resid`: EPI_RESID only -- fp32 map of the residual matrix (out0); non-null: the epilogue stages the residual through shared memory
-// by TMA (loads run under the MMA main loop) instead of reading it from global memory inside the epilogue
-int launch_umma2(int epi, bool bf16, const CUtensorMap& a, const CUtensorMap& b, const UmmaParams& p, int num_sms, cudaStream_t st,
-                 const CUtensorMap* resid = nullptr, int resid_bufs = 2);
-// 3x3 conv with C_in = 64: resident weights + 3 halo boxes per tile (conv64_kernel.cuh); a: box {64,16,10}, aux: box {64,16,8}
+// 3x3 conv with C_in = 64: resident weights + 3 halo boxes per tile (umma_kernel<MODE_CONV64>); a: box {64,16,10}, aux: box {64,16,8}
 int launch_conv64(int bn, int epi, bool bf16, const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& w, const UmmaParams& p,
                   int num_sms, cudaStream_t st);
 
-// 3x3 conv with C_in >= 128 (levels 1-2): halo boxes {64,16,10} for the pixels, streamed weight blocks (convh_kernel.cuh);
+// 3x3 conv with C_in >= 128 (levels 1-2): halo boxes {64,16,10} for the pixels, streamed weight blocks (umma_kernel<MODE_CONVH>);
 // a: box {64,16,10}, aux: box {64,16,8}, w: box {64, bn}
 bool convh_supports(int bn, const UmmaParams& p);
 int launch_convh(int bn, bool bf16, const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& w, const UmmaParams& p, int num_sms,

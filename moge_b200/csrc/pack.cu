@@ -26,7 +26,7 @@ __global__ void cast_2d_kernel(const void* src, int sdt, void* dst, int rows, in
 }
 int launch_cast_2d(const void* src, int src_dtype, void* dst, bool bf16, int rows, int cols, int src_ld, int dst_ld, cudaStream_t st) {
     const size_t total = static_cast<size_t>(rows) * dst_ld;
-    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 148 * 16));
+    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 132 * 16));
     if (bf16) cast_2d_kernel<true><<<blocks, 256, 0, st>>>(src, src_dtype, dst, rows, cols, src_ld, dst_ld);
     else cast_2d_kernel<false><<<blocks, 256, 0, st>>>(src, src_dtype, dst, rows, cols, src_ld, dst_ld);
     CUDA_TRY(cudaGetLastError());
@@ -47,7 +47,7 @@ __global__ void pack_conv_kernel(const float* w, void* dst, int Cout, int Cin, i
 }
 int launch_pack_conv(const float* w, void* dst, bool bf16, int Cout, int Cin, int taps, int dst_ld, int k_off, cudaStream_t st) {
     const size_t total = static_cast<size_t>(Cout) * taps * Cin;
-    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 148 * 16));
+    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 132 * 16));
     if (bf16) pack_conv_kernel<true><<<blocks, 256, 0, st>>>(w, dst, Cout, Cin, taps, dst_ld, k_off);
     else pack_conv_kernel<false><<<blocks, 256, 0, st>>>(w, dst, Cout, Cin, taps, dst_ld, k_off);
     CUDA_TRY(cudaGetLastError());
@@ -67,7 +67,7 @@ __global__ void pack_convT_kernel(const float* w, void* dst, int Cin, int Cout) 
 }
 int launch_pack_convT(const float* w, void* dst, bool bf16, int Cin, int Cout, cudaStream_t st) {
     const size_t total = static_cast<size_t>(4) * Cout * Cin;
-    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 148 * 16));
+    const int blocks = static_cast<int>(std::min<size_t>((total + 255) / 256, 132 * 16));
     if (bf16) pack_convT_kernel<true><<<blocks, 256, 0, st>>>(w, dst, Cin, Cout);
     else pack_convT_kernel<false><<<blocks, 256, 0, st>>>(w, dst, Cin, Cout);
     CUDA_TRY(cudaGetLastError());
@@ -97,7 +97,7 @@ __global__ void up2_expand_kernel(const float* w, float* dst, int Cout, int Cin)
 }
 int launch_up2_expand(const float* w, float* dst, int Cout, int Cin, cudaStream_t st) {
     const size_t total = static_cast<size_t>(4) * Cout * Cin * 9;
-    up2_expand_kernel<<<static_cast<int>(std::min<size_t>((total + 255) / 256, 148 * 16)), 256, 0, st>>>(w, dst, Cout, Cin);
+    up2_expand_kernel<<<static_cast<int>(std::min<size_t>((total + 255) / 256, 132 * 16)), 256, 0, st>>>(w, dst, Cout, Cin);
     CUDA_TRY(cudaGetLastError());
     return 0;
 }

@@ -69,13 +69,6 @@ int make_map_2d(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, 
     cuuint32_t box[2] = {64, box_rows};
     return encode(m, base, 2, dims, strides, box);
 }
-// fp32 row-major matrix [rows, cols] (pitch in elements): box {32 columns = 128 bytes, 32 rows}, SWIZZLE_128B
-int make_map_2d_f32(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint64_t row_pitch_elems) {
-    cuuint64_t dims[2] = {cols, rows};
-    cuuint64_t strides[1] = {row_pitch_elems * 4};
-    cuuint32_t box[2] = {32, 32};
-    return encode(m, base, 2, dims, strides, box, CU_TENSOR_MAP_DATA_TYPE_FLOAT32);
-}
 int make_map_3d(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint64_t batch, uint32_t box_rows) {
     cuuint64_t dims[3] = {cols, rows, batch};
     cuuint64_t strides[2] = {cols * 2, cols * rows * 2};

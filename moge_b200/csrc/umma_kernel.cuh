@@ -1,11 +1,19 @@
-// The one tensor-core kernel of the engine: a persistent, warp-specialised tcgen05 GEMM whose A operand is either
+// The one tensor-core kernel of the engine: a persistent, warp-specialised wgmma GEMM whose A operand is either
 // a row-major matrix (encoder linears) or an 8x16-pixel window of a padded NHWC image shifted by a filter tap
-// (decoder implicit-GEMM convolutions).  TMA -> 128B-swizzled smem ring -> tcgen05.mma (fp32 accumulators in
-// TMEM, double-buffered) -> fused epilogue straight from TMEM.
+// (decoder implicit-GEMM convolutions).  TMA -> 128B-swizzled smem ring -> wgmma (fp32 accumulators in registers)
+// -> accumulator tile staged in shared memory -> fused epilogue.
 //
-// Roles (warp-uniform): warp 0 = TMA producer (1 lane), warp 1 = MMA issuer (1 lane) + TMEM owner,
-// warps 2.. = epilogue (each warp owns the TMEM lane quarter (warp & 3); with 8 epilogue warps the two warps of a
-// quarter split the accumulator columns).
+// Roles (warpgroup-uniform): warpgroup 0 = TMA producer (one elected lane of warp 0), warpgroups 1 and 2 = consumers:
+// each issues the wgmma of its 64 rows of the 128-row tile, then all eight consumer warps run the epilogue (warp ew owns
+// rows 32 (ew & 3) .. +31; with 8 epilogue warps the two warps of a row quarter split the columns).
+//
+// Three main loops share the kernel (MODE):
+//   MODE_GEMM   one stage = one 64-wide K block of A (row tile, or one filter tap's pixel window) and of B.
+//   MODE_CONV64 3x3 convs with C_in = 64: the packed weights of the CTA's output-channel tile (9 taps [+ the fused 1x1 input
+//               block]) are loaded ONCE and stay resident; a stage is one halo box (16 px x 10 rows, one per horizontal tap
+//               offset) whose three 2 KB-aligned row windows are the A operands of the three vertical taps.
+//   MODE_CONVH  3x3 convs with C_in >= 128: the same halo boxes per 64-channel block, the three vertical-tap weight blocks
+//               streamed in the same stage.
 //
 // Reference ops covered (SURVEY.md 2c): K2 patch-embed, K4 qkv, K6 proj+LayerScale+residual, K7 fc1+GELU,
 // K8 fc2+LayerScale+residual, K9 tap projection sum, K10/K11 1x1 + UV, K12 ConvTranspose2d k2s2, K13/K14 3x3
@@ -30,9 +38,7 @@ enum : int {
                        //        straight into the heads' fp32 output maps; the heads' EPI_HEADOUT launches then accumulate
 };
 
-#ifndef MG_STAGES256
-#define MG_STAGES256 4
-#endif
+enum : int { MODE_GEMM = 0, MODE_CONV64 = 1, MODE_CONVH = 2 };
 constexpr int TILE_M = 128;
 constexpr int TILE_K = 64;     // 64 x 16-bit = one 128-byte swizzle row
 constexpr int TILE_PW = 16;    // pixel tile = 8 rows x 16 columns
@@ -71,24 +77,60 @@ struct UmmaParams {
     int stats_ld;              // partial sums per row in stats_out
 };
 
-template <int BN> struct UmmaCfg {
-    static constexpr int kStageBytes = TILE_M * 128 + BN * 128;
-    static constexpr int kStages = (BN >= 256) ? MG_STAGES256 : (BN >= 128) ? 6 : 8;
+template <int BN, int MODE = MODE_GEMM> struct UmmaCfg {
+    static constexpr int kHaloBytes = 160 * 128;                 // box {64 ch, 16 px, 10 rows}
+    static constexpr int kABytes = (MODE == MODE_GEMM) ? TILE_M * 128 : kHaloBytes;
+    static constexpr int kBBytes = (MODE == MODE_GEMM) ? BN * 128 : (MODE == MODE_CONVH) ? 3 * BN * 128 : 0;
+    static constexpr int kStageBytes = kABytes + kBBytes;
+    static constexpr int kResidentBytes = (MODE == MODE_CONV64) ? 10 * BN * 128 : 0;     // 9 taps + 1 aux block, each [BN][64]
+    // accumulator tile staged for the epilogue: 32 x 32 fp32 blocks, [row quarter][column chunk]; float4 (r, q) of a block at
+    // r * 8 + (q ^ (r & 7)) -- a lane reads its row conflict-free, 8 lanes x float4 read one row of the block conflict-free
+    static constexpr int kChunks = (BN < 32) ? 1 : BN / 32;
+    static constexpr int kAccBytes = TILE_M * kChunks * 32 * 4;
+    static constexpr int kFixedBytes = kAccBytes + kResidentBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int kFit = (kMaxDynSmem - kFixedBytes) / kStageBytes;
+    static constexpr int kStages = kFit > 8 ? 8 : kFit;
     static constexpr int kEpiWarps = (BN >= 64) ? 8 : 4;
-    static constexpr int kThreads = 64 + 32 * kEpiWarps;
-    static constexpr int kTmemCols = (2 * BN <= 32) ? 32 : (2 * BN <= 64) ? 64 : (2 * BN <= 128) ? 128 : (2 * BN <= 256) ? 256 : 512;
-    static constexpr int kScratchBytes = kEpiWarps * 4096;   // per-epilogue-warp 32x32 fp32 transpose tile
-    static constexpr int kSmemBytes = kStages * kStageBytes + 1024 /*align slack*/ + 256 /*barriers*/ + kScratchBytes;
+    static constexpr int kThreads = 384;
+    static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
     static constexpr int kColsPerWarp = (kEpiWarps == 8) ? BN / 2 : BN;
-    static_assert(kSmemBytes <= kMaxDynSmem, "umma_kernel: stage ring + scratch exceed the shared memory of one CTA");
-    static_assert((2 * kStages + 4) * 8 + 4 <= 256, "umma_kernel: barrier block overflows its 256 bytes");
+    static_assert(kStages >= 2, "umma_kernel: fewer than two ring stages fit beside the accumulator tile");
+    static_assert(kSmemBytes <= kMaxDynSmem, "umma_kernel: stage ring + accumulator tile exceed the shared memory of one CTA");
+    static_assert((2 * kStages + 1) * 8 <= 256, "umma_kernel: barrier block overflows its 256 bytes");
 };
+
+// Block of the staged accumulator tile holding rows 32 quarter .. +31, columns col .. col + 31 (col a multiple of 32).
+template <int BN>
+__device__ __forceinline__ const float4* acc_block(const float4* stg, int quarter, int col) {
+    return stg + (quarter * UmmaCfg<BN>::kChunks + (col >> 5)) * 256;
+}
+// Consumer warpgroup g (rows 64 g .. +63) writes its m64nBN accumulator fragment into the staged tile.
+template <int BN>
+__device__ __forceinline__ void acc_stage(float4* stg, const float* d, int g, int wl, int lane) {
+    float* s = reinterpret_cast<float*>(stg);
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+        const int row = 64 * g + 16 * wl + (lane >> 2) + 8 * ((i >> 1) & 1);
+        const int col = 8 * (i >> 2) + 2 * (lane & 3);
+        const int rl = row & 31, q = (col & 31) >> 2;
+        float* blk = s + ((row >> 5) * UmmaCfg<BN>::kChunks + (col >> 5)) * 1024;
+        *reinterpret_cast<float2*>(blk + (rl * 8 + (q ^ (rl & 7))) * 4 + (col & 3)) = make_float2(d[i], d[i + 1]);
+    }
+}
+// This lane's row (lane of the block) over the block's first 4 NQ columns.
+template <int NQ>
+__device__ __forceinline__ void acc_row(const float4* blk, int lane, float* v) {
+#pragma unroll
+    for (int q = 0; q < NQ; ++q) {
+        const float4 t = blk[lane * 8 + (q ^ (lane & 7))];
+        v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+    }
+}
 
 // Exact-erf GELU (nn.GELU() default, vision_transformer.py:61): gelu(x) = relu(x) - 0.5 |x| erfc(|x|/sqrt2), with
 // erfc(|x|/sqrt2) = 2^q(|x|), q a degree-5 fit of log2(erfc) on [0,6] (weighted for the GELU error; max |gelu error|
 // 7e-7 in fp32, far below the 16-bit output rounding).  5 FMA + 1 MUFU.EX2 + 4 other instructions instead of libdevice
-// erff's ~25: the fc1 epilogue is ALU-issue-bound, this is what keeps the tensor pipe fed.  (An A&S 7.1.26 variant with
-// MUFU.RCP + MUFU.EX2 was measured 25 % slower than erff: two quarter-rate MUFU ops per element are too many.)
+// erff's ~25: the fc1 epilogue is bound by instruction issue.
 // (No clamp of |x|: the polynomial keeps decreasing beyond the fitted range -- q(6) = -29.2, q(8) = -51.8, q(20) = -1019 -- so
 // |x| * 2^q just underflows to 0 for large |x|; the clamp cost one instruction per element in an epilogue that is bound by
 // instruction issue.)
@@ -143,17 +185,6 @@ __device__ __forceinline__ void ln_load(const UmmaParams& p, int mt, int quarter
     }
 }
 
-// EPI_RESID with the residual staged by TMA (umma2_kernel): per epilogue warp two 32 x 32 fp32 chunk buffers (128-byte rows,
-// SWIZZLE_128B) and their mbarriers; `rc` counts the chunks this warp has consumed (buffer = rc & 1, phase = (rc >> 1) & 1).
-struct ResidPipe {
-    uint8_t* buf;                 // 2 x 4096 bytes, 1024-byte aligned
-    uint64_t* bars;               // 2 mbarriers
-    const CUtensorMap* map;       // fp32 [M, N], box {32, 32}
-    uint32_t rc;
-    int nbuf;                     // 1 or 2 chunk buffers
-    int next_row0, next_col0;     // first row / first column (of this warp's column group) of the NEXT tile, next_row0 < 0: none
-};
-
 // DF < 0: the EPI_DEC variant (raw / ReLU copies, skip, UV, pixel shuffle) is decided at run time from the params;
 // DF >= 0: compile-time bit mask (DF_RAW | DF_RELU | DF_SKIP | DF_UV | DF_SHUFFLE) -- a much smaller hot loop.
 enum : int { DF_RAW = 1, DF_RELU = 2, DF_SKIP = 4, DF_UV = 8, DF_SHUFFLE = 16 };
@@ -174,7 +205,7 @@ static __device__ __noinline__ void store_px_border16(uint8_t* base, int b, int 
 // (4 lanes per pixel row, 8 pixels per warp instruction, 4 passes per chunk) and moves 16 bytes per load/store -- half the
 // per-byte instruction overhead of the 8-byte variant used for the row-major epilogues.
 template <int BN, int COLS, int AMODE, bool BF16, int DF>
-__device__ __forceinline__ void epilogue_dec16(const UmmaParams& p, int mt, int nt, uint32_t t_addr, float4* scr, int quarter, int lane,
+__device__ __forceinline__ void epilogue_dec16(const UmmaParams& p, int mt, int nt, const float4* stg, int quarter, int lane,
                                                int col_begin) {
     using H = H16<BF16>;
     const bool has_raw = (DF < 0) ? (p.out0 != nullptr) : ((DF & DF_RAW) != 0);
@@ -215,23 +246,17 @@ __device__ __forceinline__ void epilogue_dec16(const UmmaParams& p, int mt, int 
         eflags[i] = (ry[i] == 0 ? 1 : 0) | (ry[i] == p.H - 1 ? 2 : 0) | (rx[i] == 0 ? 4 : 0) | (rx[i] == p.W - 1 ? 8 : 0);
     }
     const float inv_wo = 1.0f / static_cast<float>(p.Wo), inv_ho = 1.0f / static_cast<float>(p.Ho);
-    // Interior tiles (every pixel inside the image and none on its border: ~70 % of the tiles of a 148x148 map) take a
-    // straight-line path: no per-row validity predicates, no border-replication bookkeeping.  ncu of the ConvTranspose launch
-    // showed this epilogue spending 57 % of its instructions on address arithmetic, predicates and branches (IMAD / ISETP / BRA /
-    // LOP3 / SEL) around 21 % of useful work (FADD, F2FP, LDS / STS, STG).  The phase of a pixel-shuffle chunk comes from a shift
-    // when C_out is a power of two (every MoGe config) instead of an integer division per chunk.
+    // Interior tiles (every pixel inside the image and none on its border: most tiles of a large map) take a straight-line
+    // path: no per-row validity predicates, no border-replication bookkeeping, which otherwise outweigh the useful work of this
+    // epilogue.  The phase of a pixel-shuffle chunk comes from a shift when C_out is a power of two (every MoGe config) instead
+    // of an integer division per chunk.
     bool interior;
     if (AMODE == AMODE_TILES) interior = tile_y0 > 0 && tile_x0 > 0 && tile_y0 + TILE_PH < p.H && tile_x0 + TILE_PW < p.W;
     else interior = false;
     const int ldo_shift = ((p.ldo & (p.ldo - 1)) == 0) ? (31 - __clz(p.ldo)) : -1;
     auto chunk = [&](int c, auto fast_tag) {
         constexpr bool FAST = decltype(fast_tag)::value;
-        float v[32];
-        tmem_ld32(t_addr + c, v);
-        tc_wait_ld();
-#pragma unroll
-        for (int q = 0; q < 8; ++q) scr[lane * 8 + (q ^ (lane & 7))] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-        __syncwarp();
+        const float4* scr = acc_block<BN>(stg, quarter, col_begin + c);
         const int col = nt * BN + col_begin + c;
         int co = col + 8 * q8, qd = 0, qmask = 15;
         size_t qoff = 0;
@@ -298,7 +323,6 @@ __device__ __forceinline__ void epilogue_dec16(const UmmaParams& p, int mt, int 
                     if (has_relu) store_px_border16(static_cast<uint8_t*>(p.out1), rb[i], Y, X, p.Ho, p.Wo, p.Hop, p.Wop, p.ldo, co, pk_relu[i]);
                 }
         }
-        __syncwarp();
     };
     if (interior) {
 #pragma unroll 1
@@ -310,15 +334,13 @@ __device__ __forceinline__ void epilogue_dec16(const UmmaParams& p, int mt, int 
 }
 
 
-// Epilogue of ONE accumulator tile for one epilogue warp (TMEM lane quarter `quarter`, columns [col_begin, col_begin+COLS)).
-// TMEM hands each thread one accumulator ROW; global memory wants warps on contiguous COLUMNS.  Every 32x32 chunk is
-// therefore transposed through a per-warp swizzled smem tile: afterwards 8 lanes x float4 cover the 32 columns of one
-// row and each warp instruction touches 4 rows (4 x 128 B), fully coalesced.
+// Epilogue of ONE accumulator tile for one epilogue warp (rows 32 quarter .. +31, columns [col_begin, col_begin+COLS)) from the
+// staged tile `stg`: 8 lanes x float4 cover the 32 columns of one row of a block and each warp instruction touches 4 rows
+// (4 x 128 B), fully coalesced.
 
 template <int BN, int COLS, int AMODE, int EPI, bool BF16, int DF = -1>
-__device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int nt, uint32_t t_addr, float4* scr, int quarter,
-                                              int lane, int col_begin, bool ln_rows_on = false, LnRows lnr = LnRows{},
-                                              ResidPipe* rp = nullptr) {
+__device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int nt, const float4* stg, int quarter,
+                                              int lane, int col_begin, bool ln_rows_on = false, LnRows lnr = LnRows{}) {
     using H = H16<BF16>;
     const bool has_raw = (DF < 0) ? (p.out0 != nullptr) : ((DF & DF_RAW) != 0);
     const bool has_relu = (DF < 0) ? (p.out1 != nullptr) : ((DF & DF_RELU) != 0);
@@ -326,7 +348,7 @@ __device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int n
     const bool has_uv = (DF < 0) ? (p.vec1 != nullptr) : ((DF & DF_UV) != 0);
     const bool shuffle = (DF < 0) ? (p.shuffle != 0) : ((DF & DF_SHUFFLE) != 0);
     if (EPI == EPI_DEC) {
-        epilogue_dec16<BN, COLS, AMODE, BF16, DF>(p, mt, nt, t_addr, scr, quarter, lane, col_begin);
+        epilogue_dec16<BN, COLS, AMODE, BF16, DF>(p, mt, nt, stg, quarter, lane, col_begin);
         return;
     }
     const int row = quarter * 32 + lane;
@@ -341,8 +363,7 @@ __device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int n
         const int px = (r % p.tiles_x) * TILE_PW + row % TILE_PW;
         const bool valid = (py < p.H) && (px < p.W);
         float v[16];
-        tmem_ld16(t_addr, v);
-        tc_wait_ld();
+        acc_row<4>(acc_block<BN>(stg, quarter, 0), lane, v);
         if (valid) {
             // accumulator columns: (phase, component); phase (qy,qx) -> output pixel (2*py+qy, 2*px+qx)
 #pragma unroll
@@ -387,8 +408,7 @@ __device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int n
         const int px = (r % p.tiles_x) * TILE_PW + row % TILE_PW;
         const bool valid = (py < p.H) && (px < p.W);
         float v[32];
-        tmem_ld32(t_addr, v);
-        tc_wait_ld();
+        acc_row<8>(acc_block<BN>(stg, quarter, 0), lane, v);
         if (valid) {
             float b8[8], gu[8], gv[8];
 #pragma unroll
@@ -464,9 +484,6 @@ __device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int n
         float ln_rs[8], st1[8], st2[8];        // st1/st2 (producers): partial sums of x and x^2 of this lane's 8 rows
 #pragma unroll
         for (int i = 0; i < 8; ++i) { ln_rs[i] = ln_on ? lnr.rs[i] : 1.f; st1[i] = 0.f; st2[i] = 0.f; }
-        // (Prefetching the fp32 residual of chunk c + 1 before chunk c is drained -- two chunks of loads in flight per warp -- was
-        // measured on one box, A/B: proj 3.68 -> 4.14 ms, fc2 7.24 -> 7.33 ms per step, i.e. SLOWER; the extra 32 registers and the
-        // deeper load queue cost more than the latency they hide.  Kept load-then-use.)
         // Full row tiles (all but the last of a GEMM) take a path without the per-row validity predicates.
         const bool full_tile = (AMODE == AMODE_ROWS) && (static_cast<long>(mt) + 1) * TILE_M <= static_cast<long>(p.M);
         auto chunk = [&](int c, auto full_tag) {
@@ -474,17 +491,7 @@ __device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int n
             const int col = nt * BN + col_begin + c;       // first global output column of this chunk
             int co = col + 4 * q4;                         // this lane's 4 columns
             float4 pre[8];
-            // (EPI_RESID -- proj / fc2 -- stalls on the latency of the fp32 residual reads: ncu long_scoreboard 7.6 warps per issue
-            // cycle at 48 % of the DRAM peak.  Issuing those reads HERE, ahead of the TMEM load and the transpose, measured SLOWER in a
-            // same-box A/B -- proj 3.41 -> 3.65 ms per step -- like the two-chunk prefetch before it: the longer live ranges cost
-            // registers / spills in an epilogue that sits at the 168-register cap.  Kept load-then-use.)
-            float v[32];
-            tmem_ld32(t_addr + c, v);
-            tc_wait_ld();
-#pragma unroll
-            for (int q = 0; q < 8; ++q)
-                scr[lane * 8 + (q ^ (lane & 7))] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
-            __syncwarp();
+            const float4* scr = acc_block<BN>(stg, quarter, col_begin + c);
             int qd = 0;
             size_t qoff = 0;                               // EPI_DEC: byte offset of this chunk relative to the centre pixel
             int qmask = 15;                                // which source-grid edges replicate for this chunk
@@ -512,7 +519,7 @@ __device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int n
                 if (EPI == EPI_DEC && shuffle) { sY[i] = 2 * ry[i] + (qd >> 1); sX[i] = 2 * rx[i] + (qd & 1); }
                 if (!FULL && !ok[i]) continue;
                 if (EPI == EPI_RESID) {
-                    if (rp == nullptr) pre[i] = *reinterpret_cast<const float4*>(static_cast<const float*>(p.out0) + roff[i] + co);
+                    pre[i] = *reinterpret_cast<const float4*>(static_cast<const float*>(p.out0) + roff[i] + co);
                 } else if (EPI == EPI_PATCH) {
                     const int t = ry[i] * p.W + rx[i];
                     pre[i] = *reinterpret_cast<const float4*>(p.vec1 + static_cast<size_t>(t) * p.ldo + co);
@@ -521,32 +528,6 @@ __device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int n
                     const float2 f0 = H::unpack(u.x), f1 = H::unpack(u.y);
                     pre[i] = make_float4(f0.x, f0.y, f1.x, f1.y);
                 }
-            }
-            if (EPI == EPI_RESID && rp != nullptr) {
-                // residual chunk from the TMA-staged buffer: row rl = 4 i + sub is one swizzled 128-byte line, this lane's 4 columns
-                // are its 16-byte chunk q4 ^ (rl & 7)
-                const uint32_t b = (rp->nbuf == 2) ? (rp->rc & 1u) : 0u;
-                mbar_wait(&rp->bars[b], ((rp->nbuf == 2) ? (rp->rc >> 1) : rp->rc) & 1u);
-                const uint8_t* rb_ = rp->buf + b * 4096;
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const int rl = 4 * i + sub;
-                    pre[i] = *reinterpret_cast<const float4*>(rb_ + rl * 128 + ((q4 ^ (rl & 7)) << 4));
-                }
-                fence_proxy_async_smem();           // these generic-proxy reads are ordered before the TMA write that refills the buffer
-                __syncwarp();
-                // refill the buffer `nbuf` chunks ahead: a later chunk of this tile, or the first chunk(s) of the next tile (they land
-                // under its main loop)
-                const int ahead = 32 * rp->nbuf;
-                int ncol = -1, nrow = 0;
-                if (c + ahead < COLS) { ncol = nt * BN + col_begin + c + ahead; nrow = mt * TILE_M + quarter * 32; }
-                else if (rp->next_row0 >= 0) { ncol = rp->next_col0 + (c + ahead - COLS); nrow = rp->next_row0; }
-                if (ncol >= 0 && elect_one()) {
-                    mbar_arrive_expect_tx(&rp->bars[b], 4096);
-                    tma_load_2d(rp->buf + b * 4096, rp->map, &rp->bars[b], ncol, nrow);
-                }
-                __syncwarp();
-                rp->rc++;
             }
             // ---- phase 2: math + stores
             uint2 pk_raw[8], pk_relu[8];
@@ -557,8 +538,6 @@ __device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int n
                 float4 a = scr[rl * 8 + (q4 ^ (rl & 7))];
                 if (!FULL && !ok[i]) continue;
                 if (EPI == EPI_STORE16 || EPI == EPI_GELU16) {
-                    // (packed FADD2 for the plain bias add measured ~5 % SLOWER on these GEMMs than four scalar FADDs -- three boxes
-                    // each way -- although the packed GELU polynomial and the packed attention softmax are wins; kept scalar)
                     float2 a01, a23;
                     if (ln_on) {      // LN(x) W^T + b = rstd * (x16 W''^T) + b'   (mean removal lives in the centred weight W'')
                         a01 = make_float2(fmaf(ln_rs[i], a.x, bias4.x), fmaf(ln_rs[i], a.y, bias4.y));
@@ -649,65 +628,73 @@ __device__ __forceinline__ void epilogue_tile(const UmmaParams& p, int mt, int n
     }
 }
 
-template <int BN, int AMODE, int EPI, bool BF16, int DF = -1>
-__global__ void __launch_bounds__(UmmaCfg<BN>::kThreads, 1)
+template <int BN, int MODE, int AMODE, int EPI, bool BF16, int DF = -1>
+__global__ void __launch_bounds__(384, 1)
 umma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAux,
             const __grid_constant__ CUtensorMap mapB, const UmmaParams p) {
-    pdl_launch_dependents();      // (the wait sits after the barrier / TMEM set-up below: that prologue overlaps the previous kernel's tail)
-    using Cfg = UmmaCfg<BN>;
-    using H = H16<BF16>;
+    pdl_launch_dependents();      // (the wait sits after the barrier set-up below: that prologue overlaps the previous kernel's tail)
+    using Cfg = UmmaCfg<BN, MODE>;
     constexpr int S = Cfg::kStages;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint64_t* full = reinterpret_cast<uint64_t*>(smem + S * Cfg::kStageBytes);
+    float4* stg = reinterpret_cast<float4*>(smem + S * Cfg::kStageBytes);
+    uint8_t* sW = smem + S * Cfg::kStageBytes + Cfg::kAccBytes;         // MODE_CONV64: resident weights
+    uint64_t* full = reinterpret_cast<uint64_t*>(sW + Cfg::kResidentBytes);
     uint64_t* empty = full + S;
-    uint64_t* tfull = empty + S;
-    uint64_t* tempty = tfull + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tempty + 2);
-    float* scratch_base = reinterpret_cast<float*>(smem + S * Cfg::kStageBytes + 256);
+    uint64_t* wfull = empty + S;
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
     const int total_tiles = p.num_m_tiles * p.num_n_tiles;
+    // stages per tile
     const int kb_taps = p.ntaps * p.kb_main;
-    const int kb_total = kb_taps + p.kb_aux;
+    const int nstage = (MODE == MODE_GEMM) ? kb_taps + p.kb_aux : (MODE == MODE_CONV64) ? 3 + p.kb_aux : 3 * p.kb_main + p.kb_aux;
 
     if (threadIdx.x == 0) {
         tma_prefetch_desc(&mapA);
         tma_prefetch_desc(&mapB);
         if (p.kb_aux) tma_prefetch_desc(&mapAux);
-        for (int s = 0; s < S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-        for (int a = 0; a < 2; ++a) { mbar_init(&tfull[a], 1); mbar_init(&tempty[a], Cfg::kEpiWarps); }
+        // empty: one arrival per consumer warp once its warpgroup's MMAs that read the stage have completed
+        for (int s = 0; s < S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
+        mbar_init(wfull, 1);
         fence_mbar_init();
     }
-    if (warp == 1) tmem_alloc(tmem_slot, Cfg::kTmemCols);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
     pdl_wait();
 
-    if (warp == 0) {
+    if (warp < 4) {
         // ================================================================== TMA producer
-        // (this warp and the MMA warp stay CONVERGED and one elected lane issues: under `if (lane == 0)` the compiler has
-        // to assume an arbitrary active mask and wraps every TMA / tcgen05 instruction in an elect-and-retry loop)
-        {
-            int s = 0; uint32_t ph = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-                const int mt = tile / p.num_n_tiles, nt = tile % p.num_n_tiles;
-                int b = 0, x0 = 0, y0 = 0;
-                if (AMODE == AMODE_TILES) {
-                    const int per_img = p.tiles_x * p.tiles_y;
-                    b = mt / per_img;
-                    const int r = mt % per_img;
-                    y0 = (r / p.tiles_x) * TILE_PH;
-                    x0 = (r % p.tiles_x) * TILE_PW;
-                }
-                for (int i = 0; i < kb_total; ++i) {
-                    mbar_wait(&empty[s], ph ^ 1);
-                    uint8_t* sa = smem + s * Cfg::kStageBytes;
-                    uint8_t* sb = sa + TILE_M * 128;
-                    if (elect_one()) {
+        // (warp 0 stays CONVERGED and one elected lane issues: under `if (lane == 0)` the compiler has to assume an
+        // arbitrary active mask and wraps every TMA instruction in an elect-and-retry loop)
+        regs_dec<40>();
+        if (warp != 0) return;
+        if (MODE == MODE_CONV64) {
+            // the weights of this CTA's output-channel tile (the grid is a multiple of num_n_tiles: nt is fixed per CTA)
+            const int nblk = 9 + p.kb_aux;
+            const int nt = static_cast<int>(blockIdx.x) % p.num_n_tiles;
+            if (elect_one()) {
+                mbar_arrive_expect_tx(wfull, nblk * BN * 128);
+                for (int t = 0; t < nblk; ++t) tma_load_2d(sW + t * BN * 128, &mapB, wfull, t * TILE_K, nt * BN);
+            }
+            __syncwarp();
+        }
+        int s = 0; uint32_t ph = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            const int mt = tile / p.num_n_tiles, nt = tile % p.num_n_tiles;
+            int b = 0, x0 = 0, y0 = 0;
+            if (AMODE == AMODE_TILES) {
+                const int per_img = p.tiles_x * p.tiles_y;
+                b = mt / per_img;
+                const int r = mt % per_img;
+                y0 = (r / p.tiles_x) * TILE_PH;
+                x0 = (r % p.tiles_x) * TILE_PW;
+            }
+            for (int i = 0; i < nstage; ++i) {
+                mbar_wait(&empty[s], ph ^ 1);
+                uint8_t* sa = smem + s * Cfg::kStageBytes;
+                uint8_t* sb = sa + Cfg::kABytes;
+                if (elect_one()) {
+                    if (MODE == MODE_GEMM) {
                         mbar_arrive_expect_tx(&full[s], Cfg::kStageBytes);
                         if (AMODE == AMODE_ROWS) {
                             tma_load_2d(sa, &mapA, &full[s], i * TILE_K, mt * TILE_M);
@@ -719,79 +706,106 @@ umma_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
                             tma_load_4d(sa, &mapAux, &full[s], (i - kb_taps) * TILE_K, x0 + 1, y0 + 1, b);
                         }
                         tma_load_2d(sb, &mapB, &full[s], i * TILE_K, nt * BN);
+                    } else if (MODE == MODE_CONV64) {
+                        if (i < 3) {
+                            mbar_arrive_expect_tx(&full[s], Cfg::kHaloBytes);
+                            tma_load_4d(sa, &mapA, &full[s], 0, x0 + i, y0, b);             // padded rows y0..y0+9 = taps dy 0..2
+                        } else {
+                            mbar_arrive_expect_tx(&full[s], TILE_M * 128);
+                            tma_load_4d(sa, &mapAux, &full[s], 0, x0 + 1, y0 + 1, b);
+                        }
+                    } else {
+                        // MODE_CONVH: stage i = (channel block c, horizontal tap dx): halo box + the weight blocks of dy = 0..2;
+                        // the aux blocks (fused 1x1 source) follow: 8-row box + one weight block
+                        const bool aux = i >= 3 * p.kb_main;
+                        if (!aux) {
+                            const int c = i / 3, dx = i % 3;
+                            mbar_arrive_expect_tx(&full[s], Cfg::kHaloBytes + 3 * BN * 128);
+                            tma_load_4d(sa, &mapA, &full[s], c * TILE_K, x0 + dx, y0, b);
+                            for (int dy = 0; dy < 3; ++dy)
+                                tma_load_2d(sb + dy * BN * 128, &mapB, &full[s], ((dy * 3 + dx) * p.kb_main + c) * TILE_K, nt * BN);
+                        } else {
+                            const int c = i - 3 * p.kb_main;
+                            mbar_arrive_expect_tx(&full[s], TILE_M * 128 + BN * 128);
+                            tma_load_4d(sa, &mapAux, &full[s], c * TILE_K, x0 + 1, y0 + 1, b);
+                            tma_load_2d(sb, &mapB, &full[s], (9 * p.kb_main + c) * TILE_K, nt * BN);
+                        }
                     }
-                    __syncwarp();
-                    if (++s == S) { s = 0; ph ^= 1; }
                 }
-            }
-        }
-    } else if (warp == 1) {
-        // ================================================================== MMA issuer
-        {
-            constexpr uint32_t idesc = make_idesc(TILE_M, BN, BF16 ? 1u : 0u);
-            int s = 0; uint32_t ph = 0;
-            int it = 0;
-            for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
-                const int acc = it & 1;
-                const uint32_t aph = (it >> 1) & 1;
-                mbar_wait(&tempty[acc], aph ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * BN;
-                for (int i = 0; i < kb_total; ++i) {
-                    mbar_wait(&full[s], ph);
-                    tc_fence_after();
-                    const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes);
-                    const uint64_t adesc = make_sdesc_sw128(sa);
-                    const uint64_t bdesc = make_sdesc_sw128(sa + TILE_M * 128);
-                    if (elect_one()) {
-#pragma unroll
-                        for (int k = 0; k < TILE_K / 16; ++k)
-                            umma_f16(d_tmem, adesc + 2 * k, bdesc + 2 * k, idesc, (i | k) != 0);
-                        umma_commit(&empty[s]);
-                        if (i == kb_total - 1) umma_commit(&tfull[acc]);
-                    }
-                    __syncwarp();
-                    if (++s == S) { s = 0; ph ^= 1; }
-                }
+                __syncwarp();
+                if (++s == S) { s = 0; ph ^= 1; }
             }
         }
     } else {
-        // ================================================================== epilogue
-        // TMEM hands each thread one accumulator ROW; global memory wants warps on contiguous COLUMNS.  Every 32x32
-        // chunk is therefore transposed through a per-warp swizzled smem tile: afterwards 8 lanes x float4 cover the
-        // 32 columns of one row and each warp instruction touches 4 rows (4 x 128 B), fully coalesced.
-        const int ew = warp - 2;
-        const int quarter = warp & 3;
+        // ================================================================== consumers: MMA, then epilogue
+        regs_inc<232>();
+        const int g = (warp - 4) >> 2;                  // consumer warpgroup: rows 64 g .. 64 g + 63 of the tile
+        const int wl = warp & 3;
+        const int ew = warp - 4;
+        const int quarter = ew & 3;
         const int col_begin = (Cfg::kEpiWarps == 8) ? (ew >> 2) * (BN / 2) : 0;
-        float4* scr = reinterpret_cast<float4*>(scratch_base + ew * 1024);
-        int it = 0;
+        const uint32_t a_off = static_cast<uint32_t>(g) * 64 * 128;
+        if (MODE == MODE_CONV64) mbar_wait(wfull, 0);
+        const uint32_t w0 = smem_u32(sW);
         LnRows lnr{}, lnn{};
         const bool ln_on = AMODE == AMODE_ROWS && (EPI == EPI_STORE16 || EPI == EPI_GELU16) && p.ln_rstd != nullptr;
         if (ln_on && static_cast<int>(blockIdx.x) < total_tiles) ln_load(p, static_cast<int>(blockIdx.x) / p.num_n_tiles, quarter, lane, lnn);
-        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x, ++it) {
+        int s = 0; uint32_t ph = 0;
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int mt = tile / p.num_n_tiles, nt = tile % p.num_n_tiles;
-            const int acc = it & 1;
-            const uint32_t aph = (it >> 1) & 1;
             if (ln_on) {        // rstd of this tile's rows (loaded one iteration ago); then issue the next tile's loads
                 lnr = lnn;
                 const int nxt = tile + static_cast<int>(gridDim.x);
                 if (nxt < total_tiles) ln_load(p, nxt / p.num_n_tiles, quarter, lane, lnn);
             }
-            mbar_wait(&tfull[acc], aph);
-            tc_fence_after();
-            const uint32_t t_addr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + col_begin;
-            epilogue_tile<BN, Cfg::kColsPerWarp, AMODE, EPI, BF16, DF>(p, mt, nt, t_addr, scr, quarter, lane, col_begin, ln_on, lnr);
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&tempty[acc]);
+            float acc[BN / 2];
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+            int prev = -1;
+            for (int i = 0; i < nstage; ++i) {
+                mbar_wait(&full[s], ph);
+                const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes) + a_off;
+                const uint32_t sb = smem_u32(smem + s * Cfg::kStageBytes + Cfg::kABytes);
+                wgmma_fence();
+                auto mma64 = [&](uint32_t a, uint32_t bb) {          // one 64-wide K block
+                    const uint64_t ad = make_sdesc_sw128(a), bd = make_sdesc_sw128(bb);
+#pragma unroll
+                    for (int k = 0; k < TILE_K / 16; ++k) Wgmma<BN, BF16>::ss(acc, ad + 2 * k, bd + 2 * k, 1u);
+                };
+                if (MODE == MODE_GEMM) {
+                    mma64(sa, sb);
+                } else if (MODE == MODE_CONV64) {
+                    if (i < 3) {
+#pragma unroll
+                        for (int dy = 0; dy < 3; ++dy) mma64(sa + dy * TILE_PW * 128, w0 + (dy * 3 + i) * BN * 128);
+                    } else {
+                        mma64(sa, w0 + 9 * BN * 128);
+                    }
+                } else {
+                    if (i < 3 * p.kb_main) {
+#pragma unroll
+                        for (int dy = 0; dy < 3; ++dy) mma64(sa + dy * TILE_PW * 128, sb + dy * BN * 128);
+                    } else {
+                        mma64(sa, sb);
+                    }
+                }
+                wgmma_commit();
+                // the MMAs of the previous stage have completed once at most this stage's group is pending: release its slot
+                wgmma_wait<1>();
+                reg_fence(acc);
+                if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+                prev = s;
+                if (++s == S) { s = 0; ph ^= 1; }
+            }
+            wgmma_wait<0>();
+            reg_fence(acc);
+            if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+            named_sync(1, 256);                          // every epilogue warp is done reading the previous tile
+            acc_stage<BN>(stg, acc, g, wl, lane);
+            named_sync(1, 256);
+            if (ew < Cfg::kEpiWarps)
+                epilogue_tile<BN, Cfg::kColsPerWarp, AMODE, EPI, BF16, DF>(p, mt, nt, stg, quarter, lane, col_begin, ln_on, lnr);
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, Cfg::kTmemCols);
     }
 }
 

@@ -5,16 +5,16 @@ namespace mg {
 
 #define INST(BN, EPI)                                                                                       \
     if (bn == BN && epi == EPI)                                                                             \
-        return bf16 ? launch_umma_inst<BN, AMODE_ROWS, EPI, true>(a, aux, b, p, num_sms, st)                \
-                    : launch_umma_inst<BN, AMODE_ROWS, EPI, false>(a, aux, b, p, num_sms, st);
+        return bf16 ? launch_umma_inst<BN, MODE_GEMM, AMODE_ROWS, EPI, true>(a, aux, b, p, num_sms, st)                \
+                    : launch_umma_inst<BN, MODE_GEMM, AMODE_ROWS, EPI, false>(a, aux, b, p, num_sms, st);
 
 int launch_umma_rows(int bn, int epi, bool bf16, const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& b,
                      const UmmaParams& p, int num_sms, cudaStream_t st) {
-    INST(256, EPI_STORE16) INST(128, EPI_STORE16)
-    INST(256, EPI_GELU16) INST(128, EPI_GELU16)
-    INST(256, EPI_RESID) INST(128, EPI_RESID)
-    INST(256, EPI_PATCH) INST(128, EPI_PATCH)
-    INST(256, EPI_DEC) INST(128, EPI_DEC)
+    INST(128, EPI_STORE16)
+    INST(128, EPI_GELU16)
+    INST(128, EPI_RESID)
+    INST(128, EPI_PATCH)
+    INST(128, EPI_DEC)
     return set_error("no umma_rows instantiation for bn=%d epi=%d", bn, epi);
 }
 #undef INST

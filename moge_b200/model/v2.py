@@ -1,4 +1,4 @@
-"""Drop-in `MoGeModel` for the MoGe-2 inference hot path, backed by libmoge_b200.so (hand-written sm_100a CUDA).
+"""Drop-in `MoGeModel` for the MoGe-2 inference hot path, backed by libmoge_b200.so (hand-written sm_90a CUDA).
 
 Mirrors the public surface of /root/reference/moge/model/v2.py:
   __init__ kwargs (v2.py:30-57), from_pretrained (v2.py:76-107), .to/.eval/.half, .device/.dtype (v2.py:59-65),
@@ -85,7 +85,7 @@ class MoGeModel:
     def onnx_compatible_mode(self, value: bool):
         if value:
             raise NotImplementedError("onnx_compatible_mode changes the resize/pos-embed numerics (modules.py:121, "
-                                      "vision_transformer.py:192) and is not provided by the B200 engine")
+                                      "vision_transformer.py:192) and is not provided by the engine")
 
     def init_weights(self):
         raise NotImplementedError("training-only (v2.py:109-110)")
@@ -208,7 +208,7 @@ class MoGeModel:
         if self._engine is not None:
             return
         if self._device.type != "cuda":
-            raise capi.MogeError("moge_b200 has no CPU path: move the model to a B200 with .to('cuda') first")
+            raise capi.MogeError("moge_b200 has no CPU path: move the model to an H100 with .to('cuda') first")
         if not self._state:
             raise capi.MogeError("no weights loaded (use from_pretrained or load_state_dict)")
         L = capi.lib()
@@ -455,7 +455,7 @@ class MoGeModel:
         precision downgrade."""
         if not use_fp16:
             raise NotImplementedError(
-                "moge_b200: use_fp16=False (full-fp32 network pass) is not provided; the B200 engine computes with 16-bit "
+                "moge_b200: use_fp16=False (full-fp32 network pass) is not provided; the engine computes with 16-bit "
                 "tensor-core operands, fp32 accumulation, an fp32 residual stream and fp32 post-processing (outputs within "
                 "1e-3 of the fp32 reference, see DESIGN.md).  Call infer(..., use_fp16=True).")
         if image.dim() == 3:

@@ -99,7 +99,7 @@ def make_state_dict(cfg: Dict, seed: int = 0, mask_bias: float = 0.7, well_posed
     solve of infer() is then well-conditioned and the five infer() outputs can be compared end to end.  It also gives the
     normal head a dominant camera-facing component, like a trained model whose normals are near unit length: with plain random
     init the three raw components are zero-mean, |n| is close to 0 on many pixels and F.normalize (v2.py:178) amplifies the
-    relative error of the raw output by sqrt(E[1/|n|^2] E[|n|^2]) ~ 1.7 (measured; DESIGN.md section 2)."""
+    relative error of the raw output by sqrt(E[1/|n|^2] E[|n|^2]) ~ 1.7 (DESIGN.md section 2)."""
     g = torch.Generator(device="cpu").manual_seed(seed)
     sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
     for name, shape in _shapes(cfg).items():

@@ -10,6 +10,7 @@ from moge.model.v2 import MoGeModel
 from moge_b200.configs import model_config, default_num_tokens
 from moge_b200.synthetic import make_state_dict, synthetic_images
 from oracle import moge_port
+from golden_io import load_golden
 from gpu_util import rel_l2
 
 pytestmark = pytest.mark.gpu
@@ -80,7 +81,7 @@ def check_forward(out, ref, tol, s=1, tols=None):
 @pytest.mark.parametrize("name", ["vits_b1_126x168_t192", "vits_b2_140x98_t117", "vits_b1_70x70_t1369_native",
                                   "vitb_b1_98x154_t150_nonormal", "vits_b1_224x224_default", "vitl_b1_112x140_t120"])
 def test_forward_and_infer_match_reference_golden(name, golden_dir):
-    gold = torch.load(os.path.join(golden_dir, name + ".pt"), weights_only=False)
+    gold = load_golden(golden_dir, name)
     meta = gold["meta"]
     model, cfg, sd = get_model(meta["size"], meta["with_normal"], meta["seed"])
     B, H, W = meta["shape"]
@@ -159,7 +160,7 @@ def test_postprocess_chain_on_reference_forward_outputs(golden_dir):
     from moge_b200 import capi
     from gpu_util import stream
     for name in ["vits_b1_126x168_t192", "vits_b2_140x98_t117", "vitl_b1_112x140_t120", "vitb_b1_98x154_t150_nonormal"]:
-        gold = torch.load(os.path.join(golden_dir, name + ".pt"), weights_only=False)
+        gold = load_golden(golden_dir, name)
         if gold["meta"]["stride"] != 1:
             continue
         fwd, ginf = gold["forward"], gold["infer"]
@@ -187,7 +188,7 @@ def test_postprocess_chain_on_reference_forward_outputs(golden_dir):
 
 
 def test_forward_matches_golden_bf16(golden_dir):
-    gold = torch.load(os.path.join(golden_dir, "vits_b1_126x168_t192.pt"), weights_only=False)
+    gold = load_golden(golden_dir, "vits_b1_126x168_t192")
     model, cfg, sd = get_model("vits", True, 0, torch.bfloat16)
     img = synthetic_images(1, 126, 168, 0)
     out = model.forward(img.to(DEV), 192)
@@ -363,7 +364,7 @@ def test_benchmark_shapes_match_reference_golden(name, golden_dir):
     the input), the API-default 60x60, the 2:1 / 1:2 mixed-aspect shapes, a 1024x768 ViT-B input, and the linear / sinh /
     sinh_exp remaps.  `_wp` cases use the well-posed synthetic checkpoint (synthetic.make_state_dict(well_posed=True)), so the
     focal/shift solve is well-conditioned and depth / points / intrinsics of infer() are asserted end to end."""
-    gold = torch.load(os.path.join(golden_dir, name + ".pt"), weights_only=False)
+    gold = load_golden(golden_dir, name)
     meta = gold["meta"]
     opt = meta.get("options", {})
     model, cfg, sd = get_model(meta["size"], meta["with_normal"], meta["seed"], well_posed=opt.get("well_posed", False),
@@ -441,7 +442,7 @@ def _gpu_oracle(cfg, sd, img, nt):
 
 
 def test_gpu_oracle_is_pinned_to_the_reference_golden(golden_dir):
-    gold = torch.load(os.path.join(golden_dir, "vitl_b1_518x518_t1369_wp.pt"), weights_only=False)
+    gold = load_golden(golden_dir, "vitl_b1_518x518_t1369_wp")
     meta = gold["meta"]
     cfg = model_config("vitl", True)
     sd = make_state_dict(cfg, meta["seed"], well_posed=True)

@@ -1,4 +1,4 @@
-"""-m gpu: operator-level parity of the hand-written sm_100a kernels (through the C ABI) against plain PyTorch
+"""-m gpu: operator-level parity of the hand-written sm_90a kernels (through the C ABI) against plain PyTorch
 fp32 references of the same op on the same (16-bit rounded) inputs."""
 import pytest
 import torch
@@ -134,7 +134,7 @@ def test_conv3x3_replicate_skip_relu(B, H, W, Cin, Cout, dtype):
 
 
 def test_conv3x3_halo_streamed_weights(monkeypatch):
-    """convh_kernel (C_in >= 128: halo boxes + streamed weights) for both tile widths, and the generic kernel it replaces."""
+    """The CONVH mode (C_in >= 128: halo boxes + streamed weights) and the generic per-tap GEMM mode it replaces."""
     for mode in ("2", "0"):
         monkeypatch.setenv("MOGE_B200_CONVH", mode)
         for dtype in (torch.float16, torch.bfloat16):
@@ -144,8 +144,7 @@ def test_conv3x3_halo_streamed_weights(monkeypatch):
 
 
 def test_conv3x3_c64_resident_weights():
-    """conv64_kernel (C_in = 64: resident weights, halo boxes, two MMA-issuing warps on alternate tiles) with one and two
-    output-channel tiles, ragged image edges."""
+    """The CONV64 mode (C_in = 64: resident weights, halo boxes) with one and two output-channel tiles, ragged image edges."""
     for dtype in (torch.float16, torch.bfloat16):
         test_conv3x3_replicate_skip_relu(2, 40, 50, 64, 64, dtype)
         test_conv3x3_replicate_skip_relu(1, 33, 47, 64, 128, dtype)

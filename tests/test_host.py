@@ -17,7 +17,7 @@ def test_library_exports_every_declared_symbol():
     L = capi.lib()
     for name in declared:
         assert hasattr(L, name), name
-    assert b"sm_100a" in L.moge_version()
+    assert b"sm_90a" in L.moge_version()
 
 
 def test_config_struct_roundtrip():
@@ -139,7 +139,7 @@ def test_serving_pipeline_needs_a_cuda_model():
         InferPipeline(m, depth=0)
 
 
-@pytest.mark.parametrize("tag", ["r1", "r2"])
+@pytest.mark.parametrize("tag", ["h100"])
 def test_committed_bench_lines_follow_the_contract(tag):
     """profiles/<tag>_bench_n1.json and <tag>_bench_reference_arm.json are real bench.py lines: check the keys the driver parses."""
     import json
@@ -163,15 +163,11 @@ def test_committed_bench_lines_follow_the_contract(tag):
         assert k in r, k
     assert abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9
     assert {"sm_mhz", "sm_max_mhz", "reasons"} <= set(eng["clocks"])
-    if tag == "r2":
-        gb = eng["gpu_baseline"]                              # same-box PyTorch-CUDA comparator, both 16-bit modes of the reference
-        for mode in ("half", "autocast"):
-            assert gb[mode]["batch1_iters"] >= 200 and gb[mode]["images_per_s"] > 0
-        assert eng["latency"]["iters"] >= 200
-        assert "SURVEY" in eng["roofline_decoder"]["bytes_definition"] and eng["roofline_decoder"]["frac_engine_bytes"] < eng["roofline_decoder"]["frac"]
-        n8 = json.load(open(os.path.join(root, "profiles", "r2_bench_n8.json")))
-        assert n8["n_gpus"] == 8 and n8["value"] == n8["value_with_gather"] and n8["value"] < n8["value_compute_only"]
-        assert n8["gather"]["bytes_to_rank0_per_step"] == 7 * eng["e2e"]["d2h_bytes_per_step"]
+    gb = eng["gpu_baseline"]                              # same-box PyTorch-CUDA comparator, both 16-bit modes of the reference
+    for mode in ("half", "autocast"):
+        assert gb[mode]["batch1_iters"] >= 200 and gb[mode]["images_per_s"] > 0
+    assert eng["latency"]["iters"] >= 200
+    assert "SURVEY" in eng["roofline_decoder"]["bytes_definition"] and eng["roofline_decoder"]["frac_engine_bytes"] < eng["roofline_decoder"]["frac"]
 
 
 def test_all_committed_profile_json_files_parse():

@@ -8,6 +8,7 @@ import torch
 from moge_b200.configs import model_config, token_grid, default_num_tokens
 from moge_b200.synthetic import make_state_dict, synthetic_images, synthetic_point_map
 from oracle import moge_port
+from golden_io import load_golden
 
 FAST_CASES = ["vits_b1_126x168_t192", "vits_b2_140x98_t117", "vitb_b1_98x154_t150_nonormal", "vits_b2_126x168_t192_wp",
               "vits_b1_98x126_t120_linear", "vits_b1_98x126_t120_sinh", "vits_b1_98x126_t120_sinh_exp"]
@@ -20,7 +21,7 @@ def rel_l2(a, b):
 
 @pytest.mark.parametrize("name", FAST_CASES)
 def test_port_matches_reference_golden(name, golden_dir):
-    gold = torch.load(os.path.join(golden_dir, name + ".pt"), weights_only=False)
+    gold = load_golden(golden_dir, name)
     meta = gold["meta"]
     opt = meta.get("options", {})
     cfg = model_config(meta["size"], meta["with_normal"])

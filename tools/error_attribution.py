@@ -1,6 +1,6 @@
 """Where the engine's fp16 deviation from the fp32 reference is born (DESIGN.md section 2, "normal tolerance").
 
-Runs on the GPU box:  python tools/error_attribution.py [--out profiles/r2_error_attribution.json]
+Runs on the GPU:  python tools/error_attribution.py [--out error_attribution.json]
 
 Three measurements on the benchmarked shape (ViT-L, 518x518, 37x37 grid), for a plain random-init checkpoint and for the
 `well_posed` one (near-unit raw normals, like a trained model):
@@ -114,7 +114,7 @@ def oracle_fwd(cfg, sdd, img, nt, capture_raw=None):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--out", default=os.path.join(ROOT, "profiles", "r2_error_attribution.json"))
+    ap.add_argument("--out", default="error_attribution.json")
     a = ap.parse_args()
     torch.backends.cuda.matmul.allow_tf32 = False
     torch.backends.cudnn.allow_tf32 = False

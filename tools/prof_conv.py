@@ -1,4 +1,4 @@
-"""Micro-benchmark of decoder convolutions / attention through the C ABI at the ViT-L batch-32 shapes (for ncu)."""
+"""Micro-benchmark of decoder convolutions / attention through the C ABI at the ViT-L batch-32 shapes."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))

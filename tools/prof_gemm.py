@@ -1,5 +1,5 @@
-"""Micro-benchmark of the tcgen05 GEMM kernel through the C ABI (moge_op_linear): encoder shapes of ViT-L at
-batch 32 x 1370 tokens.  Prints TFLOP/s per epilogue; run under ncu for the hardware counters."""
+"""Micro-benchmark of the wgmma GEMM kernel through the C ABI (moge_op_linear): encoder shapes of ViT-L at
+batch 32 x 1370 tokens.  Prints TFLOP/s per epilogue."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
