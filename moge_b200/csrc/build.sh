@@ -12,7 +12,7 @@ FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler
 # a change of flags (e.g. MG_EXTRA_FLAGS=-DMG_ATT_DEBUG) invalidates every object
 if [ "$(cat $BUILD/.flags 2>/dev/null)" != "$FLAGS" ]; then rm -f $BUILD/*.o; echo "$FLAGS" > $BUILD/.flags; fi
 pids=()
-for f in umma_rows umma_tiles conv64 convh attention elementwise pack tmap peer engine; do
+for f in gemm_rows gemm_tiles conv64 convh gemm attention elementwise pack tmap peer engine; do
   if [ ! -f $BUILD/$f.o ] || [ $f.cu -nt $BUILD/$f.o ] || [ -n "$(find . -maxdepth 1 \( -name '*.cuh' -o -name '*.h' \) -newer $BUILD/$f.o)" ] || [ ../../include/moge_b200.h -nt $BUILD/$f.o ]; then
     ( nvcc $FLAGS -Xptxas -v -c $f.cu -o $BUILD/$f.o > $BUILD/$f.log 2>&1 || { echo "FAILED $f"; grep -E "error" $BUILD/$f.log | head -20; exit 1; } ) &
     pids+=($!)

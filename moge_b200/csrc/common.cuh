@@ -16,7 +16,6 @@ namespace mg {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
     return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }
-__device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
 __device__ __forceinline__ bool elect_one() {
     uint32_t pred;
     asm volatile(
@@ -42,10 +41,6 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void fence_mbar_init() {
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-// generic-proxy writes (st.shared) -> visible to the async proxy (TMA / wgmma operand reads)
-__device__ __forceinline__ void fence_proxy_async_smem() {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -86,12 +81,6 @@ __device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uin
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
         ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
         : "memory");
 }
 __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2,
@@ -136,11 +125,6 @@ __device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return m
 __device__ __forceinline__ float2 fadd2(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
 __device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2(a.x * b.x, a.y * b.y); }
 
-__device__ __forceinline__ float fmax3(float a, float b, float c) {
-    float r;
-    asm("max.f32 %0, %1, %2, %3;" : "=f"(r) : "f"(a), "f"(b), "f"(c));
-    return r;
-}
 __device__ __forceinline__ float ex2_approx(float x) {      // MUFU.EX2, flush-to-zero
     float r;
     asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));

@@ -1,7 +1,7 @@
 // Host runtime of libmoge_b200.so: weight registry + load-time repacking, per-shape execution plans (workspace
 // layout, TMA descriptors, launch list), and the extern "C" ABI declared in include/moge_b200.h.
 #include "moge_b200.h"
-#include "umma_kernel.cuh"
+#include "gemm_kernel.cuh"
 #include "host_api.h"
 
 #include <algorithm>
@@ -35,16 +35,6 @@ struct RawWeight {
     float* p = nullptr;
     std::vector<int64_t> shape;
     size_t numel = 0;
-};
-
-struct Level { int H, W, Hp, Wp; };
-
-struct ConvW {          // packed 3x3 / 1x1 / convT weights for one launch
-    void* w = nullptr;  // [N, Ktot] 16-bit
-    float* bias = nullptr;
-    float* wu = nullptr;
-    float* wv = nullptr;
-    int N = 0, Ktot = 0, cin = 0, caux = 0, taps = 0;
 };
 
 struct StackW {
@@ -179,11 +169,6 @@ static int get_raw(moge_engine* e, const std::string& key, const RawWeight** out
         }
     }
     *out = &it->second;
-    return 0;
-}
-
-static int pick_bn(int N, std::initializer_list<int> cands) {
-    for (int c : cands) if (N % c == 0) return c;
     return 0;
 }
 
@@ -540,106 +525,32 @@ static int add_conv(moge_engine* e, Plan* pl, const ConvW& cw, const void* src, 
                     int epi, void* out_raw, void* out_relu, const void* skip, const Level& go, int out_ch, bool shuffle,
                     bool uv, float su, float sv, const std::string& name, int ncomp = 0, const float* waux = nullptr, void* out2 = nullptr,
                     int accum = 0) {
-    UmmaParams p{};
-    p.N = cw.N; p.ntaps = cw.taps; p.kb_main = cw.cin / 64; p.kb_aux = cw.caux / 64;
-    p.B = B; p.H = gs.H; p.W = gs.W;
-    p.tiles_x = (gs.W + TILE_PW - 1) / TILE_PW; p.tiles_y = (gs.H + TILE_PH - 1) / TILE_PH;
-    p.num_m_tiles = B * p.tiles_x * p.tiles_y;
-    int bn;
-    if (epi == EPI_HEADOUT) bn = 16;
-    else if (epi == EPI_NECKOUT) bn = 32;
-    else bn = pick_bn(cw.N, {128, 64, 32});
-    if (!bn) return set_error("conv: N=%d has no tile width", cw.N);
-    p.num_n_tiles = cw.N / bn;
-    p.out0 = out_raw; p.out1 = out_relu; p.bias = cw.bias;
-    p.vec1 = uv ? cw.wu : nullptr; p.vec2 = uv ? cw.wv : nullptr;
-    p.skip = skip; p.ldo = out_ch;
-    p.Ho = go.H; p.Wo = go.W; p.Hop = go.Hp; p.Wop = go.Wp;
-    p.shuffle = shuffle ? 1 : 0; p.su = su; p.sv = sv;
-    if (epi == EPI_HEADOUT) { p.vec1 = waux; p.ncomp = ncomp; p.accum = accum; }
-    p.out2 = out2;
-    const bool bf16 = e->bf16; const int sms = e->num_sms;
+    GemmLaunch g;
+    MG_TRY(gemm_conv(&g, e->bf16, cw, src, aux, gs, B, epi, out_raw, out_relu, skip, go, out_ch, shuffle, uv, su, sv, ncomp, waux, out2, accum));
     const double px = static_cast<double>(B) * gs.H * gs.W;
     const double flops = 2.0 * px * cw.N * cw.Ktot;
     double bytes = px * cw.cin * 2 + px * cw.caux * 2 + static_cast<double>(cw.N) * cw.Ktot * 2;
     if (epi == EPI_HEADOUT) bytes += 4 * px * (accum ? (ncomp == 1 ? 4 : 16) : 32 * 2) + 4 * px * (ncomp == 1 ? 4 : 16);     // 4 output pixels per low-res pixel
     else if (epi == EPI_NECKOUT) bytes += 4 * px * ((out_raw ? 16 : 0) + (out_relu ? 16 : 0) + (out2 ? 4 : 0));
     else bytes += px * cw.N * 2 * ((out_raw ? 1 : 0) + (out_relu ? 1 : 0)) + (skip ? px * cw.N * 2 : 0);
-    CUtensorMap ma, mx, mb;
-    // C_in = 64 3x3 convs (levels 3/4): resident weights + one halo box per horizontal tap (umma_kernel<MODE_CONV64>)
-    const bool use64 = cw.taps == 9 && cw.cin == 64 && (cw.caux == 0 || cw.caux == 64) && gs.Hp >= 10 &&
-                       ((epi == EPI_HEADOUT && cw.N == 16) || (epi == EPI_NECKOUT && cw.N == 32) || (epi == EPI_DEC && cw.N % 64 == 0));
-    if (use64) {
-        const int bn64 = (epi == EPI_HEADOUT) ? 16 : (epi == EPI_NECKOUT) ? 32 : 64;
-        p.num_n_tiles = cw.N / bn64;
-        MG_TRY(make_map_nhwc(&ma, src, cw.cin, gs.Wp, gs.Hp, B, 10));
-        if (cw.caux) MG_TRY(make_map_nhwc(&mx, aux, cw.caux, gs.Wp, gs.Hp, B, 8));
-        else mx = ma;
-        MG_TRY(make_map_2d(&mb, cw.w, cw.Ktot, cw.N, cw.Ktot, bn64));
-        pl->ops.add([=](cudaStream_t st) { return launch_conv64(bn64, epi, bf16, ma, mx, mb, p, sms, st); }, name, flops, bytes);
-        return 0;
-    }
-    // C_in >= 128 3x3 convs (levels 1/2): halo boxes for the pixels + streamed weights (umma_kernel<MODE_CONVH>); MOGE_B200_CONVH=0 disables
-    static const int convh_mode = [] { const char* v = getenv("MOGE_B200_CONVH"); return v ? atoi(v) : 2; }();
-    const bool useh = convh_mode != 0 && epi == EPI_DEC && cw.taps == 9 && cw.cin >= 128 && cw.cin % 64 == 0 && cw.caux % 64 == 0 &&
-                      gs.Hp >= 10 && convh_supports(bn, p);
-    if (useh) {
-        MG_TRY(make_map_nhwc(&ma, src, cw.cin, gs.Wp, gs.Hp, B, 10));
-        if (cw.caux) MG_TRY(make_map_nhwc(&mx, aux, cw.caux, gs.Wp, gs.Hp, B, 8));
-        else mx = ma;
-        MG_TRY(make_map_2d(&mb, cw.w, cw.Ktot, cw.N, cw.Ktot, bn));
-        pl->ops.add([=](cudaStream_t st) { return launch_convh(bn, bf16, ma, mx, mb, p, sms, st); }, name, flops, bytes);
-        return 0;
-    }
-    MG_TRY(make_map_nhwc(&ma, src, cw.cin, gs.Wp, gs.Hp, B));
-    if (cw.caux) MG_TRY(make_map_nhwc(&mx, aux, cw.caux, gs.Wp, gs.Hp, B));
-    else mx = ma;
-    MG_TRY(make_map_2d(&mb, cw.w, cw.Ktot, cw.N, cw.Ktot, bn));
-    pl->ops.add([=](cudaStream_t st) { return launch_umma(bn, AMODE_TILES, epi, bf16, ma, mx, mb, p, sms, st); }, name, flops, bytes);
+    const int sms = e->num_sms;
+    pl->ops.add([=](cudaStream_t st) { return launch_gemm(g, sms, st); }, name, flops, bytes);
     return 0;
 }
 
-constexpr int kStatsLd = 16;      // partial-sum slots per row of the LayerNorm statistics buffer
-struct LnIO {                     // LayerNorm-fold plumbing of one linear (see elementwise.cu)
-    void* x16 = nullptr;          // producer (EPI_RESID / EPI_PATCH): 16-bit copy of the rows it writes
-    float2* stats_out = nullptr;  // producer: partial sums
-    int* parts_out = nullptr;     // producer: number of column groups it writes per row
-    const float* ln_rstd = nullptr;       // consumer (EPI_STORE16 / EPI_GELU16)
-};
-static int add_linear(moge_engine* e, Plan* pl, const void* A, int M, int K, int lda, const void* W, int N, int epi,
-                      void* out, const float* bias, const float* v1, int ldo, const std::string& name, int T = 0, int gridw = 0,
-                      const LnIO* ln = nullptr, int force_bn = 0, int* bn_out = nullptr) {
-    UmmaParams p{};
-    p.M = M; p.N = N; p.ntaps = 1; p.kb_main = (K + 63) / 64; p.kb_aux = 0;
-    p.num_m_tiles = (M + TILE_M - 1) / TILE_M;
-    int bn = pick_bn(N, {128});
-    if (!bn) return set_error("linear: N=%d must be a multiple of 128", N);
-    if (force_bn) bn = force_bn;
-    if (bn_out) *bn_out = bn;
-    p.num_n_tiles = N / bn;
-    p.out0 = out; p.bias = bias; p.vec1 = v1; p.ldo = ldo; p.T = T; p.W = gridw;
-    double ln_extra_bytes = 0;
-    if (ln) {
-        const int parts = N / (bn / 2);             // every ROWS kernel has 8 epilogue warps: column groups of BN/2
-        p.stats_ld = kStatsLd;
-        if (ln->x16) {
-            if (parts > kStatsLd) return set_error("linear %s: %d statistics groups per row > %d", name.c_str(), parts, kStatsLd);
-            p.x16 = ln->x16; p.stats_out = ln->stats_out;
-            if (ln->parts_out) *ln->parts_out = parts;
-            ln_extra_bytes = static_cast<double>(M) * N * 2;
-        }
-        if (ln->ln_rstd) p.ln_rstd = ln->ln_rstd;
-    }
-    CUtensorMap ma, mb;
-    MG_TRY(make_map_2d(&ma, A, K, M, lda, TILE_M));
-    const bool bf16 = e->bf16; const int sms = e->num_sms;
-    MG_TRY(make_map_2d(&mb, W, K, N, lda, bn));
+// Linear over row-major A [M, K] with the engine's packed (dense [N, K]) weight W; trailing arguments as in gemm_linear.
+static int add_linear(moge_engine* e, Plan* pl, const void* A, int M, int K, const void* W, int N, int epi, void* out, const float* bias,
+                      const float* v1, int ldo, const std::string& name, const LnIO* ln = nullptr, const Level* grid = nullptr,
+                      void* out_relu = nullptr, const float* v2 = nullptr, float su = 0.f, float sv = 0.f) {
+    GemmLaunch g;
+    MG_TRY(gemm_linear(&g, e->bf16, A, M, K, W, K, N, epi, out, ldo, bias, v1, ln, grid, out_relu, v2, su, sv));
     const double flops = 2.0 * M * static_cast<double>(N) * K;
     double bytes = static_cast<double>(M) * K * 2 + static_cast<double>(N) * K * 2;
-    bytes += (epi == EPI_RESID) ? static_cast<double>(M) * N * 8 : (epi == EPI_PATCH) ? static_cast<double>(M) * N * 4 + static_cast<double>(T) * N * 4
+    bytes += (epi == EPI_RESID) ? static_cast<double>(M) * N * 8 : (epi == EPI_PATCH) ? static_cast<double>(M) * N * 4 + static_cast<double>(g.p.T) * N * 4
                                                                                       : static_cast<double>(M) * N * 2;
-    bytes += ln_extra_bytes;
-    pl->ops.add([=](cudaStream_t st) { return launch_umma(bn, AMODE_ROWS, epi, bf16, ma, ma, mb, p, sms, st); }, name, flops, bytes);
+    if (ln && ln->x16) bytes += static_cast<double>(M) * N * 2;
+    const int sms = e->num_sms;
+    pl->ops.add([=](cudaStream_t st) { return launch_gemm(g, sms, st); }, name, flops, bytes);
     return 0;
 }
 
@@ -786,11 +697,6 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     auto gname = [&](const char* base, int gi) { return G == 1 ? std::string(base) : std::string(base) + ".g" + std::to_string(gi); };
     // ---- per group: K1 resize + normalise + patchify (phase 0: reads the caller's image), K2/K3 patch embed + pos embed, cls rows
     int parts_x = 0;              // column groups per row of the statistics the NEXT consumer reads
-    int bn_patch = 0;
-    {   // one tile width for every group's patch-embed GEMM (the statistics layout must agree)
-        bn_patch = pick_bn(D, {128});
-        if (!bn_patch) return set_error("embed_dim=%d must be a multiple of 128", D);
-    }
     long prow = 0;                // first patch row of the group in `patches` / `taps`
     std::vector<long> prow0(G);
     for (int gi = 0; gi < G; ++gi) {
@@ -810,8 +716,9 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         uint8_t* ln_g = ln + static_cast<size_t>(g.row0) * D * 2;
         float2* stats_g = stats + static_cast<size_t>(g.row0) * kStatsLd;
         LnIO prod; prod.x16 = ln_g; prod.stats_out = stats_g; prod.parts_out = &parts_x;
-        MG_TRY(add_linear(e, pl, patches_g, B * T, 592, 592, e->w_patch, D, EPI_PATCH, x_g, nullptr, g.pos_table, D, gname("gemm.patch_embed", gi), T, w,
-                          fold ? &prod : nullptr, bn_patch));
+        const Level grid = level_geom(h, w, 0);
+        MG_TRY(add_linear(e, pl, patches_g, B * T, 592, e->w_patch, D, EPI_PATCH, x_g, nullptr, g.pos_table, D, gname("gemm.patch_embed", gi),
+                          fold ? &prod : nullptr, &grid));
         pl->ops.add([=](cudaStream_t st) { return launch_init_cls(x_g, P->cls_row, B, N, D, st); }, gname("init_cls", gi));
         if (fold) {
             const int parts0 = parts_x;
@@ -853,10 +760,10 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         if (fold) {
             if (i == 0) add_rstd(parts_x);
             LnIO cons; cons.ln_rstd = rstd;
-            MG_TRY(add_linear(e, pl, ln, Mi, D, D, b.wqkv_ln, 3 * D, EPI_STORE16, qkv, b.b_qkv_ln, nullptr, 3 * D, "gemm.qkv", 0, 0, &cons));
+            MG_TRY(add_linear(e, pl, ln, Mi, D, b.wqkv_ln, 3 * D, EPI_STORE16, qkv, b.b_qkv_ln, nullptr, 3 * D, "gemm.qkv", &cons));
         } else {
             pl->ops.add([=](cudaStream_t st) { return launch_layernorm(x, b.ln1g, b.ln1b, ln, Mi, D, D, 0, 0, 1, nullptr, bf16, st); }, "layernorm", 0, ln_bytes);
-            MG_TRY(add_linear(e, pl, ln, Mi, D, D, b.wqkv, 3 * D, EPI_STORE16, qkv, b.bqkv, nullptr, 3 * D, "gemm.qkv"));
+            MG_TRY(add_linear(e, pl, ln, Mi, D, b.wqkv, 3 * D, EPI_STORE16, qkv, b.bqkv, nullptr, 3 * D, "gemm.qkv"));
         }
         {
             CUtensorMap mq;
@@ -866,17 +773,17 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
                         att_flops, static_cast<double>(M) * D * 8);
         }
         if (fold) {
-            MG_TRY(add_linear(e, pl, att, Mi, D, D, b.wproj, D, EPI_RESID, x, b.bproj, b.g1, D, "gemm.proj", 0, 0, &prod));
+            MG_TRY(add_linear(e, pl, att, Mi, D, b.wproj, D, EPI_RESID, x, b.bproj, b.g1, D, "gemm.proj", &prod));
             add_rstd(parts_x);
             LnIO cons; cons.ln_rstd = rstd;
-            MG_TRY(add_linear(e, pl, ln, Mi, D, D, b.wfc1_ln, 4 * D, EPI_GELU16, hid, b.b_fc1_ln, nullptr, 4 * D, "gemm.fc1", 0, 0, &cons));
-            MG_TRY(add_linear(e, pl, hid, Mi, 4 * D, 4 * D, b.wfc2, D, EPI_RESID, x, b.bfc2, b.g2, D, "gemm.fc2", 0, 0, (i + 1 < c.depth) ? &prod : nullptr));
+            MG_TRY(add_linear(e, pl, ln, Mi, D, b.wfc1_ln, 4 * D, EPI_GELU16, hid, b.b_fc1_ln, nullptr, 4 * D, "gemm.fc1", &cons));
+            MG_TRY(add_linear(e, pl, hid, Mi, 4 * D, b.wfc2, D, EPI_RESID, x, b.bfc2, b.g2, D, "gemm.fc2", (i + 1 < c.depth) ? &prod : nullptr));
             if (i + 1 < c.depth) add_rstd(parts_x);
         } else {
-            MG_TRY(add_linear(e, pl, att, Mi, D, D, b.wproj, D, EPI_RESID, x, b.bproj, b.g1, D, "gemm.proj"));
+            MG_TRY(add_linear(e, pl, att, Mi, D, b.wproj, D, EPI_RESID, x, b.bproj, b.g1, D, "gemm.proj"));
             pl->ops.add([=](cudaStream_t st) { return launch_layernorm(x, b.ln2g, b.ln2b, ln, Mi, D, D, 0, 0, 1, nullptr, bf16, st); }, "layernorm", 0, ln_bytes);
-            MG_TRY(add_linear(e, pl, ln, Mi, D, D, b.wfc1, 4 * D, EPI_GELU16, hid, b.bfc1, nullptr, 4 * D, "gemm.fc1"));
-            MG_TRY(add_linear(e, pl, hid, Mi, 4 * D, 4 * D, b.wfc2, D, EPI_RESID, x, b.bfc2, b.g2, D, "gemm.fc2"));
+            MG_TRY(add_linear(e, pl, ln, Mi, D, b.wfc1, 4 * D, EPI_GELU16, hid, b.bfc1, nullptr, 4 * D, "gemm.fc1"));
+            MG_TRY(add_linear(e, pl, hid, Mi, 4 * D, b.wfc2, D, EPI_RESID, x, b.bfc2, b.g2, D, "gemm.fc2"));
         }
         if (tap_idx < c.num_taps && c.taps[tap_idx] == i) {
             const int j = tap_idx++;
@@ -908,22 +815,9 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         {
             const Level g0 = level_geom(h, w, 0);
             const ConvW& f = e->fold0;
-            UmmaParams p{};
-            p.M = B * T; p.N = f.N; p.ntaps = 1; p.kb_main = f.Ktot / 64; p.kb_aux = 0;
             if (f.Ktot % 64) return set_error("num_taps*embed_dim must be a multiple of 64");
-            p.num_m_tiles = (p.M + TILE_M - 1) / TILE_M;
-            const int bn = pick_bn(f.N, {128});
-            if (!bn) return set_error("neck width %d must be a multiple of 128", f.N);
-            p.num_n_tiles = f.N / bn;
-            p.B = B; p.H = h; p.W = w; p.T = T;
-            p.out0 = nb.x_raw[0]; p.out1 = c.neck.num_res_blocks[0] > 0 ? nb.x_relu[0] : nullptr;
-            p.bias = f.bias; p.vec1 = f.wu; p.vec2 = f.wv; p.ldo = f.N;
-            p.Ho = g0.H; p.Wo = g0.W; p.Hop = g0.Hp; p.Wop = g0.Wp; p.su = su; p.sv = sv;
-            CUtensorMap ma, mb;
-            MG_TRY(make_map_2d(&ma, taps_g, f.Ktot, p.M, f.Ktot, TILE_M));
-            MG_TRY(make_map_2d(&mb, f.w, f.Ktot, f.N, f.Ktot, bn));
-            pl->ops.add([=](cudaStream_t st) { return launch_umma(bn, AMODE_ROWS, EPI_DEC, bf16, ma, ma, mb, p, sms, st); }, gname("gemm.taps_proj", gi),
-                        2.0 * p.M * static_cast<double>(f.N) * f.Ktot, static_cast<double>(p.M) * f.Ktot * 2 + static_cast<double>(f.N) * f.Ktot * 2 + static_cast<double>(p.M) * f.N * 2);
+            MG_TRY(add_linear(e, pl, taps_g, B * T, f.Ktot, f.w, f.N, EPI_DEC, nb.x_raw[0], f.bias, f.wu, f.N, gname("gemm.taps_proj", gi), nullptr,
+                              &g0, c.neck.num_res_blocks[0] > 0 ? nb.x_relu[0] : nullptr, f.wv, su, sv));
         }
         void* neck_lowres[3] = {pts_lr[gi], nrm_lr[gi], msk_lr[gi]};
         const std::string sfx = G == 1 ? std::string() : ".g" + std::to_string(gi);
@@ -1276,17 +1170,10 @@ static int dev_sms() {
 int moge_op_linear(const void* x, const void* w, const float* bias, const float* gamma, void* out, int M, int N, int K, int epi,
                    int dtype, void* stream) {
     if (K % 8) return set_error("op_linear: K must be a multiple of 8");
-    const int bn = pick_bn(N, {128});
-    if (!bn) return set_error("op_linear: N must be a multiple of 128");
     if (epi < 0 || epi > 2) return set_error("op_linear: epi must be 0..2");
-    UmmaParams p{};
-    p.M = M; p.N = N; p.ntaps = 1; p.kb_main = (K + 63) / 64;
-    p.num_m_tiles = (M + TILE_M - 1) / TILE_M; p.num_n_tiles = N / bn;
-    p.out0 = out; p.bias = bias; p.vec1 = gamma; p.ldo = N;
-    CUtensorMap ma, mb;
-    MG_TRY(make_map_2d(&ma, x, K, M, K, TILE_M));
-    MG_TRY(make_map_2d(&mb, w, K, N, K, bn));
-    return launch_umma(bn, AMODE_ROWS, epi, dtype == MOGE_BF16, ma, ma, mb, p, dev_sms(), static_cast<cudaStream_t>(stream));
+    GemmLaunch g;
+    MG_TRY(gemm_linear(&g, dtype == MOGE_BF16, x, M, K, w, K, N, epi, out, N, bias, gamma));
+    return launch_gemm(g, dev_sms(), static_cast<cudaStream_t>(stream));
 }
 
 int moge_op_attention(const void* qkv, void* out, int B, int N, int D, int heads, int dtype, void* stream) {
@@ -1342,8 +1229,6 @@ int moge_op_linear_ln(const float* x, const float* ln_gamma, const float* ln_bet
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const bool bf16 = dtype == MOGE_BF16;
     if (K % 64) return set_error("op_linear_ln: K must be a multiple of 64");
-    const int bn = pick_bn(N, {128});
-    if (!bn) return set_error("op_linear_ln: N must be a multiple of 128");
     if (epi != EPI_STORE16 && epi != EPI_GELU16) return set_error("op_linear_ln: epi must be 0 (store) or 1 (GELU)");
     void *x16 = nullptr, *w16 = nullptr;
     float2* stats = nullptr;
@@ -1353,22 +1238,14 @@ int moge_op_linear_ln(const float* x, const float* ln_gamma, const float* ln_bet
         cudaMalloc(&stats, static_cast<size_t>(M) * kStatsLd * 8) != cudaSuccess || cudaMalloc(&rstd, static_cast<size_t>(M) * 4) != cudaSuccess ||
         cudaMalloc(&b2, static_cast<size_t>(N) * 4) != cudaSuccess)
         rc = set_error("op_linear_ln: cudaMalloc failed");
+    LnIO cons;
+    cons.ln_rstd = rstd;
+    GemmLaunch g;
+    if (rc == 0) rc = gemm_linear(&g, bf16, x16, M, K, w16, K, N, epi, out, N, b2, nullptr, &cons);
     if (rc == 0) rc = launch_ln_prepare(x, M, K, K, x16, K, stats, kStatsLd, 1, bf16, st);
     if (rc == 0) rc = launch_ln_rstd(stats, kStatsLd, 1, M, K, rstd, st);
     if (rc == 0) rc = launch_ln_fold(w, ln_gamma, ln_beta, bias, N, K, K, w16, b2, bf16, st);
-    if (rc == 0) {
-        UmmaParams p{};
-        p.M = M; p.N = N; p.ntaps = 1; p.kb_main = K / 64;
-        p.num_m_tiles = (M + TILE_M - 1) / TILE_M; p.num_n_tiles = N / bn;
-        p.out0 = out; p.bias = b2; p.ldo = N;
-        p.ln_rstd = rstd;
-        CUtensorMap ma, mb;
-        rc = make_map_2d(&ma, x16, K, M, K, TILE_M);
-        if (rc == 0) {
-            rc = make_map_2d(&mb, w16, K, N, K, bn);
-            if (rc == 0) rc = launch_umma(bn, AMODE_ROWS, epi, bf16, ma, ma, mb, p, dev_sms(), st);
-        }
-    }
+    if (rc == 0) rc = launch_gemm(g, dev_sms(), st);
     cudaStreamSynchronize(st);
     cudaFree(x16); cudaFree(w16); cudaFree(stats); cudaFree(rstd); cudaFree(b2);
     return rc;
@@ -1386,39 +1263,17 @@ int moge_op_conv(const void* x, const float* w, const float* bias, const void* s
     if (taps != 1 && taps != 9) return set_error("op_conv: taps must be 1 or 9");
     if (shuffle && taps != 1) return set_error("op_conv: shuffle requires taps=1");
     const int N = shuffle ? 4 * Cout : Cout;
-    const int bn = pick_bn(N, {128, 64, 32});
-    if (!bn) return set_error("op_conv: Cout must be a multiple of 32");
     const int Ktot = taps * Cin;
     void* wp = nullptr;
     CUDA_TRY(cudaMalloc(&wp, static_cast<size_t>(N) * Ktot * 2));
     int rc = shuffle ? launch_pack_convT(w, wp, bf16, Cin, Cout, st) : launch_pack_conv(w, wp, bf16, Cout, Cin, taps, Ktot, 0, st);
     if (rc == 0) {
-        Level gs{H, W, std::max(H + 2, TILE_PH), std::max(W + 2, TILE_PW)};
-        Level go = gs;
-        if (shuffle) go = Level{2 * H, 2 * W, std::max(2 * H + 2, TILE_PH), std::max(2 * W + 2, TILE_PW)};
-        UmmaParams p{};
-        p.N = N; p.ntaps = taps; p.kb_main = Cin / 64; p.kb_aux = 0;
-        p.B = B; p.H = H; p.W = W;
-        p.tiles_x = (W + TILE_PW - 1) / TILE_PW; p.tiles_y = (H + TILE_PH - 1) / TILE_PH;
-        p.num_m_tiles = B * p.tiles_x * p.tiles_y; p.num_n_tiles = N / bn;
-        p.out0 = out_raw; p.out1 = out_relu; p.bias = bias; p.skip = skip; p.ldo = Cout;
-        p.Ho = go.H; p.Wo = go.W; p.Hop = go.Hp; p.Wop = go.Wp; p.shuffle = shuffle;
-        CUtensorMap ma, mb;
-        if (taps == 9 && Cin == 64 && N % 64 == 0 && gs.Hp >= 10) {
-            p.num_n_tiles = N / 64;
-            rc = make_map_nhwc(&ma, x, Cin, gs.Wp, gs.Hp, B, 10);
-            if (rc == 0) rc = make_map_2d(&mb, wp, Ktot, N, Ktot, 64);
-            if (rc == 0) rc = launch_conv64(64, EPI_DEC, bf16, ma, ma, mb, p, dev_sms(), st);
-        } else if (taps == 9 && Cin >= 128 && gs.Hp >= 10 && convh_supports(bn, p) &&
-                   [] { const char* v = getenv("MOGE_B200_CONVH"); return v == nullptr || atoi(v) != 0; }()) {
-            rc = make_map_nhwc(&ma, x, Cin, gs.Wp, gs.Hp, B, 10);
-            if (rc == 0) rc = make_map_2d(&mb, wp, Ktot, N, Ktot, bn);
-            if (rc == 0) rc = launch_convh(bn, bf16, ma, ma, mb, p, dev_sms(), st);
-        } else {
-            rc = make_map_nhwc(&ma, x, Cin, gs.Wp, gs.Hp, B);
-            if (rc == 0) rc = make_map_2d(&mb, wp, Ktot, N, Ktot, bn);
-            if (rc == 0) rc = launch_umma(bn, AMODE_TILES, EPI_DEC, bf16, ma, ma, mb, p, dev_sms(), st);
-        }
+        ConvW cw;
+        cw.w = wp; cw.bias = const_cast<float*>(bias); cw.N = N; cw.Ktot = Ktot; cw.cin = Cin; cw.taps = taps;
+        const Level gs = level_geom(H, W, 0), go = level_geom(H, W, shuffle ? 1 : 0);
+        GemmLaunch g;
+        rc = gemm_conv(&g, bf16, cw, x, nullptr, gs, B, EPI_DEC, out_raw, out_relu, skip, go, Cout, shuffle != 0, false, 0.f, 0.f);
+        if (rc == 0) rc = launch_gemm(g, dev_sms(), st);
     }
     cudaStreamSynchronize(st);
     cudaFree(wp);

@@ -71,24 +71,42 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
 // ---- TMA descriptors (driver entry point resolved at run time; no link-time libcuda dependency)
 // 16-bit element maps with a 64-element (128-byte) inner box and SWIZZLE_128B.
 int make_map_2d(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint64_t row_pitch_elems, uint32_t box_rows);
-int make_map_3d(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint64_t batch, uint32_t box_rows);
 // padded NHWC image [B, Hp, Wp, C]: box {64 ch, 16 px, 8 rows, 1}
 int make_map_nhwc(CUtensorMap* m, const void* base, uint64_t C, uint64_t Wp, uint64_t Hp, uint64_t B, uint32_t box_rows = 8);
 
-struct UmmaParams;
-// bn in {16,32,64,128}; amode/epi as in umma_kernel.cuh
-int launch_umma(int bn, int amode, int epi, bool bf16, const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& b,
-                const UmmaParams& p, int num_sms, cudaStream_t st);
+// ---- gemm_kernel launches (gemm.cu).  The builders choose the kernel variant (main-loop mode, tile width, epilogue) and fill its
+// params and tensor maps; launch_gemm runs the result.  A builder fails (returns -1) on a shape no variant covers.
+struct GemmLaunch;
+struct Level { int H, W, Hp, Wp; };      // an image grid and its padded NHWC allocation (1-pixel replicated border)
 
-// 3x3 conv with C_in = 64: resident weights + 3 halo boxes per tile (umma_kernel<MODE_CONV64>); a: box {64,16,10}, aux: box {64,16,8}
-int launch_conv64(int bn, int epi, bool bf16, const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& w, const UmmaParams& p,
-                  int num_sms, cudaStream_t st);
+struct ConvW {          // packed 3x3 / 1x1 / convT weights for one launch
+    void* w = nullptr;  // [N, Ktot] 16-bit
+    float* bias = nullptr;
+    float* wu = nullptr;
+    float* wv = nullptr;
+    int N = 0, Ktot = 0, cin = 0, caux = 0, taps = 0;
+};
 
-// 3x3 conv with C_in >= 128 (levels 1-2): halo boxes {64,16,10} for the pixels, streamed weight blocks (umma_kernel<MODE_CONVH>);
-// a: box {64,16,10}, aux: box {64,16,8}, w: box {64, bn}
-bool convh_supports(int bn, const UmmaParams& p);
-int launch_convh(int bn, bool bf16, const CUtensorMap& a, const CUtensorMap& aux, const CUtensorMap& w, const UmmaParams& p, int num_sms,
-                 cudaStream_t st);
+constexpr int kStatsLd = 16;      // partial-sum slots per row of the LayerNorm statistics buffer
+struct LnIO {                     // LayerNorm-fold plumbing of one linear (see elementwise.cu)
+    void* x16 = nullptr;          // producer (EPI_RESID / EPI_PATCH): 16-bit copy of the rows it writes
+    float2* stats_out = nullptr;  // producer: partial sums
+    int* parts_out = nullptr;     // producer: number of column groups it writes per row
+    const float* ln_rstd = nullptr;       // consumer (EPI_STORE16 / EPI_GELU16)
+};
+
+// Linear: A [M, K] (row pitch K) times the weight W [N, K] (row pitch ldw) -> epilogue `epi` into out (row pitch ldo elements),
+// N a multiple of 128.  EPI_PATCH and EPI_DEC rows are the tokens of images on the token grid `grid`; EPI_DEC writes the padded
+// NHWC map of that grid (raw: out, ReLU copy: out_relu, UV terms v1/v2 with half extents su/sv).
+int gemm_linear(GemmLaunch* g, bool bf16, const void* A, int M, int K, const void* W, int ldw, int N, int epi, void* out, int ldo,
+                const float* bias, const float* v1, const LnIO* ln = nullptr, const Level* grid = nullptr, void* out_relu = nullptr,
+                const float* v2 = nullptr, float su = 0.f, float sv = 0.f);
+// Conv on padded NHWC maps: source src (+ aux, the fused 1x1 input block) on grid gs, output on grid go with out_ch channels.
+// Picks the main loop from the shape: CONV64 (3x3, C_in = 64), CONVH (3x3, C_in >= 128) or the per-tap GEMM.
+int gemm_conv(GemmLaunch* g, bool bf16, const ConvW& cw, const void* src, const void* aux, const Level& gs, int B, int epi,
+              void* out_raw, void* out_relu, const void* skip, const Level& go, int out_ch, bool shuffle, bool uv, float su, float sv,
+              int ncomp = 0, const float* waux = nullptr, void* out2 = nullptr, int accum = 0);
+int launch_gemm(const GemmLaunch& g, int num_sms, cudaStream_t st);
 
 // Attention over PACKED token rows (ragged batches): qkv [rows, 3D] (map: box {64, 128}), one work item per (image, head, pair
 // of 128-row query tiles); the persistent kernel's CTA c walks items [ranges[c].x, ranges[c].y).

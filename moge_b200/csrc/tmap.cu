@@ -69,12 +69,6 @@ int make_map_2d(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, 
     cuuint32_t box[2] = {64, box_rows};
     return encode(m, base, 2, dims, strides, box);
 }
-int make_map_3d(CUtensorMap* m, const void* base, uint64_t cols, uint64_t rows, uint64_t batch, uint32_t box_rows) {
-    cuuint64_t dims[3] = {cols, rows, batch};
-    cuuint64_t strides[2] = {cols * 2, cols * rows * 2};
-    cuuint32_t box[3] = {64, box_rows, 1};
-    return encode(m, base, 3, dims, strides, box);
-}
 int make_map_nhwc(CUtensorMap* m, const void* base, uint64_t C, uint64_t Wp, uint64_t Hp, uint64_t B, uint32_t box_rows) {
     cuuint64_t dims[4] = {C, Wp, Hp, B};
     cuuint64_t strides[3] = {C * 2, C * Wp * 2, C * Wp * Hp * 2};

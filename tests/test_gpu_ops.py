@@ -133,14 +133,16 @@ def test_conv3x3_replicate_skip_relu(B, H, W, Cin, Cout, dtype):
     assert border_ok(raw, H, W) and border_ok(relu, H, W)
 
 
-def test_conv3x3_halo_streamed_weights(monkeypatch):
-    """The CONVH mode (C_in >= 128: halo boxes + streamed weights) and the generic per-tap GEMM mode it replaces."""
-    for mode in ("2", "0"):
-        monkeypatch.setenv("MOGE_B200_CONVH", mode)
-        for dtype in (torch.float16, torch.bfloat16):
-            test_conv3x3_replicate_skip_relu(2, 24, 40, 256, 256, dtype)
-            test_conv3x3_replicate_skip_relu(1, 37, 37, 128, 128, dtype)
-            test_conv3x3_replicate_skip_relu(1, 21, 50, 192, 128, dtype)
+def test_conv3x3_halo_streamed_weights():
+    """3x3 convs with C_in >= 128.  Images at least 8 pixels tall (padded height >= 10, one halo box) take the CONVH mode
+    (halo boxes + streamed weights); the 6-pixel-tall ones (padded height 8) take the per-tap GEMM mode."""
+    for dtype in (torch.float16, torch.bfloat16):
+        test_conv3x3_replicate_skip_relu(2, 24, 40, 256, 256, dtype)      # CONVH
+        test_conv3x3_replicate_skip_relu(1, 37, 37, 128, 128, dtype)      # CONVH
+        test_conv3x3_replicate_skip_relu(1, 21, 50, 192, 128, dtype)      # CONVH
+        test_conv3x3_replicate_skip_relu(2, 6, 40, 256, 256, dtype)       # per-tap GEMM
+        test_conv3x3_replicate_skip_relu(1, 6, 37, 128, 128, dtype)       # per-tap GEMM
+        test_conv3x3_replicate_skip_relu(1, 6, 50, 192, 128, dtype)       # per-tap GEMM
 
 
 def test_conv3x3_c64_resident_weights():
