@@ -169,6 +169,32 @@ int moge_op_layernorm(const float* x, const float* gamma, const float* beta, voi
 int moge_op_conv(const void* x, const float* w, const float* bias, const void* skip, void* out_raw, void* out_relu,
                  int B, int H, int W, int Cin, int Cout, int taps, int shuffle, int dtype, void* stream);
 
+/* ---- truncated-L1 alignment solvers (moge/utils/alignment.py; Python: moge_b200.alignment, alias moge.utils.alignment).
+ * A problem is n elements (x, y, w), w >= 0; it is solved as align() (alignment.py:52-146) solves it: after x, y *= sign(x), either
+ * the lower weighted median of y / max(x, 1e-7) with weights w x (untruncated) or the least of sum_i min(t_i, w_i |a x_i - y_i|) over
+ * its local minima at those candidates (truncated; element 0 when there is none).  Candidate keys are the reference's fp32 values;
+ * prefix sums and objectives are fp64.  Inputs are contiguous fp32 device arrays.  Elements per problem are bounded: plain problems
+ * at n <= 12288, anchored ones at n <= 4096 points (the 64x64 grid of the reference's callers); larger n fails before any launch.
+ * The truncated solvers and the anchored ones need a workspace (256-byte aligned) of moge_align_workspace_bytes; it depends on the
+ * current device's SM count.  Results are deterministic and do not depend on the other problems of the batch. */
+enum { MOGE_ALIGN_PLAIN = 0, MOGE_ANCHOR_DEPTH = 1, MOGE_ANCHOR_POINTS_Z = 2, MOGE_ANCHOR_POINTS_XYZ = 3 };
+int moge_align_workspace_bytes(int mode, int truncated, int64_t batch, int n, size_t* bytes);
+/* align(): `batch` problems of n elements, rows x, y, w (batch, n).  trunc: NULL = untruncated, else a device pointer to one scalar
+ * (trunc_per_elem = 0) or to (batch, n) values.  Outputs (batch,): a = y_i / max(x_i, 1e-7) at the chosen element (signs flipped),
+ * loss = the objective there, index = the element.                                                                           */
+int moge_align(const float* x, const float* y, const float* w, const float* trunc, int trunc_per_elem, int64_t batch, int n, float* a,
+               float* loss, int64_t* index, void* workspace, size_t workspace_bytes, void* stream);
+/* the anchored solvers (alignment.py:163-214 depth affine, 251-302 points scale + z shift, 305-355 points scale + xyz shift):
+ * src, tgt (batch, n) for MOGE_ANCHOR_DEPTH, else (batch, n, 3); w (batch, n).  For every anchor p with w_p > 0 the problem
+ * x = src - src_p, y = tgt - tgt_p (POINTS_Z: only z is anchored; points are flattened to 3n elements, w repeated) is solved;
+ * trunc < 0 = untruncated.  Per image: the least (loss, anchor, index), ties to the smallest anchor then index; an image
+ * without a positive weight gets loss = +inf, anchor = index = -1.                                                          */
+int moge_align_anchored(const float* src, const float* tgt, const float* w, int mode, float trunc, int64_t batch, int n, float* loss,
+                        int64_t* anchor, int64_t* index, void* workspace, size_t workspace_bytes, void* stream);
+/* align_affine_lstsq (alignment.py:399-416): the least-squares solution of [sqrt(w) x, 1] (a, b)^T = sqrt(w) y per problem, as the
+ * reference's torch.linalg.lstsq call poses it (the column of ones is not weighted); w NULL = 1.  fp64 accumulation, any n.  */
+int moge_align_affine_lstsq(const float* x, const float* y, const float* w, int64_t batch, int64_t n, float* a, float* b, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -1,0 +1,1 @@
+"""Drop-in alias of the reference's `moge.utils` package: `moge.utils.alignment` resolves to the GPU solvers (moge_b200.alignment)."""

@@ -15,6 +15,8 @@ LIB_PATH = os.environ.get("MOGE_B200_LIB") or os.path.join(_HERE, "_lib", "libmo
 
 MOGE_MAX_LEVELS, MOGE_MAX_TAPS, MOGE_MAX_MLP = 8, 8, 8
 F32, F16, BF16, U8 = 0, 1, 2, 3
+ALIGN_PLAIN, ANCHOR_DEPTH, ANCHOR_POINTS_Z, ANCHOR_POINTS_XYZ = 0, 1, 2, 3
+ALIGN_MAX_POINTS = 4096          # points per anchored problem (elements per plain problem: 3x)
 REMAP = {"linear": 0, "sinh": 1, "exp": 2, "sinh_exp": 3}
 RESAMPLE = {"conv_transpose": 0, "bilinear": 1}
 
@@ -24,6 +26,7 @@ EXPORTS = [
     "moge_engine_forward_groups", "moge_engine_num_ops", "moge_engine_op_info", "moge_engine_profile", "moge_attention_work_list", "moge_recover_focal_shift",
     "moge_postprocess", "moge_peer_alloc", "moge_peer_free", "moge_peer_open", "moge_peer_close", "moge_peer_copy", "moge_peer_flag_set",
     "moge_peer_flag_wait", "moge_op_linear", "moge_op_linear_ln", "moge_op_attention", "moge_op_layernorm", "moge_op_conv",
+    "moge_align_workspace_bytes", "moge_align", "moge_align_anchored", "moge_align_affine_lstsq",
 ]
 
 
@@ -101,6 +104,11 @@ def lib() -> C.CDLL:
     L.moge_op_attention.argtypes = [vp, vp, ci, ci, ci, ci, ci, vp]
     L.moge_op_layernorm.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp]
     L.moge_op_conv.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, vp]
+    i64, sz = C.c_int64, C.c_size_t
+    L.moge_align_workspace_bytes.argtypes = [ci, ci, i64, ci, C.POINTER(sz)]
+    L.moge_align.argtypes = [vp, vp, vp, vp, ci, i64, ci, vp, vp, vp, vp, sz, vp]
+    L.moge_align_anchored.argtypes = [vp, vp, vp, ci, C.c_float, i64, ci, vp, vp, vp, vp, sz, vp]
+    L.moge_align_affine_lstsq.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("moge_last_error", "moge_version", "moge_engine_destroy"):
             getattr(L, name).restype = ci

@@ -208,3 +208,47 @@ def synthetic_point_map(batch: int, height: int, width: int, focal: float, shift
             raise ValueError(mask_mode)
         pts.append(p); masks.append(m)
     return torch.stack(pts), torch.stack(masks)
+
+
+def synthetic_alignment_case(batch_shape, n: int, seed: int = 0, single_positive: bool = False):
+    """Seeded inputs of the alignment solvers (moge_b200.alignment): points_src, points_tgt (*batch_shape, n, 3) and weight
+    (*batch_shape, n), fp32.  tgt ~ scale * src + shift per image with a known scale and shift, plus small noise, ~10 % gross
+    outliers, ~30 % zero weights, x and y components of both signs, and ~5 % of the points duplicated (src, tgt and weight) from
+    other points.  single_positive: the first image keeps one positive weight only."""
+    g = torch.Generator(device="cpu").manual_seed(3000 + seed)
+    bs = tuple(batch_shape)
+    tgt = torch.randn(*bs, n, 3, generator=g) + torch.tensor([0.0, 0.0, 3.0])
+    scale = 0.5 + torch.rand(*bs, 1, 1, generator=g)
+    shift = 0.3 * torch.randn(*bs, 1, 3, generator=g)
+    src = (tgt - shift) / scale + 0.01 * torch.randn(*bs, n, 3, generator=g)
+    outlier = torch.rand(*bs, n, 1, generator=g) < 0.1
+    src = torch.where(outlier, src + 2.0 * torch.randn(*bs, n, 3, generator=g), src)
+    weight = 0.1 + torch.rand(*bs, n, generator=g)
+    weight = torch.where(torch.rand(*bs, n, generator=g) < 0.3, torch.zeros_like(weight), weight)
+    dup = torch.randperm(n, generator=g)[: max(1, n // 20)]
+    orig = torch.randint(0, n, (dup.numel(),), generator=g)
+    src[..., dup, :], tgt[..., dup, :], weight[..., dup] = src[..., orig, :], tgt[..., orig, :], weight[..., orig]
+    if single_positive:
+        first = weight.reshape(-1, n)[0]
+        first.zero_()
+        first[n // 2] = 0.7
+    return src.contiguous(), tgt.contiguous(), weight.contiguous()
+
+
+ALIGNMENT_FUNCTIONS = ("align", "align_depth_scale", "align_depth_affine", "align_points_scale", "align_points_scale_z_shift",
+                       "align_points_scale_xyz_shift", "align_points_z_shift", "align_points_xyz_shift", "align_affine_lstsq")
+
+
+def alignment_arguments(fn: str, batch_shape, n: int, seed: int, trunc=None, single_positive: bool = False):
+    """Positional arguments of alignment function `fn` on synthetic_alignment_case(batch_shape, n, seed): depth functions, align
+    and align_affine_lstsq take the z components.  trunc: None, a float, or "per_element" (align only: a seeded (..., n) tensor);
+    align_affine_lstsq takes trunc = "weighted" for its weights (else w = None)."""
+    src, tgt, w = synthetic_alignment_case(batch_shape, n, seed, single_positive)
+    if fn == "align_affine_lstsq":
+        return (src[..., 2], tgt[..., 2], w if trunc == "weighted" else None)
+    if trunc == "per_element":
+        g = torch.Generator(device="cpu").manual_seed(4000 + seed)
+        trunc = 0.05 + 0.1 * torch.rand(*tuple(batch_shape), n, generator=g)
+    if fn in ("align", "align_depth_scale", "align_depth_affine"):
+        return (src[..., 2], tgt[..., 2], w, trunc)
+    return (src, tgt, w, trunc)
