@@ -1,4 +1,4 @@
-/* moge_b200 -- C ABI of the H100-native MoGe-2 inference engine (libmoge_b200.so, sm_90a).
+/* moge_b200 -- C ABI of the H100-native MoGe-2 (and MoGe-1) inference engine (libmoge_b200.so, sm_90a).
  *
  * The reference (microsoft/MoGe) has no FFI / plugin boundary on this path: the hot path is the Python nn.Module
  * `moge.model.v2.MoGeModel` (/root/reference/moge/model/v2.py).  This header is the boundary the replacement exports;
@@ -168,6 +168,56 @@ int moge_op_layernorm(const float* x, const float* gamma, const float* beta, voi
  * the output map is (B,2H+2,2W+2,Cout).                                                                         */
 int moge_op_conv(const void* x, const float* w, const float* bias, const void* skip, void* out_raw, void* out_relu,
                  int B, int H, int W, int Cin, int Cout, int taps, int shuffle, int dtype, void* stream);
+
+/* ---- MoGe-1 (moge/model/v1.py; Python: moge_b200.model.v1, alias moge.model.v1).  The same DINOv2 encoder as above; the decoder
+ * is v1's Head (v1.py:61-142): summed 1x1 projections of the taps, then per level a ConvTranspose2d(k2 s2) over cat(x, uv), a
+ * replicate-padded 3x3 conv and GroupNorm residual blocks, then a bilinear resize to the resized-image grid and two output blocks
+ * (points, mask).  moge_engine_create_v1 returns an engine that destroy / set_weight / finalize / num_ops / op_info / profile take
+ * unchanged; its weight keys are the reference's v1 state-dict keys.  Configs the engine does not cover fail at create. */
+enum { MOGE_V1_GROUP_NORM = 0, MOGE_V1_LAYER_NORM = 1 };
+typedef struct moge_v1_config {
+    int embed_dim, depth, num_heads;      /* DINOv2 ViT-S/B/L */
+    int num_taps;
+    int taps[MOGE_MAX_TAPS];              /* intermediate_layers as block indices (an int n means the last n blocks) */
+    int dim_proj;                         /* multiple of 128 */
+    int num_levels;                       /* len(dim_upsample) */
+    int dim_upsample[MOGE_MAX_LEVELS];    /* multiples of 64 */
+    int hidden_mult;                      /* dim_times_res_block_hidden */
+    int num_res_blocks;
+    int hidden_norm;                      /* MOGE_V1_GROUP_NORM: hidden/32 groups, MOGE_V1_LAYER_NORM: 1 group */
+    int last_res_blocks;                  /* must be 0 */
+    int last_conv_channels;               /* must be 32 */
+    int last_conv_size;                   /* must be 1 */
+    int remap_output;                     /* MOGE_REMAP_* */
+    int compute_dtype;                    /* MOGE_F16 or MOGE_BF16 */
+} moge_v1_config_t;
+int moge_engine_create_v1(const moge_v1_config_t* cfg, int device, moge_engine_t** out);
+/* workspace for B images of HxW pixels resized to (rh, rw) (v1.py:273-274: rh = int(H f), rw = int(W f)); token grid rh/14 x rw/14 */
+int moge_v1_workspace_bytes(moge_engine_t* e, int B, int H, int W, int rh, int rw, size_t* bytes);
+/* replaces MoGeModel.forward (v1.py:269-299): image (B,3,H,W) in [0,1]; points (B,H,W,3) remapped, mask (B,H,W) the raw mask
+ * output (no sigmoid), both fp32 */
+int moge_v1_forward(moge_engine_t* e, const void* image, int image_dtype, int B, int H, int W, int rh, int rw, void* workspace,
+                    size_t workspace_bytes, float* points, float* mask, void* stream);
+/* the fp32 part of MoGeModel.infer (v1.py:352-380): mask_out = mask > mask_threshold (u8), focal/shift recovery (focal_in NULL:
+ * solve both), intrinsics (B,3,3), depth = z + shift, points re-projected (force_projection) or shifted in z, points and depth
+ * +inf outside the mask (apply_mask).  points updated in place; focal, shift (B,) outputs. */
+int moge_v1_postprocess(float* points, const float* mask, float mask_threshold, const float* focal_in, int B, int H, int W,
+                        int force_projection, int apply_mask, float* depth, uint8_t* mask_out, float* intrinsics, float* focal,
+                        float* shift, void* stream);
+/* operator entry points of the v1 kernels.  resize: F.interpolate(bicubic, align_corners=False, antialias=True) of (B,C,H,W)
+ * (dtype MOGE_F32/F16/BF16) to fp32 (B,C,Ho,Wo).  group norm: relu(GroupNorm(G, C, eps 1e-5)(x) * gamma + beta) of the interior
+ * of a padded NHWC 16-bit map (B,Hp,Wp,C) (Hp = max(H+2, 8), Wp = max(W+2, 16)) into another such map, border replicated. */
+int moge_op_resize_bicubic_aa(const void* x, int dtype, int B, int C, int H, int W, int Ho, int Wo, float* out, void* stream);
+int moge_op_groupnorm_relu(const void* x, void* out, const float* gamma, const float* beta, int B, int H, int W, int C, int G,
+                           int dtype, void* stream);
+/* the MoGe-1 upsampling ConvTranspose2d(Cin + 2 -> Cout, k2 s2) over cat(x, uv): x a padded NHWC 16-bit map (B,Hp,Wp,Cin) on an
+ * H x W grid, w the PyTorch weight (Cin + 2, Cout, 2, 2) fp32, bias (Cout) fp32; the UV planes (half extents su, sv) are taken on
+ * the INPUT grid.  out: padded NHWC (B, max(2H+2, 8), max(2W+2, 16), Cout), border replicated.  Cin % 64 == 0, Cout % 32 == 0. */
+int moge_op_conv_transpose_uv(const void* x, const float* w, const float* bias, void* out, int B, int H, int W, int Cin, int Cout, float su,
+                     float sv, int dtype, void* stream);
+/* host only: taps [*lo, *lo + n) and normalised weights (w may be NULL) of output index i of the antialiased bicubic filter
+ * for a resize of `in` to `out` samples; returns n (< 0 on error) */
+int moge_bicubic_aa_weights(int in, int out, int i, int* lo, float* w, int cap);
 
 /* ---- truncated-L1 alignment solvers (moge/utils/alignment.py; Python: moge_b200.alignment, alias moge.utils.alignment).
  * A problem is n elements (x, y, w), w >= 0; it is solved as align() (alignment.py:52-146) solves it: after x, y *= sign(x), either

@@ -27,6 +27,8 @@ EXPORTS = [
     "moge_postprocess", "moge_peer_alloc", "moge_peer_free", "moge_peer_open", "moge_peer_close", "moge_peer_copy", "moge_peer_flag_set",
     "moge_peer_flag_wait", "moge_op_linear", "moge_op_linear_ln", "moge_op_attention", "moge_op_layernorm", "moge_op_conv",
     "moge_align_workspace_bytes", "moge_align", "moge_align_anchored", "moge_align_affine_lstsq",
+    "moge_engine_create_v1", "moge_v1_workspace_bytes", "moge_v1_forward", "moge_v1_postprocess", "moge_op_resize_bicubic_aa",
+    "moge_op_groupnorm_relu", "moge_bicubic_aa_weights", "moge_op_conv_transpose_uv",
 ]
 
 
@@ -46,6 +48,17 @@ class Config(C.Structure):
         ("neck", StackConfig), ("points_head", StackConfig), ("normal_head", StackConfig), ("mask_head", StackConfig),
         ("scale_head_layers", C.c_int), ("scale_head_dims", C.c_int * MOGE_MAX_MLP),
         ("remap_output", C.c_int), ("compute_dtype", C.c_int),
+    ]
+
+
+class V1Config(C.Structure):
+    """moge_v1_config_t: MoGe-1 (moge/model/v1.py)."""
+    _fields_ = [
+        ("embed_dim", C.c_int), ("depth", C.c_int), ("num_heads", C.c_int),
+        ("num_taps", C.c_int), ("taps", C.c_int * MOGE_MAX_TAPS), ("dim_proj", C.c_int),
+        ("num_levels", C.c_int), ("dim_upsample", C.c_int * MOGE_MAX_LEVELS), ("hidden_mult", C.c_int),
+        ("num_res_blocks", C.c_int), ("hidden_norm", C.c_int), ("last_res_blocks", C.c_int),
+        ("last_conv_channels", C.c_int), ("last_conv_size", C.c_int), ("remap_output", C.c_int), ("compute_dtype", C.c_int),
     ]
 
 
@@ -109,6 +122,14 @@ def lib() -> C.CDLL:
     L.moge_align.argtypes = [vp, vp, vp, vp, ci, i64, ci, vp, vp, vp, vp, sz, vp]
     L.moge_align_anchored.argtypes = [vp, vp, vp, ci, C.c_float, i64, ci, vp, vp, vp, vp, sz, vp]
     L.moge_align_affine_lstsq.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp]
+    L.moge_engine_create_v1.argtypes = [C.POINTER(V1Config), ci, C.POINTER(vp)]
+    L.moge_v1_workspace_bytes.argtypes = [vp, ci, ci, ci, ci, ci, C.POINTER(C.c_size_t)]
+    L.moge_v1_forward.argtypes = [vp, vp, ci, ci, ci, ci, ci, ci, vp, C.c_size_t, vp, vp, vp]
+    L.moge_v1_postprocess.argtypes = [vp, vp, C.c_float, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp]
+    L.moge_op_resize_bicubic_aa.argtypes = [vp, ci, ci, ci, ci, ci, ci, ci, vp, vp]
+    L.moge_op_groupnorm_relu.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]
+    L.moge_op_conv_transpose_uv.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, C.c_float, C.c_float, ci, vp]
+    L.moge_bicubic_aa_weights.argtypes = [ci, ci, ci, C.POINTER(ci), C.POINTER(C.c_float), ci]
     for name in EXPORTS:
         if name not in ("moge_last_error", "moge_version", "moge_engine_destroy"):
             getattr(L, name).restype = ci
@@ -209,6 +230,47 @@ def make_config(model_config: dict, compute_dtype: int) -> Config:
     remap = model_config.get("remap_output", "linear")
     if remap not in REMAP:
         raise ValueError(f"Invalid remap output type: {remap}")       # same error as v2.py:135
+    c.remap_output = REMAP[remap]
+    c.compute_dtype = compute_dtype
+    return c
+
+
+V1_NORMS = {"group_norm": 0, "layer_norm": 1}
+
+
+def make_v1_config(model_config: dict, compute_dtype: int) -> V1Config:
+    """MoGe-1 kwargs (v1.py:149-163, defaults as there) -> C struct.  The engine validates what it covers (moge_engine_create_v1)."""
+    from .configs import backbone_dims
+    c = V1Config()
+    D, depth, heads = backbone_dims(model_config.get("encoder", "dinov2_vitb14"))
+    c.embed_dim, c.depth, c.num_heads = D, depth, heads
+    taps = model_config.get("intermediate_layers", 4)
+    if isinstance(taps, int):                     # get_intermediate_layers(n=int): the last n blocks
+        taps = list(range(depth - taps, depth))
+    if not 0 < len(taps) <= MOGE_MAX_TAPS:
+        raise MogeError(f"{len(taps)} intermediate layers out of range")
+    c.num_taps = len(taps)
+    for i, t in enumerate(taps):
+        c.taps[i] = int(t)
+    c.dim_proj = int(model_config.get("dim_proj", 512))
+    ups = list(model_config.get("dim_upsample", [256, 128, 128]))
+    if not 0 < len(ups) <= MOGE_MAX_LEVELS:
+        raise MogeError(f"{len(ups)} upsampling levels out of range")
+    c.num_levels = len(ups)
+    for i, d in enumerate(ups):
+        c.dim_upsample[i] = int(d)
+    c.hidden_mult = int(model_config.get("dim_times_res_block_hidden", 1))
+    c.num_res_blocks = int(model_config.get("num_res_blocks", 1))
+    norm = model_config.get("res_block_norm", "group_norm")
+    if norm not in V1_NORMS:
+        raise ValueError(f"Unsupported res_block_norm: {norm}")
+    c.hidden_norm = V1_NORMS[norm]
+    c.last_res_blocks = int(model_config.get("last_res_blocks", 0))
+    c.last_conv_channels = int(model_config.get("last_conv_channels", 32))
+    c.last_conv_size = int(model_config.get("last_conv_size", 1))
+    remap = model_config.get("remap_output", "linear")
+    if remap not in REMAP:
+        raise ValueError(f"Invalid remap output type: {remap}")       # same error as v1.py:266
     c.remap_output = REMAP[remap]
     c.compute_dtype = compute_dtype
     return c

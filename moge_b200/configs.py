@@ -79,6 +79,32 @@ def model_config(size: str = "vitl", with_normal: bool = True) -> Dict:
     return copy.deepcopy(cfg)
 
 
+def v1_model_config(size: str = "vitl") -> Dict:
+    """MoGe-1 kwargs (moge.model.v1.MoGeModel(**cfg)).  ViT-L is /root/reference/configs/train/v1.json as is; ViT-S / ViT-B are
+    smaller test configurations (ViT-B also takes the list form of intermediate_layers and one res block with hidden == width)."""
+    size = size.lower()
+    if size == "vitl":
+        cfg = {"encoder": "dinov2_vitl14", "remap_output": "exp", "intermediate_layers": 4, "dim_upsample": [256, 128, 64],
+               "dim_times_res_block_hidden": 2, "num_res_blocks": 2, "num_tokens_range": [1200, 2500], "last_conv_channels": 32,
+               "last_conv_size": 1}
+    elif size == "vitb":
+        cfg = {"encoder": "dinov2_vitb14", "remap_output": "exp", "intermediate_layers": [2, 5, 8, 11], "dim_proj": 256,
+               "dim_upsample": [128, 128, 64], "dim_times_res_block_hidden": 1, "num_res_blocks": 1, "num_tokens_range": [1200, 2500]}
+    elif size == "vits":
+        cfg = {"encoder": "dinov2_vits14", "remap_output": "exp", "intermediate_layers": 4, "dim_proj": 256,
+               "dim_upsample": [128, 64, 64], "dim_times_res_block_hidden": 2, "num_res_blocks": 1, "num_tokens_range": [1200, 2500]}
+    else:
+        raise ValueError(size)
+    return copy.deepcopy(cfg)
+
+
+def v1_resized_size(height: int, width: int, num_tokens: int) -> Tuple[int, int]:
+    """(resized_height, resized_width) exactly as /root/reference/moge/model/v1.py:273-274 (int() truncation); the token grid
+    is (rh // 14, rw // 14)."""
+    resize_factor = ((num_tokens * 14 ** 2) / (height * width)) ** 0.5
+    return int(height * resize_factor), int(width * resize_factor)
+
+
 def token_grid(height: int, width: int, num_tokens: int) -> Tuple[int, int]:
     """(base_h, base_w) exactly as /root/reference/moge/model/v2.py:142-147 (Python round = half-to-even)."""
     aspect = width / height

@@ -377,7 +377,7 @@ int launch_scale_head(const float* cls, const float* const* w, const float* cons
 // points remap (v2.py:122-136), F.normalize(eps=1e-12) of the normals, sigmoid of the mask logit.
 __global__ void head_output_kernel(const float4* __restrict__ pts, const float4* __restrict__ nrm, const float* __restrict__ msk,
                                    int B, int Hl, int Wl, int H, int W, int remap, float* __restrict__ points,
-                                   float* __restrict__ normal, float* __restrict__ mask) {
+                                   float* __restrict__ normal, float* __restrict__ mask, int mask_sigmoid) {
     pdl_prologue();
     const size_t total = static_cast<size_t>(B) * H * W;
     const float rh = static_cast<float>(Hl) / H, rw = static_cast<float>(Wl) / W;
@@ -414,16 +414,17 @@ __global__ void head_output_kernel(const float4* __restrict__ pts, const float4*
         }
         if (msk != nullptr) {
             const float m = w00 * msk[i00] + w01 * msk[i01] + w10 * msk[i10] + w11 * msk[i11];
-            mask[idx] = 1.0f / (1.0f + expf(-m));
+            mask[idx] = mask_sigmoid ? 1.0f / (1.0f + expf(-m)) : m;
         }
     }
 }
 int launch_head_output(const float4* pts_lr, const float4* nrm_lr, const float* msk_lr, int B, int Hl, int Wl, int H, int W,
-                       int remap_mode, float* points, float* normal, float* mask, cudaStream_t st) {
+                       int remap_mode, float* points, float* normal, float* mask, cudaStream_t st, bool mask_sigmoid) {
     const size_t total = static_cast<size_t>(B) * H * W;
     const int threads = 256;
     const int blocks = static_cast<int>(std::min<size_t>((total + threads - 1) / threads, 132 * 16));
-    CUDA_TRY(launch_pdl(head_output_kernel, dim3(blocks), dim3(threads), 0, st, pts_lr, nrm_lr, msk_lr, B, Hl, Wl, H, W, remap_mode, points, normal, mask));
+    CUDA_TRY(launch_pdl(head_output_kernel, dim3(blocks), dim3(threads), 0, st, pts_lr, nrm_lr, msk_lr, B, Hl, Wl, H, W, remap_mode, points, normal, mask,
+                        mask_sigmoid ? 1 : 0));
     CUDA_TRY(cudaGetLastError());
     return 0;
 }

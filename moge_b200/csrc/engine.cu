@@ -71,6 +71,7 @@ struct OpList : std::vector<Op> {
 // depends on the pixel geometry (preprocess, patch/pos embed, taps, decoder, output resize) runs per group.
 struct Group {
     int B = 0, H = 0, W = 0, h = 0, w = 0;
+    int rh = 0, rw = 0;           // MoGe-1: the resized image the encoder and decoder see (0 for MoGe-2)
     int img0 = 0;                 // index of the group's first image among all images of the call
     long row0 = 0;                // first row of the group in the packed token matrices
     float* pos_table = nullptr;   // plan-owned, [h*w, D] (bicubic-resampled pos embed + patch bias)
@@ -92,10 +93,11 @@ struct Plan {
     // few microseconds each and replaying a graph removes the per-launch CPU cost.  Phase 0 / 2 launches run eagerly around it.
     cudaGraphExec_t exec = nullptr;
     int eager_runs = 0;
-    bool same_shape(const moge_group_t* g, int n) const {
+    bool same_shape(const moge_group_t* g, int n, int rh, int rw) const {
         if (static_cast<int>(groups.size()) != n) return false;
         for (int i = 0; i < n; ++i)
-            if (groups[i].B != g[i].B || groups[i].H != g[i].H || groups[i].W != g[i].W || groups[i].h != g[i].h || groups[i].w != g[i].w) return false;
+            if (groups[i].B != g[i].B || groups[i].H != g[i].H || groups[i].W != g[i].W || groups[i].h != g[i].h || groups[i].w != g[i].w ||
+                groups[i].rh != rh || groups[i].rw != rw) return false;
         return true;
     }
     ~Plan() {
@@ -104,12 +106,33 @@ struct Plan {
     }
 };
 
+// MoGe-1 decoder weights (v1.py:61-142)
+struct V1Res {            // ResidualConvBlock: GN(1, C) -> ReLU -> conv C->Hd -> GN(G2, Hd) -> ReLU -> conv Hd->C, identity skip
+    ConvW c1, c2;
+    const float *g1 = nullptr, *b1 = nullptr, *g2 = nullptr, *b2 = nullptr;
+    int G2 = 1;
+};
+struct V1Level {
+    ConvW convT, conv;      // ConvTranspose2d k2s2 over the feature channels (pixel shuffle), 3x3 replicate conv
+    float* wuv = nullptr;   // [2][4 phases][C]: the convT's UV rows, applied on the input grid
+    std::vector<V1Res> res;
+};
+struct V1W {
+    ConvW proj;             // the summed 1x1 projections of the taps as one GEMM over the concatenated taps
+    std::vector<V1Level> lv;
+    ConvW out;              // both output blocks' 3x3 convs over the feature channels: N = 32 points + 32 mask
+    float* wout = nullptr;  // launch_v1_output parameters: folded UV weights, block-diagonal 64 -> 4 map, biases
+};
+
 }  // namespace mg
 
 using namespace mg;
 
 struct moge_engine {
     moge_config_t cfg;
+    bool v1 = false;                  // created by moge_engine_create_v1: cfg holds the encoder only, v1cfg the rest
+    moge_v1_config_t v1cfg{};
+    V1W v1w;
     int device = 0, num_sms = 132;
     bool bf16 = false, finalized = false;
     std::map<std::string, RawWeight> raw;
@@ -378,10 +401,10 @@ static int pack_stack(moge_engine* e, const std::string& name, const moge_stack_
     return 0;
 }
 
-static int finalize(moge_engine* e, cudaStream_t st) {
+static int finalize_encoder(moge_engine* e, cudaStream_t st) {
     const moge_config_t& c = e->cfg;
     const int D = c.embed_dim;
-    const std::string bb = "encoder.backbone.";
+    const std::string bb = e->v1 ? "backbone." : "encoder.backbone.";
     MG_TRY(pack_linear(e, bb + "patch_embed.proj.weight", D, 588, 592, &e->w_patch, st));
     MG_TRY(vec(e, bb + "patch_embed.proj.bias", D, &e->patch_bias));
     MG_TRY(vec(e, bb + "pos_embed", (1 + 37 * 37) * D, &e->pos_embed));
@@ -421,6 +444,12 @@ static int finalize(moge_engine* e, cudaStream_t st) {
             MG_TRY(launch_ln_fold(wf->p, b.ln2g, b.ln2b, b.bfc1, 4 * D, D, D, b.wfc1_ln, b.b_fc1_ln, e->bf16, st));
         }
     }
+    return 0;
+}
+
+static int finalize_v2_decoder(moge_engine* e, cudaStream_t st) {
+    const moge_config_t& c = e->cfg;
+    const int D = c.embed_dim;
     // ---- fold: neck.input_blocks.0 o (sum_j output_projections.j)  ->  one GEMM over the concatenated taps
     {
         const int C0 = c.neck.dim_res_blocks[0], Do = c.dim_out, nt = c.num_taps;
@@ -486,6 +515,124 @@ static int finalize(moge_engine* e, cudaStream_t st) {
         e->mlp_w.push_back(w);
         e->mlp_b.push_back(b);
     }
+    return 0;
+}
+
+// ---- MoGe-1 decoder (keys head.*, v1.py:61-142).  The small folds are done on the host from copies of the fp32 staging weights.
+static int to_host(const RawWeight* w, size_t off, size_t n, std::vector<float>* out) {
+    out->resize(n);
+    CUDA_TRY(cudaMemcpy(out->data(), w->p + off, n * 4, cudaMemcpyDeviceToHost));
+    return 0;
+}
+static int to_dev(moge_engine* e, const std::vector<float>& v, float** out) {
+    MG_TRY(e->alloc(reinterpret_cast<void**>(out), v.size() * 4));
+    CUDA_TRY(cudaMemcpy(*out, v.data(), v.size() * 4, cudaMemcpyHostToDevice));
+    return 0;
+}
+
+static int finalize_v1(moge_engine* e, cudaStream_t st) {
+    const moge_v1_config_t& c = e->v1cfg;
+    const int D = c.embed_dim, nt = c.num_taps, P = c.dim_proj;
+    CUDA_TRY(cudaStreamSynchronize(st));       // the staging copies are written on st; the host reads some of them below
+    V1W& v = e->v1w;
+    // V4: sum_j projects.j(tap_j) = one GEMM over the concatenated taps [B*T, nt*D] with the summed bias
+    ConvW& pj = v.proj;
+    pj.N = P; pj.cin = nt * D; pj.taps = 1; pj.Ktot = nt * D;
+    MG_TRY(e->alloc(&pj.w, static_cast<size_t>(P) * pj.Ktot * 2));
+    MG_TRY(e->alloc(reinterpret_cast<void**>(&pj.bias), P * 4));
+    CUDA_TRY(cudaMemsetAsync(pj.bias, 0, P * 4, st));
+    float* wcat32;                             // [P, nt*D] fp32: tap j's weight in columns j*D ..
+    MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wcat32), static_cast<size_t>(P) * pj.Ktot * 4));
+    for (int j = 0; j < nt; ++j) {
+        const std::string k = "head.projects." + std::to_string(j);
+        const RawWeight* w;
+        const float* b;
+        MG_TRY(get_raw(e, k + ".weight", &w, {P, D, 1, 1}));
+        MG_TRY(vec(e, k + ".bias", P, &b));
+        CUDA_TRY(cudaMemcpy2DAsync(wcat32 + static_cast<size_t>(j) * D, static_cast<size_t>(pj.Ktot) * 4, w->p, static_cast<size_t>(D) * 4,
+                                   static_cast<size_t>(D) * 4, P, cudaMemcpyDeviceToDevice, st));
+        vec_combine_kernel<<<(P + 255) / 256, 256, 0, st>>>(pj.bias, pj.bias, 1, b, P);
+        CUDA_TRY(cudaGetLastError());
+    }
+    MG_TRY(launch_cast_2d(wcat32, MOGE_F32, pj.w, e->bf16, P, pj.Ktot, pj.Ktot, pj.Ktot, st));
+    int cin = P;
+    v.lv.assign(c.num_levels, V1Level());
+    for (int l = 0; l < c.num_levels; ++l) {
+        const int Co = c.dim_upsample[l], Hd = c.hidden_mult * Co;
+        const std::string pre = "head.upsample_blocks." + std::to_string(l) + ".";
+        V1Level& L = v.lv[l];
+        // V5: ConvTranspose2d(cin + 2 -> Co): rows 0..cin-1 through the GEMM, the two UV rows as the input-grid term
+        const RawWeight* wt;
+        const float* bt;
+        MG_TRY(get_raw(e, pre + "0.0.weight", &wt, {cin + 2, Co, 2, 2}));
+        MG_TRY(vec(e, pre + "0.0.bias", Co, &bt));
+        L.convT.N = 4 * Co; L.convT.cin = cin; L.convT.taps = 1; L.convT.Ktot = cin;
+        MG_TRY(e->alloc(&L.convT.w, static_cast<size_t>(4) * Co * cin * 2));
+        MG_TRY(launch_pack_convT(wt->p, L.convT.w, e->bf16, cin, Co, st));
+        MG_TRY(sum_bias(e, bt, nullptr, Co, &L.convT.bias, st));
+        MG_TRY(e->alloc(reinterpret_cast<void**>(&L.wuv), static_cast<size_t>(8) * Co * 4));
+        MG_TRY(launch_pack_convT_uv(wt->p, cin, Co, L.wuv, st));
+        MG_TRY(pack_conv3(e, pre + "0.1", Co, Co, "", 0, false, &L.conv, st));
+        for (int r = 0; r < c.num_res_blocks; ++r) {
+            const std::string rp = pre + std::to_string(1 + r) + ".layers.";
+            V1Res R;
+            MG_TRY(vec(e, rp + "0.weight", Co, &R.g1));
+            MG_TRY(vec(e, rp + "0.bias", Co, &R.b1));
+            MG_TRY(pack_conv3(e, rp + "2", Hd, Co, "", 0, false, &R.c1, st));
+            MG_TRY(vec(e, rp + "3.weight", Hd, &R.g2));
+            MG_TRY(vec(e, rp + "3.bias", Hd, &R.b2));
+            MG_TRY(pack_conv3(e, rp + "5", Co, Hd, "", 0, false, &R.c2, st));
+            R.G2 = c.hidden_norm == MOGE_V1_GROUP_NORM ? Hd / 32 : 1;
+            L.res.push_back(R);
+        }
+        cin = Co;
+    }
+    // V7: output blocks k = 0 (points, 3) and 1 (mask, 1): conv3x3 (cin + 2 -> 32), ReLU, conv1x1 (32 -> n_k)
+    const int lc = c.last_conv_channels, nout[2] = {3, 1};
+    std::vector<float> wcat(static_cast<size_t>(2) * lc * cin * 9), bcat(2 * lc), params(64 * 6 + 4 * 64 + 4, 0.f);
+    for (int k = 0; k < 2; ++k) {
+        const std::string ob = "head.output_block." + std::to_string(k) + ".";
+        const RawWeight *wc, *bc, *wo, *bo;
+        MG_TRY(get_raw(e, ob + "0.weight", &wc, {lc, cin + 2, 3, 3}));
+        MG_TRY(get_raw(e, ob + "0.bias", &bc, {lc}));
+        MG_TRY(get_raw(e, ob + "2.weight", &wo, {nout[k], lc, 1, 1}));
+        MG_TRY(get_raw(e, ob + "2.bias", &bo, {nout[k]}));
+        std::vector<float> hw, hb, hwo, hbo;
+        MG_TRY(to_host(wc, 0, wc->numel, &hw));
+        MG_TRY(to_host(bc, 0, bc->numel, &hb));
+        MG_TRY(to_host(wo, 0, wo->numel, &hwo));
+        MG_TRY(to_host(bo, 0, bo->numel, &hbo));
+        for (int co = 0; co < lc; ++co) {
+            const int n = k * lc + co;
+            const float* src = hw.data() + static_cast<size_t>(co) * (cin + 2) * 9;
+            std::copy(src, src + static_cast<size_t>(cin) * 9, wcat.begin() + static_cast<size_t>(n) * cin * 9);
+            bcat[n] = hb[co];
+            // UV part of the replicate-padded 3x3 conv: u depends on x only, v on y only -> six folded weights
+            const float* wu = src + static_cast<size_t>(cin) * 9;
+            const float* wv = wu + 9;
+            for (int d = 0; d < 3; ++d) {
+                params[n * 6 + d] = wu[0 * 3 + d] + wu[1 * 3 + d] + wu[2 * 3 + d];          // sum over dy, tap dx = d - 1
+                params[n * 6 + 3 + d] = wv[d * 3 + 0] + wv[d * 3 + 1] + wv[d * 3 + 2];      // sum over dx, tap dy = d - 1
+            }
+            for (int o = 0; o < nout[k]; ++o) params[64 * 6 + (k == 0 ? o : 3) * 64 + n] = hwo[static_cast<size_t>(o) * lc + co];
+        }
+        for (int o = 0; o < nout[k]; ++o) params[64 * 6 + 4 * 64 + (k == 0 ? o : 3)] = hbo[o];
+    }
+    MG_TRY(to_dev(e, params, &v.wout));
+    float* wcat_dev;
+    MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wcat_dev), wcat.size() * 4));
+    CUDA_TRY(cudaMemcpy(wcat_dev, wcat.data(), wcat.size() * 4, cudaMemcpyHostToDevice));
+    ConvW& oc = v.out;
+    oc.N = 2 * lc; oc.cin = cin; oc.taps = 9; oc.Ktot = 9 * cin;
+    MG_TRY(e->alloc(&oc.w, static_cast<size_t>(oc.N) * oc.Ktot * 2));
+    MG_TRY(launch_pack_conv(wcat_dev, oc.w, e->bf16, oc.N, cin, 9, oc.Ktot, 0, st));
+    MG_TRY(to_dev(e, bcat, &oc.bias));
+    return 0;
+}
+
+static int finalize(moge_engine* e, cudaStream_t st) {
+    MG_TRY(finalize_encoder(e, st));
+    MG_TRY(e->v1 ? finalize_v1(e, st) : finalize_v2_decoder(e, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     for (void* t : e->temps) cudaFree(t);
     e->temps.clear();
@@ -616,6 +763,170 @@ static int plan_stack(moge_engine* e, Plan* pl, const char* sname, const moge_st
     return 0;
 }
 
+// ---- MoGe-1 decoder (one shape group): workspace maps and launch list
+struct V1Bufs {
+    float *rs_tmp = nullptr, *rs_img = nullptr;     // bicubic row pass (B,3,H,rw), resized image (B,3,rh,rw)
+    void* x0 = nullptr;                             // projected taps, level 0
+    struct Lv { void *m0, *m1, *relu, *hraw, *hrelu; };
+    std::vector<Lv> lv;                             // per upsampling level (its output grid): ping-pong maps, ReLU maps
+    double2* gn_part = nullptr;
+    float2* gn_stats = nullptr;
+    void *full = nullptr, *fout = nullptr;          // last map resized to (rh, rw); the output conv's 64 channels there
+    float4* pts = nullptr;                          // (rh, rw) points before the resize to (H, W)
+    float* msk = nullptr;
+};
+
+static Level full_geom(int rh, int rw) { return Level{rh, rw, std::max(rh + 2, TILE_PH), std::max(rw + 2, TILE_PW)}; }
+
+static void v1_alloc(moge_engine* e, const Group& g, WsAlloc& ws, V1Bufs* vb) {
+    const moge_v1_config_t& c = e->v1cfg;
+    const int B = g.B;
+    vb->rs_tmp = static_cast<float*>(ws.take(static_cast<size_t>(B) * 3 * g.H * g.rw * 4));
+    vb->rs_img = static_cast<float*>(ws.take(static_cast<size_t>(B) * 3 * g.rh * g.rw * 4));
+    vb->x0 = ws.take(map_bytes(level_geom(g.h, g.w, 0), B, c.dim_proj));
+    size_t part = 0, stats = 0;
+    vb->lv.resize(c.num_levels);
+    for (int l = 0; l < c.num_levels; ++l) {
+        const Level go = level_geom(g.h, g.w, l + 1);
+        const int Co = c.dim_upsample[l], Hd = c.hidden_mult * Co;
+        const int G2 = c.hidden_norm == MOGE_V1_GROUP_NORM ? Hd / 32 : 1;
+        V1Bufs::Lv& L = vb->lv[l];
+        L.m0 = ws.take(map_bytes(go, B, Co));
+        L.m1 = ws.take(map_bytes(go, B, Co));
+        L.relu = ws.take(map_bytes(go, B, Co));
+        L.hraw = ws.take(map_bytes(go, B, Hd));
+        L.hrelu = ws.take(map_bytes(go, B, Hd));
+        part = std::max({part, static_cast<size_t>(B) * gn_tiles(go.H, go.W, Co), static_cast<size_t>(B) * gn_tiles(go.H, go.W, Hd) * G2});
+        stats = std::max(stats, static_cast<size_t>(B) * G2);
+    }
+    vb->gn_part = static_cast<double2*>(ws.take(part * 16));
+    vb->gn_stats = static_cast<float2*>(ws.take(stats * 8));
+    const Level gr = full_geom(g.rh, g.rw);
+    vb->full = ws.take(map_bytes(gr, B, c.dim_upsample[c.num_levels - 1]));
+    vb->fout = ws.take(map_bytes(gr, B, 2 * c.last_conv_channels));
+    vb->pts = static_cast<float4*>(ws.take(static_cast<size_t>(B) * g.rh * g.rw * 16));
+    vb->msk = static_cast<float*>(ws.take(static_cast<size_t>(B) * g.rh * g.rw * 4));
+}
+
+static int plan_v1_decoder(moge_engine* e, Plan* pl, const void* taps, const V1Bufs& vb) {
+    const moge_v1_config_t& c = e->v1cfg;
+    const V1W& v = e->v1w;
+    const Group& g = pl->groups[0];
+    const int B = g.B, H = g.H, W = g.W, h = g.h, w = g.w, rh = g.rh, rw = g.rw;
+    const bool bf16 = e->bf16;
+    // every UV plane of the head has the aspect of the resized image (v1.py:125, 133)
+    const float aspect = static_cast<float>(rw) / rh;
+    const float su = aspect / sqrtf(1.f + aspect * aspect), sv = 1.f / sqrtf(1.f + aspect * aspect);
+    const Level g0 = level_geom(h, w, 0);
+    MG_TRY(add_linear(e, pl, taps, B * h * w, v.proj.Ktot, v.proj.w, v.proj.N, EPI_DEC, vb.x0, v.proj.bias, nullptr, v.proj.N, "gemm.projects",
+                      nullptr, &g0));
+    const void* x = vb.x0;
+    double2* part = vb.gn_part;
+    float2* stats = vb.gn_stats;
+    auto nm = [](const char* kind, int l) { return std::string(kind) + ".l" + std::to_string(l); };
+    auto add_gn = [&](const void* src, void* dst, const Level& gl, int C, int G, const float* gamma, const float* beta, int l) {
+        const double px = static_cast<double>(B) * gl.H * gl.W;
+        pl->ops.add([=](cudaStream_t st) { return launch_gn_stats(src, gl, B, C, G, part, stats, bf16, st); }, nm("groupnorm_stats", l), 0, px * C * 2);
+        pl->ops.add([=](cudaStream_t st) { return launch_gn_relu(src, dst, gl, B, C, G, stats, gamma, beta, bf16, st); }, nm("groupnorm_relu", l), 0,
+                    px * C * 4);
+    };
+    for (int l = 0; l < c.num_levels; ++l) {
+        const V1Level& L = v.lv[l];
+        const V1Bufs::Lv& m = vb.lv[l];
+        const int Co = c.dim_upsample[l], Hd = c.hidden_mult * Co;
+        const Level gi = level_geom(h, w, l), go = level_geom(h, w, l + 1);
+        MG_TRY(add_conv(e, pl, L.convT, x, nullptr, gi, B, EPI_DEC, m.m1, nullptr, nullptr, go, Co, true, false, 0, 0, nm("convT", l)));
+        const float* wuv = L.wuv;
+        void* t = m.m1;
+        pl->ops.add([=](cudaStream_t st) { return launch_uv_convT(t, go, B, Co, wuv, su, sv, bf16, st); }, nm("uv_convT", l), 0,
+                    static_cast<double>(B) * go.H * go.W * Co * 4);
+        MG_TRY(add_conv(e, pl, L.conv, m.m1, nullptr, go, B, EPI_DEC, m.m0, nullptr, nullptr, go, Co, false, false, 0, 0, nm("conv3x3", l)));
+        void* xr = m.m0;
+        void* other = m.m1;
+        for (const V1Res& R : L.res) {
+            add_gn(xr, m.relu, go, Co, 1, R.g1, R.b1, l);
+            MG_TRY(add_conv(e, pl, R.c1, m.relu, nullptr, go, B, EPI_DEC, m.hraw, nullptr, nullptr, go, Hd, false, false, 0, 0, nm("conv3x3.res_a", l)));
+            add_gn(m.hraw, m.hrelu, go, Hd, R.G2, R.g2, R.b2, l);
+            MG_TRY(add_conv(e, pl, R.c2, m.hrelu, nullptr, go, B, EPI_DEC, other, nullptr, xr, go, Co, false, false, 0, 0, nm("conv3x3.res_b", l)));
+            std::swap(xr, other);
+        }
+        x = xr;
+    }
+    // V7: bilinear resize to the resized-image grid, both output blocks' 3x3 conv, then their UV part, ReLU and 1x1 convs
+    const int Cl = c.dim_upsample[c.num_levels - 1];
+    const Level gl = level_geom(h, w, c.num_levels), gr = full_geom(rh, rw);
+    const double pxr = static_cast<double>(B) * rh * rw;
+    void* full = vb.full;
+    pl->ops.add([=](cudaStream_t st) { return launch_resize_bilinear_nhwc(x, gl, full, gr, B, Cl, bf16, st); }, "resize_bilinear", 0,
+                static_cast<double>(B) * gl.H * gl.W * Cl * 2 + pxr * Cl * 2);
+    MG_TRY(add_conv(e, pl, v.out, vb.full, nullptr, gr, B, EPI_DEC, vb.fout, nullptr, nullptr, gr, v.out.N, false, false, 0, 0, "conv3x3.output"));
+    const void* fout = vb.fout;
+    const float* wout = v.wout;
+    float4* pts = vb.pts;
+    float* msk = vb.msk;
+    pl->ops.add([=](cudaStream_t st) { return launch_v1_output(fout, gr, B, wout, su, sv, pts, msk, bf16, st); }, "output_block", 2.0 * pxr * 64 * 10,
+                pxr * (64 * 2 + 20));
+    // V8 (phase 2: the caller's outputs): bilinear resize to (H, W), remap; the mask stays a raw logit
+    const int remap = c.remap_output;
+    Plan* P = pl;
+    pl->ops.add([=](cudaStream_t st) {
+        return launch_head_output(pts, nullptr, msk, B, rh, rw, H, W, remap, P->groups[0].points, nullptr, P->groups[0].mask, st, false);
+    }, "head_output", 0, static_cast<double>(B) * H * W * 16 + pxr * 20, 2);
+    return 0;
+}
+
+// MoGe-2 decoder maps: the groups run one after the other through ONE set of maps sized for the largest group
+struct V2Bufs {
+    StackBufs nb, hb;                               // neck, heads
+    std::vector<float4*> pts_lr, nrm_lr;            // low-resolution fp32 head outputs, per group
+    std::vector<float*> msk_lr;
+};
+
+static void alloc_v2_decoder(moge_engine* e, Plan* pl, WsAlloc& ws, V2Bufs* v) {
+    const moge_config_t& c = e->cfg;
+    const int G = static_cast<int>(pl->groups.size());
+    const int L = c.neck.num_levels;
+    auto alloc_stack = [&](const moge_stack_config_t& sc, StackBufs& sb) {
+        sb.x_raw.assign(L, nullptr); sb.x_relu.assign(L, nullptr); sb.y_relu.assign(L, nullptr); sb.t_up.assign(L, nullptr);
+        for (int l = 0; l < L; ++l) {
+            const int Cl = sc.dim_res_blocks[l];
+            // t_up[l]: resampler output feeding the 3x3 conv of level l (channels: convT -> C[l], bilinear -> C[l-1]);
+            // doubles as the second raw map of the residual ping-pong.
+            int ct = Cl;
+            if (l > 0 && sc.resamplers[l - 1] == MOGE_RESAMPLE_BILINEAR) ct = std::max(Cl, sc.dim_res_blocks[l - 1]);
+            size_t sz = 0, szt = 0;
+            for (const auto& g : pl->groups) {
+                const Level lg = level_geom(g.h, g.w, l);
+                sz = std::max(sz, map_bytes(lg, g.B, Cl));
+                szt = std::max(szt, map_bytes(lg, g.B, ct));
+            }
+            const bool folded_last = e->neck_fold && l == L - 1;      // with the neck fold no 16x-grid feature map exists at all
+            if (folded_last) continue;
+            sb.x_raw[l] = ws.take(sz);
+            if (sc.num_res_blocks[l] > 0) {
+                sb.x_relu[l] = ws.take(sz);
+                sb.y_relu[l] = ws.take(sz);
+            }
+            sb.t_up[l] = ws.take(szt);
+        }
+    };
+    alloc_stack(c.neck, v->nb);
+    // neck outputs must survive all heads: the neck's final x per level is whichever ping-pong map holds it (kept).
+    bool any_head = false;
+    for (int i = 0; i < 3; ++i) any_head |= head_cfg(e, i)->present != 0;
+    if (any_head) alloc_stack(*head_cfg(e, c.points_head.present ? 0 : c.normal_head.present ? 1 : 2), v->hb);
+    // low-resolution fp32 head outputs, PER GROUP (read by the phase-2 output kernels after every group's decoder has run)
+    v->pts_lr.assign(G, nullptr); v->nrm_lr.assign(G, nullptr); v->msk_lr.assign(G, nullptr);
+    for (int gi = 0; gi < G; ++gi) {
+        const Group& g = pl->groups[gi];
+        const Level gl = level_geom(g.h, g.w, L - 1);
+        const size_t px = static_cast<size_t>(g.B) * gl.H * gl.W;
+        if (c.points_head.present) v->pts_lr[gi] = static_cast<float4*>(ws.take(px * 16));
+        if (c.normal_head.present) v->nrm_lr[gi] = static_cast<float4*>(ws.take(px * 16));
+        if (c.mask_head.present) v->msk_lr[gi] = static_cast<float*>(ws.take(px * 4));
+    }
+}
+
 // Workspace layout + launch list of one call shape (a list of shape groups).  `dry`: only the byte count.
 static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cudaStream_t upload_stream = nullptr) {
     const moge_config_t& c = e->cfg;
@@ -644,49 +955,17 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     uint8_t* taps = static_cast<uint8_t*>(ws.take(static_cast<size_t>(TT) * c.num_taps * D * 2));
     float* cls = static_cast<float*>(ws.take(static_cast<size_t>(imgs) * D * 4));
     float* mlp_scratch = static_cast<float*>(ws.take(static_cast<size_t>(2) * imgs * 4096 * 4));
-    // ---- decoder buffers: the groups run one after the other through ONE set of maps sized for the largest group
+    // ---- decoder buffers: MoGe-1 or MoGe-2 (the encoder above is shared)
+    V1Bufs vb;
+    V2Bufs v2b;
+    if (e->v1) v1_alloc(e, pl->groups[0], ws, &vb);
+    else alloc_v2_decoder(e, pl, ws, &v2b);
     const int L = c.neck.num_levels;
-    auto alloc_stack = [&](const moge_stack_config_t& sc, StackBufs& sb) {
-        sb.x_raw.assign(L, nullptr); sb.x_relu.assign(L, nullptr); sb.y_relu.assign(L, nullptr); sb.t_up.assign(L, nullptr);
-        for (int l = 0; l < L; ++l) {
-            const int Cl = sc.dim_res_blocks[l];
-            // t_up[l]: resampler output feeding the 3x3 conv of level l (channels: convT -> C[l], bilinear -> C[l-1]);
-            // doubles as the second raw map of the residual ping-pong.
-            int ct = Cl;
-            if (l > 0 && sc.resamplers[l - 1] == MOGE_RESAMPLE_BILINEAR) ct = std::max(Cl, sc.dim_res_blocks[l - 1]);
-            size_t sz = 0, szt = 0;
-            for (const auto& g : pl->groups) {
-                const Level lg = level_geom(g.h, g.w, l);
-                sz = std::max(sz, map_bytes(lg, g.B, Cl));
-                szt = std::max(szt, map_bytes(lg, g.B, ct));
-            }
-            const bool folded_last = e->neck_fold && l == L - 1;      // with the neck fold no 16x-grid feature map exists at all
-            if (folded_last) continue;
-            sb.x_raw[l] = ws.take(sz);
-            if (sc.num_res_blocks[l] > 0) {
-                sb.x_relu[l] = ws.take(sz);
-                sb.y_relu[l] = ws.take(sz);
-            }
-            sb.t_up[l] = ws.take(szt);
-        }
-    };
-    StackBufs nb, hb;
-    alloc_stack(c.neck, nb);
-    // neck outputs must survive all heads: the neck's final x per level is whichever ping-pong map holds it (kept).
-    bool any_head = false;
-    for (int i = 0; i < 3; ++i) any_head |= head_cfg(e, i)->present != 0;
-    if (any_head) alloc_stack(*head_cfg(e, c.points_head.present ? 0 : c.normal_head.present ? 1 : 2), hb);
-    // low-resolution fp32 head outputs, PER GROUP (read by the phase-2 output kernels after every group's decoder has run)
-    std::vector<float4*> pts_lr(G, nullptr), nrm_lr(G, nullptr);
-    std::vector<float*> msk_lr(G, nullptr);
-    for (int gi = 0; gi < G; ++gi) {
-        const Group& g = pl->groups[gi];
-        const Level gl = level_geom(g.h, g.w, L - 1);
-        const size_t px = static_cast<size_t>(g.B) * gl.H * gl.W;
-        if (c.points_head.present) pts_lr[gi] = static_cast<float4*>(ws.take(px * 16));
-        if (c.normal_head.present) nrm_lr[gi] = static_cast<float4*>(ws.take(px * 16));
-        if (c.mask_head.present) msk_lr[gi] = static_cast<float*>(ws.take(px * 4));
-    }
+    StackBufs& nb = v2b.nb;
+    StackBufs& hb = v2b.hb;
+    std::vector<float4*>& pts_lr = v2b.pts_lr;
+    std::vector<float4*>& nrm_lr = v2b.nrm_lr;
+    std::vector<float*>& msk_lr = v2b.msk_lr;
     if (bytes_out) *bytes_out = ws.off + 1024;
     if (dry) return 0;
     if (ws.off > pl->ws_bytes) return set_error("workspace too small: need %zu bytes, got %zu", ws.off, pl->ws_bytes);
@@ -704,6 +983,19 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         const int B = g.B, H = g.H, W = g.W, h = g.h, w = g.w, T = h * w, N = T + 1;
         prow0[gi] = prow;
         uint8_t* patches_g = patches + static_cast<size_t>(prow) * 592 * 2;
+        if (e->v1) {
+            // MoGe-1 (v1.py:273-279): antialiased bicubic resize to (rh, rw), then the same normalise + aa-bilinear resize to
+            // (14h, 14w) + patchify as MoGe-2 (normalising after the second resize instead of between the two commutes: both
+            // resizes are convex combinations per channel and the normalisation is a per-channel affine map)
+            const int rh = g.rh, rw = g.rw;
+            float *tmp = vb.rs_tmp, *img = vb.rs_img;
+            pl->ops.add([=](cudaStream_t st) { return launch_resize_bicubic_aa(P->groups[gi].image, P->groups[gi].image_dtype, B, 3, H, W, rh, rw, tmp, img, st); },
+                        "resize_bicubic_aa", 0, static_cast<double>(B) * 3 * (static_cast<double>(H) * W * 4 + static_cast<double>(H) * rw * 8 + static_cast<double>(rh) * rw * 4), 0);
+            pl->ops.add([=](cudaStream_t st) { return launch_preprocess(img, MOGE_F32, B, rh, rw, h, w, patches_g, 592, bf16, st); },
+                        "preprocess", 0, static_cast<double>(B) * 3 * rh * rw * 4 + static_cast<double>(B) * T * 592 * 2, 0);
+            prow += static_cast<long>(B) * T;
+            continue;
+        }
         pl->ops.add([=](cudaStream_t st) { return launch_preprocess(P->groups[gi].image, P->groups[gi].image_dtype, B, H, W, h, w, patches_g, 592, bf16, st); },
                     gname("preprocess", gi), 0, static_cast<double>(B) * 3 * H * W * 4 + static_cast<double>(B) * T * 592 * 2, 0);
         prow += static_cast<long>(B) * T;
@@ -803,6 +1095,11 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         }
     }
     if (tap_idx != c.num_taps) return set_error("intermediate_layers must be increasing block indices < depth");
+    if (e->v1) {
+        MG_TRY(plan_v1_decoder(e, pl, taps, vb));
+        std::stable_sort(pl->ops.begin(), pl->ops.end(), [](const Op& a, const Op& b) { return a.phase < b.phase; });
+        return 0;
+    }
     // ---- decoder, group by group
     for (int gi = 0; gi < G; ++gi) {
         const Group& g = pl->groups[gi];
@@ -869,9 +1166,9 @@ constexpr size_t kMaxPlans = 16;
 // same shape but another workspace REPLACES the plan instead of orphaning it.  A plan owns its device buffers (pos tables,
 // attention work list) and frees them when it is replaced or evicted (LRU) -- after the device has drained, since launches
 // that read them may still be queued on the caller's stream.
-static int get_plan(moge_engine* e, const moge_group_t* groups, int n, void* ws, size_t ws_bytes, Plan** out, cudaStream_t st) {
+static int get_plan(moge_engine* e, const moge_group_t* groups, int n, void* ws, size_t ws_bytes, Plan** out, cudaStream_t st, int rh, int rw) {
     for (size_t i = 0; i < e->plans.size(); ++i) {
-        if (!e->plans[i]->same_shape(groups, n)) continue;
+        if (!e->plans[i]->same_shape(groups, n, rh, rw)) continue;
         if (e->plans[i]->ws == ws && e->plans[i]->ws_bytes == ws_bytes) {
             std::rotate(e->plans.begin() + i, e->plans.begin() + i + 1, e->plans.end());      // most recently used last
             *out = e->plans.back().get();
@@ -897,6 +1194,7 @@ static int get_plan(moge_engine* e, const moge_group_t* groups, int n, void* ws,
     for (int i = 0; i < n; ++i) {
         Group g;
         g.B = groups[i].B; g.H = groups[i].H; g.W = groups[i].W; g.h = groups[i].h; g.w = groups[i].w;
+        g.rh = rh; g.rw = rw;
         CUDA_TRY(cudaMalloc(&p, static_cast<size_t>(g.h) * g.w * D * 4));
         pl->owned.push_back(p);
         g.pos_table = static_cast<float*>(p);
@@ -929,6 +1227,31 @@ static int validate_cfg(const moge_config_t& c) {
     return 0;
 }
 
+static int validate_v1(const moge_v1_config_t& c) {
+    const int D = c.embed_dim;
+    if (!((D == 384 && c.depth == 12 && c.num_heads == 6) || (D == 768 && c.depth == 12 && c.num_heads == 12) ||
+          (D == 1024 && c.depth == 24 && c.num_heads == 16)))
+        return set_error("v1: backbone (embed_dim=%d, depth=%d, heads=%d) unsupported: DINOv2 ViT-S/B/L only", D, c.depth, c.num_heads);
+    if (c.num_taps <= 0 || c.num_taps > MOGE_MAX_TAPS) return set_error("v1: num_taps=%d out of range", c.num_taps);
+    for (int i = 0; i < c.num_taps; ++i)
+        if (c.taps[i] < 0 || c.taps[i] >= c.depth || (i > 0 && c.taps[i] <= c.taps[i - 1]))
+            return set_error("v1: intermediate_layers must be increasing block indices < depth");
+    if (c.compute_dtype != MOGE_F16 && c.compute_dtype != MOGE_BF16) return set_error("v1: compute_dtype must be MOGE_F16 or MOGE_BF16");
+    if (c.remap_output < MOGE_REMAP_LINEAR || c.remap_output > MOGE_REMAP_SINH_EXP) return set_error("v1: remap_output=%d unsupported", c.remap_output);
+    if (c.last_res_blocks != 0) return set_error("v1: last_res_blocks=%d unsupported (no released config uses it)", c.last_res_blocks);
+    if (c.last_conv_size != 1) return set_error("v1: last_conv_size=%d unsupported (no released config uses it)", c.last_conv_size);
+    if (c.last_conv_channels != 32) return set_error("v1: last_conv_channels=%d unsupported (32 only)", c.last_conv_channels);
+    if (c.hidden_norm != MOGE_V1_GROUP_NORM && c.hidden_norm != MOGE_V1_LAYER_NORM) return set_error("v1: hidden_norm=%d unsupported", c.hidden_norm);
+    if (c.num_res_blocks < 0 || c.hidden_mult < 1) return set_error("v1: num_res_blocks=%d / hidden_mult=%d out of range", c.num_res_blocks, c.hidden_mult);
+    if (c.dim_proj <= 0 || c.dim_proj % 128 || c.dim_proj > 2048) return set_error("v1: dim_proj=%d unsupported (a multiple of 128, <= 2048)", c.dim_proj);
+    if (c.num_levels < 1 || c.num_levels > MOGE_MAX_LEVELS) return set_error("v1: %d upsampling levels out of range", c.num_levels);
+    for (int l = 0; l < c.num_levels; ++l) {
+        const int C = c.dim_upsample[l], Hd = c.hidden_mult * C;
+        if (C <= 0 || C % 64 || Hd > 2048) return set_error("v1: dim_upsample[%d]=%d (hidden %d) unsupported (multiples of 64, <= 2048)", l, C, Hd);
+    }
+    return 0;
+}
+
 }  // namespace mg
 
 // ================================================================================================ C ABI
@@ -937,9 +1260,7 @@ extern "C" {
 const char* moge_last_error(void) { return mg::last_error(); }
 const char* moge_version(void) { return "moge_b200 0.1.0 sm_90a"; }
 
-int moge_engine_create(const moge_config_t* cfg, int device, moge_engine_t** out) {
-    if (!cfg || !out) return set_error("null argument");
-    MG_TRY(validate_cfg(*cfg));
+static int create_engine(const moge_config_t* cfg, int device, moge_engine_t** out) {
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) return set_error("no CUDA device: moge_b200 has no CPU fallback");
     CUDA_TRY(cudaSetDevice(device));
@@ -959,6 +1280,27 @@ int moge_engine_create(const moge_config_t* cfg, int device, moge_engine_t** out
         return set_error("stream/event creation failed");
     }
     *out = e;
+    return 0;
+}
+
+int moge_engine_create(const moge_config_t* cfg, int device, moge_engine_t** out) {
+    if (!cfg || !out) return set_error("null argument");
+    MG_TRY(validate_cfg(*cfg));
+    return create_engine(cfg, device, out);
+}
+
+int moge_engine_create_v1(const moge_v1_config_t* cfg, int device, moge_engine_t** out) {
+    if (!cfg || !out) return set_error("null argument");
+    MG_TRY(validate_v1(*cfg));
+    moge_config_t enc{};         // the encoder part only: build_plan takes the MoGe-1 decoder path for this engine
+    enc.embed_dim = cfg->embed_dim; enc.depth = cfg->depth; enc.num_heads = cfg->num_heads;
+    enc.num_taps = cfg->num_taps;
+    for (int i = 0; i < cfg->num_taps; ++i) enc.taps[i] = cfg->taps[i];
+    enc.remap_output = cfg->remap_output;
+    enc.compute_dtype = cfg->compute_dtype;
+    MG_TRY(create_engine(&enc, device, out));
+    (*out)->v1 = true;
+    (*out)->v1cfg = *cfg;
     return 0;
 }
 
@@ -1011,6 +1353,7 @@ static int check_groups(moge_engine_t* e, const moge_group_t* g, int n, bool nee
         if (!need_ptrs) continue;
         if (!g[i].image) return set_error("null argument");
         if (g[i].image_dtype != MOGE_F32 && g[i].image_dtype != MOGE_F16 && g[i].image_dtype != MOGE_BF16) return set_error("unsupported image dtype %d", g[i].image_dtype);
+        if (e->v1) continue;                 // moge_v1_forward checks its outputs
         if (g[i].points && !e->cfg.points_head.present) return set_error("points requested but the model has no points head");
         if (g[i].normal && !e->cfg.normal_head.present) return set_error("normal requested but the model has no normal head");
         if (g[i].mask_prob && !e->cfg.mask_head.present) return set_error("mask requested but the model has no mask head");
@@ -1022,6 +1365,7 @@ static int check_groups(moge_engine_t* e, const moge_group_t* g, int n, bool nee
 int moge_engine_workspace_bytes_groups(moge_engine_t* e, const moge_group_t* groups, int n, size_t* bytes) {
     if (!bytes) return set_error("null argument");
     MG_TRY(check_groups(e, groups, n, false));
+    if (e->v1) return set_error("a MoGe-1 engine takes moge_v1_workspace_bytes");
     Plan pl;
     for (int i = 0; i < n; ++i) {
         Group g;
@@ -1037,7 +1381,8 @@ int moge_engine_workspace_bytes(moge_engine_t* e, int B, int H, int W, int h, in
     return moge_engine_workspace_bytes_groups(e, &g, 1, bytes);
 }
 
-int moge_engine_forward_groups(moge_engine_t* e, const moge_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream) {
+// rh, rw: the resized image of a MoGe-1 call (0 for MoGe-2)
+static int forward_impl(moge_engine_t* e, const moge_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream, int rh, int rw) {
     if (!e || !workspace) return set_error("null argument");
     if (!e->finalized) return set_error("engine not finalized");
     MG_TRY(check_groups(e, groups, n, true));
@@ -1045,7 +1390,7 @@ int moge_engine_forward_groups(moge_engine_t* e, const moge_group_t* groups, int
     CUDA_TRY(cudaSetDevice(e->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     Plan* pl;
-    MG_TRY(get_plan(e, groups, n, workspace, workspace_bytes, &pl, st));
+    MG_TRY(get_plan(e, groups, n, workspace, workspace_bytes, &pl, st, rh, rw));
     long tokens = 0;
     for (int i = 0; i < n; ++i) {
         Group& g = pl->groups[i];
@@ -1097,6 +1442,48 @@ int moge_engine_forward_groups(moge_engine_t* e, const moge_group_t* groups, int
     }
     for (size_t i = i1; i < pl->ops.size(); ++i) MG_TRY(pl->ops[i].fn(st));
     return 0;
+}
+
+int moge_engine_forward_groups(moge_engine_t* e, const moge_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream) {
+    if (e && e->v1) return set_error("a MoGe-1 engine runs through moge_v1_forward");
+    return forward_impl(e, groups, n, workspace, workspace_bytes, stream, 0, 0);
+}
+
+static int check_v1_shape(moge_engine_t* e, int B, int H, int W, int rh, int rw) {
+    if (!e) return set_error("null argument");
+    if (!e->v1) return set_error("not a MoGe-1 engine (moge_engine_create_v1)");
+    if (B <= 0 || H <= 0 || W <= 0) return set_error("bad shape B=%d H=%d W=%d", B, H, W);
+    if (rh < 14 || rw < 14) return set_error("resized image %dx%d is smaller than one 14-pixel patch", rh, rw);
+    return 0;
+}
+
+int moge_v1_workspace_bytes(moge_engine_t* e, int B, int H, int W, int rh, int rw, size_t* bytes) {
+    if (!bytes) return set_error("null argument");
+    MG_TRY(check_v1_shape(e, B, H, W, rh, rw));
+    Plan pl;
+    Group g;
+    g.B = B; g.H = H; g.W = W; g.h = rh / 14; g.w = rw / 14; g.rh = rh; g.rw = rw;
+    pl.groups.push_back(g);
+    return build_plan(e, &pl, true, bytes);
+}
+
+int moge_v1_forward(moge_engine_t* e, const void* image, int image_dtype, int B, int H, int W, int rh, int rw, void* workspace,
+                    size_t workspace_bytes, float* points, float* mask, void* stream) {
+    MG_TRY(check_v1_shape(e, B, H, W, rh, rw));
+    if (!points || !mask) return set_error("null argument");
+    moge_group_t g{};
+    g.image = image; g.image_dtype = image_dtype; g.B = B; g.H = H; g.W = W; g.h = rh / 14; g.w = rw / 14;
+    g.points = points; g.mask_prob = mask;
+    return forward_impl(e, &g, 1, workspace, workspace_bytes, stream, rh, rw);
+}
+
+int moge_v1_postprocess(float* points, const float* mask, float mask_threshold, const float* focal_in, int B, int H, int W,
+                        int force_projection, int apply_mask, float* depth, uint8_t* mask_out, float* intrinsics, float* focal,
+                        float* shift, void* stream) {
+    if (!points || !mask || !depth || !mask_out || !intrinsics || !focal || !shift) return set_error("null argument");
+    if (B <= 0 || H <= 0 || W <= 0) return set_error("bad shape B=%d H=%d W=%d", B, H, W);
+    return launch_v1_postprocess(points, mask, mask_threshold, focal_in, B, H, W, force_projection, apply_mask, depth, mask_out, intrinsics,
+                                 focal, shift, static_cast<cudaStream_t>(stream));
 }
 
 int moge_engine_forward(moge_engine_t* e, const void* image, int image_dtype, int B, int H, int W, int h, int w, void* workspace,
@@ -1278,6 +1665,75 @@ int moge_op_conv(const void* x, const float* w, const float* bias, const void* s
     cudaStreamSynchronize(st);
     cudaFree(wp);
     return rc;
+}
+
+int moge_op_resize_bicubic_aa(const void* x, int dtype, int B, int C, int H, int W, int Ho, int Wo, float* out, void* stream) {
+    if (!x || !out) return set_error("null argument");
+    if (dtype != MOGE_F32 && dtype != MOGE_F16 && dtype != MOGE_BF16) return set_error("op_resize_bicubic_aa: unsupported dtype %d", dtype);
+    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || Ho <= 0 || Wo <= 0) return set_error("op_resize_bicubic_aa: bad shape");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float* tmp = nullptr;
+    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&tmp), static_cast<size_t>(B) * C * H * Wo * 4));
+    const int rc = launch_resize_bicubic_aa(x, dtype, B, C, H, W, Ho, Wo, tmp, out, st);
+    cudaStreamSynchronize(st);
+    cudaFree(tmp);
+    return rc;
+}
+
+int moge_op_groupnorm_relu(const void* x, void* out, const float* gamma, const float* beta, int B, int H, int W, int C, int G, int dtype,
+                           void* stream) {
+    if (!x || !out || !gamma || !beta) return set_error("null argument");
+    if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || C % 8) return set_error("op_groupnorm_relu: bad shape");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool bf16 = dtype == MOGE_BF16;
+    const Level g = level_geom(H, W, 0);
+    double2* part = nullptr;
+    float2* stats = nullptr;
+    int rc = 0;
+    if (G <= 0 || cudaMalloc(reinterpret_cast<void**>(&part), static_cast<size_t>(B) * gn_tiles(H, W, C) * G * 16) != cudaSuccess ||
+        cudaMalloc(reinterpret_cast<void**>(&stats), static_cast<size_t>(B) * G * 8) != cudaSuccess)
+        rc = set_error("op_groupnorm_relu: G=%d / cudaMalloc failed", G);
+    if (rc == 0) rc = launch_gn_stats(x, g, B, C, G, part, stats, bf16, st);
+    if (rc == 0) rc = launch_gn_relu(x, out, g, B, C, G, stats, gamma, beta, bf16, st);
+    cudaStreamSynchronize(st);
+    cudaFree(part); cudaFree(stats);
+    return rc;
+}
+
+int moge_op_conv_transpose_uv(const void* x, const float* w, const float* bias, void* out, int B, int H, int W, int Cin, int Cout, float su, float sv,
+                     int dtype, void* stream) {
+    // the engine's MoGe-1 upsampling ConvTranspose: the GEMM over the feature rows (pixel shuffle), then the input-grid UV term
+    if (!x || !w || !bias || !out) return set_error("null argument");
+    if (B <= 0 || H <= 0 || W <= 0) return set_error("op_conv_transpose_uv: bad shape");
+    if (Cin % 64 || Cout <= 0 || Cout % 32) return set_error("op_conv_transpose_uv: Cin %% 64 and Cout %% 32 must be 0");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const bool bf16 = dtype == MOGE_BF16;
+    void* wp = nullptr;
+    float* wuv = nullptr;
+    int rc = 0;
+    if (cudaMalloc(&wp, static_cast<size_t>(4) * Cout * Cin * 2) != cudaSuccess ||
+        cudaMalloc(reinterpret_cast<void**>(&wuv), static_cast<size_t>(8) * Cout * 4) != cudaSuccess)
+        rc = set_error("op_conv_transpose_uv: cudaMalloc failed");
+    if (rc == 0) rc = launch_pack_convT(w, wp, bf16, Cin, Cout, st);
+    if (rc == 0) rc = launch_pack_convT_uv(w, Cin, Cout, wuv, st);
+    if (rc == 0) {
+        ConvW cw;
+        cw.w = wp; cw.bias = const_cast<float*>(bias); cw.N = 4 * Cout; cw.Ktot = Cin; cw.cin = Cin; cw.taps = 1;
+        const Level gs = level_geom(H, W, 0), go = level_geom(H, W, 1);
+        GemmLaunch g;
+        rc = gemm_conv(&g, bf16, cw, x, nullptr, gs, B, EPI_DEC, out, nullptr, nullptr, go, Cout, true, false, 0.f, 0.f);
+        if (rc == 0) rc = launch_gemm(g, dev_sms(), st);
+        if (rc == 0) rc = launch_uv_convT(out, go, B, Cout, wuv, su, sv, bf16, st);
+    }
+    cudaStreamSynchronize(st);
+    cudaFree(wp); cudaFree(wuv);
+    return rc;
+}
+
+int moge_bicubic_aa_weights(int in, int out, int i, int* lo, float* w, int cap) {
+    if (!lo) return set_error("null argument");
+    if (in <= 0 || out <= 0 || i < 0 || i >= out) return set_error("bicubic_aa_weights: bad arguments in=%d out=%d i=%d", in, out, i);
+    return bicubic_aa_taps(in, out, i, lo, w, cap);
 }
 
 }  // extern "C"

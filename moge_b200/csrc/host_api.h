@@ -140,8 +140,9 @@ int launch_ln_rstd(const float2* stats, int ld, int parts, int rows, int D, floa
 int launch_scale_head(const float* cls, const float* const* w, const float* const* bias, const int* dims, int nlayers,
                       int B, float* out, float* scratch, cudaStream_t st);
 // K17: bilinear resize of the low-res head maps to (H,W) + remap -> points (B,H,W,3), normal (B,H,W,3), mask prob (B,H,W)
+// (mask_sigmoid = false: the resized mask logit as is, MoGe-1)
 int launch_head_output(const float4* pts_lr, const float4* nrm_lr, const float* msk_lr, int B, int Hl, int Wl, int H, int W,
-                       int remap_mode, float* points, float* normal, float* mask, cudaStream_t st);
+                       int remap_mode, float* points, float* normal, float* mask, cudaStream_t st, bool mask_sigmoid = true);
 // K18
 int launch_focal_shift(const float* points, const float* mask_prob, const uint8_t* mask_u8, int B, int H, int W,
                        const float* focal_in, float* focal_out, float* shift_out, cudaStream_t st);
@@ -149,6 +150,28 @@ int launch_focal_shift(const float* points, const float* mask_prob, const uint8_
 int launch_postprocess(float* points, const float* normal_in, const float* mask_prob, const float* metric_scale,
                        const float* focal, const float* shift, int B, int H, int W, int force_projection, int apply_mask,
                        float* depth, float* normal_out, uint8_t* mask_out, float* intrinsics, cudaStream_t st);
+
+// ---- MoGe-1 kernels (v1.cu); maps are padded NHWC 16-bit with C channels on grid g, border written
+// antialiased bicubic (a = -0.5) resize (B,C,H,W) image -> fp32 (B,C,Ho,Wo) via the fp32 row pass tmp (B,C,H,Wo)
+int launch_resize_bicubic_aa(const void* image, int dtype, int B, int C, int H, int W, int Ho, int Wo, float* tmp, float* out, cudaStream_t st);
+// host side of the same filter: taps [*lo, *lo + n) of output index i and their normalised weights (w may be NULL); returns n
+int bicubic_aa_taps(int in, int out, int i, int* lo, float* w, int cap);
+// GroupNorm(G, C) statistics (mean, rstd) per (image, group); partials: B * gn_tiles(H, W, C) * G double2 of scratch
+int gn_tiles(int H, int W, int C);
+int launch_gn_stats(const void* map, const Level& g, int B, int C, int G, double2* partials, float2* stats, bool bf16, cudaStream_t st);
+// dst = relu(gamma * (src - mean) * rstd + beta)
+int launch_gn_relu(const void* src, void* dst, const Level& g, int B, int C, int G, const float2* stats, const float* gamma, const float* beta,
+                   bool bf16, cudaStream_t st);
+// in place: + the input-grid UV term of a k2s2 ConvTranspose, wuv [2][4 phases][C]; g is the OUTPUT grid
+int launch_uv_convT(void* map, const Level& g, int B, int C, const float* wuv, float su, float sv, bool bf16, cudaStream_t st);
+// wuv [2][4][Cout] from rows Cin, Cin + 1 of a ConvTranspose2d weight (Cin + 2, Cout, 2, 2) fp32 (load time)
+int launch_pack_convT_uv(const float* w, int Cin, int Cout, float* wuv, cudaStream_t st);
+// bilinear (align_corners=False) resize of a padded map from grid gs to grid gd
+int launch_resize_bilinear_nhwc(const void* src, const Level& gs, void* dst, const Level& gd, int B, int C, bool bf16, cudaStream_t st);
+// output-block tail over the 64-channel conv output: + folded UV, ReLU, block-diagonal 64 -> 4; pts (x,y,z,-), msk fp32 per pixel
+int launch_v1_output(const void* map, const Level& g, int B, const float* wf, float su, float sv, float4* pts, float* msk, bool bf16, cudaStream_t st);
+int launch_v1_postprocess(float* points, const float* mask, float mask_threshold, const float* focal_in, int B, int H, int W, int force_projection,
+                          int apply_mask, float* depth, uint8_t* mask_out, float* intrinsics, float* focal, float* shift, cudaStream_t st);
 
 // ---- weight packing (pack.cu): generic strided gather/cast and a small fp32 GEMM for load-time folds
 int launch_cast_2d(const void* src, int src_dtype, void* dst, bool bf16, int rows, int cols, int src_ld, int dst_ld,

@@ -162,6 +162,107 @@ def _make_well_posed(cfg: Dict, sd: Dict[str, torch.Tensor], k: float = 4.0, g: 
         sd[f"normal_head.output_blocks.{last}.bias"] += torch.tensor([0.3, -0.4, -1.2])
 
 
+def _v1_shapes(cfg: Dict) -> "OrderedDict[str, tuple]":
+    """State-dict shapes of the reference `moge.model.v1.MoGeModel(**cfg)` (v1.py:145-204): its buffers, the DINOv2 backbone under
+    `backbone.`, and the Head under `head.`."""
+    D, depth, _ = backbone_dims(cfg["encoder"])
+    s: "OrderedDict[str, tuple]" = OrderedDict()
+    s["image_mean"] = (1, 3, 1, 1)
+    s["image_std"] = (1, 3, 1, 1)
+    for k, v in _shapes({"encoder": {"backbone": cfg["encoder"], "intermediate_layers": [], "dim_out": D}}).items():
+        if k.startswith("encoder.backbone."):
+            s[k[len("encoder."):]] = v
+    taps = cfg.get("intermediate_layers", 4)
+    nt = taps if isinstance(taps, int) else len(taps)
+    P = cfg.get("dim_proj", 512)
+    ups = list(cfg.get("dim_upsample", [256, 128, 128]))
+    hm, nres = cfg.get("dim_times_res_block_hidden", 1), cfg.get("num_res_blocks", 1)
+    lc, lcs, lrb = cfg.get("last_conv_channels", 32), cfg.get("last_conv_size", 1), cfg.get("last_res_blocks", 0)
+
+    def res_block(p, c, hid):
+        s[p + "layers.0.weight"] = (c,); s[p + "layers.0.bias"] = (c,)
+        s[p + "layers.2.weight"] = (hid, c, 3, 3); s[p + "layers.2.bias"] = (hid,)
+        s[p + "layers.3.weight"] = (hid,); s[p + "layers.3.bias"] = (hid,)
+        s[p + "layers.5.weight"] = (c, hid, 3, 3); s[p + "layers.5.bias"] = (c,)
+
+    for j in range(nt):
+        s[f"head.projects.{j}.weight"] = (P, D, 1, 1)
+        s[f"head.projects.{j}.bias"] = (P,)
+    for l, (ci, co) in enumerate(zip([P] + ups[:-1], ups)):
+        p = f"head.upsample_blocks.{l}."
+        s[p + "0.0.weight"] = (ci + 2, co, 2, 2); s[p + "0.0.bias"] = (co,)
+        s[p + "0.1.weight"] = (co, co, 3, 3); s[p + "0.1.bias"] = (co,)
+        for r in range(nres):
+            res_block(f"{p}{1 + r}.", co, hm * co)
+    for k, n in enumerate((3, 1)):
+        p = f"head.output_block.{k}."
+        s[p + "0.weight"] = (lc, ups[-1] + 2, 3, 3); s[p + "0.bias"] = (lc,)
+        for r in range(lrb):
+            res_block(f"{p}{1 + r}.", lc, hm * lc)
+        s[f"{p}{2 + lrb}.weight"] = (n, lc, lcs, lcs); s[f"{p}{2 + lrb}.bias"] = (n,)
+    return s
+
+
+def v1_expected_keys(cfg: Dict):
+    """State-dict keys of the reference `moge.model.v1.MoGeModel(**cfg)`, in its order."""
+    return list(_v1_shapes(cfg).keys())
+
+
+def make_v1_state_dict(cfg: Dict, seed: int = 0, mask_bias: float = 1.0, well_posed: bool = False) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded fp32 MoGe-1 state dict, values scaled as make_state_dict's.  The v1 mask is thresholded raw (no sigmoid) at 0.5, so
+    `mask_bias` lifts the mask output's bias until most pixels pass.  `well_posed=True`: the points branch of the output block
+    carries the UV planes (u, v at the centre tap of channels 0 / 1 of its 3x3 conv, kept positive through the ReLU by a bias) into
+    x / y, and its log-depth output is tempered: with remap 'exp' the point map is (g u e^z, g v e^z, e^z) + noise, a pinhole view
+    with focal ~ 1/g, so the focal/shift solve of infer() is well-conditioned."""
+    g = torch.Generator(device="cpu").manual_seed(seed)
+    sd: "OrderedDict[str, torch.Tensor]" = OrderedDict()
+    for name, shape in _v1_shapes(cfg).items():
+        def randn(std=1.0):
+            return torch.randn(shape, generator=g, dtype=torch.float32) * std
+        if name == "image_mean":
+            t = torch.tensor(IMAGE_MEAN).view(shape)
+        elif name == "image_std":
+            t = torch.tensor(IMAGE_STD).view(shape)
+        elif name.endswith("pos_embed") or name.endswith("cls_token") or name.endswith("mask_token"):
+            t = randn(0.25)
+        elif len(shape) == 1 and name.endswith(".weight"):          # LayerNorm / GroupNorm scales
+            t = 1.0 + randn(0.1)
+        elif name.endswith(".gamma"):
+            t = 0.25 + randn(0.05)
+        elif name.endswith(".bias"):
+            t = randn(0.05)
+            if name.startswith("head.output_block.1.") and shape == (1,):
+                t = t + mask_bias
+        else:
+            if ".upsample_blocks." in name and name.endswith(".0.0.weight"):
+                fan_in = shape[0]                     # ConvTranspose2d: (C_in, C_out, 2, 2)
+            else:
+                fan_in = 1
+                for d in shape[1:]:
+                    fan_in *= d
+            gain = 0.3 if (name.startswith("head.output_block.") and shape[-1] == cfg.get("last_conv_size", 1) and shape[0] <= 3) else 1.0
+            t = randn(gain / fan_in ** 0.5)
+        sd[name] = t.contiguous()
+    if well_posed:
+        _make_v1_well_posed(cfg, sd)
+    return sd
+
+
+def _make_v1_well_posed(cfg: Dict, sd: Dict[str, torch.Tensor], gf: float = 1.2, lift: float = 2.0, z_gain: float = 0.35,
+                        z_bias: float = 0.8, xy_noise: float = 0.1) -> None:
+    C = list(cfg.get("dim_upsample", [256, 128, 128]))[-1]
+    w = sd["head.output_block.0.0.weight"]
+    w[0] = 0; w[1] = 0; w[0, C, 1, 1] = 1.0; w[1, C + 1, 1, 1] = 1.0
+    b = sd["head.output_block.0.0.bias"]
+    b[0] = lift; b[1] = lift                              # relu(u + lift) = u + lift: |u|, |v| < 1
+    last = 2 + cfg.get("last_res_blocks", 0)
+    wo = sd[f"head.output_block.0.{last}.weight"]
+    bo = sd[f"head.output_block.0.{last}.bias"]
+    wo[0] *= xy_noise; wo[1] *= xy_noise; wo[2] *= z_gain
+    wo[0, 0] = gf; wo[1, 1] = gf; wo[0, 1] = 0; wo[1, 0] = 0
+    bo[0] = -gf * lift; bo[1] = -gf * lift; bo[2] += z_bias
+
+
 def save_checkpoint(path, cfg: Dict, seed: int = 0, **kw) -> None:
     """Write a reference-format checkpoint file (v2.py:99-105 reads it with weights_only=True)."""
     torch.save({"model_config": cfg, "model": make_state_dict(cfg, seed, **kw)}, path)
