@@ -245,6 +245,45 @@ int moge_align_anchored(const float* src, const float* tgt, const float* w, int 
  * reference's torch.linalg.lstsq call poses it (the column of ones is not weighted); w NULL = 1.  fp64 accumulation, any n.  */
 int moge_align_affine_lstsq(const float* x, const float* y, const float* w, int64_t batch, int64_t n, float* a, float* b, void* stream);
 
+/* ---- evaluation metrics (moge/test/metrics.py; Python: moge_b200.metrics, alias moge.test.metrics).
+ * Images are (batch, H, W) fp32 maps, (batch, H, W, 3) point maps and a (batch, H, W) uint8 mask, contiguous on the device.
+ * Every floating-point reduction is fp64 over fixed tiles set by H x W, summed in a fixed order: results do not change from run
+ * to run nor with the other images of the batch.  A variant is a prediction map plus per-image params (batch, 4) on the device:
+ * depth kinds read (scale, shift, clamp, -), points kinds (scale, shift x, y, z).  The aligned value is formed in fp32 with one
+ * rounding per operation: x s, x s + b, 1 / max(d s + b, clamp) with d = x or 1 / x, x + shift, x s + shift.          */
+#define MOGE_METRICS_MAX_SEGMENTS 256     /* segment ids per image */
+#define MOGE_METRICS_MAX_VARIANTS 8
+#define MOGE_METRICS_F1_THRESHOLDS 10
+#define MOGE_METRICS_F1_COUNTS 90         /* per image: (radius 1..3, threshold, {TP, GT, pred}) */
+#define MOGE_METRICS_OUT_SEGMENTS 17      /* moge_metrics_eval output: first per-segment entry */
+enum { MOGE_MV_DEPTH = 0, MOGE_MV_DEPTH_SCALE = 1, MOGE_MV_DEPTH_AFFINE = 2, MOGE_MV_DISPARITY = 3, MOGE_MV_DISPARITY_FROM_DEPTH = 4,
+       MOGE_MV_POINTS_SHIFT = 5, MOGE_MV_POINTS_SCALE = 6, MOGE_MV_POINTS_AFFINE = 7 };
+typedef struct { int kind; const float* src; const float* params; } moge_metric_variant_t;
+/* workspace (256-byte aligned) of moge_metrics_stats / moge_metrics_eval for S segment slots per image (0 <= S <= 256) */
+int moge_metrics_workspace_bytes(int64_t batch, int H, int W, int S, size_t* bytes);
+/* masked nearest resize to th x tw (utils3d.pt.masked_nearest_resize): lr_mask, lr_index (flat source pixel) (batch, th, tw); the
+ * valid targets in row-major order as list (batch, th*tw) with list_w = 1, padded by the first entry at list_w = 0; count (batch). */
+int moge_metrics_resize(const uint8_t* mask, int64_t batch, int H, int W, int th, int tw, uint8_t* lr_mask, int64_t* lr_index,
+                        int64_t* list, float* list_w, int32_t* count, void* stream);
+/* statistics: disp_params (batch, 4) = the least-squares (scale, shift) of disparity (disp_src, or 1 / disp_src when
+ * disp_from_depth; NULL: NaN) against 1 / gt_depth over the mask, fp32(1 / (double) max masked GT), max masked GT.  With a
+ * segmentation map seg (batch, H, W) int32, seg_ids (batch, S) sorted unique per image and seg_count (batch) ids in use:
+ * diameter (batch, S) = max over xyz of the extent of the GT points over (seg == id) & mask (NaN when empty).            */
+int moge_metrics_stats(const float* gt_depth, const float* gt_points, const uint8_t* mask, const float* disp_src, int disp_from_depth,
+                       const int32_t* seg, const int32_t* seg_ids, const int32_t* seg_count, int S, int64_t batch, int H, int W,
+                       float* disp_params, float* diameter, void* workspace, size_t workspace_bytes, void* stream);
+/* metric pass: out (batch, out_stride) doubles: [2v] = sum of rel, [2v + 1] = delta1 count of variant v, [16] = mask count; with
+ * segments, [17 + 3s + {0, 1, 2}] = (sum of |p - g| / diameter, count of |p - g| < 0.25 diameter, pixels) of slot s, where p is
+ * local_src aligned by seg_params (batch, S, 4) (scale, shift xyz).                                                        */
+int moge_metrics_eval(const float* gt_depth, const float* gt_points, const uint8_t* mask, const moge_metric_variant_t* variants,
+                      int num_variants, const float* local_src, const int32_t* seg, const int32_t* seg_ids, const int32_t* seg_count, int S,
+                      const float* seg_params, const float* seg_diameter, int64_t batch, int H, int W, double* out, int64_t out_stride,
+                      void* workspace, size_t workspace_bytes, void* stream);
+/* boundary F1 counts of a depth variant against gt_depth for radii 1, 2, 3 and the 10 sorted thresholds (host array): ADDED to
+ * counts (batch, counts_stride) int64 at [(r - 1) * 30 + t * 3 + {TP, GT, pred}]; the caller zeroes them.                    */
+int moge_metrics_boundary(const float* gt_depth, const uint8_t* mask, const moge_metric_variant_t* aligned, const float* thresholds,
+                          int64_t batch, int H, int W, int64_t* counts, int64_t counts_stride, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -29,7 +29,11 @@ EXPORTS = [
     "moge_align_workspace_bytes", "moge_align", "moge_align_anchored", "moge_align_affine_lstsq",
     "moge_engine_create_v1", "moge_v1_workspace_bytes", "moge_v1_forward", "moge_v1_postprocess", "moge_op_resize_bicubic_aa",
     "moge_op_groupnorm_relu", "moge_bicubic_aa_weights", "moge_op_conv_transpose_uv",
+    "moge_metrics_workspace_bytes", "moge_metrics_resize", "moge_metrics_stats", "moge_metrics_eval", "moge_metrics_boundary",
 ]
+METRICS_MAX_SEGMENTS, METRICS_MAX_VARIANTS, METRICS_F1_THRESHOLDS, METRICS_F1_COUNTS, METRICS_OUT_SEGMENTS = 256, 8, 10, 90, 17
+(MV_DEPTH, MV_DEPTH_SCALE, MV_DEPTH_AFFINE, MV_DISPARITY, MV_DISPARITY_FROM_DEPTH, MV_POINTS_SHIFT, MV_POINTS_SCALE,
+ MV_POINTS_AFFINE) = range(8)
 
 
 class StackConfig(C.Structure):
@@ -69,6 +73,11 @@ class Group(C.Structure):
         ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("h", C.c_int), ("w", C.c_int),
         ("points", C.c_void_p), ("normal", C.c_void_p), ("mask_prob", C.c_void_p), ("metric_scale", C.c_void_p),
     ]
+
+
+class MetricVariant(C.Structure):
+    """moge_metric_variant_t: a prediction map and its per-image (batch, 4) params on the device."""
+    _fields_ = [("kind", C.c_int), ("src", C.c_void_p), ("params", C.c_void_p)]
 
 
 class MogeError(RuntimeError):
@@ -130,6 +139,12 @@ def lib() -> C.CDLL:
     L.moge_op_groupnorm_relu.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]
     L.moge_op_conv_transpose_uv.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, C.c_float, C.c_float, ci, vp]
     L.moge_bicubic_aa_weights.argtypes = [ci, ci, ci, C.POINTER(ci), C.POINTER(C.c_float), ci]
+    L.moge_metrics_workspace_bytes.argtypes = [i64, ci, ci, ci, C.POINTER(sz)]
+    L.moge_metrics_resize.argtypes = [vp, i64, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp]
+    L.moge_metrics_stats.argtypes = [vp, vp, vp, vp, ci, vp, vp, vp, ci, i64, ci, ci, vp, vp, vp, sz, vp]
+    L.moge_metrics_eval.argtypes = [vp, vp, vp, C.POINTER(MetricVariant), ci, vp, vp, vp, vp, ci, vp, vp, i64, ci, ci, vp, i64, vp, sz,
+                                    vp]
+    L.moge_metrics_boundary.argtypes = [vp, vp, C.POINTER(MetricVariant), C.POINTER(C.c_float), i64, ci, ci, vp, i64, vp]
     for name in EXPORTS:
         if name not in ("moge_last_error", "moge_version", "moge_engine_destroy"):
             getattr(L, name).restype = ci

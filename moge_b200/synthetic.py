@@ -353,3 +353,102 @@ def alignment_arguments(fn: str, batch_shape, n: int, seed: int, trunc=None, sin
     if fn in ("align", "align_depth_scale", "align_depth_affine"):
         return (src[..., 2], tgt[..., 2], w, trunc)
     return (src, tgt, w, trunc)
+
+
+METRICS_KEYS = {
+    "moge2": ("points_metric", "depth_metric", "intrinsics"),
+    "moge1": ("points_scale_invariant", "depth_scale_invariant", "intrinsics"),
+    "depth_affine": ("depth_affine_invariant",),
+    "disparity": ("disparity_affine_invariant",),
+    "points_affine": ("points_affine_invariant",),
+}
+
+
+def _unproject(depth: torch.Tensor, fx: float, fy: float) -> torch.Tensor:
+    H, W = depth.shape
+    u = (torch.arange(W, dtype=torch.float32) + 0.5) / W
+    v = (torch.arange(H, dtype=torch.float32) + 0.5) / H
+    return torch.stack([(u[None, :] - 0.5) / fx * depth, (v[:, None] - 0.5) / fy * depth, depth], dim=-1)
+
+
+def _box(g: torch.Generator, H: int, W: int, lo: float, hi: float):
+    h = max(1, int(H * (lo + (hi - lo) * torch.rand((), generator=g).item())))
+    w = max(1, int(W * (lo + (hi - lo) * torch.rand((), generator=g).item())))
+    i = int(torch.randint(0, max(1, H - h), (), generator=g))
+    j = int(torch.randint(0, max(1, W - w), (), generator=g))
+    return i, j, h, w
+
+
+def synthetic_metrics_case(seed: int, H: int, W: int, keys, is_metric: bool = True, sharp: bool = True, segments: int = 0,
+                           negative: bool = False):
+    """(pred, gt) dicts of CPU fp32 tensors for compute_metrics, from a seeded generator.
+
+    GT: piecewise-planar depth (a tilted background plane and occluding tilted boxes), points by unprojection with normalised
+    intrinsics, a mask with box holes and 5 % dropouts.  With `segments` > 0, box segments (later ones overwrite earlier ones)
+    plus one tiny segment (under 10 low-resolution pixels), one label whose id is absent from the map and one duplicated id.
+    Predictions: GT perturbed by scale, shift, smooth noise, 1 % outliers and a blur across the occlusion edges; `negative` puts a
+    few negative depths in.  `keys` names the predicted entries (METRICS_KEYS)."""
+    g = torch.Generator().manual_seed(seed)
+    fx = 0.55 + 0.4 * torch.rand((), generator=g).item()
+    fy = fx * W / H
+    u = (torch.arange(W, dtype=torch.float32) + 0.5) / W
+    v = (torch.arange(H, dtype=torch.float32) + 0.5) / H
+    depth = 6.0 + 2.0 * (u[None, :] - 0.5) + 3.0 * (v[:, None] - 0.5)
+    for _ in range(4):
+        i, j, h, w = _box(g, H, W, 0.15, 0.4)
+        z = 1.5 + 3.0 * torch.rand((), generator=g).item()
+        tilt = 0.5 * (torch.rand(2, generator=g) - 0.5)
+        depth[i:i + h, j:j + w] = z + tilt[0] * (u[None, j:j + w] - 0.5) + tilt[1] * (v[i:i + h, None] - 0.5)
+    points = _unproject(depth, fx, fy)
+    mask = torch.ones(H, W, dtype=torch.bool)
+    for _ in range(3):
+        i, j, h, w = _box(g, H, W, 0.05, 0.15)
+        mask[i:i + h, j:j + w] = False
+    mask &= torch.rand(H, W, generator=g) > 0.05
+    K = torch.tensor([[fx, 0, 0.5], [0, fy, 0.5], [0, 0, 1]], dtype=torch.float32)
+    gt = {"depth": depth, "points": points, "depth_mask": mask, "intrinsics": K, "is_metric": is_metric, "has_sharp_boundary": sharp}
+    if segments:
+        seg = torch.zeros(H, W, dtype=torch.int32)
+        labels = {}
+        for s in range(1, segments + 1):
+            i, j, h, w = _box(g, H, W, 0.1, 0.35)
+            seg[i:i + h, j:j + w] = s
+            labels[f"seg{s}"] = s
+        ti, tj = H // 2, W // 2
+        seg[ti:ti + max(1, H // 40), tj:tj + max(1, W // 40)] = segments + 1     # tiny: a handful of low-resolution pixels
+        labels["tiny"] = segments + 1
+        labels["absent"] = segments + 1000
+        labels["duplicate"] = 1
+        gt["segmentation_mask"], gt["segmentation_labels"] = seg, labels
+    # prediction: smooth noise, blurred edges, outliers
+    smooth = torch.nn.functional.interpolate(torch.randn(1, 1, 8, 8, generator=g), size=(H, W), mode="bilinear", align_corners=False)[0, 0]
+    blurred = torch.nn.functional.avg_pool2d(depth[None, None], 5, 1, 2, count_include_pad=False)[0, 0]
+    pd = blurred * (1 + 0.03 * smooth)
+    out = torch.rand(H, W, generator=g) < 0.01
+    pd = torch.where(out, pd * (0.3 + 2 * torch.rand(H, W, generator=g)), pd)
+    if negative:
+        pd = torch.where(torch.rand(H, W, generator=g) < 0.002, -pd, pd)
+    scale, shift = 0.7 + 0.6 * torch.rand((), generator=g).item(), 0.3 * torch.rand((), generator=g).item()
+    pfx = fx * (1 + 0.1 * (torch.rand((), generator=g).item() - 0.5))
+    ppts = _unproject(pd, pfx, pfx * W / H)
+    pred = {}
+    for k in keys:
+        if k == "intrinsics":
+            pred[k] = torch.tensor([[pfx, 0, 0.5], [0, pfx * W / H, 0.5], [0, 0, 1]], dtype=torch.float32)
+        elif k == "depth_metric":
+            pred[k] = pd.clone()
+        elif k == "depth_scale_invariant":
+            pred[k] = pd * scale
+        elif k == "depth_affine_invariant":
+            pred[k] = pd * scale + shift
+        elif k == "disparity_affine_invariant":
+            pred[k] = scale / pd + 0.05 * shift
+        elif k == "points_metric":
+            pred[k] = ppts + torch.tensor([0.02, -0.01, 0.05])
+        elif k == "points_scale_invariant":
+            pred[k] = ppts * scale
+        elif k == "points_affine_invariant":
+            pred[k] = ppts * scale + torch.tensor([0.1, -0.05, shift])
+        else:
+            raise KeyError(k)
+    return pred, gt
