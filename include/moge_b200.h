@@ -154,7 +154,7 @@ int moge_op_linear(const void* x, const void* w, const float* bias, const float*
 /* y16[M,N] = epilogue(LayerNorm_eps1e-6(x32[M,K]; ln_gamma, ln_beta) @ w32[N,K]^T + bias), epi 0 or 1 as above, computed the way the
  * engine computes norm1->qkv and norm2->fc1 (dinov2/layers/block.py:84-92): the GEMM runs on the ROUNDED rows with the centred
  * weight W diag(gamma) (I - 11^T/K) (mean removal is linear), the epilogue scales by rstd[row] and adds b + W beta.
- * This is the engine's MOGE_B200_LNFOLD=1 path.  K % 64 == 0, N % 128 == 0.                                               */
+ * K % 64 == 0, N % 128 == 0.                                                                                                */
 int moge_op_linear_ln(const float* x, const float* ln_gamma, const float* ln_beta, const float* w, const float* bias, void* out, int M,
                       int N, int K, int epi, int dtype, void* stream);
 /* softmax(q k^T / 8) v per head on a fused qkv buffer (B,N,3*D) -> (B,N,D); D = heads*64 (attention.py:70-81) */

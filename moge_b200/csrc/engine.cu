@@ -11,7 +11,6 @@
 #include <string>
 #include <vector>
 #include <math.h>
-#include <stdlib.h>
 
 namespace mg {
 
@@ -44,9 +43,8 @@ struct StackW {
     std::vector<ConvW> post;                    // [level] 3x3 after the resampler (writes level l+1), fused in-block / UV
     // folded last level of a head
     ConvW headout;
-    float* waux = nullptr;          // [ncomp, 32] = output block o last-level input block (applied to the neck's last-level map)
     int ncomp = 0;
-    // neck only: its last level folded through the heads' waux (EPI_NECKOUT): N = 4 phases x 8 components
+    // neck only: its last level folded through the heads' last-level input + output blocks (EPI_NECKOUT): N = 4 phases x 8 components
     ConvW neckout;
 };
 
@@ -140,11 +138,11 @@ struct moge_engine {
     // packed encoder
     void* w_patch = nullptr;
     struct Blk {
-        void *wqkv, *wproj, *wfc1, *wfc2;
-        const float *bqkv, *bproj, *bfc1, *bfc2, *g1, *g2, *ln1g, *ln1b, *ln2g, *ln2b;
-        // LayerNorm folded into the GEMM (default; MOGE_B200_LNFOLD=0 disables): centred W diag(gamma) in 16 bit, b + W beta
+        // qkv / fc1 with norm1 / norm2 folded in: centred W diag(gamma) in 16 bit, b + W beta
         void *wqkv_ln, *wfc1_ln;
         float *b_qkv_ln, *b_fc1_ln;
+        void *wproj, *wfc2;
+        const float *bproj, *bfc2, *g1, *g2;     // g1, g2: LayerScale gamma
     };
     std::vector<Blk> blk;
     const float *norm_g = nullptr, *norm_b = nullptr, *pos_embed = nullptr, *cls_token = nullptr, *patch_bias = nullptr;
@@ -154,9 +152,6 @@ struct moge_engine {
     std::vector<std::unique_ptr<Plan>> plans;      // LRU order (most recently used last), at most kMaxPlans
     Plan* last_plan = nullptr;
     std::vector<void*> temps;         // load-time scratch (fp32 folds), freed at the end of finalize
-    bool use_graphs = true;
-    bool neck_fold = false;       // last neck level folded through the heads (EPI_NECKOUT); decided at finalize
-    bool ln_fold = true;          // LayerNorm folded into qkv / fc1 (SURVEY K4/K7); MOGE_B200_LNFOLD=0: separate layernorm kernel
     cudaStream_t own_stream = nullptr;
     cudaEvent_t ev_in = nullptr, ev_out = nullptr;
 
@@ -258,8 +253,10 @@ static int pack_conv3(moge_engine* e, const std::string& wkey, int Cout, int Cin
     return sum_bias(e, b, b_in, Cout, &cw->bias, st);
 }
 
+// waux: the [8, 32] map from the neck's last-level map to the heads' output components (points xyz | normal xyz | mask logit |
+// pad).  A head writes its [ncomp, 32] rows (output block o last-level input block) at `waux`; the neck reads all 8 rows.
 static int pack_stack(moge_engine* e, const std::string& name, const moge_stack_config_t& sc, bool is_neck, StackW* sw,
-                      cudaStream_t st, const float* waux_all = nullptr) {
+                      cudaStream_t st, float* waux) {
     const int L = sc.num_levels;
     sw->res.assign(L, {});
     sw->convT.assign(L, ConvW());
@@ -316,10 +313,10 @@ static int pack_stack(moge_engine* e, const std::string& name, const moge_stack_
         if (!fold_head_out) {
             if (is_neck) {
                 if (sc.dim_in[l + 1] != 2) return set_error("neck: dim_in[%d] must be 2 (UV planes)", l + 1);
-                if (waux_all != nullptr && l + 1 == L - 1) {
+                if (l + 1 == L - 1) {
                     // Last neck level folded through the heads (EPI_NECKOUT).  The level-(L-1) neck map m = conv3x3(up2(x)) + b + Wuv uv
                     // is consumed ONLY by the heads' last-level input blocks and, with no nonlinearity in between, by their output
-                    // blocks: head k-th component += waux_all[k, :] m.  Push waux_all through the (linear) conv: a 3x3 conv with
+                    // blocks: head k-th component += waux[k, :] m.  Push waux through the (linear) conv: a 3x3 conv with
                     // 4 phases x 8 components on the low-resolution grid; the 32-channel map at the 16x grid is never materialised.
                     const int Cn = C[l + 1], K9 = conv_cin * 9;
                     const RawWeight *wc, *wi;
@@ -333,22 +330,22 @@ static int pack_stack(moge_engine* e, const std::string& name, const moge_stack_
                     MG_TRY(launch_up2_expand(wc->p, wexp, Cn, conv_cin, st));                    // rows (phase, channel)
                     MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wfold), static_cast<size_t>(32) * K9 * 4));
                     for (int ph = 0; ph < 4; ++ph)
-                        MG_TRY(launch_sgemm(waux_all, Cn, wexp + static_cast<size_t>(ph) * Cn * K9, K9, wfold + static_cast<size_t>(ph) * 8 * K9, K9, 8, K9, Cn, 0, st));
+                        MG_TRY(launch_sgemm(waux, Cn, wexp + static_cast<size_t>(ph) * Cn * K9, K9, wfold + static_cast<size_t>(ph) * 8 * K9, K9, 8, K9, Cn, 0, st));
                     ConvW& no = sw->neckout;
                     no.N = 32; no.cin = conv_cin; no.taps = 9; no.Ktot = K9;
                     MG_TRY(e->alloc(&no.w, static_cast<size_t>(32) * K9 * 2));
                     MG_TRY(launch_pack_conv(wfold, no.w, e->bf16, 32, conv_cin, 9, K9, 0, st));
                     MG_TRY(sum_bias(e, bc, bi, Cn, &bsum, st));
                     MG_TRY(e->alloc(reinterpret_cast<void**>(&no.bias), 8 * 4));
-                    MG_TRY(launch_sgemm(waux_all, Cn, bsum, 1, no.bias, 1, 8, 1, Cn, 0, st));
+                    MG_TRY(launch_sgemm(waux, Cn, bsum, 1, no.bias, 1, 8, 1, Cn, 0, st));
                     MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wuv), 2 * Cn * 4));
                     vec_combine_kernel<<<(Cn + 255) / 256, 256, 0, st>>>(wuv, wi->p, 2, nullptr, Cn);
                     vec_combine_kernel<<<(Cn + 255) / 256, 256, 0, st>>>(wuv + Cn, wi->p + 1, 2, nullptr, Cn);
                     CUDA_TRY(cudaGetLastError());
                     MG_TRY(e->alloc(reinterpret_cast<void**>(&no.wu), 8 * 4));
                     MG_TRY(e->alloc(reinterpret_cast<void**>(&no.wv), 8 * 4));
-                    MG_TRY(launch_sgemm(waux_all, Cn, wuv, 1, no.wu, 1, 8, 1, Cn, 0, st));
-                    MG_TRY(launch_sgemm(waux_all, Cn, wuv + Cn, 1, no.wv, 1, 8, 1, Cn, 0, st));
+                    MG_TRY(launch_sgemm(waux, Cn, wuv, 1, no.wu, 1, 8, 1, Cn, 0, st));
+                    MG_TRY(launch_sgemm(waux, Cn, wuv + Cn, 1, no.wv, 1, 8, 1, Cn, 0, st));
                     continue;
                 }
                 MG_TRY(pack_conv3(e, rs + ".1", C[l + 1], conv_cin, in_key, 0, true, &sw->post[l], st, sc.resamplers[l] == MOGE_RESAMPLE_BILINEAR));
@@ -385,9 +382,7 @@ static int pack_stack(moge_engine* e, const std::string& name, const moge_stack_
             ho.N = 16; ho.cin = conv_cin; ho.taps = 9; ho.Ktot = K9;
             MG_TRY(e->alloc(&ho.w, static_cast<size_t>(16) * K9 * 2));
             MG_TRY(launch_pack_conv(wexp, ho.w, e->bf16, 16, conv_cin, 9, K9, 0, st));
-            MG_TRY(e->alloc(reinterpret_cast<void**>(&sw->waux), 3 * 32 * 4));
-            CUDA_TRY(cudaMemsetAsync(sw->waux, 0, 3 * 32 * 4, st));
-            MG_TRY(launch_sgemm(wo->p, Cl, w4->p, 32, sw->waux, 32, nc, 32, Cl, 0, st));       // [nc, 32]
+            MG_TRY(launch_sgemm(wo->p, Cl, w4->p, 32, waux, 32, nc, 32, Cl, 0, st));            // [nc, 32]
             MG_TRY(sum_bias(e, bc, b4, Cl, &bsum, st));
             MG_TRY(e->alloc(reinterpret_cast<void**>(&bfold), 16 * 4));
             CUDA_TRY(cudaMemsetAsync(bfold, 0, 16 * 4, st));
@@ -415,34 +410,28 @@ static int finalize_encoder(moge_engine* e, cudaStream_t st) {
     for (int i = 0; i < c.depth; ++i) {
         const std::string p = bb + "blocks." + std::to_string(i) + ".";
         moge_engine::Blk& b = e->blk[i];
-        b.wqkv = nullptr; b.wfc1 = nullptr;
-        if (!e->ln_fold) {       // (with the LayerNorm fold only the folded copies below are ever read)
-            MG_TRY(pack_linear(e, p + "attn.qkv.weight", 3 * D, D, D, &b.wqkv, st));
-            MG_TRY(pack_linear(e, p + "mlp.fc1.weight", 4 * D, D, D, &b.wfc1, st));
-        }
         MG_TRY(pack_linear(e, p + "attn.proj.weight", D, D, D, &b.wproj, st));
         MG_TRY(pack_linear(e, p + "mlp.fc2.weight", D, 4 * D, 4 * D, &b.wfc2, st));
-        MG_TRY(vec(e, p + "attn.qkv.bias", 3 * D, &b.bqkv));
+        const float *bqkv, *bfc1, *ln1g, *ln1b, *ln2g, *ln2b;
+        MG_TRY(vec(e, p + "attn.qkv.bias", 3 * D, &bqkv));
         MG_TRY(vec(e, p + "attn.proj.bias", D, &b.bproj));
-        MG_TRY(vec(e, p + "mlp.fc1.bias", 4 * D, &b.bfc1));
+        MG_TRY(vec(e, p + "mlp.fc1.bias", 4 * D, &bfc1));
         MG_TRY(vec(e, p + "mlp.fc2.bias", D, &b.bfc2));
         MG_TRY(vec(e, p + "ls1.gamma", D, &b.g1));
         MG_TRY(vec(e, p + "ls2.gamma", D, &b.g2));
-        MG_TRY(vec(e, p + "norm1.weight", D, &b.ln1g));
-        MG_TRY(vec(e, p + "norm1.bias", D, &b.ln1b));
-        MG_TRY(vec(e, p + "norm2.weight", D, &b.ln2g));
-        MG_TRY(vec(e, p + "norm2.bias", D, &b.ln2b));
-        if (e->ln_fold) {
-            const RawWeight *wq, *wf;
-            MG_TRY(get_raw(e, p + "attn.qkv.weight", &wq, {}));
-            MG_TRY(get_raw(e, p + "mlp.fc1.weight", &wf, {}));
-            MG_TRY(e->alloc(&b.wqkv_ln, static_cast<size_t>(3 * D) * D * 2));
-            MG_TRY(e->alloc(&b.wfc1_ln, static_cast<size_t>(4 * D) * D * 2));
-            MG_TRY(e->alloc(reinterpret_cast<void**>(&b.b_qkv_ln), static_cast<size_t>(3 * D) * 4));
-            MG_TRY(e->alloc(reinterpret_cast<void**>(&b.b_fc1_ln), static_cast<size_t>(4 * D) * 4));
-            MG_TRY(launch_ln_fold(wq->p, b.ln1g, b.ln1b, b.bqkv, 3 * D, D, D, b.wqkv_ln, b.b_qkv_ln, e->bf16, st));
-            MG_TRY(launch_ln_fold(wf->p, b.ln2g, b.ln2b, b.bfc1, 4 * D, D, D, b.wfc1_ln, b.b_fc1_ln, e->bf16, st));
-        }
+        MG_TRY(vec(e, p + "norm1.weight", D, &ln1g));
+        MG_TRY(vec(e, p + "norm1.bias", D, &ln1b));
+        MG_TRY(vec(e, p + "norm2.weight", D, &ln2g));
+        MG_TRY(vec(e, p + "norm2.bias", D, &ln2b));
+        const RawWeight *wq, *wf;
+        MG_TRY(get_raw(e, p + "attn.qkv.weight", &wq, {}));
+        MG_TRY(get_raw(e, p + "mlp.fc1.weight", &wf, {}));
+        MG_TRY(e->alloc(&b.wqkv_ln, static_cast<size_t>(3 * D) * D * 2));
+        MG_TRY(e->alloc(&b.wfc1_ln, static_cast<size_t>(4 * D) * D * 2));
+        MG_TRY(e->alloc(reinterpret_cast<void**>(&b.b_qkv_ln), static_cast<size_t>(3 * D) * 4));
+        MG_TRY(e->alloc(reinterpret_cast<void**>(&b.b_fc1_ln), static_cast<size_t>(4 * D) * 4));
+        MG_TRY(launch_ln_fold(wq->p, ln1g, ln1b, bqkv, 3 * D, D, D, b.wqkv_ln, b.b_qkv_ln, e->bf16, st));
+        MG_TRY(launch_ln_fold(wf->p, ln2g, ln2b, bfc1, 4 * D, D, D, b.wfc1_ln, b.b_fc1_ln, e->bf16, st));
     }
     return 0;
 }
@@ -484,30 +473,14 @@ static int finalize_v2_decoder(moge_engine* e, cudaStream_t st) {
         vec_combine_kernel<<<(C0 + 255) / 256, 256, 0, st>>>(f.wv, w0->p + Do + 1, Do + 2, nullptr, C0);
         CUDA_TRY(cudaGetLastError());
     }
+    // the heads' last levels first: they give the map through which the neck's last level is folded (EPI_NECKOUT)
+    float* waux;
+    MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&waux), 8 * 32 * 4));
+    CUDA_TRY(cudaMemsetAsync(waux, 0, 8 * 32 * 4, st));
+    const int row_of[3] = {0, 3, 6};          // points xyz | normal xyz | mask logit | pad
     for (int i = 0; i < 3; ++i)
-        if (head_cfg(e, i)->present) MG_TRY(pack_stack(e, head_name(i), *head_cfg(e, i), false, &e->heads[i], st));
-    // neck last: its final level can be folded through the heads' last-level input/output blocks (EPI_NECKOUT) when that level
-    // is a bilinear resampler + conv with no residual blocks and 32 channels (every MoGe-2 config); MOGE_B200_NECKFOLD=0 keeps
-    // the 32-channel map at the 16x grid and the per-head mat-vec instead
-    {
-        const int L = c.neck.num_levels;
-        bool any_head = false;
-        for (int i = 0; i < 3; ++i) any_head |= head_cfg(e, i)->present != 0;
-        const char* env = getenv("MOGE_B200_NECKFOLD");
-        e->neck_fold = !(env && env[0] == '0') && any_head && L >= 2 && c.neck.resamplers[L - 2] == MOGE_RESAMPLE_BILINEAR &&
-                       c.neck.num_res_blocks[L - 1] == 0 && c.neck.dim_res_blocks[L - 1] == 32 && c.neck.dim_res_blocks[L - 2] % 64 == 0;
-        float* waux_all = nullptr;
-        if (e->neck_fold) {
-            MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&waux_all), 8 * 32 * 4));
-            CUDA_TRY(cudaMemsetAsync(waux_all, 0, 8 * 32 * 4, st));
-            const int row_of[3] = {0, 3, 6};          // points xyz | normal xyz | mask logit | pad
-            for (int i = 0; i < 3; ++i)
-                if (head_cfg(e, i)->present)
-                    CUDA_TRY(cudaMemcpyAsync(waux_all + row_of[i] * 32, e->heads[i].waux, static_cast<size_t>(e->heads[i].ncomp) * 32 * 4,
-                                             cudaMemcpyDeviceToDevice, st));
-        }
-        MG_TRY(pack_stack(e, "neck", c.neck, true, &e->neck, st, waux_all));
-    }
+        if (head_cfg(e, i)->present) MG_TRY(pack_stack(e, head_name(i), *head_cfg(e, i), false, &e->heads[i], st, waux + row_of[i] * 32));
+    MG_TRY(pack_stack(e, "neck", c.neck, true, &e->neck, st, waux));
     for (int l = 0; l < c.scale_head_layers; ++l) {
         const float *w, *b;
         MG_TRY(vec(e, "scale_head." + std::to_string(2 * l) + ".weight", c.scale_head_dims[l] * c.scale_head_dims[l + 1], &w));
@@ -670,14 +643,14 @@ static size_t map_bytes(const Level& g, int B, int C) { return static_cast<size_
 // conv-type launch on padded NHWC maps. src/aux/skip/out buffers live in the workspace.
 static int add_conv(moge_engine* e, Plan* pl, const ConvW& cw, const void* src, const void* aux, const Level& gs, int B,
                     int epi, void* out_raw, void* out_relu, const void* skip, const Level& go, int out_ch, bool shuffle,
-                    bool uv, float su, float sv, const std::string& name, int ncomp = 0, const float* waux = nullptr, void* out2 = nullptr,
-                    int accum = 0) {
+                    bool uv, float su, float sv, const std::string& name, int ncomp = 0, void* out2 = nullptr) {
     GemmLaunch g;
-    MG_TRY(gemm_conv(&g, e->bf16, cw, src, aux, gs, B, epi, out_raw, out_relu, skip, go, out_ch, shuffle, uv, su, sv, ncomp, waux, out2, accum));
+    MG_TRY(gemm_conv(&g, e->bf16, cw, src, aux, gs, B, epi, out_raw, out_relu, skip, go, out_ch, shuffle, uv, su, sv, ncomp, out2));
     const double px = static_cast<double>(B) * gs.H * gs.W;
     const double flops = 2.0 * px * cw.N * cw.Ktot;
     double bytes = px * cw.cin * 2 + px * cw.caux * 2 + static_cast<double>(cw.N) * cw.Ktot * 2;
-    if (epi == EPI_HEADOUT) bytes += 4 * px * (accum ? (ncomp == 1 ? 4 : 16) : 32 * 2) + 4 * px * (ncomp == 1 ? 4 : 16);     // 4 output pixels per low-res pixel
+    // 4 output pixels per low-res pixel, each read (the neck's part) and written
+    if (epi == EPI_HEADOUT) bytes += 2 * (4 * px * (ncomp == 1 ? 4 : 16));
     else if (epi == EPI_NECKOUT) bytes += 4 * px * ((out_raw ? 16 : 0) + (out_relu ? 16 : 0) + (out2 ? 4 : 0));
     else bytes += px * cw.N * 2 * ((out_raw ? 1 : 0) + (out_relu ? 1 : 0)) + (skip ? px * cw.N * 2 : 0);
     const int sms = e->num_sms;
@@ -736,15 +709,14 @@ static int plan_stack(moge_engine* e, Plan* pl, const char* sname, const moge_st
             // bilinear x2 + 3x3 conv run as ONE low-resolution conv with 4 output phases (weights expanded at load time)
             const bool need_relu_b = sc.num_res_blocks[l + 1] > 0;
             if (tail) {
-                const bool acc = e->neck_fold;
-                MG_TRY(add_conv(e, pl, sw.headout, x_raw, nullptr, g, B, EPI_HEADOUT, lowres_out, nullptr, acc ? nullptr : neck_out[l + 1], gn, 0, false,
-                                false, 0, 0, nm("conv3x3up2.headout", l + 1), sw.ncomp, acc ? nullptr : sw.waux, nullptr, acc ? 1 : 0));
+                MG_TRY(add_conv(e, pl, sw.headout, x_raw, nullptr, g, B, EPI_HEADOUT, lowres_out, nullptr, nullptr, gn, 0, false,
+                                false, 0, 0, nm("conv3x3up2.headout", l + 1), sw.ncomp));
                 break;
             }
-            if (is_neck && e->neck_fold && l + 1 == L - 1) {
+            if (is_neck && l + 1 == L - 1) {
                 // the neck's last level goes straight into the heads' output maps (folded through their last input/output blocks)
                 MG_TRY(add_conv(e, pl, sw.neckout, x_raw, nullptr, g, B, EPI_NECKOUT, neck_lowres[0], neck_lowres[1], nullptr, gn, 0, false, true, su, sv,
-                                nm("conv3x3up2.neckout", l + 1), 0, nullptr, neck_lowres[2]));
+                                nm("conv3x3up2.neckout", l + 1), 0, neck_lowres[2]));
                 break;
             }
             MG_TRY(add_conv(e, pl, sw.post[l], x_raw, nullptr, g, B, EPI_DEC, sb.x_raw[l + 1], need_relu_b ? sb.x_relu[l + 1] : nullptr, nullptr, gn,
@@ -888,7 +860,8 @@ static void alloc_v2_decoder(moge_engine* e, Plan* pl, WsAlloc& ws, V2Bufs* v) {
     const int L = c.neck.num_levels;
     auto alloc_stack = [&](const moge_stack_config_t& sc, StackBufs& sb) {
         sb.x_raw.assign(L, nullptr); sb.x_relu.assign(L, nullptr); sb.y_relu.assign(L, nullptr); sb.t_up.assign(L, nullptr);
-        for (int l = 0; l < L; ++l) {
+        // no level-(L-1) map: the last levels are folded into EPI_NECKOUT / EPI_HEADOUT, which write the fp32 head outputs
+        for (int l = 0; l < L - 1; ++l) {
             const int Cl = sc.dim_res_blocks[l];
             // t_up[l]: resampler output feeding the 3x3 conv of level l (channels: convT -> C[l], bilinear -> C[l-1]);
             // doubles as the second raw map of the residual ping-pong.
@@ -900,8 +873,6 @@ static void alloc_v2_decoder(moge_engine* e, Plan* pl, WsAlloc& ws, V2Bufs* v) {
                 sz = std::max(sz, map_bytes(lg, g.B, Cl));
                 szt = std::max(szt, map_bytes(lg, g.B, ct));
             }
-            const bool folded_last = e->neck_fold && l == L - 1;      // with the neck fold no 16x-grid feature map exists at all
-            if (folded_last) continue;
             sb.x_raw[l] = ws.take(sz);
             if (sc.num_res_blocks[l] > 0) {
                 sb.x_relu[l] = ws.take(sz);
@@ -912,9 +883,7 @@ static void alloc_v2_decoder(moge_engine* e, Plan* pl, WsAlloc& ws, V2Bufs* v) {
     };
     alloc_stack(c.neck, v->nb);
     // neck outputs must survive all heads: the neck's final x per level is whichever ping-pong map holds it (kept).
-    bool any_head = false;
-    for (int i = 0; i < 3; ++i) any_head |= head_cfg(e, i)->present != 0;
-    if (any_head) alloc_stack(*head_cfg(e, c.points_head.present ? 0 : c.normal_head.present ? 1 : 2), v->hb);
+    alloc_stack(*head_cfg(e, c.points_head.present ? 0 : c.normal_head.present ? 1 : 2), v->hb);     // validate_cfg: at least one head
     // low-resolution fp32 head outputs, PER GROUP (read by the phase-2 output kernels after every group's decoder has run)
     v->pts_lr.assign(G, nullptr); v->nrm_lr.assign(G, nullptr); v->msk_lr.assign(G, nullptr);
     for (int gi = 0; gi < G; ++gi) {
@@ -946,7 +915,7 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     // ---- encoder buffers (all groups packed back to back)
     uint8_t* patches = static_cast<uint8_t*>(ws.take(static_cast<size_t>(TT) * 592 * 2));
     float* x = static_cast<float*>(ws.take(static_cast<size_t>(M) * D * 4));
-    uint8_t* ln = static_cast<uint8_t*>(ws.take(static_cast<size_t>(M) * D * 2));          // LN output, or (LN fold) the rounded residual rows x16
+    uint8_t* ln = static_cast<uint8_t*>(ws.take(static_cast<size_t>(M) * D * 2));          // the rounded residual rows x16 (LayerNorm fold)
     float2* stats = static_cast<float2*>(ws.take(static_cast<size_t>(M) * kStatsLd * 8));
     float* rstd = static_cast<float*>(ws.take(static_cast<size_t>(M) * 4));
     void* qkv = ws.take(static_cast<size_t>(M) * 3 * D * 2);
@@ -971,7 +940,6 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     if (ws.off > pl->ws_bytes) return set_error("workspace too small: need %zu bytes, got %zu", ws.off, pl->ws_bytes);
 
     Plan* P = pl;
-    const bool fold = e->ln_fold;
     const int sms = e->num_sms;
     auto gname = [&](const char* base, int gi) { return G == 1 ? std::string(base) : std::string(base) + ".g" + std::to_string(gi); };
     // ---- per group: K1 resize + normalise + patchify (phase 0: reads the caller's image), K2/K3 patch embed + pos embed, cls rows
@@ -1010,14 +978,12 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         LnIO prod; prod.x16 = ln_g; prod.stats_out = stats_g; prod.parts_out = &parts_x;
         const Level grid = level_geom(h, w, 0);
         MG_TRY(add_linear(e, pl, patches_g, B * T, 592, e->w_patch, D, EPI_PATCH, x_g, nullptr, g.pos_table, D, gname("gemm.patch_embed", gi),
-                          fold ? &prod : nullptr, &grid));
+                          &prod, &grid));
         pl->ops.add([=](cudaStream_t st) { return launch_init_cls(x_g, P->cls_row, B, N, D, st); }, gname("init_cls", gi));
-        if (fold) {
-            const int parts0 = parts_x;
-            pl->ops.add([=](cudaStream_t st) {
-                return launch_ln_prepare(x_g, B, static_cast<long>(N) * D, D, ln_g, static_cast<long>(N) * D, stats_g, static_cast<long>(N) * kStatsLd, parts0, bf16, st);
-            }, gname("ln_prepare.cls", gi));
-        }
+        const int parts0 = parts_x;
+        pl->ops.add([=](cudaStream_t st) {
+            return launch_ln_prepare(x_g, B, static_cast<long>(N) * D, D, ln_g, static_cast<long>(N) * D, stats_g, static_cast<long>(N) * kStatsLd, parts0, bf16, st);
+        }, gname("ln_prepare.cls", gi));
     }
     const int Mi = static_cast<int>(M);
     LnIO prod; prod.x16 = ln; prod.stats_out = stats; prod.parts_out = &parts_x;
@@ -1048,15 +1014,9 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     int tap_idx = 0;
     for (int i = 0; i < c.depth; ++i) {
         const moge_engine::Blk& b = e->blk[i];
-        const double ln_bytes = static_cast<double>(M) * D * 6;
-        if (fold) {
-            if (i == 0) add_rstd(parts_x);
-            LnIO cons; cons.ln_rstd = rstd;
-            MG_TRY(add_linear(e, pl, ln, Mi, D, b.wqkv_ln, 3 * D, EPI_STORE16, qkv, b.b_qkv_ln, nullptr, 3 * D, "gemm.qkv", &cons));
-        } else {
-            pl->ops.add([=](cudaStream_t st) { return launch_layernorm(x, b.ln1g, b.ln1b, ln, Mi, D, D, 0, 0, 1, nullptr, bf16, st); }, "layernorm", 0, ln_bytes);
-            MG_TRY(add_linear(e, pl, ln, Mi, D, b.wqkv, 3 * D, EPI_STORE16, qkv, b.bqkv, nullptr, 3 * D, "gemm.qkv"));
-        }
+        if (i == 0) add_rstd(parts_x);
+        LnIO cons; cons.ln_rstd = rstd;
+        MG_TRY(add_linear(e, pl, ln, Mi, D, b.wqkv_ln, 3 * D, EPI_STORE16, qkv, b.b_qkv_ln, nullptr, 3 * D, "gemm.qkv", &cons));
         {
             CUtensorMap mq;
             MG_TRY(make_map_2d(&mq, qkv, 3 * static_cast<uint64_t>(D), M, 3 * static_cast<uint64_t>(D), 128));
@@ -1064,19 +1024,11 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
             pl->ops.add([=](cudaStream_t st) { return launch_attention(mq, att, items_dev, ranges_dev, att_ctas, D, heads, bf16, st); }, "attention",
                         att_flops, static_cast<double>(M) * D * 8);
         }
-        if (fold) {
-            MG_TRY(add_linear(e, pl, att, Mi, D, b.wproj, D, EPI_RESID, x, b.bproj, b.g1, D, "gemm.proj", &prod));
-            add_rstd(parts_x);
-            LnIO cons; cons.ln_rstd = rstd;
-            MG_TRY(add_linear(e, pl, ln, Mi, D, b.wfc1_ln, 4 * D, EPI_GELU16, hid, b.b_fc1_ln, nullptr, 4 * D, "gemm.fc1", &cons));
-            MG_TRY(add_linear(e, pl, hid, Mi, 4 * D, b.wfc2, D, EPI_RESID, x, b.bfc2, b.g2, D, "gemm.fc2", (i + 1 < c.depth) ? &prod : nullptr));
-            if (i + 1 < c.depth) add_rstd(parts_x);
-        } else {
-            MG_TRY(add_linear(e, pl, att, Mi, D, b.wproj, D, EPI_RESID, x, b.bproj, b.g1, D, "gemm.proj"));
-            pl->ops.add([=](cudaStream_t st) { return launch_layernorm(x, b.ln2g, b.ln2b, ln, Mi, D, D, 0, 0, 1, nullptr, bf16, st); }, "layernorm", 0, ln_bytes);
-            MG_TRY(add_linear(e, pl, ln, Mi, D, b.wfc1, 4 * D, EPI_GELU16, hid, b.bfc1, nullptr, 4 * D, "gemm.fc1"));
-            MG_TRY(add_linear(e, pl, hid, Mi, 4 * D, b.wfc2, D, EPI_RESID, x, b.bfc2, b.g2, D, "gemm.fc2"));
-        }
+        MG_TRY(add_linear(e, pl, att, Mi, D, b.wproj, D, EPI_RESID, x, b.bproj, b.g1, D, "gemm.proj", &prod));
+        add_rstd(parts_x);
+        MG_TRY(add_linear(e, pl, ln, Mi, D, b.wfc1_ln, 4 * D, EPI_GELU16, hid, b.b_fc1_ln, nullptr, 4 * D, "gemm.fc1", &cons));
+        MG_TRY(add_linear(e, pl, hid, Mi, 4 * D, b.wfc2, D, EPI_RESID, x, b.bfc2, b.g2, D, "gemm.fc2", (i + 1 < c.depth) ? &prod : nullptr));
+        if (i + 1 < c.depth) add_rstd(parts_x);
         if (tap_idx < c.num_taps && c.taps[tap_idx] == i) {
             const int j = tap_idx++;
             const bool lasttap = (j == c.num_taps - 1);
@@ -1224,6 +1176,15 @@ static int validate_cfg(const moge_config_t& c) {
         }
         if (!first) first = s;
     }
+    // the neck's last level is folded through the heads' last-level input + output blocks (EPI_NECKOUT), which needs this shape
+    const moge_stack_config_t& n = c.neck;
+    const int L = n.num_levels;
+    if (!first) return set_error("a model without points, normal and mask heads is unsupported (no released config has one)");
+    if (n.resamplers[L - 2] != MOGE_RESAMPLE_BILINEAR)
+        return set_error("neck: resampler %d before the last level unsupported (bilinear only; no released config uses another)", n.resamplers[L - 2]);
+    if (n.num_res_blocks[L - 1] != 0)
+        return set_error("neck: %d residual blocks at the last level unsupported (no released config uses them)", n.num_res_blocks[L - 1]);
+    if (n.dim_res_blocks[L - 1] != 32) return set_error("neck: last-level width %d unsupported (32 only)", n.dim_res_blocks[L - 1]);
     return 0;
 }
 
@@ -1269,10 +1230,6 @@ static int create_engine(const moge_config_t* cfg, int device, moge_engine_t** o
     if (prop.major != 9 || prop.minor != 0) return set_error("device %d is sm_%d%d; libmoge_b200 contains sm_90a code only", device, prop.major, prop.minor);
     moge_engine* e = new moge_engine();
     e->cfg = *cfg; e->device = device; e->num_sms = prop.multiProcessorCount; e->bf16 = cfg->compute_dtype == MOGE_BF16;
-    const char* env = getenv("MOGE_B200_GRAPHS");
-    e->use_graphs = !(env && env[0] == '0');
-    const char* env3 = getenv("MOGE_B200_LNFOLD");
-    e->ln_fold = !(env3 != nullptr && env3[0] == '0');
     if (cudaStreamCreateWithFlags(&e->own_stream, cudaStreamNonBlocking) != cudaSuccess ||
         cudaEventCreateWithFlags(&e->ev_in, cudaEventDisableTiming) != cudaSuccess ||
         cudaEventCreateWithFlags(&e->ev_out, cudaEventDisableTiming) != cudaSuccess) {
@@ -1401,7 +1358,7 @@ static int forward_impl(moge_engine_t* e, const moge_group_t* groups, int n, voi
     e->last_plan = pl;
     // ---- graph replay of the workspace-only launches (small batches only: at large batch the GPU is the bottleneck and the CPU
     //      runs ahead anyway).  The first run of a plan is eager (sets kernel attributes, warms caches).
-    const bool want_graph = e->use_graphs && tokens <= 4 * 3600;
+    const bool want_graph = tokens <= 4 * 3600;
     struct PdlScope {          // programmatic dependent launch for the small calls only (host_api.h)
         bool prev;
         explicit PdlScope(bool on) : prev(pdl_scope()) { pdl_scope() = on; }

@@ -37,7 +37,7 @@ int gemm_linear(GemmLaunch* g, bool bf16, const void* A, int M, int K, const voi
 
 int gemm_conv(GemmLaunch* g, bool bf16, const ConvW& cw, const void* src, const void* aux, const Level& gs, int B, int epi,
               void* out_raw, void* out_relu, const void* skip, const Level& go, int out_ch, bool shuffle, bool uv, float su, float sv,
-              int ncomp, const float* waux, void* out2, int accum) {
+              int ncomp, void* out2) {
     GemmParams p{};
     p.N = cw.N; p.ntaps = cw.taps; p.kb_main = cw.cin / 64; p.kb_aux = cw.caux / 64;
     p.B = B; p.H = gs.H; p.W = gs.W;
@@ -48,7 +48,7 @@ int gemm_conv(GemmLaunch* g, bool bf16, const ConvW& cw, const void* src, const 
     p.skip = skip; p.ldo = out_ch;
     p.Ho = go.H; p.Wo = go.W; p.Hop = go.Hp; p.Wop = go.Wp;
     p.shuffle = shuffle ? 1 : 0; p.su = su; p.sv = sv;
-    if (epi == EPI_HEADOUT) { p.vec1 = waux; p.ncomp = ncomp; p.accum = accum; }
+    if (epi == EPI_HEADOUT) p.ncomp = ncomp;
     // tile width: fixed for the folded head / neck outputs, else the widest that divides N
     int bn = (epi == EPI_HEADOUT) ? 16 : (epi == EPI_NECKOUT) ? 32 : (cw.N % 128 == 0) ? 128 : (cw.N % 64 == 0) ? 64 : (cw.N % 32 == 0) ? 32 : 0;
     if (!bn) return set_error("conv: N=%d has no tile width", cw.N);

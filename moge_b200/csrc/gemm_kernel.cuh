@@ -32,7 +32,7 @@ enum : int {
     EPI_PATCH = 3,     // x32[b*(T+1)+1+t, col] = acc + table[t, col]                (patch embed + pos embed)
     EPI_DEC = 4,       // padded-NHWC decoder store: acc + bias (+ UV rank-2) (+ skip) -> raw and/or ReLU copies
     EPI_HEADOUT = 5,   // BN=16: (bilinear x2 + 3x3 conv + output 1x1) folded into one low-res 3x3 conv with 4 output phases,
-                       //        + folded 1x1 of the high-res neck map -> fp32 maps at the high resolution
+                       //        added to the neck's part (EPI_NECKOUT) in the fp32 maps at the high resolution
     EPI_NECKOUT = 6,   // BN=32: the neck's last level (bilinear x2 + 3x3 conv + UV 1x1) folded THROUGH the heads' last-level
                        //        input + output blocks: 4 phases x 8 components (points xyz, normal xyz, mask logit, pad) written
                        //        straight into the heads' fp32 output maps; the heads' EPI_HEADOUT launches then accumulate
@@ -56,14 +56,14 @@ struct GemmParams {
     int B, H, W;           // A-source unpadded size (AMODE_ROWS + EPI_DEC: the h x w token grid)
     int tiles_x, tiles_y;
     // epilogue operands
-    void* out0;            // EPI_STORE16/GELU16: T* ; EPI_RESID/PATCH: float* ; EPI_DEC: raw T* (or null) ; HEADOUT: float*
+    void* out0;            // EPI_STORE16/GELU16: T* ; EPI_RESID/PATCH: float* ; EPI_DEC: raw T* (or null) ;
+                           // HEADOUT: float* / float4*, added to in place (NECKOUT writes it first); NECKOUT: points float4* (or null)
     void* out1;            // EPI_DEC: ReLU copy T* (or null); NECKOUT: normal map float4* (or null)
     void* out2;            // NECKOUT: mask-logit map float* (or null)
-    int accum;             // HEADOUT: 1 = add to the values already in out0 (written by the NECKOUT launch)
     const float* bias;     // [N] (EPI_DEC shuffle: [C_out]); HEADOUT: [16]
-    const float* vec1;     // EPI_RESID: gamma[N]; EPI_PATCH: table[T, N]; EPI_DEC: wu[C] (or null); HEADOUT: waux[ncomp,32] (or null)
-    const float* vec2;     // EPI_DEC: wv[C]
-    const void* skip;      // EPI_DEC: residual input, same geometry as out ; HEADOUT: neck level-4 map (T*, 32 ch, padded)
+    const float* vec1;     // EPI_RESID: gamma[N]; EPI_PATCH: table[T, N]; EPI_DEC: wu[C] (or null); NECKOUT: wu[8]
+    const float* vec2;     // EPI_DEC: wv[C]; NECKOUT: wv[8]
+    const void* skip;      // EPI_DEC: residual input, same geometry as out
     int ldo;               // row pitch of out (elements): ROWS epilogues: N total; DEC: channels of the out buffer
     int T;                 // EPI_PATCH / ROWS+EPI_DEC: tokens per image
     int Ho, Wo, Hop, Wop;  // EPI_DEC/HEADOUT: output pixel grid and its padded allocation
@@ -329,9 +329,8 @@ __device__ __forceinline__ void epilogue_dec16(const GemmParams& p, int mt, int 
 
 
 // EPI_HEADOUT epilogue: lane = low-resolution pixel, 16 B (or 4 B) per lane, consecutive lanes = consecutive pixels of a tile row.
-template <int BN, bool BF16>
+template <int BN>
 __device__ __forceinline__ void epilogue_headout(const GemmParams& p, int mt, const float4* stg, int quarter, int lane) {
-    using H = H16<BF16>;
     const int row = quarter * 32 + lane;
     const TileOrigin org = tile_origin(p, mt);
     const int b = org.b;
@@ -348,28 +347,10 @@ __device__ __forceinline__ void epilogue_headout(const GemmParams& p, int mt, co
             float o[3];
 #pragma unroll
             for (int k = 0; k < 3; ++k) o[k] = (k < p.ncomp) ? v[ph * p.ncomp + k] + p.bias[k] : 0.f;
-            if (p.vec1 != nullptr) {
-                const uint4* src = reinterpret_cast<const uint4*>(
-                    static_cast<const uint8_t*>(p.skip) + ((static_cast<size_t>(b) * p.Hop + Y + 1) * p.Wop + X + 1) * 64);
-#pragma unroll
-                for (int q = 0; q < 4; ++q) {
-                    const uint4 u = src[q];
-                    const uint32_t w[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const float2 f = H::unpack(w[e]);
-                        const int c = q * 8 + e * 2;
-#pragma unroll
-                        for (int k = 0; k < 3; ++k)
-                            if (k < p.ncomp) o[k] += p.vec1[k * 32 + c] * f.x + p.vec1[k * 32 + c + 1] * f.y;
-                    }
-                }
-            }
             const size_t pix = (static_cast<size_t>(b) * p.Ho + Y) * p.Wo + X;
-            if (p.accum) {       // the neck's folded contribution is already there (EPI_NECKOUT)
-                if (p.ncomp == 1) o[0] += static_cast<const float*>(p.out0)[pix];
-                else { const float4 t = static_cast<const float4*>(p.out0)[pix]; o[0] += t.x; o[1] += t.y; o[2] += t.z; }
-            }
+            // the neck's folded contribution is already there (EPI_NECKOUT)
+            if (p.ncomp == 1) o[0] += static_cast<const float*>(p.out0)[pix];
+            else { const float4 t = static_cast<const float4*>(p.out0)[pix]; o[0] += t.x; o[1] += t.y; o[2] += t.z; }
             if (p.ncomp == 1) static_cast<float*>(p.out0)[pix] = o[0];
             else static_cast<float4*>(p.out0)[pix] = make_float4(o[0], o[1], o[2], 0.f);
         }
@@ -711,7 +692,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
             named_sync(1, 256);
             if (ew < Cfg::kEpiWarps) {
                 if constexpr (EPI == EPI_DEC) epilogue_dec16<BN, Cfg::kColsPerWarp, AMODE, BF16, DF>(p, mt, nt, stg, quarter, lane, col_begin);
-                else if constexpr (EPI == EPI_HEADOUT) epilogue_headout<BN, BF16>(p, mt, stg, quarter, lane);
+                else if constexpr (EPI == EPI_HEADOUT) epilogue_headout<BN>(p, mt, stg, quarter, lane);
                 else if constexpr (EPI == EPI_NECKOUT) epilogue_neckout<BN>(p, mt, stg, quarter, lane);
                 else epilogue_rows<BN, Cfg::kColsPerWarp, EPI, BF16>(p, mt, nt, stg, quarter, lane, col_begin, ln_on, lnr);
             }

@@ -54,8 +54,7 @@ struct DevOnce {
 // correctness is unchanged (the wait returns only when the predecessor grid has completed and flushed).  It matters at batch 1,
 // where a forward is ~245 kernels of a few microseconds each (also inside the captured CUDA graph).  At large batches the kernels
 // are long and early-resident dependents only get in the way, so the engine switches it on per call, for the small
-// (graph-replayed) calls only: `pdl_scope` is thread-local state read by `launch_pdl`.  MOGE_B200_PDL=0 disables it altogether.
-bool pdl_enabled();
+// (graph-replayed) calls only: `pdl_scope` is thread-local state read by `launch_pdl`.
 bool& pdl_scope();
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
@@ -63,7 +62,7 @@ inline cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, siz
     cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = (pdl_enabled() && pdl_scope()) ? 1 : 0;
+    attr[0].val.programmaticStreamSerializationAllowed = pdl_scope() ? 1 : 0;
     cfg.attrs = attr; cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
@@ -105,7 +104,7 @@ int gemm_linear(GemmLaunch* g, bool bf16, const void* A, int M, int K, const voi
 // Picks the main loop from the shape: CONV64 (3x3, C_in = 64), CONVH (3x3, C_in >= 128) or the per-tap GEMM.
 int gemm_conv(GemmLaunch* g, bool bf16, const ConvW& cw, const void* src, const void* aux, const Level& gs, int B, int epi,
               void* out_raw, void* out_relu, const void* skip, const Level& go, int out_ch, bool shuffle, bool uv, float su, float sv,
-              int ncomp = 0, const float* waux = nullptr, void* out2 = nullptr, int accum = 0);
+              int ncomp = 0, void* out2 = nullptr);
 int launch_gemm(const GemmLaunch& g, int num_sms, cudaStream_t st);
 
 // Attention over PACKED token rows (ragged batches): qkv [rows, 3D] (map: box {64, 128}), one work item per (image, head, pair

@@ -3,7 +3,6 @@
 #include "host_api.h"
 #include <stdarg.h>
 #include <stdio.h>
-#include <stdlib.h>
 #include <mutex>
 
 namespace mg {
@@ -20,11 +19,6 @@ const char* last_error() { return g_err; }
 
 bool& pdl_scope() {
     static thread_local bool on = false;
-    return on;
-}
-
-bool pdl_enabled() {
-    static const bool on = [] { const char* v = getenv("MOGE_B200_PDL"); return !(v != nullptr && v[0] == '0'); }();
     return on;
 }
 

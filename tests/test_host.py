@@ -75,6 +75,27 @@ def test_make_config_rejects_unsupported_decoders():
         capi.make_config({**cfg, "encoder": {**cfg["encoder"], "backbone": "dinov2_vitg14"}}, capi.F16)
 
 
+def _with_last_width(cfg, width):
+    stacks = [k for k in ("neck", "points_head", "normal_head", "mask_head") if k in cfg]
+    return {**cfg, **{k: {**cfg[k], "dim_res_blocks": cfg[k]["dim_res_blocks"][:-1] + [width]} for k in stacks}}
+
+
+@pytest.mark.parametrize("change,msg", [
+    (lambda c: {k: v for k, v in c.items() if not k.endswith("_head") or k == "scale_head"}, "without points, normal and mask heads"),
+    (lambda c: {**c, "neck": {**c["neck"], "resamplers": ["conv_transpose"] * 4}}, "bilinear only"),
+    (lambda c: {**c, "neck": {**c["neck"], "num_res_blocks": [0, 2, 2, 2, 1]}}, "residual blocks at the last level"),
+    (lambda c: _with_last_width(c, 64), "last-level width 64"),
+], ids=["no_heads", "neck_convT_last", "neck_res_blocks_last", "last_width_64"])
+def test_create_rejects_configs_the_neck_fold_cannot_cover(change, msg):
+    """The neck's last level always runs folded through the heads (EPI_NECKOUT); a config of another shape fails at create,
+    before the device is looked for."""
+    h = C.c_void_p()
+    c = capi.make_config(change(model_config("vits")), capi.F16)
+    assert capi.lib().moge_engine_create(C.byref(c), 0, C.byref(h)) != 0
+    err = capi.lib().moge_last_error().decode()
+    assert msg in err, err
+
+
 def test_model_plumbing_without_gpu():
     """nn.Module-like surface of the drop-in class (v2.py:59-74,109-120): dtype/device bookkeeping, training-only stubs."""
     from moge.model.v2 import MoGeModel

@@ -3,7 +3,7 @@
 loaded once per process) and the variants are interleaved `--rounds` times to average out clock / thermal drift.
 
     python tools/ab_variants.py base polyA polyB [--rounds 3] [--batch 32] [--size vitl] [--tokens 1369] [--res 518]
-        ("base" = the product library; "env:KEY=VAL" = the product library with an environment switch)  -> per variant: step ms (CUDA events over 5 infer() calls) and per-class ms from the
+        ("base" = the product library)  -> per variant: step ms (CUDA events over 5 infer() calls) and per-class ms from the
         engine's own per-launch profile (gemm / attention / conv / other)
 """
 import argparse
@@ -62,11 +62,7 @@ def main():
         for v in a.variants:
             env = dict(os.environ)
             env.pop("MOGE_B200_LIB", None)
-            if v.startswith("env:"):                       # "env:KEY=VAL[,KEY2=VAL2]": the product library with environment switches
-                for kv in v[4:].split(","):
-                    k, val = kv.split("=", 1)
-                    env[k] = val
-            elif v != "base":
+            if v != "base":
                 env["MOGE_B200_LIB"] = os.path.join(ROOT, "moge_b200", "_lib", f"libmoge_b200_{v}.so")
             try:
                 out = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=240)
