@@ -284,6 +284,38 @@ int moge_metrics_eval(const float* gt_depth, const float* gt_points, const uint8
 int moge_metrics_boundary(const float* gt_depth, const uint8_t* mask, const moge_metric_variant_t* aligned, const float* thresholds,
                           int64_t batch, int H, int W, int64_t* counts, int64_t counts_stride, void* stream);
 
+/* ---- mesh export (moge/scripts/infer.py:124-150: utils3d's depth_map_edge and build_mesh_from_map; Python: moge_b200.mesh).
+ * Maps are (batch, H, W[, C]) contiguous on the device, masks uint8 (nonzero = in), at most 2^30 pixels per image.  Results are
+ * bitwise those of the numpy restatement in oracle/utils3d_mesh.py and do not depend on the other images of the batch.        */
+#define MOGE_MESH_MAX_MAPS 8
+#define MOGE_MESH_MAX_CHANNELS 4
+/* map kinds: fp32 copied; uint8 / 255 in fp32; the pixel-centre UV ((j + 0.5) / W, (i + 0.5) / H) generated (src unused, 2 ch) */
+enum { MOGE_MESH_F32 = 0, MOGE_MESH_U8_UNIT = 1, MOGE_MESH_UV = 2 };
+enum { MOGE_MESH_HWC = 0, MOGE_MESH_CHW = 1 };
+/* one attribute map: a source (batch, H, W, C) or (batch, C, H, W); each value x is written as x * sign[c], then + offset[c] when
+ * offset[c] != 0, each one fp32 rounding; the rows of kept vertices go to dst (total vertices, C) at the image's first row.   */
+typedef struct {
+    const void* src; int kind; int channels; int layout;
+    float sign[MOGE_MESH_MAX_CHANNELS]; float offset[MOGE_MESH_MAX_CHANNELS];
+    float* dst;
+} moge_mesh_map_t;
+/* workspace (256-byte aligned) of moge_mesh_count / moge_mesh_build; one workspace carries the counts from one to the other */
+int moge_mesh_workspace_bytes(int64_t batch, int H, int W, size_t* bytes);
+/* depth_map_edge: diff = max(d) + max(-d) over the kernel_size x kernel_size window (3, 5 or 7; -inf outside the image and,
+ * with mask, off it; NaN propagates), edge = diff > *atol | diff / d > *rtol (a NULL tolerance is not tested).  out (batch, H, W)
+ * uint8 = edge, or keep & !edge when keep is given (the cleaned mask).                                                       */
+int moge_depth_edge(const float* depth, const uint8_t* mask, const uint8_t* keep, int64_t batch, int H, int W, int kernel_size,
+                    const float* atol, const float* rtol, uint8_t* out, void* stream);
+/* count pass: a quad (top-left pixel (i, j)) is kept when its four corners are in the mask (NULL: every quad), a vertex when a
+ * kept quad uses it.  totals (batch, 4) int64 on the device = (vertices, quads, first vertex row, first quad) of each image in
+ * the batch-wide outputs.                                                                                                   */
+int moge_mesh_count(const uint8_t* mask, int64_t batch, int H, int W, int64_t* totals, void* workspace, size_t workspace_bytes, void* stream);
+/* emit pass, after moge_mesh_count on the same mask, totals and workspace: the maps' rows at the kept vertices (row-major order)
+ * and the faces as vertex indices local to each image, int32: quads [(i,j), (i+1,j), (i+1,j+1), (i,j+1)] in row-major order, or
+ * with tri two triangles [a, b, c], [a, c, d] per quad (faces then holds 6 ints per quad).                                   */
+int moge_mesh_build(const uint8_t* mask, int64_t batch, int H, int W, int tri, const moge_mesh_map_t* maps, int num_maps,
+                    const int64_t* totals, int32_t* faces, void* workspace, size_t workspace_bytes, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -30,10 +30,14 @@ EXPORTS = [
     "moge_engine_create_v1", "moge_v1_workspace_bytes", "moge_v1_forward", "moge_v1_postprocess", "moge_op_resize_bicubic_aa",
     "moge_op_groupnorm_relu", "moge_bicubic_aa_weights", "moge_op_conv_transpose_uv",
     "moge_metrics_workspace_bytes", "moge_metrics_resize", "moge_metrics_stats", "moge_metrics_eval", "moge_metrics_boundary",
+    "moge_mesh_workspace_bytes", "moge_depth_edge", "moge_mesh_count", "moge_mesh_build",
 ]
 METRICS_MAX_SEGMENTS, METRICS_MAX_VARIANTS, METRICS_F1_THRESHOLDS, METRICS_F1_COUNTS, METRICS_OUT_SEGMENTS = 256, 8, 10, 90, 17
 (MV_DEPTH, MV_DEPTH_SCALE, MV_DEPTH_AFFINE, MV_DISPARITY, MV_DISPARITY_FROM_DEPTH, MV_POINTS_SHIFT, MV_POINTS_SCALE,
  MV_POINTS_AFFINE) = range(8)
+MESH_MAX_MAPS, MESH_MAX_CHANNELS = 8, 4
+MESH_F32, MESH_U8_UNIT, MESH_UV = 0, 1, 2
+MESH_HWC, MESH_CHW = 0, 1
 
 
 class StackConfig(C.Structure):
@@ -78,6 +82,12 @@ class Group(C.Structure):
 class MetricVariant(C.Structure):
     """moge_metric_variant_t: a prediction map and its per-image (batch, 4) params on the device."""
     _fields_ = [("kind", C.c_int), ("src", C.c_void_p), ("params", C.c_void_p)]
+
+
+class MeshMap(C.Structure):
+    """moge_mesh_map_t: one attribute map of a mesh build (source, kind, channels, layout, per-channel sign / offset, destination)."""
+    _fields_ = [("src", C.c_void_p), ("kind", C.c_int), ("channels", C.c_int), ("layout", C.c_int),
+                ("sign", C.c_float * MESH_MAX_CHANNELS), ("offset", C.c_float * MESH_MAX_CHANNELS), ("dst", C.c_void_p)]
 
 
 class MogeError(RuntimeError):
@@ -145,6 +155,11 @@ def lib() -> C.CDLL:
     L.moge_metrics_eval.argtypes = [vp, vp, vp, C.POINTER(MetricVariant), ci, vp, vp, vp, vp, ci, vp, vp, i64, ci, ci, vp, i64, vp, sz,
                                     vp]
     L.moge_metrics_boundary.argtypes = [vp, vp, C.POINTER(MetricVariant), C.POINTER(C.c_float), i64, ci, ci, vp, i64, vp]
+    fp = C.POINTER(C.c_float)
+    L.moge_mesh_workspace_bytes.argtypes = [i64, ci, ci, C.POINTER(sz)]
+    L.moge_depth_edge.argtypes = [vp, vp, vp, i64, ci, ci, ci, fp, fp, vp, vp]
+    L.moge_mesh_count.argtypes = [vp, i64, ci, ci, vp, vp, sz, vp]
+    L.moge_mesh_build.argtypes = [vp, i64, ci, ci, ci, C.POINTER(MeshMap), ci, vp, vp, vp, sz, vp]
     for name in EXPORTS:
         if name not in ("moge_last_error", "moge_version", "moge_engine_destroy"):
             getattr(L, name).restype = ci

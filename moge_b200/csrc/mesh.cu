@@ -1,0 +1,367 @@
+// Mesh export (moge/scripts/infer.py:124-150 of the reference): utils3d's depth_map_edge and build_mesh_from_map, restated in
+// oracle/utils3d_mesh.py, which these kernels match bit for bit.
+//
+// depth_map_edge: one CTA per 32 x 32 output tile with a halo of kernel_size / 2, a separable NaN-propagating window max of the
+// depth and of its negation (masked-out and out-of-image pixels are -inf), then diff = max(d) + max(-d) and the two tolerance
+// tests in fp32 with one rounding per operation (__fadd_rn / __fdiv_rn: the contract is bitwise).
+//
+// build_mesh_from_map: the pixels of an image are cut into fixed tiles of kTilePx in row-major order.  A quad is named by its
+// top-left pixel, so row-major pixel order is both the vertex order and the quad order of the reference's np.unique compaction.
+// A count pass writes per-tile vertex and quad counts, one CTA scans them image by image in a fixed order (integers only), and
+// the emit passes re-derive the flags, rank them inside the tile with ballots and write the vertex-index map, the gathered
+// attributes and the faces.  Nothing depends on the other images of a batch except where an image's rows land.
+#include "host_api.h"
+#include "../../include/moge_b200.h"
+#include <math.h>
+#include <stdint.h>
+#include <string.h>
+
+namespace mg {
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kWarps = kThreads / 32;
+constexpr int kRounds = 16;
+constexpr int kTilePx = kThreads * kRounds;       // pixels per count / emit tile
+constexpr int kScanThreads = 1024;
+constexpr int kEdgeT = 32;                        // edge tile: kEdgeT x kEdgeT outputs
+constexpr int kMaxR = 3;                          // kernel_size <= 7
+constexpr int kEdgeS = kEdgeT + 2 * kMaxR;
+constexpr int64_t kMaxPixels = int64_t(1) << 30;  // per image: vertex ids and triangle counts stay below 2^31
+
+struct Maps { moge_mesh_map_t m[MOGE_MESH_MAX_MAPS]; int n; };
+
+// np.max over a window: NaN propagates
+__device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b != b) ? __int_as_float(0x7fc00000) : fmaxf(a, b); }
+
+// ---------------------------------------------------------------------------------------------------- depth edge
+__global__ void __launch_bounds__(kThreads) edge_kernel(const float* __restrict__ depth, const uint8_t* __restrict__ mask,
+                                                        const uint8_t* __restrict__ keep, int H, int W, int r, float atol, int has_atol,
+                                                        float rtol, int has_rtol, uint8_t* __restrict__ out) {
+    __shared__ float s_hi[kEdgeS][kEdgeS], s_lo[kEdgeS][kEdgeS];   // d and -d; -inf outside the image and off the mask
+    __shared__ float h_hi[kEdgeS][kEdgeT], h_lo[kEdgeS][kEdgeT];   // row-pass maxima
+    const int64_t b = blockIdx.z, hw = static_cast<int64_t>(H) * W;
+    const int i0 = blockIdx.y * kEdgeT, j0 = blockIdx.x * kEdgeT, S = kEdgeT + 2 * r, k2 = 2 * r;
+    for (int k = threadIdx.x; k < S * S; k += kThreads) {
+        const int li = k / S, lj = k % S, i = i0 - r + li, j = j0 - r + lj;
+        float hi = -INFINITY, lo = -INFINITY;
+        if (i >= 0 && i < H && j >= 0 && j < W) {
+            const int64_t p = b * hw + static_cast<int64_t>(i) * W + j;
+            if (!mask || mask[p]) { const float d = depth[p]; hi = d; lo = -d; }
+        }
+        s_hi[li][lj] = hi;
+        s_lo[li][lj] = lo;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < S * kEdgeT; k += kThreads) {
+        const int li = k / kEdgeT, oj = k % kEdgeT;
+        float hi = s_hi[li][oj], lo = s_lo[li][oj];
+        for (int t = 1; t <= k2; ++t) { hi = nan_max(hi, s_hi[li][oj + t]); lo = nan_max(lo, s_lo[li][oj + t]); }
+        h_hi[li][oj] = hi;
+        h_lo[li][oj] = lo;
+    }
+    __syncthreads();
+    for (int k = threadIdx.x; k < kEdgeT * kEdgeT; k += kThreads) {
+        const int oi = k / kEdgeT, oj = k % kEdgeT, i = i0 + oi, j = j0 + oj;
+        if (i >= H || j >= W) continue;
+        float hi = h_hi[oi][oj], lo = h_lo[oi][oj];
+        for (int t = 1; t <= k2; ++t) { hi = nan_max(hi, h_hi[oi + t][oj]); lo = nan_max(lo, h_lo[oi + t][oj]); }
+        const int64_t p = b * hw + static_cast<int64_t>(i) * W + j;
+        const float diff = __fadd_rn(hi, lo);
+        bool edge = false;
+        if (has_atol) edge |= diff > atol;
+        if (has_rtol) edge |= __fdiv_rn(diff, depth[p]) > rtol;
+        out[p] = keep ? static_cast<uint8_t>(keep[p] && !edge) : static_cast<uint8_t>(edge);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------- mesh flags
+// quad (i, j) has corners (i, j), (i + 1, j), (i + 1, j + 1), (i, j + 1); m == NULL keeps every quad
+__device__ __forceinline__ bool quad_kept(const uint8_t* m, int H, int W, int i, int j) {
+    if (i < 0 || j < 0 || i >= H - 1 || j >= W - 1) return false;
+    if (!m) return true;
+    const uint8_t* r0 = m + static_cast<int64_t>(i) * W + j;
+    const uint8_t* r1 = r0 + W;
+    return r0[0] && r1[0] && r1[1] && r0[1];
+}
+__device__ __forceinline__ bool vertex_kept(const uint8_t* m, int H, int W, int i, int j) {
+    return quad_kept(m, H, W, i - 1, j - 1) || quad_kept(m, H, W, i - 1, j) || quad_kept(m, H, W, i, j - 1) || quad_kept(m, H, W, i, j);
+}
+
+__device__ __forceinline__ int block_sum_int(int v, int* red) {
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    int s = 0;
+    for (int w = 0; w < kWarps; ++w) s += red[w];
+    return s;
+}
+
+// Rank of this thread's flag among the set flags of the CTA's current round (thread order), and the round's total.  warp_tot is
+// double-buffered by round parity, so one barrier per round suffices.
+__device__ __forceinline__ int round_rank(bool flag, int (*warp_tot)[kWarps], int round, int* total) {
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const unsigned bal = __ballot_sync(0xffffffffu, flag);
+    int* wt = warp_tot[round & 1];
+    if (lane == 0) wt[warp] = __popc(bal);
+    __syncthreads();
+    int before = 0, tot = 0;
+    for (int w = 0; w < kWarps; ++w) { const int c = wt[w]; before += w < warp ? c : 0; tot += c; }
+    *total = tot;
+    return before + __popc(bal & ((1u << lane) - 1u));
+}
+
+// grid (tiles, images): per tile (kept vertices, kept quads)
+__global__ void __launch_bounds__(kThreads) count_kernel(const uint8_t* __restrict__ mask, int H, int W, int tiles, int32_t* __restrict__ counts) {
+    __shared__ int red[kWarps];
+    const int64_t b = blockIdx.y, hw = static_cast<int64_t>(H) * W;
+    const uint8_t* m = mask ? mask + b * hw : nullptr;
+    const int64_t p0 = static_cast<int64_t>(blockIdx.x) * kTilePx;
+    int nv = 0, nq = 0;
+    for (int r = 0; r < kRounds; ++r) {
+        const int64_t p = p0 + r * kThreads + threadIdx.x;
+        if (p >= hw) break;
+        const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
+        nv += vertex_kept(m, H, W, i, j);
+        nq += quad_kept(m, H, W, i, j);
+    }
+    nv = block_sum_int(nv, red);
+    nq = block_sum_int(nq, red);
+    if (threadIdx.x == 0) {
+        counts[(b * tiles + blockIdx.x) * 2] = nv;
+        counts[(b * tiles + blockIdx.x) * 2 + 1] = nq;
+    }
+}
+
+// one CTA: image by image, the exclusive scan of the tile counts (offsets inside the image), then per image (vertices, quads,
+// first vertex row, first quad) in the batch-wide outputs
+__global__ void __launch_bounds__(kScanThreads) scan_kernel(const int32_t* __restrict__ counts, int64_t batch, int tiles,
+                                                            int32_t* __restrict__ offsets, int64_t* __restrict__ totals) {
+    __shared__ int2 warp_tot[kScanThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int64_t voff = 0, qoff = 0;
+    for (int64_t b = 0; b < batch; ++b) {
+        int run_v = 0, run_q = 0;
+        for (int t0 = 0; t0 < tiles; t0 += kScanThreads) {
+            const int t = t0 + threadIdx.x;
+            const int cv = t < tiles ? counts[(b * tiles + t) * 2] : 0, cq = t < tiles ? counts[(b * tiles + t) * 2 + 1] : 0;
+            int iv = cv, iq = cq;
+            for (int o = 1; o < 32; o <<= 1) {
+                const int v = __shfl_up_sync(0xffffffffu, iv, o), q = __shfl_up_sync(0xffffffffu, iq, o);
+                if (lane >= o) { iv += v; iq += q; }
+            }
+            if (lane == 31) warp_tot[warp] = make_int2(iv, iq);
+            __syncthreads();
+            int bv = 0, bq = 0, tv = 0, tq = 0;
+            for (int w = 0; w < kScanThreads / 32; ++w) {
+                const int2 c = warp_tot[w];
+                if (w < warp) { bv += c.x; bq += c.y; }
+                tv += c.x; tq += c.y;
+            }
+            if (t < tiles) {
+                offsets[(b * tiles + t) * 2] = run_v + bv + iv - cv;
+                offsets[(b * tiles + t) * 2 + 1] = run_q + bq + iq - cq;
+            }
+            run_v += tv;
+            run_q += tq;
+            __syncthreads();
+        }
+        if (threadIdx.x == 0) {
+            totals[b * 4] = run_v;
+            totals[b * 4 + 1] = run_q;
+            totals[b * 4 + 2] = voff;
+            totals[b * 4 + 3] = qoff;
+        }
+        voff += run_v;
+        qoff += run_q;
+    }
+}
+
+// grid (tiles, images): the vertex-index map (-1 where not kept) and every map's row at each kept vertex
+__global__ void __launch_bounds__(kThreads) vertices_kernel(const uint8_t* __restrict__ mask, int H, int W, int tiles,
+                                                            const int32_t* __restrict__ offsets, const int64_t* __restrict__ totals,
+                                                            const Maps maps, int32_t* __restrict__ vmap) {
+    __shared__ int warp_tot[2][kWarps];
+    const int64_t b = blockIdx.y, hw = static_cast<int64_t>(H) * W;
+    const uint8_t* m = mask ? mask + b * hw : nullptr;
+    const int64_t p0 = static_cast<int64_t>(blockIdx.x) * kTilePx, row0 = totals[b * 4 + 2];
+    int run = offsets[(b * tiles + blockIdx.x) * 2];
+    for (int r = 0; r < kRounds; ++r) {
+        const int64_t p = p0 + r * kThreads + threadIdx.x;
+        if (p0 + r * kThreads >= hw) break;                          // uniform over the CTA
+        const bool in = p < hw;
+        const int i = in ? static_cast<int>(p / W) : 0, j = in ? static_cast<int>(p % W) : 0;
+        const bool kept = in && vertex_kept(m, H, W, i, j);
+        int total;
+        const int id = run + round_rank(kept, warp_tot, r, &total);
+        run += total;
+        if (!in) continue;
+        vmap[b * hw + p] = kept ? id : -1;
+        if (!kept) continue;
+        const int64_t row = row0 + id;
+        for (int k = 0; k < maps.n; ++k) {
+            const moge_mesh_map_t& d = maps.m[k];
+            const int C = d.channels;
+            for (int c = 0; c < C; ++c) {
+                float x;
+                if (d.kind == MOGE_MESH_UV) {
+                    x = c == 0 ? __fdiv_rn(static_cast<float>(j) + 0.5f, static_cast<float>(W)) : __fdiv_rn(static_cast<float>(i) + 0.5f, static_cast<float>(H));
+                } else {
+                    const int64_t e = d.layout == MOGE_MESH_HWC ? (b * hw + p) * C + c : (b * C + c) * hw + p;
+                    x = d.kind == MOGE_MESH_U8_UNIT ? __fdiv_rn(static_cast<float>(static_cast<const uint8_t*>(d.src)[e]), 255.f)
+                                                    : static_cast<const float*>(d.src)[e];
+                }
+                x = __fmul_rn(x, d.sign[c]);
+                if (d.offset[c] != 0.f) x = __fadd_rn(x, d.offset[c]);
+                d.dst[row * C + c] = x;
+            }
+        }
+    }
+}
+
+// grid (tiles, images): each kept quad's corners from the vertex-index map, as one quad or two triangles [a, b, c], [a, c, d]
+__global__ void __launch_bounds__(kThreads) faces_kernel(const uint8_t* __restrict__ mask, int H, int W, int tiles, int tri,
+                                                         const int32_t* __restrict__ offsets, const int64_t* __restrict__ totals,
+                                                         const int32_t* __restrict__ vmap, int32_t* __restrict__ faces) {
+    __shared__ int warp_tot[2][kWarps];
+    const int64_t b = blockIdx.y, hw = static_cast<int64_t>(H) * W;
+    const uint8_t* m = mask ? mask + b * hw : nullptr;
+    const int32_t* v = vmap + b * hw;
+    const int64_t p0 = static_cast<int64_t>(blockIdx.x) * kTilePx, quad0 = totals[b * 4 + 3];
+    int run = offsets[(b * tiles + blockIdx.x) * 2 + 1];
+    for (int r = 0; r < kRounds; ++r) {
+        const int64_t p = p0 + r * kThreads + threadIdx.x;
+        if (p0 + r * kThreads >= hw) break;
+        const bool in = p < hw;
+        const bool kept = in && quad_kept(m, H, W, static_cast<int>(p / W), static_cast<int>(p % W));
+        int total;
+        const int id = run + round_rank(kept, warp_tot, r, &total);
+        run += total;
+        if (!kept) continue;
+        const int32_t a = v[p], bb = v[p + W], c = v[p + W + 1], d = v[p + 1];
+        if (tri) {
+            int32_t* f = faces + (quad0 + id) * 6;
+            f[0] = a; f[1] = bb; f[2] = c; f[3] = a; f[4] = c; f[5] = d;
+        } else {
+            int32_t* f = faces + (quad0 + id) * 4;
+            f[0] = a; f[1] = bb; f[2] = c; f[3] = d;
+        }
+    }
+}
+
+int check_device(const char* what) {
+    int dev = 0, sms = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
+        return set_error("%s: no CUDA device: moge_b200 has no CPU fallback", what);
+    return 0;
+}
+
+int check_shape(const char* what, int64_t batch, int H, int W) {
+    if (batch <= 0 || batch > 65535) return set_error("%s: batch = %lld is outside [1, 65535]", what, static_cast<long long>(batch));
+    if (H <= 0 || W <= 0) return set_error("%s: bad map size %d x %d", what, H, W);
+    if (static_cast<int64_t>(H) * W > kMaxPixels)
+        return set_error("%s: a map of %d x %d pixels is too large (at most 2^30 per image)", what, H, W);
+    return 0;
+}
+
+int num_tiles(int H, int W) { return static_cast<int>((static_cast<int64_t>(H) * W + kTilePx - 1) / kTilePx); }
+
+// workspace layout (256-byte aligned pieces): tile counts, tile offsets, vertex-index map
+struct Layout { size_t counts, offsets, vmap, total; };
+size_t up(size_t x) { return (x + 255) / 256 * 256; }
+Layout layout(int64_t batch, int H, int W) {
+    const size_t t = static_cast<size_t>(num_tiles(H, W)), B = static_cast<size_t>(batch);
+    Layout l;
+    l.counts = 0;
+    l.offsets = l.counts + up(B * t * 2 * 4);
+    l.vmap = l.offsets + up(B * t * 2 * 4);
+    l.total = l.vmap + up(B * static_cast<size_t>(H) * W * 4);
+    return l;
+}
+
+int check_workspace(const Layout& l, void* ws, size_t bytes, const char* what) {
+    if (!ws || bytes < l.total) return set_error("%s: workspace of %zu bytes needed, %zu given", what, l.total, bytes);
+    if (reinterpret_cast<uintptr_t>(ws) % 256) return set_error("%s: workspace must be 256-byte aligned", what);
+    return 0;
+}
+
+}  // namespace
+}  // namespace mg
+
+using namespace mg;
+
+extern "C" {
+
+int moge_mesh_workspace_bytes(int64_t batch, int H, int W, size_t* bytes) {
+    if (!bytes) return set_error("null argument");
+    MG_TRY(check_shape("mesh", batch, H, W));
+    *bytes = layout(batch, H, W).total;
+    return 0;
+}
+
+int moge_depth_edge(const float* depth, const uint8_t* mask, const uint8_t* keep, int64_t batch, int H, int W, int kernel_size,
+                    const float* atol, const float* rtol, uint8_t* out, void* stream) {
+    if (!depth || !out) return set_error("null argument");
+    MG_TRY(check_shape("depth_map_edge", batch, H, W));
+    if (kernel_size < 3 || kernel_size > 2 * kMaxR + 1 || kernel_size % 2 == 0)
+        return set_error("depth_map_edge: kernel_size %d is not one of 3, 5, 7", kernel_size);
+    MG_TRY(check_device("depth_map_edge"));
+    const dim3 grid((W + kEdgeT - 1) / kEdgeT, (H + kEdgeT - 1) / kEdgeT, static_cast<unsigned>(batch));
+    edge_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(depth, mask, keep, H, W, kernel_size / 2, atol ? *atol : 0.f,
+                                                                          atol != nullptr, rtol ? *rtol : 0.f, rtol != nullptr, out);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_mesh_count(const uint8_t* mask, int64_t batch, int H, int W, int64_t* totals, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!totals) return set_error("null argument");
+    MG_TRY(check_shape("mesh_count", batch, H, W));
+    const Layout l = layout(batch, H, W);
+    MG_TRY(check_workspace(l, workspace, workspace_bytes, "mesh_count"));
+    MG_TRY(check_device("mesh_count"));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* ws = static_cast<char*>(workspace);
+    const int tiles = num_tiles(H, W);
+    int32_t* counts = reinterpret_cast<int32_t*>(ws + l.counts);
+    count_kernel<<<dim3(tiles, static_cast<unsigned>(batch)), kThreads, 0, st>>>(mask, H, W, tiles, counts);
+    CUDA_TRY(cudaGetLastError());
+    scan_kernel<<<1, kScanThreads, 0, st>>>(counts, batch, tiles, reinterpret_cast<int32_t*>(ws + l.offsets), totals);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_mesh_build(const uint8_t* mask, int64_t batch, int H, int W, int tri, const moge_mesh_map_t* maps, int num_maps,
+                    const int64_t* totals, int32_t* faces, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!totals || !faces || (num_maps && !maps)) return set_error("null argument");
+    MG_TRY(check_shape("mesh_build", batch, H, W));
+    if (num_maps < 0 || num_maps > MOGE_MESH_MAX_MAPS) return set_error("mesh_build: %d maps is outside [0, %d]", num_maps, MOGE_MESH_MAX_MAPS);
+    Maps ms;
+    memset(&ms, 0, sizeof(ms));
+    ms.n = num_maps;
+    for (int k = 0; k < num_maps; ++k) {
+        const moge_mesh_map_t& d = maps[k];
+        if (d.kind < MOGE_MESH_F32 || d.kind > MOGE_MESH_UV) return set_error("mesh_build: map %d has unknown kind %d", k, d.kind);
+        if (d.channels < 1 || d.channels > MOGE_MESH_MAX_CHANNELS) return set_error("mesh_build: map %d has %d channels", k, d.channels);
+        if (d.kind == MOGE_MESH_UV ? d.channels != 2 : !d.src) return set_error("mesh_build: map %d: a UV map has 2 channels, other maps a source", k);
+        if (d.layout != MOGE_MESH_HWC && d.layout != MOGE_MESH_CHW) return set_error("mesh_build: map %d has unknown layout %d", k, d.layout);
+        if (!d.dst) return set_error("mesh_build: map %d has no destination", k);
+        ms.m[k] = d;
+    }
+    const Layout l = layout(batch, H, W);
+    MG_TRY(check_workspace(l, workspace, workspace_bytes, "mesh_build"));
+    MG_TRY(check_device("mesh_build"));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* ws = static_cast<char*>(workspace);
+    const int tiles = num_tiles(H, W);
+    const int32_t* offsets = reinterpret_cast<const int32_t*>(ws + l.offsets);
+    int32_t* vmap = reinterpret_cast<int32_t*>(ws + l.vmap);
+    const dim3 grid(tiles, static_cast<unsigned>(batch));
+    vertices_kernel<<<grid, kThreads, 0, st>>>(mask, H, W, tiles, offsets, totals, ms, vmap);
+    CUDA_TRY(cudaGetLastError());
+    faces_kernel<<<grid, kThreads, 0, st>>>(mask, H, W, tiles, tri ? 1 : 0, offsets, totals, vmap, faces);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+}  // extern "C"

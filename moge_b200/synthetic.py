@@ -379,16 +379,9 @@ def _box(g: torch.Generator, H: int, W: int, lo: float, hi: float):
     return i, j, h, w
 
 
-def synthetic_metrics_case(seed: int, H: int, W: int, keys, is_metric: bool = True, sharp: bool = True, segments: int = 0,
-                           negative: bool = False):
-    """(pred, gt) dicts of CPU fp32 tensors for compute_metrics, from a seeded generator.
-
-    GT: piecewise-planar depth (a tilted background plane and occluding tilted boxes), points by unprojection with normalised
-    intrinsics, a mask with box holes and 5 % dropouts.  With `segments` > 0, box segments (later ones overwrite earlier ones)
-    plus one tiny segment (under 10 low-resolution pixels), one label whose id is absent from the map and one duplicated id.
-    Predictions: GT perturbed by scale, shift, smooth noise, 1 % outliers and a blur across the occlusion edges; `negative` puts a
-    few negative depths in.  `keys` names the predicted entries (METRICS_KEYS)."""
-    g = torch.Generator().manual_seed(seed)
+def _scene(g: torch.Generator, H: int, W: int):
+    """The GT scene of synthetic_metrics_case: (fx, fy, depth, points, mask) -- piecewise-planar depth (a tilted background plane
+    and occluding tilted boxes), points by unprojection with normalised intrinsics, a mask with box holes and 5 % dropouts."""
     fx = 0.55 + 0.4 * torch.rand((), generator=g).item()
     fy = fx * W / H
     u = (torch.arange(W, dtype=torch.float32) + 0.5) / W
@@ -405,6 +398,20 @@ def synthetic_metrics_case(seed: int, H: int, W: int, keys, is_metric: bool = Tr
         i, j, h, w = _box(g, H, W, 0.05, 0.15)
         mask[i:i + h, j:j + w] = False
     mask &= torch.rand(H, W, generator=g) > 0.05
+    return fx, fy, depth, points, mask
+
+
+def synthetic_metrics_case(seed: int, H: int, W: int, keys, is_metric: bool = True, sharp: bool = True, segments: int = 0,
+                           negative: bool = False):
+    """(pred, gt) dicts of CPU fp32 tensors for compute_metrics, from a seeded generator.
+
+    GT: piecewise-planar depth (a tilted background plane and occluding tilted boxes), points by unprojection with normalised
+    intrinsics, a mask with box holes and 5 % dropouts.  With `segments` > 0, box segments (later ones overwrite earlier ones)
+    plus one tiny segment (under 10 low-resolution pixels), one label whose id is absent from the map and one duplicated id.
+    Predictions: GT perturbed by scale, shift, smooth noise, 1 % outliers and a blur across the occlusion edges; `negative` puts a
+    few negative depths in.  `keys` names the predicted entries (METRICS_KEYS)."""
+    g = torch.Generator().manual_seed(seed)
+    fx, fy, depth, points, mask = _scene(g, H, W)
     K = torch.tensor([[fx, 0, 0.5], [0, fy, 0.5], [0, 0, 1]], dtype=torch.float32)
     gt = {"depth": depth, "points": points, "depth_mask": mask, "intrinsics": K, "is_metric": is_metric, "has_sharp_boundary": sharp}
     if segments:
@@ -452,3 +459,24 @@ def synthetic_metrics_case(seed: int, H: int, W: int, keys, is_metric: bool = Tr
         else:
             raise KeyError(k)
     return pred, gt
+
+
+def synthetic_mesh_case(seed: int, B: int, H: int, W: int):
+    """(output, image) for mesh_from_output, CPU tensors from a seeded generator: `output` looks like infer()'s batched output
+    (points (B, H, W, 3), depth (B, H, W), mask (B, H, W), normal (B, H, W, 3), intrinsics (B, 3, 3)) on synthetic_metrics_case's
+    GT scenes (image b from seed + b), with depth and points +inf and normals 0 off the mask as infer(apply_mask=True) leaves
+    them; normals are unit length.  `image` is (B, H, W, 3) uint8."""
+    out = {k: [] for k in ("points", "depth", "mask", "normal", "intrinsics")}
+    images = []
+    for b in range(B):
+        g = torch.Generator().manual_seed(5000 + seed + b)
+        fx, fy, depth, points, mask = _scene(g, H, W)
+        normal = torch.nn.functional.normalize(torch.randn(H, W, 3, generator=g) + torch.tensor([0.0, 0.0, -2.0]), dim=-1)
+        inf = torch.tensor(float("inf"))
+        out["depth"].append(torch.where(mask, depth, inf))
+        out["points"].append(torch.where(mask[..., None], points, inf))
+        out["normal"].append(torch.where(mask[..., None], normal, torch.zeros(())))
+        out["mask"].append(mask)
+        out["intrinsics"].append(torch.tensor([[fx, 0, 0.5], [0, fy, 0.5], [0, 0, 1]], dtype=torch.float32))
+        images.append(torch.randint(0, 256, (H, W, 3), generator=g, dtype=torch.uint8))
+    return {k: torch.stack(v) for k, v in out.items()}, torch.stack(images)
