@@ -679,7 +679,7 @@ struct StackBufs {     // per-level scratch maps of one ConvStack
 };
 
 static int plan_stack(moge_engine* e, Plan* pl, const char* sname, const moge_stack_config_t& sc, const StackW& sw, bool is_neck, int B, int h,
-                      int w, float su, float sv, StackBufs& sb, const std::vector<void*>& neck_out, void* x0_raw, void* x0_relu,
+                      int w, float su, float sv, const StackBufs& sb, const std::vector<void*>& neck_out, void* x0_raw, void* x0_relu,
                       void* lowres_out, void* const* neck_lowres = nullptr) {
     const int L = sc.num_levels;
     const int* C = sc.dim_res_blocks;
@@ -896,6 +896,76 @@ static void alloc_v2_decoder(moge_engine* e, Plan* pl, WsAlloc& ws, V2Bufs* v) {
     }
 }
 
+// MoGe-2 decoder launch list: neck and heads group by group, then every group's scale head and output resize (phase 2).
+// Group gi's encoder taps start at row prow0[gi] of `taps`; `cls` / `mlp_scratch`: the scale head's input rows and scratch, per image.
+static int plan_v2_decoder(moge_engine* e, Plan* pl, const uint8_t* taps, const std::vector<long>& prow0, const float* cls,
+                           float* mlp_scratch, const V2Bufs& v) {
+    const moge_config_t& c = e->cfg;
+    const int D = c.embed_dim;
+    const int G = static_cast<int>(pl->groups.size());
+    const int L = c.neck.num_levels;
+    const StackBufs& nb = v.nb;
+    const StackBufs& hb = v.hb;
+    Plan* P = pl;
+    auto gname = [&](const char* base, int gi) { return G == 1 ? std::string(base) : std::string(base) + ".g" + std::to_string(gi); };
+    // ---- decoder, group by group
+    for (int gi = 0; gi < G; ++gi) {
+        const Group& g = pl->groups[gi];
+        const int B = g.B, H = g.H, W = g.W, h = g.h, w = g.w, T = h * w;
+        const float aspect = static_cast<float>(W) / H;
+        const float su = aspect / sqrtf(1.f + aspect * aspect), sv = 1.f / sqrtf(1.f + aspect * aspect);
+        const uint8_t* taps_g = taps + static_cast<size_t>(prow0[gi]) * c.num_taps * D * 2;
+        std::vector<void*> neck_out(L, nullptr);
+        // neck level 0: folded projection GEMM over the concatenated taps (+UV rank-2 term) -> padded NHWC
+        {
+            const Level g0 = level_geom(h, w, 0);
+            const ConvW& f = e->fold0;
+            if (f.Ktot % 64) return set_error("num_taps*embed_dim must be a multiple of 64");
+            MG_TRY(add_linear(e, pl, taps_g, B * T, f.Ktot, f.w, f.N, EPI_DEC, nb.x_raw[0], f.bias, f.wu, f.N, gname("gemm.taps_proj", gi), nullptr,
+                              &g0, c.neck.num_res_blocks[0] > 0 ? nb.x_relu[0] : nullptr, f.wv, su, sv));
+        }
+        void* neck_lowres[3] = {v.pts_lr[gi], v.nrm_lr[gi], v.msk_lr[gi]};
+        const std::string sfx = G == 1 ? std::string() : ".g" + std::to_string(gi);
+        MG_TRY(plan_stack(e, pl, ("neck" + sfx).c_str(), c.neck, e->neck, true, B, h, w, su, sv, nb, neck_out, nb.x_raw[0], nb.x_relu[0], nullptr, neck_lowres));
+        for (int i = 0; i < 3; ++i) {
+            const moge_stack_config_t& sc = *head_cfg(e, i);
+            if (!sc.present) continue;
+            const Level g0 = level_geom(h, w, 0);
+            const StackW& sw = e->heads[i];
+            MG_TRY(add_conv(e, pl, sw.in0, neck_out[0], nullptr, g0, B, EPI_DEC, hb.x_raw[0], sc.num_res_blocks[0] > 0 ? hb.x_relu[0] : nullptr,
+                            nullptr, g0, sc.dim_res_blocks[0], false, false, 0, 0, std::string("conv1x1.") + head_name(i) + sfx + ".l0"));
+            void* lowres = i == 0 ? static_cast<void*>(v.pts_lr[gi]) : i == 1 ? static_cast<void*>(v.nrm_lr[gi]) : static_cast<void*>(v.msk_lr[gi]);
+            MG_TRY(plan_stack(e, pl, (std::string(head_name(i)) + sfx).c_str(), sc, sw, false, B, h, w, su, sv, hb, neck_out, hb.x_raw[0], hb.x_relu[0], lowres));
+        }
+    }
+    // ---- phase 2 (caller-bound outputs): scale head, K17 fused resize + remap
+    for (int gi = 0; gi < G; ++gi) {
+        const Group& g = pl->groups[gi];
+        const int B = g.B, H = g.H, W = g.W;
+        const Level gl = level_geom(g.h, g.w, L - 1);
+        if (c.scale_head_layers > 0) {
+            std::vector<const float*> mw = e->mlp_w, mb = e->mlp_b;
+            std::vector<int> dims(c.scale_head_dims, c.scale_head_dims + c.scale_head_layers + 1);
+            const int nl = c.scale_head_layers;
+            for (int d : dims) if (d > 4096) return set_error("scale head width %d > 4096", d);
+            const float* cls_g = cls + static_cast<size_t>(g.img0) * D;
+            float* scratch_g = mlp_scratch + static_cast<size_t>(2) * g.img0 * 4096;
+            pl->ops.add([=](cudaStream_t st) {
+                if (!P->groups[gi].scale) return 0;
+                return launch_scale_head(cls_g, mw.data(), mb.data(), dims.data(), nl, B, P->groups[gi].scale, scratch_g, st);
+            }, gname("scale_head", gi), 0, 0, 2);
+        }
+        const int remap = c.remap_output;
+        float4* pl_ = v.pts_lr[gi]; float4* nl_ = v.nrm_lr[gi]; float* ml_ = v.msk_lr[gi];
+        pl->ops.add([=](cudaStream_t st) {
+            const Group& gg = P->groups[gi];
+            return launch_head_output(gg.points ? pl_ : nullptr, gg.normal ? nl_ : nullptr, gg.mask ? ml_ : nullptr, B, gl.H, gl.W,
+                                      H, W, remap, gg.points, gg.normal, gg.mask, st);
+        }, gname("head_output", gi), 0, static_cast<double>(B) * H * W * 28 + static_cast<double>(B) * gl.H * gl.W * 36, 2);
+    }
+    return 0;
+}
+
 // Workspace layout + launch list of one call shape (a list of shape groups).  `dry`: only the byte count.
 static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cudaStream_t upload_stream = nullptr) {
     const moge_config_t& c = e->cfg;
@@ -929,12 +999,6 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     V2Bufs v2b;
     if (e->v1) v1_alloc(e, pl->groups[0], ws, &vb);
     else alloc_v2_decoder(e, pl, ws, &v2b);
-    const int L = c.neck.num_levels;
-    StackBufs& nb = v2b.nb;
-    StackBufs& hb = v2b.hb;
-    std::vector<float4*>& pts_lr = v2b.pts_lr;
-    std::vector<float4*>& nrm_lr = v2b.nrm_lr;
-    std::vector<float*>& msk_lr = v2b.msk_lr;
     if (bytes_out) *bytes_out = ws.off + 1024;
     if (dry) return 0;
     if (ws.off > pl->ws_bytes) return set_error("workspace too small: need %zu bytes, got %zu", ws.off, pl->ws_bytes);
@@ -1047,66 +1111,7 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         }
     }
     if (tap_idx != c.num_taps) return set_error("intermediate_layers must be increasing block indices < depth");
-    if (e->v1) {
-        MG_TRY(plan_v1_decoder(e, pl, taps, vb));
-        std::stable_sort(pl->ops.begin(), pl->ops.end(), [](const Op& a, const Op& b) { return a.phase < b.phase; });
-        return 0;
-    }
-    // ---- decoder, group by group
-    for (int gi = 0; gi < G; ++gi) {
-        const Group& g = pl->groups[gi];
-        const int B = g.B, H = g.H, W = g.W, h = g.h, w = g.w, T = h * w;
-        const float aspect = static_cast<float>(W) / H;
-        const float su = aspect / sqrtf(1.f + aspect * aspect), sv = 1.f / sqrtf(1.f + aspect * aspect);
-        uint8_t* taps_g = taps + static_cast<size_t>(prow0[gi]) * c.num_taps * D * 2;
-        std::vector<void*> neck_out(L, nullptr);
-        // neck level 0: folded projection GEMM over the concatenated taps (+UV rank-2 term) -> padded NHWC
-        {
-            const Level g0 = level_geom(h, w, 0);
-            const ConvW& f = e->fold0;
-            if (f.Ktot % 64) return set_error("num_taps*embed_dim must be a multiple of 64");
-            MG_TRY(add_linear(e, pl, taps_g, B * T, f.Ktot, f.w, f.N, EPI_DEC, nb.x_raw[0], f.bias, f.wu, f.N, gname("gemm.taps_proj", gi), nullptr,
-                              &g0, c.neck.num_res_blocks[0] > 0 ? nb.x_relu[0] : nullptr, f.wv, su, sv));
-        }
-        void* neck_lowres[3] = {pts_lr[gi], nrm_lr[gi], msk_lr[gi]};
-        const std::string sfx = G == 1 ? std::string() : ".g" + std::to_string(gi);
-        MG_TRY(plan_stack(e, pl, ("neck" + sfx).c_str(), c.neck, e->neck, true, B, h, w, su, sv, nb, neck_out, nb.x_raw[0], nb.x_relu[0], nullptr, neck_lowres));
-        for (int i = 0; i < 3; ++i) {
-            const moge_stack_config_t& sc = *head_cfg(e, i);
-            if (!sc.present) continue;
-            const Level g0 = level_geom(h, w, 0);
-            const StackW& sw = e->heads[i];
-            MG_TRY(add_conv(e, pl, sw.in0, neck_out[0], nullptr, g0, B, EPI_DEC, hb.x_raw[0], sc.num_res_blocks[0] > 0 ? hb.x_relu[0] : nullptr,
-                            nullptr, g0, sc.dim_res_blocks[0], false, false, 0, 0, std::string("conv1x1.") + head_name(i) + sfx + ".l0"));
-            void* lowres = i == 0 ? static_cast<void*>(pts_lr[gi]) : i == 1 ? static_cast<void*>(nrm_lr[gi]) : static_cast<void*>(msk_lr[gi]);
-            MG_TRY(plan_stack(e, pl, (std::string(head_name(i)) + sfx).c_str(), sc, sw, false, B, h, w, su, sv, hb, neck_out, hb.x_raw[0], hb.x_relu[0], lowres));
-        }
-    }
-    // ---- phase 2 (caller-bound outputs): scale head, K17 fused resize + remap
-    for (int gi = 0; gi < G; ++gi) {
-        const Group& g = pl->groups[gi];
-        const int B = g.B, H = g.H, W = g.W;
-        const Level gl = level_geom(g.h, g.w, L - 1);
-        if (c.scale_head_layers > 0) {
-            std::vector<const float*> mw = e->mlp_w, mb = e->mlp_b;
-            std::vector<int> dims(c.scale_head_dims, c.scale_head_dims + c.scale_head_layers + 1);
-            const int nl = c.scale_head_layers;
-            for (int d : dims) if (d > 4096) return set_error("scale head width %d > 4096", d);
-            const float* cls_g = cls + static_cast<size_t>(g.img0) * D;
-            float* scratch_g = mlp_scratch + static_cast<size_t>(2) * g.img0 * 4096;
-            pl->ops.add([=](cudaStream_t st) {
-                if (!P->groups[gi].scale) return 0;
-                return launch_scale_head(cls_g, mw.data(), mb.data(), dims.data(), nl, B, P->groups[gi].scale, scratch_g, st);
-            }, gname("scale_head", gi), 0, 0, 2);
-        }
-        const int remap = c.remap_output;
-        float4* pl_ = pts_lr[gi]; float4* nl_ = nrm_lr[gi]; float* ml_ = msk_lr[gi];
-        pl->ops.add([=](cudaStream_t st) {
-            const Group& gg = P->groups[gi];
-            return launch_head_output(gg.points ? pl_ : nullptr, gg.normal ? nl_ : nullptr, gg.mask ? ml_ : nullptr, B, gl.H, gl.W,
-                                      H, W, remap, gg.points, gg.normal, gg.mask, st);
-        }, gname("head_output", gi), 0, static_cast<double>(B) * H * W * 28 + static_cast<double>(B) * gl.H * gl.W * 36, 2);
-    }
+    MG_TRY(e->v1 ? plan_v1_decoder(e, pl, taps, vb) : plan_v2_decoder(e, pl, taps, prow0, cls, mlp_scratch, v2b));
     // launch order: phase 0, 1, 2 (stable)
     std::stable_sort(pl->ops.begin(), pl->ops.end(), [](const Op& a, const Op& b) { return a.phase < b.phase; });
     return 0;
@@ -1283,7 +1288,6 @@ int moge_engine_set_weight(moge_engine_t* e, const char* key, const void* dev_pt
     RawWeight rw;
     rw.numel = 1;
     for (int i = 0; i < ndim; ++i) { rw.shape.push_back(shape[i]); rw.numel *= static_cast<size_t>(shape[i]); }
-    // squeeze leading singleton dims of parameter-like tensors so shape checks see the logical shape
     CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&rw.p), std::max<size_t>(rw.numel, 4) * 4));
     const int blocks = static_cast<int>(std::min<size_t>((rw.numel + 255) / 256, 132 * 8));
     to_f32_kernel<<<std::max(blocks, 1), 256, 0, static_cast<cudaStream_t>(stream)>>>(dev_ptr, dtype, rw.p, rw.numel);

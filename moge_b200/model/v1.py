@@ -12,17 +12,21 @@ from __future__ import annotations
 import ctypes as C
 import warnings
 from numbers import Number
-from pathlib import Path
-from typing import IO, Any, Dict, List, Optional, Tuple, Union
+from typing import Dict, List, Tuple, Union
 
 import torch
 
 from .. import capi
-from ..configs import backbone_dims, v1_resized_size
-from . import v2 as _v2
+from ..configs import backbone_dims, default_num_tokens, v1_resized_size
+from ._engine import EngineModel
 
 
-class MoGeModel:
+class MoGeModel(EngineModel):
+    _strict_load = True             # the reference's from_pretrained loads strictly (v1.py:241)
+    _fp32_pass_error = (
+        "moge_b200: use_fp16=False (full-fp32 network pass) is not provided; the engine computes with 16-bit "
+        "tensor-core operands, fp32 accumulation and fp32 post-processing.  Call infer(..., use_fp16=True).")
+
     def __init__(self,
                  encoder: str = 'dinov2_vitb14',
                  intermediate_layers: Union[int, List[int]] = 4,
@@ -58,33 +62,7 @@ class MoGeModel:
                                  num_tokens_range=list(num_tokens_range), last_res_blocks=last_res_blocks,
                                  last_conv_channels=last_conv_channels, last_conv_size=last_conv_size)
         capi.make_v1_config(self.model_config, capi.F16)     # config errors the host can see, before any weight is loaded
-        self._state: Dict[str, torch.Tensor] = {}
-        self._device = torch.device("cpu")
-        self._param_dtype = torch.float32
-        self._engine = None
-        self._workspace: Optional[torch.Tensor] = None
-        self.training = False
-        self.max_chunk_tokens = 48 * 1370          # images per engine call = max_chunk_tokens // (tokens per image)
-
-    # nn.Module-like plumbing: the same engine-handle / dtype / device bookkeeping as the MoGe-2 class
-    device = _v2.MoGeModel.device
-    dtype = _v2.MoGeModel.dtype
-    eval = _v2.MoGeModel.eval
-    train = _v2.MoGeModel.train
-    requires_grad_ = _v2.MoGeModel.requires_grad_
-    state_dict = _v2.MoGeModel.state_dict
-    to = _v2.MoGeModel.to
-    cuda = _v2.MoGeModel.cuda
-    cpu = _v2.MoGeModel.cpu
-    half = _v2.MoGeModel.half
-    bfloat16 = _v2.MoGeModel.bfloat16
-    float = _v2.MoGeModel.float
-    _set_dtype = _v2.MoGeModel._set_dtype
-    _drop_engine = _v2.MoGeModel._drop_engine
-    __del__ = _v2.MoGeModel.__del__
-    _compute_code = _v2.MoGeModel._compute_code
-    engine_ops = _v2.MoGeModel.engine_ops
-    engine_profile = _v2.MoGeModel.engine_profile
+        super().__init__()
 
     def init_weights(self):
         raise NotImplementedError("training-only (v1.py:244-247)")
@@ -92,100 +70,32 @@ class MoGeModel:
     def enable_gradient_checkpointing(self):
         raise NotImplementedError("training-only (v1.py:249-251)")
 
-    def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = True):
-        """nn.Module.load_state_dict semantics; from_pretrained loads strictly, as v1.py:241 does."""
-        from torch.nn.modules.module import _IncompatibleKeys
+    def _expected_keys(self) -> List[str]:
         from ..synthetic import v1_expected_keys
-        want = v1_expected_keys(self.model_config)
-        wanted = set(want)
-        missing = [k for k in want if k not in state_dict]
-        unexpected = [k for k in state_dict.keys() if k not in wanted]
-        if strict and (missing or unexpected):
-            raise RuntimeError("Error(s) in loading state_dict for MoGeModel:\n\tMissing key(s): "
-                               f"{missing}\n\tUnexpected key(s): {unexpected}")
-        self._state = {k: v.detach() for k, v in state_dict.items()}
-        self._drop_engine()
-        return _IncompatibleKeys(missing, unexpected)
-
-    @classmethod
-    def from_pretrained(cls, pretrained_model_name_or_path: Union[str, Path, IO[bytes]],
-                        model_kwargs: Optional[Dict[str, Any]] = None, **hf_kwargs) -> 'MoGeModel':
-        """Load `{'model_config', 'model'}` checkpoints like v1.py:214-242 (local path, else HF hub), strictly."""
-        if Path(pretrained_model_name_or_path).exists():
-            checkpoint_path = pretrained_model_name_or_path
-        else:
-            from huggingface_hub import hf_hub_download
-            checkpoint_path = hf_hub_download(repo_id=pretrained_model_name_or_path, repo_type="model",
-                                              filename="model.pt", **hf_kwargs)
-        checkpoint = torch.load(checkpoint_path, map_location='cpu', weights_only=True)
-        model_config = checkpoint['model_config']
-        if model_kwargs is not None:
-            model_config.update(model_kwargs)
-        model = cls(**model_config)
-        model.load_state_dict(checkpoint['model'])
-        return model
+        return v1_expected_keys(self.model_config)
 
     # ------------------------------------------------------------------ engine
-    def _ensure_engine(self):
-        if self._engine is not None:
-            return
-        if self._device.type != "cuda":
-            raise capi.MogeError("moge_b200 has no CPU path: move the model to an H100 with .to('cuda') first")
-        if not self._state:
-            raise capi.MogeError("no weights loaded (use from_pretrained or load_state_dict)")
-        L = capi.lib()
+    def _create_engine(self, handle: C.c_void_p):
         cfg = capi.make_v1_config(self.model_config, self._compute_code())
-        handle = C.c_void_p()
-        with torch.cuda.device(self._device):
-            capi.check(L.moge_engine_create_v1(C.byref(cfg), self._device.index, C.byref(handle)))
-            stream = capi.current_stream()
-            try:
-                for key, t in self._state.items():
-                    if not t.is_floating_point():
-                        continue
-                    d = t.to(self._device).contiguous()
-                    if d.dtype not in (torch.float32, torch.float16, torch.bfloat16):
-                        d = d.float()
-                    shape = (C.c_int64 * max(d.dim(), 1))(*d.shape)
-                    capi.check(L.moge_engine_set_weight(handle, key.encode(), d.data_ptr(), shape, d.dim(),
-                                                        capi.torch_dtype_code(d.dtype), stream))
-                    torch.cuda.current_stream().synchronize()
-                capi.check(L.moge_engine_finalize(handle, stream))
-            except Exception:
-                L.moge_engine_destroy(handle)
-                raise
-        self._engine = handle
-
-    def _get_workspace(self, B, H, W, rh, rw) -> torch.Tensor:
-        n = C.c_size_t()
-        capi.check(capi.lib().moge_v1_workspace_bytes(self._engine, B, H, W, rh, rw, C.byref(n)))
-        need = n.value + 1024
-        if self._workspace is None or self._workspace.numel() < need:
-            self._workspace = None
-            self._workspace = torch.empty(need, dtype=torch.uint8, device=self._device)
-        return self._workspace
+        capi.check(capi.lib().moge_engine_create_v1(C.byref(cfg), self._device.index, C.byref(handle)))
 
     def _forward_raw(self, image: torch.Tensor, rh: int, rw: int):
         """Engine forward in chunks of at most `max_chunk_tokens` tokens; returns fp32 (points (B,H,W,3), raw mask (B,H,W))."""
         self._ensure_engine()
+        image = self._engine_input(image)
         B, _, H, W = image.shape
-        image = image.to(self._device)
-        if image.dtype not in (torch.float32, torch.float16, torch.bfloat16):
-            image = image.float()
-        image = image.contiguous()
         dev = self._device
-        chunk = max(1, min(B, self.max_chunk_tokens // ((rh // 14) * (rw // 14) + 1)))
+        L = capi.lib()
         with torch.cuda.device(dev):
             points = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev)
             mask = torch.empty(B, H, W, dtype=torch.float32, device=dev)
-            for lo in range(0, B, chunk):
-                n = min(chunk, B - lo)
-                ws = self._get_workspace(n, H, W, rh, rw)
-                base = ws.data_ptr()
-                aligned = (base + 1023) & ~1023
-                capi.check(capi.lib().moge_v1_forward(
-                    self._engine, image[lo:lo + n].data_ptr(), capi.torch_dtype_code(image.dtype), n, H, W, rh, rw, aligned,
-                    ws.numel() - (aligned - base), points[lo:lo + n].data_ptr(), mask[lo:lo + n].data_ptr(), capi.current_stream()))
+            for lo, n in self._chunks(B, (rh // 14) * (rw // 14) + 1):
+                nbytes = C.c_size_t()
+                capi.check(L.moge_v1_workspace_bytes(self._engine, n, H, W, rh, rw, C.byref(nbytes)))
+                ws, ws_bytes = self._workspace_for(nbytes.value)
+                capi.check(L.moge_v1_forward(
+                    self._engine, image[lo:lo + n].data_ptr(), capi.torch_dtype_code(image.dtype), n, H, W, rh, rw, ws, ws_bytes,
+                    points[lo:lo + n].data_ptr(), mask[lo:lo + n].data_ptr(), capi.current_stream()))
         return points, mask
 
     # ------------------------------------------------------------------ public API
@@ -212,32 +122,20 @@ class MoGeModel:
               use_fp16: bool = True) -> Dict[str, torch.Tensor]:
         """Same contract as v1.py:301-392 (note the argument order differs from MoGe-2's infer).  The engine multiplies in 16-bit
         with fp32 accumulation and post-processes in fp32; `use_fp16=False` (a full-fp32 network pass) is not provided."""
-        if not use_fp16:
-            raise NotImplementedError(
-                "moge_b200: use_fp16=False (full-fp32 network pass) is not provided; the engine computes with 16-bit "
-                "tensor-core operands, fp32 accumulation and fp32 post-processing.  Call infer(..., use_fp16=True).")
-        if image.dim() == 3:
-            omit_batch_dim = True
+        self._check_use_fp16(use_fp16)
+        omit_batch_dim = image.dim() == 3
+        if omit_batch_dim:
             image = image.unsqueeze(0)
-        else:
-            omit_batch_dim = False
         H, W = image.shape[-2:]
         aspect_ratio = W / H
         if num_tokens is None:
-            min_tokens, max_tokens = self.num_tokens_range
-            num_tokens = int(min_tokens + (resolution_level / 9) * (max_tokens - min_tokens))
+            num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
         rh, rw = v1_resized_size(H, W, int(num_tokens))
         points, mask = self._forward_raw(image, rh, rw)
         B = points.shape[0]
         dev = self._device
         with torch.cuda.device(dev):
-            focal_in = None
-            if fov_x is not None:
-                fx_t = torch.as_tensor(fov_x, device=dev, dtype=torch.float32)
-                focal_in = aspect_ratio / (1 + aspect_ratio ** 2) ** 0.5 / torch.tan(torch.deg2rad(fx_t / 2))
-                if focal_in.ndim == 0:
-                    focal_in = focal_in[None].expand(B)
-                focal_in = focal_in.contiguous()
+            focal_in = self._focal_in(fov_x, aspect_ratio, B)
             focal = torch.empty(B, dtype=torch.float32, device=dev)
             shift = torch.empty(B, dtype=torch.float32, device=dev)
             depth = torch.empty(B, H, W, dtype=torch.float32, device=dev)

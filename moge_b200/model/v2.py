@@ -12,14 +12,14 @@ from __future__ import annotations
 
 import warnings
 from numbers import Number
-from pathlib import Path
-from typing import IO, Any, Dict, List, Optional, Union
+from typing import Any, Dict, List, Optional, Union
 
 import ctypes as C
 import torch
 
 from .. import capi
 from ..configs import backbone_dims, default_num_tokens, token_grid
+from ._engine import EngineModel
 
 
 class _HeadMarker:
@@ -32,7 +32,13 @@ class _HeadMarker:
         return f"<moge_b200 decoder stack {self.config}>"
 
 
-class MoGeModel:
+class MoGeModel(EngineModel):
+    _strict_load = False            # the reference's from_pretrained loads with strict=False (v2.py:105)
+    _fp32_pass_error = (
+        "moge_b200: use_fp16=False (full-fp32 network pass) is not provided; the engine computes with 16-bit "
+        "tensor-core operands, fp32 accumulation, an fp32 residual stream and fp32 post-processing (outputs within "
+        "1e-3 of the fp32 reference, see DESIGN.md).  Call infer(..., use_fp16=True).")
+
     def __init__(self,
                  encoder: Dict[str, Any],
                  neck: Dict[str, Any],
@@ -59,24 +65,9 @@ class MoGeModel:
                           ("scale_head", scale_head)):
             if cfg is not None:
                 setattr(self, name, _HeadMarker(cfg))
-        self._state: Dict[str, torch.Tensor] = {}
-        self._device = torch.device("cpu")
-        self._param_dtype = torch.float32
-        self._engine = None                 # C handle
-        self._engine_key = None
-        self._workspace: Optional[torch.Tensor] = None
-        self.training = False
-        self.max_chunk_tokens = 48 * 1370          # images per engine call = max_chunk_tokens // (tokens per image)
+        super().__init__()
 
     # ------------------------------------------------------------------ nn.Module-like plumbing
-    @property
-    def device(self) -> torch.device:
-        return self._device
-
-    @property
-    def dtype(self) -> torch.dtype:
-        return self._param_dtype
-
     @property
     def onnx_compatible_mode(self) -> bool:
         return False
@@ -96,207 +87,54 @@ class MoGeModel:
     def enable_pytorch_native_sdpa(self):
         pass    # attention always runs in the engine's own kernel
 
-    def eval(self):
-        self.training = False
-        return self
-
-    def train(self, mode: bool = True):
-        if mode:
-            raise NotImplementedError("moge_b200 is an inference engine")
-        return self
-
-    def requires_grad_(self, flag: bool = False):
-        return self
-
-    def state_dict(self) -> Dict[str, torch.Tensor]:
-        return dict(self._state)
-
-    def load_state_dict(self, state_dict: Dict[str, torch.Tensor], strict: bool = True):
-        """nn.Module.load_state_dict semantics (the reference calls it with strict=False, v2.py:105): returns the
-        (missing_keys, unexpected_keys) report; strict=True raises RuntimeError when either list is non-empty."""
-        from torch.nn.modules.module import _IncompatibleKeys
+    def _expected_keys(self) -> List[str]:
         from ..synthetic import expected_keys
-        want = expected_keys(self.model_config)
-        got = set(state_dict.keys())
-        missing = [k for k in want if k not in got]
-        unexpected = [k for k in state_dict.keys() if k not in want]
-        if strict and (missing or unexpected):
-            raise RuntimeError("Error(s) in loading state_dict for MoGeModel:\n\tMissing key(s): "
-                               f"{missing}\n\tUnexpected key(s): {unexpected}")
-        self._state = {k: v.detach() for k, v in state_dict.items()}
-        self._drop_engine()
-        return _IncompatibleKeys(missing, unexpected)
-
-    def to(self, *args, **kwargs):
-        device = kwargs.get("device")
-        dtype = kwargs.get("dtype")
-        for a in args:
-            if isinstance(a, torch.dtype):
-                dtype = a
-            elif a is not None:
-                device = a
-        if dtype is not None:
-            self._set_dtype(dtype)
-        if device is not None:
-            device = torch.device(device)
-            if device.type == "cuda" and device.index is None:
-                device = torch.device("cuda", torch.cuda.current_device())
-            if device != self._device:
-                self._device = device
-                self._drop_engine()
-        return self
-
-    def cuda(self, device=None):
-        return self.to(torch.device("cuda", device if device is not None else torch.cuda.current_device()))
-
-    def cpu(self):
-        return self.to("cpu")
-
-    def half(self):
-        return self._set_dtype(torch.float16)
-
-    def bfloat16(self):
-        return self._set_dtype(torch.bfloat16)
-
-    def float(self):
-        return self._set_dtype(torch.float32)
-
-    def _set_dtype(self, dtype: torch.dtype):
-        if dtype not in (torch.float32, torch.float16, torch.bfloat16):
-            raise TypeError(f"unsupported dtype {dtype}")
-        if dtype != self._param_dtype:
-            self._param_dtype = dtype
-            self._drop_engine()
-        return self
-
-    def _drop_engine(self):
-        if self._engine is not None:
-            capi.lib().moge_engine_destroy(self._engine)
-        self._engine = None
-        self._workspace = None
-
-    def __del__(self):
-        try:
-            self._drop_engine()
-        except Exception:
-            pass
-
-    # ------------------------------------------------------------------ checkpoint
-    @classmethod
-    def from_pretrained(cls, pretrained_model_name_or_path: Union[str, Path, IO[bytes]],
-                        model_kwargs: Optional[Dict[str, Any]] = None, **hf_kwargs) -> 'MoGeModel':
-        """Load `{'model_config', 'model'}` checkpoints exactly like v2.py:76-107 (local path, else HF hub)."""
-        if Path(pretrained_model_name_or_path).exists():
-            checkpoint_path = pretrained_model_name_or_path
-        else:
-            from huggingface_hub import hf_hub_download
-            checkpoint_path = hf_hub_download(repo_id=pretrained_model_name_or_path, repo_type="model",
-                                              filename="model.pt", **hf_kwargs)
-        checkpoint = torch.load(checkpoint_path, map_location='cpu', weights_only=True)
-        model_config = checkpoint['model_config']
-        if model_kwargs is not None:
-            model_config.update(model_kwargs)
-        model = cls(**model_config)
-        model.load_state_dict(checkpoint['model'], strict=False)
-        return model
+        return expected_keys(self.model_config)
 
     # ------------------------------------------------------------------ engine
-    def _compute_code(self) -> int:
-        return capi.BF16 if self._param_dtype == torch.bfloat16 else capi.F16
-
-    def _ensure_engine(self):
-        if self._engine is not None:
-            return
-        if self._device.type != "cuda":
-            raise capi.MogeError("moge_b200 has no CPU path: move the model to an H100 with .to('cuda') first")
-        if not self._state:
-            raise capi.MogeError("no weights loaded (use from_pretrained or load_state_dict)")
-        L = capi.lib()
+    def _create_engine(self, handle: C.c_void_p):
         cfg = capi.make_config(self.model_config, self._compute_code())
-        handle = C.c_void_p()
-        with torch.cuda.device(self._device):
-            capi.check(L.moge_engine_create(C.byref(cfg), self._device.index, C.byref(handle)))
-            stream = capi.current_stream()
-            try:
-                for key, t in self._state.items():
-                    if not t.is_floating_point():
-                        continue
-                    d = t.to(self._device, non_blocking=False).contiguous()
-                    if d.dtype not in (torch.float32, torch.float16, torch.bfloat16):
-                        d = d.float()
-                    shape = (C.c_int64 * max(d.dim(), 1))(*d.shape)
-                    capi.check(L.moge_engine_set_weight(handle, key.encode(), d.data_ptr(), shape, d.dim(),
-                                                        capi.torch_dtype_code(d.dtype), stream))
-                    torch.cuda.current_stream().synchronize()
-                capi.check(L.moge_engine_finalize(handle, stream))
-            except Exception:
-                L.moge_engine_destroy(handle)
-                raise
-        self._engine = handle
+        capi.check(capi.lib().moge_engine_create(C.byref(cfg), self._device.index, C.byref(handle)))
 
-    def _get_workspace(self, B, H, W, h, w) -> torch.Tensor:
-        n = C.c_size_t()
-        capi.check(capi.lib().moge_engine_workspace_bytes(self._engine, B, H, W, h, w, C.byref(n)))
-        need = n.value + 1024
-        if self._workspace is None or self._workspace.numel() < need:
-            self._workspace = None
-            self._workspace = torch.empty(need, dtype=torch.uint8, device=self._device)
-        return self._workspace
+    def _alloc_outputs(self, B: int, H: int, W: int):
+        """fp32 (points, normal, mask_prob, metric_scale) buffers for B images of H x W, absent heads as None."""
+        dev = self._device
+        points = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev) if hasattr(self, "points_head") else None
+        normal = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev) if hasattr(self, "normal_head") else None
+        mask = torch.empty(B, H, W, dtype=torch.float32, device=dev) if hasattr(self, "mask_head") else None
+        scale = torch.empty(B, dtype=torch.float32, device=dev) if hasattr(self, "scale_head") else None
+        return points, normal, mask, scale
 
     def _forward_raw(self, image: torch.Tensor, h: int, w: int):
         """Runs the engine forward; returns fp32 (points, normal, mask_prob, metric_scale), absent heads as None."""
         self._ensure_engine()
+        image = self._engine_input(image)
         B, _, H, W = image.shape
-        if image.device != self._device:
-            image = image.to(self._device)
-        if image.dtype not in (torch.float32, torch.float16, torch.bfloat16):
-            image = image.float()
-        image = image.contiguous()
-        dev = self._device
-        # images are independent: large batches run as chunks of at most `max_chunk_tokens` tokens so that the activation
-        # workspace stays bounded (ViT-L, 1370 tokens/image: 32 images ~ 21 GB)
-        chunk = max(1, min(B, self.max_chunk_tokens // (h * w + 1)))
-        with torch.cuda.device(dev):
-            ws = self._get_workspace(chunk, H, W, h, w)
-            base = ws.data_ptr()
-            aligned = (base + 1023) & ~1023
-            points = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev) if hasattr(self, "points_head") else None
-            normal = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev) if hasattr(self, "normal_head") else None
-            mask = torch.empty(B, H, W, dtype=torch.float32, device=dev) if hasattr(self, "mask_head") else None
-            scale = torch.empty(B, dtype=torch.float32, device=dev) if hasattr(self, "scale_head") else None
-            for lo in range(0, B, chunk):
-                n = min(chunk, B - lo)
-                sub = lambda t: None if t is None else t[lo:lo + n]
-                if n != chunk:          # ragged tail: its own plan / workspace size
-                    ws = self._get_workspace(n, H, W, h, w)
-                    base = ws.data_ptr()
-                    aligned = (base + 1023) & ~1023
-                capi.check(capi.lib().moge_engine_forward(
-                    self._engine, image[lo:lo + n].data_ptr(), capi.torch_dtype_code(image.dtype), n, H, W, h, w, aligned,
-                    ws.numel() - (aligned - base), capi.ptr(sub(points)), capi.ptr(sub(normal)), capi.ptr(sub(mask)),
-                    capi.ptr(sub(scale)), capi.current_stream()))
-        return points, normal, mask, scale
+        L = capi.lib()
+        with torch.cuda.device(self._device):
+            outs = self._alloc_outputs(B, H, W)
+            for lo, n in self._chunks(B, h * w + 1):
+                nbytes = C.c_size_t()
+                capi.check(L.moge_engine_workspace_bytes(self._engine, n, H, W, h, w, C.byref(nbytes)))
+                ws, ws_bytes = self._workspace_for(nbytes.value)
+                points, normal, mask, scale = (None if t is None else t[lo:lo + n] for t in outs)
+                capi.check(L.moge_engine_forward(
+                    self._engine, image[lo:lo + n].data_ptr(), capi.torch_dtype_code(image.dtype), n, H, W, h, w, ws, ws_bytes,
+                    capi.ptr(points), capi.ptr(normal), capi.ptr(mask), capi.ptr(scale), capi.current_stream()))
+        return outs
 
     def _forward_groups(self, groups):
         """ONE engine call over several shape groups: `groups` = [(image (B,3,H,W), h, w)].  The encoder runs once over the
         packed token rows of all groups (moge_engine_forward_groups).  Returns [(points, normal, mask_prob, metric_scale)]."""
         self._ensure_engine()
-        dev = self._device
         n = len(groups)
         arr = (capi.Group * n)()
         keep, outs = [], []
-        with torch.cuda.device(dev):
+        with torch.cuda.device(self._device):
             for i, (image, h, w) in enumerate(groups):
-                if image.device != dev:
-                    image = image.to(dev)
-                if image.dtype not in (torch.float32, torch.float16, torch.bfloat16):
-                    image = image.float()
-                image = image.contiguous()
+                image = self._engine_input(image)
                 B, _, H, W = image.shape
-                points = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev) if hasattr(self, "points_head") else None
-                normal = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev) if hasattr(self, "normal_head") else None
-                mask = torch.empty(B, H, W, dtype=torch.float32, device=dev) if hasattr(self, "mask_head") else None
-                scale = torch.empty(B, dtype=torch.float32, device=dev) if hasattr(self, "scale_head") else None
+                points, normal, mask, scale = self._alloc_outputs(B, H, W)
                 g = arr[i]
                 g.image, g.image_dtype = image.data_ptr(), capi.torch_dtype_code(image.dtype)
                 g.B, g.H, g.W, g.h, g.w = B, H, W, h, w
@@ -305,14 +143,8 @@ class MoGeModel:
                 outs.append((points, normal, mask, scale))
             nbytes = C.c_size_t()
             capi.check(capi.lib().moge_engine_workspace_bytes_groups(self._engine, arr, n, C.byref(nbytes)))
-            need = nbytes.value + 1024
-            if self._workspace is None or self._workspace.numel() < need:
-                self._workspace = None
-                self._workspace = torch.empty(need, dtype=torch.uint8, device=dev)
-            base = self._workspace.data_ptr()
-            aligned = (base + 1023) & ~1023
-            capi.check(capi.lib().moge_engine_forward_groups(self._engine, arr, n, aligned, self._workspace.numel() - (aligned - base),
-                                                             capi.current_stream()))
+            ws, ws_bytes = self._workspace_for(nbytes.value)
+            capi.check(capi.lib().moge_engine_forward_groups(self._engine, arr, n, ws, ws_bytes, capi.current_stream()))
         return outs
 
     @torch.inference_mode()
@@ -322,8 +154,7 @@ class MoGeModel:
         No reference counterpart (the reference processes one shape per call; moge/scripts/infer.py:101 loops over files):
         images are bucketed by shape, the buckets are packed into engine calls of at most `max_chunk_tokens` tokens and every
         call runs the encoder ONCE over the token rows of all its buckets (ragged batching, BASELINE.json configs[2])."""
-        if not use_fp16:
-            raise NotImplementedError("moge_b200: use_fp16=False is not provided (see infer())")
+        self._check_use_fp16(use_fp16)
         if num_tokens is None:
             num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
         buckets: Dict[tuple, List[int]] = {}
@@ -335,9 +166,8 @@ class MoGeModel:
         units = []
         for (H, W, _), idx in buckets.items():
             h, w = token_grid(H, W, int(num_tokens))
-            per = max(1, self.max_chunk_tokens // (h * w + 1))
-            for lo in range(0, len(idx), per):
-                units.append((len(idx[lo:lo + per]) * (h * w + 1), H, W, h, w, idx[lo:lo + per]))
+            for lo, n in self._chunks(len(idx), h * w + 1):
+                units.append((n * (h * w + 1), H, W, h, w, idx[lo:lo + n]))
         units.sort(key=lambda u: -u[0])
         calls, cur, cur_tok = [], [], 0
         for u in units:
@@ -355,29 +185,6 @@ class MoGeModel:
                 for j, i in enumerate(idx):
                     results[i] = {k: v[j] for k, v in ret.items()}
         return results
-
-    def engine_ops(self):
-        """[(kernel name, algorithmic flops, algorithmic HBM bytes)] of the launch list of the most recent forward."""
-        L = capi.lib()
-        n = C.c_int()
-        capi.check(L.moge_engine_num_ops(self._engine, C.byref(n)))
-        out = []
-        buf = C.create_string_buffer(96)
-        fl, by = C.c_double(), C.c_double()
-        for i in range(n.value):
-            capi.check(L.moge_engine_op_info(self._engine, i, buf, 96, C.byref(fl), C.byref(by)))
-            out.append((buf.value.decode(), fl.value, by.value))
-        return out
-
-    def engine_profile(self):
-        """Replays the most recent forward with a CUDA-event pair around every launch; returns ms per launch."""
-        L = capi.lib()
-        n = C.c_int()
-        capi.check(L.moge_engine_num_ops(self._engine, C.byref(n)))
-        ms = (C.c_float * n.value)()
-        with torch.cuda.device(self._device):
-            capi.check(L.moge_engine_profile(self._engine, ms, n.value, capi.current_stream()))
-        return list(ms)
 
     # ------------------------------------------------------------------ public API
     def forward(self, image: torch.Tensor, num_tokens: Union[int, torch.LongTensor]) -> Dict[str, torch.Tensor]:
@@ -405,13 +212,7 @@ class MoGeModel:
             if points is not None:
                 focal = torch.empty(B, dtype=torch.float32, device=dev)
                 shift = torch.empty(B, dtype=torch.float32, device=dev)
-                focal_in = None
-                if fov_x is not None:
-                    fx_t = torch.as_tensor(fov_x, device=dev, dtype=torch.float32)
-                    focal_in = aspect_ratio / (1 + aspect_ratio ** 2) ** 0.5 / torch.tan(torch.deg2rad(fx_t / 2))
-                    if focal_in.ndim == 0:
-                        focal_in = focal_in[None].expand(B)
-                    focal_in = focal_in.contiguous()
+                focal_in = self._focal_in(fov_x, aspect_ratio, B)
                 capi.check(L.moge_recover_focal_shift(points.data_ptr(), capi.ptr(mask), None, B, H, W,
                                                       capi.ptr(focal_in), focal.data_ptr(), shift.data_ptr(), stream))
                 depth = torch.empty(B, H, W, dtype=torch.float32, device=dev)
@@ -453,16 +254,10 @@ class MoGeModel:
         `.bfloat16()`) with fp32 accumulation, fp32 residual stream and fp32 post-processing; a full-fp32 network pass
         (the reference's `use_fp16=False`, v2.py:241) does not exist here, so asking for it is an error rather than a silent
         precision downgrade."""
-        if not use_fp16:
-            raise NotImplementedError(
-                "moge_b200: use_fp16=False (full-fp32 network pass) is not provided; the engine computes with 16-bit "
-                "tensor-core operands, fp32 accumulation, an fp32 residual stream and fp32 post-processing (outputs within "
-                "1e-3 of the fp32 reference, see DESIGN.md).  Call infer(..., use_fp16=True).")
-        if image.dim() == 3:
-            omit_batch_dim = True
+        self._check_use_fp16(use_fp16)
+        omit_batch_dim = image.dim() == 3
+        if omit_batch_dim:
             image = image.unsqueeze(0)
-        else:
-            omit_batch_dim = False
         H, W = image.shape[-2:]
         aspect_ratio = W / H
         if num_tokens is None:

@@ -7,7 +7,7 @@ import pytest
 import torch
 
 from moge_b200 import capi
-from moge_b200.configs import model_config
+from moge_b200.configs import model_config, v1_model_config
 
 
 def test_library_exports_every_declared_symbol():
@@ -96,22 +96,40 @@ def test_create_rejects_configs_the_neck_fold_cannot_cover(change, msg):
     assert msg in err, err
 
 
-def test_model_plumbing_without_gpu():
-    """nn.Module-like surface of the drop-in class (v2.py:59-74,109-120): dtype/device bookkeeping, training-only stubs."""
-    from moge.model.v2 import MoGeModel
-    m = MoGeModel(**model_config("vits", with_normal=False), some_deprecated_kwarg=1) if False else MoGeModel(**model_config("vits", with_normal=False))
-    assert not hasattr(m, "normal_head") and hasattr(m, "points_head") and hasattr(m, "scale_head")
+def _check_model_plumbing(MoGeModel, cfg):
+    """nn.Module-like surface both drop-in classes share (EngineModel): dtype/device bookkeeping, training-only stubs."""
+    m = MoGeModel(**cfg)
     assert m.dtype == torch.float32 and m.half().dtype == torch.float16 and m.bfloat16().dtype == torch.bfloat16
     assert m.eval() is m and m.device.type == "cpu"
+    assert m.to(dtype=torch.float16).dtype == torch.float16 and m.float().dtype == torch.float32 and m.cpu() is m
+    assert m.train(False) is m and m.requires_grad_(False) is m and m.state_dict() == {}
+    with pytest.raises(NotImplementedError):
+        m.train()
+    with pytest.raises(TypeError):
+        m.to(torch.float64)
     with pytest.raises(NotImplementedError):
         m.init_weights()
     with pytest.raises(NotImplementedError):
         m.enable_gradient_checkpointing()
+    with pytest.warns(UserWarning):
+        MoGeModel(**cfg, deprecated_thing=3)          # v2.py:42-43, v1.py:166-172
+    return m
+
+
+def test_model_plumbing_without_gpu():
+    """nn.Module-like surface of the drop-in class (v2.py:59-74,109-120): dtype/device bookkeeping, training-only stubs."""
+    from moge.model.v2 import MoGeModel
+    m = _check_model_plumbing(MoGeModel, model_config("vits", with_normal=False))
+    assert not hasattr(m, "normal_head") and hasattr(m, "points_head") and hasattr(m, "scale_head")
     with pytest.raises(NotImplementedError):
         m.onnx_compatible_mode = True
     assert m.onnx_compatible_mode is False
-    with pytest.warns(UserWarning):
-        MoGeModel(**model_config("vits"), deprecated_thing=3)          # v2.py:42-43
+
+
+def test_v1_model_plumbing_without_gpu():
+    """The same surface on the MoGe-1 class (v1.py:206-251)."""
+    from moge.model.v1 import MoGeModel
+    _check_model_plumbing(MoGeModel, v1_model_config("vits"))
 
 
 def test_synthetic_checkpoint_roundtrip(tmp_path):
