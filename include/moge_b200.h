@@ -316,6 +316,36 @@ int moge_mesh_count(const uint8_t* mask, int64_t batch, int H, int W, int64_t* t
 int moge_mesh_build(const uint8_t* mask, int64_t batch, int H, int W, int tri, const moge_mesh_map_t* maps, int num_maps,
                     const int64_t* totals, int32_t* faces, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- panorama inference (moge/utils/panorama.py and moge/scripts/infer_panorama.py:83-122; Python: moge_b200.panorama).
+ * A camera is the reference's fp32 extrinsics [R | t] (R row-major) and its normalised pinhole intrinsics in fp64.  Panorama
+ * maps are equirectangular, h x w, at least 2 x 2 and at most 2^28 pixels.                                                  */
+#define MOGE_PANORAMA_MAX_VIEWS 20
+typedef struct { float R[9]; float t[3]; double fx, fy, cx, cy; } moge_panorama_camera_t;
+/* split_panorama_image: views_f32 (views, 3, res, res) = value / 255 of cv2.remap(image, INTER_LINEAR, BORDER_CONSTANT 0) at the
+ * panorama pixel of each view pixel's ray; grid (res) is the fp32 pixel-centre coordinate of uv_map; views_u8 (views, res, res, 3)
+ * the uint8 values (may be NULL).  image (H, W, 3) uint8 RGB.                                                                 */
+int moge_panorama_split(const uint8_t* image, int H, int W, const moge_panorama_camera_t* cams, int views, const float* grid, int res,
+                        float* views_f32, uint8_t* views_u8, void* stream);
+/* workspace (256-byte aligned) of moge_panorama_rhs / moge_panorama_lsmr for a level of h x w (and for every smaller level) */
+int moge_panorama_workspace_bytes(int views, int h, int w, size_t* bytes);
+/* one merge level's right-hand side: src (views, vh, vw, channels) fp32 is the distance (channels 1) or the point map whose norm
+ * is the distance (channels 3), mask (views, vh, vw) uint8, directions (h, w, 3) fp32 the panorama rays.  b fp64 and row_mask
+ * uint8 have 2hw + (h-1)(w+1) rows in the reference's order: x-gradient h*w, y-gradient (h-1) x (w+1) (column w repeats column
+ * 0, as the reference's x-wrapped grid does), Laplacian h*w; b = 0 where masked out.  pano_mask (h, w) uint8 = any view's mask. */
+int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int views, int vh, int vw, const moge_panorama_camera_t* cams,
+                      const float* directions, int h, int w, double* b, uint8_t* row_mask, uint8_t* pano_mask, void* workspace,
+                      size_t workspace_bytes, void* stream);
+/* SciPy's lsmr(A, b, atol = btol = 1e-5, x0 = log(init)) on the rows of row_mask (init NULL: x0 = None), depth (h, w) fp32 =
+ * exp(x); stats (2) int32 on the device = (iterations, istop).  One cooperative launch, no host synchronisation.            */
+int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int h, int w, const float* init, float* depth, int32_t* stats,
+                       void* workspace, size_t workspace_bytes, void* stream);
+/* cv2.resize(src, (W, H), INTER_LINEAR) of an fp32 map: the pyramid's upsampling */
+int moge_panorama_resize(const float* src, int h, int w, int H, int W, float* dst, void* stream);
+/* infer_panorama.py:120-122: depth_out (H, W) the resized depth, mask_out (H, W) uint8 the bilinear resize of the 0/1 mask > 0,
+ * points (H, W, 3) = depth_out * spherical_uv_to_directions(uv_map(H, W)).                                                   */
+int moge_panorama_finish(const float* depth, const uint8_t* mask, int h, int w, int H, int W, float* depth_out, uint8_t* mask_out,
+                         float* points, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -31,6 +31,8 @@ EXPORTS = [
     "moge_op_groupnorm_relu", "moge_bicubic_aa_weights", "moge_op_conv_transpose_uv",
     "moge_metrics_workspace_bytes", "moge_metrics_resize", "moge_metrics_stats", "moge_metrics_eval", "moge_metrics_boundary",
     "moge_mesh_workspace_bytes", "moge_depth_edge", "moge_mesh_count", "moge_mesh_build",
+    "moge_panorama_split", "moge_panorama_workspace_bytes", "moge_panorama_rhs", "moge_panorama_lsmr", "moge_panorama_resize",
+    "moge_panorama_finish",
 ]
 METRICS_MAX_SEGMENTS, METRICS_MAX_VARIANTS, METRICS_F1_THRESHOLDS, METRICS_F1_COUNTS, METRICS_OUT_SEGMENTS = 256, 8, 10, 90, 17
 (MV_DEPTH, MV_DEPTH_SCALE, MV_DEPTH_AFFINE, MV_DISPARITY, MV_DISPARITY_FROM_DEPTH, MV_POINTS_SHIFT, MV_POINTS_SCALE,
@@ -38,6 +40,7 @@ METRICS_MAX_SEGMENTS, METRICS_MAX_VARIANTS, METRICS_F1_THRESHOLDS, METRICS_F1_CO
 MESH_MAX_MAPS, MESH_MAX_CHANNELS = 8, 4
 MESH_F32, MESH_U8_UNIT, MESH_UV = 0, 1, 2
 MESH_HWC, MESH_CHW = 0, 1
+PANORAMA_MAX_VIEWS = 20
 
 
 class StackConfig(C.Structure):
@@ -88,6 +91,12 @@ class MeshMap(C.Structure):
     """moge_mesh_map_t: one attribute map of a mesh build (source, kind, channels, layout, per-channel sign / offset, destination)."""
     _fields_ = [("src", C.c_void_p), ("kind", C.c_int), ("channels", C.c_int), ("layout", C.c_int),
                 ("sign", C.c_float * MESH_MAX_CHANNELS), ("offset", C.c_float * MESH_MAX_CHANNELS), ("dst", C.c_void_p)]
+
+
+class PanoramaCamera(C.Structure):
+    """moge_panorama_camera_t: fp32 extrinsics [R | t] (R row-major) and fp64 normalised pinhole intrinsics."""
+    _fields_ = [("R", C.c_float * 9), ("t", C.c_float * 3), ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double),
+                ("cy", C.c_double)]
 
 
 class MogeError(RuntimeError):
@@ -160,6 +169,13 @@ def lib() -> C.CDLL:
     L.moge_depth_edge.argtypes = [vp, vp, vp, i64, ci, ci, ci, fp, fp, vp, vp]
     L.moge_mesh_count.argtypes = [vp, i64, ci, ci, vp, vp, sz, vp]
     L.moge_mesh_build.argtypes = [vp, i64, ci, ci, ci, C.POINTER(MeshMap), ci, vp, vp, vp, sz, vp]
+    pc = C.POINTER(PanoramaCamera)
+    L.moge_panorama_split.argtypes = [vp, ci, ci, pc, ci, vp, ci, vp, vp, vp]
+    L.moge_panorama_workspace_bytes.argtypes = [ci, ci, ci, C.POINTER(sz)]
+    L.moge_panorama_rhs.argtypes = [vp, ci, vp, ci, ci, ci, pc, vp, ci, ci, vp, vp, vp, vp, sz, vp]
+    L.moge_panorama_lsmr.argtypes = [vp, vp, ci, ci, vp, vp, vp, vp, sz, vp]
+    L.moge_panorama_resize.argtypes = [vp, ci, ci, ci, ci, vp, vp]
+    L.moge_panorama_finish.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp]
     for name in EXPORTS:
         if name not in ("moge_last_error", "moge_version", "moge_engine_destroy"):
             getattr(L, name).restype = ci

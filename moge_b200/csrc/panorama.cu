@@ -1,0 +1,655 @@
+// Panorama inference (moge/utils/panorama.py and moge/scripts/infer_panorama.py:83-122 of the reference) on the device.
+//
+// split: every view pixel's ray (the view camera's unprojection, in fp64 with one rounding per operation, as the utils3d
+// restatement in oracle/utils3d_panorama.py writes it), its spherical uv and panorama pixel, rounded to fp32 and sampled as
+// cv2.remap(INTER_LINEAR, BORDER_CONSTANT 0) samples a uint8 image: coordinates snapped to 1/32 pixel, 15-bit fixed-point
+// weights.  Bitwise equal to cv2 for the same fp32 coordinates.
+//
+// merge, per pyramid level of h x w: a sample pass projects each panorama direction into every view (fp32 rotation, fp64
+// projection) and samples log |p| with cv2's fp32 bilinear (1/32 snapping, replicate border) and the view mask with its nearest
+// rule; a right-hand-side pass forms the x / y gradients and the 5-point Laplacians of every view with their masks, sums them over
+// the views in view order in fp32 and divides by the counts in fp64.  Rows are dense: h*w x-gradient, (h-1)*(w+1) y-gradient and
+// h*w Laplacian rows; a masked-out row has b = 0 and no equation.  The y-gradient rows run over w + 1 columns because the
+// reference builds them on the x-wrapped grid: column w repeats column 0, so that equation is in the system twice.
+//
+// lsmr: SciPy's LSMR (scipy/sparse/linalg/_isolve/lsmr.py) on that stencil system in one cooperative kernel: grid-wide barriers
+// between the matrix products, fp64 u, v, h, hbar, x stored in fp64 but rounded to fp32 after each update when the level starts
+// from an initial guess (SciPy keeps x0's dtype), and the scalar recurrences and stopping rules evaluated identically by every
+// thread from deterministic reductions.  The iteration count and istop are written to the device.
+#include "host_api.h"
+#include "../../include/moge_b200.h"
+#include <cooperative_groups.h>
+#include <algorithm>
+#include <math.h>
+#include <stdint.h>
+#include <string.h>
+
+namespace cg = cooperative_groups;
+
+namespace mg {
+namespace {
+
+constexpr int kThreads = 256;
+constexpr int kLsmrThreads = 512;
+constexpr int64_t kMaxPixels = int64_t(1) << 28;
+
+struct Cams { moge_panorama_camera_t c[MOGE_PANORAMA_MAX_VIEWS]; int n; };
+
+__device__ __forceinline__ double dmul(double a, double b) { return __dmul_rn(a, b); }
+__device__ __forceinline__ double dadd(double a, double b) { return __dadd_rn(a, b); }
+__device__ __forceinline__ double dsub(double a, double b) { return __dsub_rn(a, b); }
+__device__ __forceinline__ float fmul(float a, float b) { return __fmul_rn(a, b); }
+__device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b); }
+
+// cv2's float map -> fixed point: cvRound(x * 32)
+__device__ __forceinline__ int q32(float x) { return __float2int_rn(fmul(x, 32.f)); }
+
+// ---------------------------------------------------------------------------------------------------- split
+__global__ void __launch_bounds__(kThreads) split_kernel(const uint8_t* __restrict__ img, int H, int W, const Cams cams,
+                                                         const float* __restrict__ grid, int res, float* __restrict__ out,
+                                                         uint8_t* __restrict__ out_u8) {
+    const int64_t total = static_cast<int64_t>(cams.n) * res * res;
+    for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total; idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int k = static_cast<int>(idx / (static_cast<int64_t>(res) * res));
+        const int pix = static_cast<int>(idx % (static_cast<int64_t>(res) * res)), i = pix / res, j = pix % res;
+        const moge_panorama_camera_t& c = cams.c[k];
+        // unproject_cv(uv, 1): ((u - cx) / fx, (v - cy) / fy, 1), then R^T (p - t)
+        const double p0 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[j]), c.cx), c.fx), static_cast<double>(c.t[0]));
+        const double p1 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[i]), c.cy), c.fy), static_cast<double>(c.t[1]));
+        const double p2 = dsub(1.0, static_cast<double>(c.t[2]));
+        double d[3];
+        for (int r = 0; r < 3; ++r)
+            d[r] = dadd(dadd(dmul(c.R[r], p0), dmul(c.R[3 + r], p1)), dmul(c.R[6 + r], p2));
+        // directions_to_spherical_uv
+        const double nrm = sqrt(dadd(dadd(dmul(d[0], d[0]), dmul(d[1], d[1])), dmul(d[2], d[2])));
+        const double x = __ddiv_rn(d[0], nrm), y = __ddiv_rn(d[1], nrm), z = __ddiv_rn(d[2], nrm);
+        double a = __ddiv_rn(atan2(y, x), 6.283185307179586), m = fmod(a, 1.0);
+        if (m != 0.0) { if (m < 0) m = dadd(m, 1.0); } else m = 0.0;         // numpy's floor-mod: sign of the divisor
+        const double u = dsub(1.0, m), v = __ddiv_rn(acos(z), 3.141592653589793);
+        // uv_to_pixel, fp32, cv2 fixed point
+        const int X = q32(__double2float_rn(dsub(dmul(u, static_cast<double>(W)), 0.5)));
+        const int Y = q32(__double2float_rn(dsub(dmul(v, static_cast<double>(H)), 0.5)));
+        const int ix = X >> 5, iy = Y >> 5, fx = X & 31, fy = Y & 31;
+        const int w[4] = {(32 - fx) * (32 - fy) * 32, fx * (32 - fy) * 32, (32 - fx) * fy * 32, fx * fy * 32};
+        int acc[3] = {0, 0, 0};
+        for (int t = 0; t < 4; ++t) {
+            const int yy = iy + (t >> 1), xx = ix + (t & 1);
+            if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;        // BORDER_CONSTANT 0
+            const uint8_t* s = img + (static_cast<int64_t>(yy) * W + xx) * 3;
+            for (int ch = 0; ch < 3; ++ch) acc[ch] += w[t] * s[ch];
+        }
+        for (int ch = 0; ch < 3; ++ch) {
+            const int val = min(255, max(0, (acc[ch] + (1 << 14)) >> 15));
+            out[((static_cast<int64_t>(k) * 3 + ch) * res + i) * res + j] = __double2float_rn(static_cast<double>(val) / 255.0);
+            if (out_u8) out_u8[idx * 3 + ch] = static_cast<uint8_t>(val);
+        }
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------- merge right-hand side
+__device__ __forceinline__ float log_distance(const float* __restrict__ src, int channels, int64_t e) {
+    if (channels == 1) return logf(src[e]);
+    const float* p = src + e * 3;
+    return logf(sqrtf(fadd(fadd(fmul(p[0], p[0]), fmul(p[1], p[1])), fmul(p[2], p[2]))));
+}
+
+// grid over panorama pixels: per view, the sampled log-distance (0 outside the view) and mask
+__global__ void __launch_bounds__(kThreads) sample_kernel(const float* __restrict__ src, int channels, const uint8_t* __restrict__ vmask,
+                                                          int vh, int vw, const Cams cams, const float* __restrict__ dirs, int h, int w,
+                                                          float* __restrict__ L, uint8_t* __restrict__ M) {
+    const int64_t n = static_cast<int64_t>(h) * w;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const float d0 = dirs[p * 3], d1 = dirs[p * 3 + 1], d2 = dirs[p * 3 + 2];
+        for (int k = 0; k < cams.n; ++k) {
+            const moge_panorama_camera_t& c = cams.c[k];
+            float q[3];
+            for (int r = 0; r < 3; ++r) q[r] = fadd(fadd(fadd(fmul(c.R[3 * r], d0), fmul(c.R[3 * r + 1], d1)), fmul(c.R[3 * r + 2], d2)), c.t[r]);
+            const double X = q[0], Y = q[1], Z = q[2];
+            double u = __ddiv_rn(dadd(dmul(c.fx, X), dmul(c.cx, Z)), Z), v = __ddiv_rn(dadd(dmul(c.fy, Y), dmul(c.cy, Z)), Z);
+            const bool valid = q[2] > 0.f && u > 0.0 && v > 0.0 && u < 1.0 && v < 1.0;
+            u = fmin(fmax(u, 0.0), 1.0);
+            v = fmin(fmax(v, 0.0), 1.0);
+            const float px = __double2float_rn(dsub(dmul(u, static_cast<double>(vw)), 0.5));
+            const float py = __double2float_rn(dsub(dmul(v, static_cast<double>(vh)), 0.5));
+            const int64_t base = static_cast<int64_t>(k) * vh * vw;
+            float val = 0.f;
+            uint8_t m = 0;
+            if (valid) {
+                const int Xq = q32(px), Yq = q32(py), ix = Xq >> 5, iy = Yq >> 5;
+                const float ax = static_cast<float>(Xq & 31) / 32.f, ay = static_cast<float>(Yq & 31) / 32.f;
+                const float wx[2] = {1.f - ax, ax}, wy[2] = {1.f - ay, ay};
+                float acc = 0.f;
+                for (int t = 0; t < 4; ++t) {
+                    const int yy = min(max(iy + (t >> 1), 0), vh - 1), xx = min(max(ix + (t & 1), 0), vw - 1);
+                    acc = fadd(acc, fmul(fmul(wy[t >> 1], wx[t & 1]), log_distance(src, channels, base + static_cast<int64_t>(yy) * vw + xx)));
+                }
+                val = acc;
+                const int nx = min(max(__float2int_rn(px), 0), vw - 1), ny = min(max(__float2int_rn(py), 0), vh - 1);
+                m = vmask[base + static_cast<int64_t>(ny) * vw + nx] != 0;
+            }
+            L[k * n + p] = val;
+            M[k * n + p] = m;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kThreads) rhs_kernel(const float* __restrict__ L, const uint8_t* __restrict__ M, int views, int h, int w,
+                                                       double* __restrict__ b, uint8_t* __restrict__ rm, uint8_t* __restrict__ pmask) {
+    const int64_t n = static_cast<int64_t>(h) * w;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int i = static_cast<int>(p / w), j = static_cast<int>(p % w);
+        const int64_t pr = i * static_cast<int64_t>(w) + (j + 1) % w, pl = i * static_cast<int64_t>(w) + (j + w - 1) % w;
+        const int64_t pu = static_cast<int64_t>(max(i - 1, 0)) * w + j, pd = static_cast<int64_t>(min(i + 1, h - 1)) * w + j;
+        float sx = 0.f, sy = 0.f, sl = 0.f;
+        int cx = 0, cy = 0, cl = 0, any = 0;
+        for (int k = 0; k < views; ++k) {
+            const float* Lk = L + k * n;
+            const uint8_t* Mk = M + k * n;
+            const float c = Lk[p];
+            const int mc = Mk[p], mr = Mk[pr];
+            any |= mc;
+            const int mx = mc & mr;
+            const float gx = fmul(__fsub_rn(c, Lk[pr]), static_cast<float>(mx));
+            sx = k ? fadd(sx, gx) : gx;
+            cx += mx;
+            if (i < h - 1) {
+                const int my = mc & Mk[p + w];
+                const float gy = fmul(__fsub_rn(c, Lk[p + w]), static_cast<float>(my));
+                sy = k ? fadd(sy, gy) : gy;
+                cy += my;
+            }
+            // scipy.ndimage.convolve of the edge / wrap padded map: fp64 taps in footprint order, rounded to fp32
+            const double lap = dadd(dadd(dadd(dadd(static_cast<double>(Lk[pu]), static_cast<double>(Lk[pl])), -4.0 * static_cast<double>(c)),
+                                         static_cast<double>(Lk[pr])), static_cast<double>(Lk[pd]));
+            const int ml = mc & Mk[pu] & Mk[pd] & Mk[pl] & mr;
+            const float gl = fmul(__double2float_rn(lap), static_cast<float>(ml));
+            sl = k ? fadd(sl, gl) : gl;
+            cl += ml;
+        }
+        b[p] = cx ? __ddiv_rn(static_cast<double>(sx), static_cast<double>(cx)) : 0.0;
+        rm[p] = cx > 0;
+        if (i < h - 1) {
+            const double by = cy ? __ddiv_rn(static_cast<double>(sy), static_cast<double>(cy)) : 0.0;
+            const int64_t e = n + static_cast<int64_t>(i) * (w + 1) + j;
+            b[e] = by;
+            rm[e] = cy > 0;
+            if (j == 0) { b[e + w] = by; rm[e + w] = cy > 0; }
+        }
+        const int64_t lo = n + static_cast<int64_t>(h - 1) * (w + 1);
+        b[lo + p] = cl ? __ddiv_rn(static_cast<double>(sl), static_cast<double>(cl)) : 0.0;
+        rm[lo + p] = cl > 0;
+        pmask[p] = any;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------- LSMR
+struct Lsmr {
+    const double* b; const uint8_t* rm; const float* init;
+    double *u, *v, *hv, *hb, *x, *part;        // part: 2 buffers x gridDim.x x 2 doubles
+    float* depth; int32_t* stats;
+    int h, w;
+};
+
+// deterministic grid-wide sum of two values: block tree, then every thread sums the block partials in the same order
+__device__ double2 grid_sum2(double a, double c, double* part, int buf, cg::grid_group& g) {
+    __shared__ double2 red[kLsmrThreads / 32];
+    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) red[warp] = make_double2(a, c);
+    __syncthreads();
+    double* P = part + static_cast<int64_t>(buf) * gridDim.x * 2;
+    if (threadIdx.x == 0) {
+        double s = 0, t = 0;
+        for (int k = 0; k < kLsmrThreads / 32; ++k) { s += red[k].x; t += red[k].y; }
+        P[blockIdx.x * 2] = s;
+        P[blockIdx.x * 2 + 1] = t;
+    }
+    g.sync();
+    double s = 0, t = 0;
+    for (int k = lane; k < static_cast<int>(gridDim.x); k += 32) { s += __ldcg(P + k * 2); t += __ldcg(P + k * 2 + 1); }
+    for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); t += __shfl_xor_sync(0xffffffffu, t, o); }
+    __syncthreads();
+    return make_double2(s, t);
+}
+
+__device__ __forceinline__ double sgn(double a) { return a > 0 ? 1.0 : (a < 0 ? -1.0 : 0.0); }
+__device__ void sym_ortho(double a, double b, double* c, double* s, double* r) {
+    if (b == 0) { *c = sgn(a); *s = 0; *r = fabs(a); }
+    else if (a == 0) { *c = 0; *s = sgn(b); *r = fabs(b); }
+    else if (fabs(b) > fabs(a)) { const double tau = a / b; *s = sgn(b) / sqrt(1 + tau * tau); *c = *s * tau; *r = b / *s; }
+    else { const double tau = b / a; *c = sgn(a) / sqrt(1 + tau * tau); *s = *c * tau; *r = a / *c; }
+}
+
+// (A v) at the dense rows of pixel p: x-gradient, y-gradient (i < h - 1), Laplacian (centre, up, down, left, right)
+template <typename T>
+__device__ __forceinline__ void apply_rows(const T* v, int64_t p, int i, int j, int h, int w, T* ax, T* ay, T* al) {
+    const int64_t pr = i * static_cast<int64_t>(w) + (j + 1) % w, pl = i * static_cast<int64_t>(w) + (j + w - 1) % w;
+    const int64_t pu = static_cast<int64_t>(max(i - 1, 0)) * w + j, pd = static_cast<int64_t>(min(i + 1, h - 1)) * w + j;
+    *ax = v[p] - v[pr];
+    *ay = i < h - 1 ? v[p] - v[p + w] : T(0);
+    T s = T(-4) * v[p];
+    s = s + v[pu]; s = s + v[pd]; s = s + v[pl]; s = s + v[pr];
+    *al = s;
+}
+
+// (A^T u) at column p, from the dense rows of u (zero at masked-out rows)
+__device__ __forceinline__ double apply_cols(const double* u, int64_t p, int i, int j, int h, int w) {
+    const int64_t n = static_cast<int64_t>(h) * w;
+    const double* ux = u;
+    const double* uy = u + n + static_cast<int64_t>(i) * (w + 1);           // row i of the (h-1) x (w+1) y-gradient rows
+    const double* ul = u + n + static_cast<int64_t>(h - 1) * (w + 1);
+    const int64_t pr = i * static_cast<int64_t>(w) + (j + 1) % w, pl = i * static_cast<int64_t>(w) + (j + w - 1) % w;
+    double s = ux[p] - ux[pl];
+    if (i < h - 1) { s += uy[j]; if (j == 0) s += uy[w]; }
+    if (i > 0) { s -= uy[j - (w + 1)]; if (j == 0) s -= uy[w - (w + 1)]; }
+    s += -4.0 * ul[p];
+    if (i + 1 < h) s += ul[p + w]; else s += ul[p];        // rows whose down tap is p
+    if (i > 0) s += ul[p - w]; else s += ul[p];            // rows whose up tap is p
+    s += ul[pr] + ul[pl];                                  // rows whose left / right tap is p
+    return s;
+}
+
+// the dense rows of pixel (i, j): x-gradient, y-gradient (i < h - 1) and its repeat at column w (j == 0), Laplacian; the kind
+// (0 x, 1 y, 2 Laplacian) selects the row's value in apply_rows
+__device__ __forceinline__ int pixel_rows(int64_t p, int i, int j, int h, int w, int64_t* e, int* kind) {
+    const int64_t n = static_cast<int64_t>(h) * w;
+    int c = 0;
+    e[c] = p; kind[c++] = 0;
+    if (i < h - 1) {
+        const int64_t y = n + static_cast<int64_t>(i) * (w + 1) + j;
+        e[c] = y; kind[c++] = 1;
+        if (j == 0) { e[c] = y + w; kind[c++] = 1; }
+    }
+    e[c] = n + static_cast<int64_t>(h - 1) * (w + 1) + p; kind[c++] = 2;
+    return c;
+}
+
+__global__ void __launch_bounds__(kLsmrThreads) lsmr_kernel(Lsmr a) {
+    cg::grid_group g = cg::this_grid();
+    const int h = a.h, w = a.w;
+    const int64_t n = static_cast<int64_t>(h) * w;
+    const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x, first = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    const bool x32 = a.init != nullptr;
+    const double atol = 1e-5, btol = 1e-5, ctol = 1e-8;
+    int buf = 0;
+#define FOR_PIXELS for (int64_t p = first; p < n; p += stride)
+#define PIXEL_IJ const int i = static_cast<int>(p / w), j = static_cast<int>(p % w)
+    // u = b - A x0 (fp32 product, as SciPy's fp32 csr times an fp32 x0) or u = b; ||b||, rows in use
+    double sb = 0, sm = 0, su = 0;
+    FOR_PIXELS {
+        PIXEL_IJ;
+        float ax = 0, ay = 0, al = 0;
+        if (x32) apply_rows<float>(a.init, p, i, j, h, w, &ax, &ay, &al);          // a.init holds log(init) here (see below)
+        const float av[3] = {ax, ay, al};
+        int64_t es[4];
+        int ks[4];
+        const int nr = pixel_rows(p, i, j, h, w, es, ks);
+        for (int q = 0; q < nr; ++q) {
+            const int64_t e = es[q];
+            const int r = ks[q];
+            const double bb = a.rm[e] ? a.b[e] : 0.0;
+            const double uu = a.rm[e] ? bb - static_cast<double>(av[r]) : 0.0;
+            sb += bb * bb; sm += a.rm[e]; su += uu * uu;
+            a.u[e] = x32 ? uu : bb;
+        }
+        a.x[p] = x32 ? static_cast<double>(a.init[p]) : 0.0;
+        a.hb[p] = 0.0;
+    }
+    double2 r2 = grid_sum2(sb, sm, a.part, buf, g); buf ^= 1;
+    const double normb = sqrt(r2.x);
+    const double maxiter = fmin(r2.y, static_cast<double>(n));
+    double beta = normb;
+    if (x32) { beta = sqrt(grid_sum2(su, 0, a.part, buf, g).x); buf ^= 1; }
+    double alpha = 0;
+    if (beta > 0) {
+        const double ib = 1 / beta;
+        FOR_PIXELS { PIXEL_IJ; int64_t es[4]; int ks[4]; const int nr = pixel_rows(p, i, j, h, w, es, ks); for (int q = 0; q < nr; ++q) a.u[es[q]] = ib * a.u[es[q]]; }
+        g.sync();
+        double sv = 0;
+        FOR_PIXELS { PIXEL_IJ; const double vv = apply_cols(a.u, p, i, j, h, w); a.v[p] = vv; sv += vv * vv; }
+        alpha = sqrt(grid_sum2(sv, 0, a.part, buf, g).x); buf ^= 1;
+    } else {
+        FOR_PIXELS a.v[p] = 0;
+    }
+    {
+        const double ia = alpha > 0 ? 1 / alpha : 1.0;
+        FOR_PIXELS { const double vv = alpha > 0 ? ia * a.v[p] : a.v[p]; a.v[p] = vv; a.hv[p] = vv; }
+        g.sync();
+    }
+    int itn = 0, istop = 0;
+    double zetabar = alpha * beta, alphabar = alpha, rho = 1, rhobar = 1, cbar = 1, sbar = 0;
+    double betadd = beta, betad = 0, rhodold = 1, tautildeold = 0, thetatilde = 0, zeta = 0, d = 0;
+    double normA2 = alpha * alpha, maxrbar = 0, minrbar = 1e100;
+    double normar = alpha * beta;
+    bool done = normar == 0;
+    if (!done && normb == 0) { FOR_PIXELS a.x[p] = 0; done = true; }
+    while (!done && itn < maxiter) {
+        ++itn;
+        // u = -alpha u + A v
+        double s = 0;
+        FOR_PIXELS {
+            PIXEL_IJ;
+            double ax, ay, al;
+            apply_rows<double>(a.v, p, i, j, h, w, &ax, &ay, &al);
+            const double av[3] = {ax, ay, al};
+            int64_t es[4];
+            int ks[4];
+            const int nr = pixel_rows(p, i, j, h, w, es, ks);
+            for (int q = 0; q < nr; ++q) {
+                const int64_t e = es[q];
+                const int r = ks[q];
+                const double uu = a.rm[e] ? dadd(dmul(a.u[e], -alpha), av[r]) : 0.0;
+                a.u[e] = uu;
+                s += uu * uu;
+            }
+        }
+        beta = sqrt(grid_sum2(s, 0, a.part, buf, g).x); buf ^= 1;
+        if (beta > 0) {
+            const double ib = 1 / beta;
+            FOR_PIXELS { PIXEL_IJ; int64_t es[4]; int ks[4]; const int nr = pixel_rows(p, i, j, h, w, es, ks); for (int q = 0; q < nr; ++q) a.u[es[q]] = dmul(a.u[es[q]], ib); }
+            g.sync();
+            double sv = 0;
+            FOR_PIXELS { PIXEL_IJ; const double vv = dadd(dmul(a.v[p], -beta), apply_cols(a.u, p, i, j, h, w)); a.v[p] = vv; sv += vv * vv; }
+            alpha = sqrt(grid_sum2(sv, 0, a.part, buf, g).x); buf ^= 1;
+        }
+        double chat, shat, alphahat, c, sn;
+        sym_ortho(alphabar, 0.0, &chat, &shat, &alphahat);
+        const double rhoold = rho;
+        sym_ortho(alphahat, beta, &c, &sn, &rho);
+        const double thetanew = sn * alpha;
+        alphabar = c * alpha;
+        const double rhobarold = rhobar, zetaold = zeta, thetabar = sbar * rho, rhotemp = cbar * rho;
+        sym_ortho(cbar * rho, thetanew, &cbar, &sbar, &rhobar);
+        zeta = cbar * zetabar;
+        zetabar = -sbar * zetabar;
+        const double c1 = -(thetabar * rho / (rhoold * rhobarold)), c2 = zeta / (rho * rhobar), c3 = -(thetanew / rho);
+        const bool scale_v = beta > 0 && alpha > 0;
+        const double ia = scale_v ? 1 / alpha : 1.0;
+        double sx = 0;
+        FOR_PIXELS {
+            const double vv = scale_v ? dmul(a.v[p], ia) : a.v[p];
+            a.v[p] = vv;
+            const double hb = dadd(dmul(a.hb[p], c1), a.hv[p]);
+            a.hb[p] = hb;
+            double xx = dadd(a.x[p], dmul(c2, hb));
+            if (x32) xx = static_cast<double>(__double2float_rn(xx));
+            a.x[p] = xx;
+            sx += xx * xx;
+            a.hv[p] = dadd(dmul(a.hv[p], c3), vv);
+        }
+        double normx = sqrt(grid_sum2(sx, 0, a.part, buf, g).x); buf ^= 1;
+        if (x32) normx = static_cast<double>(static_cast<float>(normx));
+        const double betaacute = chat * betadd, betacheck = -shat * betadd, betahat = c * betaacute;
+        betadd = -sn * betaacute;
+        const double thetatildeold = thetatilde;
+        double ctildeold, stildeold, rhotildeold;
+        sym_ortho(rhodold, thetabar, &ctildeold, &stildeold, &rhotildeold);
+        thetatilde = stildeold * rhobar;
+        rhodold = ctildeold * rhobar;
+        betad = -stildeold * betad + ctildeold * betahat;
+        tautildeold = (zetaold - thetatildeold * tautildeold) / rhotildeold;
+        const double taud = (zeta - thetatilde * tautildeold) / rhodold;
+        d = d + betacheck * betacheck;
+        const double normr = sqrt(d + (betad - taud) * (betad - taud) + betadd * betadd);
+        normA2 = normA2 + beta * beta;
+        const double normA = sqrt(normA2);
+        normA2 = normA2 + alpha * alpha;
+        maxrbar = fmax(maxrbar, rhobarold);
+        if (itn > 1) minrbar = fmin(minrbar, rhobarold);
+        const double condA = fmax(maxrbar, rhotemp) / fmin(minrbar, rhotemp);
+        normar = fabs(zetabar);
+        const double test1 = normr / normb;
+        const double test2 = (normA * normr) != 0 ? normar / (normA * normr) : INFINITY;
+        const double test3 = 1 / condA;
+        const double t1 = test1 / (1 + normA * normx / normb);
+        const double rtol = btol + atol * normA * normx / normb;
+        if (itn >= maxiter) istop = 7;
+        if (1 + test3 <= 1) istop = 6;
+        if (1 + test2 <= 1) istop = 5;
+        if (1 + t1 <= 1) istop = 4;
+        if (test3 <= ctol) istop = 3;
+        if (test2 <= atol) istop = 2;
+        if (test1 <= rtol) istop = 1;
+        if (istop > 0) break;
+    }
+    FOR_PIXELS a.depth[p] = x32 ? expf(static_cast<float>(a.x[p])) : __double2float_rn(exp(a.x[p]));
+    if (first == 0) { a.stats[0] = itn; a.stats[1] = istop; }
+#undef FOR_PIXELS
+#undef PIXEL_IJ
+}
+
+__global__ void log_kernel(const float* __restrict__ src, float* __restrict__ dst, int64_t n) {
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
+        dst[p] = logf(src[p]);
+}
+
+// ---------------------------------------------------------------------------------------------------- resizes and points
+// cv2.resize INTER_LINEAR source coordinate of output index d: fp32 (d + 0.5) * in / out - 0.5, clamped at the borders
+__device__ __forceinline__ void lin_coef(int d, int in, int out, int* s0, int* s1, float* f) {
+    float fx = static_cast<float>((d + 0.5) * (1.0 / (static_cast<double>(out) / in)) - 0.5);
+    int sx = static_cast<int>(floorf(fx));
+    fx -= static_cast<float>(sx);
+    if (sx < 0) { fx = 0.f; sx = 0; }
+    if (sx >= in - 1) { fx = 0.f; sx = in - 1; }
+    *s0 = sx; *s1 = min(sx + 1, in - 1); *f = fx;
+}
+
+__global__ void __launch_bounds__(kThreads) resize_kernel(const float* __restrict__ src, int h, int w, int H, int W, float* __restrict__ dst) {
+    const int64_t n = static_cast<int64_t>(H) * W;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
+        int x0, x1, y0, y1;
+        float fx, fy;
+        lin_coef(j, w, W, &x0, &x1, &fx);
+        lin_coef(i, h, H, &y0, &y1, &fy);
+        const float* r0 = src + static_cast<int64_t>(y0) * w;
+        const float* r1 = src + static_cast<int64_t>(y1) * w;
+        const float a0 = 1.f - fx, b0 = 1.f - fy;
+        const float h0 = fadd(fmul(r0[x0], a0), fmul(r0[x1], fx)), h1 = fadd(fmul(r1[x0], a0), fmul(r1[x1], fx));
+        dst[p] = fadd(fmul(h0, b0), fmul(h1, fy));
+    }
+}
+
+// cv2.resize INTER_LINEAR of a 0/1 uint8 mask (11-bit fixed-point coefficients), then > 0; and points = depth * direction
+__global__ void __launch_bounds__(kThreads) finish_kernel(const float* __restrict__ depth, const uint8_t* __restrict__ mask, int h, int w,
+                                                          int H, int W, uint8_t* __restrict__ mask_out, float* __restrict__ points) {
+    const int64_t n = static_cast<int64_t>(H) * W;
+    const double su = 0.5 / W, eu = 1.0 - 0.5 / W, sv = 0.5 / H, ev = 1.0 - 0.5 / H;
+    const double stu = W > 1 ? (eu - su) / (W - 1) : 0.0, stv = H > 1 ? (ev - sv) / (H - 1) : 0.0;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
+        int x0, x1, y0, y1;
+        float fx, fy;
+        lin_coef(j, w, W, &x0, &x1, &fx);
+        lin_coef(i, h, H, &y0, &y1, &fy);
+        const int a1 = __float2int_rn(fx * 2048.f), a0 = __float2int_rn((1.f - fx) * 2048.f);
+        const int b1 = __float2int_rn(fy * 2048.f), b0 = __float2int_rn((1.f - fy) * 2048.f);
+        const uint8_t* m0 = mask + static_cast<int64_t>(y0) * w;
+        const uint8_t* m1 = mask + static_cast<int64_t>(y1) * w;
+        const int r0 = (m0[x0] != 0) * a0 + (m0[x1] != 0) * a1, r1 = (m1[x0] != 0) * a0 + (m1[x1] != 0) * a1;
+        const int val = (((b0 * (r0 >> 4)) >> 16) + ((b1 * (r1 >> 4)) >> 16) + 2) >> 2;
+        mask_out[p] = val > 0;
+        // uv_map(H, W) (np.linspace in fp64, rounded to fp32) and spherical_uv_to_directions in fp32
+        const float u = j == W - 1 ? __double2float_rn(eu) : __double2float_rn(dadd(dmul(static_cast<double>(j), stu), su));
+        const float v = i == H - 1 ? __double2float_rn(ev) : __double2float_rn(dadd(dmul(static_cast<double>(i), stv), sv));
+        const float theta = fmul(1.f - u, 6.28318530717958647692f), phi = fmul(v, 3.14159265358979323846f);
+        const float sp = sinf(phi), d = depth[p];
+        points[p * 3] = fmul(d, fmul(sp, cosf(theta)));
+        points[p * 3 + 1] = fmul(d, fmul(sp, sinf(theta)));
+        points[p * 3 + 2] = fmul(d, cosf(phi));
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------- host side
+int check_device(const char* what, int* sms) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || *sms <= 0)
+        return set_error("%s: no CUDA device: moge_b200 has no CPU fallback", what);
+    return 0;
+}
+
+int check_size(const char* what, int h, int w) {
+    if (h < 2 || w < 2) return set_error("%s: a %d x %d map is too small (at least 2 x 2)", what, h, w);
+    if (static_cast<int64_t>(h) * w > kMaxPixels) return set_error("%s: a %d x %d map is too large (at most 2^28 pixels)", what, h, w);
+    return 0;
+}
+
+int load_cams(const char* what, const moge_panorama_camera_t* cams, int views, Cams* out) {
+    if (!cams) return set_error("%s: null cameras", what);
+    if (views < 1 || views > MOGE_PANORAMA_MAX_VIEWS) return set_error("%s: %d views is outside [1, %d]", what, views, MOGE_PANORAMA_MAX_VIEWS);
+    memset(out, 0, sizeof(*out));
+    for (int k = 0; k < views; ++k) {
+        const moge_panorama_camera_t& c = cams[k];
+        if (!(c.fx != 0) || !(c.fy != 0)) return set_error("%s: view %d has a zero focal length", what, k);
+        out->c[k] = c;
+    }
+    out->n = views;
+    return 0;
+}
+
+unsigned blocks_for(int64_t n, int sms) { return static_cast<unsigned>(std::min<int64_t>((n + kThreads - 1) / kThreads, int64_t(sms) * 16)); }
+
+size_t up(size_t x) { return (x + 255) / 256 * 256; }
+struct Layout { size_t L, M, u, v, hv, hb, x, part, logi, total; };
+Layout layout(int views, int h, int w, int max_blocks) {
+    const size_t n = static_cast<size_t>(h) * w;
+    Layout l;
+    l.L = 0;
+    l.M = l.L + up(views * n * 4);
+    l.u = l.M + up(views * n);
+    l.v = l.u + up((3 * n + h) * 8);
+    l.hv = l.v + up(n * 8);
+    l.hb = l.hv + up(n * 8);
+    l.x = l.hb + up(n * 8);
+    l.part = l.x + up(n * 8);
+    l.logi = l.part + up(static_cast<size_t>(max_blocks) * 4 * 8);
+    l.total = l.logi + up(n * 4);
+    return l;
+}
+constexpr int kMaxLsmrBlocks = 132 * 4;
+
+int check_workspace(const Layout& l, void* ws, size_t bytes, const char* what) {
+    if (!ws || bytes < l.total) return set_error("%s: workspace of %zu bytes needed, %zu given", what, l.total, bytes);
+    if (reinterpret_cast<uintptr_t>(ws) % 256) return set_error("%s: workspace must be 256-byte aligned", what);
+    return 0;
+}
+
+}  // namespace
+}  // namespace mg
+
+using namespace mg;
+
+extern "C" {
+
+int moge_panorama_split(const uint8_t* image, int H, int W, const moge_panorama_camera_t* cams, int views, const float* grid, int res,
+                        float* views_f32, uint8_t* views_u8, void* stream) {
+    if (!image || !grid || !views_f32) return set_error("null argument");
+    MG_TRY(check_size("panorama_split", H, W));
+    if (res < 1 || res > 8192) return set_error("panorama_split: resolution %d is outside [1, 8192]", res);
+    Cams cs;
+    MG_TRY(load_cams("panorama_split", cams, views, &cs));
+    int sms;
+    MG_TRY(check_device("panorama_split", &sms));
+    split_kernel<<<blocks_for(static_cast<int64_t>(views) * res * res, sms), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        image, H, W, cs, grid, res, views_f32, views_u8);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_panorama_workspace_bytes(int views, int h, int w, size_t* bytes) {
+    if (!bytes) return set_error("null argument");
+    MG_TRY(check_size("panorama_workspace_bytes", h, w));
+    if (views < 1 || views > MOGE_PANORAMA_MAX_VIEWS) return set_error("panorama_workspace_bytes: %d views is outside [1, %d]", views, MOGE_PANORAMA_MAX_VIEWS);
+    *bytes = layout(views, h, w, kMaxLsmrBlocks).total;
+    return 0;
+}
+
+int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int views, int vh, int vw, const moge_panorama_camera_t* cams,
+                      const float* directions, int h, int w, double* b, uint8_t* row_mask, uint8_t* pano_mask, void* workspace,
+                      size_t workspace_bytes, void* stream) {
+    if (!src || !mask || !directions || !b || !row_mask || !pano_mask) return set_error("null argument");
+    if (channels != 1 && channels != 3) return set_error("panorama_rhs: %d channels (1: distance, 3: points)", channels);
+    MG_TRY(check_size("panorama_rhs view", vh, vw));
+    MG_TRY(check_size("panorama_rhs", h, w));
+    Cams cs;
+    MG_TRY(load_cams("panorama_rhs", cams, views, &cs));
+    const Layout l = layout(views, h, w, kMaxLsmrBlocks);
+    MG_TRY(check_workspace(l, workspace, workspace_bytes, "panorama_rhs"));
+    int sms;
+    MG_TRY(check_device("panorama_rhs", &sms));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* ws = static_cast<char*>(workspace);
+    float* L = reinterpret_cast<float*>(ws + l.L);
+    uint8_t* M = reinterpret_cast<uint8_t*>(ws + l.M);
+    const int64_t n = static_cast<int64_t>(h) * w;
+    sample_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(src, channels, mask, vh, vw, cs, directions, h, w, L, M);
+    CUDA_TRY(cudaGetLastError());
+    rhs_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(L, M, views, h, w, b, row_mask, pano_mask);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int h, int w, const float* init, float* depth, int32_t* stats,
+                       void* workspace, size_t workspace_bytes, void* stream) {
+    if (!b || !row_mask || !depth || !stats) return set_error("null argument");
+    MG_TRY(check_size("panorama_lsmr", h, w));
+    const Layout l = layout(1, h, w, kMaxLsmrBlocks);
+    MG_TRY(check_workspace(l, workspace, workspace_bytes, "panorama_lsmr"));
+    int sms;
+    MG_TRY(check_device("panorama_lsmr", &sms));
+    int dev = 0, coop = 0, per_sm = 0;
+    CUDA_TRY(cudaGetDevice(&dev));
+    CUDA_TRY(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+    if (!coop) return set_error("panorama_lsmr: the device does not support cooperative launches");
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lsmr_kernel, kLsmrThreads, 0));
+    if (per_sm < 1) return set_error("panorama_lsmr: the solver kernel does not fit on an SM");
+    const int64_t n = static_cast<int64_t>(h) * w;
+    const int blocks = static_cast<int>(std::min<int64_t>({static_cast<int64_t>(sms) * per_sm, (n + kLsmrThreads - 1) / kLsmrThreads,
+                                                           static_cast<int64_t>(kMaxLsmrBlocks)}));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* ws = static_cast<char*>(workspace);
+    Lsmr a;
+    a.b = b; a.rm = row_mask; a.init = nullptr;
+    a.u = reinterpret_cast<double*>(ws + l.u); a.v = reinterpret_cast<double*>(ws + l.v);
+    a.hv = reinterpret_cast<double*>(ws + l.hv); a.hb = reinterpret_cast<double*>(ws + l.hb);
+    a.x = reinterpret_cast<double*>(ws + l.x); a.part = reinterpret_cast<double*>(ws + l.part);
+    a.depth = depth; a.stats = stats; a.h = h; a.w = w;
+    if (init) {                                  // x0 = log(init), fp32
+        float* logi = reinterpret_cast<float*>(ws + l.logi);
+        log_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(init, logi, n);
+        CUDA_TRY(cudaGetLastError());
+        a.init = logi;
+    }
+    void* args[] = {&a};
+    CUDA_TRY(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(lsmr_kernel), dim3(blocks), dim3(kLsmrThreads), args, 0, st));
+    return 0;
+}
+
+int moge_panorama_resize(const float* src, int h, int w, int H, int W, float* dst, void* stream) {
+    if (!src || !dst) return set_error("null argument");
+    MG_TRY(check_size("panorama_resize", h, w));
+    MG_TRY(check_size("panorama_resize", H, W));
+    int sms;
+    MG_TRY(check_device("panorama_resize", &sms));
+    resize_kernel<<<blocks_for(static_cast<int64_t>(H) * W, sms), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(src, h, w, H, W, dst);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_panorama_finish(const float* depth, const uint8_t* mask, int h, int w, int H, int W, float* depth_out, uint8_t* mask_out,
+                         float* points, void* stream) {
+    if (!depth || !mask || !depth_out || !mask_out || !points) return set_error("null argument");
+    MG_TRY(check_size("panorama_finish", h, w));
+    MG_TRY(check_size("panorama_finish", H, W));
+    int sms;
+    MG_TRY(check_device("panorama_finish", &sms));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const unsigned blocks = blocks_for(static_cast<int64_t>(H) * W, sms);
+    resize_kernel<<<blocks, kThreads, 0, st>>>(depth, h, w, H, W, depth_out);
+    CUDA_TRY(cudaGetLastError());
+    finish_kernel<<<blocks, kThreads, 0, st>>>(depth_out, mask, h, w, H, W, mask_out, points);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+}  // extern "C"

@@ -1,0 +1,306 @@
+"""Panorama inference on the GPU: the reference's `moge/scripts/infer_panorama.py:83-122` without file I/O, and the device side of
+its `moge/utils/panorama.py`.
+
+An equirectangular panorama is split into 12 perspective views (one camera per icosahedron vertex, 90 x 90 degrees), the views go
+through one `model.infer(views, fov_x=..., apply_mask=False)` call, and the views' log-distances are merged back into a panorama
+by a gradient-domain least-squares solve (SciPy's LSMR on a 4-level pyramid at up to 1920 x 960), then resized to the input.
+
+The work runs in moge_b200/csrc/panorama.cu: a split kernel that samples the uint8 panorama as cv2.remap does, a per-level
+right-hand-side pass that reads log |points| straight from the engine's output, a matrix-free LSMR in one cooperative kernel
+per level, and the resizes.  A merge never waits on the host.  The panorama ray table of each merge size is the reference's own
+numpy float32 trigonometry (`spherical_uv_to_directions`), computed once per size and kept on the device, so the projections
+see bitwise the reference's rays.  CUDA tensors only; there is no CPU fallback.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import Dict, List, Optional, Sequence, Tuple
+
+import numpy as np
+import torch
+
+from . import capi
+from .capi import MogeError
+
+__all__ = ["get_panorama_cameras", "spherical_uv_to_directions", "directions_to_spherical_uv", "uv_map", "split_panorama",
+           "merge_panorama", "finish_panorama", "infer_panorama", "last_merge_stats", "SPLIT_RESOLUTION"]
+
+SPLIT_RESOLUTION = 512                 # infer_panorama.py:90
+MERGE_WIDTH, MERGE_HEIGHT = 1920, 960  # infer_panorama.py:117
+PYRAMID_SIZE = 256                     # panorama.py:106: a level recurses while max(w, h) > 256
+MAX_PIXELS = 1 << 28
+
+
+# ------------------------------------------------------------------------------------------------------------ host geometry
+def _icosahedron_vertices() -> np.ndarray:
+    A = (1 + 5 ** 0.5) / 2
+    return np.array([[0, 1, A], [0, -1, A], [0, 1, -A], [0, -1, -A], [1, A, 0], [-1, A, 0], [1, -A, 0], [-1, -A, 0],
+                     [A, 0, 1], [A, 0, -1], [-A, 0, 1], [-A, 0, -1]], dtype=np.float32)
+
+
+def _look_at(eye, look_at, up) -> np.ndarray:
+    """OpenCV world-to-camera extrinsics: z towards look_at, x = -up x z, y = z x x."""
+    eye, look_at, up = np.asarray(eye), np.asarray(look_at), np.asarray(up)
+    z = look_at - eye
+    x = np.cross(-up, z)
+    y = np.cross(z, x)
+    x = x / np.linalg.norm(x, axis=-1, keepdims=True)
+    y = y / np.linalg.norm(y, axis=-1, keepdims=True)
+    z = z / np.linalg.norm(z, axis=-1, keepdims=True)
+    R = np.stack([x, y, z], axis=-2)
+    E = np.zeros(R.shape[:-2] + (4, 4), dtype=R.dtype)
+    E[..., :3, :3] = R
+    E[..., :3, 3] = -(R * eye[..., None, :]).sum(axis=-1)
+    E[..., 3, 3] = 1
+    return E
+
+
+def get_panorama_cameras():
+    """The reference's 12 cameras: (extrinsics (12, 4, 4) float32, [intrinsics (3, 3) float64] * 12), 90 x 90 degrees."""
+    vertices = _icosahedron_vertices()
+    fx = 0.5 / np.tan(np.deg2rad(90) / 2)
+    intrinsics = np.array([[fx, 0, 0.5], [0, fx, 0.5], [0, 0, 1]], dtype=np.float64)
+    extrinsics = _look_at([0, 0, 0], vertices, [0, 0, 1]).astype(np.float32)
+    return extrinsics, [intrinsics] * len(vertices)
+
+
+def uv_map(height: int, width: int) -> np.ndarray:
+    """Pixel-centre UV grid (height, width, 2) float32."""
+    u = np.linspace(0.5 / width, 1 - 0.5 / width, width, dtype=np.float32)
+    v = np.linspace(0.5 / height, 1 - 0.5 / height, height, dtype=np.float32)
+    u, v = np.meshgrid(u, v, indexing='xy')
+    return np.stack([u, v], axis=2)
+
+
+def spherical_uv_to_directions(uv: np.ndarray) -> np.ndarray:
+    """panorama.py:27-30."""
+    theta, phi = (1 - uv[..., 0]) * (2 * np.pi), uv[..., 1] * np.pi
+    return np.stack([np.sin(phi) * np.cos(theta), np.sin(phi) * np.sin(theta), np.cos(phi)], axis=-1)
+
+
+def directions_to_spherical_uv(directions: np.ndarray) -> np.ndarray:
+    """panorama.py:33-37."""
+    directions = directions / np.linalg.norm(directions, axis=-1, keepdims=True)
+    u = 1 - np.arctan2(directions[..., 1], directions[..., 0]) / (2 * np.pi) % 1.0
+    v = np.arccos(directions[..., 2]) / np.pi
+    return np.stack([u, v], axis=-1)
+
+
+def _cameras(extrinsics, intrinsics) -> Tuple[C.Array, int]:
+    extrinsics = np.asarray(extrinsics, dtype=np.float32)
+    intrinsics = np.asarray(intrinsics, dtype=np.float64)
+    if extrinsics.ndim != 3 or extrinsics.shape[1:] not in ((4, 4), (3, 4)):
+        raise MogeError(f"extrinsics must be (N, 4, 4), not {extrinsics.shape}")
+    n = extrinsics.shape[0]
+    if intrinsics.shape != (n, 3, 3):
+        raise MogeError(f"intrinsics must be {n} (3, 3) matrices, not {intrinsics.shape}")
+    if not 1 <= n <= capi.PANORAMA_MAX_VIEWS:
+        raise MogeError(f"{n} views is outside [1, {capi.PANORAMA_MAX_VIEWS}]")
+    cams = (capi.PanoramaCamera * n)()
+    for k in range(n):
+        cams[k].R[:] = [float(v) for v in extrinsics[k, :3, :3].reshape(-1)]
+        cams[k].t[:] = [float(v) for v in extrinsics[k, :3, 3]]
+        K = intrinsics[k]
+        cams[k].fx, cams[k].fy, cams[k].cx, cams[k].cy = float(K[0, 0]), float(K[1, 1]), float(K[0, 2]), float(K[1, 2])
+    return cams, n
+
+
+_default_cams = None
+_tables: Dict[tuple, torch.Tensor] = {}
+
+
+def _default_cameras():
+    global _default_cams
+    if _default_cams is None:
+        _default_cams = get_panorama_cameras()
+    return _default_cams
+
+
+def _table(kind: str, size: Tuple[int, int], device: torch.device) -> torch.Tensor:
+    """Device copies of host tables, made once per size: the split grid (uv_map's fp32 coordinates) and the panorama rays."""
+    key = (kind, size, device)
+    t = _tables.get(key)
+    if t is None:
+        if kind == "grid":
+            arr = uv_map(1, size[0])[0, :, 0]
+        else:
+            arr = spherical_uv_to_directions(uv_map(*size)).astype(np.float32)
+        t = torch.from_numpy(np.ascontiguousarray(arr)).to(device)
+        _tables[key] = t
+    return t
+
+
+def _check_size(what: str, h: int, w: int) -> None:
+    if h < 2 or w < 2 or h * w > MAX_PIXELS:
+        raise MogeError(f"{what}: a {h} x {w} map is outside [2 x 2, 2^28 pixels]")
+
+
+def _check_cuda(what: str, *ts) -> None:
+    for t in ts:
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise MogeError(f"{what}: expected a CUDA tensor (moge_b200 has no CPU fallback)")
+
+
+# ------------------------------------------------------------------------------------------------------------ split
+def split_panorama(image: torch.Tensor, extrinsics=None, intrinsics=None, resolution: int = SPLIT_RESOLUTION,
+                   return_uint8: bool = False):
+    """split_panorama_image on the device: image (H, W, 3) uint8 RGB CUDA tensor -> views (N, 3, res, res) float32 (value / 255,
+    the tensor infer_panorama.py:98 builds), and with return_uint8 also the uint8 views (N, res, res, 3).  Cameras default to
+    get_panorama_cameras()."""
+    if not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3:
+        raise MogeError("split_panorama: image must be a (H, W, 3) uint8 tensor")
+    H, W = image.shape[:2]
+    _check_size("split_panorama", H, W)
+    _check_cuda("split_panorama", image)
+    if not 1 <= int(resolution) <= 8192:
+        raise MogeError(f"split_panorama: resolution {resolution} is outside [1, 8192]")
+    res = int(resolution)
+    if extrinsics is None:
+        extrinsics, intrinsics = _default_cameras()
+    cams, n = _cameras(extrinsics, intrinsics)
+    dev = image.device
+    with torch.cuda.device(dev):
+        img = image.contiguous()
+        out = torch.empty(n, 3, res, res, dtype=torch.float32, device=dev)
+        u8 = torch.empty(n, res, res, 3, dtype=torch.uint8, device=dev) if return_uint8 else None
+        grid = _table("grid", (res, res), dev)
+        capi.check(capi.lib().moge_panorama_split(img.data_ptr(), H, W, cams, n, grid.data_ptr(), res, out.data_ptr(), capi.ptr(u8),
+                                                  capi.current_stream()))
+    return (out, u8) if return_uint8 else out
+
+
+# ------------------------------------------------------------------------------------------------------------ merge
+def _levels(width: int, height: int) -> List[Tuple[int, int]]:
+    sizes = [(width, height)]
+    while max(sizes[-1]) > PYRAMID_SIZE:
+        sizes.append((sizes[-1][0] // 2, sizes[-1][1] // 2))
+    return sizes[::-1]
+
+
+_last: Dict[str, object] = {}
+
+
+def num_rows(h: int, w: int) -> int:
+    """Rows of a level's system: x-gradient h*w, y-gradient (h-1) x (w+1) on the reference's x-wrapped grid (column w repeats
+    column 0), Laplacian h*w."""
+    return 2 * h * w + (h - 1) * (w + 1)
+
+
+def merge_panorama(width: int, height: int, src: torch.Tensor, mask: torch.Tensor, extrinsics=None, intrinsics=None,
+                   return_levels: bool = False):
+    """merge_panorama_depth on the device: src (N, vh, vw) distance maps, or (N, vh, vw, 3) point maps whose norms are the
+    distances (the engine's `points`), mask (N, vh, vw) bool / uint8.  Returns (depth (height, width) float32, mask (height, width)
+    bool).  With return_levels, also per level (coarsest first) a dict of its size, the fp64 right-hand side, the uint8 row mask in
+    the reference's row order (see num_rows) and the solver's fp32 depth.  The per-level iteration
+    counts and istop values are in last_merge_stats()."""
+    width, height = int(width), int(height)
+    _check_size("merge_panorama", height, width)
+    if not isinstance(src, torch.Tensor) or src.dtype != torch.float32 or src.dim() not in (3, 4) or (src.dim() == 4 and src.shape[3] != 3):
+        raise MogeError("merge_panorama: src must be float32 (N, vh, vw) distances or (N, vh, vw, 3) points")
+    if not isinstance(mask, torch.Tensor) or tuple(mask.shape) != tuple(src.shape[:3]) or mask.dtype not in (torch.bool, torch.uint8):
+        raise MogeError(f"merge_panorama: mask must be bool / uint8 of shape {tuple(src.shape[:3])}")
+    _check_cuda("merge_panorama", src, mask)
+    n, vh, vw = src.shape[:3]
+    _check_size("merge_panorama view", vh, vw)
+    if extrinsics is None:
+        extrinsics, intrinsics = _default_cameras()
+    cams, nc = _cameras(extrinsics, intrinsics)
+    if nc != n:
+        raise MogeError(f"merge_panorama: {n} views but {nc} cameras")
+    channels = 1 if src.dim() == 3 else 3
+    dev = src.device
+    L = capi.lib()
+    levels = _levels(width, height)
+    with torch.cuda.device(dev):
+        st = capi.current_stream()
+        s = src.detach().contiguous()
+        m = mask.detach().contiguous().view(torch.uint8) if mask.dtype == torch.bool else (mask != 0).contiguous().view(torch.uint8)
+        nbytes = C.c_size_t()
+        capi.check(L.moge_panorama_workspace_bytes(n, height, width, C.byref(nbytes)))
+        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        stats = torch.zeros(len(levels), 2, dtype=torch.int32, device=dev)
+        depth, init, out = None, None, []
+        for lv, (w, h) in enumerate(levels):
+            b = torch.empty(num_rows(h, w), dtype=torch.float64, device=dev)
+            rm = torch.empty(num_rows(h, w), dtype=torch.uint8, device=dev)
+            pm = torch.empty(h, w, dtype=torch.uint8, device=dev)
+            dirs = _table("dirs", (h, w), dev)
+            capi.check(L.moge_panorama_rhs(s.data_ptr(), channels, m.data_ptr(), n, vh, vw, cams, dirs.data_ptr(), h, w, b.data_ptr(),
+                                           rm.data_ptr(), pm.data_ptr(), ws.data_ptr(), ws.numel(), st))
+            depth = torch.empty(h, w, dtype=torch.float32, device=dev)
+            capi.check(L.moge_panorama_lsmr(b.data_ptr(), rm.data_ptr(), h, w, capi.ptr(init), depth.data_ptr(), stats[lv].data_ptr(),
+                                            ws.data_ptr(), ws.numel(), st))
+            if return_levels:
+                out.append({"width": w, "height": h, "b": b, "row_mask": rm, "depth": depth})
+            if lv + 1 < len(levels):
+                W2, H2 = levels[lv + 1]
+                init = torch.empty(H2, W2, dtype=torch.float32, device=dev)
+                capi.check(L.moge_panorama_resize(depth.data_ptr(), h, w, H2, W2, init.data_ptr(), st))
+    _last.update(levels=levels, stats=stats)
+    result = (depth, pm.view(torch.bool))
+    return (*result, out) if return_levels else result
+
+
+def last_merge_stats() -> List[Dict[str, int]]:
+    """Per level of the most recent merge_panorama call on this thread's process, coarsest first: width, height, LSMR iterations
+    and istop (SciPy's stopping reason).  Reading them copies the counters to the host."""
+    if not _last:
+        return []
+    stats = _last["stats"].cpu().tolist()
+    return [{"width": w, "height": h, "iterations": it, "istop": st} for (w, h), (it, st) in zip(_last["levels"], stats)]
+
+
+def finish_panorama(depth: torch.Tensor, mask: torch.Tensor, height: int, width: int):
+    """infer_panorama.py:119-122: the merged depth and mask resized to (height, width) as cv2.resize does, and the points."""
+    _check_cuda("finish_panorama", depth, mask)
+    if depth.dtype != torch.float32 or depth.dim() != 2 or tuple(mask.shape) != tuple(depth.shape):
+        raise MogeError("finish_panorama: depth must be float32 (h, w) and mask (h, w)")
+    h, w = depth.shape
+    _check_size("finish_panorama", h, w)
+    _check_size("finish_panorama", height, width)
+    dev = depth.device
+    with torch.cuda.device(dev):
+        d = depth.contiguous()
+        m = mask.contiguous().view(torch.uint8) if mask.dtype == torch.bool else (mask != 0).to(torch.uint8)
+        out_d = torch.empty(height, width, dtype=torch.float32, device=dev)
+        out_m = torch.empty(height, width, dtype=torch.uint8, device=dev)
+        points = torch.empty(height, width, 3, dtype=torch.float32, device=dev)
+        capi.check(capi.lib().moge_panorama_finish(d.data_ptr(), m.data_ptr(), h, w, height, width, out_d.data_ptr(), out_m.data_ptr(),
+                                                   points.data_ptr(), capi.current_stream()))
+    return out_d, out_m.view(torch.bool), points
+
+
+# ------------------------------------------------------------------------------------------------------------ end to end
+def _fov_x(intrinsics, device) -> torch.Tensor:
+    """infer_panorama.py:99-100: the views' horizontal fields of view in degrees, float32."""
+    K = np.asarray(intrinsics)
+    fov_x = np.rad2deg(2 * np.arctan(0.5 / K[..., 0, 0]))
+    return torch.tensor(fov_x, dtype=torch.float32, device=device)
+
+
+def infer_panorama(model, image: torch.Tensor, batch_size: Optional[int] = None) -> Dict[str, torch.Tensor]:
+    """infer_panorama.py:83-122 without file I/O.  image: (H, W, 3) uint8 RGB CUDA tensor; model: an engine MoGeModel (MoGe-1 as in
+    the reference, or MoGe-2) on the same device.  The 12 views go through one `model.infer(views, fov_x=..., apply_mask=False)`
+    call, or calls of batch_size views (the reference's --batch_size).  Returns device tensors {'depth' (H, W), 'mask' (H, W) bool,
+    'points' (H, W, 3)}."""
+    if batch_size is not None and int(batch_size) < 1:
+        raise MogeError(f"infer_panorama: batch_size {batch_size} must be positive")
+    if not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3:
+        raise MogeError("infer_panorama: image must be a (H, W, 3) uint8 tensor")
+    _check_cuda("infer_panorama", image)
+    H, W = image.shape[:2]
+    _check_size("infer_panorama", H, W)
+    extrinsics, intrinsics = _default_cameras()
+    views = split_panorama(image, extrinsics, intrinsics, SPLIT_RESOLUTION)
+    fov_x = _fov_x(intrinsics, image.device)
+    step = len(views) if batch_size is None else int(batch_size)
+    points, masks = [], []
+    for lo in range(0, len(views), step):
+        out = model.infer(views[lo:lo + step], fov_x=fov_x[lo:lo + step], apply_mask=False)
+        points.append(out['points'])
+        masks.append(out['mask'])
+    points = points[0] if len(points) == 1 else torch.cat(points)
+    masks = masks[0] if len(masks) == 1 else torch.cat(masks)
+    depth, mask = merge_panorama(min(MERGE_WIDTH, W), min(MERGE_HEIGHT, H), points, masks, extrinsics, intrinsics)
+    depth, mask, points = finish_panorama(depth, mask, H, W)
+    return {'depth': depth, 'mask': mask, 'points': points}

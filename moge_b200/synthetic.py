@@ -480,3 +480,64 @@ def synthetic_mesh_case(seed: int, B: int, H: int, W: int):
         out["intrinsics"].append(torch.tensor([[fx, 0, 0.5], [0, fy, 0.5], [0, 0, 1]], dtype=torch.float32))
         images.append(torch.randint(0, 256, (H, W, 3), generator=g, dtype=torch.uint8))
     return {k: torch.stack(v) for k, v in out.items()}, torch.stack(images)
+
+
+# ------------------------------------------------------------------------------------------------------------ panorama
+PANORAMA_ROOM_LO, PANORAMA_ROOM_HI = (-2.0, -3.0, -1.2), (4.0, 2.5, 1.8)      # box walls around the panorama's centre
+
+
+def synthetic_panorama(H: int, W: int, seed: int = 0):
+    """(H, W, 3) uint8 RGB panorama (numpy): smooth colour, a grid of lines crossing the seam, coloured seam columns, bright / dark
+    caps at the poles, seeded noise."""
+    import numpy as np
+    rs = np.random.RandomState(seed)
+    i, j = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
+    img = np.stack([128 + 100 * np.sin(2 * np.pi * j / W * 3 + c) * np.cos(np.pi * i / H * 2 + c) for c in range(3)], -1)
+    img[(j % 17 < 2) | (i % 13 < 2)] = [250, 20, 60]
+    img[:, :3] = [0, 255, 0]
+    img[:, -3:] = [0, 0, 255]
+    img[:max(2, H // 20)] = [230, 230, 230]
+    img[-max(2, H // 20):] = [10, 10, 10]
+    img = img + rs.randint(-20, 21, img.shape)
+    return np.clip(img, 0, 255).astype(np.uint8)
+
+
+def synthetic_room_views(res: int, seed: int = 7):
+    """Distance maps (12, res, res) float32 and masks (12, res, res) bool (numpy) of a box room seen from an off-centre point
+    through the 12 panorama cameras: the exact distance along each pixel's ray times (1 + 0.01 noise), three round holes per view
+    (radius res / 24 to res / 8) where the mask is off and the distance is tripled.  fp64 elementwise arithmetic, so the same
+    seed gives the same bits on any host with the same numpy."""
+    import numpy as np
+    from .panorama import get_panorama_cameras, uv_map
+    extr, intr = get_panorama_cameras()
+    lo, hi = np.array(PANORAMA_ROOM_LO), np.array(PANORAMA_ROOM_HI)
+    rs = np.random.RandomState(seed)
+    uv = uv_map(res, res).astype(np.float64)
+    ii, jj = np.meshgrid(np.arange(res), np.arange(res), indexing="ij")
+    dist, masks = [], []
+    for k in range(len(extr)):
+        K, R = intr[k], extr[k, :3, :3].astype(np.float64)
+        c = ((uv[..., 0] - K[0, 2]) / K[0, 0], (uv[..., 1] - K[1, 2]) / K[1, 1], np.ones((res, res)))
+        d = np.stack([R[0, r] * c[0] + R[1, r] * c[1] + R[2, r] * c[2] for r in range(3)], -1)
+        with np.errstate(divide="ignore", invalid="ignore"):
+            t = np.where(d > 0, hi / d, np.where(d < 0, lo / d, np.inf)).min(-1)
+        dd = t * np.sqrt((d * d).sum(-1)) * (1 + 0.01 * rs.randn(res, res))
+        m = np.ones((res, res), bool)
+        for _ in range(3):
+            ci, cj = rs.randint(0, res, 2)
+            r = rs.randint(res // 24, res // 8)
+            m &= (ii - ci) ** 2 + (jj - cj) ** 2 > r * r
+        dd[~m] *= 3.0
+        dist.append(dd.astype(np.float32))
+        masks.append(m)
+    return np.stack(dist), np.stack(masks)
+
+
+def array_digest(*arrays) -> str:
+    """SHA-256 of the arrays' bytes, in order (C order)."""
+    import hashlib
+    import numpy as np
+    h = hashlib.sha256()
+    for a in arrays:
+        h.update(np.ascontiguousarray(a).tobytes())
+    return h.hexdigest()
