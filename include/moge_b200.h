@@ -306,6 +306,17 @@ int moge_mesh_workspace_bytes(int64_t batch, int H, int W, size_t* bytes);
  * uint8 = edge, or keep & !edge when keep is given (the cleaned mask).                                                       */
 int moge_depth_edge(const float* depth, const uint8_t* mask, const uint8_t* keep, int64_t batch, int H, int W, int kernel_size,
                     const float* atol, const float* rtol, uint8_t* out, void* stream);
+/* point_map_to_normal_map (oracle/utils3d_normals.py, bitwise): points (batch, H, W, 3) fp32 -> normal (batch, H, W, 3), the
+ * normalised sum of the four normalised neighbour cross products whose neighbours and centre are in mask (zero points off the
+ * image; NULL mask: every product, including those against the zero padding).  With a mask, normals are 0 where no product is
+ * valid.  normal_mask (batch, H, W) uint8 (may be NULL) = some product valid.                                               */
+int moge_normal_map(const float* points, const uint8_t* mask, int64_t batch, int H, int W, float* normal, uint8_t* normal_mask, void* stream);
+/* normal_map_edge: the largest arccos of the dot product of a pixel's normal with those of its kernel_size window (3, 5 or 7,
+ * edge-padded; with mask, 0 where the window pixel is off it), max-pooled over the same window (NaN propagates), is compared
+ * as fp64: edge = angle > tol (radians).  With and_edge (batch, H, W) uint8, edge &= and_edge; out (batch, H, W) uint8 = edge, or
+ * keep & !edge when keep is given.  angle (may be NULL) receives the pooled fp32 angle map.  At most 65535 * 32 rows.      */
+int moge_normal_edge(const float* normals, const uint8_t* mask, const uint8_t* and_edge, const uint8_t* keep, int64_t batch, int H, int W,
+                     int kernel_size, double tol, uint8_t* out, float* angle, void* stream);
 /* count pass: a quad (top-left pixel (i, j)) is kept when its four corners are in the mask (NULL: every quad), a vertex when a
  * kept quad uses it.  totals (batch, 4) int64 on the device = (vertices, quads, first vertex row, first quad) of each image in
  * the batch-wide outputs.                                                                                                   */

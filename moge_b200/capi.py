@@ -30,7 +30,7 @@ EXPORTS = [
     "moge_engine_create_v1", "moge_v1_workspace_bytes", "moge_v1_forward", "moge_v1_postprocess", "moge_op_resize_bicubic_aa",
     "moge_op_groupnorm_relu", "moge_bicubic_aa_weights", "moge_op_conv_transpose_uv",
     "moge_metrics_workspace_bytes", "moge_metrics_resize", "moge_metrics_stats", "moge_metrics_eval", "moge_metrics_boundary",
-    "moge_mesh_workspace_bytes", "moge_depth_edge", "moge_mesh_count", "moge_mesh_build",
+    "moge_mesh_workspace_bytes", "moge_depth_edge", "moge_mesh_count", "moge_mesh_build", "moge_normal_map", "moge_normal_edge",
     "moge_panorama_split", "moge_panorama_workspace_bytes", "moge_panorama_rhs", "moge_panorama_lsmr", "moge_panorama_resize",
     "moge_panorama_finish",
 ]
@@ -169,6 +169,8 @@ def lib() -> C.CDLL:
     L.moge_depth_edge.argtypes = [vp, vp, vp, i64, ci, ci, ci, fp, fp, vp, vp]
     L.moge_mesh_count.argtypes = [vp, i64, ci, ci, vp, vp, sz, vp]
     L.moge_mesh_build.argtypes = [vp, i64, ci, ci, ci, C.POINTER(MeshMap), ci, vp, vp, vp, sz, vp]
+    L.moge_normal_map.argtypes = [vp, vp, i64, ci, ci, vp, vp, vp]
+    L.moge_normal_edge.argtypes = [vp, vp, vp, vp, i64, ci, ci, ci, C.c_double, vp, vp, vp]
     pc = C.POINTER(PanoramaCamera)
     L.moge_panorama_split.argtypes = [vp, ci, ci, pc, ci, vp, ci, vp, vp, vp]
     L.moge_panorama_workspace_bytes.argtypes = [ci, ci, ci, C.POINTER(sz)]

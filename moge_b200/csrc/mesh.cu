@@ -1,5 +1,7 @@
 // Mesh export (moge/scripts/infer.py:124-150 of the reference): utils3d's depth_map_edge and build_mesh_from_map, restated in
-// oracle/utils3d_mesh.py, which these kernels match bit for bit.
+// oracle/utils3d_mesh.py, which these kernels match bit for bit.  The panorama export (moge/scripts/infer_panorama.py:136-150)
+// adds point_map_to_normal_map and normal_map_edge, restated in oracle/utils3d_normals.py: the normals match it bit for bit, the
+// normal edges up to acosf's rounding (at most 2 ulp, as numpy's arccos) at angles within a few ulp of the threshold.
 //
 // depth_map_edge: one CTA per 32 x 32 output tile with a halo of kernel_size / 2, a separable NaN-propagating window max of the
 // depth and of its negation (masked-out and out-of-image pixels are -inf), then diff = max(d) + max(-d) and the two tolerance
@@ -72,6 +74,117 @@ __global__ void __launch_bounds__(kThreads) edge_kernel(const float* __restrict_
         if (has_atol) edge |= diff > atol;
         if (has_rtol) edge |= __fdiv_rn(diff, depth[p]) > rtol;
         out[p] = keep ? static_cast<uint8_t>(keep[p] && !edge) : static_cast<uint8_t>(edge);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------- normals
+// Vector helpers with one fp32 rounding per operation, in numpy's order (oracle/utils3d_normals.py): no contraction into FMAs.
+struct F3 { float x, y, z; };
+__device__ __forceinline__ F3 load3(const float* __restrict__ p, int64_t e) { return {p[e * 3], p[e * 3 + 1], p[e * 3 + 2]}; }
+__device__ __forceinline__ F3 sub3(F3 a, F3 b) { return {__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z)}; }
+__device__ __forceinline__ F3 add3(F3 a, F3 b) { return {__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y), __fadd_rn(a.z, b.z)}; }
+__device__ __forceinline__ F3 scale3(F3 a, float s) { return {__fmul_rn(a.x, s), __fmul_rn(a.y, s), __fmul_rn(a.z, s)}; }
+// np.cross: component a1 * b2 - a2 * b1, both products rounded
+__device__ __forceinline__ F3 cross3(F3 a, F3 b) {
+    return {__fsub_rn(__fmul_rn(a.y, b.z), __fmul_rn(a.z, b.y)), __fsub_rn(__fmul_rn(a.z, b.x), __fmul_rn(a.x, b.z)),
+            __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x))};
+}
+// (a0 * b0 + a1 * b1) + a2 * b2
+__device__ __forceinline__ float dot3(F3 a, F3 b) { return __fadd_rn(__fadd_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)), __fmul_rn(a.z, b.z)); }
+// n / (sqrt((x^2 + y^2) + z^2) + 1e-12)
+__device__ __forceinline__ F3 normalize3(F3 n) {
+    const float d = __fadd_rn(__fsqrt_rn(dot3(n, n)), 1e-12f);
+    return {__fdiv_rn(n.x, d), __fdiv_rn(n.y, d), __fdiv_rn(n.z, d)};
+}
+
+// point_map_to_normal_map: grid (pixel blocks, images), one thread per pixel.  Neighbours outside the image are zero points off
+// the mask; without a mask every product counts.  normal_mask (may be NULL) = any product valid.
+__global__ void __launch_bounds__(kThreads) normal_map_kernel(const float* __restrict__ pts, const uint8_t* __restrict__ mask, int H, int W,
+                                                              float* __restrict__ normal, uint8_t* __restrict__ normal_mask) {
+    const int64_t hw = static_cast<int64_t>(H) * W, p = static_cast<int64_t>(blockIdx.x) * kThreads + threadIdx.x;
+    if (p >= hw) return;
+    const int64_t e = static_cast<int64_t>(blockIdx.y) * hw + p;
+    const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
+    const bool hu = i > 0, hl = j > 0, hd = i + 1 < H, hr = j + 1 < W;
+    const F3 zero = {0.f, 0.f, 0.f}, c = load3(pts, e);
+    const F3 up = sub3(hu ? load3(pts, e - W) : zero, c), left = sub3(hl ? load3(pts, e - 1) : zero, c);
+    const F3 down = sub3(hd ? load3(pts, e + W) : zero, c), right = sub3(hr ? load3(pts, e + 1) : zero, c);
+    bool v0 = true, v1 = true, v2 = true, v3 = true;
+    if (mask) {
+        const bool mc = mask[e], mu = hu && mask[e - W], ml = hl && mask[e - 1], md = hd && mask[e + W], mr = hr && mask[e + 1];
+        v0 = mc && mu && ml; v1 = mc && ml && md; v2 = mc && md && mr; v3 = mc && mr && mu;
+    }
+    // (n * valid).sum(0): multiplied by 0.0 / 1.0, not selected, so a NaN in an invalid product still propagates
+    F3 s = scale3(normalize3(cross3(up, left)), v0 ? 1.f : 0.f);
+    s = add3(s, scale3(normalize3(cross3(left, down)), v1 ? 1.f : 0.f));
+    s = add3(s, scale3(normalize3(cross3(down, right)), v2 ? 1.f : 0.f));
+    s = add3(s, scale3(normalize3(cross3(right, up)), v3 ? 1.f : 0.f));
+    s = normalize3(s);
+    const bool any = v0 || v1 || v2 || v3;
+    if (mask && !any) s = zero;
+    normal[e * 3] = s.x;
+    normal[e * 3 + 1] = s.y;
+    normal[e * 3 + 2] = s.z;
+    if (normal_mask) normal_mask[e] = any;
+}
+
+// normal_map_edge: one CTA per 32 x 32 output tile.  The normals (normalised, edge-padded by clamping) and the edge-padded mask
+// of the tile with a 2r halo go to shared memory; the window-max angle map is formed on the tile with an r halo (-inf outside
+// the image: the pool's padding), then pooled separably.  NaN propagates through both maxima and is never an edge.  The edge
+// is angle > tol compared in fp64; with and_edge it is ANDed with that map, and with keep the output is keep & ~edge.
+constexpr int kNrmS = kEdgeT + 4 * kMaxR;
+__global__ void __launch_bounds__(kThreads) normal_edge_kernel(const float* __restrict__ normals, const uint8_t* __restrict__ mask,
+                                                               const uint8_t* __restrict__ and_edge, const uint8_t* __restrict__ keep, int H,
+                                                               int W, int r, double tol, uint8_t* __restrict__ out, float* __restrict__ angle) {
+    __shared__ float s_n[3][kNrmS][kNrmS];
+    __shared__ uint8_t s_m[kNrmS][kNrmS];
+    __shared__ float s_a[kEdgeS][kEdgeS];      // window-max angles
+    __shared__ float s_h[kEdgeS][kEdgeT];      // row-pass maxima
+    const int64_t b = blockIdx.z, hw = static_cast<int64_t>(H) * W;
+    const int i0 = blockIdx.y * kEdgeT, j0 = blockIdx.x * kEdgeT, SN = kEdgeT + 4 * r, SA = kEdgeT + 2 * r, k = 2 * r + 1;
+    for (int t = threadIdx.x; t < SN * SN; t += kThreads) {
+        const int li = t / SN, lj = t % SN;
+        const int i = min(max(i0 - 2 * r + li, 0), H - 1), j = min(max(j0 - 2 * r + lj, 0), W - 1);
+        const int64_t p = b * hw + static_cast<int64_t>(i) * W + j;
+        const F3 n = normalize3(load3(normals, p));
+        s_n[0][li][lj] = n.x;
+        s_n[1][li][lj] = n.y;
+        s_n[2][li][lj] = n.z;
+        s_m[li][lj] = mask ? mask[p] != 0 : 1;
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < SA * SA; t += kThreads) {
+        const int ai = t / SA, aj = t % SA, i = i0 - r + ai, j = j0 - r + aj;
+        float a = -INFINITY;
+        if (i >= 0 && i < H && j >= 0 && j < W) {
+            const F3 c = {s_n[0][ai + r][aj + r], s_n[1][ai + r][aj + r], s_n[2][ai + r][aj + r]};
+            for (int di = 0; di < k; ++di)
+                for (int dj = 0; dj < k; ++dj) {
+                    const int li = ai + di, lj = aj + dj;
+                    const float x = s_m[li][lj] ? acosf(dot3(c, {s_n[0][li][lj], s_n[1][li][lj], s_n[2][li][lj]})) : 0.f;
+                    a = nan_max(a, x);
+                }
+        }
+        s_a[ai][aj] = a;
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < SA * kEdgeT; t += kThreads) {
+        const int li = t / kEdgeT, oj = t % kEdgeT;
+        float a = s_a[li][oj];
+        for (int d = 1; d < k; ++d) a = nan_max(a, s_a[li][oj + d]);
+        s_h[li][oj] = a;
+    }
+    __syncthreads();
+    for (int t = threadIdx.x; t < kEdgeT * kEdgeT; t += kThreads) {
+        const int oi = t / kEdgeT, oj = t % kEdgeT, i = i0 + oi, j = j0 + oj;
+        if (i >= H || j >= W) continue;
+        float a = s_h[oi][oj];
+        for (int d = 1; d < k; ++d) a = nan_max(a, s_h[oi + d][oj]);
+        const int64_t p = b * hw + static_cast<int64_t>(i) * W + j;
+        bool edge = static_cast<double>(a) > tol;
+        if (and_edge) edge = edge && and_edge[p];
+        out[p] = keep ? static_cast<uint8_t>(keep[p] && !edge) : static_cast<uint8_t>(edge);
+        if (angle) angle[p] = a;
     }
 }
 
@@ -310,6 +423,32 @@ int moge_depth_edge(const float* depth, const uint8_t* mask, const uint8_t* keep
     const dim3 grid((W + kEdgeT - 1) / kEdgeT, (H + kEdgeT - 1) / kEdgeT, static_cast<unsigned>(batch));
     edge_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(depth, mask, keep, H, W, kernel_size / 2, atol ? *atol : 0.f,
                                                                           atol != nullptr, rtol ? *rtol : 0.f, rtol != nullptr, out);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_normal_map(const float* points, const uint8_t* mask, int64_t batch, int H, int W, float* normal, uint8_t* normal_mask, void* stream) {
+    if (!points || !normal) return set_error("null argument");
+    MG_TRY(check_shape("point_map_to_normal_map", batch, H, W));
+    MG_TRY(check_device("point_map_to_normal_map"));
+    const int64_t blocks = (static_cast<int64_t>(H) * W + kThreads - 1) / kThreads;
+    normal_map_kernel<<<dim3(static_cast<unsigned>(blocks), static_cast<unsigned>(batch)), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        points, mask, H, W, normal, normal_mask);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_normal_edge(const float* normals, const uint8_t* mask, const uint8_t* and_edge, const uint8_t* keep, int64_t batch, int H, int W,
+                     int kernel_size, double tol, uint8_t* out, float* angle, void* stream) {
+    if (!normals || !out) return set_error("null argument");
+    MG_TRY(check_shape("normal_map_edge", batch, H, W));
+    if (kernel_size < 3 || kernel_size > 2 * kMaxR + 1 || kernel_size % 2 == 0)
+        return set_error("normal_map_edge: kernel_size %d is not one of 3, 5, 7", kernel_size);
+    if ((H + kEdgeT - 1) / kEdgeT > 65535) return set_error("normal_map_edge: %d rows is more than %d", H, 65535 * kEdgeT);
+    MG_TRY(check_device("normal_map_edge"));
+    const dim3 grid((W + kEdgeT - 1) / kEdgeT, (H + kEdgeT - 1) / kEdgeT, static_cast<unsigned>(batch));
+    normal_edge_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(normals, mask, and_edge, keep, H, W, kernel_size / 2, tol,
+                                                                                out, angle);
     CUDA_TRY(cudaGetLastError());
     return 0;
 }

@@ -6,8 +6,13 @@ emit passes for the vertex rows and the faces.  A mesh call copies one small buf
 and waits for it (the only synchronisation of a call, for the whole batch), allocates exact-size outputs as views of one
 allocation and launches the emit passes.  Results are bitwise those of the numpy restatement in oracle/utils3d_mesh.py.
 
+The panorama script's export (moge/scripts/infer_panorama.py:136-150) adds utils3d's `point_map_to_normal_map` and
+`normal_map_edge` and is `mesh_from_panorama`: a normal-map kernel and a normal-edge kernel whose fused form writes the cleaned
+mask, then the same count and emit passes.  The normals are bitwise those of oracle/utils3d_normals.py; the normal edges may
+differ only where an angle is within a few ulp of the threshold (acosf against numpy's arccos).
+
 CUDA tensors only; there is no CPU fallback.  Divergences from utils3d: faces are int32 (utils3d returns intp), and attribute
-maps must be fp32 (uint8 colours go through `mesh_from_output`).
+maps must be fp32 (uint8 colours go through `mesh_from_output` / `mesh_from_panorama`).
 """
 from __future__ import annotations
 
@@ -20,7 +25,8 @@ import torch
 from . import capi
 from .capi import MogeError
 
-__all__ = ["depth_map_edge", "build_mesh_from_map", "build_mesh_from_map_batch", "mesh_from_output"]
+__all__ = ["depth_map_edge", "build_mesh_from_map", "build_mesh_from_map_batch", "mesh_from_output", "point_map_to_normal_map",
+           "normal_map_edge", "mesh_from_panorama"]
 
 MAX_PIXELS = 1 << 30           # per image: vertex ids and triangle counts stay below 2^31
 KERNEL_SIZES = (3, 5, 7)
@@ -268,3 +274,106 @@ def mesh_from_output(output: Dict[str, torch.Tensor], image: torch.Tensor, thres
         r["mask_cleaned"] = cleaned[b].view(torch.bool)
         results.append(r)
     return results if batched else results[0]
+
+
+# ------------------------------------------------------------------------------------------------------------ normals
+def _normal_map(points: torch.Tensor, mask: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(B, H, W, 3) fp32 points, (B, H, W) uint8 mask or None -> (normals, uint8 normal mask)."""
+    B, H, W = points.shape[:3]
+    normal = torch.empty(B, H, W, 3, dtype=torch.float32, device=points.device)
+    nmask = torch.empty(B, H, W, dtype=torch.uint8, device=points.device)
+    capi.check(capi.lib().moge_normal_map(points.data_ptr(), capi.ptr(mask), B, H, W, normal.data_ptr(), nmask.data_ptr(),
+                                          capi.current_stream()))
+    return normal, nmask
+
+
+def _normal_edge(normals: torch.Tensor, mask: Optional[torch.Tensor], and_edge: Optional[torch.Tensor], keep: Optional[torch.Tensor],
+                 tol: float, kernel_size: int, angle: Optional[torch.Tensor] = None) -> torch.Tensor:
+    B, H, W = normals.shape[:3]
+    out = torch.empty(B, H, W, dtype=torch.uint8, device=normals.device)
+    capi.check(capi.lib().moge_normal_edge(normals.data_ptr(), capi.ptr(mask), capi.ptr(and_edge), capi.ptr(keep), B, H, W,
+                                           int(kernel_size), float(np.deg2rad(tol)), out.data_ptr(), capi.ptr(angle),
+                                           capi.current_stream()))
+    return out
+
+
+def _check_normal_args(what: str, points: torch.Tensor, mask: Optional[torch.Tensor]) -> Tuple[int, int]:
+    if not isinstance(points, torch.Tensor) or points.dim() < 3 or points.shape[-1] != 3:
+        raise MogeError(f"{what}: expected a (..., H, W, 3) tensor")
+    if mask is not None and (not isinstance(mask, torch.Tensor) or tuple(mask.shape) != tuple(points.shape[:-1])):
+        raise MogeError(f"{what}: mask {tuple(getattr(mask, 'shape', ()))} does not match the map {tuple(points.shape[:-1])}")
+    H, W = points.shape[-3:-1]
+    _check_size(H, W)
+    _check_cuda(points, mask)
+    return H, W
+
+
+def point_map_to_normal_map(points: torch.Tensor, mask: torch.Tensor = None, edge_threshold: float = None):
+    """utils3d's point_map_to_normal_map on a (..., H, W, 3) fp32 point map: per pixel the normalised sum of the four normalised
+    cross products up x left, left x down, down x right, right x up of the neighbour differences (no wrap at the borders).  With
+    `mask` (..., H, W), a product counts when its two neighbours and the centre are in the mask, and (normals, normal_mask bool)
+    is returned, normals 0 off normal_mask; without, every product counts, border ones against zero points, and only the normals
+    are returned.  Bitwise the restatement in oracle/utils3d_normals.py.  edge_threshold is not supported."""
+    if edge_threshold is not None:
+        raise MogeError("point_map_to_normal_map: edge_threshold is not supported")
+    H, W = _check_normal_args("point_map_to_normal_map", points, mask)
+    p = _f32(points, "points").reshape(-1, H, W, 3)
+    m = None if mask is None else _mask_u8(mask).reshape(-1, H, W)
+    if p.shape[0] == 0:
+        normal, nmask = torch.zeros_like(p), torch.zeros(p.shape[:3], dtype=torch.uint8, device=p.device)
+    else:
+        normal, nmask = _normal_map(p, m)
+    normal = normal.reshape(points.shape)
+    if mask is None:
+        return normal
+    return normal, nmask.view(torch.bool).reshape(mask.shape)
+
+
+def normal_map_edge(normals: torch.Tensor, tol: float, kernel_size: int = 3, mask: torch.Tensor = None) -> torch.Tensor:
+    """utils3d's normal_map_edge on (..., H, W, 3) fp32 normals: True where the largest angle between a normal and those of its
+    kernel_size window (edge-padded; with `mask`, only the window's masked-in pixels), max-pooled over the same window, exceeds
+    `tol` degrees.  A dot product beyond [-1, 1] gives a NaN angle, which the pooling spreads and which is never an edge.
+    kernel_size is 3, 5 or 7."""
+    if kernel_size not in KERNEL_SIZES:
+        raise MogeError(f"normal_map_edge: kernel_size {kernel_size} is not one of 3, 5, 7")
+    H, W = _check_normal_args("normal_map_edge", normals, mask)
+    n = _f32(normals, "normals").reshape(-1, H, W, 3)
+    m = None if mask is None else _mask_u8(mask).reshape(-1, H, W)
+    if n.shape[0] == 0:
+        return torch.zeros(normals.shape[:-1], dtype=torch.bool, device=normals.device)
+    return _normal_edge(n, m, None, None, tol, kernel_size).view(torch.bool).reshape(normals.shape[:-1])
+
+
+# ------------------------------------------------------------------------------------------------------------ after infer_panorama()
+PANORAMA_NORMAL_TOL = 5.0       # infer_panorama.py:142: normal_map_edge(normals, tol=5, ...)
+
+
+def mesh_from_panorama(output: Dict[str, torch.Tensor], image: torch.Tensor, threshold: float = 0.03) -> Dict[str, torch.Tensor]:
+    """infer_panorama.py:136-144 in one call: from infer_panorama()'s output (points (H, W, 3), depth (H, W), mask (H, W)) and the
+    (H, W, 3) uint8 panorama.  The mask is cleaned where a depth edge (rtol=threshold; inf: none) and a 5-degree normal edge
+    coincide, mask & ~(depth_map_edge(depth, rtol=threshold) & normal_map_edge(normals, tol=5, mask=normals_mask)) with
+    (normals, normals_mask) = point_map_to_normal_map(points, mask), and the mesh is built with colours image / 255 and the
+    pixel-centre UVs.  No OpenGL flips, as the panorama script applies none.
+
+    Returns a dict of `faces` (int32 triangles), `vertices`, `vertex_colors`, `vertex_uvs` and `mask_cleaned`, ready for
+    save_glb(path, vertices, faces, vertex_uvs, image) and save_ply(path, vertices, faces, vertex_colors).  One host wait."""
+    points, depth, mask = output["points"], output["depth"], output["mask"]
+    if not isinstance(depth, torch.Tensor) or depth.dim() != 2:
+        raise MogeError("mesh_from_panorama: depth must be a (H, W) tensor")
+    H, W = depth.shape
+    for name, t, want in (("points", points, (H, W, 3)), ("mask", mask, (H, W)), ("image", image, (H, W, 3))):
+        if not isinstance(t, torch.Tensor) or tuple(t.shape) != want:
+            raise MogeError(f"mesh_from_panorama: {name} has shape {tuple(getattr(t, 'shape', ()))}, expected {want}")
+    if image.dtype != torch.uint8:
+        raise MogeError(f"mesh_from_panorama: image must be uint8, not {image.dtype}")
+    _check_size(H, W)
+    _check_cuda(points, depth, mask, image)
+    d = _f32(depth, "depth")[None]
+    p = _f32(points, "points")[None]
+    m = _mask_u8(mask)[None]
+    depth_edge = _edge(d, None, None, None, threshold, 3)
+    normals, nmask = _normal_map(p, m)
+    cleaned = _normal_edge(normals, nmask, depth_edge, m, PANORAMA_NORMAL_TOL, 3)
+    maps = [_Map(p, capi.MESH_F32, 3), _Map(image.contiguous(), capi.MESH_U8_UNIT, 3), _Map(None, capi.MESH_UV, 2)]
+    faces, vertices, colours, uvs = _mesh(cleaned, 1, H, W, maps, True, d.device)[0]
+    return {"faces": faces, "vertices": vertices, "vertex_colors": colours, "vertex_uvs": uvs, "mask_cleaned": cleaned[0].view(torch.bool)}

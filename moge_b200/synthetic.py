@@ -533,6 +533,38 @@ def synthetic_room_views(res: int, seed: int = 7):
     return np.stack(dist), np.stack(masks)
 
 
+def synthetic_panorama_scene(H: int, W: int, seed: int = 0):
+    """An analytic infer_panorama()-style output for mesh_from_panorama, numpy: the box room of PANORAMA_ROOM_LO / HI seen from its
+    origin, with a box standing on the floor in front of a wall (its position from the seed) occluding part of it.  Returns
+    points (H, W, 3) float32 = depth * the panorama rays, depth (H, W) float32 (the exact fp64 distance, rounded), mask (H, W)
+    bool (off in four seeded round holes and at the pole rows) and image (H, W, 3) uint8 (synthetic_panorama).  The room's
+    corners are normal edges, the box's silhouette is a depth and normal edge, and the holes cut the mask."""
+    import numpy as np
+    from .panorama import spherical_uv_to_directions, uv_map
+    rs = np.random.RandomState(seed)
+    dirs = spherical_uv_to_directions(uv_map(H, W)).astype(np.float32)
+    d = dirs.astype(np.float64)
+    lo, hi = np.array(PANORAMA_ROOM_LO), np.array(PANORAMA_ROOM_HI)
+    x0, y0 = 1.2 + 0.8 * rs.rand(), -1.5 + 1.5 * rs.rand()
+    blo, bhi = np.array([x0, y0, lo[2]]), np.array([x0 + 1.0, y0 + 1.2, lo[2] + 1.1 + 0.4 * rs.rand()])
+    with np.errstate(divide="ignore", invalid="ignore"):
+        t = np.where(d > 0, hi / d, np.where(d < 0, lo / d, np.inf)).min(-1)
+        a, b = blo / d, bhi / d
+        near, far = np.minimum(a, b).max(-1), np.maximum(a, b).min(-1)
+    hit = (near <= far) & (near > 0)
+    t = np.where(hit, np.minimum(t, near), t)
+    depth = t.astype(np.float32)
+    points = depth[..., None] * dirs
+    ii, jj = np.meshgrid(np.arange(H), np.arange(W), indexing="ij")
+    mask = np.ones((H, W), bool)
+    for _ in range(4):
+        ci, cj, r = rs.randint(0, H), rs.randint(0, W), rs.randint(max(1, H // 40), max(2, H // 12))
+        mask &= (ii - ci) ** 2 + (jj - cj) ** 2 > r * r
+    mask[:max(1, H // 64)] = False
+    mask[-max(1, H // 64):] = False
+    return points, depth, mask, synthetic_panorama(H, W, seed)
+
+
 def array_digest(*arrays) -> str:
     """SHA-256 of the arrays' bytes, in order (C order)."""
     import hashlib
