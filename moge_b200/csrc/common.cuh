@@ -92,6 +92,20 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
         : "memory");
 }
 
+// TMA tensor store from shared memory (one bulk async-group per commit of the issuing thread).  The smem box must be made
+// visible to the async proxy (fence_proxy_async by every writing thread, then a barrier) before the store is issued.
+__device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
+    asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                 : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// at most N of this thread's bulk groups still read their shared-memory source
+template <int N> __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+// at most N of this thread's bulk groups still pending (writes done)
+template <int N> __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
 // ------------------------------------------------------------------------------------------------ wgmma
 // Shared-memory matrix descriptor (sm_90 wgmma), 128-byte swizzle: dense [rows][64 x 16-bit] tiles as written by a SWIZZLE_128B
 // TMA box with a 128-byte inner extent, 8-row groups `sbo_bytes` apart.  Tile base must be 1024-byte aligned.

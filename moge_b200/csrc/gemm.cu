@@ -31,7 +31,7 @@ int gemm_linear(GemmLaunch* g, bool bf16, const void* A, int M, int K, const voi
     g->bn = bn; g->mode = MODE_GEMM; g->amode = AMODE_ROWS; g->epi = epi; g->df = -1; g->bf16 = bf16; g->p = p;
     MG_TRY(make_map_2d(&g->a, A, K, M, K, TILE_M));
     MG_TRY(make_map_2d(&g->b, W, K, N, ldw, bn));
-    g->aux = g->a;
+    g->aux = g->o0 = g->o1 = g->a;
     return 0;
 }
 
@@ -70,6 +70,11 @@ int gemm_conv(GemmLaunch* g, bool bf16, const ConvW& cw, const void* src, const 
     if (cw.caux) MG_TRY(make_map_nhwc(&g->aux, aux, cw.caux, gs.Wp, gs.Hp, B, 8));
     else g->aux = g->a;
     MG_TRY(make_map_2d(&g->b, cw.w, cw.Ktot, cw.N, cw.Ktot, bn));
+    g->o0 = g->o1 = g->a;
+    if (dec_direct(mode, epi, g->df)) {        // the epilogue's TMA stores: one box = 64 channels x 16 px x 4 rows
+        if (out_raw) MG_TRY(make_map_nhwc(&g->o0, out_raw, out_ch, go.Wp, go.Hp, B, 4));
+        if (out_relu) MG_TRY(make_map_nhwc(&g->o1, out_relu, out_ch, go.Wp, go.Hp, B, 4));
+    }
     return 0;
 }
 

@@ -5,7 +5,8 @@
 //
 // Roles (warpgroup-uniform): warpgroup 0 = TMA producer (one elected lane of warp 0), warpgroups 1 and 2 = consumers:
 // each issues the wgmma of its 64 rows of the 128-row tile, then all eight consumer warps run the epilogue (warp ew owns
-// rows 32 (ew & 3) .. +31; with 8 epilogue warps the two warps of a row quarter split the columns).
+// rows 32 (ew & 3) .. +31; with 8 epilogue warps the two warps of a row quarter split the columns).  The dec_direct variants
+// skip the staging: each consumer warpgroup stores its own 64 rows from its registers (dec_direct_epilogue).
 //
 // Three main loops share the kernel (MODE):
 //   MODE_GEMM   one stage = one 64-wide K block of A (row tile, or one filter tap's pixel window) and of B.
@@ -84,16 +85,24 @@ inline int dec_flags(const GemmParams& p) {
     return (p.out0 ? DF_RAW : 0) | (p.out1 ? DF_RELU : 0) | (p.skip ? DF_SKIP : 0) | (p.vec1 ? DF_UV : 0) | (p.shuffle ? DF_SHUFFLE : 0);
 }
 
+// The EPI_DEC variants whose consumer warpgroups finish their own rows straight from the accumulator registers (16-bit boxes in
+// shared memory -> TMA tensor stores; dec_direct_epilogue): the compile-time masks of the halo conv modes without pixel shuffle.
+// Every other epilogue stages the fp32 accumulator tile in shared memory first.
+__host__ __device__ constexpr bool dec_direct(int mode, int epi, int df) {
+    return mode != MODE_GEMM && epi == EPI_DEC && df >= 0 && (df & DF_SHUFFLE) == 0;
+}
+
 // One launch of gemm_kernel as gemm_linear / gemm_conv (gemm.cu) choose it: the kernel variant, its tensor maps and params.
 struct GemmLaunch {
     int bn, mode, amode, epi;
     int df;                    // EPI_DEC: the compile-time DF mask of the variant, or -1 (run-time flags)
     bool bf16;
     CUtensorMap a, aux, b;     // A operand, aux A operand (fused 1x1 input block), weights
+    CUtensorMap o0, o1;        // dec_direct variants: store maps of the raw and ReLU outputs (boxes {64 ch, 16 px, 4 rows})
     GemmParams p;
 };
 
-template <int BN, int MODE = MODE_GEMM> struct GemmCfg {
+template <int BN, int MODE = MODE_GEMM, bool DIRECT = false> struct GemmCfg {
     static constexpr int kHaloBytes = 160 * 128;                 // box {64 ch, 16 px, 10 rows}
     static constexpr int kABytes = (MODE == MODE_GEMM) ? TILE_M * 128 : kHaloBytes;
     static constexpr int kBBytes = (MODE == MODE_GEMM) ? BN * 128 : (MODE == MODE_CONVH) ? 3 * BN * 128 : 0;
@@ -102,8 +111,13 @@ template <int BN, int MODE = MODE_GEMM> struct GemmCfg {
     // accumulator tile staged for the epilogue: 32 x 32 fp32 blocks, [row quarter][column chunk]; float4 (r, q) of a block at
     // r * 8 + (q ^ (r & 7)) -- a lane reads its row conflict-free, 8 lanes x float4 read one row of the block conflict-free
     static constexpr int kChunks = (BN < 32) ? 1 : BN / 32;
-    static constexpr int kAccBytes = TILE_M * kChunks * 32 * 4;
-    static constexpr int kFixedBytes = kAccBytes + kResidentBytes + 1024 /*align slack*/ + 256 /*barriers*/;
+    static constexpr int kAccBytes = DIRECT ? 0 : TILE_M * kChunks * 32 * 4;
+    // DIRECT: kOutBufs 16-bit output boxes {64 ch, 16 px, 4 rows} (8 KB, 128B-swizzled) per consumer warpgroup.  One box keeps
+    // the output staging at 16 KB, which is what lets MODE_CONVH fit a third ring stage.
+    static constexpr int kOutBoxBytes = 64 * 64 * 2;
+    static constexpr int kOutBufs = 1;
+    static constexpr int kOutBytes = DIRECT ? 2 * kOutBufs * kOutBoxBytes : 0;
+    static constexpr int kFixedBytes = kAccBytes + kOutBytes + kResidentBytes + 1024 /*align slack*/ + 256 /*barriers*/;
     static constexpr int kFit = (kMaxDynSmem - kFixedBytes) / kStageBytes;
     static constexpr int kStages = kFit > 8 ? 8 : kFit;
     static constexpr int kEpiWarps = (BN >= 64) ? 8 : 4;
@@ -113,6 +127,7 @@ template <int BN, int MODE = MODE_GEMM> struct GemmCfg {
     static_assert(kStages >= 2, "gemm_kernel: fewer than two ring stages fit beside the accumulator tile");
     static_assert(kSmemBytes <= kMaxDynSmem, "gemm_kernel: stage ring + accumulator tile exceed the shared memory of one CTA");
     static_assert((2 * kStages + 1) * 8 <= 256, "gemm_kernel: barrier block overflows its 256 bytes");
+    static_assert(!DIRECT || BN % 64 == 0, "gemm_kernel: the direct EPI_DEC epilogue stores whole 64-channel boxes");
 };
 
 // Block of the staged accumulator tile holding rows 32 quarter .. +31, columns col .. col + 31 (col a multiple of 32).
@@ -327,6 +342,137 @@ __device__ __forceinline__ void epilogue_dec16(const GemmParams& p, int mt, int 
     }
 }
 
+// Direct EPI_DEC epilogue (dec_direct variants).  Consumer warpgroup g owns output rows y0 + 4 g .. +3 of the 8x16 pixel tile; in
+// the accumulator fragment a thread (warp wl, lane) holds image row y0 + 4 g + wl, columns x0 + lane / 4 (h = 0) and + 8 (h = 1),
+// channel pairs 8 (i / 4) + 2 (lane % 4) of the tile.  DecPix is that thread's view of the two pixels.
+struct DecPix {
+    int b, y0, x0, y;
+    bool interior;         // every pixel of the tile inside the image, none on its border: TMA stores, no replication
+    bool ok[2];            // pixel h inside the image
+    size_t off[2];         // byte offset of pixel h (channel 0) in the padded NHWC maps
+};
+__device__ __forceinline__ DecPix dec_pix(const GemmParams& p, int mt, int g, int wl, int lane) {
+    const TileOrigin org = tile_origin(p, mt);
+    DecPix d;
+    d.b = org.b; d.y0 = org.y0; d.x0 = org.x0;
+    d.y = org.y0 + 4 * g + wl;
+    d.interior = org.y0 > 0 && org.x0 > 0 && org.y0 + TILE_PH < p.H && org.x0 + TILE_PW < p.W;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+        const int x = org.x0 + (lane >> 2) + 8 * h;
+        d.ok[h] = d.y < p.H && x < p.W;
+        d.off[h] = ((static_cast<size_t>(org.b) * p.Hop + d.y + 1) * p.Wop + x + 1) * p.ldo * 2;
+    }
+    return d;
+}
+
+// The skip operand in the fragment layout (one packed channel pair per accumulator pair), loaded at the start of a tile so that
+// its latency hides behind the tile's MMAs.
+template <int BN>
+__device__ __forceinline__ void dec_skip_load(const GemmParams& p, const DecPix& d, int nt, int lane, uint32_t (&sk)[BN / 4]) {
+    const uint8_t* base = static_cast<const uint8_t*>(p.skip) + (static_cast<size_t>(nt) * BN + 2 * (lane & 3)) * 2;
+#pragma unroll
+    for (int k = 0; k < BN / 4; ++k) {
+        const int h = k & 1;
+        sk[k] = (d.interior || d.ok[h]) ? *reinterpret_cast<const uint32_t*>(base + d.off[h] + (k >> 1) * 16) : 0u;
+    }
+}
+
+// Epilogue of one consumer warpgroup from its accumulators, in the fp32 order of epilogue_dec16 (bias, skip, UV term): the
+// values are packed into 16-bit {64 ch, 16 px, 4 rows} boxes in shared memory (128B swizzle, the layout of the store map) and
+// each box leaves with one TMA tensor store (interior tiles) or through the replicating per-pixel stores (edge tiles).  A
+// warpgroup barrier (id 2 + g) orders the box writes against the previous reader of the buffer and the store against the writes;
+// `nbox` counts the boxes this warpgroup has issued (buffer nbox % OUTBUFS).
+template <int BN, bool BF16, int DF, int OUTBUFS>
+__device__ __forceinline__ void dec_direct_epilogue(const GemmParams& p, const CUtensorMap* map0, const CUtensorMap* map1,
+                                                    const DecPix& d, int nt, float (&acc)[BN / 2], const uint32_t* sk,
+                                                    uint8_t* sOut, int g, int wl, int lane, int& nbox) {
+    using H = H16<BF16>;
+    constexpr bool has_raw = (DF & DF_RAW) != 0, has_relu = (DF & DF_RELU) != 0;
+    constexpr bool has_skip = (DF & DF_SKIP) != 0, has_uv = (DF & DF_UV) != 0;
+    const float* bias = p.bias + nt * BN + 2 * (lane & 3);
+    float uu[2], vv[2];
+    if (has_uv) {
+        const float inv_wo = 1.0f / static_cast<float>(p.Wo), inv_ho = 1.0f / static_cast<float>(p.Ho);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int X = d.x0 + (lane >> 2) + 8 * h, Y = d.y;
+            uu[h] = p.su * ((2 * X + 1) * inv_wo - 1.0f);
+            vv[h] = p.sv * ((2 * Y + 1) * inv_ho - 1.0f);
+        }
+    }
+    auto finish = [&](int half) {       // the values of channels 64 half .. +63, in place
+#pragma unroll
+        for (int k = 16 * half; k < 16 * half + 16; ++k) {
+            const int h = k & 1, c = 8 * (k >> 1);
+            const float2 bb = *reinterpret_cast<const float2*>(bias + c);
+            float a0 = acc[2 * k] + bb.x, a1 = acc[2 * k + 1] + bb.y;
+            if (has_skip) {
+                const float2 s = H::unpack(sk[k]);
+                a0 += s.x; a1 += s.y;
+            }
+            if (has_uv) {
+                const float2 gu = *reinterpret_cast<const float2*>(p.vec1 + nt * BN + c + 2 * (lane & 3));
+                const float2 gv = *reinterpret_cast<const float2*>(p.vec2 + nt * BN + c + 2 * (lane & 3));
+                // spelled out as epilogue_dec16's `g * uu + h * vv` compiles there (the compiler contracts the other product
+                // here when left to choose, which changes the last bit)
+                a0 += __fmaf_rn(gu.x, uu[h], __fmul_rn(gv.x, vv[h]));
+                a1 += __fmaf_rn(gu.y, uu[h], __fmul_rn(gv.y, vv[h]));
+                // (at most 8 columns of wu / wv loads in flight beside the 64 accumulators)
+                if ((k & 3) == 3) asm volatile("" ::: "memory");
+            }
+            acc[2 * k] = a0; acc[2 * k + 1] = a1;
+        }
+    };
+    const int tid = wl * 32 + lane;
+    const bool leader = tid == 0;
+    auto box = [&](int half, bool relu) {
+        uint8_t* sb = sOut + (nbox % OUTBUFS) * GemmCfg<64>::kOutBoxBytes;
+        ++nbox;
+        if (leader) bulk_wait_read<OUTBUFS - 1>();     // the store that last read this buffer is done with it
+        named_sync(2 + g, 128);                         // ... and so is every thread of the edge path
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int k = 2 * (8 * half + j) + h;
+                float a0 = acc[2 * k], a1 = acc[2 * k + 1];
+                if (relu) { a0 = fmaxf(a0, 0.f); a1 = fmaxf(a1, 0.f); }
+                const int R = 16 * wl + (lane >> 2) + 8 * h;          // box row (pixel); R & 7 == lane >> 2
+                *reinterpret_cast<uint32_t*>(sb + R * 128 + ((j ^ (lane >> 2)) << 4) + 4 * (lane & 3)) = H::pack(a0, a1);
+            }
+        fence_proxy_async();
+        named_sync(2 + g, 128);
+        const int c0 = nt * BN + 64 * half;
+        if (d.interior) {
+            if (leader) {
+                tma_store_4d(relu ? map1 : map0, sb, c0, d.x0 + 1, d.y0 + 4 * g + 1, d.b);
+                bulk_commit();
+            }
+            return;
+        }
+        // edge tile: per-pixel 16-byte stores of the valid pixels, replicating the border ones into the padding
+        uint8_t* out = static_cast<uint8_t*>(relu ? p.out1 : p.out0);
+#pragma unroll
+        for (int r = 0; r < 4; ++r) {
+            const int idx = tid + 128 * r, R = idx >> 3, j = idx & 7;
+            const uint4 q = *reinterpret_cast<const uint4*>(sb + R * 128 + ((j ^ (R & 7)) << 4));
+            const int Y = d.y0 + 4 * g + (R >> 4), X = d.x0 + (R & 15);
+            if (Y >= p.H || X >= p.W) continue;
+            const int co = c0 + 8 * j;
+            *reinterpret_cast<uint4*>(out + ((static_cast<size_t>(d.b) * p.Hop + Y + 1) * p.Wop + X + 1) * p.ldo * 2 + co * 2) = q;
+            if (Y == 0 || Y == p.H - 1 || X == 0 || X == p.W - 1)
+                store_px_border16(out, d.b, Y, X, p.Ho, p.Wo, p.Hop, p.Wop, p.ldo, co, q);
+        }
+    };
+    // one 64-channel half at a time: the barriers of its boxes keep the compiler from hoisting the next half's operand loads
+#pragma unroll
+    for (int half = 0; half < BN / 64; ++half) {
+        finish(half);
+        if (has_raw) box(half, false);
+        if (has_relu) box(half, true);
+    }
+}
 
 // EPI_HEADOUT epilogue: lane = low-resolution pixel, 16 B (or 4 B) per lane, consecutive lanes = consecutive pixels of a tile row.
 template <int BN>
@@ -519,16 +665,19 @@ __device__ __forceinline__ void epilogue_rows(const GemmParams& p, int mt, int n
 template <int BN, int MODE, int AMODE, int EPI, bool BF16, int DF = -1>
 __global__ void __launch_bounds__(384, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAux,
-            const __grid_constant__ CUtensorMap mapB, const GemmParams p) {
+            const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapO0,
+            const __grid_constant__ CUtensorMap mapO1, const GemmParams p) {
     static_assert(AMODE == AMODE_ROWS || EPI == EPI_DEC || EPI == EPI_HEADOUT || EPI == EPI_NECKOUT,
                   "gemm_kernel: a pixel-tile A operand pairs only with the decoder epilogues (DEC, HEADOUT, NECKOUT)");
     pdl_launch_dependents();      // (the wait sits after the barrier set-up below: that prologue overlaps the previous kernel's tail)
-    using Cfg = GemmCfg<BN, MODE>;
+    constexpr bool DIRECT = dec_direct(MODE, EPI, DF);
+    using Cfg = GemmCfg<BN, MODE, DIRECT>;
     constexpr int S = Cfg::kStages;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    float4* stg = reinterpret_cast<float4*>(smem + S * Cfg::kStageBytes);
-    uint8_t* sW = smem + S * Cfg::kStageBytes + Cfg::kAccBytes;         // MODE_CONV64: resident weights
+    float4* stg = reinterpret_cast<float4*>(smem + S * Cfg::kStageBytes);            // staged epilogues: fp32 accumulator tile
+    uint8_t* sOut = smem + S * Cfg::kStageBytes + Cfg::kAccBytes;                     // DIRECT: 16-bit output boxes
+    uint8_t* sW = sOut + Cfg::kOutBytes;                                               // MODE_CONV64: resident weights
     uint64_t* full = reinterpret_cast<uint64_t*>(sW + Cfg::kResidentBytes);
     uint64_t* empty = full + S;
     uint64_t* wfull = empty + S;
@@ -638,6 +787,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
         const bool ln_on = AMODE == AMODE_ROWS && (EPI == EPI_STORE16 || EPI == EPI_GELU16) && p.ln_rstd != nullptr;
         if (ln_on && static_cast<int>(blockIdx.x) < total_tiles) ln_load(p, static_cast<int>(blockIdx.x) / p.num_n_tiles, quarter, lane, lnn);
         int s = 0; uint32_t ph = 0;
+        int nbox = 0;                                   // DIRECT: output boxes this warpgroup has issued
+        // stages per tile with the 3x3 taps; the rest read the aux source (fused 1x1 input block)
+        const int ntap_stage = (MODE == MODE_GEMM) ? nstage : (MODE == MODE_CONV64) ? 3 : 3 * p.kb_main;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int mt = tile / p.num_n_tiles, nt = tile % p.num_n_tiles;
             if (ln_on) {        // rstd of this tile's rows (loaded one iteration ago); then issue the next tile's loads
@@ -645,37 +797,28 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
                 const int nxt = tile + static_cast<int>(gridDim.x);
                 if (nxt < total_tiles) ln_load(p, nxt / p.num_n_tiles, quarter, lane, lnn);
             }
+            DecPix dp{};
+            uint32_t sk[DIRECT && (DF & DF_SKIP) ? BN / 4 : 1];
+            if constexpr (DIRECT) {
+                dp = dec_pix(p, mt, g, wl, lane);
+                if constexpr ((DF & DF_SKIP) != 0) dec_skip_load<BN>(p, dp, nt, lane, sk);
+            }
             float acc[BN / 2];
 #pragma unroll
             for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
             int prev = -1;
-            for (int i = 0; i < nstage; ++i) {
+            auto mma64 = [&](uint32_t a, uint32_t bb) {          // one 64-wide K block
+                const uint64_t ad = make_sdesc_sw128(a), bd = make_sdesc_sw128(bb);
+#pragma unroll
+                for (int k = 0; k < TILE_K / 16; ++k) Wgmma<BN, BF16>::ss(acc, ad + 2 * k, bd + 2 * k, 1u);
+            };
+            // one ring stage: wait for it, issue its MMAs (body(A, B) at the stage's smem addresses), release the previous one.
+            // The tap stages and the aux stages run in separate loops, so that no wgmma sits under a branch of the loop body
+            // (ptxas would serialise the wgmma of a divergent path).
+            auto stage = [&](auto body) {
                 mbar_wait(&full[s], ph);
-                const uint32_t sa = smem_u32(smem + s * Cfg::kStageBytes) + a_off;
-                const uint32_t sb = smem_u32(smem + s * Cfg::kStageBytes + Cfg::kABytes);
                 wgmma_fence();
-                auto mma64 = [&](uint32_t a, uint32_t bb) {          // one 64-wide K block
-                    const uint64_t ad = make_sdesc_sw128(a), bd = make_sdesc_sw128(bb);
-#pragma unroll
-                    for (int k = 0; k < TILE_K / 16; ++k) Wgmma<BN, BF16>::ss(acc, ad + 2 * k, bd + 2 * k, 1u);
-                };
-                if (MODE == MODE_GEMM) {
-                    mma64(sa, sb);
-                } else if (MODE == MODE_CONV64) {
-                    if (i < 3) {
-#pragma unroll
-                        for (int dy = 0; dy < 3; ++dy) mma64(sa + dy * TILE_PW * 128, w0 + (dy * 3 + i) * BN * 128);
-                    } else {
-                        mma64(sa, w0 + 9 * BN * 128);
-                    }
-                } else {
-                    if (i < 3 * p.kb_main) {
-#pragma unroll
-                        for (int dy = 0; dy < 3; ++dy) mma64(sa + dy * TILE_PW * 128, sb + dy * BN * 128);
-                    } else {
-                        mma64(sa, sb);
-                    }
-                }
+                body(smem_u32(smem + s * Cfg::kStageBytes) + a_off, smem_u32(smem + s * Cfg::kStageBytes + Cfg::kABytes));
                 wgmma_commit();
                 // the MMAs of the previous stage have completed once at most this stage's group is pending: release its slot
                 wgmma_wait<1>();
@@ -683,10 +826,34 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
                 if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
                 prev = s;
                 if (++s == S) { s = 0; ph ^= 1; }
+            };
+            for (int i = 0; i < ntap_stage; ++i) {
+                if (MODE == MODE_GEMM) {
+                    stage([&](uint32_t sa, uint32_t sb) { mma64(sa, sb); });
+                } else if (MODE == MODE_CONV64) {          // stage i = horizontal tap i; resident weights
+                    stage([&](uint32_t sa, uint32_t) {
+#pragma unroll
+                        for (int dy = 0; dy < 3; ++dy) mma64(sa + dy * TILE_PW * 128, w0 + (dy * 3 + i) * BN * 128);
+                    });
+                } else {
+                    stage([&](uint32_t sa, uint32_t sb) {
+#pragma unroll
+                        for (int dy = 0; dy < 3; ++dy) mma64(sa + dy * TILE_PW * 128, sb + dy * BN * 128);
+                    });
+                }
+            }
+            for (int i = ntap_stage; i < nstage; ++i) {
+                if (MODE == MODE_CONV64) stage([&](uint32_t sa, uint32_t) { mma64(sa, w0 + 9 * BN * 128); });
+                else stage([&](uint32_t sa, uint32_t sb) { mma64(sa, sb); });
             }
             wgmma_wait<0>();
             reg_fence(acc);
             if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
+            if constexpr (DIRECT) {
+                dec_direct_epilogue<BN, BF16, DF, Cfg::kOutBufs>(p, &mapO0, &mapO1, dp, nt, acc, sk, sOut + g * Cfg::kOutBufs * Cfg::kOutBoxBytes,
+                                                                 g, wl, lane, nbox);
+                continue;
+            }
             named_sync(1, 256);                          // every epilogue warp is done reading the previous tile
             acc_stage<BN>(stg, acc, g, wl, lane);
             named_sync(1, 256);
@@ -696,6 +863,9 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
                 else if constexpr (EPI == EPI_NECKOUT) epilogue_neckout<BN>(p, mt, stg, quarter, lane);
                 else epilogue_rows<BN, Cfg::kColsPerWarp, EPI, BF16>(p, mt, nt, stg, quarter, lane, col_begin, ln_on, lnr);
             }
+        }
+        if constexpr (DIRECT) {
+            if (wl == 0 && lane == 0) bulk_wait<0>();     // the output boxes' stores are complete before the CTA retires
         }
     }
 }

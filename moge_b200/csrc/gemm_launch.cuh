@@ -27,7 +27,7 @@ using ConvHDF = DecFlagList<128, DF_RELU, DF_RAW | DF_SKIP, DF_RAW | DF_RELU | D
 // its grid is a multiple of num_n_tiles (every CTA then sees one fixed nt).
 template <int BN, int MODE, int AMODE, int EPI, bool BF16, int DF>
 int launch_gemm_inst(const GemmLaunch& g, int num_sms, cudaStream_t st) {
-    using Cfg = GemmCfg<BN, MODE>;
+    using Cfg = GemmCfg<BN, MODE, dec_direct(MODE, EPI, DF)>;
     const GemmParams& p = g.p;
     auto kern = gemm_kernel<BN, MODE, AMODE, EPI, BF16, DF>;
     MG_SET_SMEM_ONCE(kern, Cfg::kSmemBytes);
@@ -36,7 +36,7 @@ int launch_gemm_inst(const GemmLaunch& g, int num_sms, cudaStream_t st) {
     int grid = tiles < num_sms ? tiles : num_sms;
     if (MODE == MODE_CONV64) grid = (num_sms / p.num_n_tiles) * p.num_n_tiles < tiles ? (num_sms / p.num_n_tiles) * p.num_n_tiles : tiles;
     if (grid <= 0) return set_error("gemm: %d output-channel tiles exceed the %d SMs", p.num_n_tiles, num_sms);
-    CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(Cfg::kThreads), Cfg::kSmemBytes, st, g.a, g.aux, g.b, p));
+    CUDA_TRY(launch_pdl(kern, dim3(grid), dim3(Cfg::kThreads), Cfg::kSmemBytes, st, g.a, g.aux, g.b, g.o0, g.o1, p));
     return 0;
 }
 
