@@ -19,7 +19,7 @@ int gemm_linear(GemmLaunch* g, bool bf16, const void* A, int M, int K, const voi
         p.Ho = grid->H; p.Wo = grid->W; p.Hop = grid->Hp; p.Wop = grid->Wp; p.su = su; p.sv = sv;
     }
     if (ln) {
-        const int parts = N / (bn / 2);             // every ROWS kernel has 8 epilogue warps: column groups of BN/2
+        const int parts = N / (bn / 2);             // the ROWS epilogues run in column groups of BN/2 (GemmCfg::kEpiCols)
         p.stats_ld = kStatsLd;
         if (ln->x16) {
             if (parts > kStatsLd) return set_error("linear: %d statistics groups per row > %d", parts, kStatsLd);

@@ -4,9 +4,11 @@
 // -> accumulator tile staged in shared memory -> fused epilogue.
 //
 // Roles (warpgroup-uniform): warpgroup 0 = TMA producer (one elected lane of warp 0), warpgroups 1 and 2 = consumers:
-// each issues the wgmma of its 64 rows of the 128-row tile, then all eight consumer warps run the epilogue (warp ew owns
-// rows 32 (ew & 3) .. +31; with 8 epilogue warps the two warps of a row quarter split the columns).  The dec_direct variants
-// skip the staging: each consumer warpgroup stores its own 64 rows from its registers (dec_direct_epilogue).
+// each issues the wgmma of its 64 rows of the 128-row tile and stages its accumulators in shared memory; warpgroup 3 = epilogue:
+// warp w runs the fused epilogue of rows 32 w .. +31 of the staged tile while the consumers run the next tile's MMAs.  Two
+// mbarriers hand the one staging tile back and forth: acc_full (staged, the epilogue may read it) and acc_empty (read, the
+// consumers may overwrite it).  The dec_direct variants have no epilogue warpgroup and skip the staging: each consumer warpgroup
+// stores its own 64 rows from its registers (dec_direct_epilogue).
 //
 // Three main loops share the kernel (MODE):
 //   MODE_GEMM   one stage = one 64-wide K block of A (row tile, or one filter tap's pixel window) and of B.
@@ -120,13 +122,22 @@ template <int BN, int MODE = MODE_GEMM, bool DIRECT = false> struct GemmCfg {
     static constexpr int kFixedBytes = kAccBytes + kOutBytes + kResidentBytes + 1024 /*align slack*/ + 256 /*barriers*/;
     static constexpr int kFit = (kMaxDynSmem - kFixedBytes) / kStageBytes;
     static constexpr int kStages = kFit > 8 ? 8 : kFit;
-    static constexpr int kEpiWarps = (BN >= 64) ? 8 : 4;
-    static constexpr int kThreads = 384;
+    // staged variants: a fourth warpgroup runs the epilogue (warp w = row quarter w)
+    static constexpr int kThreads = DIRECT ? 384 : 512;
+    // registers per thread after setmaxnreg, by role; 128 x (producer + 2 consumer + epilogue) must fit the 64 K of the SM.
+    // ptxas cannot allocate the EPI_DEC epilogues below 168 and spills the pixel-tile producer at 24; 40 / 152 / 168 spills 8
+    // bytes in the EPI_PATCH variant, 40 / 144 / 184 spills nothing.
+    static constexpr int kProducerRegs = 40;
+    static constexpr int kConsumerRegs = DIRECT ? 232 : 144;
+    static constexpr int kEpilogueRegs = DIRECT ? 0 : 184;
+    static_assert(kProducerRegs + 2 * kConsumerRegs + kEpilogueRegs <= 65536 / 128, "gemm_kernel: setmaxnreg split exceeds 64 K registers");
     static constexpr int kSmemBytes = kStages * kStageBytes + kFixedBytes;
-    static constexpr int kColsPerWarp = (kEpiWarps == 8) ? BN / 2 : BN;
+    // columns of one epilogue call: an epilogue warp covers BN / kEpiCols column groups of its rows, one call each (the LayerNorm
+    // statistics producers write one partial sum per group: gemm_linear's `parts`)
+    static constexpr int kEpiCols = (BN >= 64) ? BN / 2 : BN;
     static_assert(kStages >= 2, "gemm_kernel: fewer than two ring stages fit beside the accumulator tile");
     static_assert(kSmemBytes <= kMaxDynSmem, "gemm_kernel: stage ring + accumulator tile exceed the shared memory of one CTA");
-    static_assert((2 * kStages + 1) * 8 <= 256, "gemm_kernel: barrier block overflows its 256 bytes");
+    static_assert((2 * kStages + 3) * 8 <= 256, "gemm_kernel: barrier block overflows its 256 bytes");
     static_assert(!DIRECT || BN % 64 == 0, "gemm_kernel: the direct EPI_DEC epilogue stores whole 64-channel boxes");
 };
 
@@ -663,7 +674,7 @@ __device__ __forceinline__ void epilogue_rows(const GemmParams& p, int mt, int n
 }
 
 template <int BN, int MODE, int AMODE, int EPI, bool BF16, int DF = -1>
-__global__ void __launch_bounds__(384, 1)
+__global__ void __launch_bounds__(GemmCfg<BN, MODE, dec_direct(MODE, EPI, DF)>::kThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAux,
             const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapO0,
             const __grid_constant__ CUtensorMap mapO1, const GemmParams p) {
@@ -681,6 +692,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
     uint64_t* full = reinterpret_cast<uint64_t*>(sW + Cfg::kResidentBytes);
     uint64_t* empty = full + S;
     uint64_t* wfull = empty + S;
+    uint64_t* acc_full = wfull + 1;       // staged variants: the consumers have staged the tile
+    uint64_t* acc_empty = wfull + 2;      // ... the epilogue warpgroup has read it
 
     const int warp = threadIdx.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -696,6 +709,8 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
         // empty: one arrival per consumer warp once its warpgroup's MMAs that read the stage have completed
         for (int s = 0; s < S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 8); }
         mbar_init(wfull, 1);
+        mbar_init(acc_full, 256);      // every consumer thread, after its own staging writes
+        mbar_init(acc_empty, 128);     // every epilogue thread, after its own reads of the staged tile
         fence_mbar_init();
     }
     __syncthreads();
@@ -705,7 +720,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
         // ================================================================== TMA producer
         // (warp 0 stays CONVERGED and one elected lane issues: under `if (lane == 0)` the compiler has to assume an
         // arbitrary active mask and wraps every TMA instruction in an elect-and-retry loop)
-        regs_dec<40>();
+        regs_dec<Cfg::kProducerRegs>();
         if (warp != 0) return;
         if (MODE == MODE_CONV64) {
             // the weights of this CTA's output-channel tile (the grid is a multiple of num_n_tiles: nt is fixed per CTA)
@@ -772,31 +787,21 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
                 if (++s == S) { s = 0; ph ^= 1; }
             }
         }
-    } else {
-        // ================================================================== consumers: MMA, then epilogue
-        regs_inc<232>();
+    } else if (warp < 12) {
+        // ================================================================== consumers: MMA, then hand the tile to the epilogue
+        regs_inc<Cfg::kConsumerRegs>();
         const int g = (warp - 4) >> 2;                  // consumer warpgroup: rows 64 g .. 64 g + 63 of the tile
         const int wl = warp & 3;
-        const int ew = warp - 4;
-        const int quarter = ew & 3;
-        const int col_begin = (Cfg::kEpiWarps == 8) ? (ew >> 2) * (BN / 2) : 0;
         const uint32_t a_off = static_cast<uint32_t>(g) * 64 * 128;
         if (MODE == MODE_CONV64) mbar_wait(wfull, 0);
         const uint32_t w0 = smem_u32(sW);
-        LnRows lnr{}, lnn{};
-        const bool ln_on = AMODE == AMODE_ROWS && (EPI == EPI_STORE16 || EPI == EPI_GELU16) && p.ln_rstd != nullptr;
-        if (ln_on && static_cast<int>(blockIdx.x) < total_tiles) ln_load(p, static_cast<int>(blockIdx.x) / p.num_n_tiles, quarter, lane, lnn);
         int s = 0; uint32_t ph = 0;
         int nbox = 0;                                   // DIRECT: output boxes this warpgroup has issued
+        uint32_t handed = 0;                            // staged variants: tiles staged for the epilogue warpgroup so far
         // stages per tile with the 3x3 taps; the rest read the aux source (fused 1x1 input block)
         const int ntap_stage = (MODE == MODE_GEMM) ? nstage : (MODE == MODE_CONV64) ? 3 : 3 * p.kb_main;
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int mt = tile / p.num_n_tiles, nt = tile % p.num_n_tiles;
-            if (ln_on) {        // rstd of this tile's rows (loaded one iteration ago); then issue the next tile's loads
-                lnr = lnn;
-                const int nxt = tile + static_cast<int>(gridDim.x);
-                if (nxt < total_tiles) ln_load(p, nxt / p.num_n_tiles, quarter, lane, lnn);
-            }
             DecPix dp{};
             uint32_t sk[DIRECT && (DF & DF_SKIP) ? BN / 4 : 1];
             if constexpr (DIRECT) {
@@ -854,18 +859,41 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
                                                                  g, wl, lane, nbox);
                 continue;
             }
-            named_sync(1, 256);                          // every epilogue warp is done reading the previous tile
+            mbar_wait(acc_empty, (handed & 1) ^ 1);      // the epilogue warpgroup is done reading the previous tile
             acc_stage<BN>(stg, acc, g, wl, lane);
-            named_sync(1, 256);
-            if (ew < Cfg::kEpiWarps) {
-                if constexpr (EPI == EPI_DEC) epilogue_dec16<BN, Cfg::kColsPerWarp, AMODE, BF16, DF>(p, mt, nt, stg, quarter, lane, col_begin);
-                else if constexpr (EPI == EPI_HEADOUT) epilogue_headout<BN>(p, mt, stg, quarter, lane);
-                else if constexpr (EPI == EPI_NECKOUT) epilogue_neckout<BN>(p, mt, stg, quarter, lane);
-                else epilogue_rows<BN, Cfg::kColsPerWarp, EPI, BF16>(p, mt, nt, stg, quarter, lane, col_begin, ln_on, lnr);
-            }
+            mbar_arrive(acc_full);
+            ++handed;
         }
         if constexpr (DIRECT) {
             if (wl == 0 && lane == 0) bulk_wait<0>();     // the output boxes' stores are complete before the CTA retires
+        }
+    } else if constexpr (!DIRECT) {
+        // ================================================================== epilogue warpgroup (staged variants)
+        regs_inc<Cfg::kEpilogueRegs>();
+        const int quarter = warp - 12;
+        LnRows lnr{}, lnn{};
+        const bool ln_on = AMODE == AMODE_ROWS && (EPI == EPI_STORE16 || EPI == EPI_GELU16) && p.ln_rstd != nullptr;
+        if (ln_on && static_cast<int>(blockIdx.x) < total_tiles) ln_load(p, static_cast<int>(blockIdx.x) / p.num_n_tiles, quarter, lane, lnn);
+        uint32_t taken = 0;                              // tiles read from the staging tile so far
+        for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+            const int mt = tile / p.num_n_tiles, nt = tile % p.num_n_tiles;
+            if (ln_on) {        // rstd of this tile's rows (loaded one iteration ago); then issue the next tile's loads
+                lnr = lnn;
+                const int nxt = tile + static_cast<int>(gridDim.x);
+                if (nxt < total_tiles) ln_load(p, nxt / p.num_n_tiles, quarter, lane, lnn);
+            }
+            mbar_wait(acc_full, taken & 1);
+            if constexpr (EPI == EPI_HEADOUT) epilogue_headout<BN>(p, mt, stg, quarter, lane);
+            else if constexpr (EPI == EPI_NECKOUT) epilogue_neckout<BN>(p, mt, stg, quarter, lane);
+            else {
+#pragma unroll 1
+                for (int cb = 0; cb < BN; cb += Cfg::kEpiCols) {
+                    if constexpr (EPI == EPI_DEC) epilogue_dec16<BN, Cfg::kEpiCols, AMODE, BF16, DF>(p, mt, nt, stg, quarter, lane, cb);
+                    else epilogue_rows<BN, Cfg::kEpiCols, EPI, BF16>(p, mt, nt, stg, quarter, lane, cb, ln_on, lnr);
+                }
+            }
+            mbar_arrive(acc_empty);
+            ++taken;
         }
     }
 }
