@@ -34,13 +34,6 @@ def _rows(t: torch.Tensor, shape) -> torch.Tensor:
     return t.detach().reshape(shape).to(torch.float32).contiguous()
 
 
-def _workspace(mode: int, truncated: bool, batch: int, n: int, device) -> torch.Tensor:
-    L = capi.lib()
-    nbytes = capi.C.c_size_t()
-    capi.check(L.moge_align_workspace_bytes(mode, int(truncated), batch, n, capi.C.byref(nbytes)))
-    return torch.empty(max(nbytes.value, 1), dtype=torch.uint8, device=device)
-
-
 def _check_n(n: int, limit: int, what: str) -> None:
     if n < 1 or n > limit:
         raise MogeError(f"{what}: n = {n} is outside [1, {limit}] (at most {capi.ALIGN_MAX_POINTS} points per problem)")
@@ -69,7 +62,7 @@ def align(x: torch.Tensor, y: torch.Tensor, w: torch.Tensor, trunc: Optional[Uni
     a_k = torch.empty(batch, dtype=torch.float32, device=x.device)
     loss_k = torch.empty_like(a_k)
     index = torch.empty(batch, dtype=torch.int64, device=x.device)
-    ws = _workspace(capi.ALIGN_PLAIN, trunc is not None, batch, n, x.device)
+    ws = capi.workspace(capi.lib().moge_align_workspace_bytes, capi.ALIGN_PLAIN, int(trunc is not None), batch, n, device=x.device)
     capi.check(capi.lib().moge_align(xr.data_ptr(), yr.data_ptr(), wr.data_ptr(), None if t_dev is None else t_dev.data_ptr(), per_elem,
                                      batch, n, a_k.data_ptr(), loss_k.data_ptr(), index.data_ptr(), ws.data_ptr(), ws.numel(),
                                      capi.current_stream()))
@@ -98,7 +91,7 @@ def _anchored(mode: int, src: torch.Tensor, tgt: torch.Tensor, weight: torch.Ten
     loss = torch.empty(batch, dtype=torch.float32, device=src.device)
     anchor = torch.empty(batch, dtype=torch.int64, device=src.device)
     index = torch.empty_like(anchor)
-    ws = _workspace(mode, trunc is not None, batch, n, src.device)
+    ws = capi.workspace(capi.lib().moge_align_workspace_bytes, mode, int(trunc is not None), batch, n, device=src.device)
     capi.check(capi.lib().moge_align_anchored(s.data_ptr(), t.data_ptr(), w.data_ptr(), mode, -1.0 if trunc is None else trunc, batch,
                                               n, loss.data_ptr(), anchor.data_ptr(), index.data_ptr(), ws.data_ptr(), ws.numel(),
                                               capi.current_stream()))

@@ -215,6 +215,15 @@ def ptr(t) -> Optional[int]:
     return t.data_ptr()
 
 
+def workspace(query, *args, device):
+    """The uint8 workspace tensor of an op-library call: `query` is its `moge_*_workspace_bytes` entry point, called with `args`.
+    At least 256 bytes, so that its pointer is never null."""
+    import torch
+    nbytes = C.c_size_t()
+    check(query(*args, C.byref(nbytes)))
+    return torch.empty(max(nbytes.value, 256), dtype=torch.uint8, device=device)
+
+
 def current_stream() -> int:
     import torch
     return torch.cuda.current_stream().cuda_stream

@@ -16,6 +16,7 @@
 // memory and each candidate accumulates its terms there (the arrays do not fit in shared memory together at m = 12288).
 // Anchored problems (alignment.py:163-214, 251-355) form x = src - src_p, y = tgt - tgt_p on the fly from the image, staged once per
 // CTA in shared memory; each image keeps the least (loss, anchor, index) through a packed 64-bit atomicMin.
+#include "common.cuh"
 #include "host_api.h"
 #include "../../include/moge_b200.h"
 #include <math.h>
@@ -64,14 +65,6 @@ struct Source {
     }
 };
 
-__device__ __forceinline__ uint32_t order_key(float f) {
-    const uint32_t u = __float_as_uint(__fadd_rn(f, 0.f));      // -0 -> +0: equal floats give equal keys
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_value(uint32_t k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
 // breakpoint `which` (0 = A, 1 = B, 2 = C) of an element, in the reference's fp32 arithmetic
 __device__ __forceinline__ float breakpoint(const Elem& v, int which) {
     if (which == 0) return __fdiv_rn(v.y, fmaxf(v.x, kEps));
@@ -96,20 +89,6 @@ __device__ void sort_keys(uint64_t* buf, int m) {
             __syncthreads();
         }
     }
-}
-
-__device__ __forceinline__ double warp_sum(double v) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-__device__ double block_sum(double v, double* red) {
-    v = warp_sum(v);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double s = 0.0;
-    for (int i = 0; i < kWarps; ++i) s += red[i];
-    return s;
 }
 
 // Exclusive block scan of one Prefix per thread (in thread order); red holds kWarps + 1 entries.
@@ -151,7 +130,7 @@ __device__ __forceinline__ Result solve_median(const Source src, int m, uint64_t
         total += static_cast<double>(v.w) * v.x;
     }
     if (threadIdx.x == 0) *pick = m - 1;
-    total = block_sum(total, red);       // its leading __syncthreads also publishes buf
+    total = block_sum<kThreads>(total, red);       // its leading __syncthreads also publishes buf
     sort_keys(buf, m);
     // contiguous chunk per thread: local sums, scan of the chunk totals, then the first position with 2 prefix - total >= 0
     const int chunk = (m + blockDim.x - 1) / blockDim.x, c0 = min(m, static_cast<int>(threadIdx.x) * chunk), c1 = min(m, c0 + chunk);
@@ -175,7 +154,7 @@ __device__ __forceinline__ Result solve_median(const Source src, int m, uint64_t
         const Elem v = src.get(e);
         loss += static_cast<double>(v.w) * fabs(static_cast<double>(a) * v.x - v.y);
     }
-    loss = block_sum(loss, red);
+    loss = block_sum<kThreads>(loss, red);
     __syncthreads();                     // buf and *pick are rewritten by the next problem
     return {loss, static_cast<int>(static_cast<uint32_t>(chosen))};
 }
@@ -221,7 +200,7 @@ __device__ __forceinline__ Result solve_truncated(const Source src, int m, uint6
         }
         __syncthreads();
     }
-    t_total = block_sum(t_total, red);
+    t_total = block_sum<kThreads>(t_total, red);
     // least f over the candidates, ties to the smaller element; element 0 when there is no candidate
     double best = INFINITY, f0 = 0.0;
     int best_j = m;
@@ -349,20 +328,13 @@ __global__ void __launch_bounds__(kThreads) lstsq_kernel(const float* __restrict
         const double u = static_cast<double>(__fmul_rn(r, x[off + i])), v = static_cast<double>(__fmul_rn(r, y[off + i]));
         su += u; su2 += u * u; suv += u * v; sv += v;
     }
-    su = block_sum(su, red); su2 = block_sum(su2, red); suv = block_sum(suv, red); sv = block_sum(sv, red);
+    su = block_sum<kThreads>(su, red); su2 = block_sum<kThreads>(su2, red);
+    suv = block_sum<kThreads>(suv, red); sv = block_sum<kThreads>(sv, red);
     if (threadIdx.x == 0) {
         const double nn = static_cast<double>(n), det = su2 * nn - su * su;
         a_out[blockIdx.x] = static_cast<float>((nn * suv - su * sv) / det);
         b_out[blockIdx.x] = static_cast<float>((su2 * sv - su * suv) / det);
     }
-}
-
-int num_sms(int* smem_per_sm = nullptr) {
-    int dev = 0, sms = 0, smem = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
-        cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev) != cudaSuccess) return -1;
-    if (smem_per_sm) *smem_per_sm = smem;
-    return sms;
 }
 
 // launch geometry shared by the workspace query and the launches
@@ -376,9 +348,10 @@ int plan(int mode, int truncated, int64_t batch, int n, Plan* pl) {
     } else if (n <= 0 || n > kMaxPoints) {
         return set_error("align: n = %d points is outside [1, %d]", n, kMaxPoints);
     }
-    int smem_per_sm = 0;
-    const int sms = num_sms(&smem_per_sm);
-    if (sms <= 0) return set_error("align: no CUDA device: moge_b200 has no CPU fallback");
+    int sms = 0, dev = 0, smem_per_sm = 0;
+    MG_TRY(check_device("align", &sms));
+    CUDA_TRY(cudaGetDevice(&dev));
+    CUDA_TRY(cudaDeviceGetAttribute(&smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev));
     const int comps = mode == MOGE_ANCHOR_DEPTH || mode == MOGE_ALIGN_PLAIN ? 1 : 3, m = n * comps;
     int64_t ctas;
     if (mode == MOGE_ALIGN_PLAIN) {
@@ -396,16 +369,9 @@ int plan(int mode, int truncated, int64_t batch, int n, Plan* pl) {
         const int ranges = static_cast<int>(std::min<int64_t>(n, std::max<int64_t>(1, static_cast<int64_t>(sms) * per_sm / batch)));
         ctas = static_cast<int64_t>(ranges) * batch;
         pl->grid = dim3(ranges, static_cast<unsigned>(batch));
-        pl->slot_bytes = (static_cast<size_t>(batch) * 8 + 255) / 256 * 256;
+        pl->slot_bytes = WsLayout::up(static_cast<size_t>(batch) * 8);
     }
     pl->scratch_bytes = truncated ? static_cast<size_t>(ctas) * cta_scratch_doubles(m) * 8 : 0;
-    return 0;
-}
-
-int check_workspace(const Plan& pl, void* workspace, size_t bytes) {
-    const size_t need = pl.slot_bytes + pl.scratch_bytes;
-    if (need && (!workspace || bytes < need)) return set_error("align: workspace of %zu bytes needed, %zu given", need, bytes);
-    if (reinterpret_cast<uintptr_t>(workspace) % 256) return set_error("align: workspace must be 256-byte aligned");
     return 0;
 }
 
@@ -438,7 +404,7 @@ int moge_align(const float* x, const float* y, const float* w, const float* trun
     if (!x || !y || !w || !a || !loss || !index) return set_error("null argument");
     Plan pl;
     MG_TRY(plan(MOGE_ALIGN_PLAIN, trunc != nullptr, batch, n, &pl));
-    MG_TRY(check_workspace(pl, workspace, workspace_bytes));
+    MG_TRY(check_workspace(pl.slot_bytes + pl.scratch_bytes, workspace, workspace_bytes, "align"));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     double* scratch = static_cast<double*>(workspace);
     if (!trunc) return launch<align_plain_kernel<false>>(pl, st, x, y, w, trunc, 0, batch, n, a, loss, index, scratch);
@@ -451,7 +417,7 @@ int moge_align_anchored(const float* src, const float* tgt, const float* w, int 
     if (mode == MOGE_ALIGN_PLAIN) return set_error("align_anchored: mode must be one of MOGE_ANCHOR_*");
     Plan pl;
     MG_TRY(plan(mode, trunc >= 0.f, batch, n, &pl));
-    MG_TRY(check_workspace(pl, workspace, workspace_bytes));
+    MG_TRY(check_workspace(pl.slot_bytes + pl.scratch_bytes, workspace, workspace_bytes, "align"));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     unsigned long long* slots = static_cast<unsigned long long*>(workspace);
     double* scratch = reinterpret_cast<double*>(static_cast<char*>(workspace) + pl.slot_bytes);
@@ -468,7 +434,7 @@ int moge_align_affine_lstsq(const float* x, const float* y, const float* w, int6
     if (batch <= 0 || n <= 0) return set_error("align_affine_lstsq: bad shape batch=%lld n=%lld", static_cast<long long>(batch),
                                                static_cast<long long>(n));
     if (batch > 0x7fffffff) return set_error("align_affine_lstsq: batch too large");
-    if (num_sms() <= 0) return set_error("align_affine_lstsq: no CUDA device: moge_b200 has no CPU fallback");
+    MG_TRY(check_device("align_affine_lstsq"));
     lstsq_kernel<<<static_cast<unsigned>(batch), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(x, y, w, n, a, b);
     CUDA_TRY(cudaGetLastError());
     return 0;

@@ -184,5 +184,39 @@ __device__ __forceinline__ float warp_max(float v) {
     for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
     return v;
 }
+__device__ __forceinline__ double warp_sum(double v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+// Fixed-order fp64 sum over a CTA of THREADS threads (the same bits on every run, DESIGN.md): the xor butterfly inside each
+// warp, then the warp partials added serially in warp order.  Every thread gets the result; red holds THREADS / 32 doubles.
+// The leading barrier also publishes the caller's earlier shared-memory writes and keeps red from being overwritten while a
+// previous call still reads it.
+template <int THREADS>
+__device__ double block_sum(double v, double* red) {
+    v = warp_sum(v);
+    __syncthreads();
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+    __syncthreads();
+    double s = 0.0;
+#pragma unroll
+    for (int i = 0; i < THREADS / 32; ++i) s += red[i];
+    return s;
+}
+
+// Order-preserving float <-> uint32 keys: unsigned order of the keys is the float order (-0 is keyed as +0, so equal floats
+// give equal keys).  Used for sorts and for min / max through integer atomics.
+__device__ __forceinline__ uint32_t order_key(float f) {
+    const uint32_t u = __float_as_uint(__fadd_rn(f, 0.f));
+    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_value(uint32_t k) {
+    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+// torch.maximum / torch.minimum (and np.max over a window): NaN propagates
+__device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b != b) ? __int_as_float(0x7fc00000) : fmaxf(a, b); }
+__device__ __forceinline__ float nan_min(float a, float b) { return (a != a || b != b) ? __int_as_float(0x7fc00000) : fminf(a, b); }
 
 }  // namespace mg

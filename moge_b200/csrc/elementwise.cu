@@ -436,18 +436,6 @@ int launch_head_output(const float4* pts_lr, const float4* nrm_lr, const float* 
 constexpr int FS_THREADS = 256;
 constexpr int FS_PER_THREAD = 4096 / FS_THREADS;
 
-__device__ __forceinline__ double block_sum(double v, double* red) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double t = 0.0;
-#pragma unroll
-    for (int i = 0; i < FS_THREADS / 32; ++i) t += red[i];
-    return t;
-}
-
 struct FsEval { double cost, jtr, jtj, focal; };
 
 // Residuals r(s) = f(s) q - uv with q = xy/(z+s) (f in closed form or given).  Returns cost = |r(s)|^2 and, when
@@ -474,8 +462,8 @@ __device__ FsEval fs_eval(double s, bool with_jac, const float* x, const float* 
                 bq2 += px * px + py * py;
             }
         }
-    a = block_sum(a, red); bq = block_sum(bq, red);
-    if (with_jac) { a2 = block_sum(a2, red); bq2 = block_sum(bq2, red); }
+    a = block_sum<FS_THREADS>(a, red); bq = block_sum<FS_THREADS>(bq, red);
+    if (with_jac) { a2 = block_sum<FS_THREADS>(a2, red); bq2 = block_sum<FS_THREADS>(bq2, red); }
     const double f = fixed_focal ? focal_given : a / bq;
     const double f2 = fixed_focal ? focal_given : (with_jac ? a2 / bq2 : 0.0);
     double cost = 0, jtr = 0, jtj = 0;
@@ -493,8 +481,8 @@ __device__ FsEval fs_eval(double s, bool with_jac, const float* x, const float* 
             }
         }
     FsEval e;
-    e.cost = block_sum(cost, red); e.focal = f; e.jtr = 0; e.jtj = 0;
-    if (with_jac) { e.jtr = block_sum(jtr, red); e.jtj = block_sum(jtj, red); }
+    e.cost = block_sum<FS_THREADS>(cost, red); e.focal = f; e.jtr = 0; e.jtj = 0;
+    if (with_jac) { e.jtr = block_sum<FS_THREADS>(jtr, red); e.jtj = block_sum<FS_THREADS>(jtj, red); }
     return e;
 }
 

@@ -25,6 +25,26 @@ int set_error(const char* fmt, ...);
         if (_r != 0) return _r;     \
     } while (0)
 
+// ---- argument checks of the op libraries (align, metrics, mesh, panorama, losses); each returns 0 or set_error(...), with
+// `what` (the operation's name) leading the message.
+// A current CUDA device, its SM count into *sms when sms is not null.
+int check_device(const char* what, int* sms = nullptr);
+// A batch of 1 to 65535 maps of H x W > 0 pixels, at most max_pixels each.
+int check_batch_map(const char* what, int64_t batch, int H, int W, int64_t max_pixels);
+// A workspace of at least `need` bytes at a 256-byte aligned address (null only when need == 0).
+int check_workspace(size_t need, const void* ws, size_t bytes, const char* what);
+
+// Workspace layout: pieces at consecutive 256-byte aligned offsets; `total` is the workspace size.
+struct WsLayout {
+    size_t total = 0;
+    static size_t up(size_t bytes) { return (bytes + 255) / 256 * 256; }
+    size_t add(size_t bytes) {      // the offset of a new piece of `bytes`
+        const size_t off = total;
+        total += up(bytes);
+        return off;
+    }
+};
+
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) is a PER-DEVICE property of a kernel: every launcher keeps one of these
 // per kernel instantiation and sets the attribute on the first launch on each device (engines on several GPUs in one
 // process; setting it twice from two threads is harmless, so relaxed atomics are enough).

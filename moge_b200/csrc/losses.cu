@@ -5,6 +5,7 @@
 // fp64 in a fixed order into one partial per quantity, and a finalize kernel adds an image's partials in tile order.  Backward
 // passes write each pixel's gradient from one thread: a stencil pixel gathers the terms of the pairs / quads it belongs to
 // instead of scattering into them, so no float atomics are used anywhere and gradients are bitwise reproducible.
+#include "common.cuh"
 #include "host_api.h"
 #include "../../include/moge_b200.h"
 #include <math.h>
@@ -16,12 +17,8 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr int kTilePx = 8192;                 // pixels per reduction tile (32 per thread)
+constexpr int64_t kMaxPixels = int64_t(1) << 29;
 constexpr int kQ = MOGE_LOSS_SUMS;
-
-__device__ __forceinline__ double warp_sum(double v) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
 
 // Op(b, pix, acc) adds pixel pix of image b into acc[kQ] (and may write its gradient).  part == nullptr: no reduction.
 template <class Op>
@@ -274,40 +271,22 @@ struct GlobalOp {
     }
 };
 
-int check_device(const char* what) {
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-        return set_error("%s: no CUDA device: moge_b200 has no CPU fallback", what);
-    return 0;
-}
-
-int check_shape(const char* what, int64_t batch, int H, int W) {
-    if (batch <= 0 || batch > 65535) return set_error("%s: batch = %lld is outside [1, 65535]", what, static_cast<long long>(batch));
-    if (H <= 0 || W <= 0) return set_error("%s: bad image size %d x %d", what, H, W);
-    if (static_cast<int64_t>(H) * W > (static_cast<int64_t>(1) << 31) / 4) return set_error("%s: image of %d x %d pixels is too large", what, H, W);
-    return 0;
-}
-
 int num_tiles(int H, int W) { return static_cast<int>((static_cast<int64_t>(H) * W + kTilePx - 1) / kTilePx); }
 
-size_t workspace_size(int64_t batch, int H, int W) {
-    return (static_cast<size_t>(batch) * num_tiles(H, W) * kQ * 8 + 255) / 256 * 256;
-}
+size_t workspace_size(int64_t batch, int H, int W) { return WsLayout::up(static_cast<size_t>(batch) * num_tiles(H, W) * kQ * 8); }
 
 // one pass of op over every pixel; reduces into sums unless grad mode
 template <class Op>
 int run(const char* what, const Op& op, bool reduce, int64_t batch, int H, int W, double* sums, void* workspace, size_t workspace_bytes,
         void* stream) {
+    if (reduce) {
+        if (!sums) return set_error("%s: null sums", what);
+        MG_TRY(check_workspace(workspace_size(batch, H, W), workspace, workspace_bytes, what));
+    }
     MG_TRY(check_device(what));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const int tiles = num_tiles(H, W);
-    double* part = nullptr;
-    if (reduce) {
-        if (!sums) return set_error("%s: null sums", what);
-        if (!workspace || workspace_bytes < workspace_size(batch, H, W))
-            return set_error("%s: workspace of %zu bytes needed, %zu given", what, workspace_size(batch, H, W), workspace_bytes);
-        part = static_cast<double*>(workspace);
-    }
+    double* part = reduce ? static_cast<double*>(workspace) : nullptr;
     tile_kernel<Op><<<dim3(tiles, static_cast<unsigned>(batch)), kThreads, 0, st>>>(op, static_cast<int64_t>(H) * W, tiles, part);
     CUDA_TRY(cudaGetLastError());
     if (reduce) {
@@ -328,7 +307,7 @@ extern "C" {
 
 int moge_loss_workspace_bytes(int64_t batch, int H, int W, size_t* bytes) {
     if (!bytes) return set_error("null argument");
-    MG_TRY(check_shape("loss", batch, H, W));
+    MG_TRY(check_batch_map("loss", batch, H, W, kMaxPixels));
     *bytes = workspace_size(batch, H, W);
     return 0;
 }
@@ -337,7 +316,7 @@ int moge_loss_mask(int kind, const float* pred, const float* a, const float* b, 
                    float* grad, double* sums, void* workspace, size_t workspace_bytes, void* stream) {
     if (!pred || !a || !b || (coef && !grad)) return set_error("null argument");
     if (kind != MOGE_LOSS_MASK_L2 && kind != MOGE_LOSS_MASK_BCE) return set_error("loss_mask: unknown kind %d", kind);
-    MG_TRY(check_shape("loss_mask", batch, H, W));
+    MG_TRY(check_batch_map("loss_mask", batch, H, W, kMaxPixels));
     const MaskOp op{kind, pred, a, b, static_cast<int64_t>(H) * W, coef, coef ? grad : nullptr};
     return run("loss_mask", op, coef == nullptr, batch, H, W, sums, workspace, workspace_bytes, stream);
 }
@@ -345,7 +324,7 @@ int moge_loss_mask(int kind, const float* pred, const float* a, const float* b, 
 int moge_loss_stencil(int kind, const float* points, const float* gt, int64_t batch, int H, int W, const float* coef, float* grad,
                       double* sums, void* workspace, size_t workspace_bytes, void* stream) {
     if (!points || !gt || (coef && !grad)) return set_error("null argument");
-    MG_TRY(check_shape("loss_stencil", batch, H, W));
+    MG_TRY(check_batch_map("loss_stencil", batch, H, W, kMaxPixels));
     const Maps mp{points, gt, H, W, static_cast<int64_t>(H) * W};
     const float beta = static_cast<float>(3 * kDeg);
     if (kind == MOGE_LOSS_EDGE) {
@@ -366,7 +345,7 @@ int moge_loss_global(const float* pred, const float* gt, const float* params, fl
     if (!pred || !gt || !params || (pass == 2 && !grad)) return set_error("null argument");
     if (pass < 0 || pass > 2) return set_error("loss_global: unknown pass %d", pass);
     if (!(beta >= 0.f)) return set_error("loss_global: beta must be >= 0");
-    MG_TRY(check_shape("loss_global", batch, H, W));
+    MG_TRY(check_batch_map("loss_global", batch, H, W, kMaxPixels));
     const GlobalOp op{pred, gt, params, beta, pass, static_cast<int64_t>(H) * W, grad};
     return run("loss_global", op, true, batch, H, W, sums, workspace, workspace_bytes, stream);
 }

@@ -12,6 +12,7 @@
 // A count pass writes per-tile vertex and quad counts, one CTA scans them image by image in a fixed order (integers only), and
 // the emit passes re-derive the flags, rank them inside the tile with ballots and write the vertex-index map, the gathered
 // attributes and the faces.  Nothing depends on the other images of a batch except where an image's rows land.
+#include "common.cuh"
 #include "host_api.h"
 #include "../../include/moge_b200.h"
 #include <math.h>
@@ -32,9 +33,6 @@ constexpr int kEdgeS = kEdgeT + 2 * kMaxR;
 constexpr int64_t kMaxPixels = int64_t(1) << 30;  // per image: vertex ids and triangle counts stay below 2^31
 
 struct Maps { moge_mesh_map_t m[MOGE_MESH_MAX_MAPS]; int n; };
-
-// np.max over a window: NaN propagates
-__device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b != b) ? __int_as_float(0x7fc00000) : fmaxf(a, b); }
 
 // ---------------------------------------------------------------------------------------------------- depth edge
 __global__ void __launch_bounds__(kThreads) edge_kernel(const float* __restrict__ depth, const uint8_t* __restrict__ mask,
@@ -363,40 +361,19 @@ __global__ void __launch_bounds__(kThreads) faces_kernel(const uint8_t* __restri
     }
 }
 
-int check_device(const char* what) {
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-        return set_error("%s: no CUDA device: moge_b200 has no CPU fallback", what);
-    return 0;
-}
-
-int check_shape(const char* what, int64_t batch, int H, int W) {
-    if (batch <= 0 || batch > 65535) return set_error("%s: batch = %lld is outside [1, 65535]", what, static_cast<long long>(batch));
-    if (H <= 0 || W <= 0) return set_error("%s: bad map size %d x %d", what, H, W);
-    if (static_cast<int64_t>(H) * W > kMaxPixels)
-        return set_error("%s: a map of %d x %d pixels is too large (at most 2^30 per image)", what, H, W);
-    return 0;
-}
-
 int num_tiles(int H, int W) { return static_cast<int>((static_cast<int64_t>(H) * W + kTilePx - 1) / kTilePx); }
 
-// workspace layout (256-byte aligned pieces): tile counts, tile offsets, vertex-index map
+// workspace layout: tile counts, tile offsets, vertex-index map
 struct Layout { size_t counts, offsets, vmap, total; };
-size_t up(size_t x) { return (x + 255) / 256 * 256; }
 Layout layout(int64_t batch, int H, int W) {
     const size_t t = static_cast<size_t>(num_tiles(H, W)), B = static_cast<size_t>(batch);
+    WsLayout ws;
     Layout l;
-    l.counts = 0;
-    l.offsets = l.counts + up(B * t * 2 * 4);
-    l.vmap = l.offsets + up(B * t * 2 * 4);
-    l.total = l.vmap + up(B * static_cast<size_t>(H) * W * 4);
+    l.counts = ws.add(B * t * 2 * 4);
+    l.offsets = ws.add(B * t * 2 * 4);
+    l.vmap = ws.add(B * static_cast<size_t>(H) * W * 4);
+    l.total = ws.total;
     return l;
-}
-
-int check_workspace(const Layout& l, void* ws, size_t bytes, const char* what) {
-    if (!ws || bytes < l.total) return set_error("%s: workspace of %zu bytes needed, %zu given", what, l.total, bytes);
-    if (reinterpret_cast<uintptr_t>(ws) % 256) return set_error("%s: workspace must be 256-byte aligned", what);
-    return 0;
 }
 
 }  // namespace
@@ -408,7 +385,7 @@ extern "C" {
 
 int moge_mesh_workspace_bytes(int64_t batch, int H, int W, size_t* bytes) {
     if (!bytes) return set_error("null argument");
-    MG_TRY(check_shape("mesh", batch, H, W));
+    MG_TRY(check_batch_map("mesh", batch, H, W, kMaxPixels));
     *bytes = layout(batch, H, W).total;
     return 0;
 }
@@ -416,7 +393,7 @@ int moge_mesh_workspace_bytes(int64_t batch, int H, int W, size_t* bytes) {
 int moge_depth_edge(const float* depth, const uint8_t* mask, const uint8_t* keep, int64_t batch, int H, int W, int kernel_size,
                     const float* atol, const float* rtol, uint8_t* out, void* stream) {
     if (!depth || !out) return set_error("null argument");
-    MG_TRY(check_shape("depth_map_edge", batch, H, W));
+    MG_TRY(check_batch_map("depth_map_edge", batch, H, W, kMaxPixels));
     if (kernel_size < 3 || kernel_size > 2 * kMaxR + 1 || kernel_size % 2 == 0)
         return set_error("depth_map_edge: kernel_size %d is not one of 3, 5, 7", kernel_size);
     MG_TRY(check_device("depth_map_edge"));
@@ -429,7 +406,7 @@ int moge_depth_edge(const float* depth, const uint8_t* mask, const uint8_t* keep
 
 int moge_normal_map(const float* points, const uint8_t* mask, int64_t batch, int H, int W, float* normal, uint8_t* normal_mask, void* stream) {
     if (!points || !normal) return set_error("null argument");
-    MG_TRY(check_shape("point_map_to_normal_map", batch, H, W));
+    MG_TRY(check_batch_map("point_map_to_normal_map", batch, H, W, kMaxPixels));
     MG_TRY(check_device("point_map_to_normal_map"));
     const int64_t blocks = (static_cast<int64_t>(H) * W + kThreads - 1) / kThreads;
     normal_map_kernel<<<dim3(static_cast<unsigned>(blocks), static_cast<unsigned>(batch)), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
@@ -441,7 +418,7 @@ int moge_normal_map(const float* points, const uint8_t* mask, int64_t batch, int
 int moge_normal_edge(const float* normals, const uint8_t* mask, const uint8_t* and_edge, const uint8_t* keep, int64_t batch, int H, int W,
                      int kernel_size, double tol, uint8_t* out, float* angle, void* stream) {
     if (!normals || !out) return set_error("null argument");
-    MG_TRY(check_shape("normal_map_edge", batch, H, W));
+    MG_TRY(check_batch_map("normal_map_edge", batch, H, W, kMaxPixels));
     if (kernel_size < 3 || kernel_size > 2 * kMaxR + 1 || kernel_size % 2 == 0)
         return set_error("normal_map_edge: kernel_size %d is not one of 3, 5, 7", kernel_size);
     if ((H + kEdgeT - 1) / kEdgeT > 65535) return set_error("normal_map_edge: %d rows is more than %d", H, 65535 * kEdgeT);
@@ -455,9 +432,9 @@ int moge_normal_edge(const float* normals, const uint8_t* mask, const uint8_t* a
 
 int moge_mesh_count(const uint8_t* mask, int64_t batch, int H, int W, int64_t* totals, void* workspace, size_t workspace_bytes, void* stream) {
     if (!totals) return set_error("null argument");
-    MG_TRY(check_shape("mesh_count", batch, H, W));
+    MG_TRY(check_batch_map("mesh_count", batch, H, W, kMaxPixels));
     const Layout l = layout(batch, H, W);
-    MG_TRY(check_workspace(l, workspace, workspace_bytes, "mesh_count"));
+    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "mesh_count"));
     MG_TRY(check_device("mesh_count"));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     char* ws = static_cast<char*>(workspace);
@@ -473,7 +450,7 @@ int moge_mesh_count(const uint8_t* mask, int64_t batch, int H, int W, int64_t* t
 int moge_mesh_build(const uint8_t* mask, int64_t batch, int H, int W, int tri, const moge_mesh_map_t* maps, int num_maps,
                     const int64_t* totals, int32_t* faces, void* workspace, size_t workspace_bytes, void* stream) {
     if (!totals || !faces || (num_maps && !maps)) return set_error("null argument");
-    MG_TRY(check_shape("mesh_build", batch, H, W));
+    MG_TRY(check_batch_map("mesh_build", batch, H, W, kMaxPixels));
     if (num_maps < 0 || num_maps > MOGE_MESH_MAX_MAPS) return set_error("mesh_build: %d maps is outside [0, %d]", num_maps, MOGE_MESH_MAX_MAPS);
     Maps ms;
     memset(&ms, 0, sizeof(ms));
@@ -488,7 +465,7 @@ int moge_mesh_build(const uint8_t* mask, int64_t batch, int H, int W, int tri, c
         ms.m[k] = d;
     }
     const Layout l = layout(batch, H, W);
-    MG_TRY(check_workspace(l, workspace, workspace_bytes, "mesh_build"));
+    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "mesh_build"));
     MG_TRY(check_device("mesh_build"));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     char* ws = static_cast<char*>(workspace);

@@ -6,6 +6,7 @@
 // adds the partials of an image in tile order.  Only integer counters and order-independent min/max use atomics.  Per-pixel values
 // are formed in the reference's fp32 arithmetic with explicit roundings (__fmul_rn / __fadd_rn / __fdiv_rn: nvcc would otherwise
 // contract `p * s + b` into an FMA, which the reference never does).
+#include "common.cuh"
 #include "host_api.h"
 #include "../../include/moge_b200.h"
 #include <math.h>
@@ -19,6 +20,7 @@ namespace {
 constexpr int kThreads = 256;
 constexpr int kWarps = kThreads / 32;
 constexpr int kTilePx = 8192;                 // pixels per reduction tile (32 per thread)
+constexpr int64_t kMaxPixels = int64_t(1) << 29;
 constexpr int kMaxSeg = MOGE_METRICS_MAX_SEGMENTS;
 constexpr int kMaxVar = MOGE_METRICS_MAX_VARIANTS;
 constexpr int kStatQ = 5;                     // sum x, sum y, sum x^2, sum xy, n
@@ -31,17 +33,6 @@ constexpr int kBS = kBT + 2 * kHalo;
 struct Variants { moge_metric_variant_t v[kMaxVar]; int n; };
 struct Thresholds { float t[MOGE_METRICS_F1_THRESHOLDS]; };
 
-__device__ __forceinline__ uint32_t order_key(float f) {
-    const uint32_t u = __float_as_uint(__fadd_rn(f, 0.f));
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-__device__ __forceinline__ float key_value(uint32_t k) {
-    return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
-}
-
-// torch.maximum / torch.minimum: NaN propagates
-__device__ __forceinline__ float nan_max(float a, float b) { return (a != a || b != b) ? __int_as_float(0x7fc00000) : fmaxf(a, b); }
-__device__ __forceinline__ float nan_min(float a, float b) { return (a != a || b != b) ? __int_as_float(0x7fc00000) : fminf(a, b); }
 __device__ __forceinline__ float norm3(float x, float y, float z) {
     return sqrtf(__fadd_rn(__fadd_rn(__fmul_rn(x, x), __fmul_rn(y, y)), __fmul_rn(z, z)));
 }
@@ -71,21 +62,6 @@ __device__ __forceinline__ void aligned_point(const moge_metric_variant_t& v, in
 }
 
 __device__ __forceinline__ bool is_points(int kind) { return kind >= MOGE_MV_POINTS_SHIFT; }
-
-__device__ __forceinline__ double warp_sum(double v) {
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-// fixed-order block sum; every thread gets the result
-__device__ double block_sum(double v, double* red) {
-    v = warp_sum(v);
-    __syncthreads();
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
-    __syncthreads();
-    double s = 0.0;
-    for (int i = 0; i < kWarps; ++i) s += red[i];
-    return s;
-}
 
 // slot of segment id `id` in the sorted table ids[0, n), or -1
 __device__ __forceinline__ int find_slot(const int32_t* ids, int n, int32_t id) {
@@ -209,7 +185,8 @@ __global__ void __launch_bounds__(kThreads) stats_kernel(const float* __restrict
     if (mx) atomicMax(gmax + b, mx);
     if (disp_src) {
         double* out = part + (b * tiles + blockIdx.x) * kStatQ;
-        sx = block_sum(sx, red); sy = block_sum(sy, red); sxx = block_sum(sxx, red); sxy = block_sum(sxy, red); cnt = block_sum(cnt, red);
+        sx = block_sum<kThreads>(sx, red); sy = block_sum<kThreads>(sy, red); sxx = block_sum<kThreads>(sxx, red);
+        sxy = block_sum<kThreads>(sxy, red); cnt = block_sum<kThreads>(cnt, red);
         if (threadIdx.x == 0) { out[0] = sx; out[1] = sy; out[2] = sxx; out[3] = sxy; out[4] = cnt; }
     }
     __syncthreads();
@@ -343,10 +320,10 @@ __global__ void __launch_bounds__(kThreads) eval_kernel(const float* __restrict_
     }
     double* out = part + (b * tiles + blockIdx.x) * kEvalQ;
     for (int v = 0; v < vars.n; ++v) {
-        const double r = block_sum(rel[v], red), c = block_sum(static_cast<double>(cnt[v]), red);
+        const double r = block_sum<kThreads>(rel[v], red), c = block_sum<kThreads>(static_cast<double>(cnt[v]), red);
         if (threadIdx.x == 0) { out[2 * v] = r; out[2 * v + 1] = c; }
     }
-    const double nn = block_sum(static_cast<double>(n), red);
+    const double nn = block_sum<kThreads>(static_cast<double>(n), red);
     if (threadIdx.x == 0) out[2 * kMaxVar] = nn;
     __syncthreads();
     for (int s = threadIdx.x; s < ns; s += blockDim.x) {
@@ -437,41 +414,21 @@ __global__ void __launch_bounds__(kThreads) boundary_kernel(const float* __restr
     }
 }
 
-int check_device(const char* what) {
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-        return set_error("%s: no CUDA device: moge_b200 has no CPU fallback", what);
-    return 0;
-}
-
-int check_shape(const char* what, int64_t batch, int H, int W) {
-    if (batch <= 0 || batch > 65535) return set_error("%s: batch = %lld is outside [1, 65535]", what, static_cast<long long>(batch));
-    if (H <= 0 || W <= 0) return set_error("%s: bad image size %d x %d", what, H, W);
-    if (static_cast<int64_t>(H) * W > (static_cast<int64_t>(1) << 31) / 4) return set_error("%s: image of %d x %d pixels is too large", what, H, W);
-    return 0;
-}
-
 int num_tiles(int H, int W) { return static_cast<int>((static_cast<int64_t>(H) * W + kTilePx - 1) / kTilePx); }
 
-// workspace layout (256-byte aligned pieces): stats partials, gmax keys, bbox keys, eval partials, segment partials
+// workspace layout: stats partials, gmax keys, bbox keys, eval partials, segment partials
 struct Layout { size_t stat, gmax, bbox, eval, seg, total; };
-size_t up(size_t x) { return (x + 255) / 256 * 256; }
 Layout layout(int64_t batch, int H, int W, int S) {
     const size_t t = static_cast<size_t>(num_tiles(H, W)), B = static_cast<size_t>(batch);
+    WsLayout ws;
     Layout l;
-    l.stat = 0;
-    l.gmax = l.stat + up(B * t * kStatQ * 8);
-    l.bbox = l.gmax + up(B * 4);
-    l.eval = l.bbox + up(B * kMaxSeg * 6 * 4);
-    l.seg = l.eval + up(B * t * kEvalQ * 8);
-    l.total = l.seg + up(B * t * static_cast<size_t>(S) * 3 * 8);
+    l.stat = ws.add(B * t * kStatQ * 8);
+    l.gmax = ws.add(B * 4);
+    l.bbox = ws.add(B * kMaxSeg * 6 * 4);
+    l.eval = ws.add(B * t * kEvalQ * 8);
+    l.seg = ws.add(B * t * static_cast<size_t>(S) * 3 * 8);
+    l.total = ws.total;
     return l;
-}
-
-int check_workspace(const Layout& l, void* ws, size_t bytes, const char* what) {
-    if (!ws || bytes < l.total) return set_error("%s: workspace of %zu bytes needed, %zu given", what, l.total, bytes);
-    if (reinterpret_cast<uintptr_t>(ws) % 256) return set_error("%s: workspace must be 256-byte aligned", what);
-    return 0;
 }
 
 int check_segments(const char* what, const int32_t* seg, const int32_t* ids, const int32_t* count, int S) {
@@ -497,7 +454,7 @@ extern "C" {
 
 int moge_metrics_workspace_bytes(int64_t batch, int H, int W, int S, size_t* bytes) {
     if (!bytes) return set_error("null argument");
-    MG_TRY(check_shape("metrics", batch, H, W));
+    MG_TRY(check_batch_map("metrics", batch, H, W, kMaxPixels));
     if (S < 0 || S > kMaxSeg) return set_error("metrics: %d segment slots per image is outside [0, %d]", S, kMaxSeg);
     *bytes = layout(batch, H, W, S).total;
     return 0;
@@ -506,7 +463,7 @@ int moge_metrics_workspace_bytes(int64_t batch, int H, int W, int S, size_t* byt
 int moge_metrics_resize(const uint8_t* mask, int64_t batch, int H, int W, int th, int tw, uint8_t* lr_mask, int64_t* lr_index,
                         int64_t* list, float* list_w, int32_t* count, void* stream) {
     if (!mask || !lr_mask || !lr_index || !list || !list_w || !count) return set_error("null argument");
-    MG_TRY(check_shape("masked_nearest_resize", batch, H, W));
+    MG_TRY(check_batch_map("masked_nearest_resize", batch, H, W, kMaxPixels));
     if (th <= 0 || tw <= 0 || static_cast<int64_t>(th) * tw > (1 << 22))
         return set_error("masked_nearest_resize: bad target size %d x %d", th, tw);
     MG_TRY(check_device("masked_nearest_resize"));
@@ -522,11 +479,11 @@ int moge_metrics_stats(const float* gt_depth, const float* gt_points, const uint
                        const int32_t* seg, const int32_t* seg_ids, const int32_t* seg_count, int S, int64_t batch, int H, int W,
                        float* disp_params, float* diameter, void* workspace, size_t workspace_bytes, void* stream) {
     if (!gt_depth || !mask || !disp_params) return set_error("null argument");
-    MG_TRY(check_shape("metrics_stats", batch, H, W));
+    MG_TRY(check_batch_map("metrics_stats", batch, H, W, kMaxPixels));
     MG_TRY(check_segments("metrics_stats", seg, seg_ids, seg_count, S));
     if (seg && (!gt_points || !diameter)) return set_error("metrics_stats: segments need the GT points and a diameter output");
     const Layout l = layout(batch, H, W, S);
-    MG_TRY(check_workspace(l, workspace, workspace_bytes, "metrics_stats"));
+    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "metrics_stats"));
     MG_TRY(check_device("metrics_stats"));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     char* ws = static_cast<char*>(workspace);
@@ -552,7 +509,7 @@ int moge_metrics_eval(const float* gt_depth, const float* gt_points, const uint8
                       const float* seg_params, const float* seg_diameter, int64_t batch, int H, int W, double* out, int64_t out_stride,
                       void* workspace, size_t workspace_bytes, void* stream) {
     if (!gt_depth || !gt_points || !mask || !out || (num_variants && !variants)) return set_error("null argument");
-    MG_TRY(check_shape("metrics_eval", batch, H, W));
+    MG_TRY(check_batch_map("metrics_eval", batch, H, W, kMaxPixels));
     if (num_variants < 0 || num_variants > kMaxVar) return set_error("metrics_eval: %d variants is outside [0, %d]", num_variants, kMaxVar);
     MG_TRY(check_segments("metrics_eval", seg, seg_ids, seg_count, S));
     if (seg && (!local_src || !seg_params || !seg_diameter)) return set_error("metrics_eval: segments need local points, params and diameters");
@@ -565,7 +522,7 @@ int moge_metrics_eval(const float* gt_depth, const float* gt_points, const uint8
         vars.v[v] = variants[v];
     }
     const Layout l = layout(batch, H, W, S);
-    MG_TRY(check_workspace(l, workspace, workspace_bytes, "metrics_eval"));
+    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "metrics_eval"));
     MG_TRY(check_device("metrics_eval"));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     char* ws = static_cast<char*>(workspace);
@@ -584,7 +541,7 @@ int moge_metrics_eval(const float* gt_depth, const float* gt_points, const uint8
 int moge_metrics_boundary(const float* gt_depth, const uint8_t* mask, const moge_metric_variant_t* aligned, const float* thresholds,
                           int64_t batch, int H, int W, int64_t* counts, int64_t counts_stride, void* stream) {
     if (!gt_depth || !mask || !aligned || !thresholds || !counts) return set_error("null argument");
-    MG_TRY(check_shape("metrics_boundary", batch, H, W));
+    MG_TRY(check_batch_map("metrics_boundary", batch, H, W, kMaxPixels));
     MG_TRY(check_variant("metrics_boundary", *aligned));
     if (aligned->kind >= MOGE_MV_POINTS_SHIFT) return set_error("metrics_boundary: the aligned prediction must be a depth variant");
     if (counts_stride < MOGE_METRICS_F1_COUNTS) return set_error("metrics_boundary: counts_stride %lld is too small", static_cast<long long>(counts_stride));

@@ -481,13 +481,6 @@ __global__ void __launch_bounds__(kThreads) finish_kernel(const float* __restric
 }
 
 // ---------------------------------------------------------------------------------------------------- host side
-int check_device(const char* what, int* sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || *sms <= 0)
-        return set_error("%s: no CUDA device: moge_b200 has no CPU fallback", what);
-    return 0;
-}
-
 int check_size(const char* what, int h, int w) {
     if (h < 2 || w < 2) return set_error("%s: a %d x %d map is too small (at least 2 x 2)", what, h, w);
     if (static_cast<int64_t>(h) * w > kMaxPixels) return set_error("%s: a %d x %d map is too large (at most 2^28 pixels)", what, h, w);
@@ -509,30 +502,24 @@ int load_cams(const char* what, const moge_panorama_camera_t* cams, int views, C
 
 unsigned blocks_for(int64_t n, int sms) { return static_cast<unsigned>(std::min<int64_t>((n + kThreads - 1) / kThreads, int64_t(sms) * 16)); }
 
-size_t up(size_t x) { return (x + 255) / 256 * 256; }
 struct Layout { size_t L, M, u, v, hv, hb, x, part, logi, total; };
 Layout layout(int views, int h, int w, int max_blocks) {
     const size_t n = static_cast<size_t>(h) * w;
+    WsLayout ws;
     Layout l;
-    l.L = 0;
-    l.M = l.L + up(views * n * 4);
-    l.u = l.M + up(views * n);
-    l.v = l.u + up((3 * n + h) * 8);
-    l.hv = l.v + up(n * 8);
-    l.hb = l.hv + up(n * 8);
-    l.x = l.hb + up(n * 8);
-    l.part = l.x + up(n * 8);
-    l.logi = l.part + up(static_cast<size_t>(max_blocks) * 4 * 8);
-    l.total = l.logi + up(n * 4);
+    l.L = ws.add(views * n * 4);
+    l.M = ws.add(views * n);
+    l.u = ws.add((3 * n + h) * 8);
+    l.v = ws.add(n * 8);
+    l.hv = ws.add(n * 8);
+    l.hb = ws.add(n * 8);
+    l.x = ws.add(n * 8);
+    l.part = ws.add(static_cast<size_t>(max_blocks) * 4 * 8);
+    l.logi = ws.add(n * 4);
+    l.total = ws.total;
     return l;
 }
 constexpr int kMaxLsmrBlocks = 132 * 4;
-
-int check_workspace(const Layout& l, void* ws, size_t bytes, const char* what) {
-    if (!ws || bytes < l.total) return set_error("%s: workspace of %zu bytes needed, %zu given", what, l.total, bytes);
-    if (reinterpret_cast<uintptr_t>(ws) % 256) return set_error("%s: workspace must be 256-byte aligned", what);
-    return 0;
-}
 
 }  // namespace
 }  // namespace mg
@@ -574,7 +561,7 @@ int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int v
     Cams cs;
     MG_TRY(load_cams("panorama_rhs", cams, views, &cs));
     const Layout l = layout(views, h, w, kMaxLsmrBlocks);
-    MG_TRY(check_workspace(l, workspace, workspace_bytes, "panorama_rhs"));
+    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "panorama_rhs"));
     int sms;
     MG_TRY(check_device("panorama_rhs", &sms));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -594,7 +581,7 @@ int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int h, int w, c
     if (!b || !row_mask || !depth || !stats) return set_error("null argument");
     MG_TRY(check_size("panorama_lsmr", h, w));
     const Layout l = layout(1, h, w, kMaxLsmrBlocks);
-    MG_TRY(check_workspace(l, workspace, workspace_bytes, "panorama_lsmr"));
+    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "panorama_lsmr"));
     int sms;
     MG_TRY(check_device("panorama_lsmr", &sms));
     int dev = 0, coop = 0, per_sm = 0;

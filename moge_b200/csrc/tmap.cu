@@ -1,5 +1,5 @@
-// TMA tensor-map construction + thread-local error string.  cuTensorMapEncodeTiled is fetched through
-// cudaGetDriverEntryPoint so the library has no link-time dependency on libcuda.
+// TMA tensor-map construction, the thread-local error string and the op libraries' argument checks.  cuTensorMapEncodeTiled
+// is fetched through cudaGetDriverEntryPoint so the library has no link-time dependency on libcuda.
 #include "host_api.h"
 #include <stdarg.h>
 #include <stdio.h>
@@ -16,6 +16,28 @@ int set_error(const char* fmt, ...) {
     return -1;
 }
 const char* last_error() { return g_err; }
+
+int check_device(const char* what, int* sms) {
+    int dev = 0, n = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0)
+        return set_error("%s: no CUDA device: moge_b200 has no CPU fallback", what);
+    if (sms) *sms = n;
+    return 0;
+}
+
+int check_batch_map(const char* what, int64_t batch, int H, int W, int64_t max_pixels) {
+    if (batch <= 0 || batch > 65535) return set_error("%s: batch = %lld is outside [1, 65535]", what, static_cast<long long>(batch));
+    if (H <= 0 || W <= 0) return set_error("%s: bad map size %d x %d", what, H, W);
+    if (static_cast<int64_t>(H) * W > max_pixels)
+        return set_error("%s: a map of %d x %d pixels is too large (at most %lld per image)", what, H, W, static_cast<long long>(max_pixels));
+    return 0;
+}
+
+int check_workspace(size_t need, const void* ws, size_t bytes, const char* what) {
+    if (need && (!ws || bytes < need)) return set_error("%s: workspace of %zu bytes needed, %zu given", what, need, bytes);
+    if (reinterpret_cast<uintptr_t>(ws) % 256) return set_error("%s: workspace must be 256-byte aligned", what);
+    return 0;
+}
 
 bool& pdl_scope() {
     static thread_local bool on = false;

@@ -47,12 +47,6 @@ def _cuda(*ts: torch.Tensor) -> None:
             raise MogeError("moge_b200.losses operates on CUDA tensors only (no CPU fallback)")
 
 
-def _workspace(B: int, H: int, W: int, device) -> torch.Tensor:
-    nbytes = capi.C.c_size_t()
-    capi.check(capi.lib().moge_loss_workspace_bytes(B, H, W, capi.C.byref(nbytes)))
-    return torch.empty(max(nbytes.value, 256), dtype=torch.uint8, device=device)
-
-
 def _sums(B: int, device) -> torch.Tensor:
     return torch.empty(B, capi.LOSS_SUMS, dtype=torch.float64, device=device)
 
@@ -64,7 +58,7 @@ class _MaskLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, a, b, kind):
         B, H, W = x.shape
-        sums, ws = _sums(B, x.device), _workspace(B, H, W, x.device)
+        sums, ws = _sums(B, x.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=x.device)
         capi.check(capi.lib().moge_loss_mask(kind, x.data_ptr(), a.data_ptr(), b.data_ptr(), B, H, W, None, None, sums.data_ptr(),
                                              ws.data_ptr(), ws.numel(), capi.current_stream()))
         ctx.save_for_backward(x, a, b)
@@ -112,7 +106,7 @@ class _StencilLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, points, gt, kind):
         B, H, W, _ = points.shape
-        sums, ws = _sums(B, points.device), _workspace(B, H, W, points.device)
+        sums, ws = _sums(B, points.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=points.device)
         capi.check(capi.lib().moge_loss_stencil(kind, points.data_ptr(), gt.data_ptr(), B, H, W, None, None, sums.data_ptr(),
                                                 ws.data_ptr(), ws.numel(), capi.current_stream()))
         ctx.save_for_backward(points, gt)
@@ -173,7 +167,7 @@ class _GlobalLoss(torch.autograd.Function):
     def forward(ctx, pred, scale, shift, gt, fixed, beta):
         B, H, W, _ = pred.shape
         params = torch.cat([scale.detach()[:, None], shift.detach(), fixed, torch.zeros_like(fixed)], dim=-1).contiguous()
-        sums, ws = _sums(B, pred.device), _workspace(B, H, W, pred.device)
+        sums, ws = _sums(B, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=pred.device)
         capi.check(capi.lib().moge_loss_global(pred.data_ptr(), gt.data_ptr(), params.data_ptr(), beta, 1, B, H, W, None, sums.data_ptr(),
                                                ws.data_ptr(), ws.numel(), capi.current_stream()))
         ctx.save_for_backward(pred, gt, params)
@@ -189,7 +183,7 @@ class _GlobalLoss(torch.autograd.Function):
         params = params.clone()
         params[:, 6] = g.to(torch.float32) / (3 * H * W)
         grad = torch.empty_like(pred)
-        sums, ws = _sums(B, pred.device), _workspace(B, H, W, pred.device)
+        sums, ws = _sums(B, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=pred.device)
         capi.check(capi.lib().moge_loss_global(pred.data_ptr(), gt.data_ptr(), params.data_ptr(), ctx.beta, 2, B, H, W, grad.data_ptr(),
                                                sums.data_ptr(), ws.data_ptr(), ws.numel(), capi.current_stream()))
         return grad, sums[:, 0].to(torch.float32), sums[:, 1:4].to(torch.float32), None, None, None
@@ -215,7 +209,7 @@ def affine_invariant_global_loss(pred_points: torch.Tensor, gt_points: torch.Ten
     # pass 0: the per-image weighted mean of the weights, for the clamp_max
     params = torch.zeros(B, 8, dtype=torch.float32, device=dev)
     params[:, 4] = valid.to(torch.float32)
-    sums, ws = _sums(B, dev), _workspace(B, H, W, dev)
+    sums, ws = _sums(B, dev), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=dev)
     capi.check(capi.lib().moge_loss_global(pred.data_ptr(), gt.data_ptr(), params.data_ptr(), float(beta), 0, B, H, W, None,
                                            sums.data_ptr(), ws.data_ptr(), ws.numel(), capi.current_stream()))
     hw = H * W

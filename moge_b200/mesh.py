@@ -105,9 +105,7 @@ class _Map:
 def _count(mask: Optional[torch.Tensor], B: int, H: int, W: int, dev):
     """Count pass and the one device-to-host copy: returns (workspace, device totals, pinned host totals, event)."""
     L = capi.lib()
-    nbytes = C.c_size_t()
-    capi.check(L.moge_mesh_workspace_bytes(B, H, W, C.byref(nbytes)))
-    ws = torch.empty(max(nbytes.value, 256), dtype=torch.uint8, device=dev)
+    ws = capi.workspace(L.moge_mesh_workspace_bytes, B, H, W, device=dev)
     totals = torch.empty(B, 4, dtype=torch.int64, device=dev)
     capi.check(L.moge_mesh_count(capi.ptr(mask), B, H, W, totals.data_ptr(), ws.data_ptr(), ws.numel(), capi.current_stream()))
     host = torch.empty(B, 4, dtype=torch.int64, pin_memory=True)

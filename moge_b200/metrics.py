@@ -265,9 +265,7 @@ def _launch(pred: Dict[str, torch.Tensor], gt: Dict, labels: Optional[List[Dict]
         disp = (capi.MV_DISPARITY if k == "disparity_affine_invariant" else capi.MV_DISPARITY_FROM_DEPTH, preds[k])
 
     # statistics pass: disparity least squares, max GT depth, segment diameters
-    ws_bytes = capi.C.c_size_t()
-    capi.check(L.moge_metrics_workspace_bytes(B, H, W, S if has_seg else 0, capi.C.byref(ws_bytes)))
-    ws = torch.empty(max(ws_bytes.value, 256), dtype=torch.uint8, device=dev)
+    ws = capi.workspace(L.moge_metrics_workspace_bytes, B, H, W, S if has_seg else 0, device=dev)
     disp_params = torch.empty(B, 4, dtype=torch.float32, device=dev)
     seg = ids_t = nseg_t = diameter = None
     if has_seg:

@@ -215,9 +215,7 @@ def merge_panorama(width: int, height: int, src: torch.Tensor, mask: torch.Tenso
         st = capi.current_stream()
         s = src.detach().contiguous()
         m = mask.detach().contiguous().view(torch.uint8) if mask.dtype == torch.bool else (mask != 0).contiguous().view(torch.uint8)
-        nbytes = C.c_size_t()
-        capi.check(L.moge_panorama_workspace_bytes(n, height, width, C.byref(nbytes)))
-        ws = torch.empty(nbytes.value, dtype=torch.uint8, device=dev)
+        ws = capi.workspace(L.moge_panorama_workspace_bytes, n, height, width, device=dev)
         stats = torch.zeros(len(levels), 2, dtype=torch.int32, device=dev)
         depth, init, out = None, None, []
         for lv, (w, h) in enumerate(levels):

@@ -9,7 +9,7 @@ normal_loss, mask_bce_loss (v2 "A") and mask_l2_loss.  Each time is the median o
 (CUDA events around loss + loss.sum().backward(), host work included, then a device synchronise), with the fastest and slowest
 beside it.  Peak memory is torch.cuda.max_memory_allocated over one such call, less what was allocated before it.  The
 comparator is loaded from oracle/_ref/ (built by __graft_entry__.build() when MOGE_REFERENCE is set,
-oracle/compile_reference_losses.py) and is "not measured" without it; when present, losses and gradients are compared at every
+oracle/compile_reference.py) and is "not measured" without it; when present, losses and gradients are compared at every
 timed size.
 """
 import argparse
@@ -25,7 +25,7 @@ import torch  # noqa: E402
 
 from moge_b200 import losses as engine  # noqa: E402
 from moge_b200.synthetic import synthetic_loss_case  # noqa: E402
-from oracle.compile_reference_losses import load_losses  # noqa: E402
+from oracle.compile_reference import load_losses  # noqa: E402
 
 SIZES = [(512, 512), (768, 1024), (1000, 1000)]
 LOSSES = [

@@ -6,7 +6,7 @@ line with the GPU name and power limit read in the same run.
 
 Each time is the median of separately timed calls after a warm-up call (CUDA events around the whole call, host work included),
 with the fastest and slowest beside it.  The comparator is loaded from oracle/_ref/ (built by __graft_entry__.build() when
-MOGE_REFERENCE is set, oracle/compile_reference_metrics.py) and is "not measured" without it; when present, the two results are compared at every timed size.
+MOGE_REFERENCE is set, oracle/compile_reference.py) and is "not measured" without it; when present, the two results are compared at every timed size.
 """
 import argparse
 import json
@@ -22,7 +22,7 @@ import torch  # noqa: E402
 
 from moge_b200 import metrics as engine  # noqa: E402
 from moge_b200.synthetic import METRICS_KEYS, synthetic_metrics_case  # noqa: E402
-from oracle.compile_reference_metrics import load_metrics  # noqa: E402
+from oracle.compile_reference import load_metrics  # noqa: E402
 
 WORKLOADS = [(480, 640, 50), (436, 872, 50), (1365, 2048, 100)]
 

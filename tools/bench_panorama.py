@@ -113,7 +113,7 @@ def main():
     ap.add_argument("--no-reference", action="store_true")
     args = ap.parse_args()
     name, power = gpu_info()
-    from oracle.compile_reference_panorama import load_panorama
+    from oracle.compile_reference import load_panorama
     ref = None if args.no_reference else load_panorama()
     from moge.model.v1 import MoGeModel
     from moge_b200.configs import v1_model_config
