@@ -392,6 +392,28 @@ int moge_loss_stencil(int kind, const float* points, const float* gt, int64_t ba
 int moge_loss_global(const float* pred, const float* gt, const float* params, float beta, int pass, int64_t batch, int H, int W,
                      float* grad, double* sums, void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- map colourisation (moge/utils/vis.py: colorize_depth, colorize_depth_affine, colorize_disparity, colorize_normal;
+ * Python: moge_b200.vis).  Maps are (batch, H, W) fp32 contiguous on the device, masks uint8 (nonzero = in), at most 2^30 pixels
+ * per image.  Results are bitwise those of oracle/vis_port.py and do not depend on the other images of the batch.  Value kinds:
+ * MOGE_VIS_DEPTH colours 1 / depth where depth > 0 (+inf depth is disparity 0), MOGE_VIS_VALUE the value itself; NaN values and
+ * pixels off the mask are excluded.                                                                                        */
+#define MOGE_VIS_MAX_QUANTILES 4
+enum { MOGE_VIS_DEPTH = 0, MOGE_VIS_VALUE = 1 };
+/* workspace (256-byte aligned) of moge_vis_quantiles */
+int moge_vis_workspace_bytes(int64_t batch, int H, int W, size_t* bytes);
+/* np.nanquantile(values, q[i]) of each image's valid values, linear method in fp32 (q is a host array of nq values in [0, 1]):
+ * out (batch, nq) fp32 on the device, NaN for an image without a valid value.  Same bits on every run; no host wait.        */
+int moge_vis_quantiles(const float* src, int kind, const uint8_t* mask, int64_t batch, int H, int W, const float* q, int nq, float* out,
+                       void* workspace, size_t workspace_bytes, void* stream);
+/* out (batch, H, W, 3) uint8 = the 256-entry RGB table lut (device, 768 bytes) at x * 256 with matplotlib's Colormap rules
+ * (256 -> 255, below 0 -> entry 0, 256 or more -> entry 255, NaN -> black), x the value normalised by range (batch, 2) = (lo,
+ * hi) on the device as (v - lo) / (hi - lo) (NULL: not normalised), then 1 - x when invert.  bgr swaps the channels.      */
+int moge_vis_colorize(const float* src, int kind, int invert, const uint8_t* mask, int64_t batch, int H, int W, const float* range,
+                      const uint8_t* lut, int bgr, uint8_t* out, void* stream);
+/* colorize_normal: out (batch, H, W, 3) uint8 = trunc(clip(n * (0.5, -0.5, -0.5) + 0.5, 0, 1) * 255) in fp64 of normal (batch, H,
+ * W, 3) fp32, n = 0 off the mask (may be NULL); bgr swaps the channels.                                                     */
+int moge_vis_normal(const float* normal, const uint8_t* mask, int64_t batch, int H, int W, int bgr, uint8_t* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -276,11 +276,12 @@ def _fov_x(intrinsics, device) -> torch.Tensor:
     return torch.tensor(fov_x, dtype=torch.float32, device=device)
 
 
-def infer_panorama(model, image: torch.Tensor, batch_size: Optional[int] = None) -> Dict[str, torch.Tensor]:
+def infer_panorama(model, image: torch.Tensor, batch_size: Optional[int] = None, return_views: bool = False) -> Dict[str, torch.Tensor]:
     """infer_panorama.py:83-122 without file I/O.  image: (H, W, 3) uint8 RGB CUDA tensor; model: an engine MoGeModel (MoGe-1 as in
     the reference, or MoGe-2) on the same device.  The 12 views go through one `model.infer(views, fov_x=..., apply_mask=False)`
     call, or calls of batch_size views (the reference's --batch_size).  Returns device tensors {'depth' (H, W), 'mask' (H, W) bool,
-    'points' (H, W, 3)}."""
+    'points' (H, W, 3)}.  With return_views, also what the script's --splitted option writes: 'views' (12, 512, 512, 3) uint8 RGB,
+    'view_distance' (12, 512, 512) = the views' points.norm(dim=-1), and 'view_mask' (12, 512, 512) bool."""
     if batch_size is not None and int(batch_size) < 1:
         raise MogeError(f"infer_panorama: batch_size {batch_size} must be positive")
     if not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3:
@@ -289,7 +290,9 @@ def infer_panorama(model, image: torch.Tensor, batch_size: Optional[int] = None)
     H, W = image.shape[:2]
     _check_size("infer_panorama", H, W)
     extrinsics, intrinsics = _default_cameras()
-    views = split_panorama(image, extrinsics, intrinsics, SPLIT_RESOLUTION)
+    views = split_panorama(image, extrinsics, intrinsics, SPLIT_RESOLUTION, return_uint8=return_views)
+    if return_views:
+        views, views_u8 = views
     fov_x = _fov_x(intrinsics, image.device)
     step = len(views) if batch_size is None else int(batch_size)
     points, masks = [], []
@@ -300,5 +303,9 @@ def infer_panorama(model, image: torch.Tensor, batch_size: Optional[int] = None)
     points = points[0] if len(points) == 1 else torch.cat(points)
     masks = masks[0] if len(masks) == 1 else torch.cat(masks)
     depth, mask = merge_panorama(min(MERGE_WIDTH, W), min(MERGE_HEIGHT, H), points, masks, extrinsics, intrinsics)
+    view_points, view_masks = points, masks
     depth, mask, points = finish_panorama(depth, mask, H, W)
-    return {'depth': depth, 'mask': mask, 'points': points}
+    out = {'depth': depth, 'mask': mask, 'points': points}
+    if return_views:
+        out.update(views=views_u8, view_distance=view_points.norm(dim=-1), view_mask=view_masks)
+    return out
