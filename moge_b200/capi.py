@@ -10,8 +10,7 @@ import os
 from typing import Optional
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# MOGE_B200_LIB selects an A/B variant build (moge_b200/csrc/build.sh with MG_VARIANT=...); default: the product library
-LIB_PATH = os.environ.get("MOGE_B200_LIB") or os.path.join(_HERE, "_lib", "libmoge_b200.so")
+LIB_PATH = os.path.join(_HERE, "_lib", "libmoge_b200.so")
 
 MOGE_MAX_LEVELS, MOGE_MAX_TAPS, MOGE_MAX_MLP = 8, 8, 8
 F32, F16, BF16, U8 = 0, 1, 2, 3

@@ -3,13 +3,11 @@
 set -e
 cd "$(dirname "$0")"
 OUT=../_lib
-# MG_VARIANT=name builds an A/B variant next to the product library: objects in build_name/, _lib/libmoge_b200_name.so
-# (selected at run time with MOGE_B200_LIB=<path>; tools/ab_variants.py)
-BUILD=build${MG_VARIANT:+_$MG_VARIANT}
-LIB=libmoge_b200${MG_VARIANT:+_$MG_VARIANT}.so
+BUILD=build
+LIB=libmoge_b200.so
 mkdir -p $OUT $BUILD
-FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -I../../include $MG_EXTRA_FLAGS"
-# a change of flags (e.g. MG_EXTRA_FLAGS=-DMG_ATT_DEBUG) invalidates every object
+FLAGS="-gencode arch=compute_90a,code=sm_90a -lineinfo -O3 -std=c++17 -Xcompiler -fPIC -I../../include"
+# an edit of the flags line invalidates every object
 if [ "$(cat $BUILD/.flags 2>/dev/null)" != "$FLAGS" ]; then rm -f $BUILD/*.o; echo "$FLAGS" > $BUILD/.flags; fi
 pids=()
 for f in gemm_rows gemm_tiles conv64 convh gemm attention elementwise pack tmap peer engine align v1 metrics mesh panorama losses vis; do

@@ -550,7 +550,8 @@ def test_plan_cache_is_bounded_and_frees_device_memory():
 
 def test_graph_replay_with_fresh_output_tensors():
     """Batch-1 calls replay ONE CUDA graph of the workspace-only launches; the caller-bound input / output kernels run eagerly
-    around it, so keeping earlier results alive (fresh output addresses on every call) neither re-captures nor corrupts."""
+    around it, so keeping earlier results alive (fresh output addresses on every call) neither re-captures nor corrupts.
+    A call above the graph limit (4 x 3600 tokens) runs every launch eagerly, and its repeats are bitwise equal too."""
     model, cfg, sd = get_model("vits", True, 1)
     imgs = [synthetic_images(1, 98, 126, 200 + i).to(DEV) for i in range(6)]
     kept = [model.infer(im, num_tokens=63) for im in imgs]                 # results kept alive -> distinct output tensors
@@ -563,6 +564,11 @@ def test_graph_replay_with_fresh_output_tensors():
         for k in a:
             assert torch.equal(a[k], b[k]), k
     assert not torch.equal(kept[0]["depth"], kept[1]["depth"])
+    big = synthetic_images(5, 224, 224, 5).to(DEV)                          # 5 x 60 x 60 = 18 000 tokens in one call
+    a, b = model.forward(big, 3600), model.forward(big, 3600)
+    torch.cuda.synchronize()
+    for k in a:
+        assert torch.equal(a[k], b[k]), k
 
 
 @pytest.mark.skipif(torch.cuda.device_count() < 2, reason="needs two GPUs")

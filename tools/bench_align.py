@@ -13,7 +13,6 @@ is set) and is "not measured" without it; when present, the engine's outputs are
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -21,6 +20,7 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
+from measure import cuda_samples, gpu_identity, summary  # noqa: E402
 from moge_b200 import alignment as engine  # noqa: E402
 from oracle.compile_reference import load_alignment  # noqa: E402
 
@@ -44,22 +44,6 @@ def workload(mod, name, pred, gt):
     return mod.align_points_scale_z_shift(pred, gt, 1 / gt.norm(dim=-1), trunc=1.0)
 
 
-def time_ms(fn, iters, per):
-    """{median, min, max} over `iters` calls, each timed with CUDA events, in ms divided by `per` (images per call)"""
-    fn()
-    torch.cuda.synchronize()
-    samples = []
-    for _ in range(iters):
-        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        start.record()
-        fn()
-        end.record()
-        torch.cuda.synchronize()
-        samples.append(start.elapsed_time(end) / per)
-    samples.sort()
-    return {"median": samples[len(samples) // 2], "min": samples[0], "max": samples[-1], "samples": len(samples)}
-
-
 def element_evaluations(name, n):
     """anchors x elements x sorted passes per image (pass A untruncated; A, B and C truncated), summed over the workload's
     solvers; every weight is positive, so every point is an anchor"""
@@ -75,25 +59,20 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--ref-iters", type=int, default=5)
     a = ap.parse_args()
+    result = {"metric": "alignment_ms_per_image", **gpu_identity(), "n": a.n, "rows": []}
     ref = load_alignment()
-    try:
-        pl = float(subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
-                                  capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0])
-    except Exception:
-        pl = None
-    result = {"metric": "alignment_ms_per_image", "gpu": torch.cuda.get_device_name(0), "power_limit_w": pl, "n": a.n, "rows": []}
     for name in ("eval", "train"):
         for batch in a.batches:
             pred, gt = inputs(batch, a.n, 0)
             row = {"workload": name, "batch": batch, "element_evaluations_per_image": element_evaluations(name, a.n)}
-            row["engine_ms_per_image"] = time_ms(lambda: workload(engine, name, pred, gt), a.iters, batch)
+            row["engine_ms_per_image"] = summary(cuda_samples(lambda: workload(engine, name, pred, gt), a.iters), batch)
             if ref is None:
                 row["reference_ms_per_image"] = "not measured"
             else:
                 # the reference's chunked solvers allocate anchors x 3n tensors per chunk; one image at a time bounds their memory
                 def run_ref():
                     return [workload(ref, name, pred[i:i + 1], gt[i:i + 1]) for i in range(min(batch, 2))]
-                row["reference_ms_per_image"] = time_ms(run_ref, a.ref_iters, min(batch, 2))
+                row["reference_ms_per_image"] = summary(cuda_samples(run_ref, a.ref_iters), min(batch, 2))
                 got, want = workload(engine, name, pred[:2], gt[:2]), run_ref()
                 got = got if isinstance(got, tuple) else (got,)
                 worst = 0.0

@@ -16,7 +16,6 @@ Everything is written under a temporary directory.
 import argparse
 import json
 import os
-import subprocess
 import sys
 import tempfile
 import time
@@ -30,6 +29,7 @@ import cv2  # noqa: E402
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from measure import cuda_samples, gpu_identity, summary  # noqa: E402
 from moge_b200 import cli, vis  # noqa: E402
 from moge_b200.export import save_glb, save_ply  # noqa: E402
 from oracle import utils3d_mesh, vis_port  # noqa: E402
@@ -44,26 +44,6 @@ EXR = [cv2.IMWRITE_EXR_TYPE, cv2.IMWRITE_EXR_TYPE_FLOAT]
 THRESHOLD = float("inf")
 
 
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    name, power = [s.strip() for s in q.stdout.strip().splitlines()[0].split(",")]
-    return name, power
-
-
-def timed(fn, iters):
-    fn()
-    torch.cuda.synchronize()
-    times = []
-    for _ in range(iters):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        times.append(a.elapsed_time(b))
-    return float(np.median(times))
-
-
 def kernels(iters):
     rows = []
     g = torch.Generator(device="cpu").manual_seed(0)
@@ -72,8 +52,8 @@ def kernels(iters):
             depth = (torch.rand(B, H, W, generator=g) * 10 + 0.5).to(DEV)
             normal = torch.nn.functional.normalize(torch.randn(B, H, W, 3, generator=g), dim=-1).to(DEV)
             px = B * H * W
-            t_depth = timed(lambda: vis.colorize_depth(depth), iters)
-            t_normal = timed(lambda: vis.colorize_normal(normal), iters)
+            t_depth = summary(cuda_samples(lambda: vis.colorize_depth(depth), iters))["median"]
+            t_normal = summary(cuda_samples(lambda: vis.colorize_normal(normal), iters))["median"]
             # colorize_depth: 4 select passes + the colouring pass each read the depth; the colouring writes 3 bytes
             bytes_depth, bytes_normal = px * (5 * 4 + 3), px * (12 + 3)
             row = {"H": H, "W": W, "batch": B, "colorize_depth_ms": round(t_depth, 4), "colorize_normal_ms": round(t_normal, 4),
@@ -171,10 +151,7 @@ def main():
     ap.add_argument("--images", type=int, default=32)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        raise SystemExit("bench_cli needs a CUDA device")
-    name, power = gpu_info()
-    res = {"bench": "cli", "gpu": name, "power_limit": power, "kernels": kernels(a.iters), "end_to_end": end_to_end(a.images)}
+    res = {"bench": "cli", **gpu_identity(), "kernels": kernels(a.iters), "end_to_end": end_to_end(a.images)}
     line = json.dumps(res)
     print(line)
     if a.out:

@@ -15,7 +15,6 @@ timed size.
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -23,6 +22,7 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
+from measure import cuda_samples, gpu_identity, summary  # noqa: E402
 from moge_b200 import losses as engine  # noqa: E402
 from moge_b200.synthetic import synthetic_loss_case  # noqa: E402
 from oracle.compile_reference import load_losses  # noqa: E402
@@ -46,21 +46,6 @@ def call(module, fn, names, kwargs, inputs):
     return loss.detach(), args[0].grad
 
 
-def time_ms(fn, iters):
-    fn()
-    torch.cuda.synchronize()
-    samples = []
-    for _ in range(iters):
-        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        start.record()
-        fn()
-        end.record()
-        torch.cuda.synchronize()
-        samples.append(start.elapsed_time(end))
-    samples.sort()
-    return {"median": samples[len(samples) // 2], "min": samples[0], "max": samples[-1], "samples": len(samples)}
-
-
 def peak_mb(fn):
     torch.cuda.synchronize()
     base = torch.cuda.memory_allocated()
@@ -75,26 +60,20 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--ref-iters", type=int, default=10)
     a = ap.parse_args()
+    result = {"metric": "training_loss_ms_forward_backward_per_image", **gpu_identity(), "rows": []}
     ref = load_losses()
-    try:
-        pl = float(subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
-                                  capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0])
-    except Exception:
-        pl = None
-    result = {"metric": "training_loss_ms_forward_backward_per_image", "gpu": torch.cuda.get_device_name(0), "power_limit_w": pl,
-              "rows": []}
     for H, W in SIZES:
         inputs = {k: v.cuda() for k, v in synthetic_loss_case(0, (1,), H, W).items()}
         for name, fn, names, kwargs in LOSSES:
             row = {"H": H, "W": W, "loss": name}
             run_e = lambda: call(engine, fn, names, kwargs, inputs)  # noqa: E731
-            row["engine_ms"] = time_ms(run_e, a.iters)
+            row["engine_ms"] = summary(cuda_samples(run_e, a.iters))
             row["engine_peak_mb"] = peak_mb(run_e)
             if ref is None:
                 row["reference_ms"] = row["reference_peak_mb"] = "not measured"
             else:
                 run_r = lambda: call(ref, fn, names, kwargs, inputs)  # noqa: E731
-                row["reference_ms"] = time_ms(run_r, a.ref_iters)
+                row["reference_ms"] = summary(cuda_samples(run_r, a.ref_iters))
                 row["reference_peak_mb"] = peak_mb(run_r)
                 (le, ge), (lr, gr) = run_e(), run_r()
                 row["loss_rel_diff"] = float(((le.double() - lr.double()).abs() / lr.double().abs().clamp_min(1e-30)).max())

@@ -20,7 +20,6 @@ Agreement with the host path is checked bitwise for the first and last image at 
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -30,6 +29,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from measure import cuda_samples, gpu_identity, summary  # noqa: E402
 from moge_b200 import mesh as M  # noqa: E402
 from moge_b200.synthetic import synthetic_mesh_case  # noqa: E402
 from oracle import utils3d_mesh as O  # noqa: E402
@@ -37,11 +37,6 @@ from oracle import utils3d_mesh as O  # noqa: E402
 WORKLOADS = [(518, 518), (768, 1024), (1365, 2048)]
 BATCHES = (1, 8)
 HBM_BYTES_PER_S = 3.35e12
-
-
-def stats(samples):
-    samples = sorted(samples)
-    return {"median": samples[len(samples) // 2], "min": samples[0], "max": samples[-1], "samples": len(samples)}
 
 
 def kernel_bytes(B, H, W, nv, nq):
@@ -57,12 +52,7 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--host-iters", type=int, default=3)
     a = ap.parse_args()
-    try:
-        pl = float(subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
-                                  capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0])
-    except Exception:
-        pl = None
-    result = {"metric": "mesh_from_output_ms_per_image", "gpu": torch.cuda.get_device_name(0), "power_limit_w": pl,
+    result = {"metric": "mesh_from_output_ms_per_image", **gpu_identity(),
               "host_comparator": "numpy restatement of utils3d (oracle/utils3d_mesh.py), not utils3d itself",
               "host_cpus": os.cpu_count(), "hbm_data_sheet_bytes_per_s": HBM_BYTES_PER_S, "rows": []}
     for H, W in WORKLOADS:
@@ -86,16 +76,7 @@ def main():
                 ws, totals, _, _ = M._count(cleaned, B, H, W, d.device)
                 M._emit(cleaned, B, H, W, maps, True, ws, totals, faces, rows)
 
-            device_chain()
-            torch.cuda.synchronize()
-            dev = []
-            for _ in range(a.iters):
-                s, e = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                s.record()
-                device_chain()
-                e.record()
-                torch.cuda.synchronize()
-                dev.append(s.elapsed_time(e) / B)
+            dev_s = summary(cuda_samples(device_chain, a.iters), B)
 
             def end_to_end():
                 r = M.mesh_from_output(out, image)
@@ -117,7 +98,7 @@ def main():
                     maps_h = {k: out[k][0].cpu().numpy() for k in ("points", "depth", "mask", "normal")}
                     want0 = O.mesh_from_output(maps_h["points"], maps_h["depth"], maps_h["mask"], img_cpu[0].numpy(), maps_h["normal"])
                     hs.append((time.perf_counter() - t0) * 1e3)
-                host = stats(hs)
+                host = summary(hs)
             agree = True
             for b in sorted({0, B - 1}):
                 want = want0 if b == 0 else O.mesh_from_output(out_cpu["points"][b].numpy(), out_cpu["depth"][b].numpy(),
@@ -126,11 +107,10 @@ def main():
                 agree &= np.array_equal(got["faces"].numpy(), want["faces"]) and np.array_equal(got["mask_cleaned"].numpy(), want["mask_cleaned"])
                 for k in ("vertices", "vertex_colors", "vertex_uvs", "vertex_normals"):
                     agree &= got[k].numpy().tobytes() == want[k].tobytes()
-            dev_s = stats(dev)
             nbytes = kernel_bytes(B, H, W, nv, nq)
             gbs = nbytes / B / (dev_s["median"] * 1e-3) / 1e9
             row = {"H": H, "W": W, "batch": B, "vertices_per_image": nv / B, "triangles_per_image": 2 * nq / B,
-                   "engine_device_ms_per_image": dev_s, "engine_end_to_end_ms_per_image": stats(e2e),
+                   "engine_device_ms_per_image": dev_s, "engine_end_to_end_ms_per_image": summary(e2e),
                    "host_numpy_ms_per_image": host, "kernel_bytes_per_image": nbytes / B, "kernel_gb_per_s": gbs,
                    "fraction_of_3_35_tb_per_s": gbs * 1e9 / HBM_BYTES_PER_S, "bitwise_agreement": bool(agree)}
             result["rows"].append(row)

@@ -12,7 +12,6 @@ import argparse
 import json
 import math
 import os
-import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -20,26 +19,12 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
+from measure import cuda_samples, gpu_identity, summary  # noqa: E402
 from moge_b200 import metrics as engine  # noqa: E402
 from moge_b200.synthetic import METRICS_KEYS, synthetic_metrics_case  # noqa: E402
 from oracle.compile_reference import load_metrics  # noqa: E402
 
 WORKLOADS = [(480, 640, 50), (436, 872, 50), (1365, 2048, 100)]
-
-
-def time_ms(fn, iters, per):
-    fn()
-    torch.cuda.synchronize()
-    samples = []
-    for _ in range(iters):
-        start, end = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        start.record()
-        fn()
-        end.record()
-        torch.cuda.synchronize()
-        samples.append(start.elapsed_time(end) / per)
-    samples.sort()
-    return {"median": samples[len(samples) // 2], "min": samples[0], "max": samples[-1], "samples": len(samples)}
 
 
 def flat(m, prefix=""):
@@ -54,14 +39,8 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--ref-iters", type=int, default=3)
     a = ap.parse_args()
+    result = {"metric": "compute_metrics_ms_per_image", **gpu_identity(), "keys": list(METRICS_KEYS["moge2"]), "rows": []}
     ref = load_metrics()
-    try:
-        pl = float(subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
-                                  capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0])
-    except Exception:
-        pl = None
-    result = {"metric": "compute_metrics_ms_per_image", "gpu": torch.cuda.get_device_name(0), "power_limit_w": pl,
-              "keys": list(METRICS_KEYS["moge2"]), "rows": []}
     for H, W, segments in WORKLOADS:
         cases = []
         for i in range(8):
@@ -72,12 +51,12 @@ def main():
               for k in cases[0][1] if k != "segmentation_labels"}
         gt["segmentation_labels"] = [c[1]["segmentation_labels"] for c in cases]
         row = {"H": H, "W": W, "segments": segments + 3}
-        row["engine_b1_ms_per_image"] = time_ms(lambda: engine.compute_metrics(*cases[0]), a.iters, 1)
-        row["engine_b8_ms_per_image"] = time_ms(lambda: engine.compute_metrics_batch(pred, gt), a.iters, 8)
+        row["engine_b1_ms_per_image"] = summary(cuda_samples(lambda: engine.compute_metrics(*cases[0]), a.iters))
+        row["engine_b8_ms_per_image"] = summary(cuda_samples(lambda: engine.compute_metrics_batch(pred, gt), a.iters), 8)
         if ref is None:
             row["reference_ms_per_image"] = "not measured"
         else:
-            row["reference_ms_per_image"] = time_ms(lambda: ref.compute_metrics(*cases[0]), a.ref_iters, 1)
+            row["reference_ms_per_image"] = summary(cuda_samples(lambda: ref.compute_metrics(*cases[0]), a.ref_iters))
             got, want = flat(engine.compute_metrics(*cases[0])[0]), flat(ref.compute_metrics(*cases[0])[0])
             row["keys_agree"] = got.keys() == want.keys()
             row["max_abs_diff_vs_reference"] = max((abs(got[k] - want[k]) for k in want if k in got and not math.isnan(want[k])), default=None)

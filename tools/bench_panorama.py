@@ -11,7 +11,6 @@ oracle/_ref/ and cv2 / SciPy are installed; otherwise its numbers are "not measu
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -21,16 +20,11 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from measure import cuda_samples, gpu_identity  # noqa: E402
 from moge_b200 import panorama as P  # noqa: E402
 from moge_b200.synthetic import synthetic_panorama, synthetic_room_views  # noqa: E402
 
 DEV = "cuda:0"
-
-
-def gpu_info():
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True)
-    name, power = [x.strip() for x in q.stdout.strip().splitlines()[0].split(",")]
-    return name, power
 
 
 class Timer:
@@ -66,7 +60,7 @@ def staged(model, image):
 
 def merge_levels_ms(src, mask, width, height, extr, intr):
     """The merge alone, one event pair around each level's right-hand side + solve (resize included)."""
-    ms, evs = [], []
+    timers = []
     import ctypes as C
     from moge_b200 import capi
     L = capi.lib()
@@ -82,28 +76,28 @@ def merge_levels_ms(src, mask, width, height, extr, intr):
     init = None
     st = capi.current_stream()
     for lv, (w, h) in enumerate(levels):
-        e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True); e2 = torch.cuda.Event(enable_timing=True)
         b = torch.empty(P.num_rows(h, w), dtype=torch.float64, device=DEV)
         rm = torch.empty_like(b, dtype=torch.uint8)
         pm = torch.empty(h, w, dtype=torch.uint8, device=DEV)
         dirs = P._table("dirs", (h, w), torch.device(DEV))
-        e0.record()
+        t = Timer()
+        t.mark("start")
         capi.check(L.moge_panorama_rhs(s.data_ptr(), ch, m.data_ptr(), n, s.shape[1], s.shape[2], cams, dirs.data_ptr(), h, w,
                                        b.data_ptr(), rm.data_ptr(), pm.data_ptr(), ws.data_ptr(), ws.numel(), st))
-        e1.record()
+        t.mark("rhs_ms")
         depth = torch.empty(h, w, dtype=torch.float32, device=DEV)
         capi.check(L.moge_panorama_lsmr(b.data_ptr(), rm.data_ptr(), h, w, capi.ptr(init), depth.data_ptr(), stats[lv].data_ptr(),
                                         ws.data_ptr(), ws.numel(), st))
-        e2.record()
-        evs.append((w, h, e0, e1, e2))
+        t.mark("lsmr_ms")
+        timers.append(t)
         if lv + 1 < len(levels):
             W2, H2 = levels[lv + 1]
             init = torch.empty(H2, W2, dtype=torch.float32, device=DEV)
             capi.check(L.moge_panorama_resize(depth.data_ptr(), h, w, H2, W2, init.data_ptr(), st))
     torch.cuda.synchronize()
     it = stats.cpu().tolist()
-    return [{"size": f"{w}x{h}", "rhs_ms": round(a.elapsed_time(b_), 3), "lsmr_ms": round(b_.elapsed_time(c), 3), "iterations": i[0],
-             "istop": i[1]} for (w, h, a, b_, c), i in zip(evs, it)]
+    return [{"size": f"{w}x{h}", **{k: round(v, 3) for k, v in t.result().items()}, "iterations": i[0], "istop": i[1]}
+            for (w, h), t, i in zip(levels, timers, it)]
 
 
 def main():
@@ -112,7 +106,7 @@ def main():
     ap.add_argument("--out", default=None)
     ap.add_argument("--no-reference", action="store_true")
     args = ap.parse_args()
-    name, power = gpu_info()
+    gpu = gpu_identity()
     from oracle.compile_reference import load_panorama
     ref = None if args.no_reference else load_panorama()
     from moge.model.v1 import MoGeModel
@@ -122,7 +116,7 @@ def main():
     model = MoGeModel(**cfg)
     model.load_state_dict(make_v1_state_dict(cfg, 30, well_posed=True))
     model = model.to(DEV).eval()
-    result = {"gpu": name, "power_limit": power, "model": "MoGe-1 ViT-L (synthetic weights), resolution level 9", "workloads": []}
+    result = {**gpu, "model": "MoGe-1 ViT-L (synthetic weights), resolution level 9", "workloads": []}
     for H, W in ((1024, 2048), (2048, 4096)):
         img = torch.from_numpy(synthetic_panorama(H, W, 1))
         dimg = img.to(DEV)
@@ -170,16 +164,9 @@ def main():
     dist, masks = synthetic_room_views(512)
     extr, intr = P.get_panorama_cameras()
     src, msk = torch.from_numpy(dist).to(DEV), torch.from_numpy(masks).to(DEV)
-    P.merge_panorama(1920, 960, src, msk, extr, intr)
+    dep, pm = P.merge_panorama(1920, 960, src, msk, extr, intr)        # warm-up; the merge is repeatable, so also the result
     room = {"merge": "room 1920x960 from 12 x 512^2 distance maps", "levels": merge_levels_ms(src, msk, 1920, 960, extr, intr)}
-    t = []
-    for _ in range(args.steps):
-        e0 = torch.cuda.Event(enable_timing=True); e1 = torch.cuda.Event(enable_timing=True)
-        e0.record()
-        dep, pm = P.merge_panorama(1920, 960, src, msk, extr, intr)
-        e1.record()
-        torch.cuda.synchronize()
-        t.append(e0.elapsed_time(e1))
+    t = cuda_samples(lambda: P.merge_panorama(1920, 960, src, msk, extr, intr), args.steps, warmup=0)
     room["merge_ms"] = round(float(np.median(t)), 2)
     if ref is not None:
         t0 = time.perf_counter()

@@ -20,7 +20,6 @@ the threshold, where they may), and the mesh bitwise against build_mesh_from_map
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -30,6 +29,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from measure import gpu_identity, summary  # noqa: E402
 from moge_b200 import mesh as M  # noqa: E402
 from moge_b200.synthetic import synthetic_panorama, synthetic_panorama_scene  # noqa: E402
 from oracle import utils3d_mesh as OM  # noqa: E402
@@ -39,10 +39,9 @@ SIZES = [(1024, 2048), (2048, 4096)]
 DEV = "cuda"
 
 
-def stats(samples):
-    samples = sorted(samples)
-    return {"median": round(samples[len(samples) // 2], 3), "min": round(samples[0], 3), "max": round(samples[-1], 3),
-            "samples": len(samples)}
+def summary_ms(samples):
+    """summary() to the microsecond"""
+    return {k: round(v, 3) for k, v in summary(samples).items()}
 
 
 def v1_model():
@@ -109,8 +108,8 @@ def measure(out, image, iters, host_iters):
     bitwise = np.array_equal(pinned["faces"].numpy(), mesh_want[0]) and all(
         pinned[k].numpy().tobytes() == w.tobytes() for k, w in zip(("vertices", "vertex_colors", "vertex_uvs"), mesh_want[1:]))
     return {"size": f"{W}x{H}", "vertices": nv, "triangles": nf, "pixels_cleaned": int((hm & ~cleaned).sum()),
-            "engine_device_ms": stats(dev), "engine_device_clean_ms": stats(clean), "engine_device_mesh_ms": stats(mesh),
-            "engine_end_to_end_ms": stats(e2e), "host_numpy_ms": stats(hs),
+            "engine_device_ms": summary_ms(dev), "engine_device_clean_ms": summary_ms(clean),
+            "engine_device_mesh_ms": summary_ms(mesh), "engine_end_to_end_ms": summary_ms(e2e), "host_numpy_ms": summary_ms(hs),
             "agreement": {"mask_cleaned_mismatch": int((cleaned != want["mask_cleaned"]).sum()), "pixels_near_threshold": int(near.sum()),
                           "mesh_bitwise_on_engine_mask": bool(bitwise),
                           "mesh_bitwise_vs_host": bool(np.array_equal(pinned["faces"].numpy(), want["faces"])
@@ -123,10 +122,7 @@ def main():
     ap.add_argument("--host-iters", type=int, default=2)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                       timeout=30)
-    name, power = [x.strip() for x in q.stdout.strip().splitlines()[0].split(",")]
-    result = {"metric": "mesh_from_panorama_ms", "gpu": name, "power_limit": power, "host_cpus": os.cpu_count(),
+    result = {"metric": "mesh_from_panorama_ms", **gpu_identity(), "host_cpus": os.cpu_count(),
               "host_comparator": "numpy restatement of utils3d (oracle/utils3d_normals.py), not utils3d itself", "rows": []}
     model = None
     for H, W in SIZES:

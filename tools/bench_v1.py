@@ -12,7 +12,6 @@ import argparse
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
@@ -21,27 +20,7 @@ sys.path.insert(0, ROOT)
 
 import torch  # noqa: E402
 
-
-def gpu_info():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True,
-                             timeout=30).stdout.strip().splitlines()[0]
-        name, power = [s.strip() for s in out.split(",")]
-        return name, power
-    except Exception:
-        return torch.cuda.get_device_name(0), "unknown"
-
-
-def timed_calls(fn, n):
-    ts = []
-    for _ in range(n):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record()
-        fn()
-        b.record()
-        b.synchronize()
-        ts.append(a.elapsed_time(b))
-    return ts
+from measure import cuda_samples, gpu_identity  # noqa: E402
 
 
 def main():
@@ -51,8 +30,7 @@ def main():
     ap.add_argument("--iters", type=int, default=200)
     ap.add_argument("--warmup", type=int, default=10)
     a = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("bench_v1 measures on a GPU; none is visible")
+    gpu = gpu_identity()
     from moge.model.v1 import MoGeModel
     from moge_b200.configs import v1_model_config
     from moge_b200.synthetic import make_v1_state_dict, synthetic_images
@@ -69,10 +47,7 @@ def main():
     imgB = synthetic_images(a.batch, 518, 518, 1).to(dev)
 
     # batch 1 latency
-    for _ in range(a.warmup):
-        model.forward(img1, tokens)
-    torch.cuda.synchronize()
-    t1 = timed_calls(lambda: model.forward(img1, tokens), a.iters)
+    t1 = cuda_samples(lambda: model.forward(img1, tokens), a.iters, a.warmup)
     # throughput at --batch
     for _ in range(2):
         model.forward(imgB, tokens)
@@ -97,10 +72,7 @@ def main():
     with torch.inference_mode():
         def port1():
             return moge_v1_port.forward(cfg, sd16, img1.half(), tokens)
-        for _ in range(3):
-            port1()
-        torch.cuda.synchronize()
-        tp = timed_calls(port1, 20)
+        tp = cuda_samples(port1, 20, 3)
         nb = min(a.batch, 8)
         port_b = lambda: moge_v1_port.forward(cfg, sd16, imgB[:nb].half(), tokens)  # noqa: E731
         port_b()
@@ -116,11 +88,10 @@ def main():
         out = model.forward(img1, tokens)
         agree = {k: float(((out[k].double() - ref[k].double()).norm() / ref[k].double().norm()).item()) for k in ("points", "mask")}
 
-    name, power = gpu_info()
     q = statistics.quantiles(t1, n=10)
     print(json.dumps({
         "workload": "MoGe-1 ViT-L fp16, 518x518, resolution level 9 (2500 tokens, 700x700, grid 50x50), synthetic weights",
-        "gpu": name, "power_limit": power,
+        **gpu,
         "engine": {"images_per_s": round(ips, 2), "batch": a.batch, "steps": a.steps,
                    "batch1_p50_ms": round(statistics.median(t1), 3), "batch1_p90_ms": round(q[8], 3), "batch1_iters": a.iters},
         "port_fp16": {"batch1_p50_ms": round(statistics.median(tp), 3), "images_per_s": round(port_ips, 2), "batch": nb},

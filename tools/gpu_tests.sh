@@ -4,7 +4,7 @@
 mkdir -p gpurun_out
 nvidia-smi --query-gpu=name,driver_version,memory.total --format=csv > gpurun_out/gpu_info.txt 2>&1
 rc=0
-for f in tests/test_gpu_geometry.py tests/test_gpu_ops.py tests/test_gpu_conv_epilogue.py tests/test_gpu_gemm_rows.py tests/test_gpu_model.py tests/test_gpu_peer.py tests/test_gpu_alignment.py tests/test_gpu_v1.py tests/test_gpu_metrics.py tests/test_gpu_mesh.py tests/test_gpu_panorama.py tests/test_gpu_panorama_mesh.py tests/test_gpu_losses.py tests/test_gpu_vis.py tests/test_gpu_cli.py; do
+for f in tests/test_gpu_*.py; do
   name=$(basename $f .py)
   timeout 900 python -m pytest $f -q -m gpu -s "$@" > gpurun_out/$name.log 2>&1
   r=$?
