@@ -357,7 +357,7 @@ int moge_panorama_resize(const float* src, int h, int w, int H, int W, float* ds
 int moge_panorama_finish(const float* depth, const uint8_t* mask, int h, int w, int H, int W, float* depth_out, uint8_t* mask_out,
                          float* points, void* stream);
 
-/* ---- training losses, the deterministic subset of moge/train/losses.py (Python: moge_b200.losses).
+/* ---- training losses of moge/train/losses.py except normal_map_loss (Python: moge_b200.losses).
  * Maps are (batch, H, W) fp32 and point maps (batch, H, W, 3) fp32, contiguous on the device.  Each call either reduces
  * (coef NULL): sums (batch, MOGE_LOSS_SUMS) doubles, fp64 over fixed tiles set by H x W and added in tile order, so results do
  * not change from run to run nor with the other images of the batch; or computes a gradient (coef given): grad = coef[image]
@@ -391,6 +391,29 @@ int moge_loss_stencil(int kind, const float* points, const float* gt, int64_t ba
  *   pass 2: grad = d(pass 1's first sum)/dp times coef, sums = (dL/dscale, dL/dshift x, y, z).  */
 int moge_loss_global(const float* pred, const float* gt, const float* params, float beta, int pass, int64_t batch, int H, int W,
                      float* grad, double* sums, void* workspace, size_t workspace_bytes, void* stream);
+/* sampled local loss.  compute_anchor_sampling_weight's per-pixel pass: pixel (b, i, j) with mask (batch, H, W) u8 counts the
+ * num_test offsets di, dj (H, W, num_test) int64 (shared by the images) whose target (i + di, j + dj) is inside the map, valid
+ * and within radius[b, i, j] of points[b, i, j] (fp32 |d| = sqrt((dx^2 + dy^2) + dz^2)); weight (batch, H, W) fp32 =
+ * mask ? 1 / max(count, 1) : 0.  No workspace. */
+int moge_loss_anchor_weight(const float* points, const uint8_t* mask, const int64_t* di, const int64_t* dj, const float* radius,
+                            int64_t batch, int H, int W, int num_test, float* weight, void* stream);
+/* the P <= 65535 patches of side S = 2 r + 1 around anchor (P, 3) int64 (image, i, j): radius (P) = (1 / focal[image]) *
+ * half_level * gt z at the anchor; patch_mask (P, S, S) u8 marks the positions whose pixel is inside the map, valid in mask and
+ * within radius of the anchor's GT point; count (P) int32 = the marked positions.  gt (batch, H, W, 3) raw. */
+int moge_loss_patch_mask(const float* gt, const uint8_t* mask, const int64_t* anchor, const float* focal, float half_level,
+                         int64_t batch, int H, int W, int64_t P, int r, uint8_t* patch_mask, int* count, float* radius, void* stream);
+/* the local loss's passes.  params (P, MOGE_LOSS_LOCAL_PARAMS) fp32 per patch = (scale, shift x, y, z, valid (0 / 1), cap,
+ * radius, coef); at a marked position of a valid patch, q = scale p + shift and w = 1 / max(gt z, cap):
+ *   pass 0: sums (batch, 4) = (sum over valid GT of 1 / (z + 1e-7), valid count), per image (pred, anchor, params unused);
+ *   pass 1: sums (P, 4) = (sum over xyz of smooth(|q - g| w), position count, sum of min(err, 1), count of err < 1) with
+ *           err = |q - g| / radius, smooth as for moge_loss_global;
+ *   pass 2: sums (P, 4) = (dL/dscale, dL/dshift x, y, z) of pass 1's first sum times coef; with grad (batch, H, W, 3), also
+ *           dL/dpred, each pixel gathering its patches' terms in patch order.
+ * Workspace: moge_loss_workspace_bytes(batch, H, W) for pass 0, (P, S, S) for passes 1 and 2. */
+#define MOGE_LOSS_LOCAL_PARAMS 8
+int moge_loss_local(const float* pred, const float* gt, const int64_t* anchor, const float* params, const uint8_t* patch_mask,
+                    float beta, int pass, int64_t batch, int H, int W, int64_t P, int r, float* grad, double* sums, void* workspace,
+                    size_t workspace_bytes, void* stream);
 
 /* ---- map colourisation (moge/utils/vis.py: colorize_depth, colorize_depth_affine, colorize_disparity, colorize_normal;
  * Python: moge_b200.vis).  Maps are (batch, H, W) fp32 contiguous on the device, masks uint8 (nonzero = in), at most 2^30 pixels

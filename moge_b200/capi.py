@@ -32,7 +32,7 @@ EXPORTS = [
     "moge_mesh_workspace_bytes", "moge_depth_edge", "moge_mesh_count", "moge_mesh_build", "moge_normal_map", "moge_normal_edge",
     "moge_panorama_split", "moge_panorama_workspace_bytes", "moge_panorama_rhs", "moge_panorama_lsmr", "moge_panorama_resize",
     "moge_panorama_finish", "moge_loss_workspace_bytes", "moge_loss_mask", "moge_loss_stencil", "moge_loss_global",
-    "moge_vis_workspace_bytes", "moge_vis_quantiles", "moge_vis_colorize", "moge_vis_normal",
+    "moge_loss_anchor_weight", "moge_loss_patch_mask", "moge_loss_local", "moge_vis_workspace_bytes", "moge_vis_quantiles", "moge_vis_colorize", "moge_vis_normal",
 ]
 METRICS_MAX_SEGMENTS, METRICS_MAX_VARIANTS, METRICS_F1_THRESHOLDS, METRICS_F1_COUNTS, METRICS_OUT_SEGMENTS = 256, 8, 10, 90, 17
 (MV_DEPTH, MV_DEPTH_SCALE, MV_DEPTH_AFFINE, MV_DISPARITY, MV_DISPARITY_FROM_DEPTH, MV_POINTS_SHIFT, MV_POINTS_SCALE,
@@ -43,6 +43,7 @@ MESH_HWC, MESH_CHW = 0, 1
 PANORAMA_MAX_VIEWS = 20
 LOSS_SUMS = 4
 LOSS_MASK_L2, LOSS_MASK_BCE, LOSS_EDGE, LOSS_NORMAL = range(4)
+LOSS_LOCAL_PARAMS = 8
 VIS_MAX_QUANTILES = 4
 VIS_DEPTH, VIS_VALUE = 0, 1
 
@@ -186,6 +187,9 @@ def lib() -> C.CDLL:
     L.moge_loss_mask.argtypes = [ci, vp, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp]
     L.moge_loss_stencil.argtypes = [ci, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp]
     L.moge_loss_global.argtypes = [vp, vp, vp, C.c_float, ci, i64, ci, ci, vp, vp, vp, sz, vp]
+    L.moge_loss_anchor_weight.argtypes = [vp, vp, vp, vp, vp, i64, ci, ci, ci, vp, vp]
+    L.moge_loss_patch_mask.argtypes = [vp, vp, vp, vp, C.c_float, i64, ci, ci, i64, ci, vp, vp, vp, vp]
+    L.moge_loss_local.argtypes = [vp, vp, vp, vp, vp, C.c_float, ci, i64, ci, ci, i64, ci, vp, vp, vp, sz, vp]
     L.moge_vis_workspace_bytes.argtypes = [i64, ci, ci, C.POINTER(sz)]
     L.moge_vis_quantiles.argtypes = [vp, ci, vp, i64, ci, ci, fp, ci, vp, vp, sz, vp]
     L.moge_vis_colorize.argtypes = [vp, ci, ci, vp, i64, ci, ci, vp, vp, ci, vp, vp]

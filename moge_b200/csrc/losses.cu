@@ -1,5 +1,7 @@
 // Training losses (moge/train/losses.py of the reference): the per-pixel mask losses, the edge and normal stencil losses and the
-// per-pixel passes of the affine-invariant global loss, forward and backward.  Every image of a batch is independent.
+// per-pixel passes of the affine-invariant global loss, forward and backward; and the sampled local loss: its per-pixel anchor
+// counts, its patch masks, and its per-patch sums and per-pixel gradient.  Every image of a batch is independent, except that
+// the local loss's anchors are drawn (by torch, outside these kernels) over the whole batch.
 //
 // Reductions follow metrics.cu: the pixels of an image are cut into fixed tiles (set by H x W only), each CTA reduces its tile in
 // fp64 in a fixed order into one partial per quantity, and a finalize kernel adds an image's partials in tile order.  Backward
@@ -271,6 +273,203 @@ struct GlobalOp {
     }
 };
 
+// ---------------------------------------------------------------------------------------------------- local loss
+// |a - b| in fp32, summed as ((x^2 + y^2) + z^2); the fp64 square root rounded to fp32 is the fp32 square root (53 >= 2 * 24 + 2
+// bits: the double rounding is innocuous), without the fp32 slow path's call
+__device__ __forceinline__ float dist3(const float* a, const float* b) {
+    const float dx = __fsub_rn(a[0], b[0]), dy = __fsub_rn(a[1], b[1]), dz = __fsub_rn(a[2], b[2]);
+    return static_cast<float>(sqrt(static_cast<double>(__fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz)))));
+}
+
+// compute_anchor_sampling_weight: pixel (b, i, j) counts its num_test offsets (di, dj shared by the images) whose clamped target
+// is inside the map, valid and within radius[b, i, j] of it; weight = mask ? 1 / max(count, 1) : 0
+__global__ void __launch_bounds__(kThreads) anchor_weight_kernel(const float* __restrict__ points, const uint8_t* __restrict__ mask,
+                                                                 const int64_t* __restrict__ di, const int64_t* __restrict__ dj,
+                                                                 const float* __restrict__ radius, int64_t batch, int H, int W,
+                                                                 int num_test, float* __restrict__ weight) {
+    const int64_t hw = static_cast<int64_t>(H) * W;
+    const int64_t t = static_cast<int64_t>(blockIdx.x) * kThreads + threadIdx.x;
+    if (t >= batch * hw) return;
+    const int64_t b = t / hw, pix = t % hw;
+    const int i = static_cast<int>(pix / W), j = static_cast<int>(pix % W);
+    if (!mask[t]) { weight[t] = 0.f; return; }
+    const float* p = points + t * 3;
+    const float r = radius[t];
+    int count = 0;
+    for (int k = 0; k < num_test; ++k) {
+        const int64_t ti = i + di[pix * num_test + k], tj = j + dj[pix * num_test + k];
+        if (ti < 0 || ti >= H || tj < 0 || tj >= W) continue;
+        const int64_t q = b * hw + ti * W + tj;
+        if (mask[q] && dist3(points + q * 3, p) <= r) ++count;
+    }
+    weight[t] = __frcp_rn(static_cast<float>(count > 1 ? count : 1));
+}
+
+// the patches of the local loss: patch p = (image, anchor i, anchor j) = anchor[3 p ..], side S = 2 r + 1.  Position (u, v) is
+// pixel (ai - r + u, aj - r + v); it is in the patch mask when that pixel is inside the map, valid, and within the anchor's 3D
+// radius = (1 / focal) * half_level * anchor z (torch's `half_level / focal * z`).
+constexpr int kPatchPx = 4096;                  // positions per CTA of the patch-mask kernel
+
+__global__ void __launch_bounds__(kThreads) patch_mask_kernel(const float* __restrict__ gt, const uint8_t* __restrict__ mask,
+                                                              const int64_t* __restrict__ anchor, const float* __restrict__ focal,
+                                                              float half_level, int H, int W, int r, uint8_t* __restrict__ pmask,
+                                                              int* __restrict__ count, float* __restrict__ radius) {
+    __shared__ int red[kWarps];
+    const int64_t p = blockIdx.y;
+    const int S = 2 * r + 1;
+    const int64_t hw = static_cast<int64_t>(H) * W;
+    const int64_t b = anchor[p * 3], ai = anchor[p * 3 + 1], aj = anchor[p * 3 + 2];
+    const float* g0 = gt + (b * hw + ai * W + aj) * 3;
+    const float rad = __fmul_rn(__fmul_rn(__frcp_rn(focal[b]), half_level), g0[2]);
+    if (blockIdx.x == 0 && threadIdx.x == 0) radius[p] = rad;
+    int n = 0;
+    const int64_t k0 = static_cast<int64_t>(blockIdx.x) * kPatchPx, S2 = static_cast<int64_t>(S) * S;
+    for (int64_t k = k0 + threadIdx.x; k < k0 + kPatchPx && k < S2; k += kThreads) {
+        const int64_t i = ai - r + k / S, j = aj - r + k % S;
+        bool m = i >= 0 && i < H && j >= 0 && j < W;
+        if (m) {
+            const int64_t q = b * hw + i * W + j;
+            m = mask[q] && dist3(gt + q * 3, g0) <= rad;
+        }
+        pmask[p * S2 + k] = m;
+        n += m;
+    }
+    for (int o = 16; o > 0; o >>= 1) n += __shfl_xor_sync(0xffffffffu, n, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = n;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int s = 0;
+        for (int w = 0; w < kWarps; ++w) s += red[w];
+        atomicAdd(count + p, s);                // integer: the same total in any order
+    }
+}
+
+// per-patch parameters of the local loss (MOGE_LOSS_LOCAL_PARAMS floats)
+enum { LP_SCALE = 0, LP_SHIFT = 1, LP_VALID = 4, LP_CAP = 5, LP_RADIUS = 6, LP_COEF = 7 };
+
+struct LocalArgs {
+    const float* p; const float* g; const int64_t* anchor; const float* params; const uint8_t* pmask;
+    float beta; int H, W, r; int64_t P;
+};
+
+// d(smooth(|q - g| w))/dq for one coordinate, times coef; with val, also the term itself
+__device__ __forceinline__ float local_term(float diff, float w, float beta, float coef, float* val) {
+    const float e = __fmul_rn(fabsf(diff), w);
+    const bool quad = beta > 0.f && e < beta;
+    if (val) *val = beta > 0.f ? (quad ? __fdiv_rn(__fmul_rn(0.5f, __fmul_rn(e, e)), beta) : __fsub_rn(e, 0.5f * beta)) : e;
+    const float sgn = diff > 0.f ? 1.f : (diff < 0.f ? -1.f : 0.f);
+    return __fmul_rn(__fmul_rn(__fmul_rn(coef, quad ? __fdiv_rn(e, beta) : 1.f), w), sgn);
+}
+
+// pass 0: per image, (sum over valid GT of 1 / (z + 1e-7), valid count), for the harmonic mean of the GT depth
+struct HarmonicOp {
+    const float* g; int64_t hw;
+    __device__ void operator()(int64_t b, int64_t pix, double* acc) const {
+        const float* q = g + (b * hw + pix) * 3;
+        if (!(isfinite(q[0]) && isfinite(q[1]) && isfinite(q[2]))) return;
+        acc[0] += __frcp_rn(__fadd_rn(q[2], 1e-7f));
+        acc[1] += 1.0;
+    }
+};
+
+// passes 1 and 2 over the positions of a patch (its `b` is the patch), masked positions only: with q = scale p + shift,
+// pass 1: (sum of smooth(|q - g| w) over xyz, mask count, sum of min(err, 1), count of err < 1), err = |q - g| / radius;
+// pass 2: (dL/dscale, dL/dshift x, y, z) with dL/dterm = coef.
+struct PatchOp {
+    LocalArgs a; int pass;
+    __device__ void operator()(int64_t p, int64_t k, double* acc) const {
+        const int S = 2 * a.r + 1;
+        const float* pr = a.params + p * MOGE_LOSS_LOCAL_PARAMS;
+        if (pr[LP_VALID] == 0.f || !a.pmask[p * S * S + k]) return;
+        const int64_t b = a.anchor[p * 3];
+        const int64_t i = a.anchor[p * 3 + 1] - a.r + k / S, j = a.anchor[p * 3 + 2] - a.r + k % S;
+        const int64_t o = ((b * a.H + i) * a.W + j) * 3;
+        const float w = __frcp_rn(fmaxf(a.g[o + 2], pr[LP_CAP]));
+        float sq = 0.f, gscale = 0.f, loss = 0.f;
+        for (int c = 0; c < 3; ++c) {
+            const float diff = __fsub_rn(__fadd_rn(__fmul_rn(pr[LP_SCALE], a.p[o + c]), pr[LP_SHIFT + c]), a.g[o + c]);
+            if (pass == 1) {
+                float v;
+                local_term(diff, w, a.beta, 0.f, &v);
+                loss = __fadd_rn(loss, v);
+                sq = __fadd_rn(sq, __fmul_rn(diff, diff));
+            } else {
+                const float gq = local_term(diff, w, a.beta, pr[LP_COEF], nullptr);
+                gscale = __fadd_rn(gscale, __fmul_rn(gq, a.p[o + c]));
+                acc[1 + c] += gq;
+            }
+        }
+        if (pass == 1) {
+            const float err = __fdiv_rn(sqrtf(sq), pr[LP_RADIUS]);
+            acc[0] += loss;
+            acc[1] += 1.0;
+            acc[2] += err > 1.f ? 1.f : err;
+            acc[3] += err < 1.f ? 1.0 : 0.0;
+        } else {
+            acc[0] += gscale;
+        }
+    }
+};
+
+// dL/dpred of the local loss: one thread per pixel gathers, in patch order, the terms of every patch position on it.  A CTA
+// covers a kTile x kTile pixel tile of one image; it scans the patches kThreads at a time and lists, in patch order, those of
+// its image whose box meets the tile, then each thread adds the listed patches' terms at its pixels.
+constexpr int kTile = 16;
+constexpr int kRows = kTile * kTile / kThreads;  // pixels per thread
+
+__global__ void __launch_bounds__(kThreads) local_grad_kernel(LocalArgs a, float* __restrict__ grad) {
+    __shared__ int list[kThreads];
+    __shared__ int listed;
+    const int64_t b = blockIdx.z;
+    const int i0 = blockIdx.y * kTile, j0 = blockIdx.x * kTile;
+    const int lane = threadIdx.x & 31;
+    const int S = 2 * a.r + 1;
+    float g[kRows][3] = {};
+    for (int64_t c0 = 0; c0 < a.P; c0 += kThreads) {
+        if (threadIdx.x < 32) {                 // warp 0 lists the chunk's patches that meet the tile, in order
+            int n = 0;
+            for (int s = 0; s < kThreads; s += 32) {
+                const int64_t p = c0 + s + lane;
+                bool hit = false;
+                if (p < a.P && a.anchor[p * 3] == b && a.params[p * MOGE_LOSS_LOCAL_PARAMS + LP_VALID] != 0.f) {
+                    const int64_t ai = a.anchor[p * 3 + 1], aj = a.anchor[p * 3 + 2];
+                    hit = ai + a.r >= i0 && ai - a.r < i0 + kTile && aj + a.r >= j0 && aj - a.r < j0 + kTile;
+                }
+                const unsigned bal = __ballot_sync(0xffffffffu, hit);
+                if (hit) list[n + __popc(bal & ((1u << lane) - 1u))] = static_cast<int>(p);
+                n += __popc(bal);
+            }
+            if (lane == 0) listed = n;
+        }
+        __syncthreads();
+        const int n = listed;
+        for (int e = 0; e < n; ++e) {
+            const int64_t q = list[e];
+            const float* pr = a.params + q * MOGE_LOSS_LOCAL_PARAMS;
+            const int64_t u0 = a.anchor[q * 3 + 1] - a.r, v0 = a.anchor[q * 3 + 2] - a.r;
+#pragma unroll
+            for (int k = 0; k < kRows; ++k) {
+                const int i = i0 + (threadIdx.x / kTile) + k * (kThreads / kTile), j = j0 + (threadIdx.x % kTile);
+                const int64_t u = i - u0, v = j - v0;
+                if (i >= a.H || j >= a.W || u < 0 || u >= S || v < 0 || v >= S || !a.pmask[(q * S + u) * S + v]) continue;
+                const int64_t o = ((b * a.H + i) * a.W + j) * 3;
+                const float w = __frcp_rn(fmaxf(a.g[o + 2], pr[LP_CAP]));
+                for (int c = 0; c < 3; ++c) {
+                    const float diff = __fsub_rn(__fadd_rn(__fmul_rn(pr[LP_SCALE], a.p[o + c]), pr[LP_SHIFT + c]), a.g[o + c]);
+                    g[k][c] = __fadd_rn(g[k][c], __fmul_rn(local_term(diff, w, a.beta, pr[LP_COEF], nullptr), pr[LP_SCALE]));
+                }
+            }
+        }
+        __syncthreads();
+    }
+#pragma unroll
+    for (int k = 0; k < kRows; ++k) {
+        const int i = i0 + (threadIdx.x / kTile) + k * (kThreads / kTile), j = j0 + (threadIdx.x % kTile);
+        if (i >= a.H || j >= a.W) continue;
+        for (int c = 0; c < 3; ++c) grad[((b * a.H + i) * a.W + j) * 3 + c] = g[k][c];
+    }
+}
+
 int num_tiles(int H, int W) { return static_cast<int>((static_cast<int64_t>(H) * W + kTilePx - 1) / kTilePx); }
 
 size_t workspace_size(int64_t batch, int H, int W) { return WsLayout::up(static_cast<size_t>(batch) * num_tiles(H, W) * kQ * 8); }
@@ -348,6 +547,64 @@ int moge_loss_global(const float* pred, const float* gt, const float* params, fl
     MG_TRY(check_batch_map("loss_global", batch, H, W, kMaxPixels));
     const GlobalOp op{pred, gt, params, beta, pass, static_cast<int64_t>(H) * W, grad};
     return run("loss_global", op, true, batch, H, W, sums, workspace, workspace_bytes, stream);
+}
+
+int moge_loss_anchor_weight(const float* points, const uint8_t* mask, const int64_t* di, const int64_t* dj, const float* radius,
+                            int64_t batch, int H, int W, int num_test, float* weight, void* stream) {
+    if (!points || !mask || !di || !dj || !radius || !weight) return set_error("null argument");
+    MG_TRY(check_batch_map("loss_anchor_weight", batch, H, W, kMaxPixels));
+    if (num_test < 0) return set_error("loss_anchor_weight: num_test %d < 0", num_test);
+    MG_TRY(check_device("loss_anchor_weight"));
+    const int64_t n = batch * H * W;
+    anchor_weight_kernel<<<static_cast<unsigned>((n + kThreads - 1) / kThreads), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        points, mask, di, dj, radius, batch, H, W, num_test, weight);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+static int check_patches(const char* what, int64_t batch, int H, int W, int64_t P, int r) {
+    MG_TRY(check_batch_map(what, batch, H, W, kMaxPixels));
+    if (P < 1 || P > 65535) return set_error("%s: %lld patches outside [1, 65535]", what, static_cast<long long>(P));
+    if (r < 0 || r > 16383) return set_error("%s: patch radius %d outside [0, 16383]", what, r);
+    return 0;
+}
+
+int moge_loss_patch_mask(const float* gt, const uint8_t* mask, const int64_t* anchor, const float* focal, float half_level,
+                         int64_t batch, int H, int W, int64_t P, int r, uint8_t* patch_mask, int* count, float* radius, void* stream) {
+    if (!gt || !mask || !anchor || !focal || !patch_mask || !count || !radius) return set_error("null argument");
+    MG_TRY(check_patches("loss_patch_mask", batch, H, W, P, r));
+    MG_TRY(check_device("loss_patch_mask"));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const int64_t S2 = static_cast<int64_t>(2 * r + 1) * (2 * r + 1);
+    CUDA_TRY(cudaMemsetAsync(count, 0, P * sizeof(int), st));
+    patch_mask_kernel<<<dim3(static_cast<unsigned>((S2 + kPatchPx - 1) / kPatchPx), static_cast<unsigned>(P)), kThreads, 0, st>>>(
+        gt, mask, anchor, focal, half_level, H, W, r, patch_mask, count, radius);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_loss_local(const float* pred, const float* gt, const int64_t* anchor, const float* params, const uint8_t* patch_mask,
+                    float beta, int pass, int64_t batch, int H, int W, int64_t P, int r, float* grad, double* sums, void* workspace,
+                    size_t workspace_bytes, void* stream) {
+    if (!gt || (pass > 0 && (!pred || !anchor || !params || !patch_mask))) return set_error("null argument");
+    if (pass < 0 || pass > 2) return set_error("loss_local: unknown pass %d", pass);
+    if (!(beta >= 0.f)) return set_error("loss_local: beta must be >= 0");
+    if (pass == 0) {
+        MG_TRY(check_batch_map("loss_local", batch, H, W, kMaxPixels));
+        const HarmonicOp op{gt, static_cast<int64_t>(H) * W};
+        return run("loss_local", op, true, batch, H, W, sums, workspace, workspace_bytes, stream);
+    }
+    MG_TRY(check_patches("loss_local", batch, H, W, P, r));
+    const LocalArgs a{pred, gt, anchor, params, patch_mask, beta, H, W, r, P};
+    const int S = 2 * r + 1;
+    MG_TRY(run("loss_local", PatchOp{a, pass}, true, P, S, S, sums, workspace, workspace_bytes, stream));
+    if (pass == 2 && grad) {
+        const dim3 grid((W + kTile - 1) / kTile, (H + kTile - 1) / kTile, static_cast<unsigned>(batch));
+        if (batch > 65535) return set_error("loss_local: batch %lld > 65535", static_cast<long long>(batch));
+        local_grad_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(a, grad);
+        CUDA_TRY(cudaGetLastError());
+    }
+    return 0;
 }
 
 }  // extern "C"

@@ -1,8 +1,9 @@
 """Training losses on the GPU: the deterministic subset of the reference's `moge/train/losses.py` (`affine_invariant_global_loss`,
 `normal_loss`, `edge_loss`, `mask_l2_loss`, `mask_bce_loss`, `metric_scale_loss`, `monitoring`) with the reference's signatures,
 defaults, batch semantics and return conventions (loss tensors of the batch shape, or a scalar for `normal_loss`; `misc` dicts
-of Python floats under the reference's keys).  It is not a drop-in `moge.train.losses`: the sampled local loss
-(`affine_invariant_local_loss`, `compute_anchor_sampling_weight`) and `normal_map_loss` are not provided.
+of Python floats under the reference's keys).  The sampled local loss (`affine_invariant_local_loss`,
+`compute_anchor_sampling_weight`) is in moge_b200.local_loss.  It is not a drop-in `moge.train.losses`: `normal_map_loss` is
+not provided.
 
 The per-pixel work runs in the kernels of moge_b200/csrc/losses.cu, forward and backward, behind one `torch.autograd.Function`
 per loss: per-image sums are fp64 over fixed pixel tiles added in a fixed order, and each pixel's gradient is written by one
