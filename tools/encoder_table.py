@@ -1,5 +1,5 @@
-"""Per-kind table of the encoder linears from `bench.py --dump-ops` files: the `gemm.*` launches of one step summed by kind (patch
-embed, qkv, proj, fc1, fc2, taps projection), with the engine's own flops and bytes, the lower bound they imply (the larger of flops
+"""Per-kind table of the encoder from `bench.py --dump-ops` files: the `gemm.*` launches of one step summed by kind (patch
+embed, qkv, proj, fc1, fc2, taps projection) and the `attention` launches, with the engine's own flops and bytes, the lower bound they imply (the larger of flops
 at the tensor peak and bytes at the HBM peak) and the fraction of it each kind reaches.  With two files (parent, new) it adds the
 new time and the change per kind.
 
@@ -19,13 +19,18 @@ def main():
         kinds = {}
         for o in json.load(open(f)):
             if o["name"].startswith("gemm."):
-                k = kinds.setdefault(o["name"][len("gemm."):], {"n": 0, "ms": 0.0, "flops": 0.0, "bytes": 0.0})
-                k["n"] += 1
-                k["ms"] += o["ms"]
-                k["flops"] += o["flops"]
-                k["bytes"] += o["bytes"]
+                name = o["name"][len("gemm."):]
+            elif o["name"].startswith("attention"):
+                name = "attention"
+            else:
+                continue
+            k = kinds.setdefault(name, {"n": 0, "ms": 0.0, "flops": 0.0, "bytes": 0.0})
+            k["n"] += 1
+            k["ms"] += o["ms"]
+            k["flops"] += o["flops"]
+            k["bytes"] += o["bytes"]
         runs.append(kinds)
-    head = "| linear | launches | GFLOP | MB | bound ms | parent ms | frac |"
+    head = "| kind | launches | GFLOP | MB | bound ms | parent ms | frac |"
     if len(runs) > 1:
         head += " new ms | frac | change |"
     print(head)
