@@ -92,11 +92,17 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* m, uin
         : "memory");
 }
 
-// TMA tensor store from shared memory (one bulk async-group per commit of the issuing thread).  The smem box must be made
-// visible to the async proxy (fence_proxy_async by every writing thread, then a barrier) before the store is issued.
+// TMA tensor stores from shared memory (one bulk async-group per commit of the issuing thread).  The smem box must be made
+// visible to the async proxy (fence_proxy_async by every writing thread, then a barrier) before the store is issued.  Elements
+// of the box outside the tensor's extent are not written.
 __device__ __forceinline__ void tma_store_4d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3) {
     asm volatile("cp.async.bulk.tensor.4d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5}], [%1];"
                  ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+                 : "memory");
+}
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1)
                  : "memory");
 }
 __device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }

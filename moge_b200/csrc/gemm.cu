@@ -5,7 +5,17 @@ namespace mg {
 
 int gemm_linear(GemmLaunch* g, bool bf16, const void* A, int M, int K, const void* W, int ldw, int N, int epi, void* out, int ldo,
                 const float* bias, const float* v1, const LnIO* ln, const Level* grid, void* out_relu, const float* v2, float su, float sv) {
-    constexpr int bn = 128;
+    // 128 x 256 tiles with the direct epilogue where the variant exists, N allows it and there are at least four such tiles per SM;
+    // else 128 x 128 staged tiles.  At one or two wide tiles per SM (batch 1, 1370 rows) the wide tiles were the slower ones
+    // (batch-1 p50 about 0.25 ms longer on an H100): there the staged tiles' epilogue warpgroup still overlaps a CTA's later tiles,
+    // while the direct epilogue runs behind each tile's main loop.
+    bool wide = WideRows::has(epi) && N % WideRows::kBN == 0;
+    if (wide) {
+        int sms = 0;
+        MG_TRY(check_device("linear", &sms));
+        wide = static_cast<long>((M + TILE_M - 1) / TILE_M) * (N / WideRows::kBN) >= 4L * sms;
+    }
+    const int bn = wide ? WideRows::kBN : 128;
     if (N % bn) return set_error("linear: N=%d must be a multiple of %d", N, bn);
     if ((epi == EPI_PATCH || epi == EPI_DEC) && grid == nullptr) return set_error("linear: epilogue %d needs the token grid", epi);
     GemmParams p{};
@@ -32,6 +42,7 @@ int gemm_linear(GemmLaunch* g, bool bf16, const void* A, int M, int K, const voi
     MG_TRY(make_map_2d(&g->a, A, K, M, K, TILE_M));
     MG_TRY(make_map_2d(&g->b, W, K, N, ldw, bn));
     g->aux = g->o0 = g->o1 = g->a;
+    if (wide) MG_TRY(make_map_2d(&g->o0, out, N, M, ldo, 64));       // the epilogue's TMA stores: 64 columns x 64 rows
     return 0;
 }
 

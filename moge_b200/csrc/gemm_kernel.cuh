@@ -7,8 +7,8 @@
 // each issues the wgmma of its 64 rows of the 128-row tile and stages its accumulators in shared memory; warpgroup 3 = epilogue:
 // warp w runs the fused epilogue of rows 32 w .. +31 of the staged tile while the consumers run the next tile's MMAs.  Two
 // mbarriers hand the one staging tile back and forth: acc_full (staged, the epilogue may read it) and acc_empty (read, the
-// consumers may overwrite it).  The dec_direct variants have no epilogue warpgroup and skip the staging: each consumer warpgroup
-// stores its own 64 rows from its registers (dec_direct_epilogue).
+// consumers may overwrite it).  The direct variants (gemm_direct) have no epilogue warpgroup and skip the staging: each consumer
+// warpgroup stores its own 64 rows from its registers (dec_direct_epilogue, rows_direct_epilogue).
 //
 // Three main loops share the kernel (MODE):
 //   MODE_GEMM   one stage = one 64-wide K block of A (row tile, or one filter tap's pixel window) and of B.
@@ -94,13 +94,29 @@ __host__ __device__ constexpr bool dec_direct(int mode, int epi, int df) {
     return mode != MODE_GEMM && epi == EPI_DEC && df >= 0 && (df & DF_SHUFFLE) == 0;
 }
 
+// The row-major variants that run 128 x 256 tiles: the 16-bit elementwise epilogues (qkv, fc1), finished by the consumer
+// warpgroups straight from their accumulator registers (rows_direct_epilogue).  A staged fp32 tile of 256 columns (128 KB) would
+// leave room for two ring stages; without it four fit.  gemm_rows.cu instantiates exactly this list and gemm_linear selects from
+// it (when N is a multiple of the width and the rows give every SM enough tiles), so the two cannot drift apart.
+template <int BN, int... E> struct RowEpiList {
+    static constexpr int kBN = BN;
+    __host__ __device__ static constexpr bool has(int epi) { return ((epi == E) || ...); }
+};
+using WideRows = RowEpiList<256, EPI_STORE16, EPI_GELU16>;
+
+// The variants without the staged accumulator tile and its epilogue warpgroup.
+__host__ __device__ constexpr bool gemm_direct(int bn, int mode, int amode, int epi, int df) {
+    return dec_direct(mode, epi, df) || (mode == MODE_GEMM && amode == AMODE_ROWS && bn == WideRows::kBN && WideRows::has(epi));
+}
+
 // One launch of gemm_kernel as gemm_linear / gemm_conv (gemm.cu) choose it: the kernel variant, its tensor maps and params.
 struct GemmLaunch {
     int bn, mode, amode, epi;
     int df;                    // EPI_DEC: the compile-time DF mask of the variant, or -1 (run-time flags)
     bool bf16;
     CUtensorMap a, aux, b;     // A operand, aux A operand (fused 1x1 input block), weights
-    CUtensorMap o0, o1;        // dec_direct variants: store maps of the raw and ReLU outputs (boxes {64 ch, 16 px, 4 rows})
+    CUtensorMap o0, o1;        // dec_direct variants: store maps of the raw and ReLU outputs (boxes {64 ch, 16 px, 4 rows});
+                               // WideRows variants: o0 = store map of the output rows (boxes {64 columns, 64 rows})
     GemmParams p;
 };
 
@@ -114,10 +130,12 @@ template <int BN, int MODE = MODE_GEMM, bool DIRECT = false> struct GemmCfg {
     // r * 8 + (q ^ (r & 7)) -- a lane reads its row conflict-free, 8 lanes x float4 read one row of the block conflict-free
     static constexpr int kChunks = (BN < 32) ? 1 : BN / 32;
     static constexpr int kAccBytes = DIRECT ? 0 : TILE_M * kChunks * 32 * 4;
-    // DIRECT: kOutBufs 16-bit output boxes {64 ch, 16 px, 4 rows} (8 KB, 128B-swizzled) per consumer warpgroup.  One box keeps
-    // the output staging at 16 KB, which is what lets MODE_CONVH fit a third ring stage.
+    // DIRECT: kOutBufs 16-bit output boxes (8 KB, 128B-swizzled) per consumer warpgroup: {64 ch, 16 px, 4 rows} in the conv modes,
+    // {64 columns, 64 rows} in MODE_GEMM (the WideRows variants).  One box keeps the output staging at 16 KB, which is what lets
+    // MODE_CONVH fit a third ring stage; the 128 x 256 row tiles double-buffer it (4 x 48 KB stages + 32 KB still fit), so the
+    // writes of one box overlap the store of the previous one.
     static constexpr int kOutBoxBytes = 64 * 64 * 2;
-    static constexpr int kOutBufs = 1;
+    static constexpr int kOutBufs = (MODE == MODE_GEMM) ? 2 : 1;
     static constexpr int kOutBytes = DIRECT ? 2 * kOutBufs * kOutBoxBytes : 0;
     static constexpr int kFixedBytes = kAccBytes + kOutBytes + kResidentBytes + 1024 /*align slack*/ + 256 /*barriers*/;
     static constexpr int kFit = (kMaxDynSmem - kFixedBytes) / kStageBytes;
@@ -138,7 +156,8 @@ template <int BN, int MODE = MODE_GEMM, bool DIRECT = false> struct GemmCfg {
     static_assert(kStages >= 2, "gemm_kernel: fewer than two ring stages fit beside the accumulator tile");
     static_assert(kSmemBytes <= kMaxDynSmem, "gemm_kernel: stage ring + accumulator tile exceed the shared memory of one CTA");
     static_assert((2 * kStages + 3) * 8 <= 256, "gemm_kernel: barrier block overflows its 256 bytes");
-    static_assert(!DIRECT || BN % 64 == 0, "gemm_kernel: the direct EPI_DEC epilogue stores whole 64-channel boxes");
+    static_assert(!DIRECT || BN % 64 == 0, "gemm_kernel: the direct epilogues store whole 64-column boxes");
+    static_assert(!DIRECT || MODE != MODE_GEMM || kStages >= 4, "gemm_kernel: the 128 x 256 row tiles need four ring stages");
 };
 
 // Block of the staged accumulator tile holding rows 32 quarter .. +31, columns col .. col + 31 (col a multiple of 32).
@@ -485,6 +504,45 @@ __device__ __forceinline__ void dec_direct_epilogue(const GemmParams& p, const C
     }
 }
 
+// Direct row epilogue (WideRows variants, EPI_STORE16 / EPI_GELU16) of consumer warpgroup g, rows 64 g .. +63 of row tile mt:
+// in the accumulator fragment a thread (warp wl, lane) holds rows 16 wl + lane / 4 (h = 0) and + 8 (h = 1), column pairs
+// 8 c + 2 (lane % 4) of the tile, c = 0 .. BN / 8 - 1.  The arithmetic is epilogue_rows' in the same fp32 order
+// (fmaf(rstd, acc, bias), GELU, one rounding to 16 bit); rs[h] = 1 without the LayerNorm fold, and fmaf(1, a, b) is a + b exactly.
+// Per 64-column box, the box-reuse protocol of dec_direct_epilogue; the TMA store clips the rows at M, so the last row tile needs
+// no predicates.
+template <int BN, int EPI, bool BF16, int OUTBUFS>
+__device__ __forceinline__ void rows_direct_epilogue(const GemmParams& p, const CUtensorMap* map, int mt, int nt, const float (&acc)[BN / 2],
+                                                     const float (&rs)[2], uint8_t* sOut, int g, int wl, int lane, int& nbox) {
+    using H = H16<BF16>;
+    const float* bias = p.bias + nt * BN + 2 * (lane & 3);
+    const bool leader = wl == 0 && lane == 0;
+#pragma unroll
+    for (int b = 0; b < BN / 64; ++b) {
+        uint8_t* sb = sOut + (nbox % OUTBUFS) * GemmCfg<64>::kOutBoxBytes;
+        ++nbox;
+        if (leader) bulk_wait_read<OUTBUFS - 1>();     // the store that last read this buffer is done with it
+        named_sync(2 + g, 128);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+            const int c = 8 * b + j;
+            const float2 bb = *reinterpret_cast<const float2*>(bias + 8 * c);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                float2 v = make_float2(fmaf(rs[h], acc[4 * c + 2 * h], bb.x), fmaf(rs[h], acc[4 * c + 2 * h + 1], bb.y));
+                if (EPI == EPI_GELU16) v = gelu_erf2(v);
+                const int R = 16 * wl + (lane >> 2) + 8 * h;          // box row; R & 7 == lane >> 2
+                *reinterpret_cast<uint32_t*>(sb + R * 128 + ((j ^ (lane >> 2)) << 4) + 4 * (lane & 3)) = H::pack(v.x, v.y);
+            }
+        }
+        fence_proxy_async();
+        named_sync(2 + g, 128);
+        if (leader) {
+            tma_store_2d(map, sb, nt * BN + 64 * b, mt * TILE_M + 64 * g);
+            bulk_commit();
+        }
+    }
+}
+
 // EPI_HEADOUT epilogue: lane = low-resolution pixel, 16 B (or 4 B) per lane, consecutive lanes = consecutive pixels of a tile row.
 template <int BN>
 __device__ __forceinline__ void epilogue_headout(const GemmParams& p, int mt, const float4* stg, int quarter, int lane) {
@@ -674,20 +732,20 @@ __device__ __forceinline__ void epilogue_rows(const GemmParams& p, int mt, int n
 }
 
 template <int BN, int MODE, int AMODE, int EPI, bool BF16, int DF = -1>
-__global__ void __launch_bounds__(GemmCfg<BN, MODE, dec_direct(MODE, EPI, DF)>::kThreads, 1)
+__global__ void __launch_bounds__(GemmCfg<BN, MODE, gemm_direct(BN, MODE, AMODE, EPI, DF)>::kThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapAux,
             const __grid_constant__ CUtensorMap mapB, const __grid_constant__ CUtensorMap mapO0,
             const __grid_constant__ CUtensorMap mapO1, const GemmParams p) {
     static_assert(AMODE == AMODE_ROWS || EPI == EPI_DEC || EPI == EPI_HEADOUT || EPI == EPI_NECKOUT,
                   "gemm_kernel: a pixel-tile A operand pairs only with the decoder epilogues (DEC, HEADOUT, NECKOUT)");
     pdl_launch_dependents();      // (the wait sits after the barrier set-up below: that prologue overlaps the previous kernel's tail)
-    constexpr bool DIRECT = dec_direct(MODE, EPI, DF);
+    constexpr bool DIRECT = gemm_direct(BN, MODE, AMODE, EPI, DF);
     using Cfg = GemmCfg<BN, MODE, DIRECT>;
     constexpr int S = Cfg::kStages;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     float4* stg = reinterpret_cast<float4*>(smem + S * Cfg::kStageBytes);            // staged epilogues: fp32 accumulator tile
-    uint8_t* sOut = smem + S * Cfg::kStageBytes + Cfg::kAccBytes;                     // DIRECT: 16-bit output boxes
+    uint8_t* sOut = smem + S * Cfg::kStageBytes + Cfg::kAccBytes;                     // DIRECT: 16-bit output boxes (1 KB-aligned)
     uint8_t* sW = sOut + Cfg::kOutBytes;                                               // MODE_CONV64: resident weights
     uint64_t* full = reinterpret_cast<uint64_t*>(sW + Cfg::kResidentBytes);
     uint64_t* empty = full + S;
@@ -800,11 +858,26 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
         uint32_t handed = 0;                            // staged variants: tiles staged for the epilogue warpgroup so far
         // stages per tile with the 3x3 taps; the rest read the aux source (fused 1x1 input block)
         const int ntap_stage = (MODE == MODE_GEMM) ? nstage : (MODE == MODE_CONV64) ? 3 : 3 * p.kb_main;
+        // WideRows variants with the LayerNorm fold: rstd of this thread's two fragment rows, loaded one tile ahead
+        float rs[2] = {1.f, 1.f}, rs_next[2] = {1.f, 1.f};
+        auto rs_load = [&](int tile, float (&r)[2]) {
+            const long row = static_cast<long>(tile / p.num_n_tiles) * TILE_M + 64 * g + 16 * wl + (lane >> 2);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) r[h] = (row + 8 * h < p.M) ? p.ln_rstd[row + 8 * h] : 1.f;
+        };
+        constexpr bool ROWS_DIRECT = DIRECT && MODE == MODE_GEMM;
+        const bool ln_on = ROWS_DIRECT && p.ln_rstd != nullptr;
+        if (ln_on && static_cast<int>(blockIdx.x) < total_tiles) rs_load(blockIdx.x, rs_next);
         for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
             const int mt = tile / p.num_n_tiles, nt = tile % p.num_n_tiles;
+            if (ln_on) {
+                rs[0] = rs_next[0]; rs[1] = rs_next[1];
+                const int nxt = tile + static_cast<int>(gridDim.x);
+                if (nxt < total_tiles) rs_load(nxt, rs_next);
+            }
             DecPix dp{};
-            uint32_t sk[DIRECT && (DF & DF_SKIP) ? BN / 4 : 1];
-            if constexpr (DIRECT) {
+            uint32_t sk[DIRECT && !ROWS_DIRECT && (DF & DF_SKIP) ? BN / 4 : 1];
+            if constexpr (DIRECT && !ROWS_DIRECT) {
                 dp = dec_pix(p, mt, g, wl, lane);
                 if constexpr ((DF & DF_SKIP) != 0) dec_skip_load<BN>(p, dp, nt, lane, sk);
             }
@@ -854,7 +927,11 @@ gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CU
             wgmma_wait<0>();
             reg_fence(acc);
             if (prev >= 0 && lane == 0) mbar_arrive(&empty[prev]);
-            if constexpr (DIRECT) {
+            if constexpr (ROWS_DIRECT) {
+                rows_direct_epilogue<BN, EPI, BF16, Cfg::kOutBufs>(p, &mapO0, mt, nt, acc, rs, sOut + g * Cfg::kOutBufs * Cfg::kOutBoxBytes,
+                                                                   g, wl, lane, nbox);
+                continue;
+            } else if constexpr (DIRECT) {
                 dec_direct_epilogue<BN, BF16, DF, Cfg::kOutBufs>(p, &mapO0, &mapO1, dp, nt, acc, sk, sOut + g * Cfg::kOutBufs * Cfg::kOutBoxBytes,
                                                                  g, wl, lane, nbox);
                 continue;

@@ -27,7 +27,7 @@ using ConvHDF = DecFlagList<128, DF_RELU, DF_RAW | DF_SKIP, DF_RAW | DF_RELU | D
 // its grid is a multiple of num_n_tiles (every CTA then sees one fixed nt).
 template <int BN, int MODE, int AMODE, int EPI, bool BF16, int DF>
 int launch_gemm_inst(const GemmLaunch& g, int num_sms, cudaStream_t st) {
-    using Cfg = GemmCfg<BN, MODE, dec_direct(MODE, EPI, DF)>;
+    using Cfg = GemmCfg<BN, MODE, gemm_direct(BN, MODE, AMODE, EPI, DF)>;
     const GemmParams& p = g.p;
     auto kern = gemm_kernel<BN, MODE, AMODE, EPI, BF16, DF>;
     MG_SET_SMEM_ONCE(kern, Cfg::kSmemBytes);
@@ -44,6 +44,14 @@ template <int BN, int MODE, int AMODE, int EPI, int DF = -1>
 int launch_gemm_variant(const GemmLaunch& g, int num_sms, cudaStream_t st) {
     return g.bf16 ? launch_gemm_inst<BN, MODE, AMODE, EPI, true, DF>(g, num_sms, st)
                   : launch_gemm_inst<BN, MODE, AMODE, EPI, false, DF>(g, num_sms, st);
+}
+
+// The WideRows variant of epilogue g.epi (instantiates every epilogue of the list).
+template <int BN, int... E>
+int launch_gemm_wide(RowEpiList<BN, E...>, const GemmLaunch& g, int num_sms, cudaStream_t st) {
+    int rc = 0;
+    const bool found = ((g.bn == BN && g.epi == E && ((rc = launch_gemm_variant<BN, MODE_GEMM, AMODE_ROWS, E>(g, num_sms, st)), true)) || ...);
+    return found ? rc : set_error("gemm: no %d-wide row variant for epi=%d", BN, g.epi);
 }
 
 // The specialised EPI_DEC variant g.df of a mode's list (instantiates every mask of the list).
