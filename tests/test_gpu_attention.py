@@ -6,7 +6,7 @@ import torch
 import torch.nn.functional as F
 
 from moge_b200 import capi
-from gpu_util import rel_l2, stream, dt
+from gpu_util import rel_l2, stream, dt, TILE_ATTENTION, TILE_C, worst_tile
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -41,6 +41,16 @@ def test_attention_many_items_per_cta(B, N, heads, dtype):
     ref = F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(B, N, heads * 64)
     assert torch.isfinite(out.float()).all()
     assert rel_l2(out, ref) < TOL[dtype]
+    # block by block: (image, 64 query rows, head), half of a consumer warpgroup's query tile; the last block of an image lies
+    # in or next to the item's dead query tile
+    err, (img, qb, head) = worst_tile(out, ref, TILE_ATTENTION)
+    whole = rel_l2(out, ref)
+    last = qb == (N + 63) // 64 - 1
+    print(f"tile-check attention {dtype} {(B, N, heads)}: whole {whole:.3e} worst {err:.3e} at image {img} head {head} "
+          f"query block {qb}{' (last)' if last else ''} ratio {err / whole:.2f}")
+    assert err < TILE_C * TOL[dtype], (f"image {img}, head {head}, query block {qb} (rows {64 * qb}..{min(64 * qb + 64, N) - 1}"
+                                       f"{', the last block of the image' if last else ''}): error {err:.3e}, whole tensor "
+                                       f"{whole:.3e}")
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])

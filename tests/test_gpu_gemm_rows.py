@@ -7,19 +7,13 @@ import torch
 import torch.nn.functional as F
 
 from moge_b200 import capi
-from gpu_util import stream, dt
+from gpu_util import rel_l2, stream, dt, check_tiles, TILE_LINEAR
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 TOL = {torch.float16: 2e-3, torch.bfloat16: 1.2e-2}      # test_gpu_ops' tolerances for 16-bit outputs
 M = 32 * 1370
 LINEARS = {"qkv": (3072, 1024, 0), "fc1": (4096, 1024, 1), "proj": (1024, 1024, 2), "fc2": (1024, 4096, 2)}
-
-
-def rel_l2(a, b):
-    # on the device: the outputs are up to 180 M elements
-    a, b = a.double(), b.double()
-    return float((a - b).norm() / b.norm().clamp_min(1e-30))
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
@@ -41,7 +35,8 @@ def test_encoder_linear_at_bench_rows(name, dtype):
                                           dt(dtype), stream()))
             return out
 
-        ref = res + gamma * (x.float() @ w.float().t() + b)
+        gemm = gamma * (x.float() @ w.float().t() + b)
+        ref = res + gemm
         tol = 2e-5 + 1e-4
     else:
         # rows with a per-row offset and scale, so that the folded mean and variance matter
@@ -66,4 +61,8 @@ def test_encoder_linear_at_bench_rows(name, dtype):
     torch.cuda.synchronize()
     assert torch.isfinite(first.float()).all()
     assert rel_l2(first, ref) < tol
+    if epi == 2:      # the GEMM's contribution on its own, so that the fp32 residual cannot mask a tile of it
+        check_tiles(first - res, gemm, TILE_LINEAR, tol, f"linear {name} {dtype}")
+    else:
+        check_tiles(first, ref, TILE_LINEAR, tol, f"linear {name} {dtype}")
     assert torch.equal(first, second), "two identical calls differ"

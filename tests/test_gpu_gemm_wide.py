@@ -9,7 +9,7 @@ import torch
 import torch.nn.functional as F
 
 from moge_b200 import capi
-from gpu_util import stream, dt
+from gpu_util import rel_l2, stream, dt, check_tiles, TILE_LINEAR
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -17,11 +17,6 @@ TOL = {torch.float16: 2e-3, torch.bfloat16: 1.2e-2}      # test_gpu_gemm_rows' t
 K = 1024
 SENTINEL = 1234.0      # exact in fp16 and bf16
 PAD = 64               # rows past M that must stay untouched
-
-
-def rel_l2(a, b):
-    a, b = a.double(), b.double()
-    return float((a - b).norm() / b.norm().clamp_min(1e-30))
 
 
 def make_case(M, N, ln, dtype, seed):
@@ -76,7 +71,10 @@ def test_wide_tiles_accuracy_and_bounds(epi, ln, dtype, N, M):
     assert bool((out[M:] == SENTINEL).all()), "a row past M was written"
     got = out[:M]
     assert bool(torch.isfinite(got.float()).all()), "a row below M was not written"
-    assert rel_l2(got, reference(case, epi, ln)) < TOL[dtype]
+    ref = reference(case, epi, ln)
+    assert rel_l2(got, ref) < TOL[dtype]
+    # every tile, the ragged last row tile (1, 37 or 100 rows past 64 full tiles) included
+    check_tiles(got, ref, TILE_LINEAR, TOL[dtype], f"linear wide {dtype}")
 
 
 @pytest.mark.parametrize("M", [43840, 8229])

@@ -5,7 +5,8 @@ import torch
 import torch.nn.functional as F
 
 from moge_b200 import capi
-from gpu_util import rel_l2, stream, dt, to_padded_nhwc, empty_padded, from_padded_nhwc, border_ok
+from gpu_util import rel_l2, stream, dt, to_padded_nhwc, empty_padded, from_padded_nhwc, border_ok, check_tiles, tile_conv, \
+    TILE_LINEAR, TILE_ATTENTION
 
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
@@ -29,6 +30,7 @@ def test_linear_bias(M, N, K, dtype):
     ref = x.float() @ w.float().t() + b
     assert torch.isfinite(out.float()).all()
     assert rel_l2(out, ref) < TOL[dtype]
+    check_tiles(out, ref, TILE_LINEAR, TOL[dtype], f"linear {dtype}")
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
@@ -43,6 +45,7 @@ def test_linear_gelu(dtype):
     torch.cuda.synchronize()
     ref = F.gelu(x.float() @ w.float().t() + b)
     assert rel_l2(out, ref) < TOL[dtype]
+    check_tiles(out, ref, TILE_LINEAR, TOL[dtype], f"linear gelu {dtype}")
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
@@ -59,6 +62,8 @@ def test_linear_residual_layerscale(M, N, K, dtype):
     torch.cuda.synchronize()
     ref = res + gamma * (x.float() @ w.float().t() + b)
     assert rel_l2(out, ref) < (2e-5 if dtype == torch.float16 else 2e-5) + 1e-4
+    # the GEMM's contribution on its own, tile by tile, so that the fp32 residual cannot mask it
+    check_tiles(out - res, gamma * (x.float() @ w.float().t() + b), TILE_LINEAR, 2e-5 + 1e-4, f"linear residual {dtype}")
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
@@ -80,6 +85,7 @@ def test_linear_with_folded_layernorm(M, N, K, epi, dtype):
     if epi == 1:
         ref = F.gelu(ref)
     assert rel_l2(out, ref) < TOL[dtype]
+    check_tiles(out, ref, TILE_LINEAR, TOL[dtype], f"linear ln {dtype}")
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
@@ -110,6 +116,7 @@ def test_attention(B, N, heads, dtype):
     ref = F.scaled_dot_product_attention(q, k, v).transpose(1, 2).reshape(B, N, D)
     assert torch.isfinite(out.float()).all()
     assert rel_l2(out, ref) < (3e-3 if dtype == torch.float16 else 1.5e-2)
+    check_tiles(out, ref, TILE_ATTENTION, 3e-3 if dtype == torch.float16 else 1.5e-2, f"attention {dtype}")
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
@@ -131,6 +138,8 @@ def test_conv3x3_replicate_skip_relu(B, H, W, Cin, Cout, dtype):
     assert rel_l2(from_padded_nhwc(raw, H, W), ref) < TOL[dtype]
     assert rel_l2(from_padded_nhwc(relu, H, W), F.relu(ref)) < TOL[dtype]
     assert border_ok(raw, H, W) and border_ok(relu, H, W)
+    check_tiles(from_padded_nhwc(raw, H, W), ref, tile_conv(Cout), TOL[dtype], f"conv3x3 raw {dtype}")
+    check_tiles(from_padded_nhwc(relu, H, W), F.relu(ref), tile_conv(Cout), TOL[dtype], f"conv3x3 relu {dtype}")
 
 
 def test_conv3x3_halo_streamed_weights():
@@ -166,6 +175,7 @@ def test_conv1x1(dtype):
     ref = F.conv2d(x.float(), w.to(dtype).float(), b)
     assert rel_l2(from_padded_nhwc(raw, H, W), ref) < TOL[dtype]
     assert border_ok(raw, H, W)
+    check_tiles(from_padded_nhwc(raw, H, W), ref, tile_conv(Cout), TOL[dtype], f"conv1x1 {dtype}")
 
 
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
@@ -182,3 +192,5 @@ def test_conv_transpose_k2s2(B, H, W, Cin, Cout, dtype):
     ref = F.conv_transpose2d(x.float(), w.to(dtype).float(), b, stride=2)
     assert rel_l2(from_padded_nhwc(raw, 2 * H, 2 * W), ref) < TOL[dtype]
     assert border_ok(raw, 2 * H, 2 * W)
+    # tiles on the 2H x 2W output grid
+    check_tiles(from_padded_nhwc(raw, 2 * H, 2 * W), ref, tile_conv(Cout), TOL[dtype], f"convT {dtype}")

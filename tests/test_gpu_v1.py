@@ -7,7 +7,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from gpu_util import border_ok, dt, empty_padded, from_padded_nhwc, rel_l2, stream, to_padded_nhwc
+from gpu_util import border_ok, check_tiles, dt, empty_padded, from_padded_nhwc, rel_l2, stream, tile_conv, to_padded_nhwc
 from moge_b200 import capi
 from moge_b200.configs import uv_spans, v1_model_config
 from moge_b200.synthetic import make_v1_state_dict, synthetic_images
@@ -262,3 +262,5 @@ def test_op_convT_input_grid_uv(B, H, W, Cin, Cout, dtype):
     print(f"convT uv {dtype}: err {err:.2e}, output-grid convention would be {err_wrong:.2e}")
     assert err < tol, err
     assert err_wrong > 5 * tol, err_wrong
+    # tile by tile on the 2H x 2W output grid, so that a wrong UV phase at a ragged edge is named by its tile
+    check_tiles(got, ref, tile_conv(Cout), tol, f"convT uv {dtype}")
