@@ -29,8 +29,7 @@ __all__ = [
 
 
 def _rows(t: torch.Tensor, shape) -> torch.Tensor:
-    if not t.is_cuda:
-        raise MogeError("moge_b200.alignment operates on CUDA tensors only (no CPU fallback)")
+    capi.require_cuda("moge_b200.alignment", t)
     return t.detach().reshape(shape).to(torch.float32).contiguous()
 
 

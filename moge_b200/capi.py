@@ -19,22 +19,6 @@ ALIGN_MAX_POINTS = 4096          # points per anchored problem (elements per pla
 REMAP = {"linear": 0, "sinh": 1, "exp": 2, "sinh_exp": 3}
 RESAMPLE = {"conv_transpose": 0, "bilinear": 1}
 
-EXPORTS = [
-    "moge_last_error", "moge_version", "moge_engine_create", "moge_engine_destroy", "moge_engine_set_weight",
-    "moge_engine_finalize", "moge_engine_workspace_bytes", "moge_engine_forward", "moge_engine_workspace_bytes_groups",
-    "moge_engine_forward_groups", "moge_engine_num_ops", "moge_engine_op_info", "moge_engine_profile", "moge_attention_work_list", "moge_recover_focal_shift",
-    "moge_postprocess", "moge_peer_alloc", "moge_peer_free", "moge_peer_open", "moge_peer_close", "moge_peer_copy", "moge_peer_flag_set",
-    "moge_peer_flag_wait", "moge_op_linear", "moge_op_linear_ln", "moge_op_attention", "moge_op_layernorm", "moge_op_conv",
-    "moge_align_workspace_bytes", "moge_align", "moge_align_anchored", "moge_align_affine_lstsq",
-    "moge_engine_create_v1", "moge_v1_workspace_bytes", "moge_v1_forward", "moge_v1_postprocess", "moge_op_resize_bicubic_aa",
-    "moge_op_groupnorm_relu", "moge_bicubic_aa_weights", "moge_op_conv_transpose_uv",
-    "moge_metrics_workspace_bytes", "moge_metrics_resize", "moge_metrics_stats", "moge_metrics_eval", "moge_metrics_boundary",
-    "moge_mesh_workspace_bytes", "moge_depth_edge", "moge_mesh_count", "moge_mesh_build", "moge_normal_map", "moge_normal_edge",
-    "moge_panorama_split", "moge_panorama_workspace_bytes", "moge_panorama_rhs", "moge_panorama_lsmr", "moge_panorama_resize",
-    "moge_panorama_finish", "moge_loss_workspace_bytes", "moge_loss_mask", "moge_loss_stencil", "moge_loss_normal_map",
-    "moge_loss_global", "moge_loss_anchor_weight", "moge_loss_patch_mask", "moge_loss_local",
-    "moge_vis_workspace_bytes", "moge_vis_quantiles", "moge_vis_colorize", "moge_vis_normal",
-]
 METRICS_MAX_SEGMENTS, METRICS_MAX_VARIANTS, METRICS_F1_THRESHOLDS, METRICS_F1_COUNTS, METRICS_OUT_SEGMENTS = 256, 8, 10, 90, 17
 (MV_DEPTH, MV_DEPTH_SCALE, MV_DEPTH_AFFINE, MV_DISPARITY, MV_DISPARITY_FROM_DEPTH, MV_POINTS_SHIFT, MV_POINTS_SCALE,
  MV_POINTS_AFFINE) = range(8)
@@ -105,6 +89,85 @@ class PanoramaCamera(C.Structure):
                 ("cy", C.c_double)]
 
 
+vp, ci, i64, sz = C.c_void_p, C.c_int, C.c_int64, C.c_size_t
+fp, pc = C.POINTER(C.c_float), C.POINTER(PanoramaCamera)
+
+# Every entry point of include/moge_b200.h: name -> argtypes for those returning an int status, (restype, argtypes) otherwise.
+SIGNATURES = {
+    "moge_last_error": (C.c_char_p, None),
+    "moge_version": (C.c_char_p, None),
+    "moge_engine_create": [C.POINTER(Config), ci, C.POINTER(vp)],
+    "moge_engine_destroy": (None, [vp]),
+    "moge_engine_set_weight": [vp, C.c_char_p, vp, C.POINTER(i64), ci, ci, vp],
+    "moge_engine_finalize": [vp, vp],
+    "moge_engine_workspace_bytes": [vp, ci, ci, ci, ci, ci, C.POINTER(sz)],
+    "moge_engine_forward": [vp, vp, ci, ci, ci, ci, ci, ci, vp, sz, vp, vp, vp, vp, vp],
+    "moge_engine_workspace_bytes_groups": [vp, C.POINTER(Group), ci, C.POINTER(sz)],
+    "moge_engine_forward_groups": [vp, C.POINTER(Group), ci, vp, sz, vp],
+    "moge_engine_num_ops": [vp, C.POINTER(ci)],
+    "moge_attention_work_list": [C.POINTER(ci), ci, ci, ci, C.POINTER(ci), ci, C.POINTER(ci), C.POINTER(ci), C.POINTER(ci)],
+    "moge_engine_op_info": [vp, ci, C.c_char_p, ci, C.POINTER(C.c_double), C.POINTER(C.c_double)],
+    "moge_engine_profile": [vp, fp, ci, vp],
+    "moge_recover_focal_shift": [vp, vp, vp, ci, ci, ci, vp, vp, vp, vp],
+    "moge_postprocess": [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp],
+    "moge_peer_alloc": [sz, C.POINTER(vp), C.c_char_p],
+    "moge_peer_free": [vp],
+    "moge_peer_open": [C.c_char_p, C.POINTER(vp)],
+    "moge_peer_close": [vp],
+    "moge_peer_copy": [vp, vp, sz, vp],
+    "moge_peer_flag_set": [vp, ci, vp],
+    "moge_peer_flag_wait": [vp, ci, vp],
+    "moge_op_linear": [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp],
+    "moge_op_linear_ln": [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp],
+    "moge_op_attention": [vp, vp, ci, ci, ci, ci, ci, vp],
+    "moge_op_layernorm": [vp, vp, vp, vp, ci, ci, ci, vp],
+    "moge_op_conv": [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, vp],
+    "moge_align_workspace_bytes": [ci, ci, i64, ci, C.POINTER(sz)],
+    "moge_align": [vp, vp, vp, vp, ci, i64, ci, vp, vp, vp, vp, sz, vp],
+    "moge_align_anchored": [vp, vp, vp, ci, C.c_float, i64, ci, vp, vp, vp, vp, sz, vp],
+    "moge_align_affine_lstsq": [vp, vp, vp, i64, i64, vp, vp, vp],
+    "moge_engine_create_v1": [C.POINTER(V1Config), ci, C.POINTER(vp)],
+    "moge_v1_workspace_bytes": [vp, ci, ci, ci, ci, ci, C.POINTER(sz)],
+    "moge_v1_forward": [vp, vp, ci, ci, ci, ci, ci, ci, vp, sz, vp, vp, vp],
+    "moge_v1_postprocess": [vp, vp, C.c_float, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp],
+    "moge_op_resize_bicubic_aa": [vp, ci, ci, ci, ci, ci, ci, ci, vp, vp],
+    "moge_op_groupnorm_relu": [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp],
+    "moge_op_conv_transpose_uv": [vp, vp, vp, vp, ci, ci, ci, ci, ci, C.c_float, C.c_float, ci, vp],
+    "moge_bicubic_aa_weights": [ci, ci, ci, C.POINTER(ci), fp, ci],
+    "moge_metrics_workspace_bytes": [i64, ci, ci, ci, C.POINTER(sz)],
+    "moge_metrics_resize": [vp, i64, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp],
+    "moge_metrics_stats": [vp, vp, vp, vp, ci, vp, vp, vp, ci, i64, ci, ci, vp, vp, vp, sz, vp],
+    "moge_metrics_eval": [vp, vp, vp, C.POINTER(MetricVariant), ci, vp, vp, vp, vp, ci, vp, vp, i64, ci, ci, vp, i64, vp, sz,
+                          vp],
+    "moge_metrics_boundary": [vp, vp, C.POINTER(MetricVariant), fp, i64, ci, ci, vp, i64, vp],
+    "moge_mesh_workspace_bytes": [i64, ci, ci, C.POINTER(sz)],
+    "moge_depth_edge": [vp, vp, vp, i64, ci, ci, ci, fp, fp, vp, vp],
+    "moge_mesh_count": [vp, i64, ci, ci, vp, vp, sz, vp],
+    "moge_mesh_build": [vp, i64, ci, ci, ci, C.POINTER(MeshMap), ci, vp, vp, vp, sz, vp],
+    "moge_normal_map": [vp, vp, i64, ci, ci, vp, vp, vp],
+    "moge_normal_edge": [vp, vp, vp, vp, i64, ci, ci, ci, C.c_double, vp, vp, vp],
+    "moge_panorama_split": [vp, ci, ci, pc, ci, vp, ci, vp, vp, vp],
+    "moge_panorama_workspace_bytes": [ci, ci, ci, C.POINTER(sz)],
+    "moge_panorama_rhs": [vp, ci, vp, ci, ci, ci, pc, vp, ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_panorama_lsmr": [vp, vp, ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_panorama_resize": [vp, ci, ci, ci, ci, vp, vp],
+    "moge_panorama_finish": [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp],
+    "moge_loss_workspace_bytes": [i64, ci, ci, C.POINTER(sz)],
+    "moge_loss_mask": [ci, vp, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_loss_stencil": [ci, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_loss_normal_map": [vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_loss_global": [vp, vp, vp, C.c_float, ci, i64, ci, ci, vp, vp, vp, sz, vp],
+    "moge_loss_anchor_weight": [vp, vp, vp, vp, vp, i64, ci, ci, ci, vp, vp],
+    "moge_loss_patch_mask": [vp, vp, vp, vp, C.c_float, i64, ci, ci, i64, ci, vp, vp, vp, vp],
+    "moge_loss_local": [vp, vp, vp, vp, vp, C.c_float, ci, i64, ci, ci, i64, ci, vp, vp, vp, sz, vp],
+    "moge_vis_workspace_bytes": [i64, ci, ci, C.POINTER(sz)],
+    "moge_vis_quantiles": [vp, ci, vp, i64, ci, ci, fp, ci, vp, vp, sz, vp],
+    "moge_vis_colorize": [vp, ci, ci, vp, i64, ci, ci, vp, vp, ci, vp, vp],
+    "moge_vis_normal": [vp, vp, i64, ci, ci, ci, vp, vp],
+}
+EXPORTS = list(SIGNATURES)
+
+
 class MogeError(RuntimeError):
     pass
 
@@ -121,84 +184,9 @@ def lib() -> C.CDLL:
         raise MogeError(f"{LIB_PATH} not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                         "(moge_b200 has no CPU fallback)")
     L = C.CDLL(LIB_PATH)
-    vp, ci, cf = C.c_void_p, C.c_int, C.c_void_p
-    L.moge_last_error.restype = C.c_char_p
-    L.moge_version.restype = C.c_char_p
-    L.moge_engine_create.argtypes = [C.POINTER(Config), ci, C.POINTER(vp)]
-    L.moge_engine_destroy.argtypes = [vp]
-    L.moge_engine_destroy.restype = None
-    L.moge_engine_set_weight.argtypes = [vp, C.c_char_p, vp, C.POINTER(C.c_int64), ci, ci, vp]
-    L.moge_engine_finalize.argtypes = [vp, vp]
-    L.moge_engine_workspace_bytes.argtypes = [vp, ci, ci, ci, ci, ci, C.POINTER(C.c_size_t)]
-    L.moge_engine_forward.argtypes = [vp, vp, ci, ci, ci, ci, ci, ci, vp, C.c_size_t, cf, cf, cf, cf, vp]
-    L.moge_engine_workspace_bytes_groups.argtypes = [vp, C.POINTER(Group), ci, C.POINTER(C.c_size_t)]
-    L.moge_engine_forward_groups.argtypes = [vp, C.POINTER(Group), ci, vp, C.c_size_t, vp]
-    L.moge_engine_num_ops.argtypes = [vp, C.POINTER(ci)]
-    L.moge_attention_work_list.argtypes = [C.POINTER(ci), ci, ci, ci, C.POINTER(ci), ci, C.POINTER(ci), C.POINTER(ci), C.POINTER(ci)]
-    L.moge_engine_op_info.argtypes = [vp, ci, C.c_char_p, ci, C.POINTER(C.c_double), C.POINTER(C.c_double)]
-    L.moge_engine_profile.argtypes = [vp, C.POINTER(C.c_float), ci, vp]
-    L.moge_recover_focal_shift.argtypes = [vp, vp, vp, ci, ci, ci, vp, vp, vp, vp]
-    L.moge_postprocess.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
-    L.moge_peer_alloc.argtypes = [C.c_size_t, C.POINTER(vp), C.c_char_p]
-    L.moge_peer_free.argtypes = [vp]
-    L.moge_peer_open.argtypes = [C.c_char_p, C.POINTER(vp)]
-    L.moge_peer_close.argtypes = [vp]
-    L.moge_peer_copy.argtypes = [vp, vp, C.c_size_t, vp]
-    L.moge_peer_flag_set.argtypes = [vp, ci, vp]
-    L.moge_peer_flag_wait.argtypes = [vp, ci, vp]
-    L.moge_op_linear.argtypes = [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]
-    L.moge_op_linear_ln.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp]
-    L.moge_op_attention.argtypes = [vp, vp, ci, ci, ci, ci, ci, vp]
-    L.moge_op_layernorm.argtypes = [vp, vp, vp, vp, ci, ci, ci, vp]
-    L.moge_op_conv.argtypes = [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, vp]
-    i64, sz = C.c_int64, C.c_size_t
-    L.moge_align_workspace_bytes.argtypes = [ci, ci, i64, ci, C.POINTER(sz)]
-    L.moge_align.argtypes = [vp, vp, vp, vp, ci, i64, ci, vp, vp, vp, vp, sz, vp]
-    L.moge_align_anchored.argtypes = [vp, vp, vp, ci, C.c_float, i64, ci, vp, vp, vp, vp, sz, vp]
-    L.moge_align_affine_lstsq.argtypes = [vp, vp, vp, i64, i64, vp, vp, vp]
-    L.moge_engine_create_v1.argtypes = [C.POINTER(V1Config), ci, C.POINTER(vp)]
-    L.moge_v1_workspace_bytes.argtypes = [vp, ci, ci, ci, ci, ci, C.POINTER(C.c_size_t)]
-    L.moge_v1_forward.argtypes = [vp, vp, ci, ci, ci, ci, ci, ci, vp, C.c_size_t, vp, vp, vp]
-    L.moge_v1_postprocess.argtypes = [vp, vp, C.c_float, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp]
-    L.moge_op_resize_bicubic_aa.argtypes = [vp, ci, ci, ci, ci, ci, ci, ci, vp, vp]
-    L.moge_op_groupnorm_relu.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp]
-    L.moge_op_conv_transpose_uv.argtypes = [vp, vp, vp, vp, ci, ci, ci, ci, ci, C.c_float, C.c_float, ci, vp]
-    L.moge_bicubic_aa_weights.argtypes = [ci, ci, ci, C.POINTER(ci), C.POINTER(C.c_float), ci]
-    L.moge_metrics_workspace_bytes.argtypes = [i64, ci, ci, ci, C.POINTER(sz)]
-    L.moge_metrics_resize.argtypes = [vp, i64, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp]
-    L.moge_metrics_stats.argtypes = [vp, vp, vp, vp, ci, vp, vp, vp, ci, i64, ci, ci, vp, vp, vp, sz, vp]
-    L.moge_metrics_eval.argtypes = [vp, vp, vp, C.POINTER(MetricVariant), ci, vp, vp, vp, vp, ci, vp, vp, i64, ci, ci, vp, i64, vp, sz,
-                                    vp]
-    L.moge_metrics_boundary.argtypes = [vp, vp, C.POINTER(MetricVariant), C.POINTER(C.c_float), i64, ci, ci, vp, i64, vp]
-    fp = C.POINTER(C.c_float)
-    L.moge_mesh_workspace_bytes.argtypes = [i64, ci, ci, C.POINTER(sz)]
-    L.moge_depth_edge.argtypes = [vp, vp, vp, i64, ci, ci, ci, fp, fp, vp, vp]
-    L.moge_mesh_count.argtypes = [vp, i64, ci, ci, vp, vp, sz, vp]
-    L.moge_mesh_build.argtypes = [vp, i64, ci, ci, ci, C.POINTER(MeshMap), ci, vp, vp, vp, sz, vp]
-    L.moge_normal_map.argtypes = [vp, vp, i64, ci, ci, vp, vp, vp]
-    L.moge_normal_edge.argtypes = [vp, vp, vp, vp, i64, ci, ci, ci, C.c_double, vp, vp, vp]
-    pc = C.POINTER(PanoramaCamera)
-    L.moge_panorama_split.argtypes = [vp, ci, ci, pc, ci, vp, ci, vp, vp, vp]
-    L.moge_panorama_workspace_bytes.argtypes = [ci, ci, ci, C.POINTER(sz)]
-    L.moge_panorama_rhs.argtypes = [vp, ci, vp, ci, ci, ci, pc, vp, ci, ci, vp, vp, vp, vp, sz, vp]
-    L.moge_panorama_lsmr.argtypes = [vp, vp, ci, ci, vp, vp, vp, vp, sz, vp]
-    L.moge_panorama_resize.argtypes = [vp, ci, ci, ci, ci, vp, vp]
-    L.moge_panorama_finish.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp]
-    L.moge_loss_workspace_bytes.argtypes = [i64, ci, ci, C.POINTER(sz)]
-    L.moge_loss_mask.argtypes = [ci, vp, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp]
-    L.moge_loss_stencil.argtypes = [ci, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp]
-    L.moge_loss_normal_map.argtypes = [vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp]
-    L.moge_loss_global.argtypes = [vp, vp, vp, C.c_float, ci, i64, ci, ci, vp, vp, vp, sz, vp]
-    L.moge_loss_anchor_weight.argtypes = [vp, vp, vp, vp, vp, i64, ci, ci, ci, vp, vp]
-    L.moge_loss_patch_mask.argtypes = [vp, vp, vp, vp, C.c_float, i64, ci, ci, i64, ci, vp, vp, vp, vp]
-    L.moge_loss_local.argtypes = [vp, vp, vp, vp, vp, C.c_float, ci, i64, ci, ci, i64, ci, vp, vp, vp, sz, vp]
-    L.moge_vis_workspace_bytes.argtypes = [i64, ci, ci, C.POINTER(sz)]
-    L.moge_vis_quantiles.argtypes = [vp, ci, vp, i64, ci, ci, fp, ci, vp, vp, sz, vp]
-    L.moge_vis_colorize.argtypes = [vp, ci, ci, vp, i64, ci, ci, vp, vp, ci, vp, vp]
-    L.moge_vis_normal.argtypes = [vp, vp, i64, ci, ci, ci, vp, vp]
-    for name in EXPORTS:
-        if name not in ("moge_last_error", "moge_version", "moge_engine_destroy"):
-            getattr(L, name).restype = ci
+    for name, sig in SIGNATURES.items():
+        f = getattr(L, name)
+        f.restype, f.argtypes = sig if isinstance(sig, tuple) else (C.c_int, sig)
     _lib = L
     return L
 
@@ -220,11 +208,30 @@ def ptr(t) -> Optional[int]:
     """Device pointer of a contiguous CUDA tensor (None -> NULL)."""
     if t is None:
         return None
-    if not t.is_cuda:
-        raise MogeError("moge_b200 operates on CUDA tensors only (no CPU fallback)")
+    require_cuda("moge_b200", t)
     if not t.is_contiguous():
         raise MogeError("tensor must be contiguous")
     return t.data_ptr()
+
+
+def require_cuda(what: str, *tensors) -> None:
+    """Raise MogeError, naming `what`, unless every argument that is not None is a CUDA tensor."""
+    import torch
+    for t in tensors:
+        if t is not None and not (isinstance(t, torch.Tensor) and t.is_cuda):
+            raise MogeError(f"{what} operates on CUDA tensors only (no CPU fallback)")
+
+
+def mask_u8(m):
+    """The contiguous uint8 view of the detached mask `m` as bool (None -> None), as the kernels take masks."""
+    import torch
+    return None if m is None else m.detach().to(torch.bool).contiguous().view(torch.uint8)
+
+
+def check_pixels(what: str, H: int, W: int, limit: int) -> None:
+    """Raise MogeError, naming `what`, when a H x W map has more than `limit` (a power of two) pixels."""
+    if H * W > limit:
+        raise MogeError(f"{what}: a {H} x {W} map is too large: at most 2^{limit.bit_length() - 1} pixels per image")
 
 
 def workspace(query, *args, device):

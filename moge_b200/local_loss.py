@@ -37,8 +37,8 @@ import torch
 from . import alignment as A
 from . import capi
 from .capi import MogeError
-from .losses import _cuda, _points, _sums
-from .metrics import _resize
+from .losses import point_maps, sum_buffer
+from .metrics import masked_nearest_resize
 
 __all__ = ["compute_anchor_sampling_weight", "affine_invariant_local_loss"]
 
@@ -56,7 +56,7 @@ def _anchor_weight(points: torch.Tensor, mask: torch.Tensor, radius_2d: int, rad
     else:
         di, dj = (d.to(device=dev, dtype=torch.int64).contiguous() for d in draws)
     weight = torch.empty(B, H, W, dtype=torch.float32, device=dev)
-    m = mask.contiguous().view(torch.uint8)
+    m = capi.mask_u8(mask)
     capi.check(capi.lib().moge_loss_anchor_weight(points.data_ptr(), m.data_ptr(), di.data_ptr(), dj.data_ptr(), radius_3d.data_ptr(),
                                                   B, H, W, num_test, weight.data_ptr(), capi.current_stream()))
     return weight / weight.sum(dim=(-2, -1), keepdim=True).add(1e-7), (di, dj)
@@ -67,7 +67,7 @@ def compute_anchor_sampling_weight(points: torch.Tensor, mask: torch.Tensor, rad
     """Per pixel of points (..., H, W, 3) with mask (..., H, W): 1 / the number of its num_test random neighbours (offsets drawn
     in [-radius_2d, radius_2d] by two torch.randint calls, as in the reference) that are inside the map, valid and within
     radius_3d (..., H, W) of it; 0 off the mask; normalised to sum 1 per image.  Returns (..., H, W) fp32."""
-    _cuda(points, mask, radius_3d)
+    capi.require_cuda("moge_b200.local_loss", points, mask, radius_3d)
     *batch_shape, H, W, _ = points.shape
     p = points.detach().to(torch.float32).reshape(-1, H, W, 3).contiguous()
     m = mask.to(torch.bool).expand(*batch_shape, H, W).reshape(-1, H, W)
@@ -85,7 +85,7 @@ class _LocalLoss(torch.autograd.Function):
         P, S = anchor.shape[0], 2 * r + 1
         params = params.clone()
         params[:, 0], params[:, 1:4] = scale.detach(), shift.detach()
-        sums, ws = _sums(P, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, P, S, S, device=pred.device)
+        sums, ws = sum_buffer(P, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, P, S, S, device=pred.device)
         capi.check(capi.lib().moge_loss_local(pred.data_ptr(), gt.data_ptr(), anchor.data_ptr(), params.data_ptr(), pmask.data_ptr(),
                                               beta, 1, B, H, W, P, r, None, sums.data_ptr(), ws.data_ptr(), ws.numel(),
                                               capi.current_stream()))
@@ -104,7 +104,7 @@ class _LocalLoss(torch.autograd.Function):
         params = params.clone()
         params[:, 7] = g.to(torch.float32)
         grad = torch.empty_like(pred)
-        sums, ws = _sums(P, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, P, S, S, device=pred.device)
+        sums, ws = sum_buffer(P, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, P, S, S, device=pred.device)
         capi.check(capi.lib().moge_loss_local(pred.data_ptr(), gt.data_ptr(), anchor.data_ptr(), params.data_ptr(), pmask.data_ptr(),
                                               ctx.beta, 2, B, H, W, P, r, grad.data_ptr(), sums.data_ptr(), ws.data_ptr(), ws.numel(),
                                               capi.current_stream()))
@@ -117,10 +117,8 @@ def _local_loss(pred_points, gt_points, focal, global_scale, level, align_resolu
     offsets "delta_i", "delta_j" (H, W, 64) and the multinomial's "selection" (num_patches B).  info holds the draws, the kept
     patches' indices into the selection, their anchors (image, i, j), and the alignment's scale and shift before the validity
     test (None where no patch is kept)."""
-    batch_shape, H, W, pred, gt = _points(pred_points, gt_points)
-    _cuda(focal)
-    if global_scale is not None:
-        _cuda(global_scale)
+    batch_shape, H, W, pred, gt = point_maps(pred_points, gt_points)
+    capi.require_cuda("moge_b200.local_loss", focal, global_scale)
     if not beta >= 0.0:
         raise MogeError(f"beta must be >= 0 (got {beta})")
     B, dev = pred.shape[0], pred.device
@@ -146,10 +144,10 @@ def _local_loss(pred_points, gt_points, focal, global_scale, level, align_resolu
     # patch masks, kept patches
     P, r = anchor.shape[0], radius_2d
     S = 2 * r + 1
-    pmask = torch.empty(P, S, S, dtype=torch.uint8, device=dev)
+    pmask = torch.empty(P, S, S, dtype=torch.bool, device=dev)
     count = torch.empty(P, dtype=torch.int32, device=dev)
     radius = torch.empty(P, dtype=torch.float32, device=dev)
-    capi.check(capi.lib().moge_loss_patch_mask(gt.data_ptr(), gt_mask.contiguous().view(torch.uint8).data_ptr(), anchor.data_ptr(),
+    capi.check(capi.lib().moge_loss_patch_mask(gt.data_ptr(), capi.mask_u8(gt_mask).data_ptr(), anchor.data_ptr(),
                                                focal.data_ptr(), 0.5 / level, B, H, W, P, r, pmask.data_ptr(), count.data_ptr(),
                                                radius.data_ptr(), capi.current_stream()))
     kept = torch.where(count >= MINIMUM_POINTS_PER_PATCH)[0]                           # host wait 2
@@ -160,9 +158,9 @@ def _local_loss(pred_points, gt_points, focal, global_scale, level, align_resolu
     info["kept"], info["anchor"] = kept, anchor
 
     # alignment on the masked nearest resize of each patch, gathered from the full maps through the patch's offset
-    lr_mask, lr_index, _, _, _ = _resize(pmask, align_resolution, align_resolution)
-    lr_i = (anchor[:, 1, None, None] - r + lr_index // S).clamp(0, H - 1)
-    lr_j = (anchor[:, 2, None, None] - r + lr_index % S).clamp(0, W - 1)
+    lr_mask, (_, i, j) = masked_nearest_resize(mask=pmask, size=(align_resolution, align_resolution), return_index=True)
+    lr_i = (anchor[:, 1, None, None] - r + i).clamp(0, H - 1)
+    lr_j = (anchor[:, 2, None, None] - r + j).clamp(0, W - 1)
     pred_lr, gt_lr = pred[img[:, None, None], lr_i, lr_j], gt_filled[img[:, None, None], lr_i, lr_j]
     local_scale, local_shift = A.align_points_scale_xyz_shift(pred_lr.flatten(-3, -2), gt_lr.flatten(-3, -2),
                                                               lr_mask.flatten(-2) / radius[:, None].add(1e-7), trunc=trunc)
@@ -175,7 +173,7 @@ def _local_loss(pred_points, gt_points, focal, global_scale, level, align_resolu
     local_scale, local_shift = torch.where(patch_valid, local_scale, 0), torch.where(patch_valid[:, None], local_shift, 0)
 
     # the harmonic mean of the GT depth per image, for the weights' floor
-    hsums, ws = _sums(B, dev), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=dev)
+    hsums, ws = sum_buffer(B, dev), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=dev)
     capi.check(capi.lib().moge_loss_local(None, gt.data_ptr(), None, None, None, float(beta), 0, B, H, W, 0, 0, None, hsums.data_ptr(),
                                           ws.data_ptr(), ws.numel(), capi.current_stream()))
     hw = H * W

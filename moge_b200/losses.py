@@ -45,13 +45,8 @@ __all__ = [
 ]
 
 
-def _cuda(*ts: torch.Tensor) -> None:
-    for t in ts:
-        if not isinstance(t, torch.Tensor) or not t.is_cuda:
-            raise MogeError("moge_b200.losses operates on CUDA tensors only (no CPU fallback)")
-
-
-def _sums(B: int, device) -> torch.Tensor:
+def sum_buffer(B: int, device) -> torch.Tensor:
+    """An uninitialised (B, LOSS_SUMS) fp64 buffer for a loss kernel's per-image (or per-patch) sums."""
     return torch.empty(B, capi.LOSS_SUMS, dtype=torch.float64, device=device)
 
 
@@ -62,7 +57,7 @@ class _MaskLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, a, b, kind):
         B, H, W = x.shape
-        sums, ws = _sums(B, x.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=x.device)
+        sums, ws = sum_buffer(B, x.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=x.device)
         capi.check(capi.lib().moge_loss_mask(kind, x.data_ptr(), a.data_ptr(), b.data_ptr(), B, H, W, None, None, sums.data_ptr(),
                                              ws.data_ptr(), ws.numel(), capi.current_stream()))
         ctx.save_for_backward(x, a, b)
@@ -81,7 +76,7 @@ class _MaskLoss(torch.autograd.Function):
 
 
 def _mask_loss(kind: int, pred: torch.Tensor, a: torch.Tensor, b: torch.Tensor):
-    _cuda(pred, a, b)
+    capi.require_cuda("moge_b200.losses", pred, a, b)
     *batch_shape, H, W = pred.shape
     flat = (-1, H, W)
     x = pred.to(torch.float32).reshape(flat).contiguous()
@@ -98,7 +93,7 @@ def mask_l2_loss(pred_mask: torch.Tensor, gt_mask_pos: torch.Tensor, gt_mask_neg
 def mask_bce_loss(pred_mask_prob: torch.Tensor, gt_mask_pos: torch.Tensor, gt_mask_neg: torch.Tensor):
     """Mean over (H, W) of (gt_mask_pos | gt_mask_neg) * binary_cross_entropy(pred_mask_prob, gt_mask_pos), with torch's -100 log
     clamp; returns (loss (...), {})."""
-    _cuda(gt_mask_pos, gt_mask_neg)
+    capi.require_cuda("moge_b200.losses", gt_mask_pos, gt_mask_neg)
     return _mask_loss(capi.LOSS_MASK_BCE, pred_mask_prob, gt_mask_pos | gt_mask_neg, gt_mask_pos)
 
 
@@ -110,7 +105,7 @@ class _StencilLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, points, gt, kind):
         B, H, W, _ = points.shape
-        sums, ws = _sums(B, points.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=points.device)
+        sums, ws = sum_buffer(B, points.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=points.device)
         capi.check(capi.lib().moge_loss_stencil(kind, points.data_ptr(), gt.data_ptr(), B, H, W, None, None, sums.data_ptr(),
                                                 ws.data_ptr(), ws.numel(), capi.current_stream()))
         ctx.save_for_backward(points, gt)
@@ -135,8 +130,10 @@ class _StencilLoss(torch.autograd.Function):
         return grad, None, None
 
 
-def _points(points: torch.Tensor, gt_points: torch.Tensor, what: str = "point maps"):
-    _cuda(points, gt_points)
+def point_maps(points: torch.Tensor, gt_points: torch.Tensor, what: str = "point maps"):
+    """Check a prediction and its GT (..., H, W, 3) and flatten them: (batch shape, H, W, prediction, detached GT), both
+    (B, H, W, 3) contiguous fp32."""
+    capi.require_cuda("moge_b200.losses", points, gt_points)
     if points.shape != gt_points.shape or points.dim() < 3 or points.shape[-1] != 3:
         raise MogeError(f"{what} must be (..., H, W, 3) of one shape, got {tuple(points.shape)} and {tuple(gt_points.shape)}")
     *batch_shape, H, W, _ = points.shape
@@ -149,7 +146,7 @@ def normal_loss(points: torch.Tensor, gt_points: torch.Tensor):
     """The angle between each of the four triangle normals of every quad and its GT normal (clamped to [1, 90] degrees, smoothed
     below 3 degrees), where its three GT corners are valid, averaged over the batch and divided by 4 max(H, W).  Returns
     (loss (), {})."""
-    _, H, W, p, g = _points(points, gt_points)
+    _, H, W, p, g = point_maps(points, gt_points)
     return _StencilLoss.apply(p, g, capi.LOSS_NORMAL) / (4 * max(H, W)), {}
 
 
@@ -157,7 +154,7 @@ def edge_loss(points: torch.Tensor, gt_points: torch.Tensor):
     """The angle between each vertical and horizontal neighbour difference and its GT difference (clamped to [0.1, 90] degrees,
     smoothed below 3 degrees), where both GT points are valid: per image, (mean over vertical pairs + mean over horizontal pairs)
     / (2 max(H, W)).  Returns (loss (...), {})."""
-    batch_shape, H, W, p, g = _points(points, gt_points)
+    batch_shape, H, W, p, g = point_maps(points, gt_points)
     means = _StencilLoss.apply(p, g, capi.LOSS_EDGE)
     return ((means[:, 0] + means[:, 1]) / (2 * max(H, W))).reshape(batch_shape), {}
 
@@ -169,7 +166,7 @@ class _NormalMapLoss(torch.autograd.Function):
     @staticmethod
     def forward(ctx, pred, gt):
         B, H, W, _ = pred.shape
-        sums, ws = _sums(B, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=pred.device)
+        sums, ws = sum_buffer(B, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=pred.device)
         capi.check(capi.lib().moge_loss_normal_map(pred.data_ptr(), gt.data_ptr(), B, H, W, None, None, sums.data_ptr(),
                                                    ws.data_ptr(), ws.numel(), capi.current_stream()))
         ctx.save_for_backward(pred, gt)
@@ -191,7 +188,7 @@ def normal_map_loss(pred_normal: torch.Tensor, gt_normal: torch.Tensor):
     three finite coordinates (the others read as (1, 1, 1)) and angle_between(a, b) = 2 atan2(|a^ - b^|, |a^ + b^|), v^ = v / |v|
     (utils3d's half-angle form).  The mask multiplies: a zero or non-finite prediction gives NaN even at an invalid pixel, as in
     the reference.  Returns (loss (...), {})."""
-    batch_shape, _, _, p, g = _points(pred_normal, gt_normal, "normal maps")
+    batch_shape, _, _, p, g = point_maps(pred_normal, gt_normal, "normal maps")
     return _NormalMapLoss.apply(p, g).reshape(batch_shape), {}
 
 
@@ -204,7 +201,7 @@ class _GlobalLoss(torch.autograd.Function):
     def forward(ctx, pred, scale, shift, gt, fixed, beta):
         B, H, W, _ = pred.shape
         params = torch.cat([scale.detach()[:, None], shift.detach(), fixed, torch.zeros_like(fixed)], dim=-1).contiguous()
-        sums, ws = _sums(B, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=pred.device)
+        sums, ws = sum_buffer(B, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=pred.device)
         capi.check(capi.lib().moge_loss_global(pred.data_ptr(), gt.data_ptr(), params.data_ptr(), beta, 1, B, H, W, None, sums.data_ptr(),
                                                ws.data_ptr(), ws.numel(), capi.current_stream()))
         ctx.save_for_backward(pred, gt, params)
@@ -220,7 +217,7 @@ class _GlobalLoss(torch.autograd.Function):
         params = params.clone()
         params[:, 6] = g.to(torch.float32) / (3 * H * W)
         grad = torch.empty_like(pred)
-        sums, ws = _sums(B, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=pred.device)
+        sums, ws = sum_buffer(B, pred.device), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=pred.device)
         capi.check(capi.lib().moge_loss_global(pred.data_ptr(), gt.data_ptr(), params.data_ptr(), ctx.beta, 2, B, H, W, grad.data_ptr(),
                                                sums.data_ptr(), ws.data_ptr(), ws.numel(), capi.current_stream()))
         return grad, sums[:, 0].to(torch.float32), sums[:, 1:4].to(torch.float32), None, None, None
@@ -231,7 +228,7 @@ def affine_invariant_global_loss(pred_points: torch.Tensor, gt_points: torch.Ten
     """Per-image truncated-L1 scale / z-shift alignment of pred_points (..., H, W, 3) to gt_points (inf / NaN = invalid) on the
     align_resolution^2 masked nearest resize, then the weighted L1 of the aligned points.  Returns (loss (...), misc
     {'truncated_error', 'delta'}, scale (...) detached)."""
-    batch_shape, H, W, pred, gt = _points(pred_points, gt_points)
+    batch_shape, H, W, pred, gt = point_maps(pred_points, gt_points)
     if not beta >= 0.0:
         raise MogeError(f"beta must be >= 0 (got {beta})")
     B, dev = pred.shape[0], pred.device
@@ -246,7 +243,7 @@ def affine_invariant_global_loss(pred_points: torch.Tensor, gt_points: torch.Ten
     # pass 0: the per-image weighted mean of the weights, for the clamp_max
     params = torch.zeros(B, 8, dtype=torch.float32, device=dev)
     params[:, 4] = valid.to(torch.float32)
-    sums, ws = _sums(B, dev), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=dev)
+    sums, ws = sum_buffer(B, dev), capi.workspace(capi.lib().moge_loss_workspace_bytes, B, H, W, device=dev)
     capi.check(capi.lib().moge_loss_global(pred.data_ptr(), gt.data_ptr(), params.data_ptr(), float(beta), 0, B, H, W, None,
                                            sums.data_ptr(), ws.data_ptr(), ws.numel(), capi.current_stream()))
     hw = H * W
@@ -267,11 +264,11 @@ def affine_invariant_global_loss(pred_points: torch.Tensor, gt_points: torch.Ten
 
 # ------------------------------------------------------------------------------------------------------------ torch expressions
 def monitoring(points: torch.Tensor) -> Dict[str, float]:
-    _cuda(points)
+    capi.require_cuda("moge_b200.losses", points)
     return {"std": points.std().item()}
 
 
 def metric_scale_loss(scale_pred: torch.Tensor, scale_gt: torch.Tensor) -> Tuple[torch.Tensor, Dict]:
-    _cuda(scale_pred, scale_gt)
+    capi.require_cuda("moge_b200.losses", scale_pred, scale_gt)
     valid = scale_gt > 0
     return torch.where(valid, F.mse_loss(scale_pred.log(), torch.where(valid, scale_gt.log(), 0), reduction="none"), 0), {}

@@ -34,25 +34,10 @@ GL_FLIP = (1.0, -1.0, -1.0)    # OpenGL conventions (infer.py:148-150): x right,
 UV_FLIP, UV_OFFSET = (1.0, -1.0), (0.0, 1.0)
 
 
-def _check_size(H: int, W: int) -> None:
-    if H * W > MAX_PIXELS:
-        raise MogeError(f"a {H} x {W} map is too large: at most 2^30 pixels per image")
-
-
-def _check_cuda(*ts) -> None:
-    for t in ts:
-        if t is not None and (not isinstance(t, torch.Tensor) or not t.is_cuda):
-            raise MogeError("moge_b200.mesh operates on CUDA tensors only (no CPU fallback)")
-
-
 def _f32(t: torch.Tensor, what: str) -> torch.Tensor:
     if t.dtype != torch.float32:
         raise MogeError(f"{what} must be float32, not {t.dtype}")
     return t.detach().contiguous()
-
-
-def _mask_u8(m: Optional[torch.Tensor]) -> Optional[torch.Tensor]:
-    return None if m is None else m.detach().to(torch.bool).contiguous().view(torch.uint8)
 
 
 def _tol(v) -> Optional[C.c_float]:
@@ -81,10 +66,10 @@ def depth_map_edge(depth: torch.Tensor, atol: float = None, rtol: float = None, 
     if mask is not None and mask.shape != depth.shape:
         raise MogeError(f"depth_map_edge: mask {tuple(mask.shape)} does not match depth {tuple(depth.shape)}")
     H, W = depth.shape[-2:]
-    _check_size(H, W)
-    _check_cuda(depth, mask)
+    capi.check_pixels("depth_map_edge", H, W, MAX_PIXELS)
+    capi.require_cuda("moge_b200.mesh", depth, mask)
     d = _f32(depth, "depth").reshape(-1, H, W)
-    m = None if mask is None else _mask_u8(mask).reshape(-1, H, W)
+    m = None if mask is None else capi.mask_u8(mask).reshape(-1, H, W)
     if d.shape[0] == 0:
         return torch.zeros(depth.shape, dtype=torch.bool, device=depth.device)
     return _edge(d, m, None, atol, rtol, kernel_size).view(torch.bool).reshape(depth.shape)
@@ -180,7 +165,7 @@ def _map_args(maps, lead: int, what: str):
     if len(maps) > capi.MESH_MAX_MAPS:
         raise MogeError(f"{what}: at most {capi.MESH_MAX_MAPS} maps")
     H, W = shape[lead], shape[lead + 1]
-    _check_size(H, W)
+    capi.check_pixels(what, H, W, MAX_PIXELS)
     out = []
     for m in maps:
         out.append(_Map(m, capi.MESH_F32, 1 if m.dim() == lead + 2 else m.shape[-1], squeeze=m.dim() == lead + 2))
@@ -189,7 +174,7 @@ def _map_args(maps, lead: int, what: str):
 
 def _sources(ms: List[_Map], mask: Optional[torch.Tensor], what: str) -> None:
     """After every shape check: the maps and the mask are CUDA tensors, the maps fp32 and contiguous."""
-    _check_cuda(mask, *[m.src for m in ms])
+    capi.require_cuda("moge_b200.mesh", mask, *[m.src for m in ms])
     for m in ms:
         m.src = _f32(m.src, f"{what}: every map")
 
@@ -201,7 +186,7 @@ def build_mesh_from_map(*maps: torch.Tensor, mask: torch.Tensor = None, tri: boo
     if mask is not None and tuple(mask.shape) != (H, W):
         raise MogeError(f"build_mesh_from_map: mask {tuple(mask.shape)} does not match the maps {(H, W)}")
     _sources(ms, mask, "build_mesh_from_map")
-    m = None if mask is None else _mask_u8(mask)[None]
+    m = None if mask is None else capi.mask_u8(mask)[None]
     return _mesh(m, 1, H, W, ms, tri, maps[0].device)[0]
 
 
@@ -215,7 +200,7 @@ def build_mesh_from_map_batch(*maps: torch.Tensor, mask: torch.Tensor = None, tr
     _sources(ms, mask, "build_mesh_from_map_batch")
     if B == 0:
         return []
-    return _mesh(_mask_u8(mask), B, H, W, ms, tri, maps[0].device)
+    return _mesh(capi.mask_u8(mask), B, H, W, ms, tri, maps[0].device)
 
 
 # ------------------------------------------------------------------------------------------------------------ after infer()
@@ -258,10 +243,10 @@ def mesh_from_output(output: Dict[str, torch.Tensor], image: torch.Tensor, thres
     else:
         raise MogeError(f"mesh_from_output: image must be uint8 (H, W, 3) or float32 (3, H, W) matching the maps, not "
                         f"{image.dtype} {tuple(image.shape[1:])}")
-    _check_size(H, W)
-    _check_cuda(points, depth, mask, normal, image)
+    capi.check_pixels("mesh_from_output", H, W, MAX_PIXELS)
+    capi.require_cuda("moge_b200.mesh", points, depth, mask, normal, image)
     d = _f32(depth, "depth")
-    m = _mask_u8(mask)
+    m = capi.mask_u8(mask)
     cleaned = _edge(d, None, m, None, threshold, 3) if remove_edge else m.clone()
     maps = _output_maps(points, colour, normal)
     results = []
@@ -301,8 +286,8 @@ def _check_normal_args(what: str, points: torch.Tensor, mask: Optional[torch.Ten
     if mask is not None and (not isinstance(mask, torch.Tensor) or tuple(mask.shape) != tuple(points.shape[:-1])):
         raise MogeError(f"{what}: mask {tuple(getattr(mask, 'shape', ()))} does not match the map {tuple(points.shape[:-1])}")
     H, W = points.shape[-3:-1]
-    _check_size(H, W)
-    _check_cuda(points, mask)
+    capi.check_pixels(what, H, W, MAX_PIXELS)
+    capi.require_cuda("moge_b200.mesh", points, mask)
     return H, W
 
 
@@ -316,7 +301,7 @@ def point_map_to_normal_map(points: torch.Tensor, mask: torch.Tensor = None, edg
         raise MogeError("point_map_to_normal_map: edge_threshold is not supported")
     H, W = _check_normal_args("point_map_to_normal_map", points, mask)
     p = _f32(points, "points").reshape(-1, H, W, 3)
-    m = None if mask is None else _mask_u8(mask).reshape(-1, H, W)
+    m = None if mask is None else capi.mask_u8(mask).reshape(-1, H, W)
     if p.shape[0] == 0:
         normal, nmask = torch.zeros_like(p), torch.zeros(p.shape[:3], dtype=torch.uint8, device=p.device)
     else:
@@ -336,7 +321,7 @@ def normal_map_edge(normals: torch.Tensor, tol: float, kernel_size: int = 3, mas
         raise MogeError(f"normal_map_edge: kernel_size {kernel_size} is not one of 3, 5, 7")
     H, W = _check_normal_args("normal_map_edge", normals, mask)
     n = _f32(normals, "normals").reshape(-1, H, W, 3)
-    m = None if mask is None else _mask_u8(mask).reshape(-1, H, W)
+    m = None if mask is None else capi.mask_u8(mask).reshape(-1, H, W)
     if n.shape[0] == 0:
         return torch.zeros(normals.shape[:-1], dtype=torch.bool, device=normals.device)
     return _normal_edge(n, m, None, None, tol, kernel_size).view(torch.bool).reshape(normals.shape[:-1])
@@ -364,11 +349,11 @@ def mesh_from_panorama(output: Dict[str, torch.Tensor], image: torch.Tensor, thr
             raise MogeError(f"mesh_from_panorama: {name} has shape {tuple(getattr(t, 'shape', ()))}, expected {want}")
     if image.dtype != torch.uint8:
         raise MogeError(f"mesh_from_panorama: image must be uint8, not {image.dtype}")
-    _check_size(H, W)
-    _check_cuda(points, depth, mask, image)
+    capi.check_pixels("mesh_from_panorama", H, W, MAX_PIXELS)
+    capi.require_cuda("moge_b200.mesh", points, depth, mask, image)
     d = _f32(depth, "depth")[None]
     p = _f32(points, "points")[None]
-    m = _mask_u8(mask)[None]
+    m = capi.mask_u8(mask)[None]
     depth_edge = _edge(d, None, None, None, threshold, 3)
     normals, nmask = _normal_map(p, m)
     cleaned = _normal_edge(normals, nmask, depth_edge, m, PANORAMA_NORMAL_TOL, 3)

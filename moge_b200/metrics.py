@@ -81,12 +81,11 @@ def masked_nearest_resize(*image: torch.Tensor, mask: torch.Tensor, size: Tuple[
     """utils3d.pt.masked_nearest_resize: resize image(s) (..., H, W[, C]) to `size` by taking, per target pixel, the valid source
     pixel nearest its centre within a window of ceil(H / h) x ceil(W / w) source pixels.  Returns (*resized, resized_mask) and
     with return_index the index tuple (*batch indices, i, j) into the source."""
-    if not mask.is_cuda:
-        raise MogeError("masked_nearest_resize operates on CUDA tensors only (no CPU fallback)")
+    capi.require_cuda("masked_nearest_resize", mask)
     H, W = mask.shape[-2:]
     th, tw = size
     batch_shape = mask.shape[:-2]
-    lr_mask, lr_index, _, _, _ = _resize(_mask_u8(mask).reshape(-1, H, W), th, tw)
+    lr_mask, lr_index, _, _, _ = _resize(capi.mask_u8(mask).reshape(-1, H, W), th, tw)
     lr_mask = lr_mask.reshape(*batch_shape, th, tw)
     lr_index = lr_index.reshape(*batch_shape, th, tw)
     batch_indices = [torch.arange(n, device=mask.device).reshape([1] * i + [n] + [1] * (len(batch_shape) - i - 1) + [1, 1])
@@ -100,15 +99,13 @@ def masked_nearest_resize(*image: torch.Tensor, mask: torch.Tensor, size: Tuple[
 
 # ------------------------------------------------------------------------------------------------------------ kernels
 def _f32(t: torch.Tensor) -> torch.Tensor:
-    if not isinstance(t, torch.Tensor) or not t.is_cuda:
-        raise MogeError("moge_b200.metrics operates on CUDA tensors only (no CPU fallback)")
+    capi.require_cuda("moge_b200.metrics", t)
     return t.detach().to(torch.float32).contiguous()
 
 
 def _mask_u8(m: torch.Tensor) -> torch.Tensor:
-    if not isinstance(m, torch.Tensor) or not m.is_cuda:
-        raise MogeError("moge_b200.metrics operates on CUDA tensors only (no CPU fallback)")
-    return m.detach().to(torch.bool).contiguous().view(torch.uint8)
+    capi.require_cuda("moge_b200.metrics", m)
+    return capi.mask_u8(m)
 
 
 def _same_shape(*ts):

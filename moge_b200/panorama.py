@@ -131,14 +131,9 @@ def _table(kind: str, size: Tuple[int, int], device: torch.device) -> torch.Tens
 
 
 def _check_size(what: str, h: int, w: int) -> None:
-    if h < 2 or w < 2 or h * w > MAX_PIXELS:
+    if h < 2 or w < 2:
         raise MogeError(f"{what}: a {h} x {w} map is outside [2 x 2, 2^28 pixels]")
-
-
-def _check_cuda(what: str, *ts) -> None:
-    for t in ts:
-        if not isinstance(t, torch.Tensor) or not t.is_cuda:
-            raise MogeError(f"{what}: expected a CUDA tensor (moge_b200 has no CPU fallback)")
+    capi.check_pixels(what, h, w, MAX_PIXELS)
 
 
 # ------------------------------------------------------------------------------------------------------------ split
@@ -151,7 +146,7 @@ def split_panorama(image: torch.Tensor, extrinsics=None, intrinsics=None, resolu
         raise MogeError("split_panorama: image must be a (H, W, 3) uint8 tensor")
     H, W = image.shape[:2]
     _check_size("split_panorama", H, W)
-    _check_cuda("split_panorama", image)
+    capi.require_cuda("split_panorama", image)
     if not 1 <= int(resolution) <= 8192:
         raise MogeError(f"split_panorama: resolution {resolution} is outside [1, 8192]")
     res = int(resolution)
@@ -199,7 +194,7 @@ def merge_panorama(width: int, height: int, src: torch.Tensor, mask: torch.Tenso
         raise MogeError("merge_panorama: src must be float32 (N, vh, vw) distances or (N, vh, vw, 3) points")
     if not isinstance(mask, torch.Tensor) or tuple(mask.shape) != tuple(src.shape[:3]) or mask.dtype not in (torch.bool, torch.uint8):
         raise MogeError(f"merge_panorama: mask must be bool / uint8 of shape {tuple(src.shape[:3])}")
-    _check_cuda("merge_panorama", src, mask)
+    capi.require_cuda("merge_panorama", src, mask)
     n, vh, vw = src.shape[:3]
     _check_size("merge_panorama view", vh, vw)
     if extrinsics is None:
@@ -214,7 +209,7 @@ def merge_panorama(width: int, height: int, src: torch.Tensor, mask: torch.Tenso
     with torch.cuda.device(dev):
         st = capi.current_stream()
         s = src.detach().contiguous()
-        m = mask.detach().contiguous().view(torch.uint8) if mask.dtype == torch.bool else (mask != 0).contiguous().view(torch.uint8)
+        m = capi.mask_u8(mask)
         ws = capi.workspace(L.moge_panorama_workspace_bytes, n, height, width, device=dev)
         stats = torch.zeros(len(levels), 2, dtype=torch.int32, device=dev)
         depth, init, out = None, None, []
@@ -250,7 +245,7 @@ def last_merge_stats() -> List[Dict[str, int]]:
 
 def finish_panorama(depth: torch.Tensor, mask: torch.Tensor, height: int, width: int):
     """infer_panorama.py:119-122: the merged depth and mask resized to (height, width) as cv2.resize does, and the points."""
-    _check_cuda("finish_panorama", depth, mask)
+    capi.require_cuda("finish_panorama", depth, mask)
     if depth.dtype != torch.float32 or depth.dim() != 2 or tuple(mask.shape) != tuple(depth.shape):
         raise MogeError("finish_panorama: depth must be float32 (h, w) and mask (h, w)")
     h, w = depth.shape
@@ -259,7 +254,7 @@ def finish_panorama(depth: torch.Tensor, mask: torch.Tensor, height: int, width:
     dev = depth.device
     with torch.cuda.device(dev):
         d = depth.contiguous()
-        m = mask.contiguous().view(torch.uint8) if mask.dtype == torch.bool else (mask != 0).to(torch.uint8)
+        m = capi.mask_u8(mask)
         out_d = torch.empty(height, width, dtype=torch.float32, device=dev)
         out_m = torch.empty(height, width, dtype=torch.uint8, device=dev)
         points = torch.empty(height, width, 3, dtype=torch.float32, device=dev)
@@ -286,7 +281,7 @@ def infer_panorama(model, image: torch.Tensor, batch_size: Optional[int] = None,
         raise MogeError(f"infer_panorama: batch_size {batch_size} must be positive")
     if not isinstance(image, torch.Tensor) or image.dtype != torch.uint8 or image.dim() != 3 or image.shape[2] != 3:
         raise MogeError("infer_panorama: image must be a (H, W, 3) uint8 tensor")
-    _check_cuda("infer_panorama", image)
+    capi.require_cuda("infer_panorama", image)
     H, W = image.shape[:2]
     _check_size("infer_panorama", H, W)
     extrinsics, intrinsics = _default_cameras()

@@ -66,14 +66,11 @@ def _maps(what: str, x: torch.Tensor, mask: Optional[torch.Tensor], channels: in
     shape = tuple(x.shape[:-1]) if channels else tuple(x.shape)
     if mask is not None and (not isinstance(mask, torch.Tensor) or tuple(mask.shape) != shape):
         raise MogeError(f"{what}: mask {tuple(getattr(mask, 'shape', ()))} does not match the map {shape}")
-    for t in (x, mask):
-        if t is not None and not t.is_cuda:
-            raise MogeError(f"{what}: expected CUDA tensors (moge_b200 has no CPU fallback)")
+    capi.require_cuda(what, x, mask)
     H, W = shape[-2:]
-    if H * W > MAX_PIXELS:
-        raise MogeError(f"{what}: a {H} x {W} map is too large: at most 2^30 pixels per image")
+    capi.check_pixels(what, H, W, MAX_PIXELS)
     x = x.detach().contiguous().view(-1, H, W, *([channels] if channels else []))
-    m = None if mask is None else mask.detach().to(torch.bool).contiguous().view(torch.uint8).view(-1, H, W)
+    m = None if mask is None else capi.mask_u8(mask).view(-1, H, W)
     return x, m, shape
 
 
