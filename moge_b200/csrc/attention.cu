@@ -320,7 +320,7 @@ attention_kernel(const __grid_constant__ CUtensorMap mapQKV, const AttnParams p)
 }
 
 // ------------------------------------------------------------------------------------------------ host
-// Work list for `nimg` images packed back to back (image i: rows [row0[i], row0[i] + n[i])): one item per (image, head, pair of
+// Work list for `nimg` images packed back to back (image i: n[i] rows): one item per (image, head, pair of
 // query tiles).  The items are dealt out in image-major / head / query-pair order, each to the CTA with the least modelled cost
 // so far (cost of an item = kv tiles x query tiles it covers; lowest CTA index on ties), and the list is returned CTA by CTA, so
 // that `ranges` gives each CTA a contiguous piece.  Since every CTA walks its items in that order and the costs track the time,
@@ -328,19 +328,20 @@ attention_kernel(const __grid_constant__ CUtensorMap mapQKV, const AttnParams p)
 // the 6 items of a 1370-token image: about 22, 8 MB) stay in L2 for all their readers.  (Handing each CTA a run of consecutive
 // items of one (image, head) instead kept 132 of them in flight, 46 MB of K/V, and the kernel re-read K/V at about 2.2 TB/s.)
 // List scheduling keeps every CTA within one item's cost of the mean.
-void attention_work_list(const int* row0, const int* n, int nimg, int heads, int ncta, std::vector<AttnItem>* items,
-                         std::vector<int2>* ranges) {
+void attention_work_list(const int* n, int nimg, int heads, int ncta, std::vector<AttnItem>* items, std::vector<int2>* ranges) {
     std::vector<AttnItem> order;
     std::vector<double> cost;
+    int row0 = 0;
     for (int i = 0; i < nimg; ++i) {
         const int nq = (n[i] + 2 * ATT_BQ - 1) / (2 * ATT_BQ), nkv = (n[i] + ATT_BKV - 1) / ATT_BKV;
         for (int h = 0; h < heads; ++h)
             for (int q = 0; q < nq; ++q) {
-                AttnItem it; it.row0 = row0[i]; it.n = n[i]; it.q0 = q * 2 * ATT_BQ; it.head = h;
+                AttnItem it; it.row0 = row0; it.n = n[i]; it.q0 = q * 2 * ATT_BQ; it.head = h;
                 order.push_back(it);
                 const int ng = (it.q0 + ATT_BQ < n[i]) ? 2 : 1;
                 cost.push_back(static_cast<double>(nkv) * ng + 0.5);          // + per-item overhead (Q load, O store)
             }
+        row0 += n[i];
     }
     const int total = static_cast<int>(order.size());
     if (ncta > total) ncta = total;
@@ -362,6 +363,16 @@ void attention_work_list(const int* row0, const int* n, int nimg, int heads, int
         for (int i : per_cta[c]) items->push_back(order[i]);
         (*ranges)[c] = make_int2(begin, static_cast<int>(items->size()));
     }
+}
+
+int upload_attention_work(const std::vector<int>& n, int heads, int ncta, const std::function<int(void**, size_t)>& alloc, cudaStream_t st,
+                          AttnWork* w) {
+    attention_work_list(n.data(), static_cast<int>(n.size()), heads, ncta, &w->items, &w->ranges);
+    MG_TRY(alloc(reinterpret_cast<void**>(&w->items_dev), w->items.size() * sizeof(AttnItem) + 16));
+    MG_TRY(alloc(reinterpret_cast<void**>(&w->ranges_dev), w->ranges.size() * sizeof(int2) + 16));
+    CUDA_TRY(cudaMemcpyAsync(w->items_dev, w->items.data(), w->items.size() * sizeof(AttnItem), cudaMemcpyHostToDevice, st));
+    CUDA_TRY(cudaMemcpyAsync(w->ranges_dev, w->ranges.data(), w->ranges.size() * sizeof(int2), cudaMemcpyHostToDevice, st));
+    return 0;
 }
 
 int launch_attention(const CUtensorMap& mapQKV, void* out, const AttnItem* items_dev, const int2* ranges_dev, int ncta, int D, int heads,

@@ -78,6 +78,14 @@ struct Group {
     float* points = nullptr; float* normal = nullptr; float* mask = nullptr; float* scale = nullptr;
 };
 
+// The group a moge_group_t describes, with its bindings; rh, rw: MoGe-1's resized image (0 for MoGe-2)
+static Group make_group(const moge_group_t& m, int rh = 0, int rw = 0) {
+    Group g;
+    g.B = m.B; g.H = m.H; g.W = m.W; g.h = m.h; g.w = m.w; g.rh = rh; g.rw = rw;
+    g.image = m.image; g.image_dtype = m.image_dtype; g.points = m.points; g.normal = m.normal; g.mask = m.mask_prob; g.scale = m.metric_scale;
+    return g;
+}
+
 struct Plan {
     std::vector<Group> groups;
     void* ws = nullptr;
@@ -85,19 +93,18 @@ struct Plan {
     OpList ops;                    // in launch order: all phase-0 ops, then phase 1, then phase 2
     std::vector<void*> owned;      // device buffers that live and die with the plan (pos tables, cls row, attention work list)
     float* cls_row = nullptr;
-    std::vector<AttnItem> att_items; std::vector<int2> att_ranges;     // host copies (source of the async upload)
+    AttnWork att;
     // ONE CUDA graph of the phase-1 launches (they touch nothing but the workspace the plan is keyed on, so the graph never
     // goes stale when the caller passes fresh input / output tensors): the launch list of a single image is ~240 kernels of a
     // few microseconds each and replaying a graph removes the per-launch CPU cost.  Phase 0 / 2 launches run eagerly around it.
     cudaGraphExec_t exec = nullptr;
     int eager_runs = 0;
-    bool same_shape(const moge_group_t* g, int n, int rh, int rw) const {
-        if (static_cast<int>(groups.size()) != n) return false;
-        for (int i = 0; i < n; ++i)
-            if (groups[i].B != g[i].B || groups[i].H != g[i].H || groups[i].W != g[i].W || groups[i].h != g[i].h || groups[i].w != g[i].w ||
-                groups[i].rh != rh || groups[i].rw != rw) return false;
-        return true;
+    bool same_shape(const std::vector<Group>& g) const {
+        return std::equal(groups.begin(), groups.end(), g.begin(), g.end(), [](const Group& a, const Group& b) {
+            return a.B == b.B && a.H == b.H && a.W == b.W && a.h == b.h && a.w == b.w && a.rh == b.rh && a.rw == b.rw;
+        });
     }
+    int alloc(void** p, size_t bytes) { CUDA_TRY(cudaMalloc(p, bytes)); owned.push_back(*p); return 0; }
     ~Plan() {
         if (exec) cudaGraphExecDestroy(exec);
         for (void* p : owned) cudaFree(p);
@@ -631,46 +638,34 @@ struct WsAlloc {
     }
 };
 
-static Level level_geom(int h, int w, int l) {
-    Level g;
-    g.H = h << l; g.W = w << l;
-    g.Hp = std::max(g.H + 2, TILE_PH);
-    g.Wp = std::max(g.W + 2, TILE_PW);
-    return g;
-}
 static size_t map_bytes(const Level& g, int B, int C) { return static_cast<size_t>(B) * g.Hp * g.Wp * C * 2; }
 
 // conv-type launch on padded NHWC maps. src/aux/skip/out buffers live in the workspace.
-static int add_conv(moge_engine* e, Plan* pl, const ConvW& cw, const void* src, const void* aux, const Level& gs, int B,
-                    int epi, void* out_raw, void* out_relu, const void* skip, const Level& go, int out_ch, bool shuffle,
-                    bool uv, float su, float sv, const std::string& name, int ncomp = 0, void* out2 = nullptr) {
+static int add_conv(moge_engine* e, Plan* pl, const ConvArgs& a, const std::string& name) {
     GemmLaunch g;
-    MG_TRY(gemm_conv(&g, e->bf16, cw, src, aux, gs, B, epi, out_raw, out_relu, skip, go, out_ch, shuffle, uv, su, sv, ncomp, out2));
-    const double px = static_cast<double>(B) * gs.H * gs.W;
+    MG_TRY(gemm_conv(&g, e->bf16, a));
+    const ConvW& cw = a.cw;
+    const double px = static_cast<double>(a.B) * a.gs.H * a.gs.W;
     const double flops = 2.0 * px * cw.N * cw.Ktot;
     double bytes = px * cw.cin * 2 + px * cw.caux * 2 + static_cast<double>(cw.N) * cw.Ktot * 2;
     // 4 output pixels per low-res pixel, each read (the neck's part) and written
-    if (epi == EPI_HEADOUT) bytes += 2 * (4 * px * (ncomp == 1 ? 4 : 16));
-    else if (epi == EPI_NECKOUT) bytes += 4 * px * ((out_raw ? 16 : 0) + (out_relu ? 16 : 0) + (out2 ? 4 : 0));
-    else bytes += px * cw.N * 2 * ((out_raw ? 1 : 0) + (out_relu ? 1 : 0)) + (skip ? px * cw.N * 2 : 0);
-    const int sms = e->num_sms;
-    pl->ops.add([=](cudaStream_t st) { return launch_gemm(g, sms, st); }, name, flops, bytes);
+    if (a.epi == EPI_HEADOUT) bytes += 2 * (4 * px * (a.ncomp == 1 ? 4 : 16));
+    else if (a.epi == EPI_NECKOUT) bytes += 4 * px * ((a.out_raw ? 16 : 0) + (a.out_relu ? 16 : 0) + (a.out2 ? 4 : 0));
+    else bytes += px * cw.N * 2 * ((a.out_raw ? 1 : 0) + (a.out_relu ? 1 : 0)) + (a.skip ? px * cw.N * 2 : 0);
+    pl->ops.add([g, sms = e->num_sms](cudaStream_t st) { return launch_gemm(g, sms, st); }, name, flops, bytes);
     return 0;
 }
 
-// Linear over row-major A [M, K] with the engine's packed (dense [N, K]) weight W; trailing arguments as in gemm_linear.
-static int add_linear(moge_engine* e, Plan* pl, const void* A, int M, int K, const void* W, int N, int epi, void* out, const float* bias,
-                      const float* v1, int ldo, const std::string& name, const LnIO* ln = nullptr, const Level* grid = nullptr,
-                      void* out_relu = nullptr, const float* v2 = nullptr, float su = 0.f, float sv = 0.f) {
+// Linear over row-major A [M, K] with the engine's packed (dense [N, K]) weight W.
+static int add_linear(moge_engine* e, Plan* pl, const LinearArgs& a, const std::string& name) {
     GemmLaunch g;
-    MG_TRY(gemm_linear(&g, e->bf16, A, M, K, W, K, N, epi, out, ldo, bias, v1, ln, grid, out_relu, v2, su, sv));
-    const double flops = 2.0 * M * static_cast<double>(N) * K;
-    double bytes = static_cast<double>(M) * K * 2 + static_cast<double>(N) * K * 2;
-    bytes += (epi == EPI_RESID) ? static_cast<double>(M) * N * 8 : (epi == EPI_PATCH) ? static_cast<double>(M) * N * 4 + static_cast<double>(g.p.T) * N * 4
-                                                                                      : static_cast<double>(M) * N * 2;
-    if (ln && ln->x16) bytes += static_cast<double>(M) * N * 2;
-    const int sms = e->num_sms;
-    pl->ops.add([=](cudaStream_t st) { return launch_gemm(g, sms, st); }, name, flops, bytes);
+    MG_TRY(gemm_linear(&g, e->bf16, a));
+    const double M = a.M, N = a.N, K = a.K;
+    const double flops = 2.0 * M * N * K;
+    double bytes = M * K * 2 + N * K * 2;
+    bytes += (a.epi == EPI_RESID) ? M * N * 8 : (a.epi == EPI_PATCH) ? M * N * 4 + static_cast<double>(g.p.T) * N * 4 : M * N * 2;
+    if (a.ln && a.ln->x16) bytes += M * N * 2;
+    pl->ops.add([g, sms = e->num_sms](cudaStream_t st) { return launch_gemm(g, sms, st); }, name, flops, bytes);
     return 0;
 }
 
@@ -678,57 +673,77 @@ struct StackBufs {     // per-level scratch maps of one ConvStack
     std::vector<void*> x_raw, x_relu, y_relu, t_up;
 };
 
-static int plan_stack(moge_engine* e, Plan* pl, const char* sname, const moge_stack_config_t& sc, const StackW& sw, bool is_neck, int B, int h,
-                      int w, float su, float sv, const StackBufs& sb, const std::vector<void*>& neck_out, void* x0_raw, void* x0_relu,
-                      void* lowres_out, void* const* neck_lowres = nullptr) {
-    const int L = sc.num_levels;
+// What plan_stack reads: one ConvStack (the neck or a head) of one shape group.
+struct StackIn {
+    std::string name;
+    const moge_stack_config_t* sc = nullptr;
+    const StackW* sw = nullptr;
+    int B = 0, h = 0, w = 0;                // batch and token grid
+    float su = 0.f, sv = 0.f;               // UV half extents
+    const StackBufs* sb = nullptr;          // scratch maps; level 0 holds the input (x_raw[0], its ReLU x_relu[0])
+    void* const* neck_maps = nullptr;       // a head: the neck's per-level outputs, the sources of its input blocks
+};
+
+// The neck writes its per-level output maps to neck_out[l]; a head passes null.  `lowres`: the fp32 low-resolution output maps the
+// last launch writes (a head: its own; the neck: points, normal and mask).
+static int plan_stack(moge_engine* e, Plan* pl, const StackIn& in, void** neck_out, void* const* lowres) {
+    const moge_stack_config_t& sc = *in.sc;
+    const StackW& sw = *in.sw;
+    const StackBufs& sb = *in.sb;
+    const bool is_neck = neck_out != nullptr;
+    const int L = sc.num_levels, B = in.B;
     const int* C = sc.dim_res_blocks;
-    void* x_raw = x0_raw;
-    void* x_relu = x0_relu;
-    auto nm = [&](const char* kind, int l) { return std::string(kind) + "." + sname + ".l" + std::to_string(l); };
+    void* x_raw = sb.x_raw[0];
+    void* x_relu = sb.x_relu[0];
+    auto nm = [&](const char* kind, int l) { return std::string(kind) + "." + in.name + ".l" + std::to_string(l); };
     for (int l = 0; l < L; ++l) {
-        const Level g = level_geom(h, w, l);
+        const Level g = level_geom(in.h, in.w, l);
         const int nres = sc.num_res_blocks[l];
+        ConvArgs res; res.B = B; res.gs = res.go = g; res.out_ch = C[l]; res.epi = EPI_DEC;        // the residual blocks' convs
         for (int r = 0; r < nres; ++r) {
             // y = conv3(relu(x)) -> only relu(y) is ever consumed
-            MG_TRY(add_conv(e, pl, sw.res[l][2 * r], x_relu, nullptr, g, B, EPI_DEC, nullptr, sb.y_relu[l], nullptr, g, C[l], false, false, 0, 0, nm("conv3x3.res_a", l)));
+            ConvArgs ra = res; ra.cw = sw.res[l][2 * r]; ra.src = x_relu; ra.out_relu = sb.y_relu[l];
+            MG_TRY(add_conv(e, pl, ra, nm("conv3x3.res_a", l)));
             // x = x + conv3(relu(y))
             void* nraw = (x_raw == sb.x_raw[l]) ? sb.t_up[l] : sb.x_raw[l];     // ping-pong between two raw maps
-            MG_TRY(add_conv(e, pl, sw.res[l][2 * r + 1], sb.y_relu[l], nullptr, g, B, EPI_DEC, nraw, (r + 1 < nres) ? x_relu : nullptr, x_raw, g, C[l], false, false, 0, 0, nm("conv3x3.res_b", l)));
+            ConvArgs rb = res; rb.cw = sw.res[l][2 * r + 1]; rb.src = sb.y_relu[l]; rb.skip = x_raw;
+            rb.out_raw = nraw; rb.out_relu = (r + 1 < nres) ? x_relu : nullptr;
+            MG_TRY(add_conv(e, pl, rb, nm("conv3x3.res_b", l)));
             x_raw = nraw;
         }
-        if (is_neck) const_cast<std::vector<void*>&>(neck_out)[l] = x_raw;
+        if (is_neck) neck_out[l] = x_raw;
         if (l == L - 1) break;
-        const Level gn = level_geom(h, w, l + 1);
+        const Level gn = level_geom(in.h, in.w, l + 1);
         const bool tail = !is_neck && (l + 1 == L - 1);
-        const void* conv_src;
+        ConvArgs a; a.B = B; a.go = gn; a.epi = EPI_DEC;     // the level's 3x3 conv: after the convT, or with the bilinear x2 folded in
+        const char* kind = "conv3x3.post";
         if (sc.resamplers[l] == MOGE_RESAMPLE_CONV_TRANSPOSE) {
-            MG_TRY(add_conv(e, pl, sw.convT[l], x_raw, nullptr, g, B, EPI_DEC, sb.t_up[l + 1], nullptr, nullptr, gn, C[l + 1], true, false, 0, 0, nm("convT", l)));
-            conv_src = sb.t_up[l + 1];
+            ConvArgs ct = a; ct.cw = sw.convT[l]; ct.src = x_raw; ct.gs = g; ct.out_ch = C[l + 1]; ct.out_raw = sb.t_up[l + 1]; ct.shuffle = true;
+            MG_TRY(add_conv(e, pl, ct, nm("convT", l)));
+            if (tail) return set_error("%s: the last resampler must be bilinear", in.name.c_str());
+            a.src = sb.t_up[l + 1]; a.gs = gn;
+            if (!is_neck) a.aux = in.neck_maps[l + 1];
         } else {
             // bilinear x2 + 3x3 conv run as ONE low-resolution conv with 4 output phases (weights expanded at load time)
-            const bool need_relu_b = sc.num_res_blocks[l + 1] > 0;
+            a.src = x_raw; a.gs = g;
             if (tail) {
-                MG_TRY(add_conv(e, pl, sw.headout, x_raw, nullptr, g, B, EPI_HEADOUT, lowres_out, nullptr, nullptr, gn, 0, false,
-                                false, 0, 0, nm("conv3x3up2.headout", l + 1), sw.ncomp));
+                a.cw = sw.headout; a.epi = EPI_HEADOUT; a.out_raw = lowres[0]; a.ncomp = sw.ncomp;
+                MG_TRY(add_conv(e, pl, a, nm("conv3x3up2.headout", l + 1)));
                 break;
             }
             if (is_neck && l + 1 == L - 1) {
                 // the neck's last level goes straight into the heads' output maps (folded through their last input/output blocks)
-                MG_TRY(add_conv(e, pl, sw.neckout, x_raw, nullptr, g, B, EPI_NECKOUT, neck_lowres[0], neck_lowres[1], nullptr, gn, 0, false, true, su, sv,
-                                nm("conv3x3up2.neckout", l + 1), 0, neck_lowres[2]));
+                a.cw = sw.neckout; a.epi = EPI_NECKOUT; a.out_raw = lowres[0]; a.out_relu = lowres[1]; a.out2 = lowres[2];
+                a.uv = true; a.su = in.su; a.sv = in.sv;
+                MG_TRY(add_conv(e, pl, a, nm("conv3x3up2.neckout", l + 1)));
                 break;
             }
-            MG_TRY(add_conv(e, pl, sw.post[l], x_raw, nullptr, g, B, EPI_DEC, sb.x_raw[l + 1], need_relu_b ? sb.x_relu[l + 1] : nullptr, nullptr, gn,
-                            C[l + 1], true, is_neck, su, sv, nm("conv3x3up2.post", l + 1)));
-            x_raw = sb.x_raw[l + 1];
-            x_relu = sb.x_relu[l + 1];
-            continue;
+            a.shuffle = true;
+            kind = "conv3x3up2.post";
         }
-        if (tail) return set_error("%s: the last resampler must be bilinear", sname);
-        const bool need_relu = sc.num_res_blocks[l + 1] > 0;
-        MG_TRY(add_conv(e, pl, sw.post[l], conv_src, is_neck ? nullptr : neck_out[l + 1], gn, B, EPI_DEC, sb.x_raw[l + 1],
-                        need_relu ? sb.x_relu[l + 1] : nullptr, nullptr, gn, C[l + 1], false, is_neck, su, sv, nm("conv3x3.post", l + 1)));
+        a.cw = sw.post[l]; a.out_ch = C[l + 1]; a.uv = is_neck; a.su = in.su; a.sv = in.sv;
+        a.out_raw = sb.x_raw[l + 1]; a.out_relu = sc.num_res_blocks[l + 1] > 0 ? sb.x_relu[l + 1] : nullptr;
+        MG_TRY(add_conv(e, pl, a, nm(kind, l + 1)));
         x_raw = sb.x_raw[l + 1];
         x_relu = sb.x_relu[l + 1];
     }
@@ -790,8 +805,9 @@ static int plan_v1_decoder(moge_engine* e, Plan* pl, const void* taps, const V1B
     const float aspect = static_cast<float>(rw) / rh;
     const float su = aspect / sqrtf(1.f + aspect * aspect), sv = 1.f / sqrtf(1.f + aspect * aspect);
     const Level g0 = level_geom(h, w, 0);
-    MG_TRY(add_linear(e, pl, taps, B * h * w, v.proj.Ktot, v.proj.w, v.proj.N, EPI_DEC, vb.x0, v.proj.bias, nullptr, v.proj.N, "gemm.projects",
-                      nullptr, &g0));
+    LinearArgs proj; proj.A = taps; proj.M = B * h * w; proj.K = v.proj.Ktot; proj.W = v.proj.w; proj.N = v.proj.N; proj.epi = EPI_DEC;
+    proj.out = vb.x0; proj.bias = v.proj.bias; proj.grid = &g0;
+    MG_TRY(add_linear(e, pl, proj, "gemm.projects"));
     const void* x = vb.x0;
     double2* part = vb.gn_part;
     float2* stats = vb.gn_stats;
@@ -807,19 +823,24 @@ static int plan_v1_decoder(moge_engine* e, Plan* pl, const void* taps, const V1B
         const V1Bufs::Lv& m = vb.lv[l];
         const int Co = c.dim_upsample[l], Hd = c.hidden_mult * Co;
         const Level gi = level_geom(h, w, l), go = level_geom(h, w, l + 1);
-        MG_TRY(add_conv(e, pl, L.convT, x, nullptr, gi, B, EPI_DEC, m.m1, nullptr, nullptr, go, Co, true, false, 0, 0, nm("convT", l)));
+        ConvArgs lv; lv.B = B; lv.gs = lv.go = go; lv.out_ch = Co; lv.epi = EPI_DEC;        // the level's convs on its output grid
+        ConvArgs ct = lv; ct.cw = L.convT; ct.src = x; ct.gs = gi; ct.out_raw = m.m1; ct.shuffle = true;
+        MG_TRY(add_conv(e, pl, ct, nm("convT", l)));
         const float* wuv = L.wuv;
         void* t = m.m1;
         pl->ops.add([=](cudaStream_t st) { return launch_uv_convT(t, go, B, Co, wuv, su, sv, bf16, st); }, nm("uv_convT", l), 0,
                     static_cast<double>(B) * go.H * go.W * Co * 4);
-        MG_TRY(add_conv(e, pl, L.conv, m.m1, nullptr, go, B, EPI_DEC, m.m0, nullptr, nullptr, go, Co, false, false, 0, 0, nm("conv3x3", l)));
+        ConvArgs cv = lv; cv.cw = L.conv; cv.src = m.m1; cv.out_raw = m.m0;
+        MG_TRY(add_conv(e, pl, cv, nm("conv3x3", l)));
         void* xr = m.m0;
         void* other = m.m1;
         for (const V1Res& R : L.res) {
             add_gn(xr, m.relu, go, Co, 1, R.g1, R.b1, l);
-            MG_TRY(add_conv(e, pl, R.c1, m.relu, nullptr, go, B, EPI_DEC, m.hraw, nullptr, nullptr, go, Hd, false, false, 0, 0, nm("conv3x3.res_a", l)));
+            ConvArgs ra = lv; ra.cw = R.c1; ra.src = m.relu; ra.out_ch = Hd; ra.out_raw = m.hraw;
+            MG_TRY(add_conv(e, pl, ra, nm("conv3x3.res_a", l)));
             add_gn(m.hraw, m.hrelu, go, Hd, R.G2, R.g2, R.b2, l);
-            MG_TRY(add_conv(e, pl, R.c2, m.hrelu, nullptr, go, B, EPI_DEC, other, nullptr, xr, go, Co, false, false, 0, 0, nm("conv3x3.res_b", l)));
+            ConvArgs rb = lv; rb.cw = R.c2; rb.src = m.hrelu; rb.out_raw = other; rb.skip = xr;
+            MG_TRY(add_conv(e, pl, rb, nm("conv3x3.res_b", l)));
             std::swap(xr, other);
         }
         x = xr;
@@ -831,7 +852,8 @@ static int plan_v1_decoder(moge_engine* e, Plan* pl, const void* taps, const V1B
     void* full = vb.full;
     pl->ops.add([=](cudaStream_t st) { return launch_resize_bilinear_nhwc(x, gl, full, gr, B, Cl, bf16, st); }, "resize_bilinear", 0,
                 static_cast<double>(B) * gl.H * gl.W * Cl * 2 + pxr * Cl * 2);
-    MG_TRY(add_conv(e, pl, v.out, vb.full, nullptr, gr, B, EPI_DEC, vb.fout, nullptr, nullptr, gr, v.out.N, false, false, 0, 0, "conv3x3.output"));
+    ConvArgs oc; oc.cw = v.out; oc.src = vb.full; oc.gs = oc.go = gr; oc.B = B; oc.out_ch = v.out.N; oc.epi = EPI_DEC; oc.out_raw = vb.fout;
+    MG_TRY(add_conv(e, pl, oc, "conv3x3.output"));
     const void* fout = vb.fout;
     const float* wout = v.wout;
     float4* pts = vb.pts;
@@ -915,27 +937,29 @@ static int plan_v2_decoder(moge_engine* e, Plan* pl, const uint8_t* taps, const 
         const float aspect = static_cast<float>(W) / H;
         const float su = aspect / sqrtf(1.f + aspect * aspect), sv = 1.f / sqrtf(1.f + aspect * aspect);
         const uint8_t* taps_g = taps + static_cast<size_t>(prow0[gi]) * c.num_taps * D * 2;
-        std::vector<void*> neck_out(L, nullptr);
         // neck level 0: folded projection GEMM over the concatenated taps (+UV rank-2 term) -> padded NHWC
-        {
-            const Level g0 = level_geom(h, w, 0);
-            const ConvW& f = e->fold0;
-            if (f.Ktot % 64) return set_error("num_taps*embed_dim must be a multiple of 64");
-            MG_TRY(add_linear(e, pl, taps_g, B * T, f.Ktot, f.w, f.N, EPI_DEC, nb.x_raw[0], f.bias, f.wu, f.N, gname("gemm.taps_proj", gi), nullptr,
-                              &g0, c.neck.num_res_blocks[0] > 0 ? nb.x_relu[0] : nullptr, f.wv, su, sv));
-        }
-        void* neck_lowres[3] = {v.pts_lr[gi], v.nrm_lr[gi], v.msk_lr[gi]};
+        const Level g0 = level_geom(h, w, 0);
+        const ConvW& f = e->fold0;
+        if (f.Ktot % 64) return set_error("num_taps*embed_dim must be a multiple of 64");
+        LinearArgs tp; tp.A = taps_g; tp.M = B * T; tp.K = f.Ktot; tp.W = f.w; tp.N = f.N; tp.epi = EPI_DEC; tp.grid = &g0;
+        tp.out = nb.x_raw[0]; tp.out_relu = c.neck.num_res_blocks[0] > 0 ? nb.x_relu[0] : nullptr;
+        tp.bias = f.bias; tp.v1 = f.wu; tp.v2 = f.wv; tp.su = su; tp.sv = sv;
+        MG_TRY(add_linear(e, pl, tp, gname("gemm.taps_proj", gi)));
+        void* lowres[3] = {v.pts_lr[gi], v.nrm_lr[gi], v.msk_lr[gi]};
         const std::string sfx = G == 1 ? std::string() : ".g" + std::to_string(gi);
-        MG_TRY(plan_stack(e, pl, ("neck" + sfx).c_str(), c.neck, e->neck, true, B, h, w, su, sv, nb, neck_out, nb.x_raw[0], nb.x_relu[0], nullptr, neck_lowres));
+        std::vector<void*> neck_out(L, nullptr);
+        StackIn in; in.B = B; in.h = h; in.w = w; in.su = su; in.sv = sv;
+        in.name = "neck" + sfx; in.sc = &c.neck; in.sw = &e->neck; in.sb = &nb;
+        MG_TRY(plan_stack(e, pl, in, neck_out.data(), lowres));
+        in.sb = &hb; in.neck_maps = neck_out.data();
         for (int i = 0; i < 3; ++i) {
             const moge_stack_config_t& sc = *head_cfg(e, i);
             if (!sc.present) continue;
-            const Level g0 = level_geom(h, w, 0);
-            const StackW& sw = e->heads[i];
-            MG_TRY(add_conv(e, pl, sw.in0, neck_out[0], nullptr, g0, B, EPI_DEC, hb.x_raw[0], sc.num_res_blocks[0] > 0 ? hb.x_relu[0] : nullptr,
-                            nullptr, g0, sc.dim_res_blocks[0], false, false, 0, 0, std::string("conv1x1.") + head_name(i) + sfx + ".l0"));
-            void* lowres = i == 0 ? static_cast<void*>(v.pts_lr[gi]) : i == 1 ? static_cast<void*>(v.nrm_lr[gi]) : static_cast<void*>(v.msk_lr[gi]);
-            MG_TRY(plan_stack(e, pl, (std::string(head_name(i)) + sfx).c_str(), sc, sw, false, B, h, w, su, sv, hb, neck_out, hb.x_raw[0], hb.x_relu[0], lowres));
+            in.name = head_name(i) + sfx; in.sc = &sc; in.sw = &e->heads[i];
+            ConvArgs a; a.cw = e->heads[i].in0; a.src = neck_out[0]; a.gs = a.go = g0; a.B = B; a.out_ch = sc.dim_res_blocks[0]; a.epi = EPI_DEC;
+            a.out_raw = hb.x_raw[0]; a.out_relu = sc.num_res_blocks[0] > 0 ? hb.x_relu[0] : nullptr;
+            MG_TRY(add_conv(e, pl, a, "conv1x1." + in.name + ".l0"));
+            MG_TRY(plan_stack(e, pl, in, nullptr, lowres + i));
         }
     }
     // ---- phase 2 (caller-bound outputs): scale head, K17 fused resize + remap
@@ -1041,8 +1065,9 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         float2* stats_g = stats + static_cast<size_t>(g.row0) * kStatsLd;
         LnIO prod; prod.x16 = ln_g; prod.stats_out = stats_g; prod.parts_out = &parts_x;
         const Level grid = level_geom(h, w, 0);
-        MG_TRY(add_linear(e, pl, patches_g, B * T, 592, e->w_patch, D, EPI_PATCH, x_g, nullptr, g.pos_table, D, gname("gemm.patch_embed", gi),
-                          &prod, &grid));
+        LinearArgs a; a.A = patches_g; a.M = B * T; a.K = 592; a.W = e->w_patch; a.N = D; a.epi = EPI_PATCH;
+        a.out = x_g; a.v1 = g.pos_table; a.ln = &prod; a.grid = &grid;
+        MG_TRY(add_linear(e, pl, a, gname("gemm.patch_embed", gi)));
         pl->ops.add([=](cudaStream_t st) { return launch_init_cls(x_g, P->cls_row, B, N, D, st); }, gname("init_cls", gi));
         const int parts0 = parts_x;
         pl->ops.add([=](cudaStream_t st) {
@@ -1056,22 +1081,12 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     };
     // ---- attention work list (image, head, query-tile pair) over the packed rows, cost-balanced over the SMs
     {
-        std::vector<int> r0, nn;
-        for (const auto& g : pl->groups)
-            for (int b = 0; b < g.B; ++b) { r0.push_back(static_cast<int>(g.row0 + static_cast<long>(b) * (g.h * g.w + 1))); nn.push_back(g.h * g.w + 1); }
-        attention_work_list(r0.data(), nn.data(), imgs, c.num_heads, sms, &pl->att_items, &pl->att_ranges);
+        std::vector<int> n;
+        for (const auto& g : pl->groups) n.insert(n.end(), g.B, g.h * g.w + 1);
+        MG_TRY(upload_attention_work(n, c.num_heads, sms, [pl](void** p, size_t bytes) { return pl->alloc(p, bytes); }, upload_stream, &pl->att));
     }
-    AttnItem* items_dev = nullptr;
-    int2* ranges_dev = nullptr;
-    const int att_ctas = static_cast<int>(pl->att_ranges.size());
-    {
-        CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&items_dev), pl->att_items.size() * sizeof(AttnItem) + 16));
-        pl->owned.push_back(items_dev);
-        CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&ranges_dev), pl->att_ranges.size() * sizeof(int2) + 16));
-        pl->owned.push_back(ranges_dev);
-        CUDA_TRY(cudaMemcpyAsync(items_dev, pl->att_items.data(), pl->att_items.size() * sizeof(AttnItem), cudaMemcpyHostToDevice, upload_stream));
-        CUDA_TRY(cudaMemcpyAsync(ranges_dev, pl->att_ranges.data(), pl->att_ranges.size() * sizeof(int2), cudaMemcpyHostToDevice, upload_stream));
-    }
+    const AttnItem* items_dev = pl->att.items_dev; const int2* ranges_dev = pl->att.ranges_dev;
+    const int att_ctas = static_cast<int>(pl->att.ranges.size());
     double att_flops = 0;
     for (const auto& g : pl->groups) { const double N = g.h * g.w + 1; att_flops += 4.0 * g.B * N * N * D; }
     // ---- transformer blocks: ONE launch per linear / attention over the packed rows of every group
@@ -1080,7 +1095,8 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         const moge_engine::Blk& b = e->blk[i];
         if (i == 0) add_rstd(parts_x);
         LnIO cons; cons.ln_rstd = rstd;
-        MG_TRY(add_linear(e, pl, ln, Mi, D, b.wqkv_ln, 3 * D, EPI_STORE16, qkv, b.b_qkv_ln, nullptr, 3 * D, "gemm.qkv", &cons));
+        LinearArgs a; a.A = ln; a.M = Mi; a.K = D; a.W = b.wqkv_ln; a.N = 3 * D; a.epi = EPI_STORE16; a.out = qkv; a.bias = b.b_qkv_ln; a.ln = &cons;
+        MG_TRY(add_linear(e, pl, a, "gemm.qkv"));
         {
             CUtensorMap mq;
             MG_TRY(make_map_2d(&mq, qkv, 3 * static_cast<uint64_t>(D), M, 3 * static_cast<uint64_t>(D), 128));
@@ -1088,10 +1104,14 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
             pl->ops.add([=](cudaStream_t st) { return launch_attention(mq, att, items_dev, ranges_dev, att_ctas, D, heads, bf16, st); }, "attention",
                         att_flops, static_cast<double>(M) * D * 8);
         }
-        MG_TRY(add_linear(e, pl, att, Mi, D, b.wproj, D, EPI_RESID, x, b.bproj, b.g1, D, "gemm.proj", &prod));
+        a = LinearArgs(); a.A = att; a.M = Mi; a.K = D; a.W = b.wproj; a.N = D; a.epi = EPI_RESID; a.out = x; a.bias = b.bproj; a.v1 = b.g1; a.ln = &prod;
+        MG_TRY(add_linear(e, pl, a, "gemm.proj"));
         add_rstd(parts_x);
-        MG_TRY(add_linear(e, pl, ln, Mi, D, b.wfc1_ln, 4 * D, EPI_GELU16, hid, b.b_fc1_ln, nullptr, 4 * D, "gemm.fc1", &cons));
-        MG_TRY(add_linear(e, pl, hid, Mi, 4 * D, b.wfc2, D, EPI_RESID, x, b.bfc2, b.g2, D, "gemm.fc2", (i + 1 < c.depth) ? &prod : nullptr));
+        a = LinearArgs(); a.A = ln; a.M = Mi; a.K = D; a.W = b.wfc1_ln; a.N = 4 * D; a.epi = EPI_GELU16; a.out = hid; a.bias = b.b_fc1_ln; a.ln = &cons;
+        MG_TRY(add_linear(e, pl, a, "gemm.fc1"));
+        a = LinearArgs(); a.A = hid; a.M = Mi; a.K = 4 * D; a.W = b.wfc2; a.N = D; a.epi = EPI_RESID; a.out = x; a.bias = b.bfc2; a.v1 = b.g2;
+        a.ln = (i + 1 < c.depth) ? &prod : nullptr;
+        MG_TRY(add_linear(e, pl, a, "gemm.fc2"));
         if (i + 1 < c.depth) add_rstd(parts_x);
         if (tap_idx < c.num_taps && c.taps[tap_idx] == i) {
             const int j = tap_idx++;
@@ -1123,9 +1143,9 @@ constexpr size_t kMaxPlans = 16;
 // same shape but another workspace REPLACES the plan instead of orphaning it.  A plan owns its device buffers (pos tables,
 // attention work list) and frees them when it is replaced or evicted (LRU) -- after the device has drained, since launches
 // that read them may still be queued on the caller's stream.
-static int get_plan(moge_engine* e, const moge_group_t* groups, int n, void* ws, size_t ws_bytes, Plan** out, cudaStream_t st, int rh, int rw) {
+static int get_plan(moge_engine* e, const std::vector<Group>& groups, void* ws, size_t ws_bytes, Plan** out, cudaStream_t st) {
     for (size_t i = 0; i < e->plans.size(); ++i) {
-        if (!e->plans[i]->same_shape(groups, n, rh, rw)) continue;
+        if (!e->plans[i]->same_shape(groups)) continue;
         if (e->plans[i]->ws == ws && e->plans[i]->ws_bytes == ws_bytes) {
             std::rotate(e->plans.begin() + i, e->plans.begin() + i + 1, e->plans.end());      // most recently used last
             *out = e->plans.back().get();
@@ -1144,17 +1164,9 @@ static int get_plan(moge_engine* e, const moge_group_t* groups, int n, void* ws,
     std::unique_ptr<Plan> pl(new Plan());
     pl->ws = ws; pl->ws_bytes = ws_bytes;
     const int D = e->cfg.embed_dim;
-    void* p = nullptr;
-    CUDA_TRY(cudaMalloc(&p, D * 4));
-    pl->owned.push_back(p);
-    pl->cls_row = static_cast<float*>(p);
-    for (int i = 0; i < n; ++i) {
-        Group g;
-        g.B = groups[i].B; g.H = groups[i].H; g.W = groups[i].W; g.h = groups[i].h; g.w = groups[i].w;
-        g.rh = rh; g.rw = rw;
-        CUDA_TRY(cudaMalloc(&p, static_cast<size_t>(g.h) * g.w * D * 4));
-        pl->owned.push_back(p);
-        g.pos_table = static_cast<float*>(p);
+    MG_TRY(pl->alloc(reinterpret_cast<void**>(&pl->cls_row), D * 4));
+    for (Group g : groups) {
+        MG_TRY(pl->alloc(reinterpret_cast<void**>(&g.pos_table), static_cast<size_t>(g.h) * g.w * D * 4));
         MG_TRY(launch_pos_table(e->pos_embed, e->cls_token, e->patch_bias, D, g.h, g.w, g.pos_table, pl->cls_row, st));
         pl->groups.push_back(g);
     }
@@ -1328,11 +1340,7 @@ int moge_engine_workspace_bytes_groups(moge_engine_t* e, const moge_group_t* gro
     MG_TRY(check_groups(e, groups, n, false));
     if (e->v1) return set_error("a MoGe-1 engine takes moge_v1_workspace_bytes");
     Plan pl;
-    for (int i = 0; i < n; ++i) {
-        Group g;
-        g.B = groups[i].B; g.H = groups[i].H; g.W = groups[i].W; g.h = groups[i].h; g.w = groups[i].w;
-        pl.groups.push_back(g);
-    }
+    for (int i = 0; i < n; ++i) pl.groups.push_back(make_group(groups[i]));
     return build_plan(e, &pl, true, bytes);
 }
 
@@ -1342,21 +1350,26 @@ int moge_engine_workspace_bytes(moge_engine_t* e, int B, int H, int W, int h, in
     return moge_engine_workspace_bytes_groups(e, &g, 1, bytes);
 }
 
-// rh, rw: the resized image of a MoGe-1 call (0 for MoGe-2)
-static int forward_impl(moge_engine_t* e, const moge_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream, int rh, int rw) {
+// The checks of a forward call, before anything runs
+static int check_forward(moge_engine_t* e, const moge_group_t* groups, int n, const void* workspace) {
     if (!e || !workspace) return set_error("null argument");
     if (!e->finalized) return set_error("engine not finalized");
     MG_TRY(check_groups(e, groups, n, true));
     if (reinterpret_cast<uintptr_t>(workspace) & 1023) return set_error("workspace must be 1024-byte aligned");
+    return 0;
+}
+
+// groups: checked by check_forward, with their bindings
+static int forward_impl(moge_engine_t* e, const std::vector<Group>& groups, void* workspace, size_t workspace_bytes, void* stream) {
     CUDA_TRY(cudaSetDevice(e->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     Plan* pl;
-    MG_TRY(get_plan(e, groups, n, workspace, workspace_bytes, &pl, st, rh, rw));
+    MG_TRY(get_plan(e, groups, workspace, workspace_bytes, &pl, st));
     long tokens = 0;
-    for (int i = 0; i < n; ++i) {
+    for (size_t i = 0; i < groups.size(); ++i) {
         Group& g = pl->groups[i];
         g.image = groups[i].image; g.image_dtype = groups[i].image_dtype;
-        g.points = groups[i].points; g.normal = groups[i].normal; g.mask = groups[i].mask_prob; g.scale = groups[i].metric_scale;
+        g.points = groups[i].points; g.normal = groups[i].normal; g.mask = groups[i].mask; g.scale = groups[i].scale;
         tokens += static_cast<long>(g.B) * g.h * g.w;
     }
     e->last_plan = pl;
@@ -1407,7 +1420,10 @@ static int forward_impl(moge_engine_t* e, const moge_group_t* groups, int n, voi
 
 int moge_engine_forward_groups(moge_engine_t* e, const moge_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream) {
     if (e && e->v1) return set_error("a MoGe-1 engine runs through moge_v1_forward");
-    return forward_impl(e, groups, n, workspace, workspace_bytes, stream, 0, 0);
+    MG_TRY(check_forward(e, groups, n, workspace));
+    std::vector<Group> gs;
+    for (int i = 0; i < n; ++i) gs.push_back(make_group(groups[i]));
+    return forward_impl(e, gs, workspace, workspace_bytes, stream);
 }
 
 static int check_v1_shape(moge_engine_t* e, int B, int H, int W, int rh, int rw) {
@@ -1421,10 +1437,10 @@ static int check_v1_shape(moge_engine_t* e, int B, int H, int W, int rh, int rw)
 int moge_v1_workspace_bytes(moge_engine_t* e, int B, int H, int W, int rh, int rw, size_t* bytes) {
     if (!bytes) return set_error("null argument");
     MG_TRY(check_v1_shape(e, B, H, W, rh, rw));
+    moge_group_t g{};
+    g.B = B; g.H = H; g.W = W; g.h = rh / 14; g.w = rw / 14;
     Plan pl;
-    Group g;
-    g.B = B; g.H = H; g.W = W; g.h = rh / 14; g.w = rw / 14; g.rh = rh; g.rw = rw;
-    pl.groups.push_back(g);
+    pl.groups.push_back(make_group(g, rh, rw));
     return build_plan(e, &pl, true, bytes);
 }
 
@@ -1435,7 +1451,8 @@ int moge_v1_forward(moge_engine_t* e, const void* image, int image_dtype, int B,
     moge_group_t g{};
     g.image = image; g.image_dtype = image_dtype; g.B = B; g.H = H; g.W = W; g.h = rh / 14; g.w = rw / 14;
     g.points = points; g.mask_prob = mask;
-    return forward_impl(e, &g, 1, workspace, workspace_bytes, stream, rh, rw);
+    MG_TRY(check_forward(e, &g, 1, workspace));
+    return forward_impl(e, {make_group(g, rh, rw)}, workspace, workspace_bytes, stream);
 }
 
 int moge_v1_postprocess(float* points, const float* mask, float mask_threshold, const float* focal_in, int B, int H, int W,
@@ -1505,196 +1522,6 @@ int moge_postprocess(float* points, const float* normal_in, const float* mask_pr
     if (normal_in && !normal_out) return set_error("normal_out required when normal_in is given");
     return launch_postprocess(points, normal_in, mask_prob, metric_scale, focal, shift, B, H, W, force_projection, apply_mask, depth,
                               normal_out, mask_out, intrinsics, static_cast<cudaStream_t>(stream));
-}
-
-// ---------------------------------------------------------------------------------- operator-level entry points
-static int dev_sms() {
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    return sms;
-}
-
-int moge_op_linear(const void* x, const void* w, const float* bias, const float* gamma, void* out, int M, int N, int K, int epi,
-                   int dtype, void* stream) {
-    if (K % 8) return set_error("op_linear: K must be a multiple of 8");
-    if (epi < 0 || epi > 2) return set_error("op_linear: epi must be 0..2");
-    GemmLaunch g;
-    MG_TRY(gemm_linear(&g, dtype == MOGE_BF16, x, M, K, w, K, N, epi, out, N, bias, gamma));
-    return launch_gemm(g, dev_sms(), static_cast<cudaStream_t>(stream));
-}
-
-int moge_op_attention(const void* qkv, void* out, int B, int N, int D, int heads, int dtype, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    if (B <= 0 || N <= 0) return set_error("op_attention: bad shape B=%d N=%d", B, N);
-    CUtensorMap mq;
-    MG_TRY(make_map_2d(&mq, qkv, 3 * static_cast<uint64_t>(D), static_cast<uint64_t>(B) * N, 3 * static_cast<uint64_t>(D), 128));
-    std::vector<int> row0(B), n(B, N);
-    for (int b = 0; b < B; ++b) row0[b] = b * N;
-    std::vector<AttnItem> items;
-    std::vector<int2> ranges;
-    attention_work_list(row0.data(), n.data(), B, heads, dev_sms(), &items, &ranges);
-    AttnItem* items_dev = nullptr;
-    int2* ranges_dev = nullptr;
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&items_dev), items.size() * sizeof(AttnItem) + 16));
-    if (cudaMalloc(reinterpret_cast<void**>(&ranges_dev), ranges.size() * sizeof(int2) + 16) != cudaSuccess) { cudaFree(items_dev); return set_error("op_attention: cudaMalloc failed"); }
-    int rc = 0;
-    if (cudaMemcpyAsync(items_dev, items.data(), items.size() * sizeof(AttnItem), cudaMemcpyHostToDevice, st) != cudaSuccess ||
-        cudaMemcpyAsync(ranges_dev, ranges.data(), ranges.size() * sizeof(int2), cudaMemcpyHostToDevice, st) != cudaSuccess)
-        rc = set_error("op_attention: upload failed");
-    if (rc == 0) rc = launch_attention(mq, out, items_dev, ranges_dev, static_cast<int>(ranges.size()), D, heads, dtype == MOGE_BF16, st);
-    cudaStreamSynchronize(st);
-    cudaFree(items_dev); cudaFree(ranges_dev);
-    return rc;
-}
-
-int moge_attention_work_list(const int* n_tokens, int n_images, int heads, int n_ctas, int* items, int items_cap, int* ranges, int* n_items,
-                             int* n_ranges) {
-    // host only: the work list the engine uploads for the persistent attention kernel (plan time), for inspection and tests
-    if (n_images < 0 || heads <= 0 || n_ctas <= 0 || !n_tokens) return set_error("attention_work_list: bad arguments");
-    std::vector<int> row0(n_images);
-    int r = 0;
-    for (int i = 0; i < n_images; ++i) {
-        if (n_tokens[i] <= 0) return set_error("attention_work_list: image %d has %d tokens", i, n_tokens[i]);
-        row0[i] = r; r += n_tokens[i];
-    }
-    std::vector<AttnItem> it;
-    std::vector<int2> rg;
-    attention_work_list(row0.data(), n_tokens, n_images, heads, n_ctas, &it, &rg);
-    if (n_items) *n_items = static_cast<int>(it.size());
-    if (n_ranges) *n_ranges = static_cast<int>(rg.size());
-    if (items) {
-        if (items_cap < static_cast<int>(it.size())) return set_error("attention_work_list: items_cap %d < %zu", items_cap, it.size());
-        for (size_t i = 0; i < it.size(); ++i) { items[4 * i] = it[i].row0; items[4 * i + 1] = it[i].n; items[4 * i + 2] = it[i].q0; items[4 * i + 3] = it[i].head; }
-    }
-    if (ranges) for (size_t i = 0; i < rg.size(); ++i) { ranges[2 * i] = rg[i].x; ranges[2 * i + 1] = rg[i].y; }
-    return 0;
-}
-
-int moge_op_linear_ln(const float* x, const float* ln_gamma, const float* ln_beta, const float* w, const float* bias, void* out, int M,
-                      int N, int K, int epi, int dtype, void* stream) {
-    // out = epi(LayerNorm(x) W^T + bias) the way the engine computes it: rounded rows + row statistics, folded weights, one GEMM
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool bf16 = dtype == MOGE_BF16;
-    if (K % 64) return set_error("op_linear_ln: K must be a multiple of 64");
-    if (epi != EPI_STORE16 && epi != EPI_GELU16) return set_error("op_linear_ln: epi must be 0 (store) or 1 (GELU)");
-    void *x16 = nullptr, *w16 = nullptr;
-    float2* stats = nullptr;
-    float *rstd = nullptr, *b2 = nullptr;
-    int rc = 0;
-    if (cudaMalloc(&x16, static_cast<size_t>(M) * K * 2) != cudaSuccess || cudaMalloc(&w16, static_cast<size_t>(N) * K * 2) != cudaSuccess ||
-        cudaMalloc(&stats, static_cast<size_t>(M) * kStatsLd * 8) != cudaSuccess || cudaMalloc(&rstd, static_cast<size_t>(M) * 4) != cudaSuccess ||
-        cudaMalloc(&b2, static_cast<size_t>(N) * 4) != cudaSuccess)
-        rc = set_error("op_linear_ln: cudaMalloc failed");
-    LnIO cons;
-    cons.ln_rstd = rstd;
-    GemmLaunch g;
-    if (rc == 0) rc = gemm_linear(&g, bf16, x16, M, K, w16, K, N, epi, out, N, b2, nullptr, &cons);
-    if (rc == 0) rc = launch_ln_prepare(x, M, K, K, x16, K, stats, kStatsLd, 1, bf16, st);
-    if (rc == 0) rc = launch_ln_rstd(stats, kStatsLd, 1, M, K, rstd, st);
-    if (rc == 0) rc = launch_ln_fold(w, ln_gamma, ln_beta, bias, N, K, K, w16, b2, bf16, st);
-    if (rc == 0) rc = launch_gemm(g, dev_sms(), st);
-    cudaStreamSynchronize(st);
-    cudaFree(x16); cudaFree(w16); cudaFree(stats); cudaFree(rstd); cudaFree(b2);
-    return rc;
-}
-
-int moge_op_layernorm(const float* x, const float* gamma, const float* beta, void* out, int rows, int D, int dtype, void* stream) {
-    return launch_layernorm(x, gamma, beta, out, rows, D, D, 0, 0, 1, nullptr, dtype == MOGE_BF16, static_cast<cudaStream_t>(stream));
-}
-
-int moge_op_conv(const void* x, const float* w, const float* bias, const void* skip, void* out_raw, void* out_relu, int B, int H, int W,
-                 int Cin, int Cout, int taps, int shuffle, int dtype, void* stream) {
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool bf16 = dtype == MOGE_BF16;
-    if (Cin % 64) return set_error("op_conv: Cin must be a multiple of 64");
-    if (taps != 1 && taps != 9) return set_error("op_conv: taps must be 1 or 9");
-    if (shuffle && taps != 1) return set_error("op_conv: shuffle requires taps=1");
-    const int N = shuffle ? 4 * Cout : Cout;
-    const int Ktot = taps * Cin;
-    void* wp = nullptr;
-    CUDA_TRY(cudaMalloc(&wp, static_cast<size_t>(N) * Ktot * 2));
-    int rc = shuffle ? launch_pack_convT(w, wp, bf16, Cin, Cout, st) : launch_pack_conv(w, wp, bf16, Cout, Cin, taps, Ktot, 0, st);
-    if (rc == 0) {
-        ConvW cw;
-        cw.w = wp; cw.bias = const_cast<float*>(bias); cw.N = N; cw.Ktot = Ktot; cw.cin = Cin; cw.taps = taps;
-        const Level gs = level_geom(H, W, 0), go = level_geom(H, W, shuffle ? 1 : 0);
-        GemmLaunch g;
-        rc = gemm_conv(&g, bf16, cw, x, nullptr, gs, B, EPI_DEC, out_raw, out_relu, skip, go, Cout, shuffle != 0, false, 0.f, 0.f);
-        if (rc == 0) rc = launch_gemm(g, dev_sms(), st);
-    }
-    cudaStreamSynchronize(st);
-    cudaFree(wp);
-    return rc;
-}
-
-int moge_op_resize_bicubic_aa(const void* x, int dtype, int B, int C, int H, int W, int Ho, int Wo, float* out, void* stream) {
-    if (!x || !out) return set_error("null argument");
-    if (dtype != MOGE_F32 && dtype != MOGE_F16 && dtype != MOGE_BF16) return set_error("op_resize_bicubic_aa: unsupported dtype %d", dtype);
-    if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || Ho <= 0 || Wo <= 0) return set_error("op_resize_bicubic_aa: bad shape");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    float* tmp = nullptr;
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&tmp), static_cast<size_t>(B) * C * H * Wo * 4));
-    const int rc = launch_resize_bicubic_aa(x, dtype, B, C, H, W, Ho, Wo, tmp, out, st);
-    cudaStreamSynchronize(st);
-    cudaFree(tmp);
-    return rc;
-}
-
-int moge_op_groupnorm_relu(const void* x, void* out, const float* gamma, const float* beta, int B, int H, int W, int C, int G, int dtype,
-                           void* stream) {
-    if (!x || !out || !gamma || !beta) return set_error("null argument");
-    if (B <= 0 || H <= 0 || W <= 0 || C <= 0 || C % 8) return set_error("op_groupnorm_relu: bad shape");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool bf16 = dtype == MOGE_BF16;
-    const Level g = level_geom(H, W, 0);
-    double2* part = nullptr;
-    float2* stats = nullptr;
-    int rc = 0;
-    if (G <= 0 || cudaMalloc(reinterpret_cast<void**>(&part), static_cast<size_t>(B) * gn_tiles(H, W, C) * G * 16) != cudaSuccess ||
-        cudaMalloc(reinterpret_cast<void**>(&stats), static_cast<size_t>(B) * G * 8) != cudaSuccess)
-        rc = set_error("op_groupnorm_relu: G=%d / cudaMalloc failed", G);
-    if (rc == 0) rc = launch_gn_stats(x, g, B, C, G, part, stats, bf16, st);
-    if (rc == 0) rc = launch_gn_relu(x, out, g, B, C, G, stats, gamma, beta, bf16, st);
-    cudaStreamSynchronize(st);
-    cudaFree(part); cudaFree(stats);
-    return rc;
-}
-
-int moge_op_conv_transpose_uv(const void* x, const float* w, const float* bias, void* out, int B, int H, int W, int Cin, int Cout, float su, float sv,
-                     int dtype, void* stream) {
-    // the engine's MoGe-1 upsampling ConvTranspose: the GEMM over the feature rows (pixel shuffle), then the input-grid UV term
-    if (!x || !w || !bias || !out) return set_error("null argument");
-    if (B <= 0 || H <= 0 || W <= 0) return set_error("op_conv_transpose_uv: bad shape");
-    if (Cin % 64 || Cout <= 0 || Cout % 32) return set_error("op_conv_transpose_uv: Cin %% 64 and Cout %% 32 must be 0");
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const bool bf16 = dtype == MOGE_BF16;
-    void* wp = nullptr;
-    float* wuv = nullptr;
-    int rc = 0;
-    if (cudaMalloc(&wp, static_cast<size_t>(4) * Cout * Cin * 2) != cudaSuccess ||
-        cudaMalloc(reinterpret_cast<void**>(&wuv), static_cast<size_t>(8) * Cout * 4) != cudaSuccess)
-        rc = set_error("op_conv_transpose_uv: cudaMalloc failed");
-    if (rc == 0) rc = launch_pack_convT(w, wp, bf16, Cin, Cout, st);
-    if (rc == 0) rc = launch_pack_convT_uv(w, Cin, Cout, wuv, st);
-    if (rc == 0) {
-        ConvW cw;
-        cw.w = wp; cw.bias = const_cast<float*>(bias); cw.N = 4 * Cout; cw.Ktot = Cin; cw.cin = Cin; cw.taps = 1;
-        const Level gs = level_geom(H, W, 0), go = level_geom(H, W, 1);
-        GemmLaunch g;
-        rc = gemm_conv(&g, bf16, cw, x, nullptr, gs, B, EPI_DEC, out, nullptr, nullptr, go, Cout, true, false, 0.f, 0.f);
-        if (rc == 0) rc = launch_gemm(g, dev_sms(), st);
-        if (rc == 0) rc = launch_uv_convT(out, go, B, Cout, wuv, su, sv, bf16, st);
-    }
-    cudaStreamSynchronize(st);
-    cudaFree(wp); cudaFree(wuv);
-    return rc;
-}
-
-int moge_bicubic_aa_weights(int in, int out, int i, int* lo, float* w, int cap) {
-    if (!lo) return set_error("null argument");
-    if (in <= 0 || out <= 0 || i < 0 || i >= out) return set_error("bicubic_aa_weights: bad arguments in=%d out=%d i=%d", in, out, i);
-    return bicubic_aa_taps(in, out, i, lo, w, cap);
 }
 
 }  // extern "C"

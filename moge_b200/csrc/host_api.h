@@ -5,6 +5,7 @@
 #include <stdint.h>
 #include <stddef.h>
 #include <atomic>
+#include <functional>
 #include <vector>
 #include <utility>
 
@@ -97,6 +98,8 @@ int make_map_nhwc(CUtensorMap* m, const void* base, uint64_t C, uint64_t Wp, uin
 // params and tensor maps; launch_gemm runs the result.  A builder fails (returns -1) on a shape no variant covers.
 struct GemmLaunch;
 struct Level { int H, W, Hp, Wp; };      // an image grid and its padded NHWC allocation (1-pixel replicated border)
+// level l of the decoder over an h x w token grid: (h << l) x (w << l), padded to at least one pixel tile
+Level level_geom(int h, int w, int l);
 
 struct ConvW {          // packed 3x3 / 1x1 / convT weights for one launch
     void* w = nullptr;  // [N, Ktot] 16-bit
@@ -114,24 +117,60 @@ struct LnIO {                     // LayerNorm-fold plumbing of one linear (see 
     const float* ln_rstd = nullptr;       // consumer (EPI_STORE16 / EPI_GELU16)
 };
 
-// Linear: A [M, K] (row pitch K) times the weight W [N, K] (row pitch ldw) -> epilogue `epi` into out (row pitch ldo elements),
-// N a multiple of 128.  EPI_PATCH and EPI_DEC rows are the tokens of images on the token grid `grid`; EPI_DEC writes the padded
-// NHWC map of that grid (raw: out, ReLU copy: out_relu, UV terms v1/v2 with half extents su/sv).
-int gemm_linear(GemmLaunch* g, bool bf16, const void* A, int M, int K, const void* W, int ldw, int N, int epi, void* out, int ldo,
-                const float* bias, const float* v1, const LnIO* ln = nullptr, const Level* grid = nullptr, void* out_relu = nullptr,
-                const float* v2 = nullptr, float su = 0.f, float sv = 0.f);
+// Linear: A [M, K] times the weight W [N, K] (both row-major) -> epilogue `epi` (gemm_kernel.cuh) into out [M, N], N a multiple
+// of 128.  EPI_PATCH and EPI_DEC rows are the tokens of images on the token grid `grid`; EPI_DEC writes the padded NHWC map of
+// that grid (raw: out, ReLU copy: out_relu, UV terms v1/v2 with half extents su/sv).
+struct LinearArgs {
+    const void* A = nullptr;
+    const void* W = nullptr;
+    int M = 0, N = 0, K = 0;
+    int epi = 0;
+    void* out = nullptr;
+    void* out_relu = nullptr;
+    const float* bias = nullptr;
+    const float* v1 = nullptr;      // EPI_RESID: LayerScale gamma; EPI_PATCH: position table [T, N]; EPI_DEC: U weights
+    const float* v2 = nullptr;      // EPI_DEC: V weights
+    float su = 0.f, sv = 0.f;
+    const LnIO* ln = nullptr;
+    const Level* grid = nullptr;
+};
+int gemm_linear(GemmLaunch* g, bool bf16, const LinearArgs& a);
 // Conv on padded NHWC maps: source src (+ aux, the fused 1x1 input block) on grid gs, output on grid go with out_ch channels.
 // Picks the main loop from the shape: CONV64 (3x3, C_in = 64), CONVH (3x3, C_in >= 128) or the per-tap GEMM.
-int gemm_conv(GemmLaunch* g, bool bf16, const ConvW& cw, const void* src, const void* aux, const Level& gs, int B, int epi,
-              void* out_raw, void* out_relu, const void* skip, const Level& go, int out_ch, bool shuffle, bool uv, float su, float sv,
-              int ncomp = 0, void* out2 = nullptr);
+struct ConvArgs {
+    ConvW cw;
+    const void* src = nullptr;
+    const void* aux = nullptr;      // source of the fused 1x1 input block (cw.caux channels)
+    Level gs{}, go{};
+    int B = 0, out_ch = 0;
+    int epi = 0;
+    void* out_raw = nullptr;        // EPI_NECKOUT: points map
+    void* out_relu = nullptr;       // EPI_NECKOUT: normal map
+    void* out2 = nullptr;           // EPI_NECKOUT: mask map
+    const void* skip = nullptr;     // residual added to the raw output
+    bool shuffle = false;           // 4 output phases per source pixel, stored on the 2x grid go
+    bool uv = false;                // + the UV rank-2 term cw.wu * u + cw.wv * v, half extents su/sv
+    float su = 0.f, sv = 0.f;
+    int ncomp = 0;                  // EPI_HEADOUT: output components
+};
+int gemm_conv(GemmLaunch* g, bool bf16, const ConvArgs& a);
 int launch_gemm(const GemmLaunch& g, int num_sms, cudaStream_t st);
 
 // Attention over PACKED token rows (ragged batches): qkv [rows, 3D] (map: box {64, 128}), one work item per (image, head, pair
-// of 128-row query tiles); the persistent kernel's CTA c walks items [ranges[c].x, ranges[c].y).
+// of 128-row query tiles); the persistent kernel's CTA c walks items [ranges[c].x, ranges[c].y).  Image i has n[i] rows, packed
+// back to back.
 struct AttnItem { int row0, n, q0, head; };      // image's first row, its token count, first query row (image-relative), head
-void attention_work_list(const int* row0, const int* n, int nimg, int heads, int ncta, std::vector<AttnItem>* items,
-                         std::vector<int2>* ranges);
+void attention_work_list(const int* n, int nimg, int heads, int ncta, std::vector<AttnItem>* items, std::vector<int2>* ranges);
+// The work list, uploaded on st into two device buffers from `alloc`; the host copies are the source of the asynchronous upload
+// and live as long as the device copies.
+struct AttnWork {
+    std::vector<AttnItem> items;
+    std::vector<int2> ranges;          // one per CTA
+    AttnItem* items_dev = nullptr;
+    int2* ranges_dev = nullptr;
+};
+int upload_attention_work(const std::vector<int>& n, int heads, int ncta, const std::function<int(void**, size_t)>& alloc, cudaStream_t st,
+                          AttnWork* w);
 int launch_attention(const CUtensorMap& mapQKV, void* out, const AttnItem* items_dev, const int2* ranges_dev, int ncta, int D, int heads,
                      bool bf16, cudaStream_t st);
 
