@@ -169,6 +169,40 @@ int moge_op_layernorm(const float* x, const float* gamma, const float* beta, voi
 int moge_op_conv(const void* x, const float* w, const float* bias, const void* skip, void* out_raw, void* out_relu,
                  int B, int H, int W, int Cin, int Cout, int taps, int shuffle, int dtype, void* stream);
 
+/* ---- operator-level entry points of the encoder's row plumbing, each running the engine's kernels with its arguments and in its
+ * order.  T = h*w patch tokens per image, N = T + 1 rows per image (the cls row first).  LayerNorm statistics `stats` are float2
+ * (sum, sum of squares) per row and column group, MOGE_STATS_LD slots per row; `parts` is the number of groups a producer wrote. */
+#define MOGE_STATS_LD 16
+/* K1 (build_plan "preprocess"): antialiased bilinear resize of image (B,3,H,W) (dtype MOGE_F32/F16/BF16) to (14h, 14w), ImageNet
+ * normalisation, im2col -> patches (B*T, 592) 16-bit, column (c, py, px) = c*196 + py*14 + px, columns 588..591 zero. */
+int moge_op_preprocess(const void* image, int image_dtype, int B, int H, int W, int h, int w, void* patches, int dtype, void* stream);
+/* K3 (plan time, "pos table"): table (T, D) fp32 = bicubic resampling of the 37 x 37 grid of pos_embed (1 + 37*37, D) at scale
+ * ((h+0.1)/37, (w+0.1)/37), + patch_bias (D); cls_row (D) = cls_token + pos_embed[0]. */
+int moge_op_pos_table(const float* pos_embed, const float* cls_token, const float* patch_bias, int D, int h, int w, float* table,
+                      float* cls_row, void* stream);
+/* The encoder's front end for one group ("preprocess", "gemm.patch_embed", "init_cls", "ln_prepare.cls"): pos table, preprocess,
+ * the (D,3,14,14) weight w_patch packed to (D, 592), then x (B*N, D) fp32 with row b*N+1+t = patches[b*T+t] w^T + table[t] and
+ * row b*N = cls_row; x16 (B*N, D) its 16-bit copy, stats (B*N, MOGE_STATS_LD) the producer's partial sums (cls rows: slot 0, the
+ * other `*parts` slots zero). */
+int moge_op_patch_embed(const void* image, int image_dtype, int B, int H, int W, int h, int w, const float* w_patch, const float* b_patch,
+                        const float* pos_embed, const float* cls_token, int D, float* x, void* x16, float* stats, int* parts, int dtype,
+                        void* stream);
+/* "gemm.proj" / "gemm.fc2": x (M,N) fp32 += gamma * (a (M,K) w (N,K)^T + bias), a and w 16-bit, with the LayerNorm producer side:
+ * x16 (M,N) the rounded new rows, stats (M, MOGE_STATS_LD) their partial sums, *parts the groups per row.  Fails, launching
+ * nothing, when N needs more groups than MOGE_STATS_LD.  K % 8 == 0, N % 128 == 0. */
+int moge_op_linear_resid_ln(const void* a, const void* w, const float* bias, const float* gamma, float* x, void* x16, float* stats,
+                            int* parts, int M, int N, int K, int dtype, void* stream);
+/* "ln_rstd": rstd[r] = 1 / sqrt(E[x^2] - E[x]^2 + 1e-6) over D columns from slots [0, parts) of stats row r. */
+int moge_op_ln_rstd(const float* stats, int parts, int rows, int D, float* rstd, void* stream);
+/* "gemm.qkv" / "gemm.fc1" on given rows: out (M,N) 16-bit = epi(LayerNorm(x) w^T + bias) from the rounded rows x16 (M,K) and
+ * their rstd (M), with the folded weight of moge_op_linear_ln.  epi 0 = store, 1 = GELU.  K % 64 == 0, N % 128 == 0. */
+int moge_op_linear_ln_rows(const void* x16, const float* rstd, const float* ln_gamma, const float* ln_beta, const float* w, const float* bias,
+                           void* out, int M, int N, int K, int epi, int dtype, void* stream);
+/* "layernorm.tap": LayerNorm(eps=1e-6) of x (B*N, D) fp32; patch row (b, t) -> out[(b*(N-1) + t) * ld_out + col_off + d] 16-bit,
+ * the cls row of image b -> cls_out[b*D + d] fp32 (skipped when cls_out is NULL). */
+int moge_op_layernorm_taps(const float* x, const float* gamma, const float* beta, void* out, float* cls_out, int B, int N, int D,
+                           int ld_out, int col_off, int dtype, void* stream);
+
 /* ---- MoGe-1 (moge/model/v1.py; Python: moge_b200.model.v1, alias moge.model.v1).  The same DINOv2 encoder as above; the decoder
  * is v1's Head (v1.py:61-142): summed 1x1 projections of the taps, then per level a ConvTranspose2d(k2 s2) over cat(x, uv), a
  * replicate-padded 3x3 conv and GroupNorm residual blocks, then a bilinear resize to the resized-image grid and two output blocks

@@ -122,6 +122,13 @@ SIGNATURES = {
     "moge_op_attention": [vp, vp, ci, ci, ci, ci, ci, vp],
     "moge_op_layernorm": [vp, vp, vp, vp, ci, ci, ci, vp],
     "moge_op_conv": [vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, ci, ci, vp],
+    "moge_op_preprocess": [vp, ci, ci, ci, ci, ci, ci, vp, ci, vp],
+    "moge_op_pos_table": [vp, vp, vp, ci, ci, ci, vp, vp, vp],
+    "moge_op_patch_embed": [vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, ci, vp, vp, vp, C.POINTER(ci), ci, vp],
+    "moge_op_linear_resid_ln": [vp, vp, vp, vp, vp, vp, vp, C.POINTER(ci), ci, ci, ci, ci, vp],
+    "moge_op_ln_rstd": [vp, ci, ci, ci, vp, vp],
+    "moge_op_linear_ln_rows": [vp, vp, vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, vp],
+    "moge_op_layernorm_taps": [vp, vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp],
     "moge_align_workspace_bytes": [ci, ci, i64, ci, C.POINTER(sz)],
     "moge_align": [vp, vp, vp, vp, ci, i64, ci, vp, vp, vp, vp, sz, vp],
     "moge_align_anchored": [vp, vp, vp, ci, C.c_float, i64, ci, vp, vp, vp, vp, sz, vp],
