@@ -1,12 +1,10 @@
-// Host runtime of libmoge_b200.so: weight registry + load-time repacking, per-shape execution plans (workspace
-// layout, TMA descriptors, launch list), and the extern "C" ABI declared in include/moge_b200.h.
-#include "moge_b200.h"
+// Host runtime of libmoge_b200.so: per-shape execution plans (workspace layout, TMA descriptors, launch list), graph replay, and
+// the extern "C" ABI declared in include/moge_b200.h except the weight loading (weights.cu).
+#include "engine.h"
 #include "gemm_kernel.cuh"
-#include "host_api.h"
 
 #include <algorithm>
 #include <functional>
-#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -15,38 +13,6 @@
 namespace mg {
 
 const char* last_error();
-
-// ------------------------------------------------------------------------------------------------ helpers
-__global__ void to_f32_kernel(const void* src, int dtype, float* dst, size_t n) {
-    for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n; i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-        if (dtype == MOGE_F32) dst[i] = static_cast<const float*>(src)[i];
-        else if (dtype == MOGE_F16) dst[i] = __half2float(static_cast<const __half*>(src)[i]);
-        else dst[i] = __bfloat162float(static_cast<const __nv_bfloat16*>(src)[i]);
-    }
-}
-// dst[i] = a[i*lda] + (b ? b[i] : 0)
-__global__ void vec_combine_kernel(float* dst, const float* a, int lda, const float* b, int n) {
-    const int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) dst[i] = a[static_cast<size_t>(i) * lda] + (b ? b[i] : 0.f);
-}
-
-struct RawWeight {
-    float* p = nullptr;
-    std::vector<int64_t> shape;
-    size_t numel = 0;
-};
-
-struct StackW {
-    ConvW in0;                                  // heads: 1x1 input block at level 0
-    std::vector<std::vector<ConvW>> res;        // [level][2*r + {0,1}]
-    std::vector<ConvW> convT;                   // [level] (conv_transpose resampler)
-    std::vector<ConvW> post;                    // [level] 3x3 after the resampler (writes level l+1), fused in-block / UV
-    // folded last level of a head
-    ConvW headout;
-    int ncomp = 0;
-    // neck only: its last level folded through the heads' last-level input + output blocks (EPI_NECKOUT): N = 4 phases x 8 components
-    ConvW neckout;
-};
 
 struct Op {
     std::function<int(cudaStream_t)> fn;
@@ -110,521 +76,6 @@ struct Plan {
         for (void* p : owned) cudaFree(p);
     }
 };
-
-// MoGe-1 decoder weights (v1.py:61-142)
-struct V1Res {            // ResidualConvBlock: GN(1, C) -> ReLU -> conv C->Hd -> GN(G2, Hd) -> ReLU -> conv Hd->C, identity skip
-    ConvW c1, c2;
-    const float *g1 = nullptr, *b1 = nullptr, *g2 = nullptr, *b2 = nullptr;
-    int G2 = 1;
-};
-struct V1Level {
-    ConvW convT, conv;      // ConvTranspose2d k2s2 over the feature channels (pixel shuffle), 3x3 replicate conv
-    float* wuv = nullptr;   // [2][4 phases][C]: the convT's UV rows, applied on the input grid
-    std::vector<V1Res> res;
-};
-struct V1W {
-    ConvW proj;             // the summed 1x1 projections of the taps as one GEMM over the concatenated taps
-    std::vector<V1Level> lv;
-    ConvW out;              // both output blocks' 3x3 convs over the feature channels: N = 32 points + 32 mask
-    float* wout = nullptr;  // launch_v1_output parameters: folded UV weights, block-diagonal 64 -> 4 map, biases
-};
-
-}  // namespace mg
-
-using namespace mg;
-
-struct moge_engine {
-    moge_config_t cfg;
-    bool v1 = false;                  // created by moge_engine_create_v1: cfg holds the encoder only, v1cfg the rest
-    moge_v1_config_t v1cfg{};
-    V1W v1w;
-    int device = 0, num_sms = 132;
-    bool bf16 = false, finalized = false;
-    std::map<std::string, RawWeight> raw;
-    std::vector<void*> owned;         // cudaMalloc'd, freed at destroy
-    // packed encoder
-    void* w_patch = nullptr;
-    struct Blk {
-        // qkv / fc1 with norm1 / norm2 folded in: centred W diag(gamma) in 16 bit, b + W beta
-        void *wqkv_ln, *wfc1_ln;
-        float *b_qkv_ln, *b_fc1_ln;
-        void *wproj, *wfc2;
-        const float *bproj, *bfc2, *g1, *g2;     // g1, g2: LayerScale gamma
-    };
-    std::vector<Blk> blk;
-    const float *norm_g = nullptr, *norm_b = nullptr, *pos_embed = nullptr, *cls_token = nullptr, *patch_bias = nullptr;
-    ConvW fold0;                      // taps-concat GEMM: (output projections folded into neck.input_blocks.0)
-    StackW neck, heads[3];            // heads: points, normal, mask
-    std::vector<const float*> mlp_w, mlp_b;
-    std::vector<std::unique_ptr<Plan>> plans;      // LRU order (most recently used last), at most kMaxPlans
-    Plan* last_plan = nullptr;
-    std::vector<void*> temps;         // load-time scratch (fp32 folds), freed at the end of finalize
-    cudaStream_t own_stream = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-
-    int alloc(void** p, size_t bytes) {
-        CUDA_TRY(cudaMalloc(p, bytes ? bytes : 16));
-        owned.push_back(*p);
-        return 0;
-    }
-    int alloc_temp(void** p, size_t bytes) {
-        CUDA_TRY(cudaMalloc(p, bytes ? bytes : 16));
-        temps.push_back(*p);
-        return 0;
-    }
-};
-
-namespace mg {
-
-static const moge_stack_config_t* head_cfg(const moge_engine* e, int i) {
-    return i == 0 ? &e->cfg.points_head : i == 1 ? &e->cfg.normal_head : &e->cfg.mask_head;
-}
-static const char* head_name(int i) { return i == 0 ? "points_head" : i == 1 ? "normal_head" : "mask_head"; }
-
-static int get_raw(moge_engine* e, const std::string& key, const RawWeight** out, std::initializer_list<int64_t> shape) {
-    auto it = e->raw.find(key);
-    if (it == e->raw.end()) return set_error("missing weight '%s'", key.c_str());
-    if (shape.size()) {
-        if (it->second.shape.size() != shape.size() || !std::equal(shape.begin(), shape.end(), it->second.shape.begin())) {
-            std::string got;
-            for (auto d : it->second.shape) got += std::to_string(d) + ",";
-            std::string want;
-            for (auto d : shape) want += std::to_string(d) + ",";
-            return set_error("weight '%s' has shape (%s) expected (%s)", key.c_str(), got.c_str(), want.c_str());
-        }
-    }
-    *out = &it->second;
-    return 0;
-}
-
-// ------------------------------------------------------------------------------------------------ finalize
-static int pack_linear(moge_engine* e, const std::string& key, int N, int K, int Kpad, void** out, cudaStream_t st) {
-    const RawWeight* w;
-    MG_TRY(get_raw(e, key, &w, {}));
-    if (static_cast<int64_t>(w->numel) != static_cast<int64_t>(N) * K) return set_error("weight '%s': numel %zu != %d*%d", key.c_str(), w->numel, N, K);
-    MG_TRY(e->alloc(out, static_cast<size_t>(N) * Kpad * 2));
-    return launch_cast_2d(w->p, MOGE_F32, *out, e->bf16, N, K, K, Kpad, st);
-}
-static int vec(moge_engine* e, const std::string& key, int n, const float** out) {
-    const RawWeight* w;
-    MG_TRY(get_raw(e, key, &w, {}));
-    if (static_cast<int>(w->numel) != n) return set_error("weight '%s': numel %zu != %d", key.c_str(), w->numel, n);
-    *out = w->p;
-    return 0;
-}
-// bias = a + b (b optional), engine-owned
-static int sum_bias(moge_engine* e, const float* a, const float* b, int n, float** out, cudaStream_t st) {
-    MG_TRY(e->alloc(reinterpret_cast<void**>(out), static_cast<size_t>(n) * 4));
-    vec_combine_kernel<<<(n + 255) / 256, 256, 0, st>>>(*out, a, 1, b, n);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
-}
-
-// 3x3 conv (Cout,Cin,3,3) [+ aux 1x1 (Cout,Caux,1,1)] [+ UV 1x1 (Cout,2,1,1)] -> ConvW
-static int pack_conv3(moge_engine* e, const std::string& wkey, int Cout, int Cin, const std::string& in_key, int Caux,
-                      bool uv, ConvW* cw, cudaStream_t st, bool up2 = false) {
-    const RawWeight* w;
-    MG_TRY(get_raw(e, wkey + ".weight", &w, {Cout, Cin, 3, 3}));
-    const float* b;
-    MG_TRY(vec(e, wkey + ".bias", Cout, &b));
-    if (Cin % 64) return set_error("conv '%s': C_in=%d must be a multiple of 64", wkey.c_str(), Cin);
-    const float* wsrc = w->p;
-    int Nrows = Cout;
-    if (up2) {      // bilinear x2 folded into the conv: 4 output phases, run on the low-resolution grid (pack.cu)
-        float* wexp;
-        MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wexp), static_cast<size_t>(4) * Cout * Cin * 9 * 4));
-        MG_TRY(launch_up2_expand(w->p, wexp, Cout, Cin, st));
-        wsrc = wexp;
-        Nrows = 4 * Cout;
-    }
-    cw->N = Nrows; cw->cin = Cin; cw->caux = Caux; cw->taps = 9;
-    cw->Ktot = 9 * Cin + Caux;
-    MG_TRY(e->alloc(&cw->w, static_cast<size_t>(Nrows) * cw->Ktot * 2));
-    MG_TRY(launch_pack_conv(wsrc, cw->w, e->bf16, Nrows, Cin, 9, cw->Ktot, 0, st));
-    const float* b_in = nullptr;
-    if (!in_key.empty()) {
-        const RawWeight* wi;
-        if (uv) {
-            MG_TRY(get_raw(e, in_key + ".weight", &wi, {Cout, 2, 1, 1}));
-            MG_TRY(e->alloc(reinterpret_cast<void**>(&cw->wu), Cout * 4));
-            MG_TRY(e->alloc(reinterpret_cast<void**>(&cw->wv), Cout * 4));
-            vec_combine_kernel<<<(Cout + 255) / 256, 256, 0, st>>>(cw->wu, wi->p, 2, nullptr, Cout);
-            vec_combine_kernel<<<(Cout + 255) / 256, 256, 0, st>>>(cw->wv, wi->p + 1, 2, nullptr, Cout);
-        } else {
-            if (Caux % 64) return set_error("input block '%s': C=%d must be a multiple of 64", in_key.c_str(), Caux);
-            MG_TRY(get_raw(e, in_key + ".weight", &wi, {Cout, Caux, 1, 1}));
-            MG_TRY(launch_pack_conv(wi->p, cw->w, e->bf16, Cout, Caux, 1, cw->Ktot, 9 * Cin, st));
-        }
-        MG_TRY(vec(e, in_key + ".bias", Cout, &b_in));
-    }
-    return sum_bias(e, b, b_in, Cout, &cw->bias, st);
-}
-
-// waux: the [8, 32] map from the neck's last-level map to the heads' output components (points xyz | normal xyz | mask logit |
-// pad).  A head writes its [ncomp, 32] rows (output block o last-level input block) at `waux`; the neck reads all 8 rows.
-static int pack_stack(moge_engine* e, const std::string& name, const moge_stack_config_t& sc, bool is_neck, StackW* sw,
-                      cudaStream_t st, float* waux) {
-    const int L = sc.num_levels;
-    sw->res.assign(L, {});
-    sw->convT.assign(L, ConvW());
-    sw->post.assign(L, ConvW());
-    const int* C = sc.dim_res_blocks;
-    if (!is_neck) {
-        // level-0 input block: 1x1 conv C0 -> C0 on the neck's level-0 output
-        if (sc.dim_in[0] <= 0) return set_error("%s: level-0 input block required", name.c_str());
-        const RawWeight* w;
-        MG_TRY(get_raw(e, name + ".input_blocks.0.weight", &w, {C[0], sc.dim_in[0], 1, 1}));
-        if (sc.dim_in[0] % 64) return set_error("%s: level-0 C_in=%d must be a multiple of 64", name.c_str(), sc.dim_in[0]);
-        ConvW& cw = sw->in0;
-        cw.N = C[0]; cw.cin = sc.dim_in[0]; cw.taps = 1; cw.Ktot = sc.dim_in[0];
-        MG_TRY(e->alloc(&cw.w, static_cast<size_t>(cw.N) * cw.Ktot * 2));
-        MG_TRY(launch_pack_conv(w->p, cw.w, e->bf16, cw.N, cw.cin, 1, cw.Ktot, 0, st));
-        const float* b;
-        MG_TRY(vec(e, name + ".input_blocks.0.bias", C[0], &b));
-        MG_TRY(sum_bias(e, b, nullptr, C[0], &cw.bias, st));
-    }
-    for (int l = 0; l < L; ++l) {
-        const bool last = (l == L - 1);
-        if (sc.dim_out[l] > 0 && !(last && !is_neck)) return set_error("%s: output block at level %d unsupported", name.c_str(), l);
-        for (int r = 0; r < sc.num_res_blocks[l]; ++r) {
-            if (last && !is_neck) return set_error("%s: residual blocks at the last head level unsupported", name.c_str());
-            for (int k : {2, 5}) {
-                ConvW cw;
-                MG_TRY(pack_conv3(e, name + ".res_blocks." + std::to_string(l) + "." + std::to_string(r) + ".layers." + std::to_string(k),
-                                  C[l], C[l], "", 0, false, &cw, st));
-                sw->res[l].push_back(cw);
-            }
-        }
-        if (last) break;
-        const std::string rs = name + ".resamplers." + std::to_string(l);
-        const std::string in_key = sc.dim_in[l + 1] > 0 ? name + ".input_blocks." + std::to_string(l + 1) : std::string();
-        const bool fold_head_out = !is_neck && (l + 1 == L - 1);
-        int conv_cin;
-        if (sc.resamplers[l] == MOGE_RESAMPLE_CONV_TRANSPOSE) {
-            const RawWeight* w;
-            MG_TRY(get_raw(e, rs + ".0.weight", &w, {C[l], C[l + 1], 2, 2}));
-            if (C[l] % 64 || C[l + 1] % 32) return set_error("%s: convT %d->%d channel counts unsupported", name.c_str(), C[l], C[l + 1]);
-            ConvW& ct = sw->convT[l];
-            ct.N = 4 * C[l + 1]; ct.cin = C[l]; ct.taps = 1; ct.Ktot = C[l];
-            MG_TRY(e->alloc(&ct.w, static_cast<size_t>(ct.N) * ct.Ktot * 2));
-            MG_TRY(launch_pack_convT(w->p, ct.w, e->bf16, C[l], C[l + 1], st));
-            const float* b;
-            MG_TRY(vec(e, rs + ".0.bias", C[l + 1], &b));
-            MG_TRY(sum_bias(e, b, nullptr, C[l + 1], &ct.bias, st));
-            conv_cin = C[l + 1];
-        } else if (sc.resamplers[l] == MOGE_RESAMPLE_BILINEAR) {
-            conv_cin = C[l];
-        } else {
-            return set_error("%s: resampler type %d unsupported", name.c_str(), sc.resamplers[l]);
-        }
-        if (!fold_head_out) {
-            if (is_neck) {
-                if (sc.dim_in[l + 1] != 2) return set_error("neck: dim_in[%d] must be 2 (UV planes)", l + 1);
-                if (l + 1 == L - 1) {
-                    // Last neck level folded through the heads (EPI_NECKOUT).  The level-(L-1) neck map m = conv3x3(up2(x)) + b + Wuv uv
-                    // is consumed ONLY by the heads' last-level input blocks and, with no nonlinearity in between, by their output
-                    // blocks: head k-th component += waux[k, :] m.  Push waux through the (linear) conv: a 3x3 conv with
-                    // 4 phases x 8 components on the low-resolution grid; the 32-channel map at the 16x grid is never materialised.
-                    const int Cn = C[l + 1], K9 = conv_cin * 9;
-                    const RawWeight *wc, *wi;
-                    const float *bc, *bi;
-                    MG_TRY(get_raw(e, rs + ".1.weight", &wc, {Cn, conv_cin, 3, 3}));
-                    MG_TRY(vec(e, rs + ".1.bias", Cn, &bc));
-                    MG_TRY(get_raw(e, in_key + ".weight", &wi, {Cn, 2, 1, 1}));
-                    MG_TRY(vec(e, in_key + ".bias", Cn, &bi));
-                    float *wexp, *wfold, *bsum, *wuv;
-                    MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wexp), static_cast<size_t>(4) * Cn * K9 * 4));
-                    MG_TRY(launch_up2_expand(wc->p, wexp, Cn, conv_cin, st));                    // rows (phase, channel)
-                    MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wfold), static_cast<size_t>(32) * K9 * 4));
-                    for (int ph = 0; ph < 4; ++ph)
-                        MG_TRY(launch_sgemm(waux, Cn, wexp + static_cast<size_t>(ph) * Cn * K9, K9, wfold + static_cast<size_t>(ph) * 8 * K9, K9, 8, K9, Cn, 0, st));
-                    ConvW& no = sw->neckout;
-                    no.N = 32; no.cin = conv_cin; no.taps = 9; no.Ktot = K9;
-                    MG_TRY(e->alloc(&no.w, static_cast<size_t>(32) * K9 * 2));
-                    MG_TRY(launch_pack_conv(wfold, no.w, e->bf16, 32, conv_cin, 9, K9, 0, st));
-                    MG_TRY(sum_bias(e, bc, bi, Cn, &bsum, st));
-                    MG_TRY(e->alloc(reinterpret_cast<void**>(&no.bias), 8 * 4));
-                    MG_TRY(launch_sgemm(waux, Cn, bsum, 1, no.bias, 1, 8, 1, Cn, 0, st));
-                    MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wuv), 2 * Cn * 4));
-                    vec_combine_kernel<<<(Cn + 255) / 256, 256, 0, st>>>(wuv, wi->p, 2, nullptr, Cn);
-                    vec_combine_kernel<<<(Cn + 255) / 256, 256, 0, st>>>(wuv + Cn, wi->p + 1, 2, nullptr, Cn);
-                    CUDA_TRY(cudaGetLastError());
-                    MG_TRY(e->alloc(reinterpret_cast<void**>(&no.wu), 8 * 4));
-                    MG_TRY(e->alloc(reinterpret_cast<void**>(&no.wv), 8 * 4));
-                    MG_TRY(launch_sgemm(waux, Cn, wuv, 1, no.wu, 1, 8, 1, Cn, 0, st));
-                    MG_TRY(launch_sgemm(waux, Cn, wuv + Cn, 1, no.wv, 1, 8, 1, Cn, 0, st));
-                    continue;
-                }
-                MG_TRY(pack_conv3(e, rs + ".1", C[l + 1], conv_cin, in_key, 0, true, &sw->post[l], st, sc.resamplers[l] == MOGE_RESAMPLE_BILINEAR));
-            } else {
-                if (sc.dim_in[l + 1] <= 0) return set_error("%s: input block at level %d required", name.c_str(), l + 1);
-                if (sc.resamplers[l] == MOGE_RESAMPLE_BILINEAR) return set_error("%s: a bilinear resampler is supported at the last level only", name.c_str());
-                MG_TRY(pack_conv3(e, rs + ".1", C[l + 1], conv_cin, in_key, sc.dim_in[l + 1], false, &sw->post[l], st));
-            }
-        } else {
-            // head tail: conv3x3 (conv_cin -> 32) + in_block(neck_last 32 -> 32) then output block 32 -> ncomp, no
-            // nonlinearity in between  =>  one 3x3 conv conv_cin -> ncomp plus a [ncomp,32] map of the neck map.
-            const int Cl = C[L - 1], nc = sc.dim_out[L - 1];
-            if (Cl != 32 || sc.dim_in[L - 1] != 32 || nc <= 0 || nc > 3 || conv_cin % 64)
-                return set_error("%s: last level must be 32 channels with a 1..3 channel output block", name.c_str());
-            const RawWeight *wc, *w4, *wo;
-            const float *bc, *b4, *bo;
-            MG_TRY(get_raw(e, rs + ".1.weight", &wc, {Cl, conv_cin, 3, 3}));
-            MG_TRY(vec(e, rs + ".1.bias", Cl, &bc));
-            MG_TRY(get_raw(e, in_key + ".weight", &w4, {Cl, 32, 1, 1}));
-            MG_TRY(vec(e, in_key + ".bias", Cl, &b4));
-            MG_TRY(get_raw(e, name + ".output_blocks." + std::to_string(L - 1) + ".weight", &wo, {nc, Cl, 1, 1}));
-            MG_TRY(vec(e, name + ".output_blocks." + std::to_string(L - 1) + ".bias", nc, &bo));
-            float *tmpw, *bsum, *bfold;
-            const int K9 = conv_cin * 9;
-            MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&tmpw), static_cast<size_t>(16) * K9 * 4));
-            CUDA_TRY(cudaMemsetAsync(tmpw, 0, static_cast<size_t>(16) * K9 * 4, st));
-            if (sc.resamplers[l] != MOGE_RESAMPLE_BILINEAR) return set_error("%s: the last resampler must be bilinear", name.c_str());
-            MG_TRY(launch_sgemm(wo->p, Cl, wc->p, K9, tmpw, K9, nc, K9, Cl, 0, st));          // [nc, (ci,tap)] = (nc,Cin,3,3)
-            float* wexp;                                                                       // (4*nc,Cin,3,3), rows (phase, comp)
-            MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wexp), static_cast<size_t>(16) * K9 * 4));
-            CUDA_TRY(cudaMemsetAsync(wexp, 0, static_cast<size_t>(16) * K9 * 4, st));
-            MG_TRY(launch_up2_expand(tmpw, wexp, nc, conv_cin, st));
-            ConvW& ho = sw->headout;
-            ho.N = 16; ho.cin = conv_cin; ho.taps = 9; ho.Ktot = K9;
-            MG_TRY(e->alloc(&ho.w, static_cast<size_t>(16) * K9 * 2));
-            MG_TRY(launch_pack_conv(wexp, ho.w, e->bf16, 16, conv_cin, 9, K9, 0, st));
-            MG_TRY(launch_sgemm(wo->p, Cl, w4->p, 32, waux, 32, nc, 32, Cl, 0, st));            // [nc, 32]
-            MG_TRY(sum_bias(e, bc, b4, Cl, &bsum, st));
-            MG_TRY(e->alloc(reinterpret_cast<void**>(&bfold), 16 * 4));
-            CUDA_TRY(cudaMemsetAsync(bfold, 0, 16 * 4, st));
-            MG_TRY(launch_sgemm(wo->p, Cl, bsum, 1, bfold, 1, nc, 1, Cl, 0, st));
-            vec_combine_kernel<<<1, 32, 0, st>>>(bfold, bfold, 1, bo, nc);
-            CUDA_TRY(cudaGetLastError());
-            ho.bias = bfold;
-            sw->ncomp = nc;
-        }
-    }
-    return 0;
-}
-
-static int finalize_encoder(moge_engine* e, cudaStream_t st) {
-    const moge_config_t& c = e->cfg;
-    const int D = c.embed_dim;
-    const std::string bb = e->v1 ? "backbone." : "encoder.backbone.";
-    MG_TRY(pack_linear(e, bb + "patch_embed.proj.weight", D, 588, 592, &e->w_patch, st));
-    MG_TRY(vec(e, bb + "patch_embed.proj.bias", D, &e->patch_bias));
-    MG_TRY(vec(e, bb + "pos_embed", (1 + 37 * 37) * D, &e->pos_embed));
-    MG_TRY(vec(e, bb + "cls_token", D, &e->cls_token));
-    MG_TRY(vec(e, bb + "norm.weight", D, &e->norm_g));
-    MG_TRY(vec(e, bb + "norm.bias", D, &e->norm_b));
-    e->blk.resize(c.depth);
-    for (int i = 0; i < c.depth; ++i) {
-        const std::string p = bb + "blocks." + std::to_string(i) + ".";
-        moge_engine::Blk& b = e->blk[i];
-        MG_TRY(pack_linear(e, p + "attn.proj.weight", D, D, D, &b.wproj, st));
-        MG_TRY(pack_linear(e, p + "mlp.fc2.weight", D, 4 * D, 4 * D, &b.wfc2, st));
-        const float *bqkv, *bfc1, *ln1g, *ln1b, *ln2g, *ln2b;
-        MG_TRY(vec(e, p + "attn.qkv.bias", 3 * D, &bqkv));
-        MG_TRY(vec(e, p + "attn.proj.bias", D, &b.bproj));
-        MG_TRY(vec(e, p + "mlp.fc1.bias", 4 * D, &bfc1));
-        MG_TRY(vec(e, p + "mlp.fc2.bias", D, &b.bfc2));
-        MG_TRY(vec(e, p + "ls1.gamma", D, &b.g1));
-        MG_TRY(vec(e, p + "ls2.gamma", D, &b.g2));
-        MG_TRY(vec(e, p + "norm1.weight", D, &ln1g));
-        MG_TRY(vec(e, p + "norm1.bias", D, &ln1b));
-        MG_TRY(vec(e, p + "norm2.weight", D, &ln2g));
-        MG_TRY(vec(e, p + "norm2.bias", D, &ln2b));
-        const RawWeight *wq, *wf;
-        MG_TRY(get_raw(e, p + "attn.qkv.weight", &wq, {}));
-        MG_TRY(get_raw(e, p + "mlp.fc1.weight", &wf, {}));
-        MG_TRY(e->alloc(&b.wqkv_ln, static_cast<size_t>(3 * D) * D * 2));
-        MG_TRY(e->alloc(&b.wfc1_ln, static_cast<size_t>(4 * D) * D * 2));
-        MG_TRY(e->alloc(reinterpret_cast<void**>(&b.b_qkv_ln), static_cast<size_t>(3 * D) * 4));
-        MG_TRY(e->alloc(reinterpret_cast<void**>(&b.b_fc1_ln), static_cast<size_t>(4 * D) * 4));
-        MG_TRY(launch_ln_fold(wq->p, ln1g, ln1b, bqkv, 3 * D, D, D, b.wqkv_ln, b.b_qkv_ln, e->bf16, st));
-        MG_TRY(launch_ln_fold(wf->p, ln2g, ln2b, bfc1, 4 * D, D, D, b.wfc1_ln, b.b_fc1_ln, e->bf16, st));
-    }
-    return 0;
-}
-
-static int finalize_v2_decoder(moge_engine* e, cudaStream_t st) {
-    const moge_config_t& c = e->cfg;
-    const int D = c.embed_dim;
-    // ---- fold: neck.input_blocks.0 o (sum_j output_projections.j)  ->  one GEMM over the concatenated taps
-    {
-        const int C0 = c.neck.dim_res_blocks[0], Do = c.dim_out, nt = c.num_taps;
-        if (c.neck.dim_in[0] != Do + 2) return set_error("neck.dim_in[0]=%d must be encoder.dim_out+2=%d", c.neck.dim_in[0], Do + 2);
-        const RawWeight* w0;
-        MG_TRY(get_raw(e, "neck.input_blocks.0.weight", &w0, {C0, Do + 2, 1, 1}));
-        const float* b0;
-        MG_TRY(vec(e, "neck.input_blocks.0.bias", C0, &b0));
-        float *wf, *bf, *bp;
-        MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wf), static_cast<size_t>(C0) * nt * D * 4));
-        MG_TRY(e->alloc(reinterpret_cast<void**>(&bf), C0 * 4));
-        MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&bp), Do * 4));
-        CUDA_TRY(cudaMemsetAsync(bp, 0, Do * 4, st));
-        for (int j = 0; j < nt; ++j) {
-            const RawWeight* pj;
-            MG_TRY(get_raw(e, "encoder.output_projections." + std::to_string(j) + ".weight", &pj, {Do, D, 1, 1}));
-            const float* bj;
-            MG_TRY(vec(e, "encoder.output_projections." + std::to_string(j) + ".bias", Do, &bj));
-            MG_TRY(launch_sgemm(w0->p, Do + 2, pj->p, D, wf + static_cast<size_t>(j) * D, nt * D, C0, D, Do, 0, st));
-            vec_combine_kernel<<<(Do + 255) / 256, 256, 0, st>>>(bp, bp, 1, bj, Do);
-        }
-        MG_TRY(launch_sgemm(w0->p, Do + 2, bp, 1, bf, 1, C0, 1, Do, 0, st));
-        vec_combine_kernel<<<(C0 + 255) / 256, 256, 0, st>>>(bf, bf, 1, b0, C0);
-        ConvW& f = e->fold0;
-        f.N = C0; f.Ktot = nt * D; f.taps = 1; f.cin = nt * D;
-        MG_TRY(e->alloc(&f.w, static_cast<size_t>(C0) * f.Ktot * 2));
-        MG_TRY(launch_cast_2d(wf, MOGE_F32, f.w, e->bf16, C0, f.Ktot, f.Ktot, f.Ktot, st));
-        f.bias = bf;
-        MG_TRY(e->alloc(reinterpret_cast<void**>(&f.wu), C0 * 4));
-        MG_TRY(e->alloc(reinterpret_cast<void**>(&f.wv), C0 * 4));
-        vec_combine_kernel<<<(C0 + 255) / 256, 256, 0, st>>>(f.wu, w0->p + Do, Do + 2, nullptr, C0);
-        vec_combine_kernel<<<(C0 + 255) / 256, 256, 0, st>>>(f.wv, w0->p + Do + 1, Do + 2, nullptr, C0);
-        CUDA_TRY(cudaGetLastError());
-    }
-    // the heads' last levels first: they give the map through which the neck's last level is folded (EPI_NECKOUT)
-    float* waux;
-    MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&waux), 8 * 32 * 4));
-    CUDA_TRY(cudaMemsetAsync(waux, 0, 8 * 32 * 4, st));
-    const int row_of[3] = {0, 3, 6};          // points xyz | normal xyz | mask logit | pad
-    for (int i = 0; i < 3; ++i)
-        if (head_cfg(e, i)->present) MG_TRY(pack_stack(e, head_name(i), *head_cfg(e, i), false, &e->heads[i], st, waux + row_of[i] * 32));
-    MG_TRY(pack_stack(e, "neck", c.neck, true, &e->neck, st, waux));
-    for (int l = 0; l < c.scale_head_layers; ++l) {
-        const float *w, *b;
-        MG_TRY(vec(e, "scale_head." + std::to_string(2 * l) + ".weight", c.scale_head_dims[l] * c.scale_head_dims[l + 1], &w));
-        MG_TRY(vec(e, "scale_head." + std::to_string(2 * l) + ".bias", c.scale_head_dims[l + 1], &b));
-        e->mlp_w.push_back(w);
-        e->mlp_b.push_back(b);
-    }
-    return 0;
-}
-
-// ---- MoGe-1 decoder (keys head.*, v1.py:61-142).  The small folds are done on the host from copies of the fp32 staging weights.
-static int to_host(const RawWeight* w, size_t off, size_t n, std::vector<float>* out) {
-    out->resize(n);
-    CUDA_TRY(cudaMemcpy(out->data(), w->p + off, n * 4, cudaMemcpyDeviceToHost));
-    return 0;
-}
-static int to_dev(moge_engine* e, const std::vector<float>& v, float** out) {
-    MG_TRY(e->alloc(reinterpret_cast<void**>(out), v.size() * 4));
-    CUDA_TRY(cudaMemcpy(*out, v.data(), v.size() * 4, cudaMemcpyHostToDevice));
-    return 0;
-}
-
-static int finalize_v1(moge_engine* e, cudaStream_t st) {
-    const moge_v1_config_t& c = e->v1cfg;
-    const int D = c.embed_dim, nt = c.num_taps, P = c.dim_proj;
-    CUDA_TRY(cudaStreamSynchronize(st));       // the staging copies are written on st; the host reads some of them below
-    V1W& v = e->v1w;
-    // V4: sum_j projects.j(tap_j) = one GEMM over the concatenated taps [B*T, nt*D] with the summed bias
-    ConvW& pj = v.proj;
-    pj.N = P; pj.cin = nt * D; pj.taps = 1; pj.Ktot = nt * D;
-    MG_TRY(e->alloc(&pj.w, static_cast<size_t>(P) * pj.Ktot * 2));
-    MG_TRY(e->alloc(reinterpret_cast<void**>(&pj.bias), P * 4));
-    CUDA_TRY(cudaMemsetAsync(pj.bias, 0, P * 4, st));
-    float* wcat32;                             // [P, nt*D] fp32: tap j's weight in columns j*D ..
-    MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wcat32), static_cast<size_t>(P) * pj.Ktot * 4));
-    for (int j = 0; j < nt; ++j) {
-        const std::string k = "head.projects." + std::to_string(j);
-        const RawWeight* w;
-        const float* b;
-        MG_TRY(get_raw(e, k + ".weight", &w, {P, D, 1, 1}));
-        MG_TRY(vec(e, k + ".bias", P, &b));
-        CUDA_TRY(cudaMemcpy2DAsync(wcat32 + static_cast<size_t>(j) * D, static_cast<size_t>(pj.Ktot) * 4, w->p, static_cast<size_t>(D) * 4,
-                                   static_cast<size_t>(D) * 4, P, cudaMemcpyDeviceToDevice, st));
-        vec_combine_kernel<<<(P + 255) / 256, 256, 0, st>>>(pj.bias, pj.bias, 1, b, P);
-        CUDA_TRY(cudaGetLastError());
-    }
-    MG_TRY(launch_cast_2d(wcat32, MOGE_F32, pj.w, e->bf16, P, pj.Ktot, pj.Ktot, pj.Ktot, st));
-    int cin = P;
-    v.lv.assign(c.num_levels, V1Level());
-    for (int l = 0; l < c.num_levels; ++l) {
-        const int Co = c.dim_upsample[l], Hd = c.hidden_mult * Co;
-        const std::string pre = "head.upsample_blocks." + std::to_string(l) + ".";
-        V1Level& L = v.lv[l];
-        // V5: ConvTranspose2d(cin + 2 -> Co): rows 0..cin-1 through the GEMM, the two UV rows as the input-grid term
-        const RawWeight* wt;
-        const float* bt;
-        MG_TRY(get_raw(e, pre + "0.0.weight", &wt, {cin + 2, Co, 2, 2}));
-        MG_TRY(vec(e, pre + "0.0.bias", Co, &bt));
-        L.convT.N = 4 * Co; L.convT.cin = cin; L.convT.taps = 1; L.convT.Ktot = cin;
-        MG_TRY(e->alloc(&L.convT.w, static_cast<size_t>(4) * Co * cin * 2));
-        MG_TRY(launch_pack_convT(wt->p, L.convT.w, e->bf16, cin, Co, st));
-        MG_TRY(sum_bias(e, bt, nullptr, Co, &L.convT.bias, st));
-        MG_TRY(e->alloc(reinterpret_cast<void**>(&L.wuv), static_cast<size_t>(8) * Co * 4));
-        MG_TRY(launch_pack_convT_uv(wt->p, cin, Co, L.wuv, st));
-        MG_TRY(pack_conv3(e, pre + "0.1", Co, Co, "", 0, false, &L.conv, st));
-        for (int r = 0; r < c.num_res_blocks; ++r) {
-            const std::string rp = pre + std::to_string(1 + r) + ".layers.";
-            V1Res R;
-            MG_TRY(vec(e, rp + "0.weight", Co, &R.g1));
-            MG_TRY(vec(e, rp + "0.bias", Co, &R.b1));
-            MG_TRY(pack_conv3(e, rp + "2", Hd, Co, "", 0, false, &R.c1, st));
-            MG_TRY(vec(e, rp + "3.weight", Hd, &R.g2));
-            MG_TRY(vec(e, rp + "3.bias", Hd, &R.b2));
-            MG_TRY(pack_conv3(e, rp + "5", Co, Hd, "", 0, false, &R.c2, st));
-            R.G2 = c.hidden_norm == MOGE_V1_GROUP_NORM ? Hd / 32 : 1;
-            L.res.push_back(R);
-        }
-        cin = Co;
-    }
-    // V7: output blocks k = 0 (points, 3) and 1 (mask, 1): conv3x3 (cin + 2 -> 32), ReLU, conv1x1 (32 -> n_k)
-    const int lc = c.last_conv_channels, nout[2] = {3, 1};
-    std::vector<float> wcat(static_cast<size_t>(2) * lc * cin * 9), bcat(2 * lc), params(64 * 6 + 4 * 64 + 4, 0.f);
-    for (int k = 0; k < 2; ++k) {
-        const std::string ob = "head.output_block." + std::to_string(k) + ".";
-        const RawWeight *wc, *bc, *wo, *bo;
-        MG_TRY(get_raw(e, ob + "0.weight", &wc, {lc, cin + 2, 3, 3}));
-        MG_TRY(get_raw(e, ob + "0.bias", &bc, {lc}));
-        MG_TRY(get_raw(e, ob + "2.weight", &wo, {nout[k], lc, 1, 1}));
-        MG_TRY(get_raw(e, ob + "2.bias", &bo, {nout[k]}));
-        std::vector<float> hw, hb, hwo, hbo;
-        MG_TRY(to_host(wc, 0, wc->numel, &hw));
-        MG_TRY(to_host(bc, 0, bc->numel, &hb));
-        MG_TRY(to_host(wo, 0, wo->numel, &hwo));
-        MG_TRY(to_host(bo, 0, bo->numel, &hbo));
-        for (int co = 0; co < lc; ++co) {
-            const int n = k * lc + co;
-            const float* src = hw.data() + static_cast<size_t>(co) * (cin + 2) * 9;
-            std::copy(src, src + static_cast<size_t>(cin) * 9, wcat.begin() + static_cast<size_t>(n) * cin * 9);
-            bcat[n] = hb[co];
-            // UV part of the replicate-padded 3x3 conv: u depends on x only, v on y only -> six folded weights
-            const float* wu = src + static_cast<size_t>(cin) * 9;
-            const float* wv = wu + 9;
-            for (int d = 0; d < 3; ++d) {
-                params[n * 6 + d] = wu[0 * 3 + d] + wu[1 * 3 + d] + wu[2 * 3 + d];          // sum over dy, tap dx = d - 1
-                params[n * 6 + 3 + d] = wv[d * 3 + 0] + wv[d * 3 + 1] + wv[d * 3 + 2];      // sum over dx, tap dy = d - 1
-            }
-            for (int o = 0; o < nout[k]; ++o) params[64 * 6 + (k == 0 ? o : 3) * 64 + n] = hwo[static_cast<size_t>(o) * lc + co];
-        }
-        for (int o = 0; o < nout[k]; ++o) params[64 * 6 + 4 * 64 + (k == 0 ? o : 3)] = hbo[o];
-    }
-    MG_TRY(to_dev(e, params, &v.wout));
-    float* wcat_dev;
-    MG_TRY(e->alloc_temp(reinterpret_cast<void**>(&wcat_dev), wcat.size() * 4));
-    CUDA_TRY(cudaMemcpy(wcat_dev, wcat.data(), wcat.size() * 4, cudaMemcpyHostToDevice));
-    ConvW& oc = v.out;
-    oc.N = 2 * lc; oc.cin = cin; oc.taps = 9; oc.Ktot = 9 * cin;
-    MG_TRY(e->alloc(&oc.w, static_cast<size_t>(oc.N) * oc.Ktot * 2));
-    MG_TRY(launch_pack_conv(wcat_dev, oc.w, e->bf16, oc.N, cin, 9, oc.Ktot, 0, st));
-    MG_TRY(to_dev(e, bcat, &oc.bias));
-    return 0;
-}
-
-static int finalize(moge_engine* e, cudaStream_t st) {
-    MG_TRY(finalize_encoder(e, st));
-    MG_TRY(e->v1 ? finalize_v1(e, st) : finalize_v2_decoder(e, st));
-    CUDA_TRY(cudaStreamSynchronize(st));
-    for (void* t : e->temps) cudaFree(t);
-    e->temps.clear();
-    // release the fp32 staging copies of the big matrices (vectors stay: kernels read them directly)
-    for (auto& kv : e->raw) {
-        const bool keep = kv.second.shape.size() <= 1 || kv.first.find("pos_embed") != std::string::npos ||
-                          kv.first.find("cls_token") != std::string::npos || kv.first.rfind("scale_head.", 0) == 0;
-        if (!keep && kv.second.p) { cudaFree(kv.second.p); kv.second.p = nullptr; }
-    }
-    e->finalized = true;
-    return 0;
-}
 
 // ------------------------------------------------------------------------------------------------ planning
 struct WsAlloc {
@@ -1232,6 +683,8 @@ static int validate_v1(const moge_v1_config_t& c) {
 
 }  // namespace mg
 
+using namespace mg;
+
 // ================================================================================================ C ABI
 extern "C" {
 
@@ -1287,34 +740,8 @@ void moge_engine_destroy(moge_engine_t* e) {
     if (e->ev_in) cudaEventDestroy(e->ev_in);
     if (e->ev_out) cudaEventDestroy(e->ev_out);
     for (void* p : e->owned) cudaFree(p);
-    for (void* p : e->temps) cudaFree(p);
     for (auto& kv : e->raw) if (kv.second.p) cudaFree(kv.second.p);
     delete e;
-}
-
-int moge_engine_set_weight(moge_engine_t* e, const char* key, const void* dev_ptr, const int64_t* shape, int ndim, int dtype, void* stream) {
-    if (!e || !key || !dev_ptr) return set_error("null argument");
-    if (e->finalized) return set_error("engine already finalized");
-    if (dtype != MOGE_F32 && dtype != MOGE_F16 && dtype != MOGE_BF16) return set_error("weight '%s': unsupported dtype %d", key, dtype);
-    CUDA_TRY(cudaSetDevice(e->device));
-    RawWeight rw;
-    rw.numel = 1;
-    for (int i = 0; i < ndim; ++i) { rw.shape.push_back(shape[i]); rw.numel *= static_cast<size_t>(shape[i]); }
-    CUDA_TRY(cudaMalloc(reinterpret_cast<void**>(&rw.p), std::max<size_t>(rw.numel, 4) * 4));
-    const int blocks = static_cast<int>(std::min<size_t>((rw.numel + 255) / 256, 132 * 8));
-    to_f32_kernel<<<std::max(blocks, 1), 256, 0, static_cast<cudaStream_t>(stream)>>>(dev_ptr, dtype, rw.p, rw.numel);
-    CUDA_TRY(cudaGetLastError());
-    auto it = e->raw.find(key);
-    if (it != e->raw.end() && it->second.p) cudaFree(it->second.p);
-    e->raw[key] = rw;
-    return 0;
-}
-
-int moge_engine_finalize(moge_engine_t* e, void* stream) {
-    if (!e) return set_error("null engine");
-    if (e->finalized) return 0;
-    CUDA_TRY(cudaSetDevice(e->device));
-    return finalize(e, static_cast<cudaStream_t>(stream));
 }
 
 static int check_groups(moge_engine_t* e, const moge_group_t* g, int n, bool need_ptrs) {
