@@ -232,6 +232,21 @@ int moge_v1_workspace_bytes(moge_engine_t* e, int B, int H, int W, int rh, int r
  * output (no sigmoid), both fp32 */
 int moge_v1_forward(moge_engine_t* e, const void* image, int image_dtype, int B, int H, int W, int rh, int rw, void* workspace,
                     size_t workspace_bytes, float* points, float* mask, void* stream);
+/* Mixed-shape MoGe-1 batches, as moge_engine_forward_groups for MoGe-2: a call carries `n` (1..64) shape groups; the encoder runs
+ * ONCE over the token rows of all groups packed back to back, the resize, decoder and output resize run group by group through
+ * one set of decoder maps sized for the largest group.  Each group is checked as moge_v1_forward checks its arguments, before
+ * anything runs.  moge_v1_workspace_bytes / moge_v1_forward are the n = 1 case.  Python: MoGeModel.infer_many (moge.model.v1). */
+typedef struct moge_v1_group {
+    const void* image;          /* (B,3,H,W) in [0,1] */
+    int image_dtype;            /* MOGE_F32 / MOGE_F16 / MOGE_BF16 */
+    int B, H, W;                /* images and pixels of this group */
+    int rh, rw;                 /* its resized image (>= 14 each); token grid rh/14 x rw/14 */
+    float* points;              /* (B,H,W,3) */
+    float* mask;                /* (B,H,W), the raw mask output */
+} moge_v1_group_t;
+int moge_v1_workspace_bytes_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, size_t* bytes);
+int moge_v1_forward_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, void* workspace, size_t workspace_bytes,
+                           void* stream);
 /* the fp32 part of MoGeModel.infer (v1.py:352-380): mask_out = mask > mask_threshold (u8), focal/shift recovery (focal_in NULL:
  * solve both), intrinsics (B,3,3), depth = z + shift, points re-projected (force_projection) or shifted in z, points and depth
  * +inf outside the mask (apply_mask).  points updated in place; focal, shift (B,) outputs. */

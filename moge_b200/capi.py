@@ -72,6 +72,15 @@ class Group(C.Structure):
     ]
 
 
+class V1Group(C.Structure):
+    """moge_v1_group_t: one shape group of a mixed-shape MoGe-1 forward call."""
+    _fields_ = [
+        ("image", C.c_void_p), ("image_dtype", C.c_int),
+        ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("rh", C.c_int), ("rw", C.c_int),
+        ("points", C.c_void_p), ("mask", C.c_void_p),
+    ]
+
+
 class MetricVariant(C.Structure):
     """moge_metric_variant_t: a prediction map and its per-image (batch, 4) params on the device."""
     _fields_ = [("kind", C.c_int), ("src", C.c_void_p), ("params", C.c_void_p)]
@@ -136,6 +145,8 @@ SIGNATURES = {
     "moge_engine_create_v1": [C.POINTER(V1Config), ci, C.POINTER(vp)],
     "moge_v1_workspace_bytes": [vp, ci, ci, ci, ci, ci, C.POINTER(sz)],
     "moge_v1_forward": [vp, vp, ci, ci, ci, ci, ci, ci, vp, sz, vp, vp, vp],
+    "moge_v1_workspace_bytes_groups": [vp, C.POINTER(V1Group), ci, C.POINTER(sz)],
+    "moge_v1_forward_groups": [vp, C.POINTER(V1Group), ci, vp, sz, vp],
     "moge_v1_postprocess": [vp, vp, C.c_float, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp],
     "moge_op_resize_bicubic_aa": [vp, ci, ci, ci, ci, ci, ci, ci, vp, vp],
     "moge_op_groupnorm_relu": [vp, vp, vp, vp, ci, ci, ci, ci, ci, ci, vp],

@@ -201,7 +201,7 @@ static int plan_stack(moge_engine* e, Plan* pl, const StackIn& in, void** neck_o
     return 0;
 }
 
-// ---- MoGe-1 decoder (one shape group): workspace maps and launch list
+// ---- MoGe-1 decoder: the groups run one after the other through ONE set of maps sized for the largest group
 struct V1Bufs {
     float *rs_tmp = nullptr, *rs_img = nullptr;     // bicubic row pass (B,3,H,rw), resized image (B,3,rh,rw)
     void* x0 = nullptr;                             // projected taps, level 0
@@ -210,113 +210,143 @@ struct V1Bufs {
     double2* gn_part = nullptr;
     float2* gn_stats = nullptr;
     void *full = nullptr, *fout = nullptr;          // last map resized to (rh, rw); the output conv's 64 channels there
-    float4* pts = nullptr;                          // (rh, rw) points before the resize to (H, W)
-    float* msk = nullptr;
+    std::vector<float4*> pts;                       // per group: (rh, rw) points before the resize to (H, W)
+    std::vector<float*> msk;                        // per group: (rh, rw) mask logits
 };
 
 static Level full_geom(int rh, int rw) { return Level{rh, rw, std::max(rh + 2, TILE_PH), std::max(rw + 2, TILE_PW)}; }
 
-static void v1_alloc(moge_engine* e, const Group& g, WsAlloc& ws, V1Bufs* vb) {
+static void v1_alloc(moge_engine* e, const Plan* pl, WsAlloc& ws, V1Bufs* vb) {
     const moge_v1_config_t& c = e->v1cfg;
-    const int B = g.B;
-    vb->rs_tmp = static_cast<float*>(ws.take(static_cast<size_t>(B) * 3 * g.H * g.rw * 4));
-    vb->rs_img = static_cast<float*>(ws.take(static_cast<size_t>(B) * 3 * g.rh * g.rw * 4));
-    vb->x0 = ws.take(map_bytes(level_geom(g.h, g.w, 0), B, c.dim_proj));
-    size_t part = 0, stats = 0;
-    vb->lv.resize(c.num_levels);
-    for (int l = 0; l < c.num_levels; ++l) {
-        const Level go = level_geom(g.h, g.w, l + 1);
+    const int L = c.num_levels;
+    // the largest size any group needs, of each map
+    auto most = [&](const std::function<size_t(const Group&)>& f) {
+        size_t m = 0;
+        for (const Group& g : pl->groups) m = std::max(m, f(g));
+        return m;
+    };
+    // one resize scratch for every group: the phase-0 resize -> preprocess pairs are issued group by group on one stream, so a
+    // group's resize only overwrites the scratch after the previous group's preprocess has read it
+    vb->rs_tmp = static_cast<float*>(ws.take(most([](const Group& g) { return static_cast<size_t>(g.B) * 3 * g.H * g.rw * 4; })));
+    vb->rs_img = static_cast<float*>(ws.take(most([](const Group& g) { return static_cast<size_t>(g.B) * 3 * g.rh * g.rw * 4; })));
+    vb->x0 = ws.take(most([&](const Group& g) { return map_bytes(level_geom(g.h, g.w, 0), g.B, c.dim_proj); }));
+    vb->lv.resize(L);
+    for (int l = 0; l < L; ++l) {
         const int Co = c.dim_upsample[l], Hd = c.hidden_mult * Co;
-        const int G2 = c.hidden_norm == MOGE_V1_GROUP_NORM ? Hd / 32 : 1;
-        V1Bufs::Lv& L = vb->lv[l];
-        L.m0 = ws.take(map_bytes(go, B, Co));
-        L.m1 = ws.take(map_bytes(go, B, Co));
-        L.relu = ws.take(map_bytes(go, B, Co));
-        L.hraw = ws.take(map_bytes(go, B, Hd));
-        L.hrelu = ws.take(map_bytes(go, B, Hd));
-        part = std::max({part, static_cast<size_t>(B) * gn_tiles(go.H, go.W, Co), static_cast<size_t>(B) * gn_tiles(go.H, go.W, Hd) * G2});
-        stats = std::max(stats, static_cast<size_t>(B) * G2);
+        auto bytes = [&](int C) { return most([&](const Group& g) { return map_bytes(level_geom(g.h, g.w, l + 1), g.B, C); }); };
+        V1Bufs::Lv& m = vb->lv[l];
+        m.m0 = ws.take(bytes(Co));
+        m.m1 = ws.take(bytes(Co));
+        m.relu = ws.take(bytes(Co));
+        m.hraw = ws.take(bytes(Hd));
+        m.hrelu = ws.take(bytes(Hd));
     }
+    const size_t part = most([&](const Group& g) {
+        size_t p = 0;
+        for (int l = 0; l < L; ++l) {
+            const Level go = level_geom(g.h, g.w, l + 1);
+            const int Co = c.dim_upsample[l], Hd = c.hidden_mult * Co;
+            const int G2 = c.hidden_norm == MOGE_V1_GROUP_NORM ? Hd / 32 : 1;
+            p = std::max({p, static_cast<size_t>(g.B) * gn_tiles(go.H, go.W, Co), static_cast<size_t>(g.B) * gn_tiles(go.H, go.W, Hd) * G2});
+        }
+        return p;
+    });
+    const size_t stats = most([&](const Group& g) {
+        size_t s = 0;
+        for (int l = 0; l < L; ++l) {
+            const int Hd = c.hidden_mult * c.dim_upsample[l];
+            s = std::max(s, static_cast<size_t>(g.B) * (c.hidden_norm == MOGE_V1_GROUP_NORM ? Hd / 32 : 1));
+        }
+        return s;
+    });
     vb->gn_part = static_cast<double2*>(ws.take(part * 16));
     vb->gn_stats = static_cast<float2*>(ws.take(stats * 8));
-    const Level gr = full_geom(g.rh, g.rw);
-    vb->full = ws.take(map_bytes(gr, B, c.dim_upsample[c.num_levels - 1]));
-    vb->fout = ws.take(map_bytes(gr, B, 2 * c.last_conv_channels));
-    vb->pts = static_cast<float4*>(ws.take(static_cast<size_t>(B) * g.rh * g.rw * 16));
-    vb->msk = static_cast<float*>(ws.take(static_cast<size_t>(B) * g.rh * g.rw * 4));
+    vb->full = ws.take(most([&](const Group& g) { return map_bytes(full_geom(g.rh, g.rw), g.B, c.dim_upsample[L - 1]); }));
+    vb->fout = ws.take(most([&](const Group& g) { return map_bytes(full_geom(g.rh, g.rw), g.B, 2 * c.last_conv_channels); }));
+    // per group: the phase-2 output resizes read them after every group's decoder has run
+    for (const Group& g : pl->groups) {
+        vb->pts.push_back(static_cast<float4*>(ws.take(static_cast<size_t>(g.B) * g.rh * g.rw * 16)));
+        vb->msk.push_back(static_cast<float*>(ws.take(static_cast<size_t>(g.B) * g.rh * g.rw * 4)));
+    }
 }
 
-static int plan_v1_decoder(moge_engine* e, Plan* pl, const void* taps, const V1Bufs& vb) {
+// MoGe-1 decoder launch list, group by group; group gi's encoder taps start at row prow0[gi] of `taps`.
+static int plan_v1_decoder(moge_engine* e, Plan* pl, const uint8_t* taps, const std::vector<long>& prow0, const V1Bufs& vb) {
     const moge_v1_config_t& c = e->v1cfg;
     const V1W& v = e->v1w;
-    const Group& g = pl->groups[0];
-    const int B = g.B, H = g.H, W = g.W, h = g.h, w = g.w, rh = g.rh, rw = g.rw;
+    const int G = static_cast<int>(pl->groups.size());
     const bool bf16 = e->bf16;
-    // every UV plane of the head has the aspect of the resized image (v1.py:125, 133)
-    const float aspect = static_cast<float>(rw) / rh;
-    const float su = aspect / sqrtf(1.f + aspect * aspect), sv = 1.f / sqrtf(1.f + aspect * aspect);
-    const Level g0 = level_geom(h, w, 0);
-    LinearArgs proj; proj.A = taps; proj.M = B * h * w; proj.K = v.proj.Ktot; proj.W = v.proj.w; proj.N = v.proj.N; proj.epi = EPI_DEC;
-    proj.out = vb.x0; proj.bias = v.proj.bias; proj.grid = &g0;
-    MG_TRY(add_linear(e, pl, proj, "gemm.projects"));
-    const void* x = vb.x0;
-    double2* part = vb.gn_part;
-    float2* stats = vb.gn_stats;
-    auto nm = [](const char* kind, int l) { return std::string(kind) + ".l" + std::to_string(l); };
-    auto add_gn = [&](const void* src, void* dst, const Level& gl, int C, int G, const float* gamma, const float* beta, int l) {
-        const double px = static_cast<double>(B) * gl.H * gl.W;
-        pl->ops.add([=](cudaStream_t st) { return launch_gn_stats(src, gl, B, C, G, part, stats, bf16, st); }, nm("groupnorm_stats", l), 0, px * C * 2);
-        pl->ops.add([=](cudaStream_t st) { return launch_gn_relu(src, dst, gl, B, C, G, stats, gamma, beta, bf16, st); }, nm("groupnorm_relu", l), 0,
-                    px * C * 4);
-    };
-    for (int l = 0; l < c.num_levels; ++l) {
-        const V1Level& L = v.lv[l];
-        const V1Bufs::Lv& m = vb.lv[l];
-        const int Co = c.dim_upsample[l], Hd = c.hidden_mult * Co;
-        const Level gi = level_geom(h, w, l), go = level_geom(h, w, l + 1);
-        ConvArgs lv; lv.B = B; lv.gs = lv.go = go; lv.out_ch = Co; lv.epi = EPI_DEC;        // the level's convs on its output grid
-        ConvArgs ct = lv; ct.cw = L.convT; ct.src = x; ct.gs = gi; ct.out_raw = m.m1; ct.shuffle = true;
-        MG_TRY(add_conv(e, pl, ct, nm("convT", l)));
-        const float* wuv = L.wuv;
-        void* t = m.m1;
-        pl->ops.add([=](cudaStream_t st) { return launch_uv_convT(t, go, B, Co, wuv, su, sv, bf16, st); }, nm("uv_convT", l), 0,
-                    static_cast<double>(B) * go.H * go.W * Co * 4);
-        ConvArgs cv = lv; cv.cw = L.conv; cv.src = m.m1; cv.out_raw = m.m0;
-        MG_TRY(add_conv(e, pl, cv, nm("conv3x3", l)));
-        void* xr = m.m0;
-        void* other = m.m1;
-        for (const V1Res& R : L.res) {
-            add_gn(xr, m.relu, go, Co, 1, R.g1, R.b1, l);
-            ConvArgs ra = lv; ra.cw = R.c1; ra.src = m.relu; ra.out_ch = Hd; ra.out_raw = m.hraw;
-            MG_TRY(add_conv(e, pl, ra, nm("conv3x3.res_a", l)));
-            add_gn(m.hraw, m.hrelu, go, Hd, R.G2, R.g2, R.b2, l);
-            ConvArgs rb = lv; rb.cw = R.c2; rb.src = m.hrelu; rb.out_raw = other; rb.skip = xr;
-            MG_TRY(add_conv(e, pl, rb, nm("conv3x3.res_b", l)));
-            std::swap(xr, other);
-        }
-        x = xr;
-    }
-    // V7: bilinear resize to the resized-image grid, both output blocks' 3x3 conv, then their UV part, ReLU and 1x1 convs
-    const int Cl = c.dim_upsample[c.num_levels - 1];
-    const Level gl = level_geom(h, w, c.num_levels), gr = full_geom(rh, rw);
-    const double pxr = static_cast<double>(B) * rh * rw;
-    void* full = vb.full;
-    pl->ops.add([=](cudaStream_t st) { return launch_resize_bilinear_nhwc(x, gl, full, gr, B, Cl, bf16, st); }, "resize_bilinear", 0,
-                static_cast<double>(B) * gl.H * gl.W * Cl * 2 + pxr * Cl * 2);
-    ConvArgs oc; oc.cw = v.out; oc.src = vb.full; oc.gs = oc.go = gr; oc.B = B; oc.out_ch = v.out.N; oc.epi = EPI_DEC; oc.out_raw = vb.fout;
-    MG_TRY(add_conv(e, pl, oc, "conv3x3.output"));
-    const void* fout = vb.fout;
-    const float* wout = v.wout;
-    float4* pts = vb.pts;
-    float* msk = vb.msk;
-    pl->ops.add([=](cudaStream_t st) { return launch_v1_output(fout, gr, B, wout, su, sv, pts, msk, bf16, st); }, "output_block", 2.0 * pxr * 64 * 10,
-                pxr * (64 * 2 + 20));
-    // V8 (phase 2: the caller's outputs): bilinear resize to (H, W), remap; the mask stays a raw logit
-    const int remap = c.remap_output;
     Plan* P = pl;
-    pl->ops.add([=](cudaStream_t st) {
-        return launch_head_output(pts, nullptr, msk, B, rh, rw, H, W, remap, P->groups[0].points, nullptr, P->groups[0].mask, st, false);
-    }, "head_output", 0, static_cast<double>(B) * H * W * 16 + pxr * 20, 2);
+    for (int gi = 0; gi < G; ++gi) {
+        const Group& g = pl->groups[gi];
+        const int B = g.B, H = g.H, W = g.W, h = g.h, w = g.w, rh = g.rh, rw = g.rw;
+        const std::string sfx = G == 1 ? std::string() : ".g" + std::to_string(gi);
+        // every UV plane of the head has the aspect of the resized image (v1.py:125, 133)
+        const float aspect = static_cast<float>(rw) / rh;
+        const float su = aspect / sqrtf(1.f + aspect * aspect), sv = 1.f / sqrtf(1.f + aspect * aspect);
+        const Level g0 = level_geom(h, w, 0);
+        LinearArgs proj; proj.A = taps + static_cast<size_t>(prow0[gi]) * e->cfg.num_taps * e->cfg.embed_dim * 2; proj.M = B * h * w; proj.K = v.proj.Ktot;
+        proj.W = v.proj.w; proj.N = v.proj.N; proj.epi = EPI_DEC; proj.out = vb.x0; proj.bias = v.proj.bias; proj.grid = &g0;
+        MG_TRY(add_linear(e, pl, proj, "gemm.projects" + sfx));
+        const void* x = vb.x0;
+        double2* part = vb.gn_part;
+        float2* stats = vb.gn_stats;
+        auto nm = [&](const char* kind, int l) { return std::string(kind) + sfx + ".l" + std::to_string(l); };
+        auto add_gn = [&](const void* src, void* dst, const Level& gl, int C, int G2, const float* gamma, const float* beta, int l) {
+            const double px = static_cast<double>(B) * gl.H * gl.W;
+            pl->ops.add([=](cudaStream_t st) { return launch_gn_stats(src, gl, B, C, G2, part, stats, bf16, st); }, nm("groupnorm_stats", l), 0,
+                        px * C * 2);
+            pl->ops.add([=](cudaStream_t st) { return launch_gn_relu(src, dst, gl, B, C, G2, stats, gamma, beta, bf16, st); }, nm("groupnorm_relu", l), 0,
+                        px * C * 4);
+        };
+        for (int l = 0; l < c.num_levels; ++l) {
+            const V1Level& L = v.lv[l];
+            const V1Bufs::Lv& m = vb.lv[l];
+            const int Co = c.dim_upsample[l], Hd = c.hidden_mult * Co;
+            const Level gin = level_geom(h, w, l), go = level_geom(h, w, l + 1);
+            ConvArgs lv; lv.B = B; lv.gs = lv.go = go; lv.out_ch = Co; lv.epi = EPI_DEC;        // the level's convs on its output grid
+            ConvArgs ct = lv; ct.cw = L.convT; ct.src = x; ct.gs = gin; ct.out_raw = m.m1; ct.shuffle = true;
+            MG_TRY(add_conv(e, pl, ct, nm("convT", l)));
+            const float* wuv = L.wuv;
+            void* t = m.m1;
+            pl->ops.add([=](cudaStream_t st) { return launch_uv_convT(t, go, B, Co, wuv, su, sv, bf16, st); }, nm("uv_convT", l), 0,
+                        static_cast<double>(B) * go.H * go.W * Co * 4);
+            ConvArgs cv = lv; cv.cw = L.conv; cv.src = m.m1; cv.out_raw = m.m0;
+            MG_TRY(add_conv(e, pl, cv, nm("conv3x3", l)));
+            void* xr = m.m0;
+            void* other = m.m1;
+            for (const V1Res& R : L.res) {
+                add_gn(xr, m.relu, go, Co, 1, R.g1, R.b1, l);
+                ConvArgs ra = lv; ra.cw = R.c1; ra.src = m.relu; ra.out_ch = Hd; ra.out_raw = m.hraw;
+                MG_TRY(add_conv(e, pl, ra, nm("conv3x3.res_a", l)));
+                add_gn(m.hraw, m.hrelu, go, Hd, R.G2, R.g2, R.b2, l);
+                ConvArgs rb = lv; rb.cw = R.c2; rb.src = m.hrelu; rb.out_raw = other; rb.skip = xr;
+                MG_TRY(add_conv(e, pl, rb, nm("conv3x3.res_b", l)));
+                std::swap(xr, other);
+            }
+            x = xr;
+        }
+        // V7: bilinear resize to the resized-image grid, both output blocks' 3x3 conv, then their UV part, ReLU and 1x1 convs
+        const int Cl = c.dim_upsample[c.num_levels - 1];
+        const Level gl = level_geom(h, w, c.num_levels), gr = full_geom(rh, rw);
+        const double pxr = static_cast<double>(B) * rh * rw;
+        void* full = vb.full;
+        pl->ops.add([=](cudaStream_t st) { return launch_resize_bilinear_nhwc(x, gl, full, gr, B, Cl, bf16, st); }, "resize_bilinear" + sfx, 0,
+                    static_cast<double>(B) * gl.H * gl.W * Cl * 2 + pxr * Cl * 2);
+        ConvArgs oc; oc.cw = v.out; oc.src = vb.full; oc.gs = oc.go = gr; oc.B = B; oc.out_ch = v.out.N; oc.epi = EPI_DEC; oc.out_raw = vb.fout;
+        MG_TRY(add_conv(e, pl, oc, "conv3x3.output" + sfx));
+        const void* fout = vb.fout;
+        const float* wout = v.wout;
+        float4* pts = vb.pts[gi];
+        float* msk = vb.msk[gi];
+        pl->ops.add([=](cudaStream_t st) { return launch_v1_output(fout, gr, B, wout, su, sv, pts, msk, bf16, st); }, "output_block" + sfx,
+                    2.0 * pxr * 64 * 10, pxr * (64 * 2 + 20));
+        // V8 (phase 2: the caller's outputs): bilinear resize to (H, W), remap; the mask stays a raw logit
+        const int remap = c.remap_output;
+        pl->ops.add([=](cudaStream_t st) {
+            return launch_head_output(pts, nullptr, msk, B, rh, rw, H, W, remap, P->groups[gi].points, nullptr, P->groups[gi].mask, st, false);
+        }, "head_output" + sfx, 0, static_cast<double>(B) * H * W * 16 + pxr * 20, 2);
+    }
     return 0;
 }
 
@@ -472,7 +502,7 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     // ---- decoder buffers: MoGe-1 or MoGe-2 (the encoder above is shared)
     V1Bufs vb;
     V2Bufs v2b;
-    if (e->v1) v1_alloc(e, pl->groups[0], ws, &vb);
+    if (e->v1) v1_alloc(e, pl, ws, &vb);
     else alloc_v2_decoder(e, pl, ws, &v2b);
     if (bytes_out) *bytes_out = ws.off + 1024;
     if (dry) return 0;
@@ -497,9 +527,9 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
             const int rh = g.rh, rw = g.rw;
             float *tmp = vb.rs_tmp, *img = vb.rs_img;
             pl->ops.add([=](cudaStream_t st) { return launch_resize_bicubic_aa(P->groups[gi].image, P->groups[gi].image_dtype, B, 3, H, W, rh, rw, tmp, img, st); },
-                        "resize_bicubic_aa", 0, static_cast<double>(B) * 3 * (static_cast<double>(H) * W * 4 + static_cast<double>(H) * rw * 8 + static_cast<double>(rh) * rw * 4), 0);
+                        gname("resize_bicubic_aa", gi), 0, static_cast<double>(B) * 3 * (static_cast<double>(H) * W * 4 + static_cast<double>(H) * rw * 8 + static_cast<double>(rh) * rw * 4), 0);
             pl->ops.add([=](cudaStream_t st) { return launch_preprocess(img, MOGE_F32, B, rh, rw, h, w, patches_g, 592, bf16, st); },
-                        "preprocess", 0, static_cast<double>(B) * 3 * rh * rw * 4 + static_cast<double>(B) * T * 592 * 2, 0);
+                        gname("preprocess", gi), 0, static_cast<double>(B) * 3 * rh * rw * 4 + static_cast<double>(B) * T * 592 * 2, 0);
             prow += static_cast<long>(B) * T;
             continue;
         }
@@ -582,7 +612,7 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         }
     }
     if (tap_idx != c.num_taps) return set_error("intermediate_layers must be increasing block indices < depth");
-    MG_TRY(e->v1 ? plan_v1_decoder(e, pl, taps, vb) : plan_v2_decoder(e, pl, taps, prow0, cls, mlp_scratch, v2b));
+    MG_TRY(e->v1 ? plan_v1_decoder(e, pl, taps, prow0, vb) : plan_v2_decoder(e, pl, taps, prow0, cls, mlp_scratch, v2b));
     // launch order: phase 0, 1, 2 (stable)
     std::stable_sort(pl->ops.begin(), pl->ops.end(), [](const Op& a, const Op& b) { return a.phase < b.phase; });
     return 0;
@@ -861,25 +891,52 @@ static int check_v1_shape(moge_engine_t* e, int B, int H, int W, int rh, int rw)
     return 0;
 }
 
-int moge_v1_workspace_bytes(moge_engine_t* e, int B, int H, int W, int rh, int rw, size_t* bytes) {
+// The MoGe-1 groups as moge_group_t (token grid rh/14 x rw/14) and as plan groups, after the per-group checks; `outputs`: the
+// points and mask pointers are checked too (a forward)
+static int v1_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, bool outputs, std::vector<moge_group_t>* mg,
+                     std::vector<Group>* gs) {
+    if (n <= 0 || n > 64) return set_error("number of shape groups %d out of range (1..64)", n);
+    if (!groups) return set_error("null argument");
+    for (int i = 0; i < n; ++i) {
+        const moge_v1_group_t& v = groups[i];
+        MG_TRY(check_v1_shape(e, v.B, v.H, v.W, v.rh, v.rw));
+        if (outputs && (!v.points || !v.mask)) return set_error("null argument");
+        moge_group_t g{};
+        g.image = v.image; g.image_dtype = v.image_dtype; g.B = v.B; g.H = v.H; g.W = v.W; g.h = v.rh / 14; g.w = v.rw / 14;
+        g.points = v.points; g.mask_prob = v.mask;
+        mg->push_back(g);
+        gs->push_back(make_group(g, v.rh, v.rw));
+    }
+    return 0;
+}
+
+int moge_v1_workspace_bytes_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, size_t* bytes) {
     if (!bytes) return set_error("null argument");
-    MG_TRY(check_v1_shape(e, B, H, W, rh, rw));
-    moge_group_t g{};
-    g.B = B; g.H = H; g.W = W; g.h = rh / 14; g.w = rw / 14;
+    std::vector<moge_group_t> mg;
     Plan pl;
-    pl.groups.push_back(make_group(g, rh, rw));
+    MG_TRY(v1_groups(e, groups, n, false, &mg, &pl.groups));
     return build_plan(e, &pl, true, bytes);
+}
+
+int moge_v1_forward_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream) {
+    std::vector<moge_group_t> mg;
+    std::vector<Group> gs;
+    MG_TRY(v1_groups(e, groups, n, true, &mg, &gs));
+    MG_TRY(check_forward(e, mg.data(), n, workspace));
+    return forward_impl(e, gs, workspace, workspace_bytes, stream);
+}
+
+int moge_v1_workspace_bytes(moge_engine_t* e, int B, int H, int W, int rh, int rw, size_t* bytes) {
+    moge_v1_group_t g{};
+    g.B = B; g.H = H; g.W = W; g.rh = rh; g.rw = rw;
+    return moge_v1_workspace_bytes_groups(e, &g, 1, bytes);
 }
 
 int moge_v1_forward(moge_engine_t* e, const void* image, int image_dtype, int B, int H, int W, int rh, int rw, void* workspace,
                     size_t workspace_bytes, float* points, float* mask, void* stream) {
-    MG_TRY(check_v1_shape(e, B, H, W, rh, rw));
-    if (!points || !mask) return set_error("null argument");
-    moge_group_t g{};
-    g.image = image; g.image_dtype = image_dtype; g.B = B; g.H = H; g.W = W; g.h = rh / 14; g.w = rw / 14;
-    g.points = points; g.mask_prob = mask;
-    MG_TRY(check_forward(e, &g, 1, workspace));
-    return forward_impl(e, {make_group(g, rh, rw)}, workspace, workspace_bytes, stream);
+    moge_v1_group_t g{};
+    g.image = image; g.image_dtype = image_dtype; g.B = B; g.H = H; g.W = W; g.rh = rh; g.rw = rw; g.points = points; g.mask = mask;
+    return moge_v1_forward_groups(e, &g, 1, workspace, workspace_bytes, stream);
 }
 
 int moge_v1_postprocess(float* points, const float* mask, float mask_threshold, const float* focal_in, int B, int H, int W,

@@ -1,12 +1,12 @@
 """Host plumbing shared by the drop-in MoGe-2 and MoGe-1 models (v2.py, v1.py): the nn.Module-like surface, checkpoint
-loading, the engine handle with its weight upload, the activation workspace and the batch chunking.
+loading, the engine handle with its weight upload, the activation workspace, the batch chunking and the mixed-shape packing.
 Host logic only: every arithmetic step runs in the C-ABI library.
 """
 from __future__ import annotations
 
 import ctypes as C
 from pathlib import Path
-from typing import IO, Any, Dict, List, Optional, Tuple, Union
+from typing import IO, Any, Callable, Dict, List, Optional, Tuple, Union
 
 import torch
 
@@ -189,6 +189,34 @@ class EngineModel:
         ~ 21 GB)."""
         chunk = max(1, min(B, self.max_chunk_tokens // tokens_per_image))
         return [(lo, min(chunk, B - lo)) for lo in range(0, B, chunk)]
+
+    def _pack_calls(self, images, geometry: Callable[[int, int], Tuple[Tuple[int, int], int]]) -> List[List[tuple]]:
+        """The engine calls of `infer_many` over `images` (each (3, H, W)), as lists of units (H, W, geom, indices).  Images are
+        bucketed by shape and dtype; `geometry(H, W)` gives a bucket's (geom, token rows per image), geom being what the model's
+        engine call takes per group.  Each bucket is chunked like a batch (`_chunks`), and the chunks are packed largest first into
+        calls of at most `max_chunk_tokens` tokens (a unit larger than that is a call of its own).  Raises ValueError, before
+        anything touches a device, on an element that is not (3, H, W)."""
+        buckets: Dict[tuple, List[int]] = {}
+        for i, im in enumerate(images):
+            if im.dim() != 3 or im.shape[0] != 3:
+                raise ValueError(f"images[{i}] must be (3, H, W), got {tuple(im.shape)}")
+            buckets.setdefault((int(im.shape[1]), int(im.shape[2]), im.dtype), []).append(i)
+        units = []
+        for (H, W, _), idx in buckets.items():
+            geom, tokens = geometry(H, W)
+            for lo, n in self._chunks(len(idx), tokens):
+                units.append((n * tokens, (H, W, geom, idx[lo:lo + n])))
+        units.sort(key=lambda u: -u[0])
+        calls, cur, cur_tok = [], [], 0
+        for tok, unit in units:
+            if cur and cur_tok + tok > self.max_chunk_tokens:
+                calls.append(cur)
+                cur, cur_tok = [], 0
+            cur.append(unit)
+            cur_tok += tok
+        if cur:
+            calls.append(cur)
+        return calls
 
     def _engine_input(self, image: torch.Tensor) -> torch.Tensor:
         """`image` as the engine reads it: on the model's device, fp32 / fp16 / bf16, contiguous."""

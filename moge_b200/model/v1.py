@@ -4,7 +4,8 @@ Mirrors the public surface of /root/reference/moge/model/v1.py:
   __init__ kwargs incl. mask_threshold and the `trained_area_range` conversion (v1.py:149-172), from_pretrained with a strict
   load (v1.py:214-242), .to/.half/.bfloat16, .device/.dtype, forward(image, num_tokens) -> {'points', 'mask'} (v1.py:269-299),
   infer(image, fov_x, resolution_level, num_tokens, apply_mask, force_projection, use_fp16)
-      -> {'points', 'intrinsics', 'depth', 'mask'} (v1.py:301-392).
+      -> {'points', 'intrinsics', 'depth', 'mask'} (v1.py:301-392),
+and, with no reference counterpart, infer_many(images, ...) over a list of images of different sizes (one encoder pass per call).
 Host logic only: tensor allocation and checkpoint I/O use PyTorch, every arithmetic step runs in the C-ABI library.
 """
 from __future__ import annotations
@@ -12,7 +13,7 @@ from __future__ import annotations
 import ctypes as C
 import warnings
 from numbers import Number
-from typing import Dict, List, Tuple, Union
+from typing import Dict, List, Optional, Tuple, Union
 
 import torch
 
@@ -98,6 +99,49 @@ class MoGeModel(EngineModel):
                     points[lo:lo + n].data_ptr(), mask[lo:lo + n].data_ptr(), capi.current_stream()))
         return points, mask
 
+    def _forward_groups(self, groups):
+        """ONE engine call over several shape groups: `groups` = [(image (B,3,H,W), rh, rw)].  The encoder runs once over the
+        packed token rows of all groups (moge_v1_forward_groups).  Returns [(points, raw mask)], fp32, per group."""
+        self._ensure_engine()
+        n = len(groups)
+        arr = (capi.V1Group * n)()
+        keep, outs = [], []
+        dev = self._device
+        with torch.cuda.device(dev):
+            for i, (image, rh, rw) in enumerate(groups):
+                image = self._engine_input(image)
+                B, _, H, W = image.shape
+                points = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev)
+                mask = torch.empty(B, H, W, dtype=torch.float32, device=dev)
+                g = arr[i]
+                g.image, g.image_dtype = image.data_ptr(), capi.torch_dtype_code(image.dtype)
+                g.B, g.H, g.W, g.rh, g.rw = B, H, W, rh, rw
+                g.points, g.mask = points.data_ptr(), mask.data_ptr()
+                keep.append(image)
+                outs.append((points, mask))
+            nbytes = C.c_size_t()
+            capi.check(capi.lib().moge_v1_workspace_bytes_groups(self._engine, arr, n, C.byref(nbytes)))
+            ws, ws_bytes = self._workspace_for(nbytes.value)
+            capi.check(capi.lib().moge_v1_forward_groups(self._engine, arr, n, ws, ws_bytes, capi.current_stream()))
+        return outs
+
+    def _postprocess(self, points, mask, aspect_ratio, fov_x, apply_mask, force_projection) -> Dict[str, torch.Tensor]:
+        """The fp32 part of infer() (v1.py:352-380) on the raw forward outputs of one shape group; all on the device."""
+        B, H, W = mask.shape
+        dev = self._device
+        with torch.cuda.device(dev):
+            focal_in = self._focal_in(fov_x, aspect_ratio, B)
+            focal = torch.empty(B, dtype=torch.float32, device=dev)
+            shift = torch.empty(B, dtype=torch.float32, device=dev)
+            depth = torch.empty(B, H, W, dtype=torch.float32, device=dev)
+            mask_out = torch.empty(B, H, W, dtype=torch.uint8, device=dev)
+            intrinsics = torch.empty(B, 3, 3, dtype=torch.float32, device=dev)
+            capi.check(capi.lib().moge_v1_postprocess(
+                points.data_ptr(), mask.data_ptr(), float(self.mask_threshold), capi.ptr(focal_in), B, H, W,
+                int(bool(force_projection)), int(bool(apply_mask)), depth.data_ptr(), mask_out.data_ptr(), intrinsics.data_ptr(),
+                focal.data_ptr(), shift.data_ptr(), capi.current_stream()))
+        return {'points': points, 'intrinsics': intrinsics, 'depth': depth, 'mask': mask_out.view(torch.bool)}
+
     # ------------------------------------------------------------------ public API
     def forward(self, image: torch.Tensor, num_tokens: Union[int, torch.LongTensor]) -> Dict[str, torch.Tensor]:
         if image.dim() != 4 or image.shape[1] != 3:
@@ -132,20 +176,39 @@ class MoGeModel(EngineModel):
             num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
         rh, rw = v1_resized_size(H, W, int(num_tokens))
         points, mask = self._forward_raw(image, rh, rw)
-        B = points.shape[0]
-        dev = self._device
-        with torch.cuda.device(dev):
-            focal_in = self._focal_in(fov_x, aspect_ratio, B)
-            focal = torch.empty(B, dtype=torch.float32, device=dev)
-            shift = torch.empty(B, dtype=torch.float32, device=dev)
-            depth = torch.empty(B, H, W, dtype=torch.float32, device=dev)
-            mask_out = torch.empty(B, H, W, dtype=torch.uint8, device=dev)
-            intrinsics = torch.empty(B, 3, 3, dtype=torch.float32, device=dev)
-            capi.check(capi.lib().moge_v1_postprocess(
-                points.data_ptr(), mask.data_ptr(), float(self.mask_threshold), capi.ptr(focal_in), B, H, W,
-                int(bool(force_projection)), int(bool(apply_mask)), depth.data_ptr(), mask_out.data_ptr(), intrinsics.data_ptr(),
-                focal.data_ptr(), shift.data_ptr(), capi.current_stream()))
-        ret = {'points': points, 'intrinsics': intrinsics, 'depth': depth, 'mask': mask_out.view(torch.bool)}
+        ret = self._postprocess(points, mask, aspect_ratio, fov_x, apply_mask, force_projection)
         if omit_batch_dim:
             ret = {k: v.squeeze(0) for k, v in ret.items()}
         return ret
+
+    @torch.inference_mode()
+    def infer_many(self,
+                   images,
+                   fov_x: Optional[Number] = None,
+                   resolution_level: int = 9,
+                   num_tokens: int = None,
+                   apply_mask: bool = True,
+                   force_projection: bool = True,
+                   use_fp16: bool = True) -> List[Dict[str, torch.Tensor]]:
+        """`infer()` over a list of images of DIFFERENT sizes (each (3,H,W)), with infer()'s argument order: one result dict per
+        image, in order.  No reference counterpart (the reference processes one shape per call): images are bucketed by shape,
+        the buckets are packed into engine calls of at most `max_chunk_tokens` tokens and every call runs the encoder ONCE over
+        the token rows of all its buckets.  `fov_x` is one horizontal field of view for every image, or None."""
+        self._check_use_fp16(use_fp16)
+        if num_tokens is None:
+            num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
+
+        def geometry(H, W):
+            rh, rw = v1_resized_size(H, W, int(num_tokens))
+            return (rh, rw), (rh // 14) * (rw // 14) + 1
+
+        calls = self._pack_calls(images, geometry)
+        results: List[Optional[Dict[str, torch.Tensor]]] = [None] * len(images)
+        for call in calls:
+            groups = [(torch.stack([images[i].to(self._device) for i in idx]), rh, rw) for (H, W, (rh, rw), idx) in call]
+            outs = self._forward_groups(groups)
+            for (H, W, _, idx), (points, mask) in zip(call, outs):
+                ret = self._postprocess(points, mask, W / H, fov_x, apply_mask, force_projection)
+                for j, i in enumerate(idx):
+                    results[i] = {k: v[j] for k, v in ret.items()}
+        return results

@@ -157,30 +157,17 @@ class MoGeModel(EngineModel):
         self._check_use_fp16(use_fp16)
         if num_tokens is None:
             num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
-        buckets: Dict[tuple, List[int]] = {}
-        for i, im in enumerate(images):
-            if im.dim() != 3 or im.shape[0] != 3:
-                raise ValueError(f"images[{i}] must be (3, H, W), got {tuple(im.shape)}")
-            buckets.setdefault((int(im.shape[1]), int(im.shape[2]), im.dtype), []).append(i)
-        # pack buckets (largest token count first) into calls bounded by max_chunk_tokens
-        units = []
-        for (H, W, _), idx in buckets.items():
+
+        def geometry(H, W):
             h, w = token_grid(H, W, int(num_tokens))
-            for lo, n in self._chunks(len(idx), h * w + 1):
-                units.append((n * (h * w + 1), H, W, h, w, idx[lo:lo + n]))
-        units.sort(key=lambda u: -u[0])
-        calls, cur, cur_tok = [], [], 0
-        for u in units:
-            if cur and cur_tok + u[0] > self.max_chunk_tokens:
-                calls.append(cur); cur, cur_tok = [], 0
-            cur.append(u); cur_tok += u[0]
-        if cur:
-            calls.append(cur)
+            return (h, w), h * w + 1
+
+        calls = self._pack_calls(images, geometry)
         results: List[Optional[Dict[str, torch.Tensor]]] = [None] * len(images)
         for call in calls:
-            groups = [(torch.stack([images[i].to(self._device) for i in idx]), h, w) for (_, H, W, h, w, idx) in call]
+            groups = [(torch.stack([images[i].to(self._device) for i in idx]), h, w) for (H, W, (h, w), idx) in call]
             outs = self._forward_groups(groups)
-            for (_, H, W, h, w, idx), (points, normal, mask, scale) in zip(call, outs):
+            for (H, W, _, idx), (points, normal, mask, scale) in zip(call, outs):
                 ret = self._postprocess(points, normal, mask, scale, W / H, force_projection, apply_mask, fov_x)
                 for j, i in enumerate(idx):
                     results[i] = {k: v[j] for k, v in ret.items()}
