@@ -44,11 +44,18 @@ struct Group {
     float* points = nullptr; float* normal = nullptr; float* mask = nullptr; float* scale = nullptr;
 };
 
-// The group a moge_group_t describes, with its bindings; rh, rw: MoGe-1's resized image (0 for MoGe-2)
-static Group make_group(const moge_group_t& m, int rh = 0, int rw = 0) {
+// The group a public group struct describes, with its bindings
+static Group make_group(const moge_group_t& m) {
     Group g;
-    g.B = m.B; g.H = m.H; g.W = m.W; g.h = m.h; g.w = m.w; g.rh = rh; g.rw = rw;
+    g.B = m.B; g.H = m.H; g.W = m.W; g.h = m.h; g.w = m.w;
     g.image = m.image; g.image_dtype = m.image_dtype; g.points = m.points; g.normal = m.normal; g.mask = m.mask_prob; g.scale = m.metric_scale;
+    return g;
+}
+
+static Group make_group(const moge_v1_group_t& m) {     // MoGe-1: the token grid of the resized image, rh/14 x rw/14
+    Group g;
+    g.B = m.B; g.H = m.H; g.W = m.W; g.h = m.rh / 14; g.w = m.rw / 14; g.rh = m.rh; g.rw = m.rw;
+    g.image = m.image; g.image_dtype = m.image_dtype; g.points = m.points; g.mask = m.mask;
     return g;
 }
 
@@ -774,30 +781,59 @@ void moge_engine_destroy(moge_engine_t* e) {
     delete e;
 }
 
-static int check_groups(moge_engine_t* e, const moge_group_t* g, int n, bool need_ptrs) {
-    if (!e || !g) return set_error("null argument");
+// ---- a public group array as plan groups.  Every check fires in the order written here and in the entry points, so a bad call
+//      reports the same first error however else it is wrong.
+
+// The checks both public group structs share
+static int check_group_count(int n) {
     if (n <= 0 || n > 64) return set_error("number of shape groups %d out of range (1..64)", n);
+    return 0;
+}
+
+static int check_image(const void* image, int image_dtype) {
+    if (!image) return set_error("null argument");
+    if (image_dtype != MOGE_F32 && image_dtype != MOGE_F16 && image_dtype != MOGE_BF16) return set_error("unsupported image dtype %d", image_dtype);
+    return 0;
+}
+
+// MoGe-2 groups, checked; `forward`: each group's image and requested outputs too
+static int to_groups(moge_engine_t* e, const moge_group_t* g, int n, bool forward, std::vector<Group>* out) {
+    if (!e || !g) return set_error("null argument");
+    MG_TRY(check_group_count(n));
     for (int i = 0; i < n; ++i) {
         if (g[i].B <= 0 || g[i].h <= 0 || g[i].w <= 0 || g[i].H <= 0 || g[i].W <= 0)
             return set_error("bad shape B=%d H=%d W=%d h=%d w=%d", g[i].B, g[i].H, g[i].W, g[i].h, g[i].w);
-        if (!need_ptrs) continue;
-        if (!g[i].image) return set_error("null argument");
-        if (g[i].image_dtype != MOGE_F32 && g[i].image_dtype != MOGE_F16 && g[i].image_dtype != MOGE_BF16) return set_error("unsupported image dtype %d", g[i].image_dtype);
-        if (e->v1) continue;                 // moge_v1_forward checks its outputs
-        if (g[i].points && !e->cfg.points_head.present) return set_error("points requested but the model has no points head");
-        if (g[i].normal && !e->cfg.normal_head.present) return set_error("normal requested but the model has no normal head");
-        if (g[i].mask_prob && !e->cfg.mask_head.present) return set_error("mask requested but the model has no mask head");
-        if (g[i].metric_scale && e->cfg.scale_head_layers == 0) return set_error("metric_scale requested but the model has no scale head");
+        if (forward) {
+            MG_TRY(check_image(g[i].image, g[i].image_dtype));
+            if (g[i].points && !e->cfg.points_head.present) return set_error("points requested but the model has no points head");
+            if (g[i].normal && !e->cfg.normal_head.present) return set_error("normal requested but the model has no normal head");
+            if (g[i].mask_prob && !e->cfg.mask_head.present) return set_error("mask requested but the model has no mask head");
+            if (g[i].metric_scale && e->cfg.scale_head_layers == 0) return set_error("metric_scale requested but the model has no scale head");
+        }
+        out->push_back(make_group(g[i]));
+    }
+    return 0;
+}
+
+// MoGe-1 groups, checked; `forward`: each group's outputs too (its image is checked after the call's own checks, check_forward)
+static int v1_to_groups(moge_engine_t* e, const moge_v1_group_t* g, int n, bool forward, std::vector<Group>* out) {
+    MG_TRY(check_group_count(n));
+    if (!g || !e) return set_error("null argument");
+    if (!e->v1) return set_error("not a MoGe-1 engine (moge_engine_create_v1)");
+    for (int i = 0; i < n; ++i) {
+        if (g[i].B <= 0 || g[i].H <= 0 || g[i].W <= 0) return set_error("bad shape B=%d H=%d W=%d", g[i].B, g[i].H, g[i].W);
+        if (g[i].rh < 14 || g[i].rw < 14) return set_error("resized image %dx%d is smaller than one 14-pixel patch", g[i].rh, g[i].rw);
+        if (forward && (!g[i].points || !g[i].mask)) return set_error("null argument");
+        out->push_back(make_group(g[i]));
     }
     return 0;
 }
 
 int moge_engine_workspace_bytes_groups(moge_engine_t* e, const moge_group_t* groups, int n, size_t* bytes) {
     if (!bytes) return set_error("null argument");
-    MG_TRY(check_groups(e, groups, n, false));
-    if (e->v1) return set_error("a MoGe-1 engine takes moge_v1_workspace_bytes");
     Plan pl;
-    for (int i = 0; i < n; ++i) pl.groups.push_back(make_group(groups[i]));
+    MG_TRY(to_groups(e, groups, n, false, &pl.groups));
+    if (e->v1) return set_error("a MoGe-1 engine takes moge_v1_workspace_bytes");
     return build_plan(e, &pl, true, bytes);
 }
 
@@ -807,16 +843,17 @@ int moge_engine_workspace_bytes(moge_engine_t* e, int B, int H, int W, int h, in
     return moge_engine_workspace_bytes_groups(e, &g, 1, bytes);
 }
 
-// The checks of a forward call, before anything runs
-static int check_forward(moge_engine_t* e, const moge_group_t* groups, int n, const void* workspace) {
+// The checks of a forward call, before anything runs: the engine, its weights and the workspace pointer, then `groups` (the
+// group checks that come after these), then the workspace alignment
+static int check_forward(moge_engine_t* e, const void* workspace, const std::function<int()>& groups) {
     if (!e || !workspace) return set_error("null argument");
     if (!e->finalized) return set_error("engine not finalized");
-    MG_TRY(check_groups(e, groups, n, true));
+    MG_TRY(groups());
     if (reinterpret_cast<uintptr_t>(workspace) & 1023) return set_error("workspace must be 1024-byte aligned");
     return 0;
 }
 
-// groups: checked by check_forward, with their bindings
+// groups: checked, with their bindings
 static int forward_impl(moge_engine_t* e, const std::vector<Group>& groups, void* workspace, size_t workspace_bytes, void* stream) {
     CUDA_TRY(cudaSetDevice(e->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -877,52 +914,25 @@ static int forward_impl(moge_engine_t* e, const std::vector<Group>& groups, void
 
 int moge_engine_forward_groups(moge_engine_t* e, const moge_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream) {
     if (e && e->v1) return set_error("a MoGe-1 engine runs through moge_v1_forward");
-    MG_TRY(check_forward(e, groups, n, workspace));
     std::vector<Group> gs;
-    for (int i = 0; i < n; ++i) gs.push_back(make_group(groups[i]));
+    MG_TRY(check_forward(e, workspace, [&] { return to_groups(e, groups, n, true, &gs); }));
     return forward_impl(e, gs, workspace, workspace_bytes, stream);
-}
-
-static int check_v1_shape(moge_engine_t* e, int B, int H, int W, int rh, int rw) {
-    if (!e) return set_error("null argument");
-    if (!e->v1) return set_error("not a MoGe-1 engine (moge_engine_create_v1)");
-    if (B <= 0 || H <= 0 || W <= 0) return set_error("bad shape B=%d H=%d W=%d", B, H, W);
-    if (rh < 14 || rw < 14) return set_error("resized image %dx%d is smaller than one 14-pixel patch", rh, rw);
-    return 0;
-}
-
-// The MoGe-1 groups as moge_group_t (token grid rh/14 x rw/14) and as plan groups, after the per-group checks; `outputs`: the
-// points and mask pointers are checked too (a forward)
-static int v1_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, bool outputs, std::vector<moge_group_t>* mg,
-                     std::vector<Group>* gs) {
-    if (n <= 0 || n > 64) return set_error("number of shape groups %d out of range (1..64)", n);
-    if (!groups) return set_error("null argument");
-    for (int i = 0; i < n; ++i) {
-        const moge_v1_group_t& v = groups[i];
-        MG_TRY(check_v1_shape(e, v.B, v.H, v.W, v.rh, v.rw));
-        if (outputs && (!v.points || !v.mask)) return set_error("null argument");
-        moge_group_t g{};
-        g.image = v.image; g.image_dtype = v.image_dtype; g.B = v.B; g.H = v.H; g.W = v.W; g.h = v.rh / 14; g.w = v.rw / 14;
-        g.points = v.points; g.mask_prob = v.mask;
-        mg->push_back(g);
-        gs->push_back(make_group(g, v.rh, v.rw));
-    }
-    return 0;
 }
 
 int moge_v1_workspace_bytes_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, size_t* bytes) {
     if (!bytes) return set_error("null argument");
-    std::vector<moge_group_t> mg;
     Plan pl;
-    MG_TRY(v1_groups(e, groups, n, false, &mg, &pl.groups));
+    MG_TRY(v1_to_groups(e, groups, n, false, &pl.groups));
     return build_plan(e, &pl, true, bytes);
 }
 
 int moge_v1_forward_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream) {
-    std::vector<moge_group_t> mg;
     std::vector<Group> gs;
-    MG_TRY(v1_groups(e, groups, n, true, &mg, &gs));
-    MG_TRY(check_forward(e, mg.data(), n, workspace));
+    MG_TRY(v1_to_groups(e, groups, n, true, &gs));
+    MG_TRY(check_forward(e, workspace, [&] {
+        for (const Group& g : gs) MG_TRY(check_image(g.image, g.image_dtype));
+        return 0;
+    }));
     return forward_impl(e, gs, workspace, workspace_bytes, stream);
 }
 

@@ -1,5 +1,7 @@
-"""Host plumbing shared by the drop-in MoGe-2 and MoGe-1 models (v2.py, v1.py): the nn.Module-like surface, checkpoint
-loading, the engine handle with its weight upload, the activation workspace, the batch chunking and the mixed-shape packing.
+"""Host code shared by the drop-in MoGe-2 and MoGe-1 models (v2.py, v1.py): the nn.Module-like surface, checkpoint loading,
+the engine handle with its weight upload, the activation workspace, and the whole forward path: the engine call over an array
+of shape groups, the chunked single-shape forward, the mixed-shape packing, and the bodies of `forward`, `infer` and
+`infer_many`.  The model files keep their configs, the small per-model hooks and the public signatures.
 Host logic only: every arithmetic step runs in the C-ABI library.
 """
 from __future__ import annotations
@@ -11,12 +13,17 @@ from typing import IO, Any, Callable, Dict, List, Optional, Tuple, Union
 import torch
 
 from .. import capi
+from ..configs import default_num_tokens
 
 
 class EngineModel:
-    """Base of both drop-in `MoGeModel` classes.  A subclass supplies `_expected_keys()` (the checkpoint keys of its config),
-    `_create_engine(handle)` (its config struct and create call, which sets the C handle), `_strict_load` (how
-    `from_pretrained` loads) and `_fp32_pass_error` (why `use_fp16=False` is refused)."""
+    """Base of both drop-in `MoGeModel` classes.  A subclass supplies
+      `_expected_keys()` (the checkpoint keys of its config), `_create_engine(handle)` (its config struct and create call, which
+      sets the C handle), `_strict_load` (how `from_pretrained` loads) and `_fp32_pass_error` (why `use_fp16=False` is refused);
+      `_group_t`, `_c_workspace_bytes_groups`, `_c_forward_groups` (its C group struct and the names of its two group entry points);
+      `_geometry(H, W, num_tokens)` -> (geom, token rows per image), geom being what one group struct carries besides B, H, W;
+      `_alloc_outputs(B, H, W)` (its fp32 output buffers, absent heads None), `_fill_group(g, geom, outputs)`, `_output_names`
+      (the keys `forward` returns them under) and `_postprocess(outputs, aspect_ratio, fov_x, apply_mask, force_projection)`."""
 
     def __init__(self):
         self._state: Dict[str, torch.Tensor] = {}
@@ -239,6 +246,88 @@ class EngineModel:
     def _check_use_fp16(self, use_fp16: bool):
         if not use_fp16:
             raise NotImplementedError(self._fp32_pass_error)
+
+    # ------------------------------------------------------------------ forward path
+    def _engine_call(self, groups) -> None:
+        """ONE engine call over shape groups [(engine-input image (B,3,H,W), geom, outputs)], `outputs` being caller-allocated
+        buffers or views of them (`_alloc_outputs`).  The encoder runs once over the packed token rows of all groups, and each
+        group's decoder writes its outputs."""
+        self._ensure_engine()
+        arr = (self._group_t * len(groups))()
+        for g, (image, geom, outputs) in zip(arr, groups):
+            g.image, g.image_dtype = image.data_ptr(), capi.torch_dtype_code(image.dtype)
+            g.B, g.H, g.W = image.shape[0], image.shape[2], image.shape[3]
+            self._fill_group(g, geom, outputs)
+        L = capi.lib()
+        with torch.cuda.device(self._device):
+            nbytes = C.c_size_t()
+            capi.check(getattr(L, self._c_workspace_bytes_groups)(self._engine, arr, len(groups), C.byref(nbytes)))
+            ws, ws_bytes = self._workspace_for(nbytes.value)
+            capi.check(getattr(L, self._c_forward_groups)(self._engine, arr, len(groups), ws, ws_bytes, capi.current_stream()))
+
+    def _forward_groups(self, groups):
+        """ONE engine call over shape groups [(image (B,3,H,W), *geom)], into newly allocated outputs; returns them per group."""
+        bound = []
+        for image, *geom in groups:
+            image = self._engine_input(image)
+            bound.append((image, geom, self._alloc_outputs(image.shape[0], image.shape[2], image.shape[3])))
+        self._engine_call(bound)
+        return [outputs for _, _, outputs in bound]
+
+    def _forward_chunks(self, image: torch.Tensor, geom, tokens_per_image: int):
+        """The forward of a (B,3,H,W) batch of one shape: the full-batch outputs, written by one engine call per chunk of
+        `_chunks`, each over one group of the chunk's images and output views."""
+        image = self._engine_input(image)
+        B, _, H, W = image.shape
+        outputs = self._alloc_outputs(B, H, W)
+        for lo, n in self._chunks(B, tokens_per_image):
+            views = tuple(None if t is None else t[lo:lo + n] for t in outputs)
+            self._engine_call([(image[lo:lo + n], geom, views)])
+        return outputs
+
+    def forward(self, image: torch.Tensor, num_tokens: Union[int, torch.LongTensor]) -> Dict[str, torch.Tensor]:
+        if image.dim() != 4 or image.shape[1] != 3:
+            raise ValueError(f"image must be (B, 3, H, W), got {tuple(image.shape)}")
+        H, W = image.shape[-2:]
+        if isinstance(num_tokens, torch.Tensor):
+            num_tokens = int(num_tokens.item())
+        outputs = self._forward_chunks(image, *self._geometry(H, W, num_tokens))
+        return {k: v for k, v in zip(self._output_names, outputs) if v is not None}
+
+    __call__ = forward
+
+    def _infer(self, image, *, num_tokens, resolution_level, force_projection, apply_mask, fov_x, use_fp16):
+        """The body of both models' `infer`."""
+        self._check_use_fp16(use_fp16)
+        omit_batch_dim = image.dim() == 3
+        if omit_batch_dim:
+            image = image.unsqueeze(0)
+        H, W = image.shape[-2:]
+        if num_tokens is None:
+            num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
+        outputs = self._forward_chunks(image, *self._geometry(H, W, int(num_tokens)))
+        ret = self._postprocess(outputs, W / H, fov_x, apply_mask, force_projection)
+        if omit_batch_dim:
+            ret = {k: v.squeeze(0) for k, v in ret.items()}
+        return ret
+
+    def _infer_many(self, images, *, num_tokens, resolution_level, force_projection, apply_mask, fov_x,
+                    use_fp16) -> List[Dict[str, torch.Tensor]]:
+        """The body of both models' `infer_many`: the images bucketed and packed into engine calls (`_pack_calls`, then
+        `_forward_groups`), each call's groups post-processed, and the per-image results returned in input order."""
+        self._check_use_fp16(use_fp16)
+        if num_tokens is None:
+            num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
+        calls = self._pack_calls(images, lambda H, W: self._geometry(H, W, int(num_tokens)))
+        results: List[Optional[Dict[str, torch.Tensor]]] = [None] * len(images)
+        for call in calls:
+            outs = self._forward_groups([(torch.stack([images[i].to(self._device) for i in idx]), *geom)
+                                         for (H, W, geom, idx) in call])
+            for (H, W, _, idx), outputs in zip(call, outs):
+                ret = self._postprocess(outputs, W / H, fov_x, apply_mask, force_projection)
+                for j, i in enumerate(idx):
+                    results[i] = {k: v[j] for k, v in ret.items()}
+        return results
 
     # ------------------------------------------------------------------ introspection
     def engine_ops(self):

@@ -6,7 +6,9 @@ Mirrors the public surface of /root/reference/moge/model/v1.py:
   infer(image, fov_x, resolution_level, num_tokens, apply_mask, force_projection, use_fp16)
       -> {'points', 'intrinsics', 'depth', 'mask'} (v1.py:301-392),
 and, with no reference counterpart, infer_many(images, ...) over a list of images of different sizes (one encoder pass per call).
-Host logic only: tensor allocation and checkpoint I/O use PyTorch, every arithmetic step runs in the C-ABI library.
+This file holds the MoGe-1 config, its engine hooks (resized image, output buffers, group struct, post-processing) and the public
+signatures; the forward path itself (engine calls, chunking, packing, the bodies of forward / infer / infer_many) is EngineModel's
+in _engine.py.  Host logic only: tensor allocation and checkpoint I/O use PyTorch, every arithmetic step runs in the C-ABI library.
 """
 from __future__ import annotations
 
@@ -18,7 +20,7 @@ from typing import Dict, List, Optional, Tuple, Union
 import torch
 
 from .. import capi
-from ..configs import backbone_dims, default_num_tokens, v1_resized_size
+from ..configs import backbone_dims, v1_resized_size
 from ._engine import EngineModel
 
 
@@ -75,58 +77,33 @@ class MoGeModel(EngineModel):
         from ..synthetic import v1_expected_keys
         return v1_expected_keys(self.model_config)
 
-    # ------------------------------------------------------------------ engine
+    # ------------------------------------------------------------------ engine hooks (EngineModel runs the forward path)
+    _group_t = capi.V1Group
+    _c_workspace_bytes_groups = "moge_v1_workspace_bytes_groups"
+    _c_forward_groups = "moge_v1_forward_groups"
+    _output_names = ("points", "mask")
+
     def _create_engine(self, handle: C.c_void_p):
         cfg = capi.make_v1_config(self.model_config, self._compute_code())
         capi.check(capi.lib().moge_engine_create_v1(C.byref(cfg), self._device.index, C.byref(handle)))
 
-    def _forward_raw(self, image: torch.Tensor, rh: int, rw: int):
-        """Engine forward in chunks of at most `max_chunk_tokens` tokens; returns fp32 (points (B,H,W,3), raw mask (B,H,W))."""
-        self._ensure_engine()
-        image = self._engine_input(image)
-        B, _, H, W = image.shape
-        dev = self._device
-        L = capi.lib()
-        with torch.cuda.device(dev):
-            points = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev)
-            mask = torch.empty(B, H, W, dtype=torch.float32, device=dev)
-            for lo, n in self._chunks(B, (rh // 14) * (rw // 14) + 1):
-                nbytes = C.c_size_t()
-                capi.check(L.moge_v1_workspace_bytes(self._engine, n, H, W, rh, rw, C.byref(nbytes)))
-                ws, ws_bytes = self._workspace_for(nbytes.value)
-                capi.check(L.moge_v1_forward(
-                    self._engine, image[lo:lo + n].data_ptr(), capi.torch_dtype_code(image.dtype), n, H, W, rh, rw, ws, ws_bytes,
-                    points[lo:lo + n].data_ptr(), mask[lo:lo + n].data_ptr(), capi.current_stream()))
-        return points, mask
+    def _geometry(self, H: int, W: int, num_tokens):
+        """((rh, rw) resized image, token rows per image) of an H x W image at `num_tokens`, taken as given (v1.py:272-274)."""
+        rh, rw = v1_resized_size(H, W, num_tokens)
+        return (rh, rw), (rh // 14) * (rw // 14) + 1
 
-    def _forward_groups(self, groups):
-        """ONE engine call over several shape groups: `groups` = [(image (B,3,H,W), rh, rw)].  The encoder runs once over the
-        packed token rows of all groups (moge_v1_forward_groups).  Returns [(points, raw mask)], fp32, per group."""
-        self._ensure_engine()
-        n = len(groups)
-        arr = (capi.V1Group * n)()
-        keep, outs = [], []
-        dev = self._device
-        with torch.cuda.device(dev):
-            for i, (image, rh, rw) in enumerate(groups):
-                image = self._engine_input(image)
-                B, _, H, W = image.shape
-                points = torch.empty(B, H, W, 3, dtype=torch.float32, device=dev)
-                mask = torch.empty(B, H, W, dtype=torch.float32, device=dev)
-                g = arr[i]
-                g.image, g.image_dtype = image.data_ptr(), capi.torch_dtype_code(image.dtype)
-                g.B, g.H, g.W, g.rh, g.rw = B, H, W, rh, rw
-                g.points, g.mask = points.data_ptr(), mask.data_ptr()
-                keep.append(image)
-                outs.append((points, mask))
-            nbytes = C.c_size_t()
-            capi.check(capi.lib().moge_v1_workspace_bytes_groups(self._engine, arr, n, C.byref(nbytes)))
-            ws, ws_bytes = self._workspace_for(nbytes.value)
-            capi.check(capi.lib().moge_v1_forward_groups(self._engine, arr, n, ws, ws_bytes, capi.current_stream()))
-        return outs
+    def _alloc_outputs(self, B: int, H: int, W: int):
+        """fp32 (points, raw mask) buffers for B images of H x W."""
+        return (torch.empty(B, H, W, 3, dtype=torch.float32, device=self._device),
+                torch.empty(B, H, W, dtype=torch.float32, device=self._device))
 
-    def _postprocess(self, points, mask, aspect_ratio, fov_x, apply_mask, force_projection) -> Dict[str, torch.Tensor]:
+    def _fill_group(self, g: capi.V1Group, geom, outputs):
+        g.rh, g.rw = geom
+        g.points, g.mask = (t.data_ptr() for t in outputs)
+
+    def _postprocess(self, outputs, aspect_ratio, fov_x, apply_mask, force_projection) -> Dict[str, torch.Tensor]:
         """The fp32 part of infer() (v1.py:352-380) on the raw forward outputs of one shape group; all on the device."""
+        points, mask = outputs
         B, H, W = mask.shape
         dev = self._device
         with torch.cuda.device(dev):
@@ -143,18 +120,6 @@ class MoGeModel(EngineModel):
         return {'points': points, 'intrinsics': intrinsics, 'depth': depth, 'mask': mask_out.view(torch.bool)}
 
     # ------------------------------------------------------------------ public API
-    def forward(self, image: torch.Tensor, num_tokens: Union[int, torch.LongTensor]) -> Dict[str, torch.Tensor]:
-        if image.dim() != 4 or image.shape[1] != 3:
-            raise ValueError(f"image must be (B, 3, H, W), got {tuple(image.shape)}")
-        H, W = image.shape[-2:]
-        if isinstance(num_tokens, torch.Tensor):
-            num_tokens = int(num_tokens.item())
-        rh, rw = v1_resized_size(H, W, num_tokens)
-        points, mask = self._forward_raw(image, rh, rw)
-        return {'points': points, 'mask': mask}
-
-    __call__ = forward
-
     @torch.inference_mode()
     def infer(self,
               image: torch.Tensor,
@@ -166,20 +131,8 @@ class MoGeModel(EngineModel):
               use_fp16: bool = True) -> Dict[str, torch.Tensor]:
         """Same contract as v1.py:301-392 (note the argument order differs from MoGe-2's infer).  The engine multiplies in 16-bit
         with fp32 accumulation and post-processes in fp32; `use_fp16=False` (a full-fp32 network pass) is not provided."""
-        self._check_use_fp16(use_fp16)
-        omit_batch_dim = image.dim() == 3
-        if omit_batch_dim:
-            image = image.unsqueeze(0)
-        H, W = image.shape[-2:]
-        aspect_ratio = W / H
-        if num_tokens is None:
-            num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
-        rh, rw = v1_resized_size(H, W, int(num_tokens))
-        points, mask = self._forward_raw(image, rh, rw)
-        ret = self._postprocess(points, mask, aspect_ratio, fov_x, apply_mask, force_projection)
-        if omit_batch_dim:
-            ret = {k: v.squeeze(0) for k, v in ret.items()}
-        return ret
+        return self._infer(image, num_tokens=num_tokens, resolution_level=resolution_level, force_projection=force_projection,
+                           apply_mask=apply_mask, fov_x=fov_x, use_fp16=use_fp16)
 
     @torch.inference_mode()
     def infer_many(self,
@@ -194,21 +147,5 @@ class MoGeModel(EngineModel):
         image, in order.  No reference counterpart (the reference processes one shape per call): images are bucketed by shape,
         the buckets are packed into engine calls of at most `max_chunk_tokens` tokens and every call runs the encoder ONCE over
         the token rows of all its buckets.  `fov_x` is one horizontal field of view for every image, or None."""
-        self._check_use_fp16(use_fp16)
-        if num_tokens is None:
-            num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
-
-        def geometry(H, W):
-            rh, rw = v1_resized_size(H, W, int(num_tokens))
-            return (rh, rw), (rh // 14) * (rw // 14) + 1
-
-        calls = self._pack_calls(images, geometry)
-        results: List[Optional[Dict[str, torch.Tensor]]] = [None] * len(images)
-        for call in calls:
-            groups = [(torch.stack([images[i].to(self._device) for i in idx]), rh, rw) for (H, W, (rh, rw), idx) in call]
-            outs = self._forward_groups(groups)
-            for (H, W, _, idx), (points, mask) in zip(call, outs):
-                ret = self._postprocess(points, mask, W / H, fov_x, apply_mask, force_projection)
-                for j, i in enumerate(idx):
-                    results[i] = {k: v[j] for k, v in ret.items()}
-        return results
+        return self._infer_many(images, num_tokens=num_tokens, resolution_level=resolution_level,
+                                force_projection=force_projection, apply_mask=apply_mask, fov_x=fov_x, use_fp16=use_fp16)

@@ -4,9 +4,12 @@ Mirrors the public surface of /root/reference/moge/model/v2.py:
   __init__ kwargs (v2.py:30-57), from_pretrained (v2.py:76-107), .to/.eval/.half, .device/.dtype (v2.py:59-65),
   forward(image, num_tokens) -> {'points','normal','mask','metric_scale'} (v2.py:138-192),
   infer(image, num_tokens, resolution_level, force_projection, apply_mask, fov_x, use_fp16)
-      -> {'points','intrinsics','depth','mask','normal'} (v2.py:194-303).
-This file is host logic only: tensor allocation and checkpoint I/O use PyTorch, every arithmetic step of the path
-runs in the C-ABI library.  There is no CPU / eager fallback.
+      -> {'points','intrinsics','depth','mask','normal'} (v2.py:194-303),
+and, with no reference counterpart, infer_many(images, ...) over a list of images of different sizes (one encoder pass per call).
+This file holds the MoGe-2 config, its engine hooks (token grid, output heads, group struct, post-processing) and the public
+signatures; the forward path itself (engine calls, chunking, packing, the bodies of forward / infer / infer_many) is EngineModel's
+in _engine.py.  Host logic only: tensor allocation and checkpoint I/O use PyTorch, every arithmetic step of the path runs in the
+C-ABI library.  There is no CPU / eager fallback.
 """
 from __future__ import annotations
 
@@ -18,7 +21,7 @@ import ctypes as C
 import torch
 
 from .. import capi
-from ..configs import backbone_dims, default_num_tokens, token_grid
+from ..configs import backbone_dims, token_grid
 from ._engine import EngineModel
 
 
@@ -91,10 +94,20 @@ class MoGeModel(EngineModel):
         from ..synthetic import expected_keys
         return expected_keys(self.model_config)
 
-    # ------------------------------------------------------------------ engine
+    # ------------------------------------------------------------------ engine hooks (EngineModel runs the forward path)
+    _group_t = capi.Group
+    _c_workspace_bytes_groups = "moge_engine_workspace_bytes_groups"
+    _c_forward_groups = "moge_engine_forward_groups"
+    _output_names = ("points", "normal", "mask", "metric_scale")
+
     def _create_engine(self, handle: C.c_void_p):
         cfg = capi.make_config(self.model_config, self._compute_code())
         capi.check(capi.lib().moge_engine_create(C.byref(cfg), self._device.index, C.byref(handle)))
+
+    def _geometry(self, H: int, W: int, num_tokens):
+        """((h, w) token grid, token rows per image) of an H x W image at `num_tokens`, truncated to an int."""
+        h, w = token_grid(H, W, int(num_tokens))
+        return (h, w), h * w + 1
 
     def _alloc_outputs(self, B: int, H: int, W: int):
         """fp32 (points, normal, mask_prob, metric_scale) buffers for B images of H x W, absent heads as None."""
@@ -105,90 +118,13 @@ class MoGeModel(EngineModel):
         scale = torch.empty(B, dtype=torch.float32, device=dev) if hasattr(self, "scale_head") else None
         return points, normal, mask, scale
 
-    def _forward_raw(self, image: torch.Tensor, h: int, w: int):
-        """Runs the engine forward; returns fp32 (points, normal, mask_prob, metric_scale), absent heads as None."""
-        self._ensure_engine()
-        image = self._engine_input(image)
-        B, _, H, W = image.shape
-        L = capi.lib()
-        with torch.cuda.device(self._device):
-            outs = self._alloc_outputs(B, H, W)
-            for lo, n in self._chunks(B, h * w + 1):
-                nbytes = C.c_size_t()
-                capi.check(L.moge_engine_workspace_bytes(self._engine, n, H, W, h, w, C.byref(nbytes)))
-                ws, ws_bytes = self._workspace_for(nbytes.value)
-                points, normal, mask, scale = (None if t is None else t[lo:lo + n] for t in outs)
-                capi.check(L.moge_engine_forward(
-                    self._engine, image[lo:lo + n].data_ptr(), capi.torch_dtype_code(image.dtype), n, H, W, h, w, ws, ws_bytes,
-                    capi.ptr(points), capi.ptr(normal), capi.ptr(mask), capi.ptr(scale), capi.current_stream()))
-        return outs
+    def _fill_group(self, g: capi.Group, geom, outputs):
+        g.h, g.w = geom
+        g.points, g.normal, g.mask_prob, g.metric_scale = (capi.ptr(t) for t in outputs)
 
-    def _forward_groups(self, groups):
-        """ONE engine call over several shape groups: `groups` = [(image (B,3,H,W), h, w)].  The encoder runs once over the
-        packed token rows of all groups (moge_engine_forward_groups).  Returns [(points, normal, mask_prob, metric_scale)]."""
-        self._ensure_engine()
-        n = len(groups)
-        arr = (capi.Group * n)()
-        keep, outs = [], []
-        with torch.cuda.device(self._device):
-            for i, (image, h, w) in enumerate(groups):
-                image = self._engine_input(image)
-                B, _, H, W = image.shape
-                points, normal, mask, scale = self._alloc_outputs(B, H, W)
-                g = arr[i]
-                g.image, g.image_dtype = image.data_ptr(), capi.torch_dtype_code(image.dtype)
-                g.B, g.H, g.W, g.h, g.w = B, H, W, h, w
-                g.points, g.normal, g.mask_prob, g.metric_scale = capi.ptr(points), capi.ptr(normal), capi.ptr(mask), capi.ptr(scale)
-                keep.append(image)
-                outs.append((points, normal, mask, scale))
-            nbytes = C.c_size_t()
-            capi.check(capi.lib().moge_engine_workspace_bytes_groups(self._engine, arr, n, C.byref(nbytes)))
-            ws, ws_bytes = self._workspace_for(nbytes.value)
-            capi.check(capi.lib().moge_engine_forward_groups(self._engine, arr, n, ws, ws_bytes, capi.current_stream()))
-        return outs
-
-    @torch.inference_mode()
-    def infer_many(self, images, num_tokens: int = None, resolution_level: int = 9, force_projection: bool = True,
-                   apply_mask: bool = True, fov_x: Optional[Number] = None, use_fp16: bool = True) -> List[Dict[str, torch.Tensor]]:
-        """`infer()` over a list of images of DIFFERENT sizes (each (3,H,W)): one result dict per image, in order.
-        No reference counterpart (the reference processes one shape per call; moge/scripts/infer.py:101 loops over files):
-        images are bucketed by shape, the buckets are packed into engine calls of at most `max_chunk_tokens` tokens and every
-        call runs the encoder ONCE over the token rows of all its buckets (ragged batching, BASELINE.json configs[2])."""
-        self._check_use_fp16(use_fp16)
-        if num_tokens is None:
-            num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
-
-        def geometry(H, W):
-            h, w = token_grid(H, W, int(num_tokens))
-            return (h, w), h * w + 1
-
-        calls = self._pack_calls(images, geometry)
-        results: List[Optional[Dict[str, torch.Tensor]]] = [None] * len(images)
-        for call in calls:
-            groups = [(torch.stack([images[i].to(self._device) for i in idx]), h, w) for (H, W, (h, w), idx) in call]
-            outs = self._forward_groups(groups)
-            for (H, W, _, idx), (points, normal, mask, scale) in zip(call, outs):
-                ret = self._postprocess(points, normal, mask, scale, W / H, force_projection, apply_mask, fov_x)
-                for j, i in enumerate(idx):
-                    results[i] = {k: v[j] for k, v in ret.items()}
-        return results
-
-    # ------------------------------------------------------------------ public API
-    def forward(self, image: torch.Tensor, num_tokens: Union[int, torch.LongTensor]) -> Dict[str, torch.Tensor]:
-        if image.dim() != 4 or image.shape[1] != 3:
-            raise ValueError(f"image must be (B, 3, H, W), got {tuple(image.shape)}")
-        H, W = image.shape[-2:]
-        if isinstance(num_tokens, torch.Tensor):
-            num_tokens = int(num_tokens.item())
-        h, w = token_grid(H, W, int(num_tokens))
-        points, normal, mask, scale = self._forward_raw(image, h, w)
-        out = {'points': points, 'normal': normal, 'mask': mask, 'metric_scale': scale}
-        return {k: v for k, v in out.items() if v is not None}
-
-    __call__ = forward
-
-    def _postprocess(self, points, normal, mask, metric_scale, aspect_ratio, force_projection, apply_mask, fov_x):
+    def _postprocess(self, outputs, aspect_ratio, fov_x, apply_mask, force_projection) -> Dict[str, torch.Tensor]:
         """K18 + K19 of infer() (v2.py:246-298) on the raw forward outputs of one shape group; all on the device."""
+        points, normal, mask, metric_scale = outputs
         dev = self._device
         some = points if points is not None else (normal if normal is not None else mask)
         B, H, W = some.shape[0], some.shape[1], some.shape[2]
@@ -228,6 +164,7 @@ class MoGeModel(EngineModel):
                     ret['normal'] = normal
         return ret
 
+    # ------------------------------------------------------------------ public API
     @torch.inference_mode()
     def infer(self,
               image: torch.Tensor,
@@ -241,17 +178,15 @@ class MoGeModel(EngineModel):
         `.bfloat16()`) with fp32 accumulation, fp32 residual stream and fp32 post-processing; a full-fp32 network pass
         (the reference's `use_fp16=False`, v2.py:241) does not exist here, so asking for it is an error rather than a silent
         precision downgrade."""
-        self._check_use_fp16(use_fp16)
-        omit_batch_dim = image.dim() == 3
-        if omit_batch_dim:
-            image = image.unsqueeze(0)
-        H, W = image.shape[-2:]
-        aspect_ratio = W / H
-        if num_tokens is None:
-            num_tokens = default_num_tokens(self.num_tokens_range, resolution_level)
-        h, w = token_grid(H, W, int(num_tokens))
-        points, normal, mask, metric_scale = self._forward_raw(image, h, w)
-        ret = self._postprocess(points, normal, mask, metric_scale, aspect_ratio, force_projection, apply_mask, fov_x)
-        if omit_batch_dim:
-            ret = {k: v.squeeze(0) for k, v in ret.items()}
-        return ret
+        return self._infer(image, num_tokens=num_tokens, resolution_level=resolution_level, force_projection=force_projection,
+                           apply_mask=apply_mask, fov_x=fov_x, use_fp16=use_fp16)
+
+    @torch.inference_mode()
+    def infer_many(self, images, num_tokens: int = None, resolution_level: int = 9, force_projection: bool = True,
+                   apply_mask: bool = True, fov_x: Optional[Number] = None, use_fp16: bool = True) -> List[Dict[str, torch.Tensor]]:
+        """`infer()` over a list of images of DIFFERENT sizes (each (3,H,W)): one result dict per image, in order.
+        No reference counterpart (the reference processes one shape per call; moge/scripts/infer.py:101 loops over files):
+        images are bucketed by shape, the buckets are packed into engine calls of at most `max_chunk_tokens` tokens and every
+        call runs the encoder ONCE over the token rows of all its buckets (ragged batching, BASELINE.json configs[2])."""
+        return self._infer_many(images, num_tokens=num_tokens, resolution_level=resolution_level,
+                                force_projection=force_projection, apply_mask=apply_mask, fov_x=fov_x, use_fp16=use_fp16)

@@ -132,6 +132,30 @@ def test_v1_model_plumbing_without_gpu():
     _check_model_plumbing(MoGeModel, v1_model_config("vits"))
 
 
+def test_public_signatures():
+    """forward / infer / infer_many keep the parameter names, order and defaults of the reference classes (v2.py:138,194,
+    v1.py:269,301).  The two models take infer's arguments in different orders, behind one shared body."""
+    import inspect
+    from moge.model.v1 import MoGeModel as V1
+    from moge.model.v2 import MoGeModel as V2
+    E = inspect.Parameter.empty
+
+    def params(f):
+        ps = inspect.signature(f).parameters.values()
+        assert all(p.kind == inspect.Parameter.POSITIONAL_OR_KEYWORD for p in ps), f
+        return [(p.name, p.default) for p in ps]
+
+    v2_args = [("num_tokens", None), ("resolution_level", 9), ("force_projection", True), ("apply_mask", True),
+               ("fov_x", None), ("use_fp16", True)]
+    v1_args = [("fov_x", None), ("resolution_level", 9), ("num_tokens", None), ("apply_mask", True),
+               ("force_projection", True), ("use_fp16", True)]
+    for M, args in ((V2, v2_args), (V1, v1_args)):
+        assert params(M.forward) == [("self", E), ("image", E), ("num_tokens", E)]
+        assert M.__call__ is M.forward
+        assert params(M.infer) == [("self", E), ("image", E)] + args
+        assert params(M.infer_many) == [("self", E), ("images", E)] + args
+
+
 def test_synthetic_checkpoint_roundtrip(tmp_path):
     """The synthetic checkpoint is a reference-format file: {'model_config', 'model'} loadable with weights_only=True."""
     from moge.model.v2 import MoGeModel
