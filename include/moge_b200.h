@@ -405,6 +405,24 @@ int moge_panorama_resize(const float* src, int h, int w, int H, int W, float* ds
  * points (H, W, 3) = depth_out * spherical_uv_to_directions(uv_map(H, W)).                                                   */
 int moge_panorama_finish(const float* depth, const uint8_t* mask, int h, int w, int H, int W, float* depth_out, uint8_t* mask_out,
                          float* points, void* stream);
+/* Batches of 1 to MOGE_PANORAMA_MAX_BATCH panoramas of one size and one set of cameras, each item's result bitwise that of the
+ * call above on it alone.  Arrays gain a leading batch dimension: images (batch, H, W, 3), views_f32 (batch * views, 3, res, res),
+ * views_u8 (batch * views, res, res, 3), src (batch, views, vh, vw, channels), mask (batch, views, vh, vw), b and row_mask
+ * (batch, rows), pano_mask, init and depth (batch, h, w), stats (batch, 2), depth_out, mask_out (batch, H, W), points
+ * (batch, H, W, 3).  moge_panorama_lsmr_batch solves the batch's systems in one cooperative launch that ends when every system
+ * has stopped; moge_panorama_workspace_bytes_batch sizes the workspace of moge_panorama_rhs_batch / moge_panorama_lsmr_batch. */
+#define MOGE_PANORAMA_MAX_BATCH 64
+int moge_panorama_split_batch(const uint8_t* images, int batch, int H, int W, const moge_panorama_camera_t* cams, int views,
+                              const float* grid, int res, float* views_f32, uint8_t* views_u8, void* stream);
+int moge_panorama_workspace_bytes_batch(int batch, int views, int h, int w, size_t* bytes);
+int moge_panorama_rhs_batch(const float* src, int channels, const uint8_t* mask, int batch, int views, int vh, int vw,
+                            const moge_panorama_camera_t* cams, const float* directions, int h, int w, double* b, uint8_t* row_mask,
+                            uint8_t* pano_mask, void* workspace, size_t workspace_bytes, void* stream);
+int moge_panorama_lsmr_batch(const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
+                             int32_t* stats, void* workspace, size_t workspace_bytes, void* stream);
+int moge_panorama_resize_batch(const float* src, int batch, int h, int w, int H, int W, float* dst, void* stream);
+int moge_panorama_finish_batch(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
+                               uint8_t* mask_out, float* points, void* stream);
 
 /* ---- training losses of moge/train/losses.py (Python: moge_b200.losses, moge_b200.local_loss; alias moge.train.losses).
  * Maps are (batch, H, W) fp32 and point maps (batch, H, W, 3) fp32, contiguous on the device.  Each call either reduces

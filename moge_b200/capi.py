@@ -26,6 +26,7 @@ MESH_MAX_MAPS, MESH_MAX_CHANNELS = 8, 4
 MESH_F32, MESH_U8_UNIT, MESH_UV = 0, 1, 2
 MESH_HWC, MESH_CHW = 0, 1
 PANORAMA_MAX_VIEWS = 20
+PANORAMA_MAX_BATCH = 64
 LOSS_SUMS = 4
 LOSS_MASK_L2, LOSS_MASK_BCE, LOSS_EDGE, LOSS_NORMAL = range(4)
 LOSS_LOCAL_PARAMS = 8
@@ -170,6 +171,12 @@ SIGNATURES = {
     "moge_panorama_lsmr": [vp, vp, ci, ci, vp, vp, vp, vp, sz, vp],
     "moge_panorama_resize": [vp, ci, ci, ci, ci, vp, vp],
     "moge_panorama_finish": [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp],
+    "moge_panorama_split_batch": [vp, ci, ci, ci, pc, ci, vp, ci, vp, vp, vp],
+    "moge_panorama_workspace_bytes_batch": [ci, ci, ci, ci, C.POINTER(sz)],
+    "moge_panorama_rhs_batch": [vp, ci, vp, ci, ci, ci, ci, pc, vp, ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_panorama_lsmr_batch": [vp, vp, ci, ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_panorama_resize_batch": [vp, ci, ci, ci, ci, ci, vp, vp],
+    "moge_panorama_finish_batch": [vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp],
     "moge_loss_workspace_bytes": [i64, ci, ci, C.POINTER(sz)],
     "moge_loss_mask": [ci, vp, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp],
     "moge_loss_stencil": [ci, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp],

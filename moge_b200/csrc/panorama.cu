@@ -14,8 +14,11 @@
 //
 // lsmr: SciPy's LSMR (scipy/sparse/linalg/_isolve/lsmr.py) on that stencil system in one cooperative kernel: grid-wide barriers
 // between the matrix products, fp64 u, v, h, hbar, x stored in fp64 but rounded to fp32 after each update when the level starts
-// from an initial guess (SciPy keeps x0's dtype), and the scalar recurrences and stopping rules evaluated identically by every
-// thread from deterministic reductions.  The iteration count and istop are written to the device.
+// from an initial guess (SciPy keeps x0's dtype), and the scalar recurrences and stopping rules evaluated from deterministic
+// reductions.  The iteration count and istop are written to the device.  One launch solves the
+// systems of a batch of panoramas, each bitwise as alone (see lsmr_kernel); a single merge is a batch of one.
+//
+// The *_batch kernels run the per-pixel bodies of the single-panorama kernels over a leading batch dimension.
 #include "host_api.h"
 #include "../../include/moge_b200.h"
 #include <cooperative_groups.h>
@@ -45,44 +48,60 @@ __device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b)
 __device__ __forceinline__ int q32(float x) { return __float2int_rn(fmul(x, 32.f)); }
 
 // ---------------------------------------------------------------------------------------------------- split
+// view pixel idx of one panorama: out (views, 3, res, res), out_u8 (views, res, res, 3) or null
+__device__ __forceinline__ void split_pixel(const uint8_t* __restrict__ img, int H, int W, const Cams& cams, const float* __restrict__ grid,
+                                            int res, float* __restrict__ out, uint8_t* __restrict__ out_u8, int64_t idx) {
+    const int k = static_cast<int>(idx / (static_cast<int64_t>(res) * res));
+    const int pix = static_cast<int>(idx % (static_cast<int64_t>(res) * res)), i = pix / res, j = pix % res;
+    const moge_panorama_camera_t& c = cams.c[k];
+    // unproject_cv(uv, 1): ((u - cx) / fx, (v - cy) / fy, 1), then R^T (p - t)
+    const double p0 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[j]), c.cx), c.fx), static_cast<double>(c.t[0]));
+    const double p1 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[i]), c.cy), c.fy), static_cast<double>(c.t[1]));
+    const double p2 = dsub(1.0, static_cast<double>(c.t[2]));
+    double d[3];
+    for (int r = 0; r < 3; ++r)
+        d[r] = dadd(dadd(dmul(c.R[r], p0), dmul(c.R[3 + r], p1)), dmul(c.R[6 + r], p2));
+    // directions_to_spherical_uv
+    const double nrm = sqrt(dadd(dadd(dmul(d[0], d[0]), dmul(d[1], d[1])), dmul(d[2], d[2])));
+    const double x = __ddiv_rn(d[0], nrm), y = __ddiv_rn(d[1], nrm), z = __ddiv_rn(d[2], nrm);
+    double a = __ddiv_rn(atan2(y, x), 6.283185307179586), m = fmod(a, 1.0);
+    if (m != 0.0) { if (m < 0) m = dadd(m, 1.0); } else m = 0.0;         // numpy's floor-mod: sign of the divisor
+    const double u = dsub(1.0, m), v = __ddiv_rn(acos(z), 3.141592653589793);
+    // uv_to_pixel, fp32, cv2 fixed point
+    const int X = q32(__double2float_rn(dsub(dmul(u, static_cast<double>(W)), 0.5)));
+    const int Y = q32(__double2float_rn(dsub(dmul(v, static_cast<double>(H)), 0.5)));
+    const int ix = X >> 5, iy = Y >> 5, fx = X & 31, fy = Y & 31;
+    const int w[4] = {(32 - fx) * (32 - fy) * 32, fx * (32 - fy) * 32, (32 - fx) * fy * 32, fx * fy * 32};
+    int acc[3] = {0, 0, 0};
+    for (int t = 0; t < 4; ++t) {
+        const int yy = iy + (t >> 1), xx = ix + (t & 1);
+        if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;        // BORDER_CONSTANT 0
+        const uint8_t* s = img + (static_cast<int64_t>(yy) * W + xx) * 3;
+        for (int ch = 0; ch < 3; ++ch) acc[ch] += w[t] * s[ch];
+    }
+    for (int ch = 0; ch < 3; ++ch) {
+        const int val = min(255, max(0, (acc[ch] + (1 << 14)) >> 15));
+        out[((static_cast<int64_t>(k) * 3 + ch) * res + i) * res + j] = __double2float_rn(static_cast<double>(val) / 255.0);
+        if (out_u8) out_u8[idx * 3 + ch] = static_cast<uint8_t>(val);
+    }
+}
+
 __global__ void __launch_bounds__(kThreads) split_kernel(const uint8_t* __restrict__ img, int H, int W, const Cams cams,
                                                          const float* __restrict__ grid, int res, float* __restrict__ out,
                                                          uint8_t* __restrict__ out_u8) {
     const int64_t total = static_cast<int64_t>(cams.n) * res * res;
+    for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total; idx += static_cast<int64_t>(gridDim.x) * blockDim.x)
+        split_pixel(img, H, W, cams, grid, res, out, out_u8, idx);
+}
+
+// split_kernel over `batch` panoramas of H x W: images (batch, H, W, 3), out (batch * views, 3, res, res)
+__global__ void __launch_bounds__(kThreads) split_batch_kernel(const uint8_t* __restrict__ img, int batch, int H, int W, const Cams cams,
+                                                               const float* __restrict__ grid, int res, float* __restrict__ out,
+                                                               uint8_t* __restrict__ out_u8) {
+    const int64_t per = static_cast<int64_t>(cams.n) * res * res, total = per * batch;
     for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total; idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int k = static_cast<int>(idx / (static_cast<int64_t>(res) * res));
-        const int pix = static_cast<int>(idx % (static_cast<int64_t>(res) * res)), i = pix / res, j = pix % res;
-        const moge_panorama_camera_t& c = cams.c[k];
-        // unproject_cv(uv, 1): ((u - cx) / fx, (v - cy) / fy, 1), then R^T (p - t)
-        const double p0 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[j]), c.cx), c.fx), static_cast<double>(c.t[0]));
-        const double p1 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[i]), c.cy), c.fy), static_cast<double>(c.t[1]));
-        const double p2 = dsub(1.0, static_cast<double>(c.t[2]));
-        double d[3];
-        for (int r = 0; r < 3; ++r)
-            d[r] = dadd(dadd(dmul(c.R[r], p0), dmul(c.R[3 + r], p1)), dmul(c.R[6 + r], p2));
-        // directions_to_spherical_uv
-        const double nrm = sqrt(dadd(dadd(dmul(d[0], d[0]), dmul(d[1], d[1])), dmul(d[2], d[2])));
-        const double x = __ddiv_rn(d[0], nrm), y = __ddiv_rn(d[1], nrm), z = __ddiv_rn(d[2], nrm);
-        double a = __ddiv_rn(atan2(y, x), 6.283185307179586), m = fmod(a, 1.0);
-        if (m != 0.0) { if (m < 0) m = dadd(m, 1.0); } else m = 0.0;         // numpy's floor-mod: sign of the divisor
-        const double u = dsub(1.0, m), v = __ddiv_rn(acos(z), 3.141592653589793);
-        // uv_to_pixel, fp32, cv2 fixed point
-        const int X = q32(__double2float_rn(dsub(dmul(u, static_cast<double>(W)), 0.5)));
-        const int Y = q32(__double2float_rn(dsub(dmul(v, static_cast<double>(H)), 0.5)));
-        const int ix = X >> 5, iy = Y >> 5, fx = X & 31, fy = Y & 31;
-        const int w[4] = {(32 - fx) * (32 - fy) * 32, fx * (32 - fy) * 32, (32 - fx) * fy * 32, fx * fy * 32};
-        int acc[3] = {0, 0, 0};
-        for (int t = 0; t < 4; ++t) {
-            const int yy = iy + (t >> 1), xx = ix + (t & 1);
-            if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;        // BORDER_CONSTANT 0
-            const uint8_t* s = img + (static_cast<int64_t>(yy) * W + xx) * 3;
-            for (int ch = 0; ch < 3; ++ch) acc[ch] += w[t] * s[ch];
-        }
-        for (int ch = 0; ch < 3; ++ch) {
-            const int val = min(255, max(0, (acc[ch] + (1 << 14)) >> 15));
-            out[((static_cast<int64_t>(k) * 3 + ch) * res + i) * res + j] = __double2float_rn(static_cast<double>(val) / 255.0);
-            if (out_u8) out_u8[idx * 3 + ch] = static_cast<uint8_t>(val);
-        }
+        const int64_t q = idx / per;
+        split_pixel(img + q * H * W * 3, H, W, cams, grid, res, out + q * per * 3, out_u8 ? out_u8 + q * per * 3 : nullptr, idx - q * per);
     }
 }
 
@@ -93,125 +112,128 @@ __device__ __forceinline__ float log_distance(const float* __restrict__ src, int
     return logf(sqrtf(fadd(fadd(fmul(p[0], p[0]), fmul(p[1], p[1])), fmul(p[2], p[2]))));
 }
 
-// grid over panorama pixels: per view, the sampled log-distance (0 outside the view) and mask
+// panorama pixel p of one merge: per view, the sampled log-distance (0 outside the view) and mask
+__device__ __forceinline__ void sample_pixel(const float* __restrict__ src, int channels, const uint8_t* __restrict__ vmask, int vh, int vw,
+                                             const Cams& cams, const float* __restrict__ dirs, int64_t n, float* __restrict__ L,
+                                             uint8_t* __restrict__ M, int64_t p) {
+    const float d0 = dirs[p * 3], d1 = dirs[p * 3 + 1], d2 = dirs[p * 3 + 2];
+    for (int k = 0; k < cams.n; ++k) {
+        const moge_panorama_camera_t& c = cams.c[k];
+        float q[3];
+        for (int r = 0; r < 3; ++r) q[r] = fadd(fadd(fadd(fmul(c.R[3 * r], d0), fmul(c.R[3 * r + 1], d1)), fmul(c.R[3 * r + 2], d2)), c.t[r]);
+        const double X = q[0], Y = q[1], Z = q[2];
+        double u = __ddiv_rn(dadd(dmul(c.fx, X), dmul(c.cx, Z)), Z), v = __ddiv_rn(dadd(dmul(c.fy, Y), dmul(c.cy, Z)), Z);
+        const bool valid = q[2] > 0.f && u > 0.0 && v > 0.0 && u < 1.0 && v < 1.0;
+        u = fmin(fmax(u, 0.0), 1.0);
+        v = fmin(fmax(v, 0.0), 1.0);
+        const float px = __double2float_rn(dsub(dmul(u, static_cast<double>(vw)), 0.5));
+        const float py = __double2float_rn(dsub(dmul(v, static_cast<double>(vh)), 0.5));
+        const int64_t base = static_cast<int64_t>(k) * vh * vw;
+        float val = 0.f;
+        uint8_t m = 0;
+        if (valid) {
+            const int Xq = q32(px), Yq = q32(py), ix = Xq >> 5, iy = Yq >> 5;
+            const float ax = static_cast<float>(Xq & 31) / 32.f, ay = static_cast<float>(Yq & 31) / 32.f;
+            const float wx[2] = {1.f - ax, ax}, wy[2] = {1.f - ay, ay};
+            float acc = 0.f;
+            for (int t = 0; t < 4; ++t) {
+                const int yy = min(max(iy + (t >> 1), 0), vh - 1), xx = min(max(ix + (t & 1), 0), vw - 1);
+                acc = fadd(acc, fmul(fmul(wy[t >> 1], wx[t & 1]), log_distance(src, channels, base + static_cast<int64_t>(yy) * vw + xx)));
+            }
+            val = acc;
+            const int nx = min(max(__float2int_rn(px), 0), vw - 1), ny = min(max(__float2int_rn(py), 0), vh - 1);
+            m = vmask[base + static_cast<int64_t>(ny) * vw + nx] != 0;
+        }
+        L[k * n + p] = val;
+        M[k * n + p] = m;
+    }
+}
+
 __global__ void __launch_bounds__(kThreads) sample_kernel(const float* __restrict__ src, int channels, const uint8_t* __restrict__ vmask,
                                                           int vh, int vw, const Cams cams, const float* __restrict__ dirs, int h, int w,
                                                           float* __restrict__ L, uint8_t* __restrict__ M) {
     const int64_t n = static_cast<int64_t>(h) * w;
-    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const float d0 = dirs[p * 3], d1 = dirs[p * 3 + 1], d2 = dirs[p * 3 + 2];
-        for (int k = 0; k < cams.n; ++k) {
-            const moge_panorama_camera_t& c = cams.c[k];
-            float q[3];
-            for (int r = 0; r < 3; ++r) q[r] = fadd(fadd(fadd(fmul(c.R[3 * r], d0), fmul(c.R[3 * r + 1], d1)), fmul(c.R[3 * r + 2], d2)), c.t[r]);
-            const double X = q[0], Y = q[1], Z = q[2];
-            double u = __ddiv_rn(dadd(dmul(c.fx, X), dmul(c.cx, Z)), Z), v = __ddiv_rn(dadd(dmul(c.fy, Y), dmul(c.cy, Z)), Z);
-            const bool valid = q[2] > 0.f && u > 0.0 && v > 0.0 && u < 1.0 && v < 1.0;
-            u = fmin(fmax(u, 0.0), 1.0);
-            v = fmin(fmax(v, 0.0), 1.0);
-            const float px = __double2float_rn(dsub(dmul(u, static_cast<double>(vw)), 0.5));
-            const float py = __double2float_rn(dsub(dmul(v, static_cast<double>(vh)), 0.5));
-            const int64_t base = static_cast<int64_t>(k) * vh * vw;
-            float val = 0.f;
-            uint8_t m = 0;
-            if (valid) {
-                const int Xq = q32(px), Yq = q32(py), ix = Xq >> 5, iy = Yq >> 5;
-                const float ax = static_cast<float>(Xq & 31) / 32.f, ay = static_cast<float>(Yq & 31) / 32.f;
-                const float wx[2] = {1.f - ax, ax}, wy[2] = {1.f - ay, ay};
-                float acc = 0.f;
-                for (int t = 0; t < 4; ++t) {
-                    const int yy = min(max(iy + (t >> 1), 0), vh - 1), xx = min(max(ix + (t & 1), 0), vw - 1);
-                    acc = fadd(acc, fmul(fmul(wy[t >> 1], wx[t & 1]), log_distance(src, channels, base + static_cast<int64_t>(yy) * vw + xx)));
-                }
-                val = acc;
-                const int nx = min(max(__float2int_rn(px), 0), vw - 1), ny = min(max(__float2int_rn(py), 0), vh - 1);
-                m = vmask[base + static_cast<int64_t>(ny) * vw + nx] != 0;
-            }
-            L[k * n + p] = val;
-            M[k * n + p] = m;
-        }
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
+        sample_pixel(src, channels, vmask, vh, vw, cams, dirs, n, L, M, p);
+}
+
+// sample_kernel over `batch` merges: src (batch, views, vh, vw, channels), vmask (batch, views, vh, vw), L and M (batch, views, h, w)
+__global__ void __launch_bounds__(kThreads) sample_batch_kernel(const float* __restrict__ src, int channels, const uint8_t* __restrict__ vmask,
+                                                                int batch, int vh, int vw, const Cams cams, const float* __restrict__ dirs,
+                                                                int h, int w, float* __restrict__ L, uint8_t* __restrict__ M) {
+    const int64_t n = static_cast<int64_t>(h) * w, views = static_cast<int64_t>(cams.n) * vh * vw;
+    for (int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; t < n * batch; t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int64_t q = t / n;
+        sample_pixel(src + q * views * channels, channels, vmask + q * views, vh, vw, cams, dirs, n, L + q * cams.n * n, M + q * cams.n * n, t - q * n);
     }
+}
+
+// panorama pixel p of one merge: its rows of b and row_mask (see the header) and pano_mask
+__device__ __forceinline__ void rhs_pixel(const float* __restrict__ L, const uint8_t* __restrict__ M, int views, int h, int w, int64_t n,
+                                          double* __restrict__ b, uint8_t* __restrict__ rm, uint8_t* __restrict__ pmask, int64_t p) {
+    const int i = static_cast<int>(p / w), j = static_cast<int>(p % w);
+    const int64_t pr = i * static_cast<int64_t>(w) + (j + 1) % w, pl = i * static_cast<int64_t>(w) + (j + w - 1) % w;
+    const int64_t pu = static_cast<int64_t>(max(i - 1, 0)) * w + j, pd = static_cast<int64_t>(min(i + 1, h - 1)) * w + j;
+    float sx = 0.f, sy = 0.f, sl = 0.f;
+    int cx = 0, cy = 0, cl = 0, any = 0;
+    for (int k = 0; k < views; ++k) {
+        const float* Lk = L + k * n;
+        const uint8_t* Mk = M + k * n;
+        const float c = Lk[p];
+        const int mc = Mk[p], mr = Mk[pr];
+        any |= mc;
+        const int mx = mc & mr;
+        const float gx = fmul(__fsub_rn(c, Lk[pr]), static_cast<float>(mx));
+        sx = k ? fadd(sx, gx) : gx;
+        cx += mx;
+        if (i < h - 1) {
+            const int my = mc & Mk[p + w];
+            const float gy = fmul(__fsub_rn(c, Lk[p + w]), static_cast<float>(my));
+            sy = k ? fadd(sy, gy) : gy;
+            cy += my;
+        }
+        // scipy.ndimage.convolve of the edge / wrap padded map: fp64 taps in footprint order, rounded to fp32
+        const double lap = dadd(dadd(dadd(dadd(static_cast<double>(Lk[pu]), static_cast<double>(Lk[pl])), -4.0 * static_cast<double>(c)),
+                                     static_cast<double>(Lk[pr])), static_cast<double>(Lk[pd]));
+        const int ml = mc & Mk[pu] & Mk[pd] & Mk[pl] & mr;
+        const float gl = fmul(__double2float_rn(lap), static_cast<float>(ml));
+        sl = k ? fadd(sl, gl) : gl;
+        cl += ml;
+    }
+    b[p] = cx ? __ddiv_rn(static_cast<double>(sx), static_cast<double>(cx)) : 0.0;
+    rm[p] = cx > 0;
+    if (i < h - 1) {
+        const double by = cy ? __ddiv_rn(static_cast<double>(sy), static_cast<double>(cy)) : 0.0;
+        const int64_t e = n + static_cast<int64_t>(i) * (w + 1) + j;
+        b[e] = by;
+        rm[e] = cy > 0;
+        if (j == 0) { b[e + w] = by; rm[e + w] = cy > 0; }
+    }
+    const int64_t lo = n + static_cast<int64_t>(h - 1) * (w + 1);
+    b[lo + p] = cl ? __ddiv_rn(static_cast<double>(sl), static_cast<double>(cl)) : 0.0;
+    rm[lo + p] = cl > 0;
+    pmask[p] = any;
 }
 
 __global__ void __launch_bounds__(kThreads) rhs_kernel(const float* __restrict__ L, const uint8_t* __restrict__ M, int views, int h, int w,
                                                        double* __restrict__ b, uint8_t* __restrict__ rm, uint8_t* __restrict__ pmask) {
     const int64_t n = static_cast<int64_t>(h) * w;
-    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int i = static_cast<int>(p / w), j = static_cast<int>(p % w);
-        const int64_t pr = i * static_cast<int64_t>(w) + (j + 1) % w, pl = i * static_cast<int64_t>(w) + (j + w - 1) % w;
-        const int64_t pu = static_cast<int64_t>(max(i - 1, 0)) * w + j, pd = static_cast<int64_t>(min(i + 1, h - 1)) * w + j;
-        float sx = 0.f, sy = 0.f, sl = 0.f;
-        int cx = 0, cy = 0, cl = 0, any = 0;
-        for (int k = 0; k < views; ++k) {
-            const float* Lk = L + k * n;
-            const uint8_t* Mk = M + k * n;
-            const float c = Lk[p];
-            const int mc = Mk[p], mr = Mk[pr];
-            any |= mc;
-            const int mx = mc & mr;
-            const float gx = fmul(__fsub_rn(c, Lk[pr]), static_cast<float>(mx));
-            sx = k ? fadd(sx, gx) : gx;
-            cx += mx;
-            if (i < h - 1) {
-                const int my = mc & Mk[p + w];
-                const float gy = fmul(__fsub_rn(c, Lk[p + w]), static_cast<float>(my));
-                sy = k ? fadd(sy, gy) : gy;
-                cy += my;
-            }
-            // scipy.ndimage.convolve of the edge / wrap padded map: fp64 taps in footprint order, rounded to fp32
-            const double lap = dadd(dadd(dadd(dadd(static_cast<double>(Lk[pu]), static_cast<double>(Lk[pl])), -4.0 * static_cast<double>(c)),
-                                         static_cast<double>(Lk[pr])), static_cast<double>(Lk[pd]));
-            const int ml = mc & Mk[pu] & Mk[pd] & Mk[pl] & mr;
-            const float gl = fmul(__double2float_rn(lap), static_cast<float>(ml));
-            sl = k ? fadd(sl, gl) : gl;
-            cl += ml;
-        }
-        b[p] = cx ? __ddiv_rn(static_cast<double>(sx), static_cast<double>(cx)) : 0.0;
-        rm[p] = cx > 0;
-        if (i < h - 1) {
-            const double by = cy ? __ddiv_rn(static_cast<double>(sy), static_cast<double>(cy)) : 0.0;
-            const int64_t e = n + static_cast<int64_t>(i) * (w + 1) + j;
-            b[e] = by;
-            rm[e] = cy > 0;
-            if (j == 0) { b[e + w] = by; rm[e + w] = cy > 0; }
-        }
-        const int64_t lo = n + static_cast<int64_t>(h - 1) * (w + 1);
-        b[lo + p] = cl ? __ddiv_rn(static_cast<double>(sl), static_cast<double>(cl)) : 0.0;
-        rm[lo + p] = cl > 0;
-        pmask[p] = any;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
+        rhs_pixel(L, M, views, h, w, n, b, rm, pmask, p);
+}
+
+// rhs_kernel over `batch` merges: L and M (batch, views, h, w), b and rm (batch, rows), pmask (batch, h, w)
+__global__ void __launch_bounds__(kThreads) rhs_batch_kernel(const float* __restrict__ L, const uint8_t* __restrict__ M, int batch, int views,
+                                                             int h, int w, double* __restrict__ b, uint8_t* __restrict__ rm,
+                                                             uint8_t* __restrict__ pmask) {
+    const int64_t n = static_cast<int64_t>(h) * w, rows = 2 * n + static_cast<int64_t>(h - 1) * (w + 1);
+    for (int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; t < n * batch; t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int64_t q = t / n;
+        rhs_pixel(L + q * views * n, M + q * views * n, views, h, w, n, b + q * rows, rm + q * rows, pmask + q * n, t - q * n);
     }
 }
 
 // ---------------------------------------------------------------------------------------------------- LSMR
-struct Lsmr {
-    const double* b; const uint8_t* rm; const float* init;
-    double *u, *v, *hv, *hb, *x, *part;        // part: 2 buffers x gridDim.x x 2 doubles
-    float* depth; int32_t* stats;
-    int h, w;
-};
-
-// deterministic grid-wide sum of two values: block tree, then every thread sums the block partials in the same order
-__device__ double2 grid_sum2(double a, double c, double* part, int buf, cg::grid_group& g) {
-    __shared__ double2 red[kLsmrThreads / 32];
-    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (lane == 0) red[warp] = make_double2(a, c);
-    __syncthreads();
-    double* P = part + static_cast<int64_t>(buf) * gridDim.x * 2;
-    if (threadIdx.x == 0) {
-        double s = 0, t = 0;
-        for (int k = 0; k < kLsmrThreads / 32; ++k) { s += red[k].x; t += red[k].y; }
-        P[blockIdx.x * 2] = s;
-        P[blockIdx.x * 2 + 1] = t;
-    }
-    g.sync();
-    double s = 0, t = 0;
-    for (int k = lane; k < static_cast<int>(gridDim.x); k += 32) { s += __ldcg(P + k * 2); t += __ldcg(P + k * 2 + 1); }
-    for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); t += __shfl_xor_sync(0xffffffffu, t, o); }
-    __syncthreads();
-    return make_double2(s, t);
-}
-
 __device__ __forceinline__ double sgn(double a) { return a > 0 ? 1.0 : (a < 0 ? -1.0 : 0.0); }
 __device__ void sym_ortho(double a, double b, double* c, double* s, double* r) {
     if (b == 0) { *c = sgn(a); *s = 0; *r = fabs(a); }
@@ -264,158 +286,297 @@ __device__ __forceinline__ int pixel_rows(int64_t p, int i, int j, int h, int w,
     return c;
 }
 
+// P independent systems of one level size in one cooperative launch, sharing each iteration's four grid barriers (the single
+// merge is P = 1).  A system's reductions do not depend on P: its pixels are split over `vblocks` virtual blocks of 512 threads,
+// one per SM (at most ceil(n / 512)): virtual block k, thread t takes pixels k * 512 + t, stepping by vblocks * 512, reduces them
+// with a warp-shuffle and block tree to the block's partial, and the partials are summed in virtual-block order.  The P * vblocks
+// virtual blocks are dealt to the real blocks in contiguous runs of per_block, so a real block serves at most kMaxLocal systems
+// (the host checks it) and evaluates each one's scalar recurrences once, in shared memory.  A system that stops keeps its x and
+// stats and does no more work; the launch ends when every system has stopped.
+constexpr int kMaxLocal = 4;
+
+struct Lsmr {
+    const double* b; const uint8_t* rm; const float* init;     // b, rm (batch, rows); init (batch, n) = log(init) or null
+    double *u, *v, *hv, *hb, *x, *part;        // u (batch, rows); v, hv, hb, x (batch, n); part: 2 buffers x batch * vblocks x 2
+    float* depth; int32_t* stats; int* stop;   // depth (batch, n), stats (batch, 2); stop (batch): the system has stopped
+    int h, w, batch, vblocks, per_block;
+};
+
+// one system's scalars: SciPy's lsmr locals, and the tests that do not depend on normx
+struct LsmrScalars {
+    double normb, maxiter, alpha, beta, zetabar, alphabar, rho, rhobar, cbar, sbar, betadd, betad, rhodold, tautildeold, thetatilde;
+    double zeta, d, normA2, maxrbar, minrbar, normar, c1, c2, c3, normA, test1, test2, test3;
+    int itn, istop;
+    bool done, zero_x;
+};
+
+// the block tree of one virtual block: its partial sums of (a, c) to P[0], P[1]
+__device__ void block_partial(double a, double c, double* P) {
+    __shared__ double2 red[kLsmrThreads / 32];
+    for (int o = 16; o > 0; o >>= 1) { a += __shfl_xor_sync(0xffffffffu, a, o); c += __shfl_xor_sync(0xffffffffu, c, o); }
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) red[warp] = make_double2(a, c);
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s = 0, t = 0;
+        for (int k = 0; k < kLsmrThreads / 32; ++k) { s += red[k].x; t += red[k].y; }
+        P[0] = s;
+        P[1] = t;
+    }
+    __syncthreads();
+}
+
+// after the barrier: the sum of the `count` partials at P in order (lane-strided, then a warp tree), in every lane of the warp
+__device__ double2 partial_sum(const double* P, int count) {
+    const int lane = threadIdx.x & 31;
+    double s = 0, t = 0;
+    for (int k = lane; k < count; k += 32) { s += __ldcg(P + k * 2); t += __ldcg(P + k * 2 + 1); }
+    for (int o = 16; o > 0; o >>= 1) { s += __shfl_xor_sync(0xffffffffu, s, o); t += __shfl_xor_sync(0xffffffffu, t, o); }
+    return make_double2(s, t);
+}
+
 __global__ void __launch_bounds__(kLsmrThreads) lsmr_kernel(Lsmr a) {
     cg::grid_group g = cg::this_grid();
-    const int h = a.h, w = a.w;
-    const int64_t n = static_cast<int64_t>(h) * w;
-    const int64_t stride = static_cast<int64_t>(gridDim.x) * blockDim.x, first = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x;
+    __shared__ LsmrScalars S[kMaxLocal];
+    const int h = a.h, w = a.w, VB = a.vblocks;
+    const int64_t n = static_cast<int64_t>(h) * w, rows = 2 * n + static_cast<int64_t>(h - 1) * (w + 1);
+    const int64_t stride = static_cast<int64_t>(VB) * kLsmrThreads, items = static_cast<int64_t>(a.batch) * VB;
+    const int i0 = blockIdx.x * a.per_block, i1 = static_cast<int>(min(static_cast<int64_t>(i0 + a.per_block), items));
+    const int s0 = i0 / VB, nloc = (i1 - 1) / VB - s0 + 1;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const bool lead = lane == 0 && warp < nloc;                   // evaluates the scalars of local system `warp`
+    const bool owner = warp < nloc && (s0 + warp) * VB >= i0;     // this block holds that system's virtual block 0
     const bool x32 = a.init != nullptr;
     const double atol = 1e-5, btol = 1e-5, ctol = 1e-8;
     int buf = 0;
-#define FOR_PIXELS for (int64_t p = first; p < n; p += stride)
+    double2 r = make_double2(0, 0);
+#define FOR_ITEMS for (int it = i0; it < i1; ++it)
+#define ITEM                                                                                                                 \
+    const int sy = it / VB, vb = it - sy * VB;                                                                               \
+    [[maybe_unused]] const LsmrScalars& q = S[sy - s0];                                                                      \
+    [[maybe_unused]] const double* b = a.b + sy * rows;                                                                      \
+    [[maybe_unused]] const uint8_t* rm = a.rm + sy * rows;                                                                   \
+    [[maybe_unused]] double *u = a.u + sy * rows, *v = a.v + sy * n, *hv = a.hv + sy * n, *hb = a.hb + sy * n, *x = a.x + sy * n
+#define FOR_PIXELS for (int64_t p = vb * static_cast<int64_t>(kLsmrThreads) + threadIdx.x; p < n; p += stride)
 #define PIXEL_IJ const int i = static_cast<int>(p / w), j = static_cast<int>(p % w)
-    // u = b - A x0 (fp32 product, as SciPy's fp32 csr times an fp32 x0) or u = b; ||b||, rows in use
-    double sb = 0, sm = 0, su = 0;
-    FOR_PIXELS {
-        PIXEL_IJ;
-        float ax = 0, ay = 0, al = 0;
-        if (x32) apply_rows<float>(a.init, p, i, j, h, w, &ax, &ay, &al);          // a.init holds log(init) here (see below)
-        const float av[3] = {ax, ay, al};
-        int64_t es[4];
-        int ks[4];
-        const int nr = pixel_rows(p, i, j, h, w, es, ks);
-        for (int q = 0; q < nr; ++q) {
-            const int64_t e = es[q];
-            const int r = ks[q];
-            const double bb = a.rm[e] ? a.b[e] : 0.0;
-            const double uu = a.rm[e] ? bb - static_cast<double>(av[r]) : 0.0;
-            sb += bb * bb; sm += a.rm[e]; su += uu * uu;
-            a.u[e] = x32 ? uu : bb;
-        }
-        a.x[p] = x32 ? static_cast<double>(a.init[p]) : 0.0;
-        a.hb[p] = 0.0;
-    }
-    double2 r2 = grid_sum2(sb, sm, a.part, buf, g); buf ^= 1;
-    const double normb = sqrt(r2.x);
-    const double maxiter = fmin(r2.y, static_cast<double>(n));
-    double beta = normb;
-    if (x32) { beta = sqrt(grid_sum2(su, 0, a.part, buf, g).x); buf ^= 1; }
-    double alpha = 0;
-    if (beta > 0) {
-        const double ib = 1 / beta;
-        FOR_PIXELS { PIXEL_IJ; int64_t es[4]; int ks[4]; const int nr = pixel_rows(p, i, j, h, w, es, ks); for (int q = 0; q < nr; ++q) a.u[es[q]] = ib * a.u[es[q]]; }
-        g.sync();
-        double sv = 0;
-        FOR_PIXELS { PIXEL_IJ; const double vv = apply_cols(a.u, p, i, j, h, w); a.v[p] = vv; sv += vv * vv; }
-        alpha = sqrt(grid_sum2(sv, 0, a.part, buf, g).x); buf ^= 1;
-    } else {
-        FOR_PIXELS a.v[p] = 0;
-    }
-    {
-        const double ia = alpha > 0 ? 1 / alpha : 1.0;
-        FOR_PIXELS { const double vv = alpha > 0 ? ia * a.v[p] : a.v[p]; a.v[p] = vv; a.hv[p] = vv; }
-        g.sync();
-    }
-    int itn = 0, istop = 0;
-    double zetabar = alpha * beta, alphabar = alpha, rho = 1, rhobar = 1, cbar = 1, sbar = 0;
-    double betadd = beta, betad = 0, rhodold = 1, tautildeold = 0, thetatilde = 0, zeta = 0, d = 0;
-    double normA2 = alpha * alpha, maxrbar = 0, minrbar = 1e100;
-    double normar = alpha * beta;
-    bool done = normar == 0;
-    if (!done && normb == 0) { FOR_PIXELS a.x[p] = 0; done = true; }
-    while (!done && itn < maxiter) {
-        ++itn;
-        // u = -alpha u + A v
-        double s = 0;
+#define PARTIAL(v0, v1) block_partial(v0, v1, a.part + (static_cast<int64_t>(buf) * items + it) * 2)
+#define SUM (r = warp < nloc ? partial_sum(a.part + (static_cast<int64_t>(buf) * items + static_cast<int64_t>(s0 + warp) * VB) * 2, VB) \
+                             : make_double2(0, 0), buf ^= 1)
+    // u = b - A x0 or u = b; ||b||, rows in use; ||u|| (into the other buffer)
+    FOR_ITEMS {
+        ITEM;
+        const float* init = x32 ? a.init + sy * n : nullptr;
+        double sb = 0, sm = 0, su = 0;
         FOR_PIXELS {
             PIXEL_IJ;
-            double ax, ay, al;
-            apply_rows<double>(a.v, p, i, j, h, w, &ax, &ay, &al);
-            const double av[3] = {ax, ay, al};
+            float ax = 0, ay = 0, al = 0;
+            if (x32) apply_rows<float>(init, p, i, j, h, w, &ax, &ay, &al);
+            const float av[3] = {ax, ay, al};
             int64_t es[4];
             int ks[4];
             const int nr = pixel_rows(p, i, j, h, w, es, ks);
-            for (int q = 0; q < nr; ++q) {
-                const int64_t e = es[q];
-                const int r = ks[q];
-                const double uu = a.rm[e] ? dadd(dmul(a.u[e], -alpha), av[r]) : 0.0;
-                a.u[e] = uu;
-                s += uu * uu;
+            for (int k = 0; k < nr; ++k) {
+                const int64_t e = es[k];
+                const double bb = rm[e] ? b[e] : 0.0;
+                const double uu = rm[e] ? bb - static_cast<double>(av[ks[k]]) : 0.0;
+                sb += bb * bb; sm += rm[e]; su += uu * uu;
+                u[e] = x32 ? uu : bb;
+            }
+            x[p] = x32 ? static_cast<double>(init[p]) : 0.0;
+            hb[p] = 0.0;
+        }
+        PARTIAL(sb, sm);
+        buf ^= 1; PARTIAL(su, 0); buf ^= 1;
+    }
+    g.sync();
+    SUM;
+    if (lead) { S[warp].normb = sqrt(r.x); S[warp].maxiter = fmin(r.y, static_cast<double>(n)); S[warp].beta = S[warp].normb; }
+    SUM;
+    if (lead && x32) S[warp].beta = sqrt(r.x);
+    __syncthreads();
+    FOR_ITEMS {
+        ITEM;
+        if (q.beta > 0) {
+            const double ib = 1 / q.beta;
+            FOR_PIXELS { PIXEL_IJ; int64_t es[4]; int ks[4]; const int nr = pixel_rows(p, i, j, h, w, es, ks); for (int k = 0; k < nr; ++k) u[es[k]] = ib * u[es[k]]; }
+        }
+    }
+    g.sync();
+    FOR_ITEMS {
+        ITEM;
+        double sv = 0;
+        if (q.beta > 0) { FOR_PIXELS { PIXEL_IJ; const double vv = apply_cols(u, p, i, j, h, w); v[p] = vv; sv += vv * vv; } }
+        else { FOR_PIXELS v[p] = 0; }
+        PARTIAL(sv, 0);
+    }
+    g.sync();
+    SUM;
+    if (lead) S[warp].alpha = S[warp].beta > 0 ? sqrt(r.x) : 0.0;
+    __syncthreads();
+    FOR_ITEMS {
+        ITEM;
+        const double alpha = q.alpha, ia = alpha > 0 ? 1 / alpha : 1.0;
+        FOR_PIXELS { const double vv = alpha > 0 ? ia * v[p] : v[p]; v[p] = vv; hv[p] = vv; }
+    }
+    if (lead) {
+        LsmrScalars& q = S[warp];
+        const double alpha = q.alpha, beta = q.beta;
+        q.itn = 0; q.istop = 0;
+        q.zetabar = alpha * beta; q.alphabar = alpha; q.rho = 1; q.rhobar = 1; q.cbar = 1; q.sbar = 0;
+        q.betadd = beta; q.betad = 0; q.rhodold = 1; q.tautildeold = 0; q.thetatilde = 0; q.zeta = 0; q.d = 0;
+        q.normA2 = alpha * alpha; q.maxrbar = 0; q.minrbar = 1e100;
+        q.normar = alpha * beta;
+        q.zero_x = q.normar != 0 && q.normb == 0;
+        q.done = q.normar == 0 || q.zero_x || !(q.itn < q.maxiter);
+        if (owner) a.stop[s0 + warp] = q.done;
+    }
+    __syncthreads();
+    FOR_ITEMS { ITEM; if (q.zero_x) { FOR_PIXELS x[p] = 0; } }
+    g.sync();
+    for (;;) {
+        // u = -alpha u + A v
+        FOR_ITEMS {
+            ITEM;
+            double s = 0;
+            if (!q.done) {
+                const double alpha = q.alpha;
+                FOR_PIXELS {
+                    PIXEL_IJ;
+                    double ax, ay, al;
+                    apply_rows<double>(v, p, i, j, h, w, &ax, &ay, &al);
+                    const double av[3] = {ax, ay, al};
+                    int64_t es[4];
+                    int ks[4];
+                    const int nr = pixel_rows(p, i, j, h, w, es, ks);
+                    for (int k = 0; k < nr; ++k) {
+                        const int64_t e = es[k];
+                        const double uu = rm[e] ? dadd(dmul(u[e], -alpha), av[ks[k]]) : 0.0;
+                        u[e] = uu;
+                        s += uu * uu;
+                    }
+                }
+            }
+            PARTIAL(s, 0);
+        }
+        g.sync();
+        SUM;
+        // the stop flags were written before this barrier and are next written after two more
+        bool all = true;
+        for (int k = lane; k < a.batch; k += 32) all = all && __ldcg(a.stop + k) != 0;
+        if (__all_sync(0xffffffffu, all)) break;
+        if (lead && !S[warp].done) { ++S[warp].itn; S[warp].beta = sqrt(r.x); }
+        __syncthreads();
+        FOR_ITEMS {
+            ITEM;
+            if (!q.done && q.beta > 0) {
+                const double ib = 1 / q.beta;
+                FOR_PIXELS { PIXEL_IJ; int64_t es[4]; int ks[4]; const int nr = pixel_rows(p, i, j, h, w, es, ks); for (int k = 0; k < nr; ++k) u[es[k]] = dmul(u[es[k]], ib); }
             }
         }
-        beta = sqrt(grid_sum2(s, 0, a.part, buf, g).x); buf ^= 1;
-        if (beta > 0) {
-            const double ib = 1 / beta;
-            FOR_PIXELS { PIXEL_IJ; int64_t es[4]; int ks[4]; const int nr = pixel_rows(p, i, j, h, w, es, ks); for (int q = 0; q < nr; ++q) a.u[es[q]] = dmul(a.u[es[q]], ib); }
-            g.sync();
+        g.sync();
+        FOR_ITEMS {
+            ITEM;
             double sv = 0;
-            FOR_PIXELS { PIXEL_IJ; const double vv = dadd(dmul(a.v[p], -beta), apply_cols(a.u, p, i, j, h, w)); a.v[p] = vv; sv += vv * vv; }
-            alpha = sqrt(grid_sum2(sv, 0, a.part, buf, g).x); buf ^= 1;
+            if (!q.done && q.beta > 0) {
+                const double beta = q.beta;
+                FOR_PIXELS { PIXEL_IJ; const double vv = dadd(dmul(v[p], -beta), apply_cols(u, p, i, j, h, w)); v[p] = vv; sv += vv * vv; }
+            }
+            PARTIAL(sv, 0);
         }
-        double chat, shat, alphahat, c, sn;
-        sym_ortho(alphabar, 0.0, &chat, &shat, &alphahat);
-        const double rhoold = rho;
-        sym_ortho(alphahat, beta, &c, &sn, &rho);
-        const double thetanew = sn * alpha;
-        alphabar = c * alpha;
-        const double rhobarold = rhobar, zetaold = zeta, thetabar = sbar * rho, rhotemp = cbar * rho;
-        sym_ortho(cbar * rho, thetanew, &cbar, &sbar, &rhobar);
-        zeta = cbar * zetabar;
-        zetabar = -sbar * zetabar;
-        const double c1 = -(thetabar * rho / (rhoold * rhobarold)), c2 = zeta / (rho * rhobar), c3 = -(thetanew / rho);
-        const bool scale_v = beta > 0 && alpha > 0;
-        const double ia = scale_v ? 1 / alpha : 1.0;
-        double sx = 0;
-        FOR_PIXELS {
-            const double vv = scale_v ? dmul(a.v[p], ia) : a.v[p];
-            a.v[p] = vv;
-            const double hb = dadd(dmul(a.hb[p], c1), a.hv[p]);
-            a.hb[p] = hb;
-            double xx = dadd(a.x[p], dmul(c2, hb));
-            if (x32) xx = static_cast<double>(__double2float_rn(xx));
-            a.x[p] = xx;
-            sx += xx * xx;
-            a.hv[p] = dadd(dmul(a.hv[p], c3), vv);
+        g.sync();
+        SUM;
+        if (lead && !S[warp].done) {
+            LsmrScalars& q = S[warp];
+            const double beta = q.beta;
+            if (beta > 0) q.alpha = sqrt(r.x);
+            const double alpha = q.alpha;
+            double chat, shat, alphahat, c, sn;
+            sym_ortho(q.alphabar, 0.0, &chat, &shat, &alphahat);
+            const double rhoold = q.rho;
+            sym_ortho(alphahat, beta, &c, &sn, &q.rho);
+            const double rho = q.rho;
+            const double thetanew = sn * alpha;
+            q.alphabar = c * alpha;
+            const double rhobarold = q.rhobar, zetaold = q.zeta, thetabar = q.sbar * rho, rhotemp = q.cbar * rho;
+            sym_ortho(q.cbar * rho, thetanew, &q.cbar, &q.sbar, &q.rhobar);
+            const double rhobar = q.rhobar;
+            q.zeta = q.cbar * q.zetabar;
+            q.zetabar = -q.sbar * q.zetabar;
+            q.c1 = -(thetabar * rho / (rhoold * rhobarold)); q.c2 = q.zeta / (rho * rhobar); q.c3 = -(thetanew / rho);
+            const double betaacute = chat * q.betadd, betacheck = -shat * q.betadd, betahat = c * betaacute;
+            q.betadd = -sn * betaacute;
+            const double thetatildeold = q.thetatilde;
+            double ctildeold, stildeold, rhotildeold;
+            sym_ortho(q.rhodold, thetabar, &ctildeold, &stildeold, &rhotildeold);
+            q.thetatilde = stildeold * rhobar;
+            q.rhodold = ctildeold * rhobar;
+            q.betad = -stildeold * q.betad + ctildeold * betahat;
+            q.tautildeold = (zetaold - thetatildeold * q.tautildeold) / rhotildeold;
+            const double taud = (q.zeta - q.thetatilde * q.tautildeold) / q.rhodold;
+            q.d = q.d + betacheck * betacheck;
+            const double normr = sqrt(q.d + (q.betad - taud) * (q.betad - taud) + q.betadd * q.betadd);
+            q.normA2 = q.normA2 + beta * beta;
+            q.normA = sqrt(q.normA2);
+            q.normA2 = q.normA2 + alpha * alpha;
+            q.maxrbar = fmax(q.maxrbar, rhobarold);
+            if (q.itn > 1) q.minrbar = fmin(q.minrbar, rhobarold);
+            const double condA = fmax(q.maxrbar, rhotemp) / fmin(q.minrbar, rhotemp);
+            q.normar = fabs(q.zetabar);
+            q.test1 = normr / q.normb;
+            q.test2 = (q.normA * normr) != 0 ? q.normar / (q.normA * normr) : INFINITY;
+            q.test3 = 1 / condA;
         }
-        double normx = sqrt(grid_sum2(sx, 0, a.part, buf, g).x); buf ^= 1;
-        if (x32) normx = static_cast<double>(static_cast<float>(normx));
-        const double betaacute = chat * betadd, betacheck = -shat * betadd, betahat = c * betaacute;
-        betadd = -sn * betaacute;
-        const double thetatildeold = thetatilde;
-        double ctildeold, stildeold, rhotildeold;
-        sym_ortho(rhodold, thetabar, &ctildeold, &stildeold, &rhotildeold);
-        thetatilde = stildeold * rhobar;
-        rhodold = ctildeold * rhobar;
-        betad = -stildeold * betad + ctildeold * betahat;
-        tautildeold = (zetaold - thetatildeold * tautildeold) / rhotildeold;
-        const double taud = (zeta - thetatilde * tautildeold) / rhodold;
-        d = d + betacheck * betacheck;
-        const double normr = sqrt(d + (betad - taud) * (betad - taud) + betadd * betadd);
-        normA2 = normA2 + beta * beta;
-        const double normA = sqrt(normA2);
-        normA2 = normA2 + alpha * alpha;
-        maxrbar = fmax(maxrbar, rhobarold);
-        if (itn > 1) minrbar = fmin(minrbar, rhobarold);
-        const double condA = fmax(maxrbar, rhotemp) / fmin(minrbar, rhotemp);
-        normar = fabs(zetabar);
-        const double test1 = normr / normb;
-        const double test2 = (normA * normr) != 0 ? normar / (normA * normr) : INFINITY;
-        const double test3 = 1 / condA;
-        const double t1 = test1 / (1 + normA * normx / normb);
-        const double rtol = btol + atol * normA * normx / normb;
-        if (itn >= maxiter) istop = 7;
-        if (1 + test3 <= 1) istop = 6;
-        if (1 + test2 <= 1) istop = 5;
-        if (1 + t1 <= 1) istop = 4;
-        if (test3 <= ctol) istop = 3;
-        if (test2 <= atol) istop = 2;
-        if (test1 <= rtol) istop = 1;
-        if (istop > 0) break;
+        __syncthreads();
+        FOR_ITEMS {
+            ITEM;
+            double sx = 0;
+            if (!q.done) {
+                const bool scale_v = q.beta > 0 && q.alpha > 0;
+                const double ia = scale_v ? 1 / q.alpha : 1.0, c1 = q.c1, c2 = q.c2, c3 = q.c3;
+                FOR_PIXELS {
+                    const double vv = scale_v ? dmul(v[p], ia) : v[p];
+                    v[p] = vv;
+                    const double hbv = dadd(dmul(hb[p], c1), hv[p]);
+                    hb[p] = hbv;
+                    double xx = dadd(x[p], dmul(c2, hbv));
+                    if (x32) xx = static_cast<double>(__double2float_rn(xx));
+                    x[p] = xx;
+                    sx += xx * xx;
+                    hv[p] = dadd(dmul(hv[p], c3), vv);
+                }
+            }
+            PARTIAL(sx, 0);
+        }
+        g.sync();
+        SUM;
+        if (lead && !S[warp].done) {
+            LsmrScalars& q = S[warp];
+            double normx = sqrt(r.x);
+            if (x32) normx = static_cast<double>(static_cast<float>(normx));
+            const double t1 = q.test1 / (1 + q.normA * normx / q.normb);
+            const double rtol = btol + atol * q.normA * normx / q.normb;
+            int istop = 0;
+            if (q.itn >= q.maxiter) istop = 7;
+            if (1 + q.test3 <= 1) istop = 6;
+            if (1 + q.test2 <= 1) istop = 5;
+            if (1 + t1 <= 1) istop = 4;
+            if (q.test3 <= ctol) istop = 3;
+            if (q.test2 <= atol) istop = 2;
+            if (q.test1 <= rtol) istop = 1;
+            q.istop = istop;
+            q.done = istop > 0 || !(q.itn < q.maxiter);
+            if (owner) a.stop[s0 + warp] = q.done;
+        }
+        __syncthreads();
     }
-    FOR_PIXELS a.depth[p] = x32 ? expf(static_cast<float>(a.x[p])) : __double2float_rn(exp(a.x[p]));
-    if (first == 0) { a.stats[0] = itn; a.stats[1] = istop; }
+    FOR_ITEMS { ITEM; float* depth = a.depth + sy * n; FOR_PIXELS depth[p] = x32 ? expf(static_cast<float>(x[p])) : __double2float_rn(exp(x[p])); }
+    if (lead && owner) { a.stats[(s0 + warp) * 2] = S[warp].itn; a.stats[(s0 + warp) * 2 + 1] = S[warp].istop; }
+#undef FOR_ITEMS
+#undef ITEM
 #undef FOR_PIXELS
 #undef PIXEL_IJ
+#undef PARTIAL
+#undef SUM
 }
 
 __global__ void log_kernel(const float* __restrict__ src, float* __restrict__ dst, int64_t n) {
@@ -434,51 +595,87 @@ __device__ __forceinline__ void lin_coef(int d, int in, int out, int* s0, int* s
     *s0 = sx; *s1 = min(sx + 1, in - 1); *f = fx;
 }
 
+// output pixel p of one map
+__device__ __forceinline__ void resize_pixel(const float* __restrict__ src, int h, int w, int H, int W, float* __restrict__ dst, int64_t p) {
+    const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
+    int x0, x1, y0, y1;
+    float fx, fy;
+    lin_coef(j, w, W, &x0, &x1, &fx);
+    lin_coef(i, h, H, &y0, &y1, &fy);
+    const float* r0 = src + static_cast<int64_t>(y0) * w;
+    const float* r1 = src + static_cast<int64_t>(y1) * w;
+    const float a0 = 1.f - fx, b0 = 1.f - fy;
+    const float h0 = fadd(fmul(r0[x0], a0), fmul(r0[x1], fx)), h1 = fadd(fmul(r1[x0], a0), fmul(r1[x1], fx));
+    dst[p] = fadd(fmul(h0, b0), fmul(h1, fy));
+}
+
 __global__ void __launch_bounds__(kThreads) resize_kernel(const float* __restrict__ src, int h, int w, int H, int W, float* __restrict__ dst) {
     const int64_t n = static_cast<int64_t>(H) * W;
-    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
-        int x0, x1, y0, y1;
-        float fx, fy;
-        lin_coef(j, w, W, &x0, &x1, &fx);
-        lin_coef(i, h, H, &y0, &y1, &fy);
-        const float* r0 = src + static_cast<int64_t>(y0) * w;
-        const float* r1 = src + static_cast<int64_t>(y1) * w;
-        const float a0 = 1.f - fx, b0 = 1.f - fy;
-        const float h0 = fadd(fmul(r0[x0], a0), fmul(r0[x1], fx)), h1 = fadd(fmul(r1[x0], a0), fmul(r1[x1], fx));
-        dst[p] = fadd(fmul(h0, b0), fmul(h1, fy));
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
+        resize_pixel(src, h, w, H, W, dst, p);
+}
+
+// resize_kernel over `batch` maps: src (batch, h, w), dst (batch, H, W)
+__global__ void __launch_bounds__(kThreads) resize_batch_kernel(const float* __restrict__ src, int batch, int h, int w, int H, int W,
+                                                                float* __restrict__ dst) {
+    const int64_t n = static_cast<int64_t>(H) * W;
+    for (int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; t < n * batch; t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int64_t q = t / n;
+        resize_pixel(src + q * h * w, h, w, H, W, dst + q * n, t - q * n);
     }
 }
 
 // cv2.resize INTER_LINEAR of a 0/1 uint8 mask (11-bit fixed-point coefficients), then > 0; and points = depth * direction
+// output pixel p of one map; su .. stv are uv_map's linspace ends and steps
+__device__ __forceinline__ void finish_pixel(const float* __restrict__ depth, const uint8_t* __restrict__ mask, int h, int w, int H, int W,
+                                             uint8_t* __restrict__ mask_out, float* __restrict__ points, double su, double eu, double sv,
+                                             double ev, double stu, double stv, int64_t p) {
+    const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
+    int x0, x1, y0, y1;
+    float fx, fy;
+    lin_coef(j, w, W, &x0, &x1, &fx);
+    lin_coef(i, h, H, &y0, &y1, &fy);
+    const int a1 = __float2int_rn(fx * 2048.f), a0 = __float2int_rn((1.f - fx) * 2048.f);
+    const int b1 = __float2int_rn(fy * 2048.f), b0 = __float2int_rn((1.f - fy) * 2048.f);
+    const uint8_t* m0 = mask + static_cast<int64_t>(y0) * w;
+    const uint8_t* m1 = mask + static_cast<int64_t>(y1) * w;
+    const int r0 = (m0[x0] != 0) * a0 + (m0[x1] != 0) * a1, r1 = (m1[x0] != 0) * a0 + (m1[x1] != 0) * a1;
+    const int val = (((b0 * (r0 >> 4)) >> 16) + ((b1 * (r1 >> 4)) >> 16) + 2) >> 2;
+    mask_out[p] = val > 0;
+    // uv_map(H, W) (np.linspace in fp64, rounded to fp32) and spherical_uv_to_directions in fp32
+    const float u = j == W - 1 ? __double2float_rn(eu) : __double2float_rn(dadd(dmul(static_cast<double>(j), stu), su));
+    const float v = i == H - 1 ? __double2float_rn(ev) : __double2float_rn(dadd(dmul(static_cast<double>(i), stv), sv));
+    const float theta = fmul(1.f - u, 6.28318530717958647692f), phi = fmul(v, 3.14159265358979323846f);
+    const float sp = sinf(phi), d = depth[p];
+    points[p * 3] = fmul(d, fmul(sp, cosf(theta)));
+    points[p * 3 + 1] = fmul(d, fmul(sp, sinf(theta)));
+    points[p * 3 + 2] = fmul(d, cosf(phi));
+}
+
+#define FINISH_UV                                                                    \
+    const double su = 0.5 / W, eu = 1.0 - 0.5 / W, sv = 0.5 / H, ev = 1.0 - 0.5 / H; \
+    const double stu = W > 1 ? (eu - su) / (W - 1) : 0.0, stv = H > 1 ? (ev - sv) / (H - 1) : 0.0
+
 __global__ void __launch_bounds__(kThreads) finish_kernel(const float* __restrict__ depth, const uint8_t* __restrict__ mask, int h, int w,
                                                           int H, int W, uint8_t* __restrict__ mask_out, float* __restrict__ points) {
     const int64_t n = static_cast<int64_t>(H) * W;
-    const double su = 0.5 / W, eu = 1.0 - 0.5 / W, sv = 0.5 / H, ev = 1.0 - 0.5 / H;
-    const double stu = W > 1 ? (eu - su) / (W - 1) : 0.0, stv = H > 1 ? (ev - sv) / (H - 1) : 0.0;
-    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
-        int x0, x1, y0, y1;
-        float fx, fy;
-        lin_coef(j, w, W, &x0, &x1, &fx);
-        lin_coef(i, h, H, &y0, &y1, &fy);
-        const int a1 = __float2int_rn(fx * 2048.f), a0 = __float2int_rn((1.f - fx) * 2048.f);
-        const int b1 = __float2int_rn(fy * 2048.f), b0 = __float2int_rn((1.f - fy) * 2048.f);
-        const uint8_t* m0 = mask + static_cast<int64_t>(y0) * w;
-        const uint8_t* m1 = mask + static_cast<int64_t>(y1) * w;
-        const int r0 = (m0[x0] != 0) * a0 + (m0[x1] != 0) * a1, r1 = (m1[x0] != 0) * a0 + (m1[x1] != 0) * a1;
-        const int val = (((b0 * (r0 >> 4)) >> 16) + ((b1 * (r1 >> 4)) >> 16) + 2) >> 2;
-        mask_out[p] = val > 0;
-        // uv_map(H, W) (np.linspace in fp64, rounded to fp32) and spherical_uv_to_directions in fp32
-        const float u = j == W - 1 ? __double2float_rn(eu) : __double2float_rn(dadd(dmul(static_cast<double>(j), stu), su));
-        const float v = i == H - 1 ? __double2float_rn(ev) : __double2float_rn(dadd(dmul(static_cast<double>(i), stv), sv));
-        const float theta = fmul(1.f - u, 6.28318530717958647692f), phi = fmul(v, 3.14159265358979323846f);
-        const float sp = sinf(phi), d = depth[p];
-        points[p * 3] = fmul(d, fmul(sp, cosf(theta)));
-        points[p * 3 + 1] = fmul(d, fmul(sp, sinf(theta)));
-        points[p * 3 + 2] = fmul(d, cosf(phi));
+    FINISH_UV;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
+        finish_pixel(depth, mask, h, w, H, W, mask_out, points, su, eu, sv, ev, stu, stv, p);
+}
+
+// finish_kernel over `batch` maps: depth (batch, H, W) (already resized), mask (batch, h, w), mask_out (batch, H, W), points (batch, H, W, 3)
+__global__ void __launch_bounds__(kThreads) finish_batch_kernel(const float* __restrict__ depth, const uint8_t* __restrict__ mask, int batch,
+                                                                int h, int w, int H, int W, uint8_t* __restrict__ mask_out,
+                                                                float* __restrict__ points) {
+    const int64_t n = static_cast<int64_t>(H) * W;
+    FINISH_UV;
+    for (int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; t < n * batch; t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int64_t q = t / n;
+        finish_pixel(depth + q * n, mask + q * h * w, h, w, H, W, mask_out + q * n, points + q * n * 3, su, eu, sv, ev, stu, stv, t - q * n);
     }
 }
+#undef FINISH_UV
 
 // ---------------------------------------------------------------------------------------------------- host side
 int check_size(const char* what, int h, int w) {
@@ -502,24 +699,78 @@ int load_cams(const char* what, const moge_panorama_camera_t* cams, int views, C
 
 unsigned blocks_for(int64_t n, int sms) { return static_cast<unsigned>(std::min<int64_t>((n + kThreads - 1) / kThreads, int64_t(sms) * 16)); }
 
-struct Layout { size_t L, M, u, v, hv, hb, x, part, logi, total; };
-Layout layout(int views, int h, int w, int max_blocks) {
-    const size_t n = static_cast<size_t>(h) * w;
+// the single merge's workspace, or (batch > 0) that of `batch` merges, which adds the batched solver's stop flags
+// the workspace of `batch` merges of up to h x w with `views` views
+struct Layout { size_t L, M, u, v, hv, hb, x, part, logi, stop, total; };
+constexpr int kMaxLsmrBlocks = 132 * 4;            // virtual blocks per system
+Layout layout(int views, int h, int w, int batch = 1) {
+    const size_t n = static_cast<size_t>(h) * w, m = batch;
     WsLayout ws;
     Layout l;
-    l.L = ws.add(views * n * 4);
-    l.M = ws.add(views * n);
-    l.u = ws.add((3 * n + h) * 8);
-    l.v = ws.add(n * 8);
-    l.hv = ws.add(n * 8);
-    l.hb = ws.add(n * 8);
-    l.x = ws.add(n * 8);
-    l.part = ws.add(static_cast<size_t>(max_blocks) * 4 * 8);
-    l.logi = ws.add(n * 4);
+    l.L = ws.add(m * views * n * 4);
+    l.M = ws.add(m * views * n);
+    l.u = ws.add(m * (3 * n + h) * 8);
+    l.v = ws.add(m * n * 8);
+    l.hv = ws.add(m * n * 8);
+    l.hb = ws.add(m * n * 8);
+    l.x = ws.add(m * n * 8);
+    l.part = ws.add(m * kMaxLsmrBlocks * 4 * 8);
+    l.logi = ws.add(m * n * 4);
+    l.stop = ws.add(m * 4);
     l.total = ws.total;
     return l;
 }
-constexpr int kMaxLsmrBlocks = 132 * 4;
+
+int check_batch(const char* what, int batch) {
+    if (batch < 1 || batch > MOGE_PANORAMA_MAX_BATCH)
+        return set_error("%s: a batch of %d panoramas is outside [1, %d]", what, batch, MOGE_PANORAMA_MAX_BATCH);
+    return 0;
+}
+
+// the LSMR solve of `batch` systems of h x w: the virtual partition, the real grid over at most the co-resident blocks, the launch
+int lsmr(const char* what, const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
+         int32_t* stats, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!b || !row_mask || !depth || !stats) return set_error("null argument");
+    MG_TRY(check_batch(what, batch));
+    MG_TRY(check_size(what, h, w));
+    const Layout l = layout(1, h, w, batch);
+    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, what));
+    int sms, dev = 0, coop = 0, per_sm = 0;
+    MG_TRY(check_device(what, &sms));
+    CUDA_TRY(cudaGetDevice(&dev));
+    CUDA_TRY(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+    if (!coop) return set_error("%s: the device does not support cooperative launches", what);
+    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lsmr_kernel, kLsmrThreads, 0));
+    if (per_sm < 1) return set_error("%s: the solver kernel does not fit on an SM", what);
+    const int64_t n = static_cast<int64_t>(h) * w;
+    const int vblocks = static_cast<int>(std::min<int64_t>({sms, (n + kLsmrThreads - 1) / kLsmrThreads, kMaxLsmrBlocks}));
+    const int items = batch * vblocks, resident = sms * per_sm;
+    const int per_block = (items + resident - 1) / resident, blocks = (items + per_block - 1) / per_block;
+    for (int k = 0; k < blocks; ++k) {
+        const int i0 = k * per_block, i1 = std::min(i0 + per_block, items);
+        if ((i1 - 1) / vblocks - i0 / vblocks + 1 > kMaxLocal)
+            return set_error("%s: a block would serve more than %d systems (%d virtual blocks each, %d per block)", what, kMaxLocal,
+                             vblocks, per_block);
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* ws = static_cast<char*>(workspace);
+    Lsmr a;
+    a.b = b; a.rm = row_mask; a.init = nullptr;
+    a.u = reinterpret_cast<double*>(ws + l.u); a.v = reinterpret_cast<double*>(ws + l.v);
+    a.hv = reinterpret_cast<double*>(ws + l.hv); a.hb = reinterpret_cast<double*>(ws + l.hb);
+    a.x = reinterpret_cast<double*>(ws + l.x); a.part = reinterpret_cast<double*>(ws + l.part);
+    a.depth = depth; a.stats = stats; a.stop = reinterpret_cast<int*>(ws + l.stop);
+    a.h = h; a.w = w; a.batch = batch; a.vblocks = vblocks; a.per_block = per_block;
+    if (init) {                                  // x0 = log(init), fp32
+        float* logi = reinterpret_cast<float*>(ws + l.logi);
+        log_kernel<<<blocks_for(n * batch, sms), kThreads, 0, st>>>(init, logi, n * batch);
+        CUDA_TRY(cudaGetLastError());
+        a.init = logi;
+    }
+    void* args[] = {&a};
+    CUDA_TRY(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(lsmr_kernel), dim3(blocks), dim3(kLsmrThreads), args, 0, st));
+    return 0;
+}
 
 }  // namespace
 }  // namespace mg
@@ -547,7 +798,7 @@ int moge_panorama_workspace_bytes(int views, int h, int w, size_t* bytes) {
     if (!bytes) return set_error("null argument");
     MG_TRY(check_size("panorama_workspace_bytes", h, w));
     if (views < 1 || views > MOGE_PANORAMA_MAX_VIEWS) return set_error("panorama_workspace_bytes: %d views is outside [1, %d]", views, MOGE_PANORAMA_MAX_VIEWS);
-    *bytes = layout(views, h, w, kMaxLsmrBlocks).total;
+    *bytes = layout(views, h, w).total;
     return 0;
 }
 
@@ -560,7 +811,7 @@ int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int v
     MG_TRY(check_size("panorama_rhs", h, w));
     Cams cs;
     MG_TRY(load_cams("panorama_rhs", cams, views, &cs));
-    const Layout l = layout(views, h, w, kMaxLsmrBlocks);
+    const Layout l = layout(views, h, w);
     MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "panorama_rhs"));
     int sms;
     MG_TRY(check_device("panorama_rhs", &sms));
@@ -578,38 +829,7 @@ int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int v
 
 int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int h, int w, const float* init, float* depth, int32_t* stats,
                        void* workspace, size_t workspace_bytes, void* stream) {
-    if (!b || !row_mask || !depth || !stats) return set_error("null argument");
-    MG_TRY(check_size("panorama_lsmr", h, w));
-    const Layout l = layout(1, h, w, kMaxLsmrBlocks);
-    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "panorama_lsmr"));
-    int sms;
-    MG_TRY(check_device("panorama_lsmr", &sms));
-    int dev = 0, coop = 0, per_sm = 0;
-    CUDA_TRY(cudaGetDevice(&dev));
-    CUDA_TRY(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-    if (!coop) return set_error("panorama_lsmr: the device does not support cooperative launches");
-    CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lsmr_kernel, kLsmrThreads, 0));
-    if (per_sm < 1) return set_error("panorama_lsmr: the solver kernel does not fit on an SM");
-    const int64_t n = static_cast<int64_t>(h) * w;
-    const int blocks = static_cast<int>(std::min<int64_t>({static_cast<int64_t>(sms) * per_sm, (n + kLsmrThreads - 1) / kLsmrThreads,
-                                                           static_cast<int64_t>(kMaxLsmrBlocks)}));
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    char* ws = static_cast<char*>(workspace);
-    Lsmr a;
-    a.b = b; a.rm = row_mask; a.init = nullptr;
-    a.u = reinterpret_cast<double*>(ws + l.u); a.v = reinterpret_cast<double*>(ws + l.v);
-    a.hv = reinterpret_cast<double*>(ws + l.hv); a.hb = reinterpret_cast<double*>(ws + l.hb);
-    a.x = reinterpret_cast<double*>(ws + l.x); a.part = reinterpret_cast<double*>(ws + l.part);
-    a.depth = depth; a.stats = stats; a.h = h; a.w = w;
-    if (init) {                                  // x0 = log(init), fp32
-        float* logi = reinterpret_cast<float*>(ws + l.logi);
-        log_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(init, logi, n);
-        CUDA_TRY(cudaGetLastError());
-        a.init = logi;
-    }
-    void* args[] = {&a};
-    CUDA_TRY(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(lsmr_kernel), dim3(blocks), dim3(kLsmrThreads), args, 0, st));
-    return 0;
+    return lsmr("panorama_lsmr", b, row_mask, 1, h, w, init, depth, stats, workspace, workspace_bytes, stream);
 }
 
 int moge_panorama_resize(const float* src, int h, int w, int H, int W, float* dst, void* stream) {
@@ -635,6 +855,94 @@ int moge_panorama_finish(const float* depth, const uint8_t* mask, int h, int w, 
     resize_kernel<<<blocks, kThreads, 0, st>>>(depth, h, w, H, W, depth_out);
     CUDA_TRY(cudaGetLastError());
     finish_kernel<<<blocks, kThreads, 0, st>>>(depth_out, mask, h, w, H, W, mask_out, points);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+// ---- batches of panoramas of one size, with the same cameras
+int moge_panorama_split_batch(const uint8_t* images, int batch, int H, int W, const moge_panorama_camera_t* cams, int views,
+                              const float* grid, int res, float* views_f32, uint8_t* views_u8, void* stream) {
+    if (!images || !grid || !views_f32) return set_error("null argument");
+    MG_TRY(check_batch("panorama_split_batch", batch));
+    MG_TRY(check_size("panorama_split_batch", H, W));
+    if (res < 1 || res > 8192) return set_error("panorama_split_batch: resolution %d is outside [1, 8192]", res);
+    Cams cs;
+    MG_TRY(load_cams("panorama_split_batch", cams, views, &cs));
+    int sms;
+    MG_TRY(check_device("panorama_split_batch", &sms));
+    split_batch_kernel<<<blocks_for(static_cast<int64_t>(batch) * views * res * res, sms), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        images, batch, H, W, cs, grid, res, views_f32, views_u8);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_panorama_workspace_bytes_batch(int batch, int views, int h, int w, size_t* bytes) {
+    if (!bytes) return set_error("null argument");
+    MG_TRY(check_batch("panorama_workspace_bytes_batch", batch));
+    MG_TRY(check_size("panorama_workspace_bytes_batch", h, w));
+    if (views < 1 || views > MOGE_PANORAMA_MAX_VIEWS)
+        return set_error("panorama_workspace_bytes_batch: %d views is outside [1, %d]", views, MOGE_PANORAMA_MAX_VIEWS);
+    *bytes = layout(views, h, w, batch).total;
+    return 0;
+}
+
+int moge_panorama_rhs_batch(const float* src, int channels, const uint8_t* mask, int batch, int views, int vh, int vw,
+                            const moge_panorama_camera_t* cams, const float* directions, int h, int w, double* b, uint8_t* row_mask,
+                            uint8_t* pano_mask, void* workspace, size_t workspace_bytes, void* stream) {
+    if (!src || !mask || !directions || !b || !row_mask || !pano_mask) return set_error("null argument");
+    if (channels != 1 && channels != 3) return set_error("panorama_rhs_batch: %d channels (1: distance, 3: points)", channels);
+    MG_TRY(check_batch("panorama_rhs_batch", batch));
+    MG_TRY(check_size("panorama_rhs_batch view", vh, vw));
+    MG_TRY(check_size("panorama_rhs_batch", h, w));
+    Cams cs;
+    MG_TRY(load_cams("panorama_rhs_batch", cams, views, &cs));
+    const Layout l = layout(views, h, w, batch);
+    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "panorama_rhs_batch"));
+    int sms;
+    MG_TRY(check_device("panorama_rhs_batch", &sms));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    char* ws = static_cast<char*>(workspace);
+    float* L = reinterpret_cast<float*>(ws + l.L);
+    uint8_t* M = reinterpret_cast<uint8_t*>(ws + l.M);
+    const int64_t n = static_cast<int64_t>(h) * w * batch;
+    sample_batch_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(src, channels, mask, batch, vh, vw, cs, directions, h, w, L, M);
+    CUDA_TRY(cudaGetLastError());
+    rhs_batch_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(L, M, batch, views, h, w, b, row_mask, pano_mask);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_panorama_lsmr_batch(const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
+                             int32_t* stats, void* workspace, size_t workspace_bytes, void* stream) {
+    return lsmr("panorama_lsmr_batch", b, row_mask, batch, h, w, init, depth, stats, workspace, workspace_bytes, stream);
+}
+
+int moge_panorama_resize_batch(const float* src, int batch, int h, int w, int H, int W, float* dst, void* stream) {
+    if (!src || !dst) return set_error("null argument");
+    MG_TRY(check_batch("panorama_resize_batch", batch));
+    MG_TRY(check_size("panorama_resize_batch", h, w));
+    MG_TRY(check_size("panorama_resize_batch", H, W));
+    int sms;
+    MG_TRY(check_device("panorama_resize_batch", &sms));
+    resize_batch_kernel<<<blocks_for(static_cast<int64_t>(H) * W * batch, sms), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        src, batch, h, w, H, W, dst);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int moge_panorama_finish_batch(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
+                               uint8_t* mask_out, float* points, void* stream) {
+    if (!depth || !mask || !depth_out || !mask_out || !points) return set_error("null argument");
+    MG_TRY(check_batch("panorama_finish_batch", batch));
+    MG_TRY(check_size("panorama_finish_batch", h, w));
+    MG_TRY(check_size("panorama_finish_batch", H, W));
+    int sms;
+    MG_TRY(check_device("panorama_finish_batch", &sms));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const unsigned blocks = blocks_for(static_cast<int64_t>(H) * W * batch, sms);
+    resize_batch_kernel<<<blocks, kThreads, 0, st>>>(depth, batch, h, w, H, W, depth_out);
+    CUDA_TRY(cudaGetLastError());
+    finish_batch_kernel<<<blocks, kThreads, 0, st>>>(depth_out, mask, batch, h, w, H, W, mask_out, points);
     CUDA_TRY(cudaGetLastError());
     return 0;
 }

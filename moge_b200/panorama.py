@@ -5,6 +5,10 @@ An equirectangular panorama is split into 12 perspective views (one camera per i
 through one `model.infer(views, fov_x=..., apply_mask=False)` call, and the views' log-distances are merged back into a panorama
 by a gradient-domain least-squares solve (SciPy's LSMR on a 4-level pyramid at up to 1920 x 960), then resized to the input.
 
+The batch forms (`split_panoramas`, `merge_panoramas`, `finish_panoramas`, `infer_panoramas`) take up to 64 panoramas of one size
+with the same cameras and give each one bitwise what the single call gives it; the merge solves every panorama's system of a
+level in one cooperative launch, so the panoramas share that launch's grid barriers.
+
 The work runs in moge_b200/csrc/panorama.cu: a split kernel that samples the uint8 panorama as cv2.remap does, a per-level
 right-hand-side pass that reads log |points| straight from the engine's output, a matrix-free LSMR in one cooperative kernel
 per level, and the resizes.  A merge never waits on the host.  The panorama ray table of each merge size is the reference's own
@@ -23,12 +27,14 @@ from . import capi
 from .capi import MogeError
 
 __all__ = ["get_panorama_cameras", "spherical_uv_to_directions", "directions_to_spherical_uv", "uv_map", "split_panorama",
-           "merge_panorama", "finish_panorama", "infer_panorama", "last_merge_stats", "SPLIT_RESOLUTION"]
+           "merge_panorama", "finish_panorama", "infer_panorama", "last_merge_stats", "split_panoramas", "merge_panoramas",
+           "finish_panoramas", "infer_panoramas", "SPLIT_RESOLUTION", "MAX_BATCH"]
 
 SPLIT_RESOLUTION = 512                 # infer_panorama.py:90
 MERGE_WIDTH, MERGE_HEIGHT = 1920, 960  # infer_panorama.py:117
 PYRAMID_SIZE = 256                     # panorama.py:106: a level recurses while max(w, h) > 256
 MAX_PIXELS = 1 << 28
+MAX_BATCH = 64                         # panoramas per batched call (MOGE_PANORAMA_MAX_BATCH)
 
 
 # ------------------------------------------------------------------------------------------------------------ host geometry
@@ -229,18 +235,24 @@ def merge_panorama(width: int, height: int, src: torch.Tensor, mask: torch.Tenso
                 W2, H2 = levels[lv + 1]
                 init = torch.empty(H2, W2, dtype=torch.float32, device=dev)
                 capi.check(L.moge_panorama_resize(depth.data_ptr(), h, w, H2, W2, init.data_ptr(), st))
-    _last.update(levels=levels, stats=stats)
+    _last.update(levels=levels, stats=stats, batched=False)
     result = (depth, pm.view(torch.bool))
     return (*result, out) if return_levels else result
 
 
-def last_merge_stats() -> List[Dict[str, int]]:
+def last_merge_stats() -> list:
     """Per level of the most recent merge_panorama call on this thread's process, coarsest first: width, height, LSMR iterations
-    and istop (SciPy's stopping reason).  Reading them copies the counters to the host."""
+    and istop (SciPy's stopping reason).  After merge_panoramas, one such list per panorama.  Reading them copies the counters to
+    the host."""
     if not _last:
         return []
     stats = _last["stats"].cpu().tolist()
-    return [{"width": w, "height": h, "iterations": it, "istop": st} for (w, h), (it, st) in zip(_last["levels"], stats)]
+
+    def per_level(rows):
+        return [{"width": w, "height": h, "iterations": it, "istop": st} for (w, h), (it, st) in zip(_last["levels"], rows)]
+    if _last["batched"]:
+        return [per_level([lv[k] for lv in stats]) for k in range(len(stats[0]))]
+    return per_level(stats)
 
 
 def finish_panorama(depth: torch.Tensor, mask: torch.Tensor, height: int, width: int):
@@ -260,6 +272,121 @@ def finish_panorama(depth: torch.Tensor, mask: torch.Tensor, height: int, width:
         points = torch.empty(height, width, 3, dtype=torch.float32, device=dev)
         capi.check(capi.lib().moge_panorama_finish(d.data_ptr(), m.data_ptr(), h, w, height, width, out_d.data_ptr(), out_m.data_ptr(),
                                                    points.data_ptr(), capi.current_stream()))
+    return out_d, out_m.view(torch.bool), points
+
+
+# ------------------------------------------------------------------------------------------------------------ batches
+def _check_batch(what: str, batch: int) -> None:
+    if not 1 <= batch <= MAX_BATCH:
+        raise MogeError(f"{what}: a batch of {batch} panoramas is outside [1, {MAX_BATCH}]")
+
+
+def _check_images(what: str, images) -> Tuple[int, int, int]:
+    if not isinstance(images, torch.Tensor) or images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] != 3:
+        raise MogeError(f"{what}: images must be a (P, H, W, 3) uint8 tensor")
+    P, H, W = images.shape[:3]
+    _check_batch(what, P)
+    _check_size(what, H, W)
+    capi.require_cuda(what, images)
+    return P, H, W
+
+
+def split_panoramas(images: torch.Tensor, extrinsics=None, intrinsics=None, resolution: int = SPLIT_RESOLUTION,
+                    return_uint8: bool = False):
+    """split_panorama of P panoramas of one size in one launch: images (P, H, W, 3) uint8 RGB CUDA tensor -> views
+    (P, N, 3, res, res) float32, and with return_uint8 also (P, N, res, res, 3) uint8; each panorama's views are bitwise its
+    split_panorama."""
+    P, H, W = _check_images("split_panoramas", images)
+    if not 1 <= int(resolution) <= 8192:
+        raise MogeError(f"split_panoramas: resolution {resolution} is outside [1, 8192]")
+    res = int(resolution)
+    if extrinsics is None:
+        extrinsics, intrinsics = _default_cameras()
+    cams, n = _cameras(extrinsics, intrinsics)
+    dev = images.device
+    with torch.cuda.device(dev):
+        img = images.contiguous()
+        out = torch.empty(P, n, 3, res, res, dtype=torch.float32, device=dev)
+        u8 = torch.empty(P, n, res, res, 3, dtype=torch.uint8, device=dev) if return_uint8 else None
+        grid = _table("grid", (res, res), dev)
+        capi.check(capi.lib().moge_panorama_split_batch(img.data_ptr(), P, H, W, cams, n, grid.data_ptr(), res, out.data_ptr(),
+                                                        capi.ptr(u8), capi.current_stream()))
+    return (out, u8) if return_uint8 else out
+
+
+def merge_panoramas(width: int, height: int, src: torch.Tensor, mask: torch.Tensor, extrinsics=None, intrinsics=None,
+                    return_levels: bool = False):
+    """merge_panorama of P panoramas with the same cameras: src (P, N, vh, vw) distances or (P, N, vh, vw, 3) points, mask
+    (P, N, vh, vw).  Returns (depth (P, height, width) float32, mask (P, height, width) bool), each panorama's bitwise its
+    merge_panorama, and with return_levels the per-level dicts with a leading P on b, row_mask and depth.  Each level's P
+    systems are solved in one cooperative launch; last_merge_stats() then gives one per-level list per panorama."""
+    width, height = int(width), int(height)
+    _check_size("merge_panoramas", height, width)
+    if not isinstance(src, torch.Tensor) or src.dtype != torch.float32 or src.dim() not in (4, 5) or (src.dim() == 5 and src.shape[4] != 3):
+        raise MogeError("merge_panoramas: src must be float32 (P, N, vh, vw) distances or (P, N, vh, vw, 3) points")
+    if not isinstance(mask, torch.Tensor) or tuple(mask.shape) != tuple(src.shape[:4]) or mask.dtype not in (torch.bool, torch.uint8):
+        raise MogeError(f"merge_panoramas: mask must be bool / uint8 of shape {tuple(src.shape[:4])}")
+    P, n, vh, vw = src.shape[:4]
+    _check_batch("merge_panoramas", P)
+    capi.require_cuda("merge_panoramas", src, mask)
+    _check_size("merge_panoramas view", vh, vw)
+    if extrinsics is None:
+        extrinsics, intrinsics = _default_cameras()
+    cams, nc = _cameras(extrinsics, intrinsics)
+    if nc != n:
+        raise MogeError(f"merge_panoramas: {n} views but {nc} cameras")
+    channels = 1 if src.dim() == 4 else 3
+    dev = src.device
+    L = capi.lib()
+    levels = _levels(width, height)
+    with torch.cuda.device(dev):
+        st = capi.current_stream()
+        s = src.detach().contiguous()
+        m = capi.mask_u8(mask)
+        ws = capi.workspace(L.moge_panorama_workspace_bytes_batch, P, n, height, width, device=dev)
+        stats = torch.zeros(len(levels), P, 2, dtype=torch.int32, device=dev)
+        depth, init, out = None, None, []
+        for lv, (w, h) in enumerate(levels):
+            b = torch.empty(P, num_rows(h, w), dtype=torch.float64, device=dev)
+            rm = torch.empty(P, num_rows(h, w), dtype=torch.uint8, device=dev)
+            pm = torch.empty(P, h, w, dtype=torch.uint8, device=dev)
+            dirs = _table("dirs", (h, w), dev)
+            capi.check(L.moge_panorama_rhs_batch(s.data_ptr(), channels, m.data_ptr(), P, n, vh, vw, cams, dirs.data_ptr(), h, w,
+                                                 b.data_ptr(), rm.data_ptr(), pm.data_ptr(), ws.data_ptr(), ws.numel(), st))
+            depth = torch.empty(P, h, w, dtype=torch.float32, device=dev)
+            capi.check(L.moge_panorama_lsmr_batch(b.data_ptr(), rm.data_ptr(), P, h, w, capi.ptr(init), depth.data_ptr(),
+                                                  stats[lv].data_ptr(), ws.data_ptr(), ws.numel(), st))
+            if return_levels:
+                out.append({"width": w, "height": h, "b": b, "row_mask": rm, "depth": depth})
+            if lv + 1 < len(levels):
+                W2, H2 = levels[lv + 1]
+                init = torch.empty(P, H2, W2, dtype=torch.float32, device=dev)
+                capi.check(L.moge_panorama_resize_batch(depth.data_ptr(), P, h, w, H2, W2, init.data_ptr(), st))
+    _last.update(levels=levels, stats=stats, batched=True)
+    result = (depth, pm.view(torch.bool))
+    return (*result, out) if return_levels else result
+
+
+def finish_panoramas(depth: torch.Tensor, mask: torch.Tensor, height: int, width: int):
+    """finish_panorama of P merged maps: depth (P, h, w) float32 and mask (P, h, w) -> depth (P, height, width), mask
+    (P, height, width) bool and points (P, height, width, 3)."""
+    if not isinstance(depth, torch.Tensor) or not isinstance(mask, torch.Tensor) or depth.dtype != torch.float32 or depth.dim() != 3 \
+            or tuple(mask.shape) != tuple(depth.shape):
+        raise MogeError("finish_panoramas: depth must be float32 (P, h, w) and mask (P, h, w)")
+    P, h, w = depth.shape
+    _check_batch("finish_panoramas", P)
+    capi.require_cuda("finish_panoramas", depth, mask)
+    _check_size("finish_panoramas", h, w)
+    _check_size("finish_panoramas", height, width)
+    dev = depth.device
+    with torch.cuda.device(dev):
+        d = depth.contiguous()
+        m = capi.mask_u8(mask)
+        out_d = torch.empty(P, height, width, dtype=torch.float32, device=dev)
+        out_m = torch.empty(P, height, width, dtype=torch.uint8, device=dev)
+        points = torch.empty(P, height, width, 3, dtype=torch.float32, device=dev)
+        capi.check(capi.lib().moge_panorama_finish_batch(d.data_ptr(), m.data_ptr(), P, h, w, height, width, out_d.data_ptr(),
+                                                         out_m.data_ptr(), points.data_ptr(), capi.current_stream()))
     return out_d, out_m.view(torch.bool), points
 
 
@@ -300,6 +427,39 @@ def infer_panorama(model, image: torch.Tensor, batch_size: Optional[int] = None,
     depth, mask = merge_panorama(min(MERGE_WIDTH, W), min(MERGE_HEIGHT, H), points, masks, extrinsics, intrinsics)
     view_points, view_masks = points, masks
     depth, mask, points = finish_panorama(depth, mask, H, W)
+    out = {'depth': depth, 'mask': mask, 'points': points}
+    if return_views:
+        out.update(views=views_u8, view_distance=view_points.norm(dim=-1), view_mask=view_masks)
+    return out
+
+
+def infer_panoramas(model, images: torch.Tensor, batch_size: Optional[int] = None, return_views: bool = False) -> Dict[str, torch.Tensor]:
+    """infer_panorama of P panoramas of one size: images (P, H, W, 3) uint8 RGB CUDA tensor.  The 12P views go through
+    `model.infer(views, fov_x=..., apply_mask=False)` in one call, or in calls of batch_size views that may straddle panoramas;
+    the split, the merge and the finish run once for the whole batch.  Returns device tensors {'depth' (P, H, W), 'mask'
+    (P, H, W) bool, 'points' (P, H, W, 3)}, and with return_views 'views', 'view_distance' and 'view_mask' with a leading P.
+    Each panorama's outputs are bitwise its infer_panorama."""
+    if batch_size is not None and int(batch_size) < 1:
+        raise MogeError(f"infer_panoramas: batch_size {batch_size} must be positive")
+    P, H, W = _check_images("infer_panoramas", images)
+    extrinsics, intrinsics = _default_cameras()
+    views = split_panoramas(images, extrinsics, intrinsics, SPLIT_RESOLUTION, return_uint8=return_views)
+    if return_views:
+        views, views_u8 = views
+    n = views.shape[1]
+    flat = views.view(P * n, *views.shape[2:])
+    fov_x = _fov_x(intrinsics, images.device).repeat(P)
+    step = len(flat) if batch_size is None else int(batch_size)
+    points, masks = [], []
+    for lo in range(0, len(flat), step):
+        out = model.infer(flat[lo:lo + step], fov_x=fov_x[lo:lo + step], apply_mask=False)
+        points.append(out['points'])
+        masks.append(out['mask'])
+    points = points[0] if len(points) == 1 else torch.cat(points)
+    masks = masks[0] if len(masks) == 1 else torch.cat(masks)
+    view_points, view_masks = points.reshape(P, n, *points.shape[1:]), masks.reshape(P, n, *masks.shape[1:])
+    depth, mask = merge_panoramas(min(MERGE_WIDTH, W), min(MERGE_HEIGHT, H), view_points, view_masks, extrinsics, intrinsics)
+    depth, mask, points = finish_panoramas(depth, mask, H, W)
     out = {'depth': depth, 'mask': mask, 'points': points}
     if return_views:
         out.update(views=views_u8, view_distance=view_points.norm(dim=-1), view_mask=view_masks)

@@ -19,7 +19,8 @@ ANON = re.compile(r"\d+_GLOBAL__N__[0-9a-f]{8}_\d+_\w+?_cu_[0-9a-f]{8}")
 
 
 def sass(obj):
-    """{kernel: SASS text} of one object file."""
+    """{kernel: SASS text} of one object file.  Runs of blanks are collapsed: cuobjdump pads its columns to the object's widest
+    instruction, so the padding changes with the other kernels of the unit."""
     out = subprocess.run([CUOBJDUMP, "-sass", obj], check=True, capture_output=True, text=True).stdout
     kernels, name = {}, None
     for line in ANON.sub("ANON", out).splitlines():
@@ -28,7 +29,7 @@ def sass(obj):
             name = m.group(1)
             kernels[name] = []
         elif name is not None:
-            kernels[name].append(line.strip())
+            kernels[name].append(re.sub(r"[ \t]+", " ", line.strip()))
     return {k: "\n".join(v).strip() for k, v in kernels.items()}
 
 
