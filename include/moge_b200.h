@@ -510,6 +510,35 @@ int moge_vis_colorize(const float* src, int kind, int invert, const uint8_t* mas
  * W, 3) fp32, n = 0 off the mask (may be NULL); bgr swaps the channels.                                                     */
 int moge_vis_normal(const float* normal, const uint8_t* mask, int64_t batch, int H, int W, int bgr, uint8_t* out, void* stream);
 
+/* ---- geometry utilities (moge/utils/geometry_torch.py: refine_depth_with_normal, dilate_with_mask, theshold_depth_change,
+ * gaussian_blur_2d; Python: moge_b200.geometry).  Maps are (batch, H, W) fp32 contiguous on the device, masks uint8 (nonzero =
+ * in), at most 2^30 pixels per map.  No atomics: the same inputs give the same bits on every run.  Kernel sizes are odd.     */
+#define MOGE_GEOMETRY_MAX_REFINE_KERNEL 9
+#define MOGE_GEOMETRY_MAX_POOL_KERNEL 15
+#define MOGE_GEOMETRY_MAX_BLUR_KERNEL 31
+enum { MOGE_DILATE_MEAN = 0, MOGE_DILATE_MIN = 1, MOGE_DILATE_MAX = 2, MOGE_DILATE_MEDIAN = 3 };
+/* workspace (256-byte aligned) of moge_refine_depth_with_normal */
+int moge_geometry_workspace_bytes(int64_t batch, int H, int W, size_t* bytes);
+/* refine_depth_with_normal: depth is clamped to at least eps IN PLACE (NaN stays NaN); normal (batch, H, W, 3), intrinsics
+ * (batch, 3, 3) fp32; out (batch, H, W) = exp of the log-depth after `iterations` Jacobi sweeps of the kernel_size (3 to
+ * MOGE_GEOMETRY_MAX_REFINE_KERNEL) bilateral stencil at the pixels kernel_size / 2 or more from the border, the input
+ * log-depth elsewhere. */
+int moge_refine_depth_with_normal(float* depth, const float* normal, const float* intrinsics, int64_t batch, int H, int W,
+                                  int iterations, float damp, float eps, int kernel_size, float* out, void* workspace,
+                                  size_t workspace_bytes, void* stream);
+/* one dilate_with_mask step over the 3 x 3 cross (outside the map: invalid): out = input where mask, else the filter
+ * (MOGE_DILATE_*) of the valid neighbours; mask_out = mask or any valid neighbour.  out and mask_out must not alias the inputs. */
+int moge_dilate_with_mask(const float* input, const uint8_t* mask, int64_t batch, int H, int W, int filter, float* out,
+                          uint8_t* mask_out, void* stream);
+/* theshold_depth_change: pool_max ? (masked window max > depth * factor) : (masked window min < depth * factor), out uint8 0 / 1;
+ * the window is kernel_size (1 to MOGE_GEOMETRY_MAX_POOL_KERNEL) square, NaN propagating, factor = 1 +- rtol in fp32. */
+int moge_threshold_depth_change(const float* depth, const uint8_t* mask, int64_t batch, int H, int W, int pool_max, float factor,
+                                int kernel_size, uint8_t* out, void* stream);
+/* gaussian_blur_2d of `planes` (H, W) maps with replicate padding: the kernel_size (1 to MOGE_GEOMETRY_MAX_BLUR_KERNEL) square
+ * kernel is the outer product of the host array kernel1d (kernel_size fp32 values), each product rounded once in fp32. */
+int moge_gaussian_blur_2d(const float* input, int64_t planes, int H, int W, const float* kernel1d, int kernel_size, float* out,
+                          void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -32,6 +32,8 @@ LOSS_MASK_L2, LOSS_MASK_BCE, LOSS_EDGE, LOSS_NORMAL = range(4)
 LOSS_LOCAL_PARAMS = 8
 VIS_MAX_QUANTILES = 4
 VIS_DEPTH, VIS_VALUE = 0, 1
+GEOMETRY_MAX_REFINE_KERNEL, GEOMETRY_MAX_POOL_KERNEL, GEOMETRY_MAX_BLUR_KERNEL = 9, 15, 31
+DILATE = {"mean": 0, "min": 1, "max": 2, "median": 3}
 
 
 class StackConfig(C.Structure):
@@ -189,6 +191,11 @@ SIGNATURES = {
     "moge_vis_quantiles": [vp, ci, vp, i64, ci, ci, fp, ci, vp, vp, sz, vp],
     "moge_vis_colorize": [vp, ci, ci, vp, i64, ci, ci, vp, vp, ci, vp, vp],
     "moge_vis_normal": [vp, vp, i64, ci, ci, ci, vp, vp],
+    "moge_geometry_workspace_bytes": [i64, ci, ci, C.POINTER(sz)],
+    "moge_refine_depth_with_normal": [vp, vp, vp, i64, ci, ci, ci, C.c_float, C.c_float, ci, vp, vp, sz, vp],
+    "moge_dilate_with_mask": [vp, vp, i64, ci, ci, ci, vp, vp, vp],
+    "moge_threshold_depth_change": [vp, vp, i64, ci, ci, ci, C.c_float, ci, vp, vp],
+    "moge_gaussian_blur_2d": [vp, i64, ci, ci, fp, ci, vp, vp],
 }
 EXPORTS = list(SIGNATURES)
 

@@ -634,3 +634,44 @@ def synthetic_normal_map_case(seed: int, batch_shape, H: int, W: int, empty_imag
     gt = torch.where(bad[..., None] & (torch.arange(3) == coord), value, gt)
     shape = (*batch_shape, H, W, 3)
     return {"pred_normal": pred.reshape(shape).contiguous(), "gt_normal": gt.reshape(shape).contiguous()}
+
+
+def synthetic_geometry_case(seed: int, batch_shape, H: int, W: int, mask_mode: str = "sparse"):
+    """Inputs of the geometry utilities (moge_b200.geometry) as a dict of CPU fp32 / bool tensors, from a seeded generator
+    (arithmetic and sqrt only): depth (..., H, W) > 0, the piecewise-planar depth of _scene; normal (..., H, W, 3), unit normals
+    of its points by central differences (one-sided at the border), turned to face the camera and tilted by noise of 0.05;
+    intrinsics (..., 3, 3), normalised, with the principal point within 0.02 of the centre; mask (..., H, W): 'all', 'none',
+    'sparse' (about 30 % valid) or 'scene' (_scene's mask); image (prod(batch_shape), 3, H, W) in [0, 1)."""
+    g = torch.Generator().manual_seed(4000 + seed)
+    n = 1
+    for d in batch_shape:
+        n *= d
+    depths, normals, intrs, masks = [], [], [], []
+    for _ in range(n):
+        fx, fy, depth, points, scene_mask = _scene(g, H, W)
+        cx, cy = (0.5 + 0.04 * (torch.rand(2, generator=g) - 0.5)).tolist()
+        K = torch.tensor([[fx, 0.0, cx], [0.0, fy, cy], [0.0, 0.0, 1.0]], dtype=torch.float32)
+        jr, jl = torch.arange(W).add(1).clamp_max(W - 1), torch.arange(W).sub(1).clamp_min(0)
+        ib, it = torch.arange(H).add(1).clamp_max(H - 1), torch.arange(H).sub(1).clamp_min(0)
+        du, dv = points[:, jr] - points[:, jl], points[ib] - points[it]
+        nx = du[..., 1] * dv[..., 2] - du[..., 2] * dv[..., 1]
+        ny = du[..., 2] * dv[..., 0] - du[..., 0] * dv[..., 2]
+        nz = du[..., 0] * dv[..., 1] - du[..., 1] * dv[..., 0]
+        nrm = torch.stack([nx, ny, nz], dim=-1)
+        nrm = torch.where(nz[..., None] > 0, -nrm, nrm)
+        nrm = _unit(_unit(nrm) + 0.05 * torch.randn(H, W, 3, generator=g))
+        if mask_mode == "all":
+            mask = torch.ones(H, W, dtype=torch.bool)
+        elif mask_mode == "none":
+            mask = torch.zeros(H, W, dtype=torch.bool)
+        elif mask_mode == "sparse":
+            mask = torch.rand(H, W, generator=g) < 0.3
+        elif mask_mode == "scene":
+            mask = scene_mask
+        else:
+            raise ValueError(mask_mode)
+        depths.append(depth); normals.append(nrm); intrs.append(K); masks.append(mask)
+    image = torch.rand(n, 3, H, W, generator=g)
+    shape = (*batch_shape, H, W)
+    return {"depth": torch.stack(depths).reshape(shape), "normal": torch.stack(normals).reshape(*shape, 3).contiguous(),
+            "intrinsics": torch.stack(intrs).reshape(*batch_shape, 3, 3), "mask": torch.stack(masks).reshape(shape), "image": image}
