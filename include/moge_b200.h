@@ -381,48 +381,36 @@ int moge_mesh_build(const uint8_t* mask, int64_t batch, int H, int W, int tri, c
  * maps are equirectangular, h x w, at least 2 x 2 and at most 2^28 pixels.                                                  */
 #define MOGE_PANORAMA_MAX_VIEWS 20
 typedef struct { float R[9]; float t[3]; double fx, fy, cx, cy; } moge_panorama_camera_t;
-/* split_panorama_image: views_f32 (views, 3, res, res) = value / 255 of cv2.remap(image, INTER_LINEAR, BORDER_CONSTANT 0) at the
- * panorama pixel of each view pixel's ray; grid (res) is the fp32 pixel-centre coordinate of uv_map; views_u8 (views, res, res, 3)
- * the uint8 values (may be NULL).  image (H, W, 3) uint8 RGB.                                                                 */
-int moge_panorama_split(const uint8_t* image, int H, int W, const moge_panorama_camera_t* cams, int views, const float* grid, int res,
-                        float* views_f32, uint8_t* views_u8, void* stream);
-/* workspace (256-byte aligned) of moge_panorama_rhs / moge_panorama_lsmr for a level of h x w (and for every smaller level) */
-int moge_panorama_workspace_bytes(int views, int h, int w, size_t* bytes);
-/* one merge level's right-hand side: src (views, vh, vw, channels) fp32 is the distance (channels 1) or the point map whose norm
- * is the distance (channels 3), mask (views, vh, vw) uint8, directions (h, w, 3) fp32 the panorama rays.  b fp64 and row_mask
- * uint8 have 2hw + (h-1)(w+1) rows in the reference's order: x-gradient h*w, y-gradient (h-1) x (w+1) (column w repeats column
- * 0, as the reference's x-wrapped grid does), Laplacian h*w; b = 0 where masked out.  pano_mask (h, w) uint8 = any view's mask. */
-int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int views, int vh, int vw, const moge_panorama_camera_t* cams,
-                      const float* directions, int h, int w, double* b, uint8_t* row_mask, uint8_t* pano_mask, void* workspace,
-                      size_t workspace_bytes, void* stream);
-/* SciPy's lsmr(A, b, atol = btol = 1e-5, x0 = log(init)) on the rows of row_mask (init NULL: x0 = None), depth (h, w) fp32 =
- * exp(x); stats (2) int32 on the device = (iterations, istop).  One cooperative launch, no host synchronisation.            */
-int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int h, int w, const float* init, float* depth, int32_t* stats,
-                       void* workspace, size_t workspace_bytes, void* stream);
-/* cv2.resize(src, (W, H), INTER_LINEAR) of an fp32 map: the pyramid's upsampling */
-int moge_panorama_resize(const float* src, int h, int w, int H, int W, float* dst, void* stream);
-/* infer_panorama.py:120-122: depth_out (H, W) the resized depth, mask_out (H, W) uint8 the bilinear resize of the 0/1 mask > 0,
- * points (H, W, 3) = depth_out * spherical_uv_to_directions(uv_map(H, W)).                                                   */
-int moge_panorama_finish(const float* depth, const uint8_t* mask, int h, int w, int H, int W, float* depth_out, uint8_t* mask_out,
-                         float* points, void* stream);
-/* Batches of 1 to MOGE_PANORAMA_MAX_BATCH panoramas of one size and one set of cameras, each item's result bitwise that of the
- * call above on it alone.  Arrays gain a leading batch dimension: images (batch, H, W, 3), views_f32 (batch * views, 3, res, res),
- * views_u8 (batch * views, res, res, 3), src (batch, views, vh, vw, channels), mask (batch, views, vh, vw), b and row_mask
- * (batch, rows), pano_mask, init and depth (batch, h, w), stats (batch, 2), depth_out, mask_out (batch, H, W), points
- * (batch, H, W, 3).  moge_panorama_lsmr_batch solves the batch's systems in one cooperative launch that ends when every system
- * has stopped; moge_panorama_workspace_bytes_batch sizes the workspace of moge_panorama_rhs_batch / moge_panorama_lsmr_batch. */
+/* Every call takes a batch of 1 to MOGE_PANORAMA_MAX_BATCH panoramas of one size and one set of cameras; each panorama's result
+ * is bitwise what it gets in a batch of one.  Arrays have a leading batch dimension.                                          */
 #define MOGE_PANORAMA_MAX_BATCH 64
-int moge_panorama_split_batch(const uint8_t* images, int batch, int H, int W, const moge_panorama_camera_t* cams, int views,
-                              const float* grid, int res, float* views_f32, uint8_t* views_u8, void* stream);
-int moge_panorama_workspace_bytes_batch(int batch, int views, int h, int w, size_t* bytes);
-int moge_panorama_rhs_batch(const float* src, int channels, const uint8_t* mask, int batch, int views, int vh, int vw,
-                            const moge_panorama_camera_t* cams, const float* directions, int h, int w, double* b, uint8_t* row_mask,
-                            uint8_t* pano_mask, void* workspace, size_t workspace_bytes, void* stream);
-int moge_panorama_lsmr_batch(const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
-                             int32_t* stats, void* workspace, size_t workspace_bytes, void* stream);
-int moge_panorama_resize_batch(const float* src, int batch, int h, int w, int H, int W, float* dst, void* stream);
-int moge_panorama_finish_batch(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
-                               uint8_t* mask_out, float* points, void* stream);
+/* split_panorama_image: views_f32 (batch * views, 3, res, res) = value / 255 of cv2.remap(image, INTER_LINEAR, BORDER_CONSTANT 0)
+ * at the panorama pixel of each view pixel's ray; grid (res) is the fp32 pixel-centre coordinate of uv_map; views_u8
+ * (batch * views, res, res, 3) the uint8 values (may be NULL).  images (batch, H, W, 3) uint8 RGB.                           */
+int moge_panorama_split(const uint8_t* images, int batch, int H, int W, const moge_panorama_camera_t* cams, int views, const float* grid,
+                        int res, float* views_f32, uint8_t* views_u8, void* stream);
+/* workspace (256-byte aligned) of moge_panorama_rhs / moge_panorama_lsmr for `batch` merges of a level of h x w (and for every
+ * smaller level) */
+int moge_panorama_workspace_bytes(int batch, int views, int h, int w, size_t* bytes);
+/* one merge level's right-hand side: src (batch, views, vh, vw, channels) fp32 is the distance (channels 1) or the point map whose
+ * norm is the distance (channels 3), mask (batch, views, vh, vw) uint8, directions (h, w, 3) fp32 the panorama rays.  b fp64 and
+ * row_mask uint8 are (batch, rows) with 2hw + (h-1)(w+1) rows in the reference's order: x-gradient h*w, y-gradient (h-1) x (w+1)
+ * (column w repeats column 0, as the reference's x-wrapped grid does), Laplacian h*w; b = 0 where masked out.  pano_mask
+ * (batch, h, w) uint8 = any view's mask.                                                                                     */
+int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int batch, int views, int vh, int vw,
+                      const moge_panorama_camera_t* cams, const float* directions, int h, int w, double* b, uint8_t* row_mask,
+                      uint8_t* pano_mask, void* workspace, size_t workspace_bytes, void* stream);
+/* SciPy's lsmr(A, b, atol = btol = 1e-5, x0 = log(init)) on the rows of row_mask (init NULL: x0 = None), depth (batch, h, w)
+ * fp32 = exp(x); stats (batch, 2) int32 on the device = (iterations, istop).  One cooperative launch for the whole batch, which
+ * ends when every system has stopped; no host synchronisation.                                                               */
+int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
+                       int32_t* stats, void* workspace, size_t workspace_bytes, void* stream);
+/* cv2.resize(src, (W, H), INTER_LINEAR) of fp32 maps, src (batch, h, w), dst (batch, H, W): the pyramid's upsampling */
+int moge_panorama_resize(const float* src, int batch, int h, int w, int H, int W, float* dst, void* stream);
+/* infer_panorama.py:120-122: depth_out (batch, H, W) the resized depth, mask_out (batch, H, W) uint8 the bilinear resize of the
+ * 0/1 mask > 0, points (batch, H, W, 3) = depth_out * spherical_uv_to_directions(uv_map(H, W)).                             */
+int moge_panorama_finish(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
+                         uint8_t* mask_out, float* points, void* stream);
 
 /* ---- training losses of moge/train/losses.py (Python: moge_b200.losses, moge_b200.local_loss; alias moge.train.losses).
  * Maps are (batch, H, W) fp32 and point maps (batch, H, W, 3) fp32, contiguous on the device.  Each call either reduces

@@ -167,18 +167,12 @@ SIGNATURES = {
     "moge_mesh_build": [vp, i64, ci, ci, ci, C.POINTER(MeshMap), ci, vp, vp, vp, sz, vp],
     "moge_normal_map": [vp, vp, i64, ci, ci, vp, vp, vp],
     "moge_normal_edge": [vp, vp, vp, vp, i64, ci, ci, ci, C.c_double, vp, vp, vp],
-    "moge_panorama_split": [vp, ci, ci, pc, ci, vp, ci, vp, vp, vp],
-    "moge_panorama_workspace_bytes": [ci, ci, ci, C.POINTER(sz)],
-    "moge_panorama_rhs": [vp, ci, vp, ci, ci, ci, pc, vp, ci, ci, vp, vp, vp, vp, sz, vp],
-    "moge_panorama_lsmr": [vp, vp, ci, ci, vp, vp, vp, vp, sz, vp],
-    "moge_panorama_resize": [vp, ci, ci, ci, ci, vp, vp],
-    "moge_panorama_finish": [vp, vp, ci, ci, ci, ci, vp, vp, vp, vp],
-    "moge_panorama_split_batch": [vp, ci, ci, ci, pc, ci, vp, ci, vp, vp, vp],
-    "moge_panorama_workspace_bytes_batch": [ci, ci, ci, ci, C.POINTER(sz)],
-    "moge_panorama_rhs_batch": [vp, ci, vp, ci, ci, ci, ci, pc, vp, ci, ci, vp, vp, vp, vp, sz, vp],
-    "moge_panorama_lsmr_batch": [vp, vp, ci, ci, ci, vp, vp, vp, vp, sz, vp],
-    "moge_panorama_resize_batch": [vp, ci, ci, ci, ci, ci, vp, vp],
-    "moge_panorama_finish_batch": [vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp],
+    "moge_panorama_split": [vp, ci, ci, ci, pc, ci, vp, ci, vp, vp, vp],
+    "moge_panorama_workspace_bytes": [ci, ci, ci, ci, C.POINTER(sz)],
+    "moge_panorama_rhs": [vp, ci, vp, ci, ci, ci, ci, pc, vp, ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_panorama_lsmr": [vp, vp, ci, ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_panorama_resize": [vp, ci, ci, ci, ci, ci, vp, vp],
+    "moge_panorama_finish": [vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp],
     "moge_loss_workspace_bytes": [i64, ci, ci, C.POINTER(sz)],
     "moge_loss_mask": [ci, vp, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp],
     "moge_loss_stencil": [ci, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp],

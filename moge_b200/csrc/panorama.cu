@@ -18,7 +18,8 @@
 // reductions.  The iteration count and istop are written to the device.  One launch solves the
 // systems of a batch of panoramas, each bitwise as alone (see lsmr_kernel); a single merge is a batch of one.
 //
-// The *_batch kernels run the per-pixel bodies of the single-panorama kernels over a leading batch dimension.
+// Every stage takes a batch of panoramas of one size with one set of cameras.  The per-pixel kernels take the panorama from
+// blockIdx.y and stride over its pixels in x, so each thread does the same work at any batch size.
 #include "host_api.h"
 #include "../../include/moge_b200.h"
 #include <cooperative_groups.h>
@@ -48,60 +49,48 @@ __device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b)
 __device__ __forceinline__ int q32(float x) { return __float2int_rn(fmul(x, 32.f)); }
 
 // ---------------------------------------------------------------------------------------------------- split
-// view pixel idx of one panorama: out (views, 3, res, res), out_u8 (views, res, res, 3) or null
-__device__ __forceinline__ void split_pixel(const uint8_t* __restrict__ img, int H, int W, const Cams& cams, const float* __restrict__ grid,
-                                            int res, float* __restrict__ out, uint8_t* __restrict__ out_u8, int64_t idx) {
-    const int k = static_cast<int>(idx / (static_cast<int64_t>(res) * res));
-    const int pix = static_cast<int>(idx % (static_cast<int64_t>(res) * res)), i = pix / res, j = pix % res;
-    const moge_panorama_camera_t& c = cams.c[k];
-    // unproject_cv(uv, 1): ((u - cx) / fx, (v - cy) / fy, 1), then R^T (p - t)
-    const double p0 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[j]), c.cx), c.fx), static_cast<double>(c.t[0]));
-    const double p1 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[i]), c.cy), c.fy), static_cast<double>(c.t[1]));
-    const double p2 = dsub(1.0, static_cast<double>(c.t[2]));
-    double d[3];
-    for (int r = 0; r < 3; ++r)
-        d[r] = dadd(dadd(dmul(c.R[r], p0), dmul(c.R[3 + r], p1)), dmul(c.R[6 + r], p2));
-    // directions_to_spherical_uv
-    const double nrm = sqrt(dadd(dadd(dmul(d[0], d[0]), dmul(d[1], d[1])), dmul(d[2], d[2])));
-    const double x = __ddiv_rn(d[0], nrm), y = __ddiv_rn(d[1], nrm), z = __ddiv_rn(d[2], nrm);
-    double a = __ddiv_rn(atan2(y, x), 6.283185307179586), m = fmod(a, 1.0);
-    if (m != 0.0) { if (m < 0) m = dadd(m, 1.0); } else m = 0.0;         // numpy's floor-mod: sign of the divisor
-    const double u = dsub(1.0, m), v = __ddiv_rn(acos(z), 3.141592653589793);
-    // uv_to_pixel, fp32, cv2 fixed point
-    const int X = q32(__double2float_rn(dsub(dmul(u, static_cast<double>(W)), 0.5)));
-    const int Y = q32(__double2float_rn(dsub(dmul(v, static_cast<double>(H)), 0.5)));
-    const int ix = X >> 5, iy = Y >> 5, fx = X & 31, fy = Y & 31;
-    const int w[4] = {(32 - fx) * (32 - fy) * 32, fx * (32 - fy) * 32, (32 - fx) * fy * 32, fx * fy * 32};
-    int acc[3] = {0, 0, 0};
-    for (int t = 0; t < 4; ++t) {
-        const int yy = iy + (t >> 1), xx = ix + (t & 1);
-        if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;        // BORDER_CONSTANT 0
-        const uint8_t* s = img + (static_cast<int64_t>(yy) * W + xx) * 3;
-        for (int ch = 0; ch < 3; ++ch) acc[ch] += w[t] * s[ch];
-    }
-    for (int ch = 0; ch < 3; ++ch) {
-        const int val = min(255, max(0, (acc[ch] + (1 << 14)) >> 15));
-        out[((static_cast<int64_t>(k) * 3 + ch) * res + i) * res + j] = __double2float_rn(static_cast<double>(val) / 255.0);
-        if (out_u8) out_u8[idx * 3 + ch] = static_cast<uint8_t>(val);
-    }
-}
-
+// panorama blockIdx.y of the batch: img (batch, H, W, 3), out (batch * views, 3, res, res), out_u8 (batch * views, res, res, 3) or null
 __global__ void __launch_bounds__(kThreads) split_kernel(const uint8_t* __restrict__ img, int H, int W, const Cams cams,
                                                          const float* __restrict__ grid, int res, float* __restrict__ out,
                                                          uint8_t* __restrict__ out_u8) {
-    const int64_t total = static_cast<int64_t>(cams.n) * res * res;
-    for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total; idx += static_cast<int64_t>(gridDim.x) * blockDim.x)
-        split_pixel(img, H, W, cams, grid, res, out, out_u8, idx);
-}
-
-// split_kernel over `batch` panoramas of H x W: images (batch, H, W, 3), out (batch * views, 3, res, res)
-__global__ void __launch_bounds__(kThreads) split_batch_kernel(const uint8_t* __restrict__ img, int batch, int H, int W, const Cams cams,
-                                                               const float* __restrict__ grid, int res, float* __restrict__ out,
-                                                               uint8_t* __restrict__ out_u8) {
-    const int64_t per = static_cast<int64_t>(cams.n) * res * res, total = per * batch;
+    const int64_t total = static_cast<int64_t>(cams.n) * res * res, pano = blockIdx.y;
+    img += pano * H * W * 3;
+    out += pano * total * 3;
+    if (out_u8) out_u8 += pano * total * 3;
     for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total; idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int64_t q = idx / per;
-        split_pixel(img + q * H * W * 3, H, W, cams, grid, res, out + q * per * 3, out_u8 ? out_u8 + q * per * 3 : nullptr, idx - q * per);
+        const int k = static_cast<int>(idx / (static_cast<int64_t>(res) * res));
+        const int pix = static_cast<int>(idx % (static_cast<int64_t>(res) * res)), i = pix / res, j = pix % res;
+        const moge_panorama_camera_t& c = cams.c[k];
+        // unproject_cv(uv, 1): ((u - cx) / fx, (v - cy) / fy, 1), then R^T (p - t)
+        const double p0 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[j]), c.cx), c.fx), static_cast<double>(c.t[0]));
+        const double p1 = dsub(__ddiv_rn(dsub(static_cast<double>(grid[i]), c.cy), c.fy), static_cast<double>(c.t[1]));
+        const double p2 = dsub(1.0, static_cast<double>(c.t[2]));
+        double d[3];
+        for (int r = 0; r < 3; ++r)
+            d[r] = dadd(dadd(dmul(c.R[r], p0), dmul(c.R[3 + r], p1)), dmul(c.R[6 + r], p2));
+        // directions_to_spherical_uv
+        const double nrm = sqrt(dadd(dadd(dmul(d[0], d[0]), dmul(d[1], d[1])), dmul(d[2], d[2])));
+        const double x = __ddiv_rn(d[0], nrm), y = __ddiv_rn(d[1], nrm), z = __ddiv_rn(d[2], nrm);
+        double a = __ddiv_rn(atan2(y, x), 6.283185307179586), m = fmod(a, 1.0);
+        if (m != 0.0) { if (m < 0) m = dadd(m, 1.0); } else m = 0.0;         // numpy's floor-mod: sign of the divisor
+        const double u = dsub(1.0, m), v = __ddiv_rn(acos(z), 3.141592653589793);
+        // uv_to_pixel, fp32, cv2 fixed point
+        const int X = q32(__double2float_rn(dsub(dmul(u, static_cast<double>(W)), 0.5)));
+        const int Y = q32(__double2float_rn(dsub(dmul(v, static_cast<double>(H)), 0.5)));
+        const int ix = X >> 5, iy = Y >> 5, fx = X & 31, fy = Y & 31;
+        const int w[4] = {(32 - fx) * (32 - fy) * 32, fx * (32 - fy) * 32, (32 - fx) * fy * 32, fx * fy * 32};
+        int acc[3] = {0, 0, 0};
+        for (int t = 0; t < 4; ++t) {
+            const int yy = iy + (t >> 1), xx = ix + (t & 1);
+            if (yy < 0 || yy >= H || xx < 0 || xx >= W) continue;        // BORDER_CONSTANT 0
+            const uint8_t* s = img + (static_cast<int64_t>(yy) * W + xx) * 3;
+            for (int ch = 0; ch < 3; ++ch) acc[ch] += w[t] * s[ch];
+        }
+        for (int ch = 0; ch < 3; ++ch) {
+            const int val = min(255, max(0, (acc[ch] + (1 << 14)) >> 15));
+            out[((static_cast<int64_t>(k) * 3 + ch) * res + i) * res + j] = __double2float_rn(static_cast<double>(val) / 255.0);
+            if (out_u8) out_u8[idx * 3 + ch] = static_cast<uint8_t>(val);
+        }
     }
 }
 
@@ -112,124 +101,100 @@ __device__ __forceinline__ float log_distance(const float* __restrict__ src, int
     return logf(sqrtf(fadd(fadd(fmul(p[0], p[0]), fmul(p[1], p[1])), fmul(p[2], p[2]))));
 }
 
-// panorama pixel p of one merge: per view, the sampled log-distance (0 outside the view) and mask
-__device__ __forceinline__ void sample_pixel(const float* __restrict__ src, int channels, const uint8_t* __restrict__ vmask, int vh, int vw,
-                                             const Cams& cams, const float* __restrict__ dirs, int64_t n, float* __restrict__ L,
-                                             uint8_t* __restrict__ M, int64_t p) {
-    const float d0 = dirs[p * 3], d1 = dirs[p * 3 + 1], d2 = dirs[p * 3 + 2];
-    for (int k = 0; k < cams.n; ++k) {
-        const moge_panorama_camera_t& c = cams.c[k];
-        float q[3];
-        for (int r = 0; r < 3; ++r) q[r] = fadd(fadd(fadd(fmul(c.R[3 * r], d0), fmul(c.R[3 * r + 1], d1)), fmul(c.R[3 * r + 2], d2)), c.t[r]);
-        const double X = q[0], Y = q[1], Z = q[2];
-        double u = __ddiv_rn(dadd(dmul(c.fx, X), dmul(c.cx, Z)), Z), v = __ddiv_rn(dadd(dmul(c.fy, Y), dmul(c.cy, Z)), Z);
-        const bool valid = q[2] > 0.f && u > 0.0 && v > 0.0 && u < 1.0 && v < 1.0;
-        u = fmin(fmax(u, 0.0), 1.0);
-        v = fmin(fmax(v, 0.0), 1.0);
-        const float px = __double2float_rn(dsub(dmul(u, static_cast<double>(vw)), 0.5));
-        const float py = __double2float_rn(dsub(dmul(v, static_cast<double>(vh)), 0.5));
-        const int64_t base = static_cast<int64_t>(k) * vh * vw;
-        float val = 0.f;
-        uint8_t m = 0;
-        if (valid) {
-            const int Xq = q32(px), Yq = q32(py), ix = Xq >> 5, iy = Yq >> 5;
-            const float ax = static_cast<float>(Xq & 31) / 32.f, ay = static_cast<float>(Yq & 31) / 32.f;
-            const float wx[2] = {1.f - ax, ax}, wy[2] = {1.f - ay, ay};
-            float acc = 0.f;
-            for (int t = 0; t < 4; ++t) {
-                const int yy = min(max(iy + (t >> 1), 0), vh - 1), xx = min(max(ix + (t & 1), 0), vw - 1);
-                acc = fadd(acc, fmul(fmul(wy[t >> 1], wx[t & 1]), log_distance(src, channels, base + static_cast<int64_t>(yy) * vw + xx)));
-            }
-            val = acc;
-            const int nx = min(max(__float2int_rn(px), 0), vw - 1), ny = min(max(__float2int_rn(py), 0), vh - 1);
-            m = vmask[base + static_cast<int64_t>(ny) * vw + nx] != 0;
-        }
-        L[k * n + p] = val;
-        M[k * n + p] = m;
-    }
-}
-
+// panorama blockIdx.y of the batch, per pixel and view: the sampled log-distance (0 outside the view) and mask.  src
+// (batch * views, vh, vw, channels), vmask (batch * views, vh, vw), L and M (batch * views, h, w)
 __global__ void __launch_bounds__(kThreads) sample_kernel(const float* __restrict__ src, int channels, const uint8_t* __restrict__ vmask,
                                                           int vh, int vw, const Cams cams, const float* __restrict__ dirs, int h, int w,
                                                           float* __restrict__ L, uint8_t* __restrict__ M) {
     const int64_t n = static_cast<int64_t>(h) * w;
-    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
-        sample_pixel(src, channels, vmask, vh, vw, cams, dirs, n, L, M, p);
-}
-
-// sample_kernel over `batch` merges: src (batch, views, vh, vw, channels), vmask (batch, views, vh, vw), L and M (batch, views, h, w)
-__global__ void __launch_bounds__(kThreads) sample_batch_kernel(const float* __restrict__ src, int channels, const uint8_t* __restrict__ vmask,
-                                                                int batch, int vh, int vw, const Cams cams, const float* __restrict__ dirs,
-                                                                int h, int w, float* __restrict__ L, uint8_t* __restrict__ M) {
-    const int64_t n = static_cast<int64_t>(h) * w, views = static_cast<int64_t>(cams.n) * vh * vw;
-    for (int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; t < n * batch; t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int64_t q = t / n;
-        sample_pixel(src + q * views * channels, channels, vmask + q * views, vh, vw, cams, dirs, n, L + q * cams.n * n, M + q * cams.n * n, t - q * n);
-    }
-}
-
-// panorama pixel p of one merge: its rows of b and row_mask (see the header) and pano_mask
-__device__ __forceinline__ void rhs_pixel(const float* __restrict__ L, const uint8_t* __restrict__ M, int views, int h, int w, int64_t n,
-                                          double* __restrict__ b, uint8_t* __restrict__ rm, uint8_t* __restrict__ pmask, int64_t p) {
-    const int i = static_cast<int>(p / w), j = static_cast<int>(p % w);
-    const int64_t pr = i * static_cast<int64_t>(w) + (j + 1) % w, pl = i * static_cast<int64_t>(w) + (j + w - 1) % w;
-    const int64_t pu = static_cast<int64_t>(max(i - 1, 0)) * w + j, pd = static_cast<int64_t>(min(i + 1, h - 1)) * w + j;
-    float sx = 0.f, sy = 0.f, sl = 0.f;
-    int cx = 0, cy = 0, cl = 0, any = 0;
-    for (int k = 0; k < views; ++k) {
-        const float* Lk = L + k * n;
-        const uint8_t* Mk = M + k * n;
-        const float c = Lk[p];
-        const int mc = Mk[p], mr = Mk[pr];
-        any |= mc;
-        const int mx = mc & mr;
-        const float gx = fmul(__fsub_rn(c, Lk[pr]), static_cast<float>(mx));
-        sx = k ? fadd(sx, gx) : gx;
-        cx += mx;
-        if (i < h - 1) {
-            const int my = mc & Mk[p + w];
-            const float gy = fmul(__fsub_rn(c, Lk[p + w]), static_cast<float>(my));
-            sy = k ? fadd(sy, gy) : gy;
-            cy += my;
+    const int k0 = blockIdx.y * cams.n;            // the panorama's first view in the batch
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const float d0 = dirs[p * 3], d1 = dirs[p * 3 + 1], d2 = dirs[p * 3 + 2];
+        for (int k = 0; k < cams.n; ++k) {
+            const moge_panorama_camera_t& c = cams.c[k];
+            float q[3];
+            for (int r = 0; r < 3; ++r) q[r] = fadd(fadd(fadd(fmul(c.R[3 * r], d0), fmul(c.R[3 * r + 1], d1)), fmul(c.R[3 * r + 2], d2)), c.t[r]);
+            const double X = q[0], Y = q[1], Z = q[2];
+            double u = __ddiv_rn(dadd(dmul(c.fx, X), dmul(c.cx, Z)), Z), v = __ddiv_rn(dadd(dmul(c.fy, Y), dmul(c.cy, Z)), Z);
+            const bool valid = q[2] > 0.f && u > 0.0 && v > 0.0 && u < 1.0 && v < 1.0;
+            u = fmin(fmax(u, 0.0), 1.0);
+            v = fmin(fmax(v, 0.0), 1.0);
+            const float px = __double2float_rn(dsub(dmul(u, static_cast<double>(vw)), 0.5));
+            const float py = __double2float_rn(dsub(dmul(v, static_cast<double>(vh)), 0.5));
+            const int64_t base = static_cast<int64_t>(k0 + k) * vh * vw;
+            float val = 0.f;
+            uint8_t m = 0;
+            if (valid) {
+                const int Xq = q32(px), Yq = q32(py), ix = Xq >> 5, iy = Yq >> 5;
+                const float ax = static_cast<float>(Xq & 31) / 32.f, ay = static_cast<float>(Yq & 31) / 32.f;
+                const float wx[2] = {1.f - ax, ax}, wy[2] = {1.f - ay, ay};
+                float acc = 0.f;
+                for (int t = 0; t < 4; ++t) {
+                    const int yy = min(max(iy + (t >> 1), 0), vh - 1), xx = min(max(ix + (t & 1), 0), vw - 1);
+                    acc = fadd(acc, fmul(fmul(wy[t >> 1], wx[t & 1]), log_distance(src, channels, base + static_cast<int64_t>(yy) * vw + xx)));
+                }
+                val = acc;
+                const int nx = min(max(__float2int_rn(px), 0), vw - 1), ny = min(max(__float2int_rn(py), 0), vh - 1);
+                m = vmask[base + static_cast<int64_t>(ny) * vw + nx] != 0;
+            }
+            L[(k0 + k) * n + p] = val;
+            M[(k0 + k) * n + p] = m;
         }
-        // scipy.ndimage.convolve of the edge / wrap padded map: fp64 taps in footprint order, rounded to fp32
-        const double lap = dadd(dadd(dadd(dadd(static_cast<double>(Lk[pu]), static_cast<double>(Lk[pl])), -4.0 * static_cast<double>(c)),
-                                     static_cast<double>(Lk[pr])), static_cast<double>(Lk[pd]));
-        const int ml = mc & Mk[pu] & Mk[pd] & Mk[pl] & mr;
-        const float gl = fmul(__double2float_rn(lap), static_cast<float>(ml));
-        sl = k ? fadd(sl, gl) : gl;
-        cl += ml;
     }
-    b[p] = cx ? __ddiv_rn(static_cast<double>(sx), static_cast<double>(cx)) : 0.0;
-    rm[p] = cx > 0;
-    if (i < h - 1) {
-        const double by = cy ? __ddiv_rn(static_cast<double>(sy), static_cast<double>(cy)) : 0.0;
-        const int64_t e = n + static_cast<int64_t>(i) * (w + 1) + j;
-        b[e] = by;
-        rm[e] = cy > 0;
-        if (j == 0) { b[e + w] = by; rm[e + w] = cy > 0; }
-    }
-    const int64_t lo = n + static_cast<int64_t>(h - 1) * (w + 1);
-    b[lo + p] = cl ? __ddiv_rn(static_cast<double>(sl), static_cast<double>(cl)) : 0.0;
-    rm[lo + p] = cl > 0;
-    pmask[p] = any;
 }
 
+// panorama blockIdx.y of the batch, per pixel: its rows of b and row_mask (see the header) and pano_mask.  L and M
+// (batch * views, h, w), b and rm (batch, rows), pmask (batch, h, w)
 __global__ void __launch_bounds__(kThreads) rhs_kernel(const float* __restrict__ L, const uint8_t* __restrict__ M, int views, int h, int w,
                                                        double* __restrict__ b, uint8_t* __restrict__ rm, uint8_t* __restrict__ pmask) {
-    const int64_t n = static_cast<int64_t>(h) * w;
-    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
-        rhs_pixel(L, M, views, h, w, n, b, rm, pmask, p);
-}
-
-// rhs_kernel over `batch` merges: L and M (batch, views, h, w), b and rm (batch, rows), pmask (batch, h, w)
-__global__ void __launch_bounds__(kThreads) rhs_batch_kernel(const float* __restrict__ L, const uint8_t* __restrict__ M, int batch, int views,
-                                                             int h, int w, double* __restrict__ b, uint8_t* __restrict__ rm,
-                                                             uint8_t* __restrict__ pmask) {
-    const int64_t n = static_cast<int64_t>(h) * w, rows = 2 * n + static_cast<int64_t>(h - 1) * (w + 1);
-    for (int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; t < n * batch; t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int64_t q = t / n;
-        rhs_pixel(L + q * views * n, M + q * views * n, views, h, w, n, b + q * rows, rm + q * rows, pmask + q * n, t - q * n);
+    const int64_t n = static_cast<int64_t>(h) * w, rows = 2 * n + static_cast<int64_t>(h - 1) * (w + 1), pano = blockIdx.y;
+    const int k0 = blockIdx.y * views;             // the panorama's first view in the batch
+    b += pano * rows;
+    rm += pano * rows;
+    pmask += pano * n;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int i = static_cast<int>(p / w), j = static_cast<int>(p % w);
+        const int64_t pr = i * static_cast<int64_t>(w) + (j + 1) % w, pl = i * static_cast<int64_t>(w) + (j + w - 1) % w;
+        const int64_t pu = static_cast<int64_t>(max(i - 1, 0)) * w + j, pd = static_cast<int64_t>(min(i + 1, h - 1)) * w + j;
+        float sx = 0.f, sy = 0.f, sl = 0.f;
+        int cx = 0, cy = 0, cl = 0, any = 0;
+        for (int k = 0; k < views; ++k) {
+            const float* Lk = L + (k0 + k) * n;
+            const uint8_t* Mk = M + (k0 + k) * n;
+            const float c = Lk[p];
+            const int mc = Mk[p], mr = Mk[pr];
+            any |= mc;
+            const int mx = mc & mr;
+            const float gx = fmul(__fsub_rn(c, Lk[pr]), static_cast<float>(mx));
+            sx = k ? fadd(sx, gx) : gx;
+            cx += mx;
+            if (i < h - 1) {
+                const int my = mc & Mk[p + w];
+                const float gy = fmul(__fsub_rn(c, Lk[p + w]), static_cast<float>(my));
+                sy = k ? fadd(sy, gy) : gy;
+                cy += my;
+            }
+            // scipy.ndimage.convolve of the edge / wrap padded map: fp64 taps in footprint order, rounded to fp32
+            const double lap = dadd(dadd(dadd(dadd(static_cast<double>(Lk[pu]), static_cast<double>(Lk[pl])), -4.0 * static_cast<double>(c)),
+                                         static_cast<double>(Lk[pr])), static_cast<double>(Lk[pd]));
+            const int ml = mc & Mk[pu] & Mk[pd] & Mk[pl] & mr;
+            const float gl = fmul(__double2float_rn(lap), static_cast<float>(ml));
+            sl = k ? fadd(sl, gl) : gl;
+            cl += ml;
+        }
+        b[p] = cx ? __ddiv_rn(static_cast<double>(sx), static_cast<double>(cx)) : 0.0;
+        rm[p] = cx > 0;
+        if (i < h - 1) {
+            const double by = cy ? __ddiv_rn(static_cast<double>(sy), static_cast<double>(cy)) : 0.0;
+            const int64_t e = n + static_cast<int64_t>(i) * (w + 1) + j;
+            b[e] = by;
+            rm[e] = cy > 0;
+            if (j == 0) { b[e + w] = by; rm[e + w] = cy > 0; }
+        }
+        const int64_t lo = n + static_cast<int64_t>(h - 1) * (w + 1);
+        b[lo + p] = cl ? __ddiv_rn(static_cast<double>(sl), static_cast<double>(cl)) : 0.0;
+        rm[lo + p] = cl > 0;
+        pmask[p] = any;
     }
 }
 
@@ -595,87 +560,61 @@ __device__ __forceinline__ void lin_coef(int d, int in, int out, int* s0, int* s
     *s0 = sx; *s1 = min(sx + 1, in - 1); *f = fx;
 }
 
-// output pixel p of one map
-__device__ __forceinline__ void resize_pixel(const float* __restrict__ src, int h, int w, int H, int W, float* __restrict__ dst, int64_t p) {
-    const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
-    int x0, x1, y0, y1;
-    float fx, fy;
-    lin_coef(j, w, W, &x0, &x1, &fx);
-    lin_coef(i, h, H, &y0, &y1, &fy);
-    const float* r0 = src + static_cast<int64_t>(y0) * w;
-    const float* r1 = src + static_cast<int64_t>(y1) * w;
-    const float a0 = 1.f - fx, b0 = 1.f - fy;
-    const float h0 = fadd(fmul(r0[x0], a0), fmul(r0[x1], fx)), h1 = fadd(fmul(r1[x0], a0), fmul(r1[x1], fx));
-    dst[p] = fadd(fmul(h0, b0), fmul(h1, fy));
-}
-
+// panorama blockIdx.y of the batch: src (batch, h, w), dst (batch, H, W)
 __global__ void __launch_bounds__(kThreads) resize_kernel(const float* __restrict__ src, int h, int w, int H, int W, float* __restrict__ dst) {
-    const int64_t n = static_cast<int64_t>(H) * W;
-    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
-        resize_pixel(src, h, w, H, W, dst, p);
-}
-
-// resize_kernel over `batch` maps: src (batch, h, w), dst (batch, H, W)
-__global__ void __launch_bounds__(kThreads) resize_batch_kernel(const float* __restrict__ src, int batch, int h, int w, int H, int W,
-                                                                float* __restrict__ dst) {
-    const int64_t n = static_cast<int64_t>(H) * W;
-    for (int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; t < n * batch; t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int64_t q = t / n;
-        resize_pixel(src + q * h * w, h, w, H, W, dst + q * n, t - q * n);
+    const int64_t n = static_cast<int64_t>(H) * W, pano = blockIdx.y;
+    src += pano * h * w;
+    dst += pano * n;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
+        int x0, x1, y0, y1;
+        float fx, fy;
+        lin_coef(j, w, W, &x0, &x1, &fx);
+        lin_coef(i, h, H, &y0, &y1, &fy);
+        const float* r0 = src + static_cast<int64_t>(y0) * w;
+        const float* r1 = src + static_cast<int64_t>(y1) * w;
+        const float a0 = 1.f - fx, b0 = 1.f - fy;
+        const float h0 = fadd(fmul(r0[x0], a0), fmul(r0[x1], fx)), h1 = fadd(fmul(r1[x0], a0), fmul(r1[x1], fx));
+        dst[p] = fadd(fmul(h0, b0), fmul(h1, fy));
     }
 }
 
-// cv2.resize INTER_LINEAR of a 0/1 uint8 mask (11-bit fixed-point coefficients), then > 0; and points = depth * direction
-// output pixel p of one map; su .. stv are uv_map's linspace ends and steps
-__device__ __forceinline__ void finish_pixel(const float* __restrict__ depth, const uint8_t* __restrict__ mask, int h, int w, int H, int W,
-                                             uint8_t* __restrict__ mask_out, float* __restrict__ points, double su, double eu, double sv,
-                                             double ev, double stu, double stv, int64_t p) {
-    const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
-    int x0, x1, y0, y1;
-    float fx, fy;
-    lin_coef(j, w, W, &x0, &x1, &fx);
-    lin_coef(i, h, H, &y0, &y1, &fy);
-    const int a1 = __float2int_rn(fx * 2048.f), a0 = __float2int_rn((1.f - fx) * 2048.f);
-    const int b1 = __float2int_rn(fy * 2048.f), b0 = __float2int_rn((1.f - fy) * 2048.f);
-    const uint8_t* m0 = mask + static_cast<int64_t>(y0) * w;
-    const uint8_t* m1 = mask + static_cast<int64_t>(y1) * w;
-    const int r0 = (m0[x0] != 0) * a0 + (m0[x1] != 0) * a1, r1 = (m1[x0] != 0) * a0 + (m1[x1] != 0) * a1;
-    const int val = (((b0 * (r0 >> 4)) >> 16) + ((b1 * (r1 >> 4)) >> 16) + 2) >> 2;
-    mask_out[p] = val > 0;
-    // uv_map(H, W) (np.linspace in fp64, rounded to fp32) and spherical_uv_to_directions in fp32
-    const float u = j == W - 1 ? __double2float_rn(eu) : __double2float_rn(dadd(dmul(static_cast<double>(j), stu), su));
-    const float v = i == H - 1 ? __double2float_rn(ev) : __double2float_rn(dadd(dmul(static_cast<double>(i), stv), sv));
-    const float theta = fmul(1.f - u, 6.28318530717958647692f), phi = fmul(v, 3.14159265358979323846f);
-    const float sp = sinf(phi), d = depth[p];
-    points[p * 3] = fmul(d, fmul(sp, cosf(theta)));
-    points[p * 3 + 1] = fmul(d, fmul(sp, sinf(theta)));
-    points[p * 3 + 2] = fmul(d, cosf(phi));
-}
-
-#define FINISH_UV                                                                    \
-    const double su = 0.5 / W, eu = 1.0 - 0.5 / W, sv = 0.5 / H, ev = 1.0 - 0.5 / H; \
-    const double stu = W > 1 ? (eu - su) / (W - 1) : 0.0, stv = H > 1 ? (ev - sv) / (H - 1) : 0.0
-
+// cv2.resize INTER_LINEAR of a 0/1 uint8 mask (11-bit fixed-point coefficients), then > 0; and points = depth * direction.
+// Panorama blockIdx.y of the batch: depth (batch, H, W) (already resized), mask (batch, h, w), mask_out (batch, H, W), points
+// (batch, H, W, 3)
 __global__ void __launch_bounds__(kThreads) finish_kernel(const float* __restrict__ depth, const uint8_t* __restrict__ mask, int h, int w,
                                                           int H, int W, uint8_t* __restrict__ mask_out, float* __restrict__ points) {
-    const int64_t n = static_cast<int64_t>(H) * W;
-    FINISH_UV;
-    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
-        finish_pixel(depth, mask, h, w, H, W, mask_out, points, su, eu, sv, ev, stu, stv, p);
-}
-
-// finish_kernel over `batch` maps: depth (batch, H, W) (already resized), mask (batch, h, w), mask_out (batch, H, W), points (batch, H, W, 3)
-__global__ void __launch_bounds__(kThreads) finish_batch_kernel(const float* __restrict__ depth, const uint8_t* __restrict__ mask, int batch,
-                                                                int h, int w, int H, int W, uint8_t* __restrict__ mask_out,
-                                                                float* __restrict__ points) {
-    const int64_t n = static_cast<int64_t>(H) * W;
-    FINISH_UV;
-    for (int64_t t = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; t < n * batch; t += static_cast<int64_t>(gridDim.x) * blockDim.x) {
-        const int64_t q = t / n;
-        finish_pixel(depth + q * n, mask + q * h * w, h, w, H, W, mask_out + q * n, points + q * n * 3, su, eu, sv, ev, stu, stv, t - q * n);
+    const int64_t n = static_cast<int64_t>(H) * W, pano = blockIdx.y;
+    depth += pano * n;
+    mask += pano * h * w;
+    mask_out += pano * n;
+    points += pano * n * 3;
+    // uv_map's linspace ends and steps
+    const double su = 0.5 / W, eu = 1.0 - 0.5 / W, sv = 0.5 / H, ev = 1.0 - 0.5 / H;
+    const double stu = W > 1 ? (eu - su) / (W - 1) : 0.0, stv = H > 1 ? (ev - sv) / (H - 1) : 0.0;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
+        const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
+        int x0, x1, y0, y1;
+        float fx, fy;
+        lin_coef(j, w, W, &x0, &x1, &fx);
+        lin_coef(i, h, H, &y0, &y1, &fy);
+        const int a1 = __float2int_rn(fx * 2048.f), a0 = __float2int_rn((1.f - fx) * 2048.f);
+        const int b1 = __float2int_rn(fy * 2048.f), b0 = __float2int_rn((1.f - fy) * 2048.f);
+        const uint8_t* m0 = mask + static_cast<int64_t>(y0) * w;
+        const uint8_t* m1 = mask + static_cast<int64_t>(y1) * w;
+        const int r0 = (m0[x0] != 0) * a0 + (m0[x1] != 0) * a1, r1 = (m1[x0] != 0) * a0 + (m1[x1] != 0) * a1;
+        const int val = (((b0 * (r0 >> 4)) >> 16) + ((b1 * (r1 >> 4)) >> 16) + 2) >> 2;
+        mask_out[p] = val > 0;
+        // uv_map(H, W) (np.linspace in fp64, rounded to fp32) and spherical_uv_to_directions in fp32
+        const float u = j == W - 1 ? __double2float_rn(eu) : __double2float_rn(dadd(dmul(static_cast<double>(j), stu), su));
+        const float v = i == H - 1 ? __double2float_rn(ev) : __double2float_rn(dadd(dmul(static_cast<double>(i), stv), sv));
+        const float theta = fmul(1.f - u, 6.28318530717958647692f), phi = fmul(v, 3.14159265358979323846f);
+        const float sp = sinf(phi), d = depth[p];
+        points[p * 3] = fmul(d, fmul(sp, cosf(theta)));
+        points[p * 3 + 1] = fmul(d, fmul(sp, sinf(theta)));
+        points[p * 3 + 2] = fmul(d, cosf(phi));
     }
 }
-#undef FINISH_UV
 
 // ---------------------------------------------------------------------------------------------------- host side
 int check_size(const char* what, int h, int w) {
@@ -699,11 +638,10 @@ int load_cams(const char* what, const moge_panorama_camera_t* cams, int views, C
 
 unsigned blocks_for(int64_t n, int sms) { return static_cast<unsigned>(std::min<int64_t>((n + kThreads - 1) / kThreads, int64_t(sms) * 16)); }
 
-// the single merge's workspace, or (batch > 0) that of `batch` merges, which adds the batched solver's stop flags
 // the workspace of `batch` merges of up to h x w with `views` views
 struct Layout { size_t L, M, u, v, hv, hb, x, part, logi, stop, total; };
 constexpr int kMaxLsmrBlocks = 132 * 4;            // virtual blocks per system
-Layout layout(int views, int h, int w, int batch = 1) {
+Layout layout(int views, int h, int w, int batch) {
     const size_t n = static_cast<size_t>(h) * w, m = batch;
     WsLayout ws;
     Layout l;
@@ -779,39 +717,42 @@ using namespace mg;
 
 extern "C" {
 
-int moge_panorama_split(const uint8_t* image, int H, int W, const moge_panorama_camera_t* cams, int views, const float* grid, int res,
-                        float* views_f32, uint8_t* views_u8, void* stream) {
-    if (!image || !grid || !views_f32) return set_error("null argument");
+int moge_panorama_split(const uint8_t* images, int batch, int H, int W, const moge_panorama_camera_t* cams, int views, const float* grid,
+                        int res, float* views_f32, uint8_t* views_u8, void* stream) {
+    if (!images || !grid || !views_f32) return set_error("null argument");
+    MG_TRY(check_batch("panorama_split", batch));
     MG_TRY(check_size("panorama_split", H, W));
     if (res < 1 || res > 8192) return set_error("panorama_split: resolution %d is outside [1, 8192]", res);
     Cams cs;
     MG_TRY(load_cams("panorama_split", cams, views, &cs));
     int sms;
     MG_TRY(check_device("panorama_split", &sms));
-    split_kernel<<<blocks_for(static_cast<int64_t>(views) * res * res, sms), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        image, H, W, cs, grid, res, views_f32, views_u8);
+    split_kernel<<<dim3(blocks_for(static_cast<int64_t>(views) * res * res, sms), batch), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        images, H, W, cs, grid, res, views_f32, views_u8);
     CUDA_TRY(cudaGetLastError());
     return 0;
 }
 
-int moge_panorama_workspace_bytes(int views, int h, int w, size_t* bytes) {
+int moge_panorama_workspace_bytes(int batch, int views, int h, int w, size_t* bytes) {
     if (!bytes) return set_error("null argument");
+    MG_TRY(check_batch("panorama_workspace_bytes", batch));
     MG_TRY(check_size("panorama_workspace_bytes", h, w));
     if (views < 1 || views > MOGE_PANORAMA_MAX_VIEWS) return set_error("panorama_workspace_bytes: %d views is outside [1, %d]", views, MOGE_PANORAMA_MAX_VIEWS);
-    *bytes = layout(views, h, w).total;
+    *bytes = layout(views, h, w, batch).total;
     return 0;
 }
 
-int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int views, int vh, int vw, const moge_panorama_camera_t* cams,
-                      const float* directions, int h, int w, double* b, uint8_t* row_mask, uint8_t* pano_mask, void* workspace,
-                      size_t workspace_bytes, void* stream) {
+int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int batch, int views, int vh, int vw,
+                      const moge_panorama_camera_t* cams, const float* directions, int h, int w, double* b, uint8_t* row_mask,
+                      uint8_t* pano_mask, void* workspace, size_t workspace_bytes, void* stream) {
     if (!src || !mask || !directions || !b || !row_mask || !pano_mask) return set_error("null argument");
     if (channels != 1 && channels != 3) return set_error("panorama_rhs: %d channels (1: distance, 3: points)", channels);
+    MG_TRY(check_batch("panorama_rhs", batch));
     MG_TRY(check_size("panorama_rhs view", vh, vw));
     MG_TRY(check_size("panorama_rhs", h, w));
     Cams cs;
     MG_TRY(load_cams("panorama_rhs", cams, views, &cs));
-    const Layout l = layout(views, h, w);
+    const Layout l = layout(views, h, w, batch);
     MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "panorama_rhs"));
     int sms;
     MG_TRY(check_device("panorama_rhs", &sms));
@@ -819,130 +760,45 @@ int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int v
     char* ws = static_cast<char*>(workspace);
     float* L = reinterpret_cast<float*>(ws + l.L);
     uint8_t* M = reinterpret_cast<uint8_t*>(ws + l.M);
-    const int64_t n = static_cast<int64_t>(h) * w;
-    sample_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(src, channels, mask, vh, vw, cs, directions, h, w, L, M);
+    const dim3 grid(blocks_for(static_cast<int64_t>(h) * w, sms), batch);
+    sample_kernel<<<grid, kThreads, 0, st>>>(src, channels, mask, vh, vw, cs, directions, h, w, L, M);
     CUDA_TRY(cudaGetLastError());
-    rhs_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(L, M, views, h, w, b, row_mask, pano_mask);
+    rhs_kernel<<<grid, kThreads, 0, st>>>(L, M, views, h, w, b, row_mask, pano_mask);
     CUDA_TRY(cudaGetLastError());
     return 0;
 }
 
-int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int h, int w, const float* init, float* depth, int32_t* stats,
-                       void* workspace, size_t workspace_bytes, void* stream) {
-    return lsmr("panorama_lsmr", b, row_mask, 1, h, w, init, depth, stats, workspace, workspace_bytes, stream);
+int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
+                       int32_t* stats, void* workspace, size_t workspace_bytes, void* stream) {
+    return lsmr("panorama_lsmr", b, row_mask, batch, h, w, init, depth, stats, workspace, workspace_bytes, stream);
 }
 
-int moge_panorama_resize(const float* src, int h, int w, int H, int W, float* dst, void* stream) {
+int moge_panorama_resize(const float* src, int batch, int h, int w, int H, int W, float* dst, void* stream) {
     if (!src || !dst) return set_error("null argument");
+    MG_TRY(check_batch("panorama_resize", batch));
     MG_TRY(check_size("panorama_resize", h, w));
     MG_TRY(check_size("panorama_resize", H, W));
     int sms;
     MG_TRY(check_device("panorama_resize", &sms));
-    resize_kernel<<<blocks_for(static_cast<int64_t>(H) * W, sms), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(src, h, w, H, W, dst);
+    resize_kernel<<<dim3(blocks_for(static_cast<int64_t>(H) * W, sms), batch), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        src, h, w, H, W, dst);
     CUDA_TRY(cudaGetLastError());
     return 0;
 }
 
-int moge_panorama_finish(const float* depth, const uint8_t* mask, int h, int w, int H, int W, float* depth_out, uint8_t* mask_out,
-                         float* points, void* stream) {
+int moge_panorama_finish(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
+                         uint8_t* mask_out, float* points, void* stream) {
     if (!depth || !mask || !depth_out || !mask_out || !points) return set_error("null argument");
+    MG_TRY(check_batch("panorama_finish", batch));
     MG_TRY(check_size("panorama_finish", h, w));
     MG_TRY(check_size("panorama_finish", H, W));
     int sms;
     MG_TRY(check_device("panorama_finish", &sms));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const unsigned blocks = blocks_for(static_cast<int64_t>(H) * W, sms);
-    resize_kernel<<<blocks, kThreads, 0, st>>>(depth, h, w, H, W, depth_out);
+    const dim3 grid(blocks_for(static_cast<int64_t>(H) * W, sms), batch);
+    resize_kernel<<<grid, kThreads, 0, st>>>(depth, h, w, H, W, depth_out);
     CUDA_TRY(cudaGetLastError());
-    finish_kernel<<<blocks, kThreads, 0, st>>>(depth_out, mask, h, w, H, W, mask_out, points);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
-}
-
-// ---- batches of panoramas of one size, with the same cameras
-int moge_panorama_split_batch(const uint8_t* images, int batch, int H, int W, const moge_panorama_camera_t* cams, int views,
-                              const float* grid, int res, float* views_f32, uint8_t* views_u8, void* stream) {
-    if (!images || !grid || !views_f32) return set_error("null argument");
-    MG_TRY(check_batch("panorama_split_batch", batch));
-    MG_TRY(check_size("panorama_split_batch", H, W));
-    if (res < 1 || res > 8192) return set_error("panorama_split_batch: resolution %d is outside [1, 8192]", res);
-    Cams cs;
-    MG_TRY(load_cams("panorama_split_batch", cams, views, &cs));
-    int sms;
-    MG_TRY(check_device("panorama_split_batch", &sms));
-    split_batch_kernel<<<blocks_for(static_cast<int64_t>(batch) * views * res * res, sms), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        images, batch, H, W, cs, grid, res, views_f32, views_u8);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
-}
-
-int moge_panorama_workspace_bytes_batch(int batch, int views, int h, int w, size_t* bytes) {
-    if (!bytes) return set_error("null argument");
-    MG_TRY(check_batch("panorama_workspace_bytes_batch", batch));
-    MG_TRY(check_size("panorama_workspace_bytes_batch", h, w));
-    if (views < 1 || views > MOGE_PANORAMA_MAX_VIEWS)
-        return set_error("panorama_workspace_bytes_batch: %d views is outside [1, %d]", views, MOGE_PANORAMA_MAX_VIEWS);
-    *bytes = layout(views, h, w, batch).total;
-    return 0;
-}
-
-int moge_panorama_rhs_batch(const float* src, int channels, const uint8_t* mask, int batch, int views, int vh, int vw,
-                            const moge_panorama_camera_t* cams, const float* directions, int h, int w, double* b, uint8_t* row_mask,
-                            uint8_t* pano_mask, void* workspace, size_t workspace_bytes, void* stream) {
-    if (!src || !mask || !directions || !b || !row_mask || !pano_mask) return set_error("null argument");
-    if (channels != 1 && channels != 3) return set_error("panorama_rhs_batch: %d channels (1: distance, 3: points)", channels);
-    MG_TRY(check_batch("panorama_rhs_batch", batch));
-    MG_TRY(check_size("panorama_rhs_batch view", vh, vw));
-    MG_TRY(check_size("panorama_rhs_batch", h, w));
-    Cams cs;
-    MG_TRY(load_cams("panorama_rhs_batch", cams, views, &cs));
-    const Layout l = layout(views, h, w, batch);
-    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "panorama_rhs_batch"));
-    int sms;
-    MG_TRY(check_device("panorama_rhs_batch", &sms));
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    char* ws = static_cast<char*>(workspace);
-    float* L = reinterpret_cast<float*>(ws + l.L);
-    uint8_t* M = reinterpret_cast<uint8_t*>(ws + l.M);
-    const int64_t n = static_cast<int64_t>(h) * w * batch;
-    sample_batch_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(src, channels, mask, batch, vh, vw, cs, directions, h, w, L, M);
-    CUDA_TRY(cudaGetLastError());
-    rhs_batch_kernel<<<blocks_for(n, sms), kThreads, 0, st>>>(L, M, batch, views, h, w, b, row_mask, pano_mask);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
-}
-
-int moge_panorama_lsmr_batch(const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
-                             int32_t* stats, void* workspace, size_t workspace_bytes, void* stream) {
-    return lsmr("panorama_lsmr_batch", b, row_mask, batch, h, w, init, depth, stats, workspace, workspace_bytes, stream);
-}
-
-int moge_panorama_resize_batch(const float* src, int batch, int h, int w, int H, int W, float* dst, void* stream) {
-    if (!src || !dst) return set_error("null argument");
-    MG_TRY(check_batch("panorama_resize_batch", batch));
-    MG_TRY(check_size("panorama_resize_batch", h, w));
-    MG_TRY(check_size("panorama_resize_batch", H, W));
-    int sms;
-    MG_TRY(check_device("panorama_resize_batch", &sms));
-    resize_batch_kernel<<<blocks_for(static_cast<int64_t>(H) * W * batch, sms), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        src, batch, h, w, H, W, dst);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
-}
-
-int moge_panorama_finish_batch(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
-                               uint8_t* mask_out, float* points, void* stream) {
-    if (!depth || !mask || !depth_out || !mask_out || !points) return set_error("null argument");
-    MG_TRY(check_batch("panorama_finish_batch", batch));
-    MG_TRY(check_size("panorama_finish_batch", h, w));
-    MG_TRY(check_size("panorama_finish_batch", H, W));
-    int sms;
-    MG_TRY(check_device("panorama_finish_batch", &sms));
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const unsigned blocks = blocks_for(static_cast<int64_t>(H) * W * batch, sms);
-    resize_batch_kernel<<<blocks, kThreads, 0, st>>>(depth, batch, h, w, H, W, depth_out);
-    CUDA_TRY(cudaGetLastError());
-    finish_batch_kernel<<<blocks, kThreads, 0, st>>>(depth_out, mask, batch, h, w, H, W, mask_out, points);
+    finish_kernel<<<grid, kThreads, 0, st>>>(depth_out, mask, h, w, H, W, mask_out, points);
     CUDA_TRY(cudaGetLastError());
     return 0;
 }

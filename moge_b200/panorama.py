@@ -6,8 +6,9 @@ through one `model.infer(views, fov_x=..., apply_mask=False)` call, and the view
 by a gradient-domain least-squares solve (SciPy's LSMR on a 4-level pyramid at up to 1920 x 960), then resized to the input.
 
 The batch forms (`split_panoramas`, `merge_panoramas`, `finish_panoramas`, `infer_panoramas`) take up to 64 panoramas of one size
-with the same cameras and give each one bitwise what the single call gives it; the merge solves every panorama's system of a
-level in one cooperative launch, so the panoramas share that launch's grid barriers.
+with the same cameras; the merge solves every panorama's system of a level in one cooperative launch, so the panoramas share
+that launch's grid barriers.  The single-panorama functions run the same code as a batch of one, so each panorama of a batch
+gets bitwise what its single call gives it.
 
 The work runs in moge_b200/csrc/panorama.cu: a split kernel that samples the uint8 panorama as cv2.remap does, a per-level
 right-hand-side pass that reads log |points| straight from the engine's output, a matrix-free LSMR in one cooperative kernel
@@ -142,7 +143,45 @@ def _check_size(what: str, h: int, w: int) -> None:
     capi.check_pixels(what, h, w, MAX_PIXELS)
 
 
+def _check_batch(what: str, batch: int) -> None:
+    if not 1 <= batch <= MAX_BATCH:
+        raise MogeError(f"{what}: a batch of {batch} panoramas is outside [1, {MAX_BATCH}]")
+
+
+def _check_images(what: str, images) -> Tuple[int, int, int]:
+    if not isinstance(images, torch.Tensor) or images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] != 3:
+        raise MogeError(f"{what}: images must be a (P, H, W, 3) uint8 tensor")
+    P, H, W = images.shape[:3]
+    _check_batch(what, P)
+    _check_size(what, H, W)
+    capi.require_cuda(what, images)
+    return P, H, W
+
+
+# Each stage has one implementation over a batch of P panoramas (_split, _merge, _finish, _infer), called after the public
+# function's own argument checks with the name it raises under; a single-panorama function passes a batch of one and drops
+# the leading dimension of the results.
+
 # ------------------------------------------------------------------------------------------------------------ split
+def _split(what: str, images: torch.Tensor, extrinsics, intrinsics, resolution: int, return_uint8: bool):
+    P, H, W = images.shape[:3]
+    if not 1 <= int(resolution) <= 8192:
+        raise MogeError(f"{what}: resolution {resolution} is outside [1, 8192]")
+    res = int(resolution)
+    if extrinsics is None:
+        extrinsics, intrinsics = _default_cameras()
+    cams, n = _cameras(extrinsics, intrinsics)
+    dev = images.device
+    with torch.cuda.device(dev):
+        img = images.contiguous()
+        out = torch.empty(P, n, 3, res, res, dtype=torch.float32, device=dev)
+        u8 = torch.empty(P, n, res, res, 3, dtype=torch.uint8, device=dev) if return_uint8 else None
+        grid = _table("grid", (res, res), dev)
+        capi.check(capi.lib().moge_panorama_split(img.data_ptr(), P, H, W, cams, n, grid.data_ptr(), res, out.data_ptr(), capi.ptr(u8),
+                                                  capi.current_stream()))
+    return out, u8
+
+
 def split_panorama(image: torch.Tensor, extrinsics=None, intrinsics=None, resolution: int = SPLIT_RESOLUTION,
                    return_uint8: bool = False):
     """split_panorama_image on the device: image (H, W, 3) uint8 RGB CUDA tensor -> views (N, 3, res, res) float32 (value / 255,
@@ -153,20 +192,17 @@ def split_panorama(image: torch.Tensor, extrinsics=None, intrinsics=None, resolu
     H, W = image.shape[:2]
     _check_size("split_panorama", H, W)
     capi.require_cuda("split_panorama", image)
-    if not 1 <= int(resolution) <= 8192:
-        raise MogeError(f"split_panorama: resolution {resolution} is outside [1, 8192]")
-    res = int(resolution)
-    if extrinsics is None:
-        extrinsics, intrinsics = _default_cameras()
-    cams, n = _cameras(extrinsics, intrinsics)
-    dev = image.device
-    with torch.cuda.device(dev):
-        img = image.contiguous()
-        out = torch.empty(n, 3, res, res, dtype=torch.float32, device=dev)
-        u8 = torch.empty(n, res, res, 3, dtype=torch.uint8, device=dev) if return_uint8 else None
-        grid = _table("grid", (res, res), dev)
-        capi.check(capi.lib().moge_panorama_split(img.data_ptr(), H, W, cams, n, grid.data_ptr(), res, out.data_ptr(), capi.ptr(u8),
-                                                  capi.current_stream()))
+    out, u8 = _split("split_panorama", image[None], extrinsics, intrinsics, resolution, return_uint8)
+    return (out[0], u8[0]) if return_uint8 else out[0]
+
+
+def split_panoramas(images: torch.Tensor, extrinsics=None, intrinsics=None, resolution: int = SPLIT_RESOLUTION,
+                    return_uint8: bool = False):
+    """split_panorama of P panoramas of one size in one launch: images (P, H, W, 3) uint8 RGB CUDA tensor -> views
+    (P, N, 3, res, res) float32, and with return_uint8 also (P, N, res, res, 3) uint8; each panorama's views are bitwise its
+    split_panorama."""
+    _check_images("split_panoramas", images)
+    out, u8 = _split("split_panoramas", images, extrinsics, intrinsics, resolution, return_uint8)
     return (out, u8) if return_uint8 else out
 
 
@@ -187,6 +223,48 @@ def num_rows(h: int, w: int) -> int:
     return 2 * h * w + (h - 1) * (w + 1)
 
 
+def _merge(what: str, width: int, height: int, src: torch.Tensor, mask: torch.Tensor, extrinsics, intrinsics, return_levels: bool):
+    """The merge of src (P, N, vh, vw[, 3]) and mask (P, N, vh, vw), whose types and shapes the caller has checked."""
+    P, n, vh, vw = src.shape[:4]
+    _check_batch(what, P)
+    capi.require_cuda(what, src, mask)
+    _check_size(f"{what} view", vh, vw)
+    if extrinsics is None:
+        extrinsics, intrinsics = _default_cameras()
+    cams, nc = _cameras(extrinsics, intrinsics)
+    if nc != n:
+        raise MogeError(f"{what}: {n} views but {nc} cameras")
+    channels = 1 if src.dim() == 4 else 3
+    dev = src.device
+    L = capi.lib()
+    levels = _levels(width, height)
+    with torch.cuda.device(dev):
+        st = capi.current_stream()
+        s = src.detach().contiguous()
+        m = capi.mask_u8(mask)
+        ws = capi.workspace(L.moge_panorama_workspace_bytes, P, n, height, width, device=dev)
+        stats = torch.zeros(len(levels), P, 2, dtype=torch.int32, device=dev)
+        depth, init, out = None, None, []
+        for lv, (w, h) in enumerate(levels):
+            b = torch.empty(P, num_rows(h, w), dtype=torch.float64, device=dev)
+            rm = torch.empty(P, num_rows(h, w), dtype=torch.uint8, device=dev)
+            pm = torch.empty(P, h, w, dtype=torch.uint8, device=dev)
+            dirs = _table("dirs", (h, w), dev)
+            capi.check(L.moge_panorama_rhs(s.data_ptr(), channels, m.data_ptr(), P, n, vh, vw, cams, dirs.data_ptr(), h, w, b.data_ptr(),
+                                           rm.data_ptr(), pm.data_ptr(), ws.data_ptr(), ws.numel(), st))
+            depth = torch.empty(P, h, w, dtype=torch.float32, device=dev)
+            capi.check(L.moge_panorama_lsmr(b.data_ptr(), rm.data_ptr(), P, h, w, capi.ptr(init), depth.data_ptr(), stats[lv].data_ptr(),
+                                            ws.data_ptr(), ws.numel(), st))
+            if return_levels:
+                out.append({"width": w, "height": h, "b": b, "row_mask": rm, "depth": depth})
+            if lv + 1 < len(levels):
+                W2, H2 = levels[lv + 1]
+                init = torch.empty(P, H2, W2, dtype=torch.float32, device=dev)
+                capi.check(L.moge_panorama_resize(depth.data_ptr(), P, h, w, H2, W2, init.data_ptr(), st))
+    _last.update(levels=levels, stats=stats)
+    return depth, pm.view(torch.bool), out
+
+
 def merge_panorama(width: int, height: int, src: torch.Tensor, mask: torch.Tensor, extrinsics=None, intrinsics=None,
                    return_levels: bool = False):
     """merge_panorama_depth on the device: src (N, vh, vw) distance maps, or (N, vh, vw, 3) point maps whose norms are the
@@ -200,118 +278,12 @@ def merge_panorama(width: int, height: int, src: torch.Tensor, mask: torch.Tenso
         raise MogeError("merge_panorama: src must be float32 (N, vh, vw) distances or (N, vh, vw, 3) points")
     if not isinstance(mask, torch.Tensor) or tuple(mask.shape) != tuple(src.shape[:3]) or mask.dtype not in (torch.bool, torch.uint8):
         raise MogeError(f"merge_panorama: mask must be bool / uint8 of shape {tuple(src.shape[:3])}")
-    capi.require_cuda("merge_panorama", src, mask)
-    n, vh, vw = src.shape[:3]
-    _check_size("merge_panorama view", vh, vw)
-    if extrinsics is None:
-        extrinsics, intrinsics = _default_cameras()
-    cams, nc = _cameras(extrinsics, intrinsics)
-    if nc != n:
-        raise MogeError(f"merge_panorama: {n} views but {nc} cameras")
-    channels = 1 if src.dim() == 3 else 3
-    dev = src.device
-    L = capi.lib()
-    levels = _levels(width, height)
-    with torch.cuda.device(dev):
-        st = capi.current_stream()
-        s = src.detach().contiguous()
-        m = capi.mask_u8(mask)
-        ws = capi.workspace(L.moge_panorama_workspace_bytes, n, height, width, device=dev)
-        stats = torch.zeros(len(levels), 2, dtype=torch.int32, device=dev)
-        depth, init, out = None, None, []
-        for lv, (w, h) in enumerate(levels):
-            b = torch.empty(num_rows(h, w), dtype=torch.float64, device=dev)
-            rm = torch.empty(num_rows(h, w), dtype=torch.uint8, device=dev)
-            pm = torch.empty(h, w, dtype=torch.uint8, device=dev)
-            dirs = _table("dirs", (h, w), dev)
-            capi.check(L.moge_panorama_rhs(s.data_ptr(), channels, m.data_ptr(), n, vh, vw, cams, dirs.data_ptr(), h, w, b.data_ptr(),
-                                           rm.data_ptr(), pm.data_ptr(), ws.data_ptr(), ws.numel(), st))
-            depth = torch.empty(h, w, dtype=torch.float32, device=dev)
-            capi.check(L.moge_panorama_lsmr(b.data_ptr(), rm.data_ptr(), h, w, capi.ptr(init), depth.data_ptr(), stats[lv].data_ptr(),
-                                            ws.data_ptr(), ws.numel(), st))
-            if return_levels:
-                out.append({"width": w, "height": h, "b": b, "row_mask": rm, "depth": depth})
-            if lv + 1 < len(levels):
-                W2, H2 = levels[lv + 1]
-                init = torch.empty(H2, W2, dtype=torch.float32, device=dev)
-                capi.check(L.moge_panorama_resize(depth.data_ptr(), h, w, H2, W2, init.data_ptr(), st))
-    _last.update(levels=levels, stats=stats, batched=False)
-    result = (depth, pm.view(torch.bool))
-    return (*result, out) if return_levels else result
-
-
-def last_merge_stats() -> list:
-    """Per level of the most recent merge_panorama call on this thread's process, coarsest first: width, height, LSMR iterations
-    and istop (SciPy's stopping reason).  After merge_panoramas, one such list per panorama.  Reading them copies the counters to
-    the host."""
-    if not _last:
-        return []
-    stats = _last["stats"].cpu().tolist()
-
-    def per_level(rows):
-        return [{"width": w, "height": h, "iterations": it, "istop": st} for (w, h), (it, st) in zip(_last["levels"], rows)]
-    if _last["batched"]:
-        return [per_level([lv[k] for lv in stats]) for k in range(len(stats[0]))]
-    return per_level(stats)
-
-
-def finish_panorama(depth: torch.Tensor, mask: torch.Tensor, height: int, width: int):
-    """infer_panorama.py:119-122: the merged depth and mask resized to (height, width) as cv2.resize does, and the points."""
-    capi.require_cuda("finish_panorama", depth, mask)
-    if depth.dtype != torch.float32 or depth.dim() != 2 or tuple(mask.shape) != tuple(depth.shape):
-        raise MogeError("finish_panorama: depth must be float32 (h, w) and mask (h, w)")
-    h, w = depth.shape
-    _check_size("finish_panorama", h, w)
-    _check_size("finish_panorama", height, width)
-    dev = depth.device
-    with torch.cuda.device(dev):
-        d = depth.contiguous()
-        m = capi.mask_u8(mask)
-        out_d = torch.empty(height, width, dtype=torch.float32, device=dev)
-        out_m = torch.empty(height, width, dtype=torch.uint8, device=dev)
-        points = torch.empty(height, width, 3, dtype=torch.float32, device=dev)
-        capi.check(capi.lib().moge_panorama_finish(d.data_ptr(), m.data_ptr(), h, w, height, width, out_d.data_ptr(), out_m.data_ptr(),
-                                                   points.data_ptr(), capi.current_stream()))
-    return out_d, out_m.view(torch.bool), points
-
-
-# ------------------------------------------------------------------------------------------------------------ batches
-def _check_batch(what: str, batch: int) -> None:
-    if not 1 <= batch <= MAX_BATCH:
-        raise MogeError(f"{what}: a batch of {batch} panoramas is outside [1, {MAX_BATCH}]")
-
-
-def _check_images(what: str, images) -> Tuple[int, int, int]:
-    if not isinstance(images, torch.Tensor) or images.dtype != torch.uint8 or images.dim() != 4 or images.shape[3] != 3:
-        raise MogeError(f"{what}: images must be a (P, H, W, 3) uint8 tensor")
-    P, H, W = images.shape[:3]
-    _check_batch(what, P)
-    _check_size(what, H, W)
-    capi.require_cuda(what, images)
-    return P, H, W
-
-
-def split_panoramas(images: torch.Tensor, extrinsics=None, intrinsics=None, resolution: int = SPLIT_RESOLUTION,
-                    return_uint8: bool = False):
-    """split_panorama of P panoramas of one size in one launch: images (P, H, W, 3) uint8 RGB CUDA tensor -> views
-    (P, N, 3, res, res) float32, and with return_uint8 also (P, N, res, res, 3) uint8; each panorama's views are bitwise its
-    split_panorama."""
-    P, H, W = _check_images("split_panoramas", images)
-    if not 1 <= int(resolution) <= 8192:
-        raise MogeError(f"split_panoramas: resolution {resolution} is outside [1, 8192]")
-    res = int(resolution)
-    if extrinsics is None:
-        extrinsics, intrinsics = _default_cameras()
-    cams, n = _cameras(extrinsics, intrinsics)
-    dev = images.device
-    with torch.cuda.device(dev):
-        img = images.contiguous()
-        out = torch.empty(P, n, 3, res, res, dtype=torch.float32, device=dev)
-        u8 = torch.empty(P, n, res, res, 3, dtype=torch.uint8, device=dev) if return_uint8 else None
-        grid = _table("grid", (res, res), dev)
-        capi.check(capi.lib().moge_panorama_split_batch(img.data_ptr(), P, H, W, cams, n, grid.data_ptr(), res, out.data_ptr(),
-                                                        capi.ptr(u8), capi.current_stream()))
-    return (out, u8) if return_uint8 else out
+    depth, pm, levels = _merge("merge_panorama", width, height, src[None], mask[None], extrinsics, intrinsics, return_levels)
+    _last["stats"] = _last["stats"][:, 0]
+    result = (depth[0], pm[0])
+    if return_levels:
+        return (*result, [{k: v[0] if isinstance(v, torch.Tensor) else v for k, v in lv.items()} for lv in levels])
+    return result
 
 
 def merge_panoramas(width: int, height: int, src: torch.Tensor, mask: torch.Tensor, extrinsics=None, intrinsics=None,
@@ -326,45 +298,49 @@ def merge_panoramas(width: int, height: int, src: torch.Tensor, mask: torch.Tens
         raise MogeError("merge_panoramas: src must be float32 (P, N, vh, vw) distances or (P, N, vh, vw, 3) points")
     if not isinstance(mask, torch.Tensor) or tuple(mask.shape) != tuple(src.shape[:4]) or mask.dtype not in (torch.bool, torch.uint8):
         raise MogeError(f"merge_panoramas: mask must be bool / uint8 of shape {tuple(src.shape[:4])}")
-    P, n, vh, vw = src.shape[:4]
-    _check_batch("merge_panoramas", P)
-    capi.require_cuda("merge_panoramas", src, mask)
-    _check_size("merge_panoramas view", vh, vw)
-    if extrinsics is None:
-        extrinsics, intrinsics = _default_cameras()
-    cams, nc = _cameras(extrinsics, intrinsics)
-    if nc != n:
-        raise MogeError(f"merge_panoramas: {n} views but {nc} cameras")
-    channels = 1 if src.dim() == 4 else 3
-    dev = src.device
-    L = capi.lib()
-    levels = _levels(width, height)
+    depth, pm, levels = _merge("merge_panoramas", width, height, src, mask, extrinsics, intrinsics, return_levels)
+    return (depth, pm, levels) if return_levels else (depth, pm)
+
+
+def last_merge_stats() -> list:
+    """Per level of the most recent merge_panorama call on this thread's process, coarsest first: width, height, LSMR iterations
+    and istop (SciPy's stopping reason).  After merge_panoramas, one such list per panorama.  Reading them copies the counters to
+    the host."""
+    if not _last:
+        return []
+    batched = _last["stats"].dim() == 3              # (levels, P, 2) after merge_panoramas, (levels, 2) after merge_panorama
+    stats = _last["stats"].cpu().tolist()
+
+    def per_level(rows):
+        return [{"width": w, "height": h, "iterations": it, "istop": st} for (w, h), (it, st) in zip(_last["levels"], rows)]
+    if batched:
+        return [per_level([lv[k] for lv in stats]) for k in range(len(stats[0]))]
+    return per_level(stats)
+
+
+# ------------------------------------------------------------------------------------------------------------ finish
+def _finish(what: str, depth: torch.Tensor, mask: torch.Tensor, height: int, width: int):
+    P, h, w = depth.shape
+    _check_size(what, h, w)
+    _check_size(what, height, width)
+    dev = depth.device
     with torch.cuda.device(dev):
-        st = capi.current_stream()
-        s = src.detach().contiguous()
+        d = depth.contiguous()
         m = capi.mask_u8(mask)
-        ws = capi.workspace(L.moge_panorama_workspace_bytes_batch, P, n, height, width, device=dev)
-        stats = torch.zeros(len(levels), P, 2, dtype=torch.int32, device=dev)
-        depth, init, out = None, None, []
-        for lv, (w, h) in enumerate(levels):
-            b = torch.empty(P, num_rows(h, w), dtype=torch.float64, device=dev)
-            rm = torch.empty(P, num_rows(h, w), dtype=torch.uint8, device=dev)
-            pm = torch.empty(P, h, w, dtype=torch.uint8, device=dev)
-            dirs = _table("dirs", (h, w), dev)
-            capi.check(L.moge_panorama_rhs_batch(s.data_ptr(), channels, m.data_ptr(), P, n, vh, vw, cams, dirs.data_ptr(), h, w,
-                                                 b.data_ptr(), rm.data_ptr(), pm.data_ptr(), ws.data_ptr(), ws.numel(), st))
-            depth = torch.empty(P, h, w, dtype=torch.float32, device=dev)
-            capi.check(L.moge_panorama_lsmr_batch(b.data_ptr(), rm.data_ptr(), P, h, w, capi.ptr(init), depth.data_ptr(),
-                                                  stats[lv].data_ptr(), ws.data_ptr(), ws.numel(), st))
-            if return_levels:
-                out.append({"width": w, "height": h, "b": b, "row_mask": rm, "depth": depth})
-            if lv + 1 < len(levels):
-                W2, H2 = levels[lv + 1]
-                init = torch.empty(P, H2, W2, dtype=torch.float32, device=dev)
-                capi.check(L.moge_panorama_resize_batch(depth.data_ptr(), P, h, w, H2, W2, init.data_ptr(), st))
-    _last.update(levels=levels, stats=stats, batched=True)
-    result = (depth, pm.view(torch.bool))
-    return (*result, out) if return_levels else result
+        out_d = torch.empty(P, height, width, dtype=torch.float32, device=dev)
+        out_m = torch.empty(P, height, width, dtype=torch.uint8, device=dev)
+        points = torch.empty(P, height, width, 3, dtype=torch.float32, device=dev)
+        capi.check(capi.lib().moge_panorama_finish(d.data_ptr(), m.data_ptr(), P, h, w, height, width, out_d.data_ptr(),
+                                                   out_m.data_ptr(), points.data_ptr(), capi.current_stream()))
+    return out_d, out_m.view(torch.bool), points
+
+
+def finish_panorama(depth: torch.Tensor, mask: torch.Tensor, height: int, width: int):
+    """infer_panorama.py:119-122: the merged depth and mask resized to (height, width) as cv2.resize does, and the points."""
+    capi.require_cuda("finish_panorama", depth, mask)
+    if depth.dtype != torch.float32 or depth.dim() != 2 or tuple(mask.shape) != tuple(depth.shape):
+        raise MogeError("finish_panorama: depth must be float32 (h, w) and mask (h, w)")
+    return tuple(t[0] for t in _finish("finish_panorama", depth[None], mask[None], height, width))
 
 
 def finish_panoramas(depth: torch.Tensor, mask: torch.Tensor, height: int, width: int):
@@ -373,21 +349,9 @@ def finish_panoramas(depth: torch.Tensor, mask: torch.Tensor, height: int, width
     if not isinstance(depth, torch.Tensor) or not isinstance(mask, torch.Tensor) or depth.dtype != torch.float32 or depth.dim() != 3 \
             or tuple(mask.shape) != tuple(depth.shape):
         raise MogeError("finish_panoramas: depth must be float32 (P, h, w) and mask (P, h, w)")
-    P, h, w = depth.shape
-    _check_batch("finish_panoramas", P)
+    _check_batch("finish_panoramas", depth.shape[0])
     capi.require_cuda("finish_panoramas", depth, mask)
-    _check_size("finish_panoramas", h, w)
-    _check_size("finish_panoramas", height, width)
-    dev = depth.device
-    with torch.cuda.device(dev):
-        d = depth.contiguous()
-        m = capi.mask_u8(mask)
-        out_d = torch.empty(P, height, width, dtype=torch.float32, device=dev)
-        out_m = torch.empty(P, height, width, dtype=torch.uint8, device=dev)
-        points = torch.empty(P, height, width, 3, dtype=torch.float32, device=dev)
-        capi.check(capi.lib().moge_panorama_finish_batch(d.data_ptr(), m.data_ptr(), P, h, w, height, width, out_d.data_ptr(),
-                                                         out_m.data_ptr(), points.data_ptr(), capi.current_stream()))
-    return out_d, out_m.view(torch.bool), points
+    return _finish("finish_panoramas", depth, mask, height, width)
 
 
 # ------------------------------------------------------------------------------------------------------------ end to end
@@ -396,6 +360,30 @@ def _fov_x(intrinsics, device) -> torch.Tensor:
     K = np.asarray(intrinsics)
     fov_x = np.rad2deg(2 * np.arctan(0.5 / K[..., 0, 0]))
     return torch.tensor(fov_x, dtype=torch.float32, device=device)
+
+
+def _infer(what: str, model, images: torch.Tensor, batch_size: Optional[int], return_views: bool) -> Dict[str, torch.Tensor]:
+    P, H, W = images.shape[:3]
+    extrinsics, intrinsics = _default_cameras()
+    views, views_u8 = _split(what, images, extrinsics, intrinsics, SPLIT_RESOLUTION, return_views)
+    n = views.shape[1]
+    flat = views.view(P * n, *views.shape[2:])
+    fov_x = _fov_x(intrinsics, images.device).repeat(P)
+    step = len(flat) if batch_size is None else int(batch_size)
+    points, masks = [], []
+    for lo in range(0, len(flat), step):
+        out = model.infer(flat[lo:lo + step], fov_x=fov_x[lo:lo + step], apply_mask=False)
+        points.append(out['points'])
+        masks.append(out['mask'])
+    points = points[0] if len(points) == 1 else torch.cat(points)
+    masks = masks[0] if len(masks) == 1 else torch.cat(masks)
+    view_points, view_masks = points.reshape(P, n, *points.shape[1:]), masks.reshape(P, n, *masks.shape[1:])
+    depth, mask, _ = _merge(what, min(MERGE_WIDTH, W), min(MERGE_HEIGHT, H), view_points, view_masks, extrinsics, intrinsics, False)
+    depth, mask, points = _finish(what, depth, mask, H, W)
+    out = {'depth': depth, 'mask': mask, 'points': points}
+    if return_views:
+        out.update(views=views_u8, view_distance=view_points.norm(dim=-1), view_mask=view_masks)
+    return out
 
 
 def infer_panorama(model, image: torch.Tensor, batch_size: Optional[int] = None, return_views: bool = False) -> Dict[str, torch.Tensor]:
@@ -411,26 +399,9 @@ def infer_panorama(model, image: torch.Tensor, batch_size: Optional[int] = None,
     capi.require_cuda("infer_panorama", image)
     H, W = image.shape[:2]
     _check_size("infer_panorama", H, W)
-    extrinsics, intrinsics = _default_cameras()
-    views = split_panorama(image, extrinsics, intrinsics, SPLIT_RESOLUTION, return_uint8=return_views)
-    if return_views:
-        views, views_u8 = views
-    fov_x = _fov_x(intrinsics, image.device)
-    step = len(views) if batch_size is None else int(batch_size)
-    points, masks = [], []
-    for lo in range(0, len(views), step):
-        out = model.infer(views[lo:lo + step], fov_x=fov_x[lo:lo + step], apply_mask=False)
-        points.append(out['points'])
-        masks.append(out['mask'])
-    points = points[0] if len(points) == 1 else torch.cat(points)
-    masks = masks[0] if len(masks) == 1 else torch.cat(masks)
-    depth, mask = merge_panorama(min(MERGE_WIDTH, W), min(MERGE_HEIGHT, H), points, masks, extrinsics, intrinsics)
-    view_points, view_masks = points, masks
-    depth, mask, points = finish_panorama(depth, mask, H, W)
-    out = {'depth': depth, 'mask': mask, 'points': points}
-    if return_views:
-        out.update(views=views_u8, view_distance=view_points.norm(dim=-1), view_mask=view_masks)
-    return out
+    out = _infer("infer_panorama", model, image[None], batch_size, return_views)
+    _last["stats"] = _last["stats"][:, 0]
+    return {k: v[0] for k, v in out.items()}
 
 
 def infer_panoramas(model, images: torch.Tensor, batch_size: Optional[int] = None, return_views: bool = False) -> Dict[str, torch.Tensor]:
@@ -441,26 +412,5 @@ def infer_panoramas(model, images: torch.Tensor, batch_size: Optional[int] = Non
     Each panorama's outputs are bitwise its infer_panorama."""
     if batch_size is not None and int(batch_size) < 1:
         raise MogeError(f"infer_panoramas: batch_size {batch_size} must be positive")
-    P, H, W = _check_images("infer_panoramas", images)
-    extrinsics, intrinsics = _default_cameras()
-    views = split_panoramas(images, extrinsics, intrinsics, SPLIT_RESOLUTION, return_uint8=return_views)
-    if return_views:
-        views, views_u8 = views
-    n = views.shape[1]
-    flat = views.view(P * n, *views.shape[2:])
-    fov_x = _fov_x(intrinsics, images.device).repeat(P)
-    step = len(flat) if batch_size is None else int(batch_size)
-    points, masks = [], []
-    for lo in range(0, len(flat), step):
-        out = model.infer(flat[lo:lo + step], fov_x=fov_x[lo:lo + step], apply_mask=False)
-        points.append(out['points'])
-        masks.append(out['mask'])
-    points = points[0] if len(points) == 1 else torch.cat(points)
-    masks = masks[0] if len(masks) == 1 else torch.cat(masks)
-    view_points, view_masks = points.reshape(P, n, *points.shape[1:]), masks.reshape(P, n, *masks.shape[1:])
-    depth, mask = merge_panoramas(min(MERGE_WIDTH, W), min(MERGE_HEIGHT, H), view_points, view_masks, extrinsics, intrinsics)
-    depth, mask, points = finish_panoramas(depth, mask, H, W)
-    out = {'depth': depth, 'mask': mask, 'points': points}
-    if return_views:
-        out.update(views=views_u8, view_distance=view_points.norm(dim=-1), view_mask=view_masks)
-    return out
+    _check_images("infer_panoramas", images)
+    return _infer("infer_panoramas", model, images, batch_size, return_views)

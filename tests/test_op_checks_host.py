@@ -53,7 +53,8 @@ CASES = {
     "metrics_stats_slots": ("metrics_stats", lambda: L.moge_metrics_stats(P, P, P, None, 0, P, P, P, 300, 1, 8, 8, P, P, P, BIG, None),
                             "outside"),
     "metrics_stats_ws_small": ("metrics_stats", lambda: L.moge_metrics_stats(P, P, P, P, 0, None, None, None, 0, 1, 8, 8, P, None, 256,
-                                                                             16, None), "bytes needed"),
+                                                                             16, None),
+                                     "bytes needed"),
     "metrics_stats_ws_null": ("metrics_stats", lambda: L.moge_metrics_stats(P, P, P, P, 0, None, None, None, 0, 1, 8, 8, P, None, None,
                                                                             BIG, None), "bytes needed"),
     "metrics_stats_ws_align": ("metrics_stats", lambda: L.moge_metrics_stats(P, P, P, P, 0, None, None, None, 0, 1, 8, 8, P, None, 264,
@@ -82,22 +83,30 @@ CASES = {
     "mesh_build_ws_small": ("mesh_build", lambda: L.moge_mesh_build(None, 1, 8, 8, 1, maps(), 1, P, P, 256, 16, None), "bytes needed"),
     "mesh_build_ws_align": ("mesh_build", lambda: L.moge_mesh_build(None, 1, 8, 8, 1, maps(), 1, P, P, 264, BIG, None),
                             "256-byte aligned"),
-    # panorama
-    "panorama_views": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(21, 8, 8, C.byref(NB)), "outside"),
-    "panorama_small": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(1, 1, 8, C.byref(NB)), "too small"),
-    "panorama_too_large": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(1, 40000, 30000, C.byref(NB)),
-                           "too large"),
-    "panorama_split_res": ("panorama_split", lambda: L.moge_panorama_split(P, 8, 8, camera(), 1, P, 0, P, None, None), "outside"),
-    "panorama_split_views": ("panorama_split", lambda: L.moge_panorama_split(P, 8, 8, camera(), 0, P, 8, P, None, None), "outside"),
-    "panorama_split_cams": ("panorama_split", lambda: L.moge_panorama_split(P, 8, 8, None, 1, P, 8, P, None, None), "null cameras"),
-    "panorama_rhs_null": ("", lambda: L.moge_panorama_rhs(P, 1, P, 1, 8, 8, camera(), P, 8, 8, None, P, P, 256, BIG, None),
-                          "null argument"),
-    "panorama_rhs_ws_small": ("panorama_rhs", lambda: L.moge_panorama_rhs(P, 1, P, 1, 8, 8, camera(), P, 8, 8, P, P, P, 256, 16, None),
-                              "bytes needed"),
-    "panorama_rhs_ws_align": ("panorama_rhs", lambda: L.moge_panorama_rhs(P, 1, P, 1, 8, 8, camera(), P, 8, 8, P, P, P, 264, BIG, None),
-                              "256-byte aligned"),
-    "panorama_lsmr_ws_small": ("panorama_lsmr", lambda: L.moge_panorama_lsmr(P, P, 8, 8, None, P, P, 256, 16, None), "bytes needed"),
-    "panorama_lsmr_ws_align": ("panorama_lsmr", lambda: L.moge_panorama_lsmr(P, P, 8, 8, None, P, P, 264, BIG, None), "256-byte aligned"),
+    # panorama: every entry point takes a batch; batch1 cases are one panorama
+    "panorama_batch_range": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(65, 1, 8, 8, C.byref(NB)),
+                             "batch of 65 panoramas"),
+    "panorama_batch1_views": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(1, 21, 8, 8, C.byref(NB)), "outside"),
+    "panorama_batch1_small": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(1, 1, 1, 8, C.byref(NB)), "too small"),
+    "panorama_batch1_too_large": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(1, 1, 40000, 30000, C.byref(NB)),
+                                  "too large"),
+    "panorama_batch1_split_res": ("panorama_split", lambda: L.moge_panorama_split(P, 1, 8, 8, camera(), 1, P, 0, P, None, None), "outside"),
+    "panorama_batch1_split_views": ("panorama_split", lambda: L.moge_panorama_split(P, 1, 8, 8, camera(), 0, P, 8, P, None, None),
+                                    "outside"),
+    "panorama_batch1_split_cams": ("panorama_split", lambda: L.moge_panorama_split(P, 1, 8, 8, None, 1, P, 8, P, None, None),
+                                   "null cameras"),
+    "panorama_batch1_rhs_null": ("", lambda: L.moge_panorama_rhs(P, 1, P, 1, 1, 8, 8, camera(), P, 8, 8, None, P, P, 256, BIG, None),
+                                 "null argument"),
+    "panorama_batch1_rhs_ws_small": ("panorama_rhs",
+                                     lambda: L.moge_panorama_rhs(P, 1, P, 1, 1, 8, 8, camera(), P, 8, 8, P, P, P, 256, 16, None),
+                                     "bytes needed"),
+    "panorama_batch1_rhs_ws_align": ("panorama_rhs",
+                                     lambda: L.moge_panorama_rhs(P, 1, P, 1, 1, 8, 8, camera(), P, 8, 8, P, P, P, 264, BIG, None),
+                                     "256-byte aligned"),
+    "panorama_batch1_lsmr_ws_small": ("panorama_lsmr", lambda: L.moge_panorama_lsmr(P, P, 1, 8, 8, None, P, P, 256, 16, None),
+                                      "bytes needed"),
+    "panorama_batch1_lsmr_ws_align": ("panorama_lsmr", lambda: L.moge_panorama_lsmr(P, P, 1, 8, 8, None, P, P, 264, BIG, None),
+                                      "256-byte aligned"),
     # losses
     "loss_batch": ("loss", lambda: L.moge_loss_workspace_bytes(0, 8, 8, C.byref(NB)), "outside"),
     "loss_size": ("loss", lambda: L.moge_loss_workspace_bytes(1, 8, 0, C.byref(NB)), "size"),
@@ -135,7 +144,7 @@ NO_DEVICE = {
     "align_affine_lstsq": ("align_affine_lstsq", lambda: L.moge_align_affine_lstsq(P, P, None, 1, 8, P, P, None)),
     "masked_nearest_resize": ("masked_nearest_resize", lambda: L.moge_metrics_resize(P, 1, 8, 8, 4, 4, P, P, P, P, P, None)),
     "mesh_count": ("mesh_count", lambda: L.moge_mesh_count(None, 1, 8, 8, P, 256, BIG, None)),
-    "panorama_resize": ("panorama_resize", lambda: L.moge_panorama_resize(P, 8, 8, 16, 16, P, None)),
+    "panorama_batch1_resize": ("panorama_resize", lambda: L.moge_panorama_resize(P, 1, 8, 8, 16, 16, P, None)),
     "loss_mask": ("loss_mask", lambda: L.moge_loss_mask(capi.LOSS_MASK_L2, P, P, P, 1, 8, 8, None, None, P, 256, BIG, None)),
 }
 

@@ -1,5 +1,6 @@
 """Batched panorama inference, host side (no GPU): the argument checks of split_panoramas, merge_panoramas, finish_panoramas and
-infer_panoramas fail with MogeError before any device work, and the batched C entry points are in the ABI table."""
+infer_panoramas fail with MogeError before any device work, and the panorama C entry points, which all take a batch, are in the
+ABI table."""
 import pytest
 import torch
 
@@ -8,9 +9,9 @@ from moge_b200 import panorama as P
 from moge_b200.capi import MogeError
 
 
-def test_batch_entry_points_in_signature_table():
-    for name in ("moge_panorama_split_batch", "moge_panorama_rhs_batch", "moge_panorama_lsmr_batch",
-                 "moge_panorama_workspace_bytes_batch", "moge_panorama_resize_batch", "moge_panorama_finish_batch"):
+def test_panorama_entry_points_in_signature_table():
+    for name in ("moge_panorama_split", "moge_panorama_rhs", "moge_panorama_lsmr", "moge_panorama_workspace_bytes",
+                 "moge_panorama_resize", "moge_panorama_finish"):
         assert name in capi.SIGNATURES and name in capi.EXPORTS
     assert capi.PANORAMA_MAX_BATCH == P.MAX_BATCH == 64
 

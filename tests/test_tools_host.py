@@ -8,8 +8,8 @@ import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 TOOLS = os.path.join(ROOT, "tools")
-BENCH = ["bench_align", "bench_cli", "bench_losses", "bench_mesh", "bench_metrics", "bench_panorama", "bench_panorama_mesh",
-         "bench_v1"]
+BENCH = ["bench_align", "bench_cli", "bench_losses", "bench_mesh", "bench_metrics", "bench_panorama", "bench_panorama_batch",
+         "bench_panorama_mesh", "bench_v1"]
 CALLS = [(name, "--help") for name in BENCH + ["prof_gemm"]] + [(name,) for name in BENCH]
 
 

@@ -67,7 +67,7 @@ def merge_levels_ms(src, mask, width, height, extr, intr):
     cams, n = P._cameras(extr, intr)
     levels = P._levels(width, height)
     nb = C.c_size_t()
-    capi.check(L.moge_panorama_workspace_bytes(n, height, width, C.byref(nb)))
+    capi.check(L.moge_panorama_workspace_bytes(1, n, height, width, C.byref(nb)))
     ws = torch.empty(nb.value, dtype=torch.uint8, device=DEV)
     stats = torch.zeros(len(levels), 2, dtype=torch.int32, device=DEV)
     s = src.contiguous()
@@ -82,18 +82,18 @@ def merge_levels_ms(src, mask, width, height, extr, intr):
         dirs = P._table("dirs", (h, w), torch.device(DEV))
         t = Timer()
         t.mark("start")
-        capi.check(L.moge_panorama_rhs(s.data_ptr(), ch, m.data_ptr(), n, s.shape[1], s.shape[2], cams, dirs.data_ptr(), h, w,
+        capi.check(L.moge_panorama_rhs(s.data_ptr(), ch, m.data_ptr(), 1, n, s.shape[1], s.shape[2], cams, dirs.data_ptr(), h, w,
                                        b.data_ptr(), rm.data_ptr(), pm.data_ptr(), ws.data_ptr(), ws.numel(), st))
         t.mark("rhs_ms")
         depth = torch.empty(h, w, dtype=torch.float32, device=DEV)
-        capi.check(L.moge_panorama_lsmr(b.data_ptr(), rm.data_ptr(), h, w, capi.ptr(init), depth.data_ptr(), stats[lv].data_ptr(),
+        capi.check(L.moge_panorama_lsmr(b.data_ptr(), rm.data_ptr(), 1, h, w, capi.ptr(init), depth.data_ptr(), stats[lv].data_ptr(),
                                         ws.data_ptr(), ws.numel(), st))
         t.mark("lsmr_ms")
         timers.append(t)
         if lv + 1 < len(levels):
             W2, H2 = levels[lv + 1]
             init = torch.empty(H2, W2, dtype=torch.float32, device=DEV)
-            capi.check(L.moge_panorama_resize(depth.data_ptr(), h, w, H2, W2, init.data_ptr(), st))
+            capi.check(L.moge_panorama_resize(depth.data_ptr(), 1, h, w, H2, W2, init.data_ptr(), st))
     torch.cuda.synchronize()
     it = stats.cpu().tolist()
     return [{"size": f"{w}x{h}", **{k: round(v, 3) for k, v in t.result().items()}, "iterations": i[0], "istop": i[1]}
