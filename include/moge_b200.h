@@ -268,6 +268,39 @@ int moge_op_conv_transpose_uv(const void* x, const float* w, const float* bias, 
  * for a resize of `in` to `out` samples; returns n (< 0 on error) */
 int moge_bicubic_aa_weights(int in, int out, int i, int* lo, float* w, int cap);
 
+/* ---- the DINOv2 backbone on its own (moge/model/dinov2: models/vision_transformer.py DinoVisionTransformer, hub/backbones.py;
+ * Python: moge_b200.dinov2, aliases under moge.model.dinov2).  The same encoder kernels as the MoGe engines; the input is an image
+ * that is already normalised (no resize, no mean / std), its H and W multiples of 14.  moge_dino_create returns an engine that
+ * destroy / set_weight / finalize / num_ops / op_info / profile take unchanged; its weight keys are the backbone's own state-dict
+ * keys (patch_embed.proj.weight, blocks.{i}.attn.qkv.weight, norm.weight, pos_embed, ...; mask_token is not read).  Configs the
+ * encoder kernels do not cover fail at create: registers, SwiGLU / identity FFNs (ViT-g), other patch sizes, antialiased or
+ * offset-free pos-embed interpolation, head_dim != 64, embed_dim not a multiple of 128 or above 1024. */
+enum { MOGE_DINO_FFN_MLP = 0, MOGE_DINO_FFN_SWIGLU = 1, MOGE_DINO_FFN_IDENTITY = 2 };
+typedef struct moge_dino_config {
+    int embed_dim, depth, num_heads;
+    int patch_size;                       /* 14 only */
+    int num_register_tokens;              /* 0 only */
+    float interpolate_offset;             /* 0.1 only */
+    int interpolate_antialias;            /* 0 only */
+    int ffn_layer;                        /* MOGE_DINO_FFN_MLP only */
+    int compute_dtype;                    /* MOGE_F16 or MOGE_BF16 */
+} moge_dino_config_t;
+int moge_dino_create(const moge_dino_config_t* cfg, int device, moge_engine_t** out);
+/* forward flags: MOGE_DINO_NORM applies the final LayerNorm (`norm`) to the exported rows; MOGE_DINO_CHANNEL_MAJOR writes the
+ * patch tokens as (B, D, h, w) instead of (B, T, D) */
+#define MOGE_DINO_NORM 1
+#define MOGE_DINO_CHANNEL_MAJOR 2
+int moge_dino_workspace_bytes(moge_engine_t* e, int B, int H, int W, const int* layers, int n_layers, int flags, size_t* bytes);
+/* x (B,3,H,W), dtype x_dtype (MOGE_F32/F16/BF16), normalised; h = H/14, w = W/14, T = h*w.  layers: n_layers (0..depth) strictly
+ * increasing block indices; after block layers[j] the residual stream (or its final LayerNorm, MOGE_DINO_NORM) is written, fp32:
+ *   out_tokens  layer j at out_tokens + j*B*T*D, as (B,T,D) or, with MOGE_DINO_CHANNEL_MAJOR, (B,D,h,w)
+ *   out_cls     layer j's class-token rows at out_cls + j*B*D, (B,D)
+ *   out_prenorm the residual stream after the last block, (B,T+1,D), the class token first
+ * Any output may be NULL.  Rows are normalised with fixed-order statistics and no atomics: the outputs of an image are bitwise the
+ * same run to run. */
+int moge_dino_forward(moge_engine_t* e, const void* x, int x_dtype, int B, int H, int W, const int* layers, int n_layers, int flags,
+                      float* out_tokens, float* out_cls, float* out_prenorm, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- truncated-L1 alignment solvers (moge/utils/alignment.py; Python: moge_b200.alignment, alias moge.utils.alignment).
  * A problem is n elements (x, y, w), w >= 0; it is solved as align() (alignment.py:52-146) solves it: after x, y *= sign(x), either
  * the lower weighted median of y / max(x, 1e-7) with weights w x (untruncated) or the least of sum_i min(t_i, w_i |a x_i - y_i|) over

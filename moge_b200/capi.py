@@ -34,6 +34,8 @@ VIS_MAX_QUANTILES = 4
 VIS_DEPTH, VIS_VALUE = 0, 1
 GEOMETRY_MAX_REFINE_KERNEL, GEOMETRY_MAX_POOL_KERNEL, GEOMETRY_MAX_BLUR_KERNEL = 9, 15, 31
 DILATE = {"mean": 0, "min": 1, "max": 2, "median": 3}
+DINO_FFN = {"mlp": 0, "swiglu": 1, "swiglufused": 1, "identity": 2}
+DINO_NORM, DINO_CHANNEL_MAJOR = 1, 2
 
 
 class StackConfig(C.Structure):
@@ -81,6 +83,15 @@ class V1Group(C.Structure):
         ("image", C.c_void_p), ("image_dtype", C.c_int),
         ("B", C.c_int), ("H", C.c_int), ("W", C.c_int), ("rh", C.c_int), ("rw", C.c_int),
         ("points", C.c_void_p), ("mask", C.c_void_p),
+    ]
+
+
+class DinoConfig(C.Structure):
+    """moge_dino_config_t: the DINOv2 backbone on its own (moge/model/dinov2)."""
+    _fields_ = [
+        ("embed_dim", C.c_int), ("depth", C.c_int), ("num_heads", C.c_int), ("patch_size", C.c_int),
+        ("num_register_tokens", C.c_int), ("interpolate_offset", C.c_float), ("interpolate_antialias", C.c_int),
+        ("ffn_layer", C.c_int), ("compute_dtype", C.c_int),
     ]
 
 
@@ -190,6 +201,9 @@ SIGNATURES = {
     "moge_dilate_with_mask": [vp, vp, i64, ci, ci, ci, vp, vp, vp],
     "moge_threshold_depth_change": [vp, vp, i64, ci, ci, ci, C.c_float, ci, vp, vp],
     "moge_gaussian_blur_2d": [vp, i64, ci, ci, fp, ci, vp, vp],
+    "moge_dino_create": [C.POINTER(DinoConfig), ci, C.POINTER(vp)],
+    "moge_dino_workspace_bytes": [vp, ci, ci, ci, C.POINTER(ci), ci, ci, C.POINTER(sz)],
+    "moge_dino_forward": [vp, vp, ci, ci, ci, ci, C.POINTER(ci), ci, ci, vp, vp, vp, vp, sz, vp],
 }
 EXPORTS = list(SIGNATURES)
 

@@ -42,6 +42,14 @@ struct Group {
     // bindings (set per forward)
     const void* image = nullptr; int image_dtype = 0;
     float* points = nullptr; float* normal = nullptr; float* mask = nullptr; float* scale = nullptr;
+    float* tokens = nullptr; float* cls_out = nullptr; float* prenorm = nullptr;     // DINOv2 backbone outputs (moge_dino_forward)
+};
+
+// What a DINOv2 backbone plan exports besides its shape: the blocks whose rows it writes (increasing) and the MOGE_DINO_* flags
+struct DinoKey {
+    std::vector<int> layers;
+    int flags = 0;
+    bool operator==(const DinoKey& o) const { return layers == o.layers && flags == o.flags; }
 };
 
 // The group a public group struct describes, with its bindings
@@ -61,6 +69,7 @@ static Group make_group(const moge_v1_group_t& m) {     // MoGe-1: the token gri
 
 struct Plan {
     std::vector<Group> groups;
+    DinoKey dino;                  // a DINOv2 backbone plan's exports (empty for the MoGe engines)
     void* ws = nullptr;
     size_t ws_bytes = 0;
     OpList ops;                    // in launch order: all phase-0 ops, then phase 1, then phase 2
@@ -478,6 +487,34 @@ static int plan_v2_decoder(moge_engine* e, Plan* pl, const uint8_t* taps, const 
     return 0;
 }
 
+// DINOv2 backbone outputs (phase 2: the caller's buffers, bound per call): each exported block's rows from the snapshot taken after
+// it, or from the stream itself for the last block, through the final LayerNorm or raw; then the pre-norm stream.  One group.
+static int plan_dino_outputs(moge_engine* e, Plan* pl, const float* x, const std::vector<float*>& snaps) {
+    const int D = e->cfg.embed_dim, depth = e->cfg.depth;
+    const Group& g = pl->groups[0];
+    const int B = g.B, T = g.h * g.w, N = T + 1;
+    const bool norm = pl->dino.flags & MOGE_DINO_NORM, chw = pl->dino.flags & MOGE_DINO_CHANNEL_MAJOR;
+    const float* ng = norm ? e->norm_g : nullptr;
+    const float* nb = norm ? e->norm_b : nullptr;
+    Plan* P = pl;
+    size_t s = 0;
+    for (size_t j = 0; j < pl->dino.layers.size(); ++j) {
+        const float* src = pl->dino.layers[j] == depth - 1 ? x : snaps[s++];
+        const size_t tok_off = j * static_cast<size_t>(B) * T * D, cls_off = j * static_cast<size_t>(B) * D;
+        pl->ops.add([=](cudaStream_t st) {
+            const Group& gg = P->groups[0];
+            return launch_dino_export(src, B, N, D, ng, nb, chw, gg.tokens ? gg.tokens + tok_off : nullptr,
+                                      gg.cls_out ? gg.cls_out + cls_off : nullptr, st);
+        }, chw ? "dino_export_chw" : "dino_export", 0, static_cast<double>(B) * N * D * 8, 2);
+    }
+    const size_t bytes = static_cast<size_t>(B) * N * D * 4;
+    pl->ops.add([=](cudaStream_t st) {
+        if (P->groups[0].prenorm) CUDA_TRY(cudaMemcpyAsync(P->groups[0].prenorm, x, bytes, cudaMemcpyDeviceToDevice, st));
+        return 0;
+    }, "dino_prenorm", 0, 2.0 * bytes, 2);
+    return 0;
+}
+
 // Workspace layout + launch list of one call shape (a list of shape groups).  `dry`: only the byte count.
 static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cudaStream_t upload_stream = nullptr) {
     const moge_config_t& c = e->cfg;
@@ -509,8 +546,15 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
     // ---- decoder buffers: MoGe-1 or MoGe-2 (the encoder above is shared)
     V1Bufs vb;
     V2Bufs v2b;
-    if (e->v1) v1_alloc(e, pl, ws, &vb);
-    else alloc_v2_decoder(e, pl, ws, &v2b);
+    std::vector<float*> snaps;      // DINOv2 backbone: the residual stream after each exported block but the last
+    if (e->dino) {
+        for (int l : pl->dino.layers)
+            if (l != c.depth - 1) snaps.push_back(static_cast<float*>(ws.take(static_cast<size_t>(M) * D * 4)));
+    } else if (e->v1) {
+        v1_alloc(e, pl, ws, &vb);
+    } else {
+        alloc_v2_decoder(e, pl, ws, &v2b);
+    }
     if (bytes_out) *bytes_out = ws.off + 1024;
     if (dry) return 0;
     if (ws.off > pl->ws_bytes) return set_error("workspace too small: need %zu bytes, got %zu", ws.off, pl->ws_bytes);
@@ -527,6 +571,13 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         const int B = g.B, H = g.H, W = g.W, h = g.h, w = g.w, T = h * w, N = T + 1;
         prow0[gi] = prow;
         uint8_t* patches_g = patches + static_cast<size_t>(prow) * 592 * 2;
+        if (e->dino) {
+            // the backbone's input is already normalised and a whole number of patches: no resize, no mean / std
+            pl->ops.add([=](cudaStream_t st) { return launch_dino_patchify(P->groups[gi].image, P->groups[gi].image_dtype, B, H, W, patches_g, bf16, st); },
+                        gname("dino_patchify", gi), 0, static_cast<double>(B) * 3 * H * W * 4 + static_cast<double>(B) * T * 592 * 2, 0);
+            prow += static_cast<long>(B) * T;
+            continue;
+        }
         if (e->v1) {
             // MoGe-1 (v1.py:273-279): antialiased bicubic resize to (rh, rw), then the same normalise + aa-bilinear resize to
             // (14h, 14w) + patchify as MoGe-2 (normalising after the second resize instead of between the two commutes: both
@@ -601,6 +652,13 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         a.ln = (i + 1 < c.depth) ? &prod : nullptr;
         MG_TRY(add_linear(e, pl, a, "gemm.fc2"));
         if (i + 1 < c.depth) add_rstd(parts_x);
+        if (e->dino && i + 1 < c.depth && std::find(pl->dino.layers.begin(), pl->dino.layers.end(), i) != pl->dino.layers.end()) {
+            // the rows the export reads after the last block are overwritten by the next one: keep a copy (phase 1, workspace only)
+            float* dst = snaps[std::find(pl->dino.layers.begin(), pl->dino.layers.end(), i) - pl->dino.layers.begin()];
+            const size_t bytes = static_cast<size_t>(M) * D * 4;
+            pl->ops.add([=](cudaStream_t st) { CUDA_TRY(cudaMemcpyAsync(dst, x, bytes, cudaMemcpyDeviceToDevice, st)); return 0; },
+                        "dino_snapshot", 0, 2.0 * bytes);
+        }
         if (tap_idx < c.num_taps && c.taps[tap_idx] == i) {
             const int j = tap_idx++;
             const bool lasttap = (j == c.num_taps - 1);
@@ -619,7 +677,8 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         }
     }
     if (tap_idx != c.num_taps) return set_error("intermediate_layers must be increasing block indices < depth");
-    MG_TRY(e->v1 ? plan_v1_decoder(e, pl, taps, prow0, vb) : plan_v2_decoder(e, pl, taps, prow0, cls, mlp_scratch, v2b));
+    if (e->dino) MG_TRY(plan_dino_outputs(e, pl, x, snaps));
+    else MG_TRY(e->v1 ? plan_v1_decoder(e, pl, taps, prow0, vb) : plan_v2_decoder(e, pl, taps, prow0, cls, mlp_scratch, v2b));
     // launch order: phase 0, 1, 2 (stable)
     std::stable_sort(pl->ops.begin(), pl->ops.end(), [](const Op& a, const Op& b) { return a.phase < b.phase; });
     return 0;
@@ -631,9 +690,10 @@ constexpr size_t kMaxPlans = 16;
 // same shape but another workspace REPLACES the plan instead of orphaning it.  A plan owns its device buffers (pos tables,
 // attention work list) and frees them when it is replaced or evicted (LRU) -- after the device has drained, since launches
 // that read them may still be queued on the caller's stream.
-static int get_plan(moge_engine* e, const std::vector<Group>& groups, void* ws, size_t ws_bytes, Plan** out, cudaStream_t st) {
+static int get_plan(moge_engine* e, const std::vector<Group>& groups, const DinoKey& dino, void* ws, size_t ws_bytes, Plan** out,
+                    cudaStream_t st) {
     for (size_t i = 0; i < e->plans.size(); ++i) {
-        if (!e->plans[i]->same_shape(groups)) continue;
+        if (!e->plans[i]->same_shape(groups) || !(e->plans[i]->dino == dino)) continue;
         if (e->plans[i]->ws == ws && e->plans[i]->ws_bytes == ws_bytes) {
             std::rotate(e->plans.begin() + i, e->plans.begin() + i + 1, e->plans.end());      // most recently used last
             *out = e->plans.back().get();
@@ -650,7 +710,7 @@ static int get_plan(moge_engine* e, const std::vector<Group>& groups, void* ws, 
         e->plans.erase(e->plans.begin());
     }
     std::unique_ptr<Plan> pl(new Plan());
-    pl->ws = ws; pl->ws_bytes = ws_bytes;
+    pl->ws = ws; pl->ws_bytes = ws_bytes; pl->dino = dino;
     const int D = e->cfg.embed_dim;
     MG_TRY(pl->alloc(reinterpret_cast<void**>(&pl->cls_row), D * 4));
     for (Group g : groups) {
@@ -718,6 +778,25 @@ static int validate_v1(const moge_v1_config_t& c) {
     return 0;
 }
 
+static int validate_dino(const moge_dino_config_t& c) {
+    const int D = c.embed_dim;
+    if (c.ffn_layer != MOGE_DINO_FFN_MLP)
+        return set_error("dinov2: ffn_layer %s unsupported: the encoder kernels run the GELU MLP only (ViT-g uses SwiGLU)",
+                         c.ffn_layer == MOGE_DINO_FFN_SWIGLU ? "swiglu" : c.ffn_layer == MOGE_DINO_FFN_IDENTITY ? "identity" : "(unknown)");
+    if (D <= 0 || D % 128 || D > 1024)
+        return set_error("dinov2: embed_dim=%d unsupported (a multiple of 128, <= 1024: ViT-S/B/L; ViT-g is not covered)", D);
+    if (c.num_heads * 64 != D) return set_error("dinov2: head_dim must be 64 (embed_dim=%d, num_heads=%d)", D, c.num_heads);
+    if (c.depth <= 0 || c.depth > 64) return set_error("dinov2: depth=%d out of range (1..64)", c.depth);
+    if (c.patch_size != 14) return set_error("dinov2: patch_size=%d unsupported (14 only)", c.patch_size);
+    if (c.num_register_tokens != 0)
+        return set_error("dinov2: %d register tokens unsupported (the engine's rows are the class token and the patches only)",
+                         c.num_register_tokens);
+    if (c.interpolate_antialias) return set_error("dinov2: antialiased pos-embed interpolation unsupported");
+    if (c.interpolate_offset != 0.1f) return set_error("dinov2: interpolate_offset=%g unsupported (0.1 only)", c.interpolate_offset);
+    if (c.compute_dtype != MOGE_F16 && c.compute_dtype != MOGE_BF16) return set_error("dinov2: compute_dtype must be MOGE_F16 or MOGE_BF16");
+    return 0;
+}
+
 }  // namespace mg
 
 using namespace mg;
@@ -765,6 +844,17 @@ int moge_engine_create_v1(const moge_v1_config_t* cfg, int device, moge_engine_t
     MG_TRY(create_engine(&enc, device, out));
     (*out)->v1 = true;
     (*out)->v1cfg = *cfg;
+    return 0;
+}
+
+int moge_dino_create(const moge_dino_config_t* cfg, int device, moge_engine_t** out) {
+    if (!cfg || !out) return set_error("null argument");
+    MG_TRY(validate_dino(*cfg));
+    moge_config_t enc{};         // the encoder part only: build_plan exports the backbone's rows instead of running a decoder
+    enc.embed_dim = cfg->embed_dim; enc.depth = cfg->depth; enc.num_heads = cfg->num_heads;
+    enc.compute_dtype = cfg->compute_dtype;
+    MG_TRY(create_engine(&enc, device, out));
+    (*out)->dino = true;
     return 0;
 }
 
@@ -829,11 +919,34 @@ static int v1_to_groups(moge_engine_t* e, const moge_v1_group_t* g, int n, bool 
     return 0;
 }
 
+// A DINOv2 backbone call as one plan group and its key, checked before anything runs: the engine, the shape, the layer list and
+// flags; `forward`: the input too
+static int dino_group(moge_engine_t* e, const void* x, int x_dtype, int B, int H, int W, const int* layers, int n_layers, int flags,
+                      bool forward, Group* g, DinoKey* key) {
+    if (!e) return set_error("null argument");
+    if (!e->dino) return set_error("not a DINOv2 backbone engine (moge_dino_create)");
+    if (B <= 0 || H <= 0 || W <= 0) return set_error("dinov2: bad shape B=%d H=%d W=%d", B, H, W);
+    if (H % 14 || W % 14) return set_error("dinov2: input %d x %d is not a multiple of the patch size 14", H, W);
+    if (n_layers < 0 || n_layers > e->cfg.depth) return set_error("dinov2: %d layers out of range (0..%d)", n_layers, e->cfg.depth);
+    if (n_layers > 0 && !layers) return set_error("null argument");
+    for (int j = 0; j < n_layers; ++j)
+        if (layers[j] < 0 || layers[j] >= e->cfg.depth || (j > 0 && layers[j] <= layers[j - 1]))
+            return set_error("dinov2: layers must be increasing block indices < depth (%d)", e->cfg.depth);
+    if (flags & ~(MOGE_DINO_NORM | MOGE_DINO_CHANNEL_MAJOR)) return set_error("dinov2: unknown flags 0x%x", flags);
+    if (forward) MG_TRY(check_image(x, x_dtype));
+    g->B = B; g->H = H; g->W = W; g->h = H / 14; g->w = W / 14;
+    g->image = x; g->image_dtype = x_dtype;
+    key->layers.assign(layers, layers + n_layers);
+    key->flags = flags;
+    return 0;
+}
+
 int moge_engine_workspace_bytes_groups(moge_engine_t* e, const moge_group_t* groups, int n, size_t* bytes) {
     if (!bytes) return set_error("null argument");
     Plan pl;
     MG_TRY(to_groups(e, groups, n, false, &pl.groups));
     if (e->v1) return set_error("a MoGe-1 engine takes moge_v1_workspace_bytes");
+    if (e->dino) return set_error("a DINOv2 backbone engine takes moge_dino_workspace_bytes");
     return build_plan(e, &pl, true, bytes);
 }
 
@@ -854,16 +967,18 @@ static int check_forward(moge_engine_t* e, const void* workspace, const std::fun
 }
 
 // groups: checked, with their bindings
-static int forward_impl(moge_engine_t* e, const std::vector<Group>& groups, void* workspace, size_t workspace_bytes, void* stream) {
+static int forward_impl(moge_engine_t* e, const std::vector<Group>& groups, void* workspace, size_t workspace_bytes, void* stream,
+                        const DinoKey& dino = DinoKey()) {
     CUDA_TRY(cudaSetDevice(e->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     Plan* pl;
-    MG_TRY(get_plan(e, groups, workspace, workspace_bytes, &pl, st));
+    MG_TRY(get_plan(e, groups, dino, workspace, workspace_bytes, &pl, st));
     long tokens = 0;
     for (size_t i = 0; i < groups.size(); ++i) {
         Group& g = pl->groups[i];
         g.image = groups[i].image; g.image_dtype = groups[i].image_dtype;
         g.points = groups[i].points; g.normal = groups[i].normal; g.mask = groups[i].mask; g.scale = groups[i].scale;
+        g.tokens = groups[i].tokens; g.cls_out = groups[i].cls_out; g.prenorm = groups[i].prenorm;
         tokens += static_cast<long>(g.B) * g.h * g.w;
     }
     e->last_plan = pl;
@@ -914,6 +1029,7 @@ static int forward_impl(moge_engine_t* e, const std::vector<Group>& groups, void
 
 int moge_engine_forward_groups(moge_engine_t* e, const moge_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream) {
     if (e && e->v1) return set_error("a MoGe-1 engine runs through moge_v1_forward");
+    if (e && e->dino) return set_error("a DINOv2 backbone engine runs through moge_dino_forward");
     std::vector<Group> gs;
     MG_TRY(check_forward(e, workspace, [&] { return to_groups(e, groups, n, true, &gs); }));
     return forward_impl(e, gs, workspace, workspace_bytes, stream);
@@ -964,6 +1080,23 @@ int moge_engine_forward(moge_engine_t* e, const void* image, int image_dtype, in
     g.image = image; g.image_dtype = image_dtype; g.B = B; g.H = H; g.W = W; g.h = h; g.w = w;
     g.points = points; g.normal = normal; g.mask_prob = mask_prob; g.metric_scale = metric_scale;
     return moge_engine_forward_groups(e, &g, 1, workspace, workspace_bytes, stream);
+}
+
+int moge_dino_workspace_bytes(moge_engine_t* e, int B, int H, int W, const int* layers, int n_layers, int flags, size_t* bytes) {
+    if (!bytes) return set_error("null argument");
+    Plan pl;
+    pl.groups.resize(1);
+    MG_TRY(dino_group(e, nullptr, 0, B, H, W, layers, n_layers, flags, false, &pl.groups[0], &pl.dino));
+    return build_plan(e, &pl, true, bytes);
+}
+
+int moge_dino_forward(moge_engine_t* e, const void* x, int x_dtype, int B, int H, int W, const int* layers, int n_layers, int flags,
+                      float* out_tokens, float* out_cls, float* out_prenorm, void* workspace, size_t workspace_bytes, void* stream) {
+    std::vector<Group> gs(1);
+    DinoKey key;
+    MG_TRY(check_forward(e, workspace, [&] { return dino_group(e, x, x_dtype, B, H, W, layers, n_layers, flags, true, &gs[0], &key); }));
+    gs[0].tokens = out_tokens; gs[0].cls_out = out_cls; gs[0].prenorm = out_prenorm;
+    return forward_impl(e, gs, workspace, workspace_bytes, stream, key);
 }
 
 int moge_engine_num_ops(moge_engine_t* e, int* n) {

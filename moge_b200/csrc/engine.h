@@ -56,6 +56,7 @@ struct moge_engine {
     moge_config_t cfg;
     bool v1 = false;                  // created by moge_engine_create_v1: cfg holds the encoder only, v1cfg the rest
     moge_v1_config_t v1cfg{};
+    bool dino = false;                // created by moge_dino_create: the backbone alone, its own weight keys, no decoder
     mg::V1W v1w;
     int device = 0, num_sms = 132;
     bool bf16 = false, finalized = false;

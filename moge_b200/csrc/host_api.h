@@ -209,6 +209,14 @@ int launch_postprocess(float* points, const float* normal_in, const float* mask_
                        const float* focal, const float* shift, int B, int H, int W, int force_projection, int apply_mask,
                        float* depth, float* normal_out, uint8_t* mask_out, float* intrinsics, cudaStream_t st);
 
+// ---- DINOv2 backbone ends (dinov2.cu)
+// image (B,3,H,W) already normalised, H and W multiples of 14 -> patch-embed A rows [B*T, 592] 16-bit (columns as launch_preprocess)
+int launch_dino_patchify(const void* image, int image_dtype, int B, int H, int W, void* patches, bool bf16, cudaStream_t st);
+// x [B*N, D] fp32 (N = T + 1, class row first) -> fp32 patch rows `tokens` as (B,T,D) or, channel_major, (B,D,T); class rows `cls`
+// (B,D).  gamma/beta: the LayerNorm (eps 1e-6) applied on the way, null: the raw rows.  Either output may be null.
+int launch_dino_export(const float* x, int B, int N, int D, const float* gamma, const float* beta, bool channel_major, float* tokens,
+                       float* cls, cudaStream_t st);
+
 // ---- MoGe-1 kernels (v1.cu); maps are padded NHWC 16-bit with C channels on grid g, border written
 // antialiased bicubic (a = -0.5) resize (B,C,H,W) image -> fp32 (B,C,Ho,Wo) via the fp32 row pass tmp (B,C,H,Wo)
 int launch_resize_bicubic_aa(const void* image, int dtype, int B, int C, int H, int W, int Ho, int Wo, float* tmp, float* out, cudaStream_t st);

@@ -304,7 +304,7 @@ static int finalize_encoder(Loader& ctx) {
     moge_engine* e = ctx.e;
     const moge_config_t& c = e->cfg;
     const int D = c.embed_dim;
-    const std::string bb = e->v1 ? "backbone." : "encoder.backbone.";
+    const std::string bb = e->dino ? "" : e->v1 ? "backbone." : "encoder.backbone.";
     MG_TRY(pack_linear(ctx, bb + "patch_embed.proj.weight", {D, 3, 14, 14}, 592, &e->w_patch));
     MG_TRY(ctx.keep(bb + "patch_embed.proj.bias", {D}, &e->patch_bias));
     MG_TRY(ctx.keep(bb + "pos_embed", {1, 1 + 37 * 37, D}, &e->pos_embed));
@@ -488,7 +488,7 @@ static int finalize_v1(Loader& ctx) {
 static int finalize(moge_engine* e, cudaStream_t st) {
     Loader ctx(e, st);
     MG_TRY(finalize_encoder(ctx));
-    MG_TRY(e->v1 ? finalize_v1(ctx) : finalize_v2_decoder(ctx));
+    if (!e->dino) MG_TRY(e->v1 ? finalize_v1(ctx) : finalize_v2_decoder(ctx));
     CUDA_TRY(cudaStreamSynchronize(st));
     // release the staging copies no kernel reads at run time
     for (auto& kv : e->raw)

@@ -67,7 +67,7 @@ class EngineModel:
         missing = [k for k in want if k not in state_dict]
         unexpected = [k for k in state_dict.keys() if k not in wanted]
         if strict and (missing or unexpected):
-            raise RuntimeError("Error(s) in loading state_dict for MoGeModel:\n\tMissing key(s): "
+            raise RuntimeError(f"Error(s) in loading state_dict for {type(self).__name__}:\n\tMissing key(s): "
                                f"{missing}\n\tUnexpected key(s): {unexpected}")
         self._state = {k: v.detach() for k, v in state_dict.items()}
         self._drop_engine()

@@ -675,3 +675,18 @@ def synthetic_geometry_case(seed: int, batch_shape, H: int, W: int, mask_mode: s
     shape = (*batch_shape, H, W)
     return {"depth": torch.stack(depths).reshape(shape), "normal": torch.stack(normals).reshape(*shape, 3).contiguous(),
             "intrinsics": torch.stack(intrs).reshape(*batch_shape, 3, 3), "mask": torch.stack(masks).reshape(shape), "image": image}
+
+
+def make_dinov2_state_dict(size: str = "vits", seed: int = 0) -> "OrderedDict[str, torch.Tensor]":
+    """Seeded fp32 state dict of a DINOv2 ViT-S/B/L/14 backbone under its own keys (moge/model/dinov2): the `encoder.backbone.*`
+    tensors of the synthetic MoGe-2 state dict of the same size and seed, with the prefix dropped."""
+    from .configs import model_config
+    p = "encoder.backbone."
+    return OrderedDict((k[len(p):], v) for k, v in make_state_dict(model_config(size), seed).items() if k.startswith(p))
+
+
+def synthetic_dino_input(batch: int, height: int, width: int, seed: int = 0) -> torch.Tensor:
+    """(B, 3, H, W) fp32: a normalised image as the DINOv2 backbone takes it (ImageNet mean / std applied), seeded."""
+    mean = torch.tensor(IMAGE_MEAN).view(1, 3, 1, 1)
+    std = torch.tensor(IMAGE_STD).view(1, 3, 1, 1)
+    return (synthetic_images(batch, height, width, seed) - mean) / std
