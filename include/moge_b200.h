@@ -300,6 +300,21 @@ int moge_dino_workspace_bytes(moge_engine_t* e, int B, int H, int W, const int* 
  * same run to run. */
 int moge_dino_forward(moge_engine_t* e, const void* x, int x_dtype, int B, int H, int W, const int* layers, int n_layers, int flags,
                       float* out_tokens, float* out_cls, float* out_prenorm, void* workspace, size_t workspace_bytes, void* stream);
+/* Mixed-shape backbone batches: a call carries `n` (1..MOGE_DINO_MAX_GROUPS) shape groups, each the arguments of one
+ * moge_dino_forward call with its outputs laid out as documented there for that group's B, H, W.  `layers` and `flags` apply to
+ * every group.  The encoder runs once over the token rows of all groups packed back to back; the front end and each exported
+ * block's export are one launch each over all groups.  An image's outputs are bitwise those it gets in a call of its own.
+ * moge_dino_forward and moge_dino_workspace_bytes are the n = 1 case. */
+#define MOGE_DINO_MAX_GROUPS 64
+typedef struct moge_dino_group {
+    const void* x; int x_dtype;
+    int B, H, W;
+    float* out_tokens; float* out_cls; float* out_prenorm;     /* any may be NULL */
+} moge_dino_group_t;
+int moge_dino_workspace_bytes_groups(moge_engine_t* e, const moge_dino_group_t* groups, int n, const int* layers, int n_layers,
+                                     int flags, size_t* bytes);
+int moge_dino_forward_groups(moge_engine_t* e, const moge_dino_group_t* groups, int n, const int* layers, int n_layers, int flags,
+                             void* workspace, size_t workspace_bytes, void* stream);
 
 /* ---- truncated-L1 alignment solvers (moge/utils/alignment.py; Python: moge_b200.alignment, alias moge.utils.alignment).
  * A problem is n elements (x, y, w), w >= 0; it is solved as align() (alignment.py:52-146) solves it: after x, y *= sign(x), either

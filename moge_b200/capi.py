@@ -36,6 +36,7 @@ GEOMETRY_MAX_REFINE_KERNEL, GEOMETRY_MAX_POOL_KERNEL, GEOMETRY_MAX_BLUR_KERNEL =
 DILATE = {"mean": 0, "min": 1, "max": 2, "median": 3}
 DINO_FFN = {"mlp": 0, "swiglu": 1, "swiglufused": 1, "identity": 2}
 DINO_NORM, DINO_CHANNEL_MAJOR = 1, 2
+DINO_MAX_GROUPS = 64
 
 
 class StackConfig(C.Structure):
@@ -92,6 +93,14 @@ class DinoConfig(C.Structure):
         ("embed_dim", C.c_int), ("depth", C.c_int), ("num_heads", C.c_int), ("patch_size", C.c_int),
         ("num_register_tokens", C.c_int), ("interpolate_offset", C.c_float), ("interpolate_antialias", C.c_int),
         ("ffn_layer", C.c_int), ("compute_dtype", C.c_int),
+    ]
+
+
+class DinoGroup(C.Structure):
+    """moge_dino_group_t: one shape group of a mixed-shape backbone call."""
+    _fields_ = [
+        ("x", C.c_void_p), ("x_dtype", C.c_int), ("B", C.c_int), ("H", C.c_int), ("W", C.c_int),
+        ("out_tokens", C.c_void_p), ("out_cls", C.c_void_p), ("out_prenorm", C.c_void_p),
     ]
 
 
@@ -204,6 +213,8 @@ SIGNATURES = {
     "moge_dino_create": [C.POINTER(DinoConfig), ci, C.POINTER(vp)],
     "moge_dino_workspace_bytes": [vp, ci, ci, ci, C.POINTER(ci), ci, ci, C.POINTER(sz)],
     "moge_dino_forward": [vp, vp, ci, ci, ci, ci, C.POINTER(ci), ci, ci, vp, vp, vp, vp, sz, vp],
+    "moge_dino_workspace_bytes_groups": [vp, C.POINTER(DinoGroup), ci, C.POINTER(ci), ci, ci, C.POINTER(sz)],
+    "moge_dino_forward_groups": [vp, C.POINTER(DinoGroup), ci, C.POINTER(ci), ci, ci, vp, sz, vp],
 }
 EXPORTS = list(SIGNATURES)
 

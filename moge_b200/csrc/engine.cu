@@ -488,30 +488,39 @@ static int plan_v2_decoder(moge_engine* e, Plan* pl, const uint8_t* taps, const 
 }
 
 // DINOv2 backbone outputs (phase 2: the caller's buffers, bound per call): each exported block's rows from the snapshot taken after
-// it, or from the stream itself for the last block, through the final LayerNorm or raw; then the pre-norm stream.  One group.
+// it, or from the stream itself for the last block, through the final LayerNorm or raw, one launch over every group; then the
+// pre-norm stream, one copy per group (a group's rows are contiguous, each image's class row first).
 static int plan_dino_outputs(moge_engine* e, Plan* pl, const float* x, const std::vector<float*>& snaps) {
     const int D = e->cfg.embed_dim, depth = e->cfg.depth;
-    const Group& g = pl->groups[0];
-    const int B = g.B, T = g.h * g.w, N = T + 1;
+    const int G = static_cast<int>(pl->groups.size());
     const bool norm = pl->dino.flags & MOGE_DINO_NORM, chw = pl->dino.flags & MOGE_DINO_CHANNEL_MAJOR;
     const float* ng = norm ? e->norm_g : nullptr;
     const float* nb = norm ? e->norm_b : nullptr;
     Plan* P = pl;
+    long M = 0;
+    for (const Group& g : pl->groups) M += static_cast<long>(g.B) * (g.h * g.w + 1);
     size_t s = 0;
     for (size_t j = 0; j < pl->dino.layers.size(); ++j) {
         const float* src = pl->dino.layers[j] == depth - 1 ? x : snaps[s++];
-        const size_t tok_off = j * static_cast<size_t>(B) * T * D, cls_off = j * static_cast<size_t>(B) * D;
         pl->ops.add([=](cudaStream_t st) {
-            const Group& gg = P->groups[0];
-            return launch_dino_export(src, B, N, D, ng, nb, chw, gg.tokens ? gg.tokens + tok_off : nullptr,
-                                      gg.cls_out ? gg.cls_out + cls_off : nullptr, st);
-        }, chw ? "dino_export_chw" : "dino_export", 0, static_cast<double>(B) * N * D * 8, 2);
+            DinoExportOut outs[MOGE_DINO_MAX_GROUPS];
+            for (int gi = 0; gi < G; ++gi) {
+                const Group& g = P->groups[gi];
+                const int T = g.h * g.w;
+                outs[gi].B = g.B; outs[gi].N = T + 1;
+                outs[gi].tokens = g.tokens ? g.tokens + j * static_cast<size_t>(g.B) * T * D : nullptr;
+                outs[gi].cls = g.cls_out ? g.cls_out + j * static_cast<size_t>(g.B) * D : nullptr;
+            }
+            return launch_dino_export(src, outs, G, D, ng, nb, chw, st);
+        }, chw ? "dino_export_chw" : "dino_export", 0, static_cast<double>(M) * D * 8, 2);
     }
-    const size_t bytes = static_cast<size_t>(B) * N * D * 4;
     pl->ops.add([=](cudaStream_t st) {
-        if (P->groups[0].prenorm) CUDA_TRY(cudaMemcpyAsync(P->groups[0].prenorm, x, bytes, cudaMemcpyDeviceToDevice, st));
+        for (const Group& g : P->groups)
+            if (g.prenorm)
+                CUDA_TRY(cudaMemcpyAsync(g.prenorm, x + static_cast<size_t>(g.row0) * D, static_cast<size_t>(g.B) * (g.h * g.w + 1) * D * 4,
+                                         cudaMemcpyDeviceToDevice, st));
         return 0;
-    }, "dino_prenorm", 0, 2.0 * bytes, 2);
+    }, "dino_prenorm", 0, static_cast<double>(M) * D * 8, 2);
     return 0;
 }
 
@@ -571,10 +580,7 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         const int B = g.B, H = g.H, W = g.W, h = g.h, w = g.w, T = h * w, N = T + 1;
         prow0[gi] = prow;
         uint8_t* patches_g = patches + static_cast<size_t>(prow) * 592 * 2;
-        if (e->dino) {
-            // the backbone's input is already normalised and a whole number of patches: no resize, no mean / std
-            pl->ops.add([=](cudaStream_t st) { return launch_dino_patchify(P->groups[gi].image, P->groups[gi].image_dtype, B, H, W, patches_g, bf16, st); },
-                        gname("dino_patchify", gi), 0, static_cast<double>(B) * 3 * H * W * 4 + static_cast<double>(B) * T * 592 * 2, 0);
+        if (e->dino) {           // one front-end launch over every group, below
             prow += static_cast<long>(B) * T;
             continue;
         }
@@ -594,6 +600,20 @@ static int build_plan(moge_engine* e, Plan* pl, bool dry, size_t* bytes_out, cud
         pl->ops.add([=](cudaStream_t st) { return launch_preprocess(P->groups[gi].image, P->groups[gi].image_dtype, B, H, W, h, w, patches_g, 592, bf16, st); },
                     gname("preprocess", gi), 0, static_cast<double>(B) * 3 * H * W * 4 + static_cast<double>(B) * T * 592 * 2, 0);
         prow += static_cast<long>(B) * T;
+    }
+    if (e->dino) {
+        // the backbone's input is already normalised and a whole number of patches: no resize, no mean / std.  Each group's image
+        // is read in its own dtype and shape into its patch rows.
+        double bytes = 0;
+        for (const Group& g : pl->groups) bytes += static_cast<double>(g.B) * 3 * g.H * g.W * 4 + static_cast<double>(g.B) * g.h * g.w * 592 * 2;
+        pl->ops.add([=](cudaStream_t st) {
+            DinoPatchIn in[MOGE_DINO_MAX_GROUPS];
+            for (int gi = 0; gi < G; ++gi) {
+                const Group& g = P->groups[gi];
+                in[gi].image = g.image; in[gi].image_dtype = g.image_dtype; in[gi].B = g.B; in[gi].H = g.H; in[gi].W = g.W;
+            }
+            return launch_dino_patchify(in, G, patches, bf16, st);
+        }, "dino_patchify", 0, bytes, 0);
     }
     for (int gi = 0; gi < G; ++gi) {
         const Group& g = pl->groups[gi];
@@ -875,6 +895,7 @@ void moge_engine_destroy(moge_engine_t* e) {
 //      reports the same first error however else it is wrong.
 
 // The checks both public group structs share
+static_assert(MOGE_DINO_MAX_GROUPS == 64, "the backbone's group tables (dinov2.cu) hold as many groups as any call carries");
 static int check_group_count(int n) {
     if (n <= 0 || n > 64) return set_error("number of shape groups %d out of range (1..64)", n);
     return 0;
@@ -919,23 +940,37 @@ static int v1_to_groups(moge_engine_t* e, const moge_v1_group_t* g, int n, bool 
     return 0;
 }
 
-// A DINOv2 backbone call as one plan group and its key, checked before anything runs: the engine, the shape, the layer list and
-// flags; `forward`: the input too
-static int dino_group(moge_engine_t* e, const void* x, int x_dtype, int B, int H, int W, const int* layers, int n_layers, int flags,
-                      bool forward, Group* g, DinoKey* key) {
-    if (!e) return set_error("null argument");
+// A DINOv2 backbone call as plan groups and its key, checked before anything runs: the group count, the engine, each group's shape,
+// the layer list and flags; `forward`: each group's input too.  A group's error names its index when the call has several.
+static int dino_groups(moge_engine_t* e, const moge_dino_group_t* groups, int n, const int* layers, int n_layers, int flags, bool forward,
+                       std::vector<Group>* out, DinoKey* key) {
+    MG_TRY(check_group_count(n));
+    if (!e || !groups) return set_error("null argument");
     if (!e->dino) return set_error("not a DINOv2 backbone engine (moge_dino_create)");
-    if (B <= 0 || H <= 0 || W <= 0) return set_error("dinov2: bad shape B=%d H=%d W=%d", B, H, W);
-    if (H % 14 || W % 14) return set_error("dinov2: input %d x %d is not a multiple of the patch size 14", H, W);
+    auto at = [n](int i) { return n > 1 ? "group " + std::to_string(i) + ": " : std::string(); };
+    for (int i = 0; i < n; ++i) {
+        const moge_dino_group_t& g = groups[i];
+        if (g.B <= 0 || g.H <= 0 || g.W <= 0) return set_error("dinov2: %sbad shape B=%d H=%d W=%d", at(i).c_str(), g.B, g.H, g.W);
+        if (g.H % 14 || g.W % 14)
+            return set_error("dinov2: %sinput %d x %d is not a multiple of the patch size 14", at(i).c_str(), g.H, g.W);
+    }
     if (n_layers < 0 || n_layers > e->cfg.depth) return set_error("dinov2: %d layers out of range (0..%d)", n_layers, e->cfg.depth);
     if (n_layers > 0 && !layers) return set_error("null argument");
     for (int j = 0; j < n_layers; ++j)
         if (layers[j] < 0 || layers[j] >= e->cfg.depth || (j > 0 && layers[j] <= layers[j - 1]))
             return set_error("dinov2: layers must be increasing block indices < depth (%d)", e->cfg.depth);
     if (flags & ~(MOGE_DINO_NORM | MOGE_DINO_CHANNEL_MAJOR)) return set_error("dinov2: unknown flags 0x%x", flags);
-    if (forward) MG_TRY(check_image(x, x_dtype));
-    g->B = B; g->H = H; g->W = W; g->h = H / 14; g->w = W / 14;
-    g->image = x; g->image_dtype = x_dtype;
+    for (int i = 0; i < n; ++i) {
+        const moge_dino_group_t& m = groups[i];
+        if (forward && !m.x) return set_error("%snull argument", at(i).c_str());
+        if (forward && m.x_dtype != MOGE_F32 && m.x_dtype != MOGE_F16 && m.x_dtype != MOGE_BF16)
+            return set_error("%sunsupported image dtype %d", at(i).c_str(), m.x_dtype);
+        Group g;
+        g.B = m.B; g.H = m.H; g.W = m.W; g.h = m.H / 14; g.w = m.W / 14;
+        g.image = m.x; g.image_dtype = m.x_dtype;
+        g.tokens = m.out_tokens; g.cls_out = m.out_cls; g.prenorm = m.out_prenorm;
+        out->push_back(g);
+    }
     key->layers.assign(layers, layers + n_layers);
     key->flags = flags;
     return 0;
@@ -1082,21 +1117,34 @@ int moge_engine_forward(moge_engine_t* e, const void* image, int image_dtype, in
     return moge_engine_forward_groups(e, &g, 1, workspace, workspace_bytes, stream);
 }
 
-int moge_dino_workspace_bytes(moge_engine_t* e, int B, int H, int W, const int* layers, int n_layers, int flags, size_t* bytes) {
+int moge_dino_workspace_bytes_groups(moge_engine_t* e, const moge_dino_group_t* groups, int n, const int* layers, int n_layers,
+                                     int flags, size_t* bytes) {
     if (!bytes) return set_error("null argument");
     Plan pl;
-    pl.groups.resize(1);
-    MG_TRY(dino_group(e, nullptr, 0, B, H, W, layers, n_layers, flags, false, &pl.groups[0], &pl.dino));
+    MG_TRY(dino_groups(e, groups, n, layers, n_layers, flags, false, &pl.groups, &pl.dino));
     return build_plan(e, &pl, true, bytes);
+}
+
+int moge_dino_forward_groups(moge_engine_t* e, const moge_dino_group_t* groups, int n, const int* layers, int n_layers, int flags,
+                             void* workspace, size_t workspace_bytes, void* stream) {
+    MG_TRY(check_group_count(n));
+    std::vector<Group> gs;
+    DinoKey key;
+    MG_TRY(check_forward(e, workspace, [&] { return dino_groups(e, groups, n, layers, n_layers, flags, true, &gs, &key); }));
+    return forward_impl(e, gs, workspace, workspace_bytes, stream, key);
+}
+
+int moge_dino_workspace_bytes(moge_engine_t* e, int B, int H, int W, const int* layers, int n_layers, int flags, size_t* bytes) {
+    moge_dino_group_t g{};
+    g.B = B; g.H = H; g.W = W;
+    return moge_dino_workspace_bytes_groups(e, &g, 1, layers, n_layers, flags, bytes);
 }
 
 int moge_dino_forward(moge_engine_t* e, const void* x, int x_dtype, int B, int H, int W, const int* layers, int n_layers, int flags,
                       float* out_tokens, float* out_cls, float* out_prenorm, void* workspace, size_t workspace_bytes, void* stream) {
-    std::vector<Group> gs(1);
-    DinoKey key;
-    MG_TRY(check_forward(e, workspace, [&] { return dino_group(e, x, x_dtype, B, H, W, layers, n_layers, flags, true, &gs[0], &key); }));
-    gs[0].tokens = out_tokens; gs[0].cls_out = out_cls; gs[0].prenorm = out_prenorm;
-    return forward_impl(e, gs, workspace, workspace_bytes, stream, key);
+    moge_dino_group_t g{};
+    g.x = x; g.x_dtype = x_dtype; g.B = B; g.H = H; g.W = W; g.out_tokens = out_tokens; g.out_cls = out_cls; g.out_prenorm = out_prenorm;
+    return moge_dino_forward_groups(e, &g, 1, layers, n_layers, flags, workspace, workspace_bytes, stream);
 }
 
 int moge_engine_num_ops(moge_engine_t* e, int* n) {

@@ -209,13 +209,24 @@ int launch_postprocess(float* points, const float* normal_in, const float* mask_
                        const float* focal, const float* shift, int B, int H, int W, int force_projection, int apply_mask,
                        float* depth, float* normal_out, uint8_t* mask_out, float* intrinsics, cudaStream_t st);
 
-// ---- DINOv2 backbone ends (dinov2.cu)
-// image (B,3,H,W) already normalised, H and W multiples of 14 -> patch-embed A rows [B*T, 592] 16-bit (columns as launch_preprocess)
-int launch_dino_patchify(const void* image, int image_dtype, int B, int H, int W, void* patches, bool bf16, cudaStream_t st);
-// x [B*N, D] fp32 (N = T + 1, class row first) -> fp32 patch rows `tokens` as (B,T,D) or, channel_major, (B,D,T); class rows `cls`
-// (B,D).  gamma/beta: the LayerNorm (eps 1e-6) applied on the way, null: the raw rows.  Either output may be null.
-int launch_dino_export(const float* x, int B, int N, int D, const float* gamma, const float* beta, bool channel_major, float* tokens,
-                       float* cls, cudaStream_t st);
+// ---- DINOv2 backbone ends (dinov2.cu): one launch over the n (1..MOGE_DINO_MAX_GROUPS) shape groups of a call, whose rows are
+//      packed back to back in group order
+// group: image (B,3,H,W) already normalised, H and W multiples of 14 -> its B*T patch-embed A rows [*, 592] 16-bit in `patches`
+// (columns as launch_preprocess)
+struct DinoPatchIn {
+    const void* image; int image_dtype;
+    int B, H, W;
+};
+int launch_dino_patchify(const DinoPatchIn* groups, int n, void* patches, bool bf16, cudaStream_t st);
+// group: its B*N rows of x [*, D] fp32 (N = T + 1, class row first) -> fp32 patch rows `tokens` as (B,T,D) or, channel_major,
+// (B,D,T); class rows `cls` (B,D).  gamma/beta: the LayerNorm (eps 1e-6) applied on the way, null: the raw rows.  Either output
+// may be null.
+struct DinoExportOut {
+    int B, N;
+    float* tokens; float* cls;
+};
+int launch_dino_export(const float* x, const DinoExportOut* groups, int n, int D, const float* gamma, const float* beta,
+                       bool channel_major, cudaStream_t st);
 
 // ---- MoGe-1 kernels (v1.cu); maps are padded NHWC 16-bit with C channels on grid g, border written
 // antialiased bicubic (a = -0.5) resize (B,C,H,W) image -> fp32 (B,C,Ho,Wo) via the fp32 row pass tmp (B,C,H,Wo)

@@ -3,7 +3,10 @@ the warp-specialised attention, the bicubic pos-embed table) on their own, with 
 
 Mirrors the public surface of the reference's moge/model/dinov2 package:
   DinoVisionTransformer (models/vision_transformer.py:44-340): get_intermediate_layers, forward_features, forward, and the
-      nn.Module-like plumbing of the MoGe models (.to / .half / .bfloat16, state_dict, load_state_dict);
+      nn.Module-like plumbing of the MoGe models (.to / .half / .bfloat16, state_dict, load_state_dict); and, for lists of
+      (3, H, W) images of mixed shapes, get_intermediate_layers_many, forward_features_many and forward_many, one encoder pass
+      per engine call over the token rows of every shape (the reference's forward_features_list needs xformers and stays
+      refused);
   vit_small / vit_base / vit_large (vision_transformer.py:351-390);
   dinov2_vits14 / dinov2_vitb14 / dinov2_vitl14 (hub/backbones.py:64-82), pretrained=False only: there is no download, load a
       state dict instead.
@@ -114,57 +117,102 @@ class DinoVisionTransformer(EngineModel):
             raise AssertionError(f"only {len(found)} / {len(take)} blocks found")
         return found
 
-    def _check_input(self, x) -> Tuple[int, int, int]:
-        if isinstance(x, list):
-            raise _unsupported("a list of images (forward_features_list) is not provided: call once per shape")
-        if not isinstance(x, torch.Tensor) or x.dim() != 4 or x.shape[1] != 3:
-            raise ValueError(f"x must be a (B, 3, H, W) tensor, got {tuple(x.shape) if isinstance(x, torch.Tensor) else type(x)}")
-        if x.dtype not in (torch.float32, torch.float16, torch.bfloat16):
-            raise TypeError(f"x must be float32, float16 or bfloat16, got {x.dtype}")
-        B, _, H, W = x.shape
+    def _check_hw(self, H: int, W: int):
         # dinov2/layers/patch_embed.py:72-73 (its messages)
         if H % self.patch_size:
             raise AssertionError(f"Input image height {H} is not a multiple of patch height {self.patch_size}")
         if W % self.patch_size:
             raise AssertionError(f"Input image width {W} is not a multiple of patch width: {self.patch_size}")
+
+    def _check_input(self, x) -> Tuple[int, int, int]:
+        if isinstance(x, list):
+            raise _unsupported("a list of images (forward_features_list) is not provided: call forward_features_many or "
+                               "get_intermediate_layers_many")
+        if not isinstance(x, torch.Tensor) or x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError(f"x must be a (B, 3, H, W) tensor, got {tuple(x.shape) if isinstance(x, torch.Tensor) else type(x)}")
+        if x.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+            raise TypeError(f"x must be float32, float16 or bfloat16, got {x.dtype}")
+        B, _, H, W = x.shape
+        self._check_hw(H, W)
         if B == 0:
             raise ValueError("x has no images")
         return B, H, W
 
+    def _check_images(self, images):
+        """The `_many` calls' argument checks, before any device work: a list of (3, H, W) fp32 / fp16 / bf16 tensors, H and W
+        multiples of 14."""
+        if not isinstance(images, list):
+            raise TypeError(f"images must be a list of (3, H, W) tensors, got {type(images).__name__}")
+        for i, im in enumerate(images):
+            if not isinstance(im, torch.Tensor) or im.dim() != 3 or im.shape[0] != 3:
+                raise ValueError(f"images[{i}] must be (3, H, W), got {tuple(im.shape) if isinstance(im, torch.Tensor) else type(im)}")
+            if im.dtype not in (torch.float32, torch.float16, torch.bfloat16):
+                raise TypeError(f"images[{i}] must be float32, float16 or bfloat16, got {im.dtype}")
+            self._check_hw(im.shape[1], im.shape[2])
+
     # ------------------------------------------------------------------ forward path
-    def _run(self, x: torch.Tensor, layers: List[int], flags: int, tokens: bool, cls: bool, prenorm: bool):
-        """One backbone pass over x (B,3,H,W): (tokens (L,B,T,D) or (L,B,D,h,w), cls (L,B,D), prenorm (B,T+1,D)), each None unless
-        asked for, L = len(layers).  Large batches run as chunks (`_chunks`); a chunk's outputs are copied into the batch's."""
-        B, H, W = x.shape[0], x.shape[2], x.shape[3]
-        h, w = H // self.patch_size, W // self.patch_size
-        T, D, L = h * w, self.embed_dim, len(layers)
-        x = self._engine_input(x)
+    def _alloc(self, b: int, h: int, w: int, L: int, flags: int, tokens: bool, cls: bool, prenorm: bool):
+        """The fp32 outputs of b images on an h x w token grid, each None unless asked for: tokens (L,b,T,D) or (L,b,D,h,w), cls
+        (L,b,D), prenorm (b,T+1,D)."""
+        T, D = h * w, self.embed_dim
+        f = dict(dtype=torch.float32, device=self._device)
+        tshape = (L, b, D, h, w) if flags & capi.DINO_CHANNEL_MAJOR else (L, b, T, D)
+        return (torch.empty(tshape, **f) if tokens and L else None, torch.empty((L, b, D), **f) if cls and L else None,
+                torch.empty((b, T + 1, D), **f) if prenorm else None)
+
+    def _dino_call(self, groups, layers: List[int], flags: int):
+        """ONE engine call over shape groups [(engine input (b,3,H,W), outputs of `_alloc`)]: the encoder runs once over the token
+        rows of every group, and each group's outputs are written to its buffers."""
         self._ensure_engine()
-        tshape = (lambda b: (L, b, D, h, w)) if flags & capi.DINO_CHANNEL_MAJOR else (lambda b: (L, b, T, D))
-
-        def alloc(b):
-            f = dict(dtype=torch.float32, device=self._device)
-            return (torch.empty(tshape(b), **f) if tokens and L else None, torch.empty((L, b, D), **f) if cls and L else None,
-                    torch.empty((b, T + 1, D), **f) if prenorm else None)
-
-        out = alloc(B)
-        chunks = self._chunks(B, T + 1)
+        arr = (capi.DinoGroup * len(groups))()
+        for g, (x, outs) in zip(arr, groups):
+            g.x, g.x_dtype = x.data_ptr(), capi.torch_dtype_code(x.dtype)
+            g.B, g.H, g.W = x.shape[0], x.shape[2], x.shape[3]
+            g.out_tokens, g.out_cls, g.out_prenorm = (None if t is None else t.data_ptr() for t in outs)
+        L = len(layers)
         lay = (C.c_int * max(L, 1))(*layers)
         lib = capi.lib()
         with torch.cuda.device(self._device):
-            for lo, n in chunks:
-                part = out if len(chunks) == 1 else alloc(n)
-                nbytes = C.c_size_t()
-                capi.check(lib.moge_dino_workspace_bytes(self._engine, n, H, W, lay, L, flags, C.byref(nbytes)))
-                ws, ws_bytes = self._workspace_for(nbytes.value)
-                capi.check(lib.moge_dino_forward(self._engine, x[lo:lo + n].data_ptr(), capi.torch_dtype_code(x.dtype), n, H, W,
-                                                 lay, L, flags, *(None if t is None else t.data_ptr() for t in part), ws, ws_bytes,
-                                                 capi.current_stream()))
-                if part is not out:
-                    for full, p, dim in zip(out, part, (1, 1, 0)):
-                        if full is not None:
-                            full.narrow(dim, lo, n).copy_(p)
+            nbytes = C.c_size_t()
+            capi.check(lib.moge_dino_workspace_bytes_groups(self._engine, arr, len(groups), lay, L, flags, C.byref(nbytes)))
+            ws, ws_bytes = self._workspace_for(nbytes.value)
+            capi.check(lib.moge_dino_forward_groups(self._engine, arr, len(groups), lay, L, flags, ws, ws_bytes,
+                                                    capi.current_stream()))
+
+    def _run(self, x: torch.Tensor, layers: List[int], flags: int, tokens: bool, cls: bool, prenorm: bool):
+        """One backbone pass over x (B,3,H,W): the batch's outputs (`_alloc`), L = len(layers).  Large batches run as chunks
+        (`_chunks`), one engine call each; a chunk's outputs are copied into the batch's."""
+        B, H, W = x.shape[0], x.shape[2], x.shape[3]
+        h, w = H // self.patch_size, W // self.patch_size
+        want = (len(layers), flags, tokens, cls, prenorm)
+        x = self._engine_input(x)
+        out = self._alloc(B, h, w, *want)
+        chunks = self._chunks(B, h * w + 1)
+        for lo, n in chunks:
+            part = out if len(chunks) == 1 else self._alloc(n, h, w, *want)
+            self._dino_call([(x[lo:lo + n], part)], layers, flags)
+            if part is not out:
+                for full, p, dim in zip(out, part, (1, 1, 0)):
+                    if full is not None:
+                        full.narrow(dim, lo, n).copy_(p)
         return out
+
+    def _run_many(self, images: List[torch.Tensor], layers: List[int], flags: int, tokens: bool, cls: bool, prenorm: bool):
+        """One backbone pass over checked (3, H, W) images of any shapes: per image, in input order, its outputs (`_alloc`) with the
+        batch dimension dropped, as views of its group's buffers.  The images are bucketed by shape and dtype and packed into engine
+        calls of at most `max_chunk_tokens` tokens and MOGE_DINO_MAX_GROUPS shape groups (`_pack_calls`)."""
+        p = self.patch_size
+        calls = self._pack_calls(images, lambda H, W: ((H // p, W // p), (H // p) * (W // p) + 1), max_units=capi.DINO_MAX_GROUPS)
+        want = (len(layers), flags, tokens, cls, prenorm)
+        results: List[Optional[tuple]] = [None] * len(images)
+        for call in calls:
+            groups = [(self._engine_input(torch.stack([images[i].to(self._device) for i in idx])), self._alloc(len(idx), h, w, *want))
+                      for (_, _, (h, w), idx) in call]
+            self._dino_call(groups, layers, flags)
+            for (_, _, _, idx), (_, (t, c, pre)) in zip(call, groups):
+                for j, i in enumerate(idx):
+                    results[i] = (None if t is None else t[:, j], None if c is None else c[:, j], None if pre is None else pre[j])
+        return results
 
     def get_intermediate_layers(self, x: torch.Tensor, n: Union[int, Sequence] = 1, reshape: bool = False,
                                 return_class_token: bool = False, norm=True) -> Tuple[Union[torch.Tensor, Tuple[torch.Tensor]]]:
@@ -206,6 +254,40 @@ class DinoVisionTransformer(EngineModel):
         return self._run(x, [self.n_blocks - 1], capi.DINO_NORM, False, True, False)[1][0]
 
     __call__ = forward
+
+    # ------------------------------------------------------------------ mixed-shape lists
+    def get_intermediate_layers_many(self, images: List[torch.Tensor], n: Union[int, Sequence] = 1, reshape: bool = False,
+                                     return_class_token: bool = False, norm=True) -> List[tuple]:
+        """`get_intermediate_layers` over a list of (3, H, W) images of any shapes (H and W multiples of 14) and dtypes: entry i is
+        bitwise `get_intermediate_layers(images[i][None], ...)` with the batch dimension dropped.  Each engine call runs the
+        encoder once over the token rows of every shape it carries (`_run_many`)."""
+        self._check_images(images)
+        layers = self._layers(n)
+        if not layers:
+            return [() for _ in images]
+        flags = (capi.DINO_NORM if norm else 0) | (capi.DINO_CHANNEL_MAJOR if reshape else 0)
+        out = []
+        for tokens, cls, _ in self._run_many(images, layers, flags, True, return_class_token, False):
+            outputs = list(tokens.unbind(0))
+            out.append(tuple(zip(outputs, cls.unbind(0))) if return_class_token else tuple(outputs))
+        return out
+
+    def forward_features_many(self, images: List[torch.Tensor]) -> List[Dict[str, Optional[torch.Tensor]]]:
+        """`forward_features` over a list of (3, H, W) images of any shapes: one dict per image, in input order, with the batch
+        dimension dropped and `masks` None."""
+        self._check_images(images)
+        return [{
+            "x_norm_clstoken": cls[0],
+            "x_norm_regtokens": tokens.new_empty((0, self.embed_dim)),
+            "x_norm_patchtokens": tokens[0],
+            "x_prenorm": prenorm,
+            "masks": None,
+        } for tokens, cls, prenorm in self._run_many(images, [self.n_blocks - 1], capi.DINO_NORM, True, True, True)]
+
+    def forward_many(self, images: List[torch.Tensor]) -> List[torch.Tensor]:
+        """`forward` over a list of (3, H, W) images of any shapes: the normed class token (D,) of each image, in input order."""
+        self._check_images(images)
+        return [cls[0] for _, cls, _ in self._run_many(images, [self.n_blocks - 1], capi.DINO_NORM, False, True, False)]
 
 
 # ---------------------------------------------------------------------------------------------- constructors

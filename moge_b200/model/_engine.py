@@ -197,12 +197,14 @@ class EngineModel:
         chunk = max(1, min(B, self.max_chunk_tokens // tokens_per_image))
         return [(lo, min(chunk, B - lo)) for lo in range(0, B, chunk)]
 
-    def _pack_calls(self, images, geometry: Callable[[int, int], Tuple[Tuple[int, int], int]]) -> List[List[tuple]]:
+    def _pack_calls(self, images, geometry: Callable[[int, int], Tuple[Tuple[int, int], int]],
+                    max_units: Optional[int] = None) -> List[List[tuple]]:
         """The engine calls of `infer_many` over `images` (each (3, H, W)), as lists of units (H, W, geom, indices).  Images are
         bucketed by shape and dtype; `geometry(H, W)` gives a bucket's (geom, token rows per image), geom being what the model's
         engine call takes per group.  Each bucket is chunked like a batch (`_chunks`), and the chunks are packed largest first into
-        calls of at most `max_chunk_tokens` tokens (a unit larger than that is a call of its own).  Raises ValueError, before
-        anything touches a device, on an element that is not (3, H, W)."""
+        calls of at most `max_chunk_tokens` tokens (a unit larger than that is a call of its own) and, given `max_units`, at most
+        that many units (shape groups).  Raises ValueError, before anything touches a device, on an element that is not
+        (3, H, W)."""
         buckets: Dict[tuple, List[int]] = {}
         for i, im in enumerate(images):
             if im.dim() != 3 or im.shape[0] != 3:
@@ -216,7 +218,7 @@ class EngineModel:
         units.sort(key=lambda u: -u[0])
         calls, cur, cur_tok = [], [], 0
         for tok, unit in units:
-            if cur and cur_tok + tok > self.max_chunk_tokens:
+            if cur and (cur_tok + tok > self.max_chunk_tokens or len(cur) == max_units):
                 calls.append(cur)
                 cur, cur_tok = [], 0
             cur.append(unit)
