@@ -429,8 +429,10 @@ int moge_mesh_build(const uint8_t* mask, int64_t batch, int H, int W, int tri, c
  * maps are equirectangular, h x w, at least 2 x 2 and at most 2^28 pixels.                                                  */
 #define MOGE_PANORAMA_MAX_VIEWS 20
 typedef struct { float R[9]; float t[3]; double fx, fy, cx, cy; } moge_panorama_camera_t;
-/* Every call takes a batch of 1 to MOGE_PANORAMA_MAX_BATCH panoramas of one size and one set of cameras; each panorama's result
- * is bitwise what it gets in a batch of one.  Arrays have a leading batch dimension.                                          */
+/* Every call takes 1 to MOGE_PANORAMA_MAX_BATCH panoramas with one set of cameras; each panorama's result is bitwise what it
+ * gets in a call of its own.  The `_groups` entry points (after these) take an array of per-panorama sizes and pointers, so the
+ * panoramas of a call may differ in size; the entry points here take `batch` panoramas of one size with arrays that have a
+ * leading batch dimension, and are implemented as the `_groups` call over those panoramas back to back.                     */
 #define MOGE_PANORAMA_MAX_BATCH 64
 /* split_panorama_image: views_f32 (batch * views, 3, res, res) = value / 255 of cv2.remap(image, INTER_LINEAR, BORDER_CONSTANT 0)
  * at the panorama pixel of each view pixel's ray; grid (res) is the fp32 pixel-centre coordinate of uv_map; views_u8
@@ -459,6 +461,54 @@ int moge_panorama_resize(const float* src, int batch, int h, int w, int H, int W
  * 0/1 mask > 0, points (batch, H, W, 3) = depth_out * spherical_uv_to_directions(uv_map(H, W)).                             */
 int moge_panorama_finish(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
                          uint8_t* mask_out, float* points, void* stream);
+/* Mixed-size calls: `n` (1..MOGE_PANORAMA_MAX_BATCH) entries, one per panorama, each with its own sizes and pointers; each kernel
+ * is one launch over all of them.  With several entries, an entry's error names its index.  The entry count is checked first,
+ * and every argument before the device is touched.
+ * split: panorama k's image (H, W, 3) uint8 RGB; its views go to views_f32 / views_u8 from view view0 on.                    */
+typedef struct moge_panorama_split {
+    const uint8_t* image;
+    int H, W;
+    int view0;
+} moge_panorama_split_t;
+int moge_panorama_split_groups(const moge_panorama_split_t* panos, int n, const moge_panorama_camera_t* cams, int views,
+                               const float* grid, int res, float* views_f32, uint8_t* views_u8, void* stream);
+/* One merge level of one panorama, h x w, as moge_panorama_rhs writes it (directions, b, row_mask, pano_mask; its views are views
+ * view0 .. view0 + views - 1 of src and mask) and moge_panorama_lsmr solves it (b, row_mask, init or NULL, depth, stats (2)).
+ * Each call reads the fields it names.  The systems of one lsmr call share one cooperative launch; a system's reductions depend
+ * on its own size only, so it gets bitwise its single-call result.  The workspace of a call fits any call whose entries are
+ * each no larger (so the finest levels' workspace serves every coarser level).                                               */
+typedef struct moge_panorama_level {
+    int h, w;
+    int view0;
+    const float* directions;
+    double* b;
+    uint8_t* row_mask;
+    uint8_t* pano_mask;
+    const float* init;
+    float* depth;
+    int32_t* stats;
+} moge_panorama_level_t;
+int moge_panorama_workspace_bytes_groups(const moge_panorama_level_t* levels, int n, int views, size_t* bytes);
+int moge_panorama_rhs_groups(const float* src, int channels, const uint8_t* mask, int views, int vh, int vw,
+                             const moge_panorama_camera_t* cams, const moge_panorama_level_t* levels, int n, void* workspace,
+                             size_t workspace_bytes, void* stream);
+int moge_panorama_lsmr_groups(const moge_panorama_level_t* levels, int n, void* workspace, size_t workspace_bytes, void* stream);
+/* resize: src (h, w) -> dst (H, W).  finish: depth (h, w) and mask (h, w) -> depth_out, mask_out and points at (H, W).        */
+typedef struct moge_panorama_resize {
+    const float* src;
+    int h, w, H, W;
+    float* dst;
+} moge_panorama_resize_t;
+int moge_panorama_resize_groups(const moge_panorama_resize_t* maps, int n, void* stream);
+typedef struct moge_panorama_finish {
+    const float* depth;
+    const uint8_t* mask;
+    int h, w, H, W;
+    float* depth_out;
+    uint8_t* mask_out;
+    float* points;
+} moge_panorama_finish_t;
+int moge_panorama_finish_groups(const moge_panorama_finish_t* maps, int n, void* stream);
 
 /* ---- training losses of moge/train/losses.py (Python: moge_b200.losses, moge_b200.local_loss; alias moge.train.losses).
  * Maps are (batch, H, W) fp32 and point maps (batch, H, W, 3) fp32, contiguous on the device.  Each call either reduces

@@ -121,6 +121,29 @@ class PanoramaCamera(C.Structure):
                 ("cy", C.c_double)]
 
 
+class PanoramaSplit(C.Structure):
+    """moge_panorama_split_t: one panorama of a mixed-size split."""
+    _fields_ = [("image", C.c_void_p), ("H", C.c_int), ("W", C.c_int), ("view0", C.c_int)]
+
+
+class PanoramaLevel(C.Structure):
+    """moge_panorama_level_t: one panorama's merge level in a mixed-size rhs / lsmr call."""
+    _fields_ = [("h", C.c_int), ("w", C.c_int), ("view0", C.c_int), ("directions", C.c_void_p), ("b", C.c_void_p),
+                ("row_mask", C.c_void_p), ("pano_mask", C.c_void_p), ("init", C.c_void_p), ("depth", C.c_void_p),
+                ("stats", C.c_void_p)]
+
+
+class PanoramaResize(C.Structure):
+    """moge_panorama_resize_t: one map of a mixed-size resize."""
+    _fields_ = [("src", C.c_void_p), ("h", C.c_int), ("w", C.c_int), ("H", C.c_int), ("W", C.c_int), ("dst", C.c_void_p)]
+
+
+class PanoramaFinish(C.Structure):
+    """moge_panorama_finish_t: one panorama of a mixed-size finish."""
+    _fields_ = [("depth", C.c_void_p), ("mask", C.c_void_p), ("h", C.c_int), ("w", C.c_int), ("H", C.c_int), ("W", C.c_int),
+                ("depth_out", C.c_void_p), ("mask_out", C.c_void_p), ("points", C.c_void_p)]
+
+
 vp, ci, i64, sz = C.c_void_p, C.c_int, C.c_int64, C.c_size_t
 fp, pc = C.POINTER(C.c_float), C.POINTER(PanoramaCamera)
 
@@ -193,6 +216,12 @@ SIGNATURES = {
     "moge_panorama_lsmr": [vp, vp, ci, ci, ci, vp, vp, vp, vp, sz, vp],
     "moge_panorama_resize": [vp, ci, ci, ci, ci, ci, vp, vp],
     "moge_panorama_finish": [vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp],
+    "moge_panorama_split_groups": [C.POINTER(PanoramaSplit), ci, pc, ci, vp, ci, vp, vp, vp],
+    "moge_panorama_workspace_bytes_groups": [C.POINTER(PanoramaLevel), ci, ci, C.POINTER(sz)],
+    "moge_panorama_rhs_groups": [vp, ci, vp, ci, ci, ci, pc, C.POINTER(PanoramaLevel), ci, vp, sz, vp],
+    "moge_panorama_lsmr_groups": [C.POINTER(PanoramaLevel), ci, vp, sz, vp],
+    "moge_panorama_resize_groups": [C.POINTER(PanoramaResize), ci, vp],
+    "moge_panorama_finish_groups": [C.POINTER(PanoramaFinish), ci, vp],
     "moge_loss_workspace_bytes": [i64, ci, ci, C.POINTER(sz)],
     "moge_loss_mask": [ci, vp, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp],
     "moge_loss_stencil": [ci, vp, vp, i64, ci, ci, vp, vp, vp, vp, sz, vp],

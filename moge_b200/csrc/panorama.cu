@@ -18,14 +18,18 @@
 // reductions.  The iteration count and istop are written to the device.  One launch solves the
 // systems of a batch of panoramas, each bitwise as alone (see lsmr_kernel); a single merge is a batch of one.
 //
-// Every stage takes a batch of panoramas of one size with one set of cameras.  The per-pixel kernels take the panorama from
-// blockIdx.y and stride over its pixels in x, so each thread does the same work at any batch size.
+// Every stage takes up to MOGE_PANORAMA_MAX_BATCH panoramas, each of its own size, with one set of cameras.  They reach the
+// kernels as a table passed by value (__grid_constant__, read in place from the parameter bank), so a launch uploads nothing.
+// The per-pixel kernels take the panorama from blockIdx.y and stride over its pixels in x, so each thread does the same work
+// at any batch size and mix of sizes; the LSMR finds a virtual block's system by a binary search on the systems' first
+// virtual blocks.  A batch of one size is the case where every entry has the same size.
 #include "host_api.h"
 #include "../../include/moge_b200.h"
 #include <cooperative_groups.h>
 #include <algorithm>
 #include <math.h>
 #include <stdint.h>
+#include <stdio.h>
 #include <string.h>
 
 namespace cg = cooperative_groups;
@@ -49,14 +53,20 @@ __device__ __forceinline__ float fadd(float a, float b) { return __fadd_rn(a, b)
 __device__ __forceinline__ int q32(float x) { return __float2int_rn(fmul(x, 32.f)); }
 
 // ---------------------------------------------------------------------------------------------------- split
-// panorama blockIdx.y of the batch: img (batch, H, W, 3), out (batch * views, 3, res, res), out_u8 (batch * views, res, res, 3) or null
-__global__ void __launch_bounds__(kThreads) split_kernel(const uint8_t* __restrict__ img, int H, int W, const Cams cams,
+struct SplitPano { const uint8_t* img; int H, W, view0; };
+struct SplitTable { SplitPano p[MOGE_PANORAMA_MAX_BATCH]; };
+
+// panorama blockIdx.y of the table: img (H, W, 3); its views are out (views, 3, res, res) and out_u8 (views, res, res, 3) (or
+// null) from view view0 on
+__global__ void __launch_bounds__(kThreads) split_kernel(const __grid_constant__ SplitTable tab, const Cams cams,
                                                          const float* __restrict__ grid, int res, float* __restrict__ out,
                                                          uint8_t* __restrict__ out_u8) {
-    const int64_t total = static_cast<int64_t>(cams.n) * res * res, pano = blockIdx.y;
-    img += pano * H * W * 3;
-    out += pano * total * 3;
-    if (out_u8) out_u8 += pano * total * 3;
+    const SplitPano& pano = tab.p[blockIdx.y];
+    const uint8_t* __restrict__ img = pano.img;
+    const int H = pano.H, W = pano.W;
+    const int64_t total = static_cast<int64_t>(cams.n) * res * res, first = static_cast<int64_t>(pano.view0) * res * res;
+    out += first * 3;
+    if (out_u8) out_u8 += first * 3;
     for (int64_t idx = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; idx < total; idx += static_cast<int64_t>(gridDim.x) * blockDim.x) {
         const int k = static_cast<int>(idx / (static_cast<int64_t>(res) * res));
         const int pix = static_cast<int>(idx % (static_cast<int64_t>(res) * res)), i = pix / res, j = pix % res;
@@ -101,13 +111,22 @@ __device__ __forceinline__ float log_distance(const float* __restrict__ src, int
     return logf(sqrtf(fadd(fadd(fmul(p[0], p[0]), fmul(p[1], p[1])), fmul(p[2], p[2]))));
 }
 
-// panorama blockIdx.y of the batch, per pixel and view: the sampled log-distance (0 outside the view) and mask.  src
-// (batch * views, vh, vw, channels), vmask (batch * views, vh, vw), L and M (batch * views, h, w)
+// One merge level of each panorama of a call: its size, its first view in the call's views, its ray table, its sampled maps
+// in the workspace and its outputs.
+struct LevelSys { const float* dirs; float* L; uint8_t* M; double* b; uint8_t* rm; uint8_t* pmask; int h, w, view0; };
+struct LevelTable { LevelSys s[MOGE_PANORAMA_MAX_BATCH]; };
+
+// panorama blockIdx.y of the table, per pixel and view: the sampled log-distance (0 outside the view) and mask.  src
+// (call views, vh, vw, channels), vmask (call views, vh, vw); the panorama's L and M (views, h, w)
 __global__ void __launch_bounds__(kThreads) sample_kernel(const float* __restrict__ src, int channels, const uint8_t* __restrict__ vmask,
-                                                          int vh, int vw, const Cams cams, const float* __restrict__ dirs, int h, int w,
-                                                          float* __restrict__ L, uint8_t* __restrict__ M) {
+                                                          int vh, int vw, const Cams cams, const __grid_constant__ LevelTable tab) {
+    const LevelSys& sys = tab.s[blockIdx.y];
+    const int h = sys.h, w = sys.w;
+    const float* __restrict__ dirs = sys.dirs;
+    float* __restrict__ L = sys.L;
+    uint8_t* __restrict__ M = sys.M;
     const int64_t n = static_cast<int64_t>(h) * w;
-    const int k0 = blockIdx.y * cams.n;            // the panorama's first view in the batch
+    const int k0 = sys.view0;                      // the panorama's first view in the call
     for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
         const float d0 = dirs[p * 3], d1 = dirs[p * 3 + 1], d2 = dirs[p * 3 + 2];
         for (int k = 0; k < cams.n; ++k) {
@@ -137,21 +156,24 @@ __global__ void __launch_bounds__(kThreads) sample_kernel(const float* __restric
                 const int nx = min(max(__float2int_rn(px), 0), vw - 1), ny = min(max(__float2int_rn(py), 0), vh - 1);
                 m = vmask[base + static_cast<int64_t>(ny) * vw + nx] != 0;
             }
-            L[(k0 + k) * n + p] = val;
-            M[(k0 + k) * n + p] = m;
+            L[k * n + p] = val;
+            M[k * n + p] = m;
         }
     }
 }
 
-// panorama blockIdx.y of the batch, per pixel: its rows of b and row_mask (see the header) and pano_mask.  L and M
-// (batch * views, h, w), b and rm (batch, rows), pmask (batch, h, w)
-__global__ void __launch_bounds__(kThreads) rhs_kernel(const float* __restrict__ L, const uint8_t* __restrict__ M, int views, int h, int w,
-                                                       double* __restrict__ b, uint8_t* __restrict__ rm, uint8_t* __restrict__ pmask) {
-    const int64_t n = static_cast<int64_t>(h) * w, rows = 2 * n + static_cast<int64_t>(h - 1) * (w + 1), pano = blockIdx.y;
-    const int k0 = blockIdx.y * views;             // the panorama's first view in the batch
-    b += pano * rows;
-    rm += pano * rows;
-    pmask += pano * n;
+// panorama blockIdx.y of the table, per pixel: its rows of b and row_mask (see the header) and pano_mask.  The panorama's L
+// and M (views, h, w), b and rm (rows), pmask (h, w).  Four blocks per SM, as before the table: its fields would otherwise
+// take the kernel past 64 registers.
+__global__ void __launch_bounds__(kThreads, 4) rhs_kernel(const __grid_constant__ LevelTable tab, int views) {
+    const LevelSys& sys = tab.s[blockIdx.y];
+    const int h = sys.h, w = sys.w;
+    const float* __restrict__ L = sys.L;
+    const uint8_t* __restrict__ M = sys.M;
+    double* __restrict__ b = sys.b;
+    uint8_t* __restrict__ rm = sys.rm;
+    uint8_t* __restrict__ pmask = sys.pmask;
+    const int64_t n = static_cast<int64_t>(h) * w;
     for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
         const int i = static_cast<int>(p / w), j = static_cast<int>(p % w);
         const int64_t pr = i * static_cast<int64_t>(w) + (j + 1) % w, pl = i * static_cast<int64_t>(w) + (j + w - 1) % w;
@@ -159,8 +181,8 @@ __global__ void __launch_bounds__(kThreads) rhs_kernel(const float* __restrict__
         float sx = 0.f, sy = 0.f, sl = 0.f;
         int cx = 0, cy = 0, cl = 0, any = 0;
         for (int k = 0; k < views; ++k) {
-            const float* Lk = L + (k0 + k) * n;
-            const uint8_t* Mk = M + (k0 + k) * n;
+            const float* Lk = L + k * n;
+            const uint8_t* Mk = M + k * n;
             const float c = Lk[p];
             const int mc = Mk[p], mr = Mk[pr];
             any |= mc;
@@ -251,21 +273,42 @@ __device__ __forceinline__ int pixel_rows(int64_t p, int i, int j, int h, int w,
     return c;
 }
 
-// P independent systems of one level size in one cooperative launch, sharing each iteration's four grid barriers (the single
-// merge is P = 1).  A system's reductions do not depend on P: its pixels are split over `vblocks` virtual blocks of 512 threads,
-// one per SM (at most ceil(n / 512)): virtual block k, thread t takes pixels k * 512 + t, stepping by vblocks * 512, reduces them
-// with a warp-shuffle and block tree to the block's partial, and the partials are summed in virtual-block order.  The P * vblocks
-// virtual blocks are dealt to the real blocks in contiguous runs of per_block, so a real block serves at most kMaxLocal systems
-// (the host checks it) and evaluates each one's scalar recurrences once, in shared memory.  A system that stops keeps its x and
+// P independent systems, each of its own level size, in one cooperative launch, sharing each iteration's four grid barriers
+// (the single merge is P = 1).  A system's reductions depend on its own size only, not on P nor on the other systems: its
+// pixels are split over `vblocks` virtual blocks of 512 threads, one per SM (at most ceil(n / 512)): virtual block k, thread t
+// takes pixels k * 512 + t, stepping by vblocks * 512, reduces them with a warp-shuffle and block tree to the block's partial,
+// and the partials are summed in virtual-block order.  The systems' virtual blocks are numbered back to back (system s from
+// item0) and dealt to the real blocks in contiguous runs of per_block, so a real block serves at most kMaxLocal systems (the
+// host checks it) and evaluates each one's scalar recurrences once, in shared memory.  A system that stops keeps its x and
 // stats and does no more work; the launch ends when every system has stopped.
 constexpr int kMaxLocal = 4;
 
-struct Lsmr {
-    const double* b; const uint8_t* rm; const float* init;     // b, rm (batch, rows); init (batch, n) = log(init) or null
-    double *u, *v, *hv, *hb, *x, *part;        // u (batch, rows); v, hv, hb, x (batch, n); part: 2 buffers x batch * vblocks x 2
-    float* depth; int32_t* stats; int* stop;   // depth (batch, n), stats (batch, 2); stop (batch): the system has stopped
-    int h, w, batch, vblocks, per_block;
+struct LsmrSys {
+    const double* b; const uint8_t* rm; const float* init;     // b, rm (rows); init (n) = log(init) or null
+    float* depth; int32_t* stats;                               // depth (n), stats (2)
+    double *u, *v, *hv, *hb, *x, *part;                         // u (rows); v, hv, hb, x (n); part: 2 buffers x vblocks x 2
+    int h, w, vblocks, item0;                                   // item0: the system's first virtual block
 };
+struct LsmrTable {
+    LsmrSys s[MOGE_PANORAMA_MAX_BATCH];
+    int* stop;                                 // (n): the system has stopped
+    int n, items, per_block;
+};
+
+// a system's LSMR arrays in its workspace piece, in this order, each padded to 32 doubles: u (rows), v, hv, hb, x (n each),
+// then the partials (2 buffers x vblocks x 2)
+__host__ __device__ __forceinline__ int64_t pad32(int64_t k) { return (k + 31) & ~int64_t(31); }
+__host__ __device__ __forceinline__ int64_t lsmr_rows(int h, int w) { return 2 * static_cast<int64_t>(h) * w + static_cast<int64_t>(h - 1) * (w + 1); }
+
+// the system that virtual block `item` belongs to: the last one whose item0 is <= item
+__device__ __forceinline__ int find_system(const LsmrTable& a, int item) {
+    int lo = 0, hi = a.n - 1;
+    while (lo < hi) {
+        const int mid = (lo + hi + 1) >> 1;
+        if (a.s[mid].item0 <= item) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
 
 // one system's scalars: SciPy's lsmr locals, and the tests that do not depend on normx
 struct LsmrScalars {
@@ -300,37 +343,38 @@ __device__ double2 partial_sum(const double* P, int count) {
     return make_double2(s, t);
 }
 
-__global__ void __launch_bounds__(kLsmrThreads) lsmr_kernel(Lsmr a) {
+__global__ void __launch_bounds__(kLsmrThreads) lsmr_kernel(const __grid_constant__ LsmrTable a) {
     cg::grid_group g = cg::this_grid();
     __shared__ LsmrScalars S[kMaxLocal];
-    const int h = a.h, w = a.w, VB = a.vblocks;
-    const int64_t n = static_cast<int64_t>(h) * w, rows = 2 * n + static_cast<int64_t>(h - 1) * (w + 1);
-    const int64_t stride = static_cast<int64_t>(VB) * kLsmrThreads, items = static_cast<int64_t>(a.batch) * VB;
-    const int i0 = blockIdx.x * a.per_block, i1 = static_cast<int>(min(static_cast<int64_t>(i0 + a.per_block), items));
-    const int s0 = i0 / VB, nloc = (i1 - 1) / VB - s0 + 1;
+    const int i0 = blockIdx.x * a.per_block, i1 = min(i0 + a.per_block, a.items);
+    const int s0 = find_system(a, i0), nloc = find_system(a, i1 - 1) - s0 + 1;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const bool lead = lane == 0 && warp < nloc;                   // evaluates the scalars of local system `warp`
-    const bool owner = warp < nloc && (s0 + warp) * VB >= i0;     // this block holds that system's virtual block 0
-    const bool x32 = a.init != nullptr;
+    const bool owner = warp < nloc && a.s[s0 + warp].item0 >= i0; // this block holds that system's virtual block 0
     const double atol = 1e-5, btol = 1e-5, ctol = 1e-8;
     int buf = 0;
     double2 r = make_double2(0, 0);
 #define FOR_ITEMS for (int it = i0; it < i1; ++it)
 #define ITEM                                                                                                                 \
-    const int sy = it / VB, vb = it - sy * VB;                                                                               \
+    const int sy = find_system(a, it);                                                                                       \
+    const LsmrSys& ls = a.s[sy];                                                                                             \
+    const int h = ls.h, w = ls.w, vb = it - ls.item0;                                                                        \
+    const int64_t n = static_cast<int64_t>(h) * w, stride = static_cast<int64_t>(ls.vblocks) * kLsmrThreads;                 \
+    [[maybe_unused]] const bool x32 = ls.init != nullptr;                                                                    \
     [[maybe_unused]] const LsmrScalars& q = S[sy - s0];                                                                      \
-    [[maybe_unused]] const double* b = a.b + sy * rows;                                                                      \
-    [[maybe_unused]] const uint8_t* rm = a.rm + sy * rows;                                                                   \
-    [[maybe_unused]] double *u = a.u + sy * rows, *v = a.v + sy * n, *hv = a.hv + sy * n, *hb = a.hb + sy * n, *x = a.x + sy * n
+    [[maybe_unused]] const double* b = ls.b;                                                                                 \
+    [[maybe_unused]] const uint8_t* rm = ls.rm;                                                                              \
+    [[maybe_unused]] double *u = ls.u, *v = ls.v, *hv = ls.hv, *hb = ls.hb, *x = ls.x
 #define FOR_PIXELS for (int64_t p = vb * static_cast<int64_t>(kLsmrThreads) + threadIdx.x; p < n; p += stride)
 #define PIXEL_IJ const int i = static_cast<int>(p / w), j = static_cast<int>(p % w)
-#define PARTIAL(v0, v1) block_partial(v0, v1, a.part + (static_cast<int64_t>(buf) * items + it) * 2)
-#define SUM (r = warp < nloc ? partial_sum(a.part + (static_cast<int64_t>(buf) * items + static_cast<int64_t>(s0 + warp) * VB) * 2, VB) \
+#define PARTIAL(v0, v1) block_partial(v0, v1, ls.part + (static_cast<int64_t>(buf) * ls.vblocks + vb) * 2)
+#define SUM (r = warp < nloc ? partial_sum(a.s[s0 + warp].part + static_cast<int64_t>(buf) * a.s[s0 + warp].vblocks * 2,       \
+                                           a.s[s0 + warp].vblocks)                                                           \
                              : make_double2(0, 0), buf ^= 1)
     // u = b - A x0 or u = b; ||b||, rows in use; ||u|| (into the other buffer)
     FOR_ITEMS {
         ITEM;
-        const float* init = x32 ? a.init + sy * n : nullptr;
+        const float* init = ls.init;
         double sb = 0, sm = 0, su = 0;
         FOR_PIXELS {
             PIXEL_IJ;
@@ -355,9 +399,14 @@ __global__ void __launch_bounds__(kLsmrThreads) lsmr_kernel(Lsmr a) {
     }
     g.sync();
     SUM;
-    if (lead) { S[warp].normb = sqrt(r.x); S[warp].maxiter = fmin(r.y, static_cast<double>(n)); S[warp].beta = S[warp].normb; }
+    if (lead) {
+        const LsmrSys& ls = a.s[s0 + warp];
+        S[warp].normb = sqrt(r.x);
+        S[warp].maxiter = fmin(r.y, static_cast<double>(static_cast<int64_t>(ls.h) * ls.w));
+        S[warp].beta = S[warp].normb;
+    }
     SUM;
-    if (lead && x32) S[warp].beta = sqrt(r.x);
+    if (lead && a.s[s0 + warp].init != nullptr) S[warp].beta = sqrt(r.x);
     __syncthreads();
     FOR_ITEMS {
         ITEM;
@@ -427,7 +476,7 @@ __global__ void __launch_bounds__(kLsmrThreads) lsmr_kernel(Lsmr a) {
         SUM;
         // the stop flags were written before this barrier and are next written after two more
         bool all = true;
-        for (int k = lane; k < a.batch; k += 32) all = all && __ldcg(a.stop + k) != 0;
+        for (int k = lane; k < a.n; k += 32) all = all && __ldcg(a.stop + k) != 0;
         if (__all_sync(0xffffffffu, all)) break;
         if (lead && !S[warp].done) { ++S[warp].itn; S[warp].beta = sqrt(r.x); }
         __syncthreads();
@@ -517,7 +566,7 @@ __global__ void __launch_bounds__(kLsmrThreads) lsmr_kernel(Lsmr a) {
         if (lead && !S[warp].done) {
             LsmrScalars& q = S[warp];
             double normx = sqrt(r.x);
-            if (x32) normx = static_cast<double>(static_cast<float>(normx));
+            if (a.s[s0 + warp].init != nullptr) normx = static_cast<double>(static_cast<float>(normx));
             const double t1 = q.test1 / (1 + q.normA * normx / q.normb);
             const double rtol = btol + atol * q.normA * normx / q.normb;
             int istop = 0;
@@ -534,8 +583,8 @@ __global__ void __launch_bounds__(kLsmrThreads) lsmr_kernel(Lsmr a) {
         }
         __syncthreads();
     }
-    FOR_ITEMS { ITEM; float* depth = a.depth + sy * n; FOR_PIXELS depth[p] = x32 ? expf(static_cast<float>(x[p])) : __double2float_rn(exp(x[p])); }
-    if (lead && owner) { a.stats[(s0 + warp) * 2] = S[warp].itn; a.stats[(s0 + warp) * 2 + 1] = S[warp].istop; }
+    FOR_ITEMS { ITEM; float* depth = ls.depth; FOR_PIXELS depth[p] = x32 ? expf(static_cast<float>(x[p])) : __double2float_rn(exp(x[p])); }
+    if (lead && owner) { a.s[s0 + warp].stats[0] = S[warp].itn; a.s[s0 + warp].stats[1] = S[warp].istop; }
 #undef FOR_ITEMS
 #undef ITEM
 #undef FOR_PIXELS
@@ -544,8 +593,15 @@ __global__ void __launch_bounds__(kLsmrThreads) lsmr_kernel(Lsmr a) {
 #undef SUM
 }
 
-__global__ void log_kernel(const float* __restrict__ src, float* __restrict__ dst, int64_t n) {
-    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
+struct LogMap { const float* src; float* dst; int64_t n; };
+struct LogTable { LogMap m[MOGE_PANORAMA_MAX_BATCH]; };
+
+// map blockIdx.y of the table: dst = log(src)
+__global__ void log_kernel(const __grid_constant__ LogTable tab) {
+    const LogMap& m = tab.m[blockIdx.y];
+    const float* __restrict__ src = m.src;
+    float* __restrict__ dst = m.dst;
+    for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < m.n; p += static_cast<int64_t>(gridDim.x) * blockDim.x)
         dst[p] = logf(src[p]);
 }
 
@@ -560,11 +616,16 @@ __device__ __forceinline__ void lin_coef(int d, int in, int out, int* s0, int* s
     *s0 = sx; *s1 = min(sx + 1, in - 1); *f = fx;
 }
 
-// panorama blockIdx.y of the batch: src (batch, h, w), dst (batch, H, W)
-__global__ void __launch_bounds__(kThreads) resize_kernel(const float* __restrict__ src, int h, int w, int H, int W, float* __restrict__ dst) {
-    const int64_t n = static_cast<int64_t>(H) * W, pano = blockIdx.y;
-    src += pano * h * w;
-    dst += pano * n;
+struct ResizeMap { const float* src; float* dst; int h, w, H, W; };
+struct ResizeTable { ResizeMap m[MOGE_PANORAMA_MAX_BATCH]; };
+
+// map blockIdx.y of the table: src (h, w) -> dst (H, W)
+__global__ void __launch_bounds__(kThreads) resize_kernel(const __grid_constant__ ResizeTable tab) {
+    const ResizeMap& m = tab.m[blockIdx.y];
+    const float* __restrict__ src = m.src;
+    float* __restrict__ dst = m.dst;
+    const int h = m.h, w = m.w, H = m.H, W = m.W;
+    const int64_t n = static_cast<int64_t>(H) * W;
     for (int64_t p = blockIdx.x * static_cast<int64_t>(blockDim.x) + threadIdx.x; p < n; p += static_cast<int64_t>(gridDim.x) * blockDim.x) {
         const int i = static_cast<int>(p / W), j = static_cast<int>(p % W);
         int x0, x1, y0, y1;
@@ -580,15 +641,18 @@ __global__ void __launch_bounds__(kThreads) resize_kernel(const float* __restric
 }
 
 // cv2.resize INTER_LINEAR of a 0/1 uint8 mask (11-bit fixed-point coefficients), then > 0; and points = depth * direction.
-// Panorama blockIdx.y of the batch: depth (batch, H, W) (already resized), mask (batch, h, w), mask_out (batch, H, W), points
-// (batch, H, W, 3)
-__global__ void __launch_bounds__(kThreads) finish_kernel(const float* __restrict__ depth, const uint8_t* __restrict__ mask, int h, int w,
-                                                          int H, int W, uint8_t* __restrict__ mask_out, float* __restrict__ points) {
-    const int64_t n = static_cast<int64_t>(H) * W, pano = blockIdx.y;
-    depth += pano * n;
-    mask += pano * h * w;
-    mask_out += pano * n;
-    points += pano * n * 3;
+// Panorama blockIdx.y of the table: depth (H, W) (already resized), mask (h, w), mask_out (H, W), points (H, W, 3)
+struct FinishMap { const float* depth; const uint8_t* mask; uint8_t* mask_out; float* points; int h, w, H, W; };
+struct FinishTable { FinishMap m[MOGE_PANORAMA_MAX_BATCH]; };
+
+__global__ void __launch_bounds__(kThreads) finish_kernel(const __grid_constant__ FinishTable tab) {
+    const FinishMap& m = tab.m[blockIdx.y];
+    const float* __restrict__ depth = m.depth;
+    const uint8_t* __restrict__ mask = m.mask;
+    uint8_t* __restrict__ mask_out = m.mask_out;
+    float* __restrict__ points = m.points;
+    const int h = m.h, w = m.w, H = m.H, W = m.W;
+    const int64_t n = static_cast<int64_t>(H) * W;
     // uv_map's linspace ends and steps
     const double su = 0.5 / W, eu = 1.0 - 0.5 / W, sv = 0.5 / H, ev = 1.0 - 0.5 / H;
     const double stu = W > 1 ? (eu - su) / (W - 1) : 0.0, stv = H > 1 ? (ev - sv) / (H - 1) : 0.0;
@@ -638,26 +702,16 @@ int load_cams(const char* what, const moge_panorama_camera_t* cams, int views, C
 
 unsigned blocks_for(int64_t n, int sms) { return static_cast<unsigned>(std::min<int64_t>((n + kThreads - 1) / kThreads, int64_t(sms) * 16)); }
 
-// the workspace of `batch` merges of up to h x w with `views` views
-struct Layout { size_t L, M, u, v, hv, hb, x, part, logi, stop, total; };
-constexpr int kMaxLsmrBlocks = 132 * 4;            // virtual blocks per system
-Layout layout(int views, int h, int w, int batch) {
-    const size_t n = static_cast<size_t>(h) * w, m = batch;
-    WsLayout ws;
-    Layout l;
-    l.L = ws.add(m * views * n * 4);
-    l.M = ws.add(m * views * n);
-    l.u = ws.add(m * (3 * n + h) * 8);
-    l.v = ws.add(m * n * 8);
-    l.hv = ws.add(m * n * 8);
-    l.hb = ws.add(m * n * 8);
-    l.x = ws.add(m * n * 8);
-    l.part = ws.add(m * kMaxLsmrBlocks * 4 * 8);
-    l.logi = ws.add(m * n * 4);
-    l.stop = ws.add(m * 4);
-    l.total = ws.total;
-    return l;
-}
+// an entry's name in messages: the operation's, and in a call of several panoramas also the entry's index
+struct Name {
+    char s[96];
+    Name(const char* what, int k, bool indexed) {
+        if (indexed) snprintf(s, sizeof(s), "%s: panorama %d", what, k);
+        else snprintf(s, sizeof(s), "%s", what);
+    }
+};
+
+int null_argument(const Name& nm, bool indexed) { return indexed ? set_error("%s: null argument", nm.s) : set_error("null argument"); }
 
 int check_batch(const char* what, int batch) {
     if (batch < 1 || batch > MOGE_PANORAMA_MAX_BATCH)
@@ -665,13 +719,111 @@ int check_batch(const char* what, int batch) {
     return 0;
 }
 
-// the LSMR solve of `batch` systems of h x w: the virtual partition, the real grid over at most the co-resident blocks, the launch
-int lsmr(const char* what, const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
-         int32_t* stats, void* workspace, size_t workspace_bytes, void* stream) {
-    if (!b || !row_mask || !depth || !stats) return set_error("null argument");
-    MG_TRY(check_batch(what, batch));
-    MG_TRY(check_size(what, h, w));
-    const Layout l = layout(1, h, w, batch);
+// the workspace of one call's merges: per system its sampled maps L and M, its LSMR arrays (see LsmrSys) and log(init);
+// then the call's stop flags.  Nothing in it outlives a call, and a call whose levels are each no larger fits in the workspace
+// of a bigger one, so the workspace of a pyramid's finest levels serves every coarser level.
+constexpr int kMaxLsmrBlocks = 132 * 4;            // virtual blocks per system
+struct SysLayout { size_t L, M, lsmr, logi; };
+struct Layout { SysLayout s[MOGE_PANORAMA_MAX_BATCH]; size_t stop, total; };
+int max_vblocks(int64_t n) { return static_cast<int>(std::min<int64_t>((n + kLsmrThreads - 1) / kLsmrThreads, kMaxLsmrBlocks)); }
+Layout layout(int views, const moge_panorama_level_t* lv, int count) {
+    WsLayout ws;
+    Layout l;
+    for (int k = 0; k < count; ++k) {
+        const int h = lv[k].h, w = lv[k].w;
+        const size_t n = static_cast<size_t>(h) * w;
+        l.s[k].L = ws.add(views * n * 4);
+        l.s[k].M = ws.add(views * n);
+        l.s[k].lsmr = ws.add((pad32(lsmr_rows(h, w)) + 4 * pad32(n) + 4 * max_vblocks(n)) * 8);
+        l.s[k].logi = ws.add(n * 4);
+    }
+    l.stop = ws.add(static_cast<size_t>(count) * 4);
+    l.total = ws.total;
+    return l;
+}
+
+int check_levels(const char* what, bool indexed, const moge_panorama_level_t* lv, int count) {
+    if (!lv) return set_error("null argument");
+    MG_TRY(check_batch(what, count));
+    for (int k = 0; k < count; ++k) MG_TRY(check_size(Name(what, k, indexed).s, lv[k].h, lv[k].w));
+    return 0;
+}
+
+int workspace_bytes(const char* what, bool indexed, const moge_panorama_level_t* lv, int count, int views, size_t* bytes) {
+    if (!bytes) return set_error("null argument");
+    MG_TRY(check_levels(what, indexed, lv, count));
+    if (views < 1 || views > MOGE_PANORAMA_MAX_VIEWS) return set_error("%s: %d views is outside [1, %d]", what, views, MOGE_PANORAMA_MAX_VIEWS);
+    *bytes = layout(views, lv, count).total;
+    return 0;
+}
+
+int split(const char* what, bool indexed, const moge_panorama_split_t* panos, int count, const moge_panorama_camera_t* cams, int views,
+          const float* grid, int res, float* views_f32, uint8_t* views_u8, void* stream) {
+    if (!panos || !grid || !views_f32) return set_error("null argument");
+    MG_TRY(check_batch(what, count));
+    SplitTable tab{};
+    for (int k = 0; k < count; ++k) {
+        const Name nm(what, k, indexed);
+        if (!panos[k].image) return null_argument(nm, indexed);
+        MG_TRY(check_size(nm.s, panos[k].H, panos[k].W));
+        if (panos[k].view0 < 0) return set_error("%s: first view %d is negative", nm.s, panos[k].view0);
+        tab.p[k] = {panos[k].image, panos[k].H, panos[k].W, panos[k].view0};
+    }
+    if (res < 1 || res > 8192) return set_error("%s: resolution %d is outside [1, 8192]", what, res);
+    Cams cs;
+    MG_TRY(load_cams(what, cams, views, &cs));
+    int sms;
+    MG_TRY(check_device(what, &sms));
+    split_kernel<<<dim3(blocks_for(static_cast<int64_t>(views) * res * res, sms), count), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+        tab, cs, grid, res, views_f32, views_u8);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int rhs(const char* what, bool indexed, const float* src, int channels, const uint8_t* mask, int views, int vh, int vw,
+        const moge_panorama_camera_t* cams, const moge_panorama_level_t* lv, int count, void* workspace, size_t workspace_bytes,
+        void* stream) {
+    if (!src || !mask) return set_error("null argument");
+    if (channels != 1 && channels != 3) return set_error("%s: %d channels (1: distance, 3: points)", what, channels);
+    MG_TRY(check_levels(what, indexed, lv, count));
+    for (int k = 0; k < count; ++k) {
+        const Name nm(what, k, indexed);
+        if (!lv[k].directions || !lv[k].b || !lv[k].row_mask || !lv[k].pano_mask) return null_argument(nm, indexed);
+        if (lv[k].view0 < 0) return set_error("%s: first view %d is negative", nm.s, lv[k].view0);
+    }
+    char vname[112];
+    snprintf(vname, sizeof(vname), "%s view", what);
+    MG_TRY(check_size(vname, vh, vw));
+    Cams cs;
+    MG_TRY(load_cams(what, cams, views, &cs));
+    const Layout l = layout(views, lv, count);
+    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, what));
+    int sms;
+    MG_TRY(check_device(what, &sms));
+    char* ws = static_cast<char*>(workspace);
+    LevelTable tab{};
+    int64_t most = 0;
+    for (int k = 0; k < count; ++k) {
+        const moge_panorama_level_t& e = lv[k];
+        tab.s[k] = {e.directions, reinterpret_cast<float*>(ws + l.s[k].L), reinterpret_cast<uint8_t*>(ws + l.s[k].M), e.b, e.row_mask,
+                    e.pano_mask, e.h, e.w, e.view0};
+        most = std::max<int64_t>(most, static_cast<int64_t>(e.h) * e.w);
+    }
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const dim3 grid(blocks_for(most, sms), count);
+    sample_kernel<<<grid, kThreads, 0, st>>>(src, channels, mask, vh, vw, cs, tab);
+    CUDA_TRY(cudaGetLastError());
+    rhs_kernel<<<grid, kThreads, 0, st>>>(tab, views);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+// the LSMR solves of `count` systems: the virtual partition, the real grid over at most the co-resident blocks, the launch
+int lsmr(const char* what, bool indexed, const moge_panorama_level_t* lv, int count, void* workspace, size_t workspace_bytes, void* stream) {
+    MG_TRY(check_levels(what, indexed, lv, count));
+    for (int k = 0; k < count; ++k)
+        if (!lv[k].b || !lv[k].row_mask || !lv[k].depth || !lv[k].stats) return null_argument(Name(what, k, indexed), indexed);
+    const Layout l = layout(1, lv, count);
     MG_TRY(check_workspace(l.total, workspace, workspace_bytes, what));
     int sms, dev = 0, coop = 0, per_sm = 0;
     MG_TRY(check_device(what, &sms));
@@ -680,34 +832,113 @@ int lsmr(const char* what, const double* b, const uint8_t* row_mask, int batch, 
     if (!coop) return set_error("%s: the device does not support cooperative launches", what);
     CUDA_TRY(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, lsmr_kernel, kLsmrThreads, 0));
     if (per_sm < 1) return set_error("%s: the solver kernel does not fit on an SM", what);
-    const int64_t n = static_cast<int64_t>(h) * w;
-    const int vblocks = static_cast<int>(std::min<int64_t>({sms, (n + kLsmrThreads - 1) / kLsmrThreads, kMaxLsmrBlocks}));
-    const int items = batch * vblocks, resident = sms * per_sm;
-    const int per_block = (items + resident - 1) / resident, blocks = (items + per_block - 1) / per_block;
-    for (int k = 0; k < blocks; ++k) {
-        const int i0 = k * per_block, i1 = std::min(i0 + per_block, items);
-        if ((i1 - 1) / vblocks - i0 / vblocks + 1 > kMaxLocal)
-            return set_error("%s: a block would serve more than %d systems (%d virtual blocks each, %d per block)", what, kMaxLocal,
-                             vblocks, per_block);
-    }
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     char* ws = static_cast<char*>(workspace);
-    Lsmr a;
-    a.b = b; a.rm = row_mask; a.init = nullptr;
-    a.u = reinterpret_cast<double*>(ws + l.u); a.v = reinterpret_cast<double*>(ws + l.v);
-    a.hv = reinterpret_cast<double*>(ws + l.hv); a.hb = reinterpret_cast<double*>(ws + l.hb);
-    a.x = reinterpret_cast<double*>(ws + l.x); a.part = reinterpret_cast<double*>(ws + l.part);
-    a.depth = depth; a.stats = stats; a.stop = reinterpret_cast<int*>(ws + l.stop);
-    a.h = h; a.w = w; a.batch = batch; a.vblocks = vblocks; a.per_block = per_block;
-    if (init) {                                  // x0 = log(init), fp32
-        float* logi = reinterpret_cast<float*>(ws + l.logi);
-        log_kernel<<<blocks_for(n * batch, sms), kThreads, 0, st>>>(init, logi, n * batch);
+    LsmrTable a{};
+    LogTable logs{};
+    int items = 0, nlog = 0;
+    int64_t most = 0;
+    for (int k = 0; k < count; ++k) {
+        const moge_panorama_level_t& e = lv[k];
+        const int64_t n = static_cast<int64_t>(e.h) * e.w;
+        const int vblocks = std::min(sms, max_vblocks(n));
+        const float* init = nullptr;
+        if (e.init) {                                // x0 = log(init), fp32
+            float* logi = reinterpret_cast<float*>(ws + l.s[k].logi);
+            logs.m[nlog++] = {e.init, logi, n};
+            most = std::max(most, n);
+            init = logi;
+        }
+        double* u = reinterpret_cast<double*>(ws + l.s[k].lsmr);
+        double* v = u + pad32(lsmr_rows(e.h, e.w));
+        a.s[k] = {e.b, e.row_mask, init, e.depth, e.stats, u, v, v + pad32(n), v + 2 * pad32(n), v + 3 * pad32(n), v + 4 * pad32(n),
+                  e.h, e.w, vblocks, items};
+        items += vblocks;
+    }
+    const int resident = sms * per_sm;
+    const int per_block = (items + resident - 1) / resident, blocks = (items + per_block - 1) / per_block;
+    for (int b = 0, s0 = 0; b < blocks; ++b) {       // the systems of each real block's run of virtual blocks
+        const int i0 = b * per_block, i1 = std::min(i0 + per_block, items);
+        while (s0 + 1 < count && a.s[s0 + 1].item0 <= i0) ++s0;
+        int s1 = s0;
+        while (s1 + 1 < count && a.s[s1 + 1].item0 <= i1 - 1) ++s1;
+        if (s1 - s0 + 1 > kMaxLocal)
+            return set_error("%s: a block would serve more than %d systems (%d virtual blocks per block)", what, kMaxLocal, per_block);
+    }
+    a.stop = reinterpret_cast<int*>(ws + l.stop);
+    a.n = count; a.items = items; a.per_block = per_block;
+    if (nlog) {
+        log_kernel<<<dim3(blocks_for(most, sms), nlog), kThreads, 0, st>>>(logs);
         CUDA_TRY(cudaGetLastError());
-        a.init = logi;
     }
     void* args[] = {&a};
     CUDA_TRY(cudaLaunchCooperativeKernel(reinterpret_cast<void*>(lsmr_kernel), dim3(blocks), dim3(kLsmrThreads), args, 0, st));
     return 0;
+}
+
+int resize(const char* what, bool indexed, const moge_panorama_resize_t* maps, int count, void* stream) {
+    if (!maps) return set_error("null argument");
+    MG_TRY(check_batch(what, count));
+    ResizeTable tab{};
+    int64_t most = 0;
+    for (int k = 0; k < count; ++k) {
+        const Name nm(what, k, indexed);
+        const moge_panorama_resize_t& m = maps[k];
+        if (!m.src || !m.dst) return null_argument(nm, indexed);
+        MG_TRY(check_size(nm.s, m.h, m.w));
+        MG_TRY(check_size(nm.s, m.H, m.W));
+        tab.m[k] = {m.src, m.dst, m.h, m.w, m.H, m.W};
+        most = std::max<int64_t>(most, static_cast<int64_t>(m.H) * m.W);
+    }
+    int sms;
+    MG_TRY(check_device(what, &sms));
+    resize_kernel<<<dim3(blocks_for(most, sms), count), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(tab);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+int finish(const char* what, bool indexed, const moge_panorama_finish_t* maps, int count, void* stream) {
+    if (!maps) return set_error("null argument");
+    MG_TRY(check_batch(what, count));
+    ResizeTable rt{};
+    FinishTable ft{};
+    int64_t most = 0;
+    for (int k = 0; k < count; ++k) {
+        const Name nm(what, k, indexed);
+        const moge_panorama_finish_t& m = maps[k];
+        if (!m.depth || !m.mask || !m.depth_out || !m.mask_out || !m.points) return null_argument(nm, indexed);
+        MG_TRY(check_size(nm.s, m.h, m.w));
+        MG_TRY(check_size(nm.s, m.H, m.W));
+        rt.m[k] = {m.depth, m.depth_out, m.h, m.w, m.H, m.W};
+        ft.m[k] = {m.depth_out, m.mask, m.mask_out, m.points, m.h, m.w, m.H, m.W};
+        most = std::max<int64_t>(most, static_cast<int64_t>(m.H) * m.W);
+    }
+    int sms;
+    MG_TRY(check_device(what, &sms));
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const dim3 grid(blocks_for(most, sms), count);
+    resize_kernel<<<grid, kThreads, 0, st>>>(rt);
+    CUDA_TRY(cudaGetLastError());
+    finish_kernel<<<grid, kThreads, 0, st>>>(ft);
+    CUDA_TRY(cudaGetLastError());
+    return 0;
+}
+
+// the `batch` same-size levels of the one-size entry points, back to back in b, row_mask (rows each), pano_mask, init and depth
+// (h * w each) and stats (2 each); the caller has checked batch
+void one_size_levels(int batch, int views, int h, int w, const float* directions, double* b, uint8_t* row_mask, uint8_t* pano_mask,
+                     const float* init, float* depth, int32_t* stats, moge_panorama_level_t* lv) {
+    const int64_t n = static_cast<int64_t>(h) * w, rows = lsmr_rows(h, w);
+    for (int k = 0; k < batch; ++k) {
+        moge_panorama_level_t& e = lv[k];
+        e.h = h; e.w = w; e.view0 = k * views; e.directions = directions;
+        e.b = b ? b + k * rows : nullptr;
+        e.row_mask = row_mask ? row_mask + k * rows : nullptr;
+        e.pano_mask = pano_mask ? pano_mask + k * n : nullptr;
+        e.init = init ? init + k * n : nullptr;
+        e.depth = depth ? depth + k * n : nullptr;
+        e.stats = stats ? stats + 2 * k : nullptr;
+    }
 }
 
 }  // namespace
@@ -717,90 +948,88 @@ using namespace mg;
 
 extern "C" {
 
+int moge_panorama_split_groups(const moge_panorama_split_t* panos, int n, const moge_panorama_camera_t* cams, int views, const float* grid,
+                               int res, float* views_f32, uint8_t* views_u8, void* stream) {
+    return split("panorama_split_groups", true, panos, n, cams, views, grid, res, views_f32, views_u8, stream);
+}
+
 int moge_panorama_split(const uint8_t* images, int batch, int H, int W, const moge_panorama_camera_t* cams, int views, const float* grid,
                         int res, float* views_f32, uint8_t* views_u8, void* stream) {
     if (!images || !grid || !views_f32) return set_error("null argument");
     MG_TRY(check_batch("panorama_split", batch));
-    MG_TRY(check_size("panorama_split", H, W));
-    if (res < 1 || res > 8192) return set_error("panorama_split: resolution %d is outside [1, 8192]", res);
-    Cams cs;
-    MG_TRY(load_cams("panorama_split", cams, views, &cs));
-    int sms;
-    MG_TRY(check_device("panorama_split", &sms));
-    split_kernel<<<dim3(blocks_for(static_cast<int64_t>(views) * res * res, sms), batch), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        images, H, W, cs, grid, res, views_f32, views_u8);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
+    moge_panorama_split_t panos[MOGE_PANORAMA_MAX_BATCH];
+    for (int k = 0; k < batch; ++k) panos[k] = {images + static_cast<int64_t>(k) * H * W * 3, H, W, k * std::max(views, 0)};
+    return split("panorama_split", false, panos, batch, cams, views, grid, res, views_f32, views_u8, stream);
+}
+
+int moge_panorama_workspace_bytes_groups(const moge_panorama_level_t* levels, int n, int views, size_t* bytes) {
+    return workspace_bytes("panorama_workspace_bytes_groups", true, levels, n, views, bytes);
 }
 
 int moge_panorama_workspace_bytes(int batch, int views, int h, int w, size_t* bytes) {
     if (!bytes) return set_error("null argument");
     MG_TRY(check_batch("panorama_workspace_bytes", batch));
-    MG_TRY(check_size("panorama_workspace_bytes", h, w));
-    if (views < 1 || views > MOGE_PANORAMA_MAX_VIEWS) return set_error("panorama_workspace_bytes: %d views is outside [1, %d]", views, MOGE_PANORAMA_MAX_VIEWS);
-    *bytes = layout(views, h, w, batch).total;
-    return 0;
+    moge_panorama_level_t lv[MOGE_PANORAMA_MAX_BATCH];
+    one_size_levels(batch, 0, h, w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, lv);
+    return workspace_bytes("panorama_workspace_bytes", false, lv, batch, views, bytes);
+}
+
+int moge_panorama_rhs_groups(const float* src, int channels, const uint8_t* mask, int views, int vh, int vw,
+                             const moge_panorama_camera_t* cams, const moge_panorama_level_t* levels, int n, void* workspace,
+                             size_t workspace_bytes, void* stream) {
+    return rhs("panorama_rhs_groups", true, src, channels, mask, views, vh, vw, cams, levels, n, workspace, workspace_bytes, stream);
 }
 
 int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int batch, int views, int vh, int vw,
                       const moge_panorama_camera_t* cams, const float* directions, int h, int w, double* b, uint8_t* row_mask,
                       uint8_t* pano_mask, void* workspace, size_t workspace_bytes, void* stream) {
     if (!src || !mask || !directions || !b || !row_mask || !pano_mask) return set_error("null argument");
-    if (channels != 1 && channels != 3) return set_error("panorama_rhs: %d channels (1: distance, 3: points)", channels);
     MG_TRY(check_batch("panorama_rhs", batch));
-    MG_TRY(check_size("panorama_rhs view", vh, vw));
-    MG_TRY(check_size("panorama_rhs", h, w));
-    Cams cs;
-    MG_TRY(load_cams("panorama_rhs", cams, views, &cs));
-    const Layout l = layout(views, h, w, batch);
-    MG_TRY(check_workspace(l.total, workspace, workspace_bytes, "panorama_rhs"));
-    int sms;
-    MG_TRY(check_device("panorama_rhs", &sms));
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    char* ws = static_cast<char*>(workspace);
-    float* L = reinterpret_cast<float*>(ws + l.L);
-    uint8_t* M = reinterpret_cast<uint8_t*>(ws + l.M);
-    const dim3 grid(blocks_for(static_cast<int64_t>(h) * w, sms), batch);
-    sample_kernel<<<grid, kThreads, 0, st>>>(src, channels, mask, vh, vw, cs, directions, h, w, L, M);
-    CUDA_TRY(cudaGetLastError());
-    rhs_kernel<<<grid, kThreads, 0, st>>>(L, M, views, h, w, b, row_mask, pano_mask);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
+    moge_panorama_level_t lv[MOGE_PANORAMA_MAX_BATCH];
+    one_size_levels(batch, std::max(views, 0), h, w, directions, b, row_mask, pano_mask, nullptr, nullptr, nullptr, lv);
+    return rhs("panorama_rhs", false, src, channels, mask, views, vh, vw, cams, lv, batch, workspace, workspace_bytes, stream);
+}
+
+int moge_panorama_lsmr_groups(const moge_panorama_level_t* levels, int n, void* workspace, size_t workspace_bytes, void* stream) {
+    return lsmr("panorama_lsmr_groups", true, levels, n, workspace, workspace_bytes, stream);
 }
 
 int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
                        int32_t* stats, void* workspace, size_t workspace_bytes, void* stream) {
-    return lsmr("panorama_lsmr", b, row_mask, batch, h, w, init, depth, stats, workspace, workspace_bytes, stream);
+    if (!b || !row_mask || !depth || !stats) return set_error("null argument");
+    MG_TRY(check_batch("panorama_lsmr", batch));
+    moge_panorama_level_t lv[MOGE_PANORAMA_MAX_BATCH];
+    one_size_levels(batch, 0, h, w, nullptr, const_cast<double*>(b), const_cast<uint8_t*>(row_mask), nullptr, init, depth, stats, lv);
+    return lsmr("panorama_lsmr", false, lv, batch, workspace, workspace_bytes, stream);
+}
+
+int moge_panorama_resize_groups(const moge_panorama_resize_t* maps, int n, void* stream) {
+    return resize("panorama_resize_groups", true, maps, n, stream);
 }
 
 int moge_panorama_resize(const float* src, int batch, int h, int w, int H, int W, float* dst, void* stream) {
     if (!src || !dst) return set_error("null argument");
     MG_TRY(check_batch("panorama_resize", batch));
-    MG_TRY(check_size("panorama_resize", h, w));
-    MG_TRY(check_size("panorama_resize", H, W));
-    int sms;
-    MG_TRY(check_device("panorama_resize", &sms));
-    resize_kernel<<<dim3(blocks_for(static_cast<int64_t>(H) * W, sms), batch), kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-        src, h, w, H, W, dst);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
+    moge_panorama_resize_t maps[MOGE_PANORAMA_MAX_BATCH];
+    for (int k = 0; k < batch; ++k)
+        maps[k] = {src + static_cast<int64_t>(k) * h * w, h, w, H, W, dst + static_cast<int64_t>(k) * H * W};
+    return resize("panorama_resize", false, maps, batch, stream);
+}
+
+int moge_panorama_finish_groups(const moge_panorama_finish_t* maps, int n, void* stream) {
+    return finish("panorama_finish_groups", true, maps, n, stream);
 }
 
 int moge_panorama_finish(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
                          uint8_t* mask_out, float* points, void* stream) {
     if (!depth || !mask || !depth_out || !mask_out || !points) return set_error("null argument");
     MG_TRY(check_batch("panorama_finish", batch));
-    MG_TRY(check_size("panorama_finish", h, w));
-    MG_TRY(check_size("panorama_finish", H, W));
-    int sms;
-    MG_TRY(check_device("panorama_finish", &sms));
-    cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const dim3 grid(blocks_for(static_cast<int64_t>(H) * W, sms), batch);
-    resize_kernel<<<grid, kThreads, 0, st>>>(depth, h, w, H, W, depth_out);
-    CUDA_TRY(cudaGetLastError());
-    finish_kernel<<<grid, kThreads, 0, st>>>(depth_out, mask, h, w, H, W, mask_out, points);
-    CUDA_TRY(cudaGetLastError());
-    return 0;
+    moge_panorama_finish_t maps[MOGE_PANORAMA_MAX_BATCH];
+    for (int k = 0; k < batch; ++k) {
+        const int64_t in = static_cast<int64_t>(k) * h * w, out = static_cast<int64_t>(k) * H * W;
+        maps[k] = {depth + in, mask + in, h, w, H, W, depth_out + out, mask_out + out, points + out * 3};
+    }
+    return finish("panorama_finish", false, maps, batch, stream);
 }
 
 }  // extern "C"
