@@ -77,29 +77,23 @@ int moge_engine_set_weight(moge_engine_t* e, const char* key, const void* dev_pt
  * first missing key.  Must be called once after the last set_weight and before forward. */
 int moge_engine_finalize(moge_engine_t* e, void* stream);
 
-/* workspace (activations) size for a forward of B images of HxW pixels on an hxw token grid */
-int moge_engine_workspace_bytes(moge_engine_t* e, int B, int H, int W, int h, int w, size_t* bytes);
-
-/* replaces MoGeModel.forward (v2.py:138-192).  image: (B,3,H,W) in [0,1], dtype image_dtype.  h,w: token grid
- * (v2.py:142-147, computed by the caller).  Outputs are fp32, caller-allocated; pass NULL for absent heads:
- *   points (B,H,W,3)  normal (B,H,W,3)  mask_prob (B,H,W)  metric_scale (B,)                                     */
-int moge_engine_forward(moge_engine_t* e, const void* image, int image_dtype, int B, int H, int W, int h, int w,
-                        void* workspace, size_t workspace_bytes, float* points, float* normal, float* mask_prob,
-                        float* metric_scale, void* stream);
-
-/* Mixed-shape ("ragged") batches -- BASELINE.json configs[2]; the reference has no counterpart (a batch tensor has one shape and
- * its nested-tensor path, dinov2/layers/block.py:160-259, is dead code without xformers).  A call carries `n` shape groups; the
- * encoder (every linear, the attention) runs ONCE over the token rows of all groups packed back to back, the per-pixel stages
- * (resize/patchify, pos embed, decoder, output resize) run group by group.  moge_engine_forward is the n = 1 case. */
+/* replaces MoGeModel.forward (v2.py:138-192).  A call carries `n` shape groups; one image shape is a call with one group.
+ * Per group: image (B,3,H,W) in [0,1], dtype image_dtype; h,w its token grid (v2.py:142-147, computed by the caller).  Outputs
+ * are fp32, caller-allocated; pass NULL for absent heads.
+ * Mixed-shape ("ragged") batches -- BASELINE.json configs[2]; the reference has no counterpart (a batch tensor has one shape and
+ * its nested-tensor path, dinov2/layers/block.py:160-259, is dead code without xformers).  The encoder (every linear, the
+ * attention) runs ONCE over the token rows of all groups packed back to back, the per-pixel stages (resize/patchify, pos embed,
+ * decoder, output resize) run group by group. */
 typedef struct moge_group {
     const void* image;          /* (B,3,H,W) in [0,1] */
     int image_dtype;            /* MOGE_F32 / MOGE_F16 / MOGE_BF16 */
-    int B, H, W, h, w;          /* images, pixels, token grid of this group */
+    int B, H, W, h, w;          /* images, pixels, token grid of this group (computed by the caller) */
     float* points;              /* (B,H,W,3) or NULL */
     float* normal;              /* (B,H,W,3) or NULL */
     float* mask_prob;           /* (B,H,W) or NULL */
     float* metric_scale;        /* (B,) or NULL */
 } moge_group_t;
+/* workspace (activations) size for a forward of these groups */
 int moge_engine_workspace_bytes_groups(moge_engine_t* e, const moge_group_t* groups, int n, size_t* bytes);
 int moge_engine_forward_groups(moge_engine_t* e, const moge_group_t* groups, int n, void* workspace, size_t workspace_bytes,
                                void* stream);
@@ -226,24 +220,20 @@ typedef struct moge_v1_config {
     int compute_dtype;                    /* MOGE_F16 or MOGE_BF16 */
 } moge_v1_config_t;
 int moge_engine_create_v1(const moge_v1_config_t* cfg, int device, moge_engine_t** out);
-/* workspace for B images of HxW pixels resized to (rh, rw) (v1.py:273-274: rh = int(H f), rw = int(W f)); token grid rh/14 x rw/14 */
-int moge_v1_workspace_bytes(moge_engine_t* e, int B, int H, int W, int rh, int rw, size_t* bytes);
-/* replaces MoGeModel.forward (v1.py:269-299): image (B,3,H,W) in [0,1]; points (B,H,W,3) remapped, mask (B,H,W) the raw mask
- * output (no sigmoid), both fp32 */
-int moge_v1_forward(moge_engine_t* e, const void* image, int image_dtype, int B, int H, int W, int rh, int rw, void* workspace,
-                    size_t workspace_bytes, float* points, float* mask, void* stream);
-/* Mixed-shape MoGe-1 batches, as moge_engine_forward_groups for MoGe-2: a call carries `n` (1..64) shape groups; the encoder runs
- * ONCE over the token rows of all groups packed back to back, the resize, decoder and output resize run group by group through
- * one set of decoder maps sized for the largest group.  Each group is checked as moge_v1_forward checks its arguments, before
- * anything runs.  moge_v1_workspace_bytes / moge_v1_forward are the n = 1 case.  Python: MoGeModel.infer_many (moge.model.v1). */
+/* replaces MoGeModel.forward (v1.py:269-299), as moge_engine_forward_groups for MoGe-2: a call carries `n` (1..64) shape groups;
+ * one image shape is a call with one group.  The encoder runs ONCE over the token rows of all groups packed back to back, the
+ * resize, decoder and output resize run group by group through one set of decoder maps sized for the largest group.  Every group
+ * is checked before anything runs.  Outputs are fp32.  Python: MoGeModel.forward / infer / infer_many (moge.model.v1). */
 typedef struct moge_v1_group {
     const void* image;          /* (B,3,H,W) in [0,1] */
     int image_dtype;            /* MOGE_F32 / MOGE_F16 / MOGE_BF16 */
     int B, H, W;                /* images and pixels of this group */
-    int rh, rw;                 /* its resized image (>= 14 each); token grid rh/14 x rw/14 */
-    float* points;              /* (B,H,W,3) */
-    float* mask;                /* (B,H,W), the raw mask output */
+    int rh, rw;                 /* its resized image (>= 14 each; v1.py:273-274: rh = int(H f), rw = int(W f)); token grid
+                                   rh/14 x rw/14 */
+    float* points;              /* (B,H,W,3), remapped */
+    float* mask;                /* (B,H,W), the raw mask output (no sigmoid) */
 } moge_v1_group_t;
+/* workspace for a forward of these groups */
 int moge_v1_workspace_bytes_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, size_t* bytes);
 int moge_v1_forward_groups(moge_engine_t* e, const moge_v1_group_t* groups, int n, void* workspace, size_t workspace_bytes,
                            void* stream);
@@ -290,21 +280,16 @@ int moge_dino_create(const moge_dino_config_t* cfg, int device, moge_engine_t** 
  * patch tokens as (B, D, h, w) instead of (B, T, D) */
 #define MOGE_DINO_NORM 1
 #define MOGE_DINO_CHANNEL_MAJOR 2
-int moge_dino_workspace_bytes(moge_engine_t* e, int B, int H, int W, const int* layers, int n_layers, int flags, size_t* bytes);
-/* x (B,3,H,W), dtype x_dtype (MOGE_F32/F16/BF16), normalised; h = H/14, w = W/14, T = h*w.  layers: n_layers (0..depth) strictly
- * increasing block indices; after block layers[j] the residual stream (or its final LayerNorm, MOGE_DINO_NORM) is written, fp32:
+/* A call carries `n` (1..MOGE_DINO_MAX_GROUPS) shape groups; one image shape is a call with one group.  `layers` and `flags` apply
+ * to every group.  Per group: x (B,3,H,W), dtype x_dtype (MOGE_F32/F16/BF16), normalised; h = H/14, w = W/14, T = h*w.  layers:
+ * n_layers (0..depth) strictly increasing block indices; after block layers[j] the residual stream (or its final LayerNorm,
+ * MOGE_DINO_NORM) is written, fp32:
  *   out_tokens  layer j at out_tokens + j*B*T*D, as (B,T,D) or, with MOGE_DINO_CHANNEL_MAJOR, (B,D,h,w)
  *   out_cls     layer j's class-token rows at out_cls + j*B*D, (B,D)
  *   out_prenorm the residual stream after the last block, (B,T+1,D), the class token first
  * Any output may be NULL.  Rows are normalised with fixed-order statistics and no atomics: the outputs of an image are bitwise the
- * same run to run. */
-int moge_dino_forward(moge_engine_t* e, const void* x, int x_dtype, int B, int H, int W, const int* layers, int n_layers, int flags,
-                      float* out_tokens, float* out_cls, float* out_prenorm, void* workspace, size_t workspace_bytes, void* stream);
-/* Mixed-shape backbone batches: a call carries `n` (1..MOGE_DINO_MAX_GROUPS) shape groups, each the arguments of one
- * moge_dino_forward call with its outputs laid out as documented there for that group's B, H, W.  `layers` and `flags` apply to
- * every group.  The encoder runs once over the token rows of all groups packed back to back; the front end and each exported
- * block's export are one launch each over all groups.  An image's outputs are bitwise those it gets in a call of its own.
- * moge_dino_forward and moge_dino_workspace_bytes are the n = 1 case. */
+ * same run to run.  The encoder runs once over the token rows of all groups packed back to back; the front end and each exported
+ * block's export are one launch each over all groups.  An image's outputs are bitwise those it gets in a call of its own. */
 #define MOGE_DINO_MAX_GROUPS 64
 typedef struct moge_dino_group {
     const void* x; int x_dtype;
@@ -429,55 +414,35 @@ int moge_mesh_build(const uint8_t* mask, int64_t batch, int H, int W, int tri, c
  * maps are equirectangular, h x w, at least 2 x 2 and at most 2^28 pixels.                                                  */
 #define MOGE_PANORAMA_MAX_VIEWS 20
 typedef struct { float R[9]; float t[3]; double fx, fy, cx, cy; } moge_panorama_camera_t;
-/* Every call takes 1 to MOGE_PANORAMA_MAX_BATCH panoramas with one set of cameras; each panorama's result is bitwise what it
- * gets in a call of its own.  The `_groups` entry points (after these) take an array of per-panorama sizes and pointers, so the
- * panoramas of a call may differ in size; the entry points here take `batch` panoramas of one size with arrays that have a
- * leading batch dimension, and are implemented as the `_groups` call over those panoramas back to back.                     */
+/* Every call takes `n` (1..MOGE_PANORAMA_MAX_BATCH) entries, one per panorama, each with its own sizes and pointers, and one set of
+ * cameras; a single panorama is a call with one entry.  Each kernel is one launch over all entries, and each panorama's result is
+ * bitwise what it gets in a call of its own.  An entry's error names its index.  The entry count is checked first, and every
+ * argument before the device is touched.                                                                                     */
 #define MOGE_PANORAMA_MAX_BATCH 64
-/* split_panorama_image: views_f32 (batch * views, 3, res, res) = value / 255 of cv2.remap(image, INTER_LINEAR, BORDER_CONSTANT 0)
- * at the panorama pixel of each view pixel's ray; grid (res) is the fp32 pixel-centre coordinate of uv_map; views_u8
- * (batch * views, res, res, 3) the uint8 values (may be NULL).  images (batch, H, W, 3) uint8 RGB.                           */
-int moge_panorama_split(const uint8_t* images, int batch, int H, int W, const moge_panorama_camera_t* cams, int views, const float* grid,
-                        int res, float* views_f32, uint8_t* views_u8, void* stream);
-/* workspace (256-byte aligned) of moge_panorama_rhs / moge_panorama_lsmr for `batch` merges of a level of h x w (and for every
- * smaller level) */
-int moge_panorama_workspace_bytes(int batch, int views, int h, int w, size_t* bytes);
-/* one merge level's right-hand side: src (batch, views, vh, vw, channels) fp32 is the distance (channels 1) or the point map whose
- * norm is the distance (channels 3), mask (batch, views, vh, vw) uint8, directions (h, w, 3) fp32 the panorama rays.  b fp64 and
- * row_mask uint8 are (batch, rows) with 2hw + (h-1)(w+1) rows in the reference's order: x-gradient h*w, y-gradient (h-1) x (w+1)
- * (column w repeats column 0, as the reference's x-wrapped grid does), Laplacian h*w; b = 0 where masked out.  pano_mask
- * (batch, h, w) uint8 = any view's mask.                                                                                     */
-int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int batch, int views, int vh, int vw,
-                      const moge_panorama_camera_t* cams, const float* directions, int h, int w, double* b, uint8_t* row_mask,
-                      uint8_t* pano_mask, void* workspace, size_t workspace_bytes, void* stream);
-/* SciPy's lsmr(A, b, atol = btol = 1e-5, x0 = log(init)) on the rows of row_mask (init NULL: x0 = None), depth (batch, h, w)
- * fp32 = exp(x); stats (batch, 2) int32 on the device = (iterations, istop).  One cooperative launch for the whole batch, which
- * ends when every system has stopped; no host synchronisation.                                                               */
-int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
-                       int32_t* stats, void* workspace, size_t workspace_bytes, void* stream);
-/* cv2.resize(src, (W, H), INTER_LINEAR) of fp32 maps, src (batch, h, w), dst (batch, H, W): the pyramid's upsampling */
-int moge_panorama_resize(const float* src, int batch, int h, int w, int H, int W, float* dst, void* stream);
-/* infer_panorama.py:120-122: depth_out (batch, H, W) the resized depth, mask_out (batch, H, W) uint8 the bilinear resize of the
- * 0/1 mask > 0, points (batch, H, W, 3) = depth_out * spherical_uv_to_directions(uv_map(H, W)).                             */
-int moge_panorama_finish(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
-                         uint8_t* mask_out, float* points, void* stream);
-/* Mixed-size calls: `n` (1..MOGE_PANORAMA_MAX_BATCH) entries, one per panorama, each with its own sizes and pointers; each kernel
- * is one launch over all of them.  With several entries, an entry's error names its index.  The entry count is checked first,
- * and every argument before the device is touched.
- * split: panorama k's image (H, W, 3) uint8 RGB; its views go to views_f32 / views_u8 from view view0 on.                    */
-typedef struct moge_panorama_split {
+/* split_panorama_image: views_f32 (views total, 3, res, res) = value / 255 of cv2.remap(image, INTER_LINEAR, BORDER_CONSTANT 0) at
+ * the panorama pixel of each view pixel's ray; grid (res) is the fp32 pixel-centre coordinate of uv_map; views_u8 (views total,
+ * res, res, 3) the uint8 values (may be NULL).  Panorama k's image is (H, W, 3) uint8 RGB; its `views` views go to views_f32 /
+ * views_u8 from view view0 on.                                                                                               */
+typedef struct {
     const uint8_t* image;
     int H, W;
     int view0;
 } moge_panorama_split_t;
 int moge_panorama_split_groups(const moge_panorama_split_t* panos, int n, const moge_panorama_camera_t* cams, int views,
                                const float* grid, int res, float* views_f32, uint8_t* views_u8, void* stream);
-/* One merge level of one panorama, h x w, as moge_panorama_rhs writes it (directions, b, row_mask, pano_mask; its views are views
- * view0 .. view0 + views - 1 of src and mask) and moge_panorama_lsmr solves it (b, row_mask, init or NULL, depth, stats (2)).
- * Each call reads the fields it names.  The systems of one lsmr call share one cooperative launch; a system's reductions depend
- * on its own size only, so it gets bitwise its single-call result.  The workspace of a call fits any call whose entries are
+/* One merge level of one panorama, h x w.  Each call reads the fields it names.
+ * rhs: the level's right-hand side.  src (views total, vh, vw, channels) fp32 is the distance (channels 1) or the point map whose
+ * norm is the distance (channels 3), mask (views total, vh, vw) uint8; the entry's views are view0 .. view0 + views - 1 of them.
+ * directions (h, w, 3) fp32 are the panorama rays.  b fp64 and row_mask uint8 hold 2hw + (h-1)(w+1) rows in the reference's
+ * order: x-gradient h*w, y-gradient (h-1) x (w+1) (column w repeats column 0, as the reference's x-wrapped grid does), Laplacian
+ * h*w; b = 0 where masked out.  pano_mask (h, w) uint8 = any view's mask.
+ * lsmr: SciPy's lsmr(A, b, atol = btol = 1e-5, x0 = log(init)) on the rows of row_mask (init NULL: x0 = None), depth (h, w) fp32
+ * = exp(x); stats (2) int32 on the device = (iterations, istop).  The systems of one call share one cooperative launch, which ends
+ * when every system has stopped; no host synchronisation.  A system's reductions depend on its own size only, so it gets bitwise
+ * its single-call result.
+ * workspace_bytes: the workspace (256-byte aligned) of rhs and lsmr.  The workspace of a call fits any call whose entries are
  * each no larger (so the finest levels' workspace serves every coarser level).                                               */
-typedef struct moge_panorama_level {
+typedef struct {
     int h, w;
     int view0;
     const float* directions;
@@ -493,14 +458,16 @@ int moge_panorama_rhs_groups(const float* src, int channels, const uint8_t* mask
                              const moge_panorama_camera_t* cams, const moge_panorama_level_t* levels, int n, void* workspace,
                              size_t workspace_bytes, void* stream);
 int moge_panorama_lsmr_groups(const moge_panorama_level_t* levels, int n, void* workspace, size_t workspace_bytes, void* stream);
-/* resize: src (h, w) -> dst (H, W).  finish: depth (h, w) and mask (h, w) -> depth_out, mask_out and points at (H, W).        */
-typedef struct moge_panorama_resize {
+/* cv2.resize(src, (W, H), INTER_LINEAR) of fp32 maps, src (h, w) -> dst (H, W): the pyramid's upsampling */
+typedef struct {
     const float* src;
     int h, w, H, W;
     float* dst;
 } moge_panorama_resize_t;
 int moge_panorama_resize_groups(const moge_panorama_resize_t* maps, int n, void* stream);
-typedef struct moge_panorama_finish {
+/* infer_panorama.py:120-122: from depth (h, w) and mask (h, w), depth_out (H, W) the resized depth, mask_out (H, W) uint8 the
+ * bilinear resize of the 0/1 mask > 0, points (H, W, 3) = depth_out * spherical_uv_to_directions(uv_map(H, W)).              */
+typedef struct {
     const float* depth;
     const uint8_t* mask;
     int h, w, H, W;

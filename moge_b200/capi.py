@@ -155,8 +155,6 @@ SIGNATURES = {
     "moge_engine_destroy": (None, [vp]),
     "moge_engine_set_weight": [vp, C.c_char_p, vp, C.POINTER(i64), ci, ci, vp],
     "moge_engine_finalize": [vp, vp],
-    "moge_engine_workspace_bytes": [vp, ci, ci, ci, ci, ci, C.POINTER(sz)],
-    "moge_engine_forward": [vp, vp, ci, ci, ci, ci, ci, ci, vp, sz, vp, vp, vp, vp, vp],
     "moge_engine_workspace_bytes_groups": [vp, C.POINTER(Group), ci, C.POINTER(sz)],
     "moge_engine_forward_groups": [vp, C.POINTER(Group), ci, vp, sz, vp],
     "moge_engine_num_ops": [vp, C.POINTER(ci)],
@@ -189,8 +187,6 @@ SIGNATURES = {
     "moge_align_anchored": [vp, vp, vp, ci, C.c_float, i64, ci, vp, vp, vp, vp, sz, vp],
     "moge_align_affine_lstsq": [vp, vp, vp, i64, i64, vp, vp, vp],
     "moge_engine_create_v1": [C.POINTER(V1Config), ci, C.POINTER(vp)],
-    "moge_v1_workspace_bytes": [vp, ci, ci, ci, ci, ci, C.POINTER(sz)],
-    "moge_v1_forward": [vp, vp, ci, ci, ci, ci, ci, ci, vp, sz, vp, vp, vp],
     "moge_v1_workspace_bytes_groups": [vp, C.POINTER(V1Group), ci, C.POINTER(sz)],
     "moge_v1_forward_groups": [vp, C.POINTER(V1Group), ci, vp, sz, vp],
     "moge_v1_postprocess": [vp, vp, C.c_float, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp],
@@ -210,12 +206,6 @@ SIGNATURES = {
     "moge_mesh_build": [vp, i64, ci, ci, ci, C.POINTER(MeshMap), ci, vp, vp, vp, sz, vp],
     "moge_normal_map": [vp, vp, i64, ci, ci, vp, vp, vp],
     "moge_normal_edge": [vp, vp, vp, vp, i64, ci, ci, ci, C.c_double, vp, vp, vp],
-    "moge_panorama_split": [vp, ci, ci, ci, pc, ci, vp, ci, vp, vp, vp],
-    "moge_panorama_workspace_bytes": [ci, ci, ci, ci, C.POINTER(sz)],
-    "moge_panorama_rhs": [vp, ci, vp, ci, ci, ci, ci, pc, vp, ci, ci, vp, vp, vp, vp, sz, vp],
-    "moge_panorama_lsmr": [vp, vp, ci, ci, ci, vp, vp, vp, vp, sz, vp],
-    "moge_panorama_resize": [vp, ci, ci, ci, ci, ci, vp, vp],
-    "moge_panorama_finish": [vp, vp, ci, ci, ci, ci, ci, vp, vp, vp, vp],
     "moge_panorama_split_groups": [C.POINTER(PanoramaSplit), ci, pc, ci, vp, ci, vp, vp, vp],
     "moge_panorama_workspace_bytes_groups": [C.POINTER(PanoramaLevel), ci, ci, C.POINTER(sz)],
     "moge_panorama_rhs_groups": [vp, ci, vp, ci, ci, ci, pc, C.POINTER(PanoramaLevel), ci, vp, sz, vp],
@@ -240,8 +230,6 @@ SIGNATURES = {
     "moge_threshold_depth_change": [vp, vp, i64, ci, ci, ci, C.c_float, ci, vp, vp],
     "moge_gaussian_blur_2d": [vp, i64, ci, ci, fp, ci, vp, vp],
     "moge_dino_create": [C.POINTER(DinoConfig), ci, C.POINTER(vp)],
-    "moge_dino_workspace_bytes": [vp, ci, ci, ci, C.POINTER(ci), ci, ci, C.POINTER(sz)],
-    "moge_dino_forward": [vp, vp, ci, ci, ci, ci, C.POINTER(ci), ci, ci, vp, vp, vp, vp, sz, vp],
     "moge_dino_workspace_bytes_groups": [vp, C.POINTER(DinoGroup), ci, C.POINTER(ci), ci, ci, C.POINTER(sz)],
     "moge_dino_forward_groups": [vp, C.POINTER(DinoGroup), ci, C.POINTER(ci), ci, ci, vp, sz, vp],
 }

@@ -42,7 +42,7 @@ struct Group {
     // bindings (set per forward)
     const void* image = nullptr; int image_dtype = 0;
     float* points = nullptr; float* normal = nullptr; float* mask = nullptr; float* scale = nullptr;
-    float* tokens = nullptr; float* cls_out = nullptr; float* prenorm = nullptr;     // DINOv2 backbone outputs (moge_dino_forward)
+    float* tokens = nullptr; float* cls_out = nullptr; float* prenorm = nullptr;     // DINOv2 backbone outputs (moge_dino_forward_groups)
 };
 
 // What a DINOv2 backbone plan exports besides its shape: the blocks whose rows it writes (increasing) and the MOGE_DINO_* flags
@@ -980,15 +980,9 @@ int moge_engine_workspace_bytes_groups(moge_engine_t* e, const moge_group_t* gro
     if (!bytes) return set_error("null argument");
     Plan pl;
     MG_TRY(to_groups(e, groups, n, false, &pl.groups));
-    if (e->v1) return set_error("a MoGe-1 engine takes moge_v1_workspace_bytes");
-    if (e->dino) return set_error("a DINOv2 backbone engine takes moge_dino_workspace_bytes");
+    if (e->v1) return set_error("a MoGe-1 engine takes moge_v1_workspace_bytes_groups");
+    if (e->dino) return set_error("a DINOv2 backbone engine takes moge_dino_workspace_bytes_groups");
     return build_plan(e, &pl, true, bytes);
-}
-
-int moge_engine_workspace_bytes(moge_engine_t* e, int B, int H, int W, int h, int w, size_t* bytes) {
-    moge_group_t g{};
-    g.B = B; g.H = H; g.W = W; g.h = h; g.w = w;
-    return moge_engine_workspace_bytes_groups(e, &g, 1, bytes);
 }
 
 // The checks of a forward call, before anything runs: the engine, its weights and the workspace pointer, then `groups` (the
@@ -1063,8 +1057,8 @@ static int forward_impl(moge_engine_t* e, const std::vector<Group>& groups, void
 }
 
 int moge_engine_forward_groups(moge_engine_t* e, const moge_group_t* groups, int n, void* workspace, size_t workspace_bytes, void* stream) {
-    if (e && e->v1) return set_error("a MoGe-1 engine runs through moge_v1_forward");
-    if (e && e->dino) return set_error("a DINOv2 backbone engine runs through moge_dino_forward");
+    if (e && e->v1) return set_error("a MoGe-1 engine runs through moge_v1_forward_groups");
+    if (e && e->dino) return set_error("a DINOv2 backbone engine runs through moge_dino_forward_groups");
     std::vector<Group> gs;
     MG_TRY(check_forward(e, workspace, [&] { return to_groups(e, groups, n, true, &gs); }));
     return forward_impl(e, gs, workspace, workspace_bytes, stream);
@@ -1087,19 +1081,6 @@ int moge_v1_forward_groups(moge_engine_t* e, const moge_v1_group_t* groups, int 
     return forward_impl(e, gs, workspace, workspace_bytes, stream);
 }
 
-int moge_v1_workspace_bytes(moge_engine_t* e, int B, int H, int W, int rh, int rw, size_t* bytes) {
-    moge_v1_group_t g{};
-    g.B = B; g.H = H; g.W = W; g.rh = rh; g.rw = rw;
-    return moge_v1_workspace_bytes_groups(e, &g, 1, bytes);
-}
-
-int moge_v1_forward(moge_engine_t* e, const void* image, int image_dtype, int B, int H, int W, int rh, int rw, void* workspace,
-                    size_t workspace_bytes, float* points, float* mask, void* stream) {
-    moge_v1_group_t g{};
-    g.image = image; g.image_dtype = image_dtype; g.B = B; g.H = H; g.W = W; g.rh = rh; g.rw = rw; g.points = points; g.mask = mask;
-    return moge_v1_forward_groups(e, &g, 1, workspace, workspace_bytes, stream);
-}
-
 int moge_v1_postprocess(float* points, const float* mask, float mask_threshold, const float* focal_in, int B, int H, int W,
                         int force_projection, int apply_mask, float* depth, uint8_t* mask_out, float* intrinsics, float* focal,
                         float* shift, void* stream) {
@@ -1107,14 +1088,6 @@ int moge_v1_postprocess(float* points, const float* mask, float mask_threshold, 
     if (B <= 0 || H <= 0 || W <= 0) return set_error("bad shape B=%d H=%d W=%d", B, H, W);
     return launch_v1_postprocess(points, mask, mask_threshold, focal_in, B, H, W, force_projection, apply_mask, depth, mask_out, intrinsics,
                                  focal, shift, static_cast<cudaStream_t>(stream));
-}
-
-int moge_engine_forward(moge_engine_t* e, const void* image, int image_dtype, int B, int H, int W, int h, int w, void* workspace,
-                        size_t workspace_bytes, float* points, float* normal, float* mask_prob, float* metric_scale, void* stream) {
-    moge_group_t g{};
-    g.image = image; g.image_dtype = image_dtype; g.B = B; g.H = H; g.W = W; g.h = h; g.w = w;
-    g.points = points; g.normal = normal; g.mask_prob = mask_prob; g.metric_scale = metric_scale;
-    return moge_engine_forward_groups(e, &g, 1, workspace, workspace_bytes, stream);
 }
 
 int moge_dino_workspace_bytes_groups(moge_engine_t* e, const moge_dino_group_t* groups, int n, const int* layers, int n_layers,
@@ -1132,19 +1105,6 @@ int moge_dino_forward_groups(moge_engine_t* e, const moge_dino_group_t* groups, 
     DinoKey key;
     MG_TRY(check_forward(e, workspace, [&] { return dino_groups(e, groups, n, layers, n_layers, flags, true, &gs, &key); }));
     return forward_impl(e, gs, workspace, workspace_bytes, stream, key);
-}
-
-int moge_dino_workspace_bytes(moge_engine_t* e, int B, int H, int W, const int* layers, int n_layers, int flags, size_t* bytes) {
-    moge_dino_group_t g{};
-    g.B = B; g.H = H; g.W = W;
-    return moge_dino_workspace_bytes_groups(e, &g, 1, layers, n_layers, flags, bytes);
-}
-
-int moge_dino_forward(moge_engine_t* e, const void* x, int x_dtype, int B, int H, int W, const int* layers, int n_layers, int flags,
-                      float* out_tokens, float* out_cls, float* out_prenorm, void* workspace, size_t workspace_bytes, void* stream) {
-    moge_dino_group_t g{};
-    g.x = x; g.x_dtype = x_dtype; g.B = B; g.H = H; g.W = W; g.out_tokens = out_tokens; g.out_cls = out_cls; g.out_prenorm = out_prenorm;
-    return moge_dino_forward_groups(e, &g, 1, layers, n_layers, flags, workspace, workspace_bytes, stream);
 }
 
 int moge_engine_num_ops(moge_engine_t* e, int* n) {
@@ -1165,7 +1125,7 @@ int moge_engine_op_info(moge_engine_t* e, int idx, char* name, int name_cap, dou
 }
 
 int moge_engine_profile(moge_engine_t* e, float* ms, int cap, void* stream) {
-    if (!e || !e->last_plan || !ms) return set_error("profile: run moge_engine_forward once first");
+    if (!e || !e->last_plan || !ms) return set_error("profile: run moge_engine_forward_groups once first");
     Plan* pl = e->last_plan;
     const int n = static_cast<int>(pl->ops.size());
     if (cap < n) return set_error("profile: need room for %d ops", n);

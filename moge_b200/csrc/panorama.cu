@@ -702,16 +702,13 @@ int load_cams(const char* what, const moge_panorama_camera_t* cams, int views, C
 
 unsigned blocks_for(int64_t n, int sms) { return static_cast<unsigned>(std::min<int64_t>((n + kThreads - 1) / kThreads, int64_t(sms) * 16)); }
 
-// an entry's name in messages: the operation's, and in a call of several panoramas also the entry's index
+// an entry's name in messages: the operation's and the entry's index
 struct Name {
     char s[96];
-    Name(const char* what, int k, bool indexed) {
-        if (indexed) snprintf(s, sizeof(s), "%s: panorama %d", what, k);
-        else snprintf(s, sizeof(s), "%s", what);
-    }
+    Name(const char* what, int k) { snprintf(s, sizeof(s), "%s: panorama %d", what, k); }
 };
 
-int null_argument(const Name& nm, bool indexed) { return indexed ? set_error("%s: null argument", nm.s) : set_error("null argument"); }
+int null_argument(const Name& nm) { return set_error("%s: null argument", nm.s); }
 
 int check_batch(const char* what, int batch) {
     if (batch < 1 || batch > MOGE_PANORAMA_MAX_BATCH)
@@ -742,29 +739,29 @@ Layout layout(int views, const moge_panorama_level_t* lv, int count) {
     return l;
 }
 
-int check_levels(const char* what, bool indexed, const moge_panorama_level_t* lv, int count) {
+int check_levels(const char* what, const moge_panorama_level_t* lv, int count) {
     if (!lv) return set_error("null argument");
     MG_TRY(check_batch(what, count));
-    for (int k = 0; k < count; ++k) MG_TRY(check_size(Name(what, k, indexed).s, lv[k].h, lv[k].w));
+    for (int k = 0; k < count; ++k) MG_TRY(check_size(Name(what, k).s, lv[k].h, lv[k].w));
     return 0;
 }
 
-int workspace_bytes(const char* what, bool indexed, const moge_panorama_level_t* lv, int count, int views, size_t* bytes) {
+int workspace_bytes(const char* what, const moge_panorama_level_t* lv, int count, int views, size_t* bytes) {
     if (!bytes) return set_error("null argument");
-    MG_TRY(check_levels(what, indexed, lv, count));
+    MG_TRY(check_levels(what, lv, count));
     if (views < 1 || views > MOGE_PANORAMA_MAX_VIEWS) return set_error("%s: %d views is outside [1, %d]", what, views, MOGE_PANORAMA_MAX_VIEWS);
     *bytes = layout(views, lv, count).total;
     return 0;
 }
 
-int split(const char* what, bool indexed, const moge_panorama_split_t* panos, int count, const moge_panorama_camera_t* cams, int views,
+int split(const char* what, const moge_panorama_split_t* panos, int count, const moge_panorama_camera_t* cams, int views,
           const float* grid, int res, float* views_f32, uint8_t* views_u8, void* stream) {
     if (!panos || !grid || !views_f32) return set_error("null argument");
     MG_TRY(check_batch(what, count));
     SplitTable tab{};
     for (int k = 0; k < count; ++k) {
-        const Name nm(what, k, indexed);
-        if (!panos[k].image) return null_argument(nm, indexed);
+        const Name nm(what, k);
+        if (!panos[k].image) return null_argument(nm);
         MG_TRY(check_size(nm.s, panos[k].H, panos[k].W));
         if (panos[k].view0 < 0) return set_error("%s: first view %d is negative", nm.s, panos[k].view0);
         tab.p[k] = {panos[k].image, panos[k].H, panos[k].W, panos[k].view0};
@@ -780,15 +777,15 @@ int split(const char* what, bool indexed, const moge_panorama_split_t* panos, in
     return 0;
 }
 
-int rhs(const char* what, bool indexed, const float* src, int channels, const uint8_t* mask, int views, int vh, int vw,
+int rhs(const char* what, const float* src, int channels, const uint8_t* mask, int views, int vh, int vw,
         const moge_panorama_camera_t* cams, const moge_panorama_level_t* lv, int count, void* workspace, size_t workspace_bytes,
         void* stream) {
     if (!src || !mask) return set_error("null argument");
     if (channels != 1 && channels != 3) return set_error("%s: %d channels (1: distance, 3: points)", what, channels);
-    MG_TRY(check_levels(what, indexed, lv, count));
+    MG_TRY(check_levels(what, lv, count));
     for (int k = 0; k < count; ++k) {
-        const Name nm(what, k, indexed);
-        if (!lv[k].directions || !lv[k].b || !lv[k].row_mask || !lv[k].pano_mask) return null_argument(nm, indexed);
+        const Name nm(what, k);
+        if (!lv[k].directions || !lv[k].b || !lv[k].row_mask || !lv[k].pano_mask) return null_argument(nm);
         if (lv[k].view0 < 0) return set_error("%s: first view %d is negative", nm.s, lv[k].view0);
     }
     char vname[112];
@@ -819,10 +816,10 @@ int rhs(const char* what, bool indexed, const float* src, int channels, const ui
 }
 
 // the LSMR solves of `count` systems: the virtual partition, the real grid over at most the co-resident blocks, the launch
-int lsmr(const char* what, bool indexed, const moge_panorama_level_t* lv, int count, void* workspace, size_t workspace_bytes, void* stream) {
-    MG_TRY(check_levels(what, indexed, lv, count));
+int lsmr(const char* what, const moge_panorama_level_t* lv, int count, void* workspace, size_t workspace_bytes, void* stream) {
+    MG_TRY(check_levels(what, lv, count));
     for (int k = 0; k < count; ++k)
-        if (!lv[k].b || !lv[k].row_mask || !lv[k].depth || !lv[k].stats) return null_argument(Name(what, k, indexed), indexed);
+        if (!lv[k].b || !lv[k].row_mask || !lv[k].depth || !lv[k].stats) return null_argument(Name(what, k));
     const Layout l = layout(1, lv, count);
     MG_TRY(check_workspace(l.total, workspace, workspace_bytes, what));
     int sms, dev = 0, coop = 0, per_sm = 0;
@@ -876,15 +873,15 @@ int lsmr(const char* what, bool indexed, const moge_panorama_level_t* lv, int co
     return 0;
 }
 
-int resize(const char* what, bool indexed, const moge_panorama_resize_t* maps, int count, void* stream) {
+int resize(const char* what, const moge_panorama_resize_t* maps, int count, void* stream) {
     if (!maps) return set_error("null argument");
     MG_TRY(check_batch(what, count));
     ResizeTable tab{};
     int64_t most = 0;
     for (int k = 0; k < count; ++k) {
-        const Name nm(what, k, indexed);
+        const Name nm(what, k);
         const moge_panorama_resize_t& m = maps[k];
-        if (!m.src || !m.dst) return null_argument(nm, indexed);
+        if (!m.src || !m.dst) return null_argument(nm);
         MG_TRY(check_size(nm.s, m.h, m.w));
         MG_TRY(check_size(nm.s, m.H, m.W));
         tab.m[k] = {m.src, m.dst, m.h, m.w, m.H, m.W};
@@ -897,16 +894,16 @@ int resize(const char* what, bool indexed, const moge_panorama_resize_t* maps, i
     return 0;
 }
 
-int finish(const char* what, bool indexed, const moge_panorama_finish_t* maps, int count, void* stream) {
+int finish(const char* what, const moge_panorama_finish_t* maps, int count, void* stream) {
     if (!maps) return set_error("null argument");
     MG_TRY(check_batch(what, count));
     ResizeTable rt{};
     FinishTable ft{};
     int64_t most = 0;
     for (int k = 0; k < count; ++k) {
-        const Name nm(what, k, indexed);
+        const Name nm(what, k);
         const moge_panorama_finish_t& m = maps[k];
-        if (!m.depth || !m.mask || !m.depth_out || !m.mask_out || !m.points) return null_argument(nm, indexed);
+        if (!m.depth || !m.mask || !m.depth_out || !m.mask_out || !m.points) return null_argument(nm);
         MG_TRY(check_size(nm.s, m.h, m.w));
         MG_TRY(check_size(nm.s, m.H, m.W));
         rt.m[k] = {m.depth, m.depth_out, m.h, m.w, m.H, m.W};
@@ -924,23 +921,6 @@ int finish(const char* what, bool indexed, const moge_panorama_finish_t* maps, i
     return 0;
 }
 
-// the `batch` same-size levels of the one-size entry points, back to back in b, row_mask (rows each), pano_mask, init and depth
-// (h * w each) and stats (2 each); the caller has checked batch
-void one_size_levels(int batch, int views, int h, int w, const float* directions, double* b, uint8_t* row_mask, uint8_t* pano_mask,
-                     const float* init, float* depth, int32_t* stats, moge_panorama_level_t* lv) {
-    const int64_t n = static_cast<int64_t>(h) * w, rows = lsmr_rows(h, w);
-    for (int k = 0; k < batch; ++k) {
-        moge_panorama_level_t& e = lv[k];
-        e.h = h; e.w = w; e.view0 = k * views; e.directions = directions;
-        e.b = b ? b + k * rows : nullptr;
-        e.row_mask = row_mask ? row_mask + k * rows : nullptr;
-        e.pano_mask = pano_mask ? pano_mask + k * n : nullptr;
-        e.init = init ? init + k * n : nullptr;
-        e.depth = depth ? depth + k * n : nullptr;
-        e.stats = stats ? stats + 2 * k : nullptr;
-    }
-}
-
 }  // namespace
 }  // namespace mg
 
@@ -950,86 +930,29 @@ extern "C" {
 
 int moge_panorama_split_groups(const moge_panorama_split_t* panos, int n, const moge_panorama_camera_t* cams, int views, const float* grid,
                                int res, float* views_f32, uint8_t* views_u8, void* stream) {
-    return split("panorama_split_groups", true, panos, n, cams, views, grid, res, views_f32, views_u8, stream);
-}
-
-int moge_panorama_split(const uint8_t* images, int batch, int H, int W, const moge_panorama_camera_t* cams, int views, const float* grid,
-                        int res, float* views_f32, uint8_t* views_u8, void* stream) {
-    if (!images || !grid || !views_f32) return set_error("null argument");
-    MG_TRY(check_batch("panorama_split", batch));
-    moge_panorama_split_t panos[MOGE_PANORAMA_MAX_BATCH];
-    for (int k = 0; k < batch; ++k) panos[k] = {images + static_cast<int64_t>(k) * H * W * 3, H, W, k * std::max(views, 0)};
-    return split("panorama_split", false, panos, batch, cams, views, grid, res, views_f32, views_u8, stream);
+    return split("panorama_split_groups", panos, n, cams, views, grid, res, views_f32, views_u8, stream);
 }
 
 int moge_panorama_workspace_bytes_groups(const moge_panorama_level_t* levels, int n, int views, size_t* bytes) {
-    return workspace_bytes("panorama_workspace_bytes_groups", true, levels, n, views, bytes);
-}
-
-int moge_panorama_workspace_bytes(int batch, int views, int h, int w, size_t* bytes) {
-    if (!bytes) return set_error("null argument");
-    MG_TRY(check_batch("panorama_workspace_bytes", batch));
-    moge_panorama_level_t lv[MOGE_PANORAMA_MAX_BATCH];
-    one_size_levels(batch, 0, h, w, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, lv);
-    return workspace_bytes("panorama_workspace_bytes", false, lv, batch, views, bytes);
+    return workspace_bytes("panorama_workspace_bytes_groups", levels, n, views, bytes);
 }
 
 int moge_panorama_rhs_groups(const float* src, int channels, const uint8_t* mask, int views, int vh, int vw,
                              const moge_panorama_camera_t* cams, const moge_panorama_level_t* levels, int n, void* workspace,
                              size_t workspace_bytes, void* stream) {
-    return rhs("panorama_rhs_groups", true, src, channels, mask, views, vh, vw, cams, levels, n, workspace, workspace_bytes, stream);
-}
-
-int moge_panorama_rhs(const float* src, int channels, const uint8_t* mask, int batch, int views, int vh, int vw,
-                      const moge_panorama_camera_t* cams, const float* directions, int h, int w, double* b, uint8_t* row_mask,
-                      uint8_t* pano_mask, void* workspace, size_t workspace_bytes, void* stream) {
-    if (!src || !mask || !directions || !b || !row_mask || !pano_mask) return set_error("null argument");
-    MG_TRY(check_batch("panorama_rhs", batch));
-    moge_panorama_level_t lv[MOGE_PANORAMA_MAX_BATCH];
-    one_size_levels(batch, std::max(views, 0), h, w, directions, b, row_mask, pano_mask, nullptr, nullptr, nullptr, lv);
-    return rhs("panorama_rhs", false, src, channels, mask, views, vh, vw, cams, lv, batch, workspace, workspace_bytes, stream);
+    return rhs("panorama_rhs_groups", src, channels, mask, views, vh, vw, cams, levels, n, workspace, workspace_bytes, stream);
 }
 
 int moge_panorama_lsmr_groups(const moge_panorama_level_t* levels, int n, void* workspace, size_t workspace_bytes, void* stream) {
-    return lsmr("panorama_lsmr_groups", true, levels, n, workspace, workspace_bytes, stream);
-}
-
-int moge_panorama_lsmr(const double* b, const uint8_t* row_mask, int batch, int h, int w, const float* init, float* depth,
-                       int32_t* stats, void* workspace, size_t workspace_bytes, void* stream) {
-    if (!b || !row_mask || !depth || !stats) return set_error("null argument");
-    MG_TRY(check_batch("panorama_lsmr", batch));
-    moge_panorama_level_t lv[MOGE_PANORAMA_MAX_BATCH];
-    one_size_levels(batch, 0, h, w, nullptr, const_cast<double*>(b), const_cast<uint8_t*>(row_mask), nullptr, init, depth, stats, lv);
-    return lsmr("panorama_lsmr", false, lv, batch, workspace, workspace_bytes, stream);
+    return lsmr("panorama_lsmr_groups", levels, n, workspace, workspace_bytes, stream);
 }
 
 int moge_panorama_resize_groups(const moge_panorama_resize_t* maps, int n, void* stream) {
-    return resize("panorama_resize_groups", true, maps, n, stream);
-}
-
-int moge_panorama_resize(const float* src, int batch, int h, int w, int H, int W, float* dst, void* stream) {
-    if (!src || !dst) return set_error("null argument");
-    MG_TRY(check_batch("panorama_resize", batch));
-    moge_panorama_resize_t maps[MOGE_PANORAMA_MAX_BATCH];
-    for (int k = 0; k < batch; ++k)
-        maps[k] = {src + static_cast<int64_t>(k) * h * w, h, w, H, W, dst + static_cast<int64_t>(k) * H * W};
-    return resize("panorama_resize", false, maps, batch, stream);
+    return resize("panorama_resize_groups", maps, n, stream);
 }
 
 int moge_panorama_finish_groups(const moge_panorama_finish_t* maps, int n, void* stream) {
-    return finish("panorama_finish_groups", true, maps, n, stream);
-}
-
-int moge_panorama_finish(const float* depth, const uint8_t* mask, int batch, int h, int w, int H, int W, float* depth_out,
-                         uint8_t* mask_out, float* points, void* stream) {
-    if (!depth || !mask || !depth_out || !mask_out || !points) return set_error("null argument");
-    MG_TRY(check_batch("panorama_finish", batch));
-    moge_panorama_finish_t maps[MOGE_PANORAMA_MAX_BATCH];
-    for (int k = 0; k < batch; ++k) {
-        const int64_t in = static_cast<int64_t>(k) * h * w, out = static_cast<int64_t>(k) * H * W;
-        maps[k] = {depth + in, mask + in, h, w, H, W, depth_out + out, mask_out + out, points + out * 3};
-    }
-    return finish("panorama_finish", false, maps, batch, stream);
+    return finish("panorama_finish_groups", maps, n, stream);
 }
 
 }  // extern "C"

@@ -120,20 +120,22 @@ def test_bad_inputs_raise_before_device_work():
         m.get_intermediate_layers(torch.zeros(1, 3, 98, 98))
 
 
-def test_c_abi_signatures():
-    for n in ("moge_dino_create", "moge_dino_workspace_bytes", "moge_dino_forward"):
+def test_c_abi_group_signatures():
+    for n in ("moge_dino_create", "moge_dino_workspace_bytes_groups", "moge_dino_forward_groups"):
         assert n in capi.SIGNATURES and n in capi.EXPORTS
     c = capi.DinoConfig()
     c.interpolate_offset = 0.1
     assert C.sizeof(c) == 9 * 4
 
 
-def test_c_checks_without_a_device():
+def test_c_group_checks_without_a_device():
     """The entry points' own checks: a null config or engine fails before anything touches a device."""
     L = capi.lib()
     h = C.c_void_p()
     assert L.moge_dino_create(None, 0, C.byref(h)) != 0 and b"null argument" in L.moge_last_error()
     n = C.c_size_t()
     lay = (C.c_int * 1)(11)
-    assert L.moge_dino_workspace_bytes(None, 1, 98, 98, lay, 1, 1, C.byref(n)) != 0 and b"null argument" in L.moge_last_error()
-    assert L.moge_dino_forward(None, None, 0, 1, 98, 98, lay, 1, 1, None, None, None, None, 0, None) != 0
+    g = (capi.DinoGroup * 1)()
+    g[0].B, g[0].H, g[0].W = 1, 98, 98
+    assert L.moge_dino_workspace_bytes_groups(None, g, 1, lay, 1, 1, C.byref(n)) != 0 and b"null argument" in L.moge_last_error()
+    assert L.moge_dino_forward_groups(None, g, 1, lay, 1, 1, None, 0, None) != 0 and b"null argument" in L.moge_last_error()

@@ -296,7 +296,7 @@ def test_from_pretrained_roundtrip(tmp_path):
     assert out["points"].shape == (70, 98, 3)
 
 
-def test_c_abi_error_paths():
+def test_c_abi_group_error_paths():
     """Error behaviour through the C ABI: negative return code + message, no crash, engine stays usable."""
     import ctypes as C
     from moge_b200 import capi
@@ -305,16 +305,17 @@ def test_c_abi_error_paths():
     img = synthetic_images(1, 70, 98, 3).to(DEV)
     model.forward(img, 100)                                   # makes sure the engine exists
     n = C.c_size_t()
-    assert L.moge_engine_workspace_bytes(model._engine, 0, 70, 98, 7, 10, C.byref(n)) != 0
+    g = (capi.Group * 1)()
+    g[0].B, g[0].H, g[0].W, g[0].h, g[0].w = 0, 70, 98, 7, 10
+    assert L.moge_engine_workspace_bytes_groups(model._engine, g, 1, C.byref(n)) != 0
     assert b"bad shape" in L.moge_last_error()
     pts = torch.empty(1, 70, 98, 3, device=DEV)
     ws = torch.empty(1 << 20, dtype=torch.uint8, device=DEV)
     base = (ws.data_ptr() + 1023) & ~1023
-    rc = L.moge_engine_forward(model._engine, img.data_ptr(), capi.F32, 1, 70, 98, 7, 10, base, 1 << 19, pts.data_ptr(), None, None, None,
-                               capi.current_stream())
+    g[0].image, g[0].image_dtype, g[0].B, g[0].points = img.data_ptr(), capi.F32, 1, pts.data_ptr()
+    rc = L.moge_engine_forward_groups(model._engine, g, 1, base, 1 << 19, capi.current_stream())
     assert rc != 0 and b"workspace too small" in L.moge_last_error()
-    rc = L.moge_engine_forward(model._engine, img.data_ptr(), capi.F32, 1, 70, 98, 7, 10, base + 8, 1 << 19, pts.data_ptr(), None, None, None,
-                               capi.current_stream())
+    rc = L.moge_engine_forward_groups(model._engine, g, 1, base + 8, 1 << 19, capi.current_stream())
     assert rc != 0 and b"aligned" in L.moge_last_error()
     assert L.moge_engine_set_weight(model._engine, b"x", img.data_ptr(), (C.c_int64 * 1)(3), 1, capi.F32, None) != 0   # finalized
     h = C.c_void_p()

@@ -23,6 +23,27 @@ def camera():
     return c
 
 
+def split():
+    e = (capi.PanoramaSplit * 1)()
+    e[0].image, e[0].H, e[0].W = P, 8, 8
+    return e
+
+
+def level(h=8, w=8, **ptrs):
+    """One panorama's h x w merge level; every pointer but init is the stand-in unless `ptrs` gives it."""
+    lv = (capi.PanoramaLevel * 1)()
+    lv[0].h, lv[0].w = h, w
+    for name in ("directions", "b", "row_mask", "pano_mask", "depth", "stats"):
+        setattr(lv[0], name, ptrs.get(name, P))
+    return lv
+
+
+def resize():
+    m = (capi.PanoramaResize * 1)()
+    m[0].src, m[0].h, m[0].w, m[0].H, m[0].W, m[0].dst = P, 8, 8, 16, 16, P
+    return m
+
+
 def maps(kind=capi.MESH_F32, channels=1):
     m = (capi.MeshMap * 1)()
     m[0].src, m[0].kind, m[0].channels, m[0].dst = P, kind, channels, P
@@ -83,29 +104,33 @@ CASES = {
     "mesh_build_ws_small": ("mesh_build", lambda: L.moge_mesh_build(None, 1, 8, 8, 1, maps(), 1, P, P, 256, 16, None), "bytes needed"),
     "mesh_build_ws_align": ("mesh_build", lambda: L.moge_mesh_build(None, 1, 8, 8, 1, maps(), 1, P, P, 264, BIG, None),
                             "256-byte aligned"),
-    # panorama: every entry point takes a batch; batch1 cases are one panorama
-    "panorama_batch_range": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(65, 1, 8, 8, C.byref(NB)),
-                             "batch of 65 panoramas"),
-    "panorama_batch1_views": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(1, 21, 8, 8, C.byref(NB)), "outside"),
-    "panorama_batch1_small": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(1, 1, 1, 8, C.byref(NB)), "too small"),
-    "panorama_batch1_too_large": ("panorama_workspace_bytes", lambda: L.moge_panorama_workspace_bytes(1, 1, 40000, 30000, C.byref(NB)),
-                                  "too large"),
-    "panorama_batch1_split_res": ("panorama_split", lambda: L.moge_panorama_split(P, 1, 8, 8, camera(), 1, P, 0, P, None, None), "outside"),
-    "panorama_batch1_split_views": ("panorama_split", lambda: L.moge_panorama_split(P, 1, 8, 8, camera(), 0, P, 8, P, None, None),
-                                    "outside"),
-    "panorama_batch1_split_cams": ("panorama_split", lambda: L.moge_panorama_split(P, 1, 8, 8, None, 1, P, 8, P, None, None),
+    # panorama: the `_groups` entry points, with one entry except for the count
+    "panorama_groups_count": ("panorama_workspace_bytes_groups",
+                              lambda: L.moge_panorama_workspace_bytes_groups(level(), 65, 1, C.byref(NB)), "batch of 65 panoramas"),
+    "panorama_groups_views": ("panorama_workspace_bytes_groups",
+                              lambda: L.moge_panorama_workspace_bytes_groups(level(), 1, 21, C.byref(NB)), "outside"),
+    "panorama_groups_small": ("panorama_workspace_bytes_groups",
+                              lambda: L.moge_panorama_workspace_bytes_groups(level(1, 8), 1, 1, C.byref(NB)), "too small"),
+    "panorama_groups_too_large": ("panorama_workspace_bytes_groups",
+                                  lambda: L.moge_panorama_workspace_bytes_groups(level(40000, 30000), 1, 1, C.byref(NB)), "too large"),
+    "panorama_groups_split_res": ("panorama_split_groups",
+                                  lambda: L.moge_panorama_split_groups(split(), 1, camera(), 1, P, 0, P, None, None), "outside"),
+    "panorama_groups_split_views": ("panorama_split_groups",
+                                    lambda: L.moge_panorama_split_groups(split(), 1, camera(), 0, P, 8, P, None, None), "outside"),
+    "panorama_groups_split_cams": ("panorama_split_groups", lambda: L.moge_panorama_split_groups(split(), 1, None, 1, P, 8, P, None, None),
                                    "null cameras"),
-    "panorama_batch1_rhs_null": ("", lambda: L.moge_panorama_rhs(P, 1, P, 1, 1, 8, 8, camera(), P, 8, 8, None, P, P, 256, BIG, None),
+    "panorama_groups_rhs_null": ("panorama_rhs_groups",
+                                 lambda: L.moge_panorama_rhs_groups(P, 1, P, 1, 8, 8, camera(), level(b=None), 1, 256, BIG, None),
                                  "null argument"),
-    "panorama_batch1_rhs_ws_small": ("panorama_rhs",
-                                     lambda: L.moge_panorama_rhs(P, 1, P, 1, 1, 8, 8, camera(), P, 8, 8, P, P, P, 256, 16, None),
+    "panorama_groups_rhs_ws_small": ("panorama_rhs_groups",
+                                     lambda: L.moge_panorama_rhs_groups(P, 1, P, 1, 8, 8, camera(), level(), 1, 256, 16, None),
                                      "bytes needed"),
-    "panorama_batch1_rhs_ws_align": ("panorama_rhs",
-                                     lambda: L.moge_panorama_rhs(P, 1, P, 1, 1, 8, 8, camera(), P, 8, 8, P, P, P, 264, BIG, None),
+    "panorama_groups_rhs_ws_align": ("panorama_rhs_groups",
+                                     lambda: L.moge_panorama_rhs_groups(P, 1, P, 1, 8, 8, camera(), level(), 1, 264, BIG, None),
                                      "256-byte aligned"),
-    "panorama_batch1_lsmr_ws_small": ("panorama_lsmr", lambda: L.moge_panorama_lsmr(P, P, 1, 8, 8, None, P, P, 256, 16, None),
+    "panorama_groups_lsmr_ws_small": ("panorama_lsmr_groups", lambda: L.moge_panorama_lsmr_groups(level(), 1, 256, 16, None),
                                       "bytes needed"),
-    "panorama_batch1_lsmr_ws_align": ("panorama_lsmr", lambda: L.moge_panorama_lsmr(P, P, 1, 8, 8, None, P, P, 264, BIG, None),
+    "panorama_groups_lsmr_ws_align": ("panorama_lsmr_groups", lambda: L.moge_panorama_lsmr_groups(level(), 1, 264, BIG, None),
                                       "256-byte aligned"),
     # losses
     "loss_batch": ("loss", lambda: L.moge_loss_workspace_bytes(0, 8, 8, C.byref(NB)), "outside"),
@@ -144,7 +169,7 @@ NO_DEVICE = {
     "align_affine_lstsq": ("align_affine_lstsq", lambda: L.moge_align_affine_lstsq(P, P, None, 1, 8, P, P, None)),
     "masked_nearest_resize": ("masked_nearest_resize", lambda: L.moge_metrics_resize(P, 1, 8, 8, 4, 4, P, P, P, P, P, None)),
     "mesh_count": ("mesh_count", lambda: L.moge_mesh_count(None, 1, 8, 8, P, 256, BIG, None)),
-    "panorama_batch1_resize": ("panorama_resize", lambda: L.moge_panorama_resize(P, 1, 8, 8, 16, 16, P, None)),
+    "panorama_groups_resize": ("panorama_resize_groups", lambda: L.moge_panorama_resize_groups(resize(), 1, None)),
     "loss_mask": ("loss_mask", lambda: L.moge_loss_mask(capi.LOSS_MASK_L2, P, P, P, 1, 8, 8, None, None, P, 256, BIG, None)),
 }
 

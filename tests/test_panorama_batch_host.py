@@ -1,6 +1,5 @@
 """Batched panorama inference, host side (no GPU): the argument checks of split_panoramas, merge_panoramas, finish_panoramas and
-infer_panoramas fail with MogeError before any device work, and the panorama C entry points, which all take a batch, are in the
-ABI table."""
+infer_panoramas fail with MogeError before any device work, and the C library's batch limit is the Python one."""
 import pytest
 import torch
 
@@ -9,14 +8,8 @@ from moge_b200 import panorama as P
 from moge_b200.capi import MogeError
 
 
-def test_panorama_entry_points_in_signature_table():
-    for name in ("moge_panorama_split", "moge_panorama_rhs", "moge_panorama_lsmr", "moge_panorama_workspace_bytes",
-                 "moge_panorama_resize", "moge_panorama_finish"):
-        assert name in capi.SIGNATURES and name in capi.EXPORTS
-    assert capi.PANORAMA_MAX_BATCH == P.MAX_BATCH == 64
-
-
 def test_split_panoramas_checks():
+    assert capi.PANORAMA_MAX_BATCH == P.MAX_BATCH == 64
     imgs = torch.zeros(2, 64, 128, 3, dtype=torch.uint8)
     with pytest.raises(MogeError, match="CUDA"):
         P.split_panoramas(imgs)

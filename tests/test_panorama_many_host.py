@@ -141,7 +141,7 @@ def test_group_null_arguments_rejected_without_device():
     assert "panorama 1: a 1 x 8 map is too small" in _error(L.moge_panorama_lsmr_groups(lv, 2, 256, 256, None))
 
 
-def test_group_workspace_bytes():
+def test_group_workspace_bytes_grow_with_entries():
     L = capi.lib()
 
     def nbytes(sizes):
@@ -149,9 +149,6 @@ def test_group_workspace_bytes():
         capi.check(L.moge_panorama_workspace_bytes_groups(_levels_array(sizes), len(sizes), 12, C.byref(out)))
         return out.value
 
-    one = C.c_size_t()
-    capi.check(L.moge_panorama_workspace_bytes(3, 12, 960, 1920, C.byref(one)))
-    assert one.value == nbytes([(960, 1920)] * 3)                          # the one-size entry point is the one-size groups call
     mixed = [(960, 1920), (384, 768), (100, 200)]
     assert nbytes(mixed) > nbytes(mixed[1:]) > nbytes(mixed[2:]) > 0
     # a call whose entries are each no larger fits in the workspace: every coarser level of a pyramid does

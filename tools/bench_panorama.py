@@ -20,6 +20,7 @@ sys.path.insert(0, ROOT)
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from bench_panorama_batch import merge_levels  # noqa: E402
 from measure import cuda_samples, gpu_identity  # noqa: E402
 from moge_b200 import panorama as P  # noqa: E402
 from moge_b200.synthetic import synthetic_panorama, synthetic_room_views  # noqa: E402
@@ -59,45 +60,10 @@ def staged(model, image):
 
 
 def merge_levels_ms(src, mask, width, height, extr, intr):
-    """The merge alone, one event pair around each level's right-hand side + solve (resize included)."""
-    timers = []
-    import ctypes as C
-    from moge_b200 import capi
-    L = capi.lib()
-    cams, n = P._cameras(extr, intr)
-    levels = P._levels(width, height)
-    nb = C.c_size_t()
-    capi.check(L.moge_panorama_workspace_bytes(1, n, height, width, C.byref(nb)))
-    ws = torch.empty(nb.value, dtype=torch.uint8, device=DEV)
-    stats = torch.zeros(len(levels), 2, dtype=torch.int32, device=DEV)
-    s = src.contiguous()
-    m = mask.contiguous().view(torch.uint8)
-    ch = 1 if s.dim() == 3 else 3
-    init = None
-    st = capi.current_stream()
-    for lv, (w, h) in enumerate(levels):
-        b = torch.empty(P.num_rows(h, w), dtype=torch.float64, device=DEV)
-        rm = torch.empty_like(b, dtype=torch.uint8)
-        pm = torch.empty(h, w, dtype=torch.uint8, device=DEV)
-        dirs = P._table("dirs", (h, w), torch.device(DEV))
-        t = Timer()
-        t.mark("start")
-        capi.check(L.moge_panorama_rhs(s.data_ptr(), ch, m.data_ptr(), 1, n, s.shape[1], s.shape[2], cams, dirs.data_ptr(), h, w,
-                                       b.data_ptr(), rm.data_ptr(), pm.data_ptr(), ws.data_ptr(), ws.numel(), st))
-        t.mark("rhs_ms")
-        depth = torch.empty(h, w, dtype=torch.float32, device=DEV)
-        capi.check(L.moge_panorama_lsmr(b.data_ptr(), rm.data_ptr(), 1, h, w, capi.ptr(init), depth.data_ptr(), stats[lv].data_ptr(),
-                                        ws.data_ptr(), ws.numel(), st))
-        t.mark("lsmr_ms")
-        timers.append(t)
-        if lv + 1 < len(levels):
-            W2, H2 = levels[lv + 1]
-            init = torch.empty(H2, W2, dtype=torch.float32, device=DEV)
-            capi.check(L.moge_panorama_resize(depth.data_ptr(), 1, h, w, H2, W2, init.data_ptr(), st))
-    torch.cuda.synchronize()
-    it = stats.cpu().tolist()
-    return [{"size": f"{w}x{h}", **{k: round(v, 3) for k, v in t.result().items()}, "iterations": i[0], "istop": i[1]}
-            for (w, h), t, i in zip(levels, timers, it)]
+    """The merge of one panorama alone, src (N, vh, vw[, 3]) and mask (N, vh, vw): per level its size, the ms of its right-hand
+    side and of its LSMR solve, its iteration count and istop."""
+    return [{**lv, "rhs_ms": round(lv["rhs_ms"], 3), "lsmr_ms": round(lv["lsmr_ms"], 3), "iterations": lv["iterations"][0],
+             "istop": lv["istop"][0]} for lv in merge_levels(src[None], mask[None], width, height, extr, intr)]
 
 
 def main():
